@@ -227,6 +227,11 @@ struct Step {
     int stream = 0;
     std::vector<int> waits;
     int record = -1;
+    // fused z + y stage (fft_zy_fused_kernel): prm is the z pass, prm_y the y pass; zyf holds the counters, advanced by
+    // every launch
+    bool zy = false;
+    FftParams prm_y{};
+    ZyFused zyf{};
 };
 
 struct Schedule {
@@ -263,6 +268,7 @@ struct dfft_plan_s {
     int* groups_d = nullptr;  // [3][P] group member lists on device
     std::vector<int> grp[3];
     int* err_d = nullptr;
+    size_t l2_bytes = size_t(50) << 20;           // L2 of the plan's GPU (geometry-only plans: an H100's 50 MB)
     unsigned long long epoch = 0;
     unsigned long long ticket[4] = {0, 0, 0, 0};  // per-phase rendezvous counters (same sequence on every rank)
     cudaStream_t aux[2] = {nullptr, nullptr};     // exchange stream (high priority), follow-up stream
@@ -370,6 +376,49 @@ static SegN mkseg(void* base, long long sA0, long long sA1, long long sN, size_t
     return r;
 }
 
+// Whether the z and y passes run as one fused launch (fft_zy_fused_kernel): one-rank slab C2C plans of the full 3D
+// transform with Ny == Nz of an instantiated length (zy_fused_length) whose array is larger than the L2 — below that the
+// three passes are L2-resident already and gain nothing.
+static bool zy_fused(const dfft_plan_s* p, int inverse, int d) {
+    const Geometry& g = p->g;
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3) return false;
+    if (g.ny != g.nz || !zy_fused_length(ilog2_exact(g.ny))) return false;
+    // the fused stage reads and writes the blocked hand-over layout of the x pass
+    if (p->blocked_ch <= 0 || g.nz % size_t(p->blocked_ch) || (inverse && !p->blocked_inv)) return false;
+    return g.ny * g.nz * p->esize * g.nx > p->l2_bytes;
+}
+
+// one launch of z and y: zs = the z pass, ys = the y pass (of the same direction), phase = timer section
+static int fuse_zy(dfft_plan_s* p, Step zs, const Step& ys, const char* label, const char* phase, Step& out) {
+    if (zs.log2n != ys.log2n) return fail(DFFT_ERR_STATE, "internal: fused z + y stage needs Ny == Nz");
+    out = zs;
+    out.zy = true;
+    out.label = label;
+    out.phase = phase;
+    out.prm_y = ys.prm;
+    out.zyf = ZyFused{};
+    // Groups of one plane; phase A runs L planes ahead of phase B: L + 1 planes of intermediate in flight, a third of the
+    // L2 (512^2 complex-double: L = 3; L = 2, L = 5 and groups of two planes were slower, DESIGN.md section 3.4).
+    out.zyf.order.nx = int(p->g.nx);
+    out.zyf.order.gpp = 1;
+    {
+        const long long ahead = (long long)(p->l2_bytes / (3 * p->g.ny * p->g.nz * p->esize)) - 1;
+        out.zyf.order.ahead = int(ahead < 1 ? 1 : ahead);
+    }
+    out.zyf.err = p->err_d;
+    out.zyf.timeout_cycles = p->rendezvous_timeout_cycles;
+    if (!p->tabs.dry) {
+        // [0] ticket counter, [1 + g] per-group counters; zeroed once, then only ever incremented (epoch targets)
+        const size_t bytes = sizeof(unsigned long long) * (1 + size_t(out.zyf.order.groups()));
+        void* c = nullptr;
+        if (cudaMalloc(&c, bytes) != cudaSuccess) return fail(DFFT_ERR_CUDA, "fused z + y stage: counter allocation failed");
+        p->tabs.bytes.push_back(c);  // freed with the schedules
+        if (cudaMemset(c, 0, bytes) != cudaSuccess) return fail(DFFT_ERR_CUDA, "fused z + y stage: counter initialisation failed");
+        out.zyf.ctr = reinterpret_cast<unsigned long long*>(c);
+    }
+    return DFFT_SUCCESS;
+}
+
 static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     const Geometry& g = p->g;
     const int me = p->rank, P = p->P;
@@ -428,6 +477,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
 
     const size_t nzc = g.nzc;
     const bool zyx = g.decomp == DFFT_SLAB_Z_THEN_YX;
+    const bool zy = zy_fused(p, inverse, d);  // one fused launch for the z and y passes
     int rc;
 
     // sizes of this rank
@@ -513,7 +563,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
             }
         }
         if (g.decomp == DFFT_SLAB_ZY_THEN_X) s1.phase = nullptr;
-        sc.steps.push_back(s1);
+        if (!zy) sc.steps.push_back(s1);
         if (t1_a2a) { x1.phase = zyx ? "Transpose (Finished All2All)" : "First Transpose (Finished All2All)"; x1.group = 1; sc.steps.push_back(x1); }
         else if (G1.size() > 1) rendezvous(1, 1, zyx ? "Transpose (Finished Receive)" : "First Transpose (Finished Receive)");
 
@@ -616,7 +666,13 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
                 return mkseg(eptr(slotp(SS, me), x2.soff[q], es), (long long)(nyq * nz_j), 0, (long long)nz_j, g.oy.start[q]);
             });
         }
-        if (have_tail) { const char* ph = s2.phase; s2.phase = nullptr; sc.steps.push_back(s2); s2t.phase = ph; sc.steps.push_back(s2t); }
+        if (zy) {
+            if (have_tail || t1_a2a || t2_a2a || G1.size() > 1 || G2.size() > 1) return fail(DFFT_ERR_STATE, "internal: fused z + y stage");
+            Step f;
+            rc = fuse_zy(p, s1, s2, "zy pass", s2.phase, f);
+            if (rc) return rc;
+            sc.steps.push_back(f);
+        } else if (have_tail) { const char* ph = s2.phase; s2.phase = nullptr; sc.steps.push_back(s2); s2t.phase = ph; sc.steps.push_back(s2t); }
         else sc.steps.push_back(s2);
         const bool slab = g.decomp == DFFT_SLAB_ZY_THEN_X;
         if (t2_a2a) { x2.phase = slab ? "Transpose (Finished All2All)" : "Second Transpose (Finished All2All)"; x2.group = 2; sc.steps.push_back(x2); }
@@ -799,7 +855,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
             const char* ph = s2.phase; s2.phase = nullptr; s2t.phase = ph;
             sc.steps.push_back(s2);
             sc.steps.push_back(s2t);
-        } else {
+        } else if (!zy) {
             sc.steps.push_back(s2);
         }
         if (G1.size() > 1) rendezvous(1, 1, "First Transpose (Finished Receive)");
@@ -810,7 +866,15 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         s1.prm.in = single_view(slotp(D1, me), (long long)(ny_j * nzc), (long long)nzc, 1);
         s1.prm.out = single_view(nullptr, zpitch_out * (long long)ny_j, zpitch_out, 1);
         s1.out_user = 2;
-        sc.steps.push_back(s1);
+        if (zy) {
+            if (any_rem || G1.size() > 1 || G2.size() > 1) return fail(DFFT_ERR_STATE, "internal: fused z + y stage");
+            Step f;
+            rc = fuse_zy(p, s1, s2, "yz pass", s1.phase, f);
+            if (rc) return rc;
+            sc.steps.push_back(f);
+        } else {
+            sc.steps.push_back(s1);
+        }
         sc.built = true;
         return DFFT_SUCCESS;
     }
@@ -1770,7 +1834,16 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
             // views on the caller's buffers store a byte offset in seg[0].base
             if (s.in_user == 1) prm.in.seg[0].base = (char*)const_cast<void*>(in) + (size_t)s.prm.in.seg[0].base;
             if (s.out_user == 2) prm.out.seg[0].base = (char*)out + (size_t)s.prm.out.seg[0].base;
-            cudaError_t e = p->prec == DFFT_F64 ? launch_pass_f64(s.log2n, s.kind, prm, ss) : launch_pass_f32(s.log2n, s.kind, prm, ss);
+            cudaError_t e;
+            if (s.zy) {
+                ZyFused f = s.zyf;
+                f.epoch += 1;
+                unsigned long long tickets = 0;
+                e = p->prec == DFFT_F64 ? launch_zy_fused_f64(s.log2n, prm, s.prm_y, f, &tickets, ss) : launch_zy_fused_f32(s.log2n, prm, s.prm_y, f, &tickets, ss);
+                if (e == cudaSuccess) { s.zyf.epoch = f.epoch; s.zyf.ticket_base += tickets; }
+            } else {
+                e = p->prec == DFFT_F64 ? launch_pass_f64(s.log2n, s.kind, prm, ss) : launch_pass_f32(s.log2n, s.kind, prm, ss);
+            }
             if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("FFT pass launch failed: ") + cudaGetErrorString(e));
             ++launches;
             CK_CUDA(mark(s.phase, 1, s.label));
@@ -2175,6 +2248,10 @@ int dfft_plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, in
             return fail(DFFT_ERR_CUDA, "stream / event creation failed");
         }
     }
+    {
+        int l2 = 0;
+        if (cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, comm->device) == cudaSuccess && l2 > 0) p->l2_bytes = size_t(l2);
+    }
     int rc = plan_setup_flags(p);
     if (rc == DFFT_SUCCESS && allocate) rc = plan_setup_memory(p, nullptr);
     if (rc != DFFT_SUCCESS) {
@@ -2264,6 +2341,9 @@ int dfft_plan_wait(dfft_plan_t p) {
     CK_CUDA(cudaMemcpy(&err, p->err_d, sizeof(int), cudaMemcpyDeviceToHost));
     if (err) {
         cudaMemset(p->err_d, 0, sizeof(int));
+        if (err == ZY_ERR_TIMEOUT)
+            return fail(DFFT_ERR_TIMEOUT, "fused z + y stage: a wait for the other phase timed out (DFFT_RENDEZVOUS_TIMEOUT_S); results are "
+                                          "invalid and the plan must be destroyed");
         if (err >= 100)
             return fail(DFFT_ERR_TIMEOUT, "a peer rank gave up waiting at a device rendezvous (phase " + std::to_string(err - 100) +
                                               "); results are invalid and the plan must be destroyed");
@@ -2545,7 +2625,21 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
     }
     o += "],\"steps\":[";
     bool first = true;
+    std::vector<Step> listed;  // the fused z + y stage is listed as its two phases, in the order they consume data
     for (const Step& s_ : sc.steps) {
+        if (!s_.zy) { listed.push_back(s_); continue; }
+        Step z = s_, y = s_;
+        z.zy = y.zy = false;
+        y.kind = PASS_C2C_TILED;
+        y.prm = s_.prm_y;
+        y.in_user = y.out_user = 0;
+        const bool inv = s_.prm.inverse != 0;
+        z.label = inv ? "yz pass: z phase" : "zy pass: z phase";
+        y.label = inv ? "yz pass: y phase" : "zy pass: y phase";
+        if (inv) { listed.push_back(y); listed.push_back(z); }
+        else { listed.push_back(z); listed.push_back(y); }
+    }
+    for (const Step& s_ : listed) {
         if (!first) o += ",";
         first = false;
         o += "{\"type\":" + std::to_string(int(s_.type)) + ",\"label\":\"" + s_.label + "\",\"stream\":" + std::to_string(s_.stream) +

@@ -195,4 +195,53 @@ cudaError_t launch_pass(PassKind kind, const FftParams& p, cudaStream_t stream) 
 
 template cudaError_t launch_pass<DFFT_T, DFFT_LOG2N>(PassKind, const FftParams&, cudaStream_t);
 
+#if DFFT_LOG2N == 8 || DFFT_LOG2N == 9
+static bool aligned128(const void* base, long long elems_a, long long elems_b, long long elems_c) {
+    constexpr long long es = sizeof(cx<DFFT_T>);
+    return reinterpret_cast<unsigned long long>(base) % 128 == 0 && (elems_a * es) % 128 == 0 && (elems_b * es) % 128 == 0 && (elems_c * es) % 128 == 0;
+}
+
+template <typename T, int LOG2N>
+cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFused& f_in, unsigned long long* tickets, cudaStream_t stream) {
+    static_assert(zy_fused_length(LOG2N), "fused z + y stage: length not instantiated");
+    using Z = ZyShape<T, LOG2N>;
+    constexpr int TB = Z::TB;
+    const bool inv = pz.inverse != 0;
+    if (pz.in.nseg != 1 || pz.out.nseg != 1 || py.in.nseg != 1 || py.out.nseg != 1 || pz.in.sN != 1 || pz.out.sN != 1) return cudaErrorInvalidValue;
+    if (pz.inverse != py.inverse || py.tile_swz != 0 || pz.A0 != py.A0 || pz.A1 % TB || py.B % TB || f_in.order.nx != pz.A0 || f_in.order.gpp < 1 || f_in.order.ahead < 1)
+        return cudaErrorInvalidValue;
+    ZyFused f = f_in;
+    const int z_per_plane = pz.A1 / TB, y_per_plane = py.A1 * (py.B / TB);  // tiles = work items
+    f.order.na = inv ? y_per_plane : z_per_plane;
+    f.order.nb = inv ? z_per_plane : y_per_plane;
+    // phase B reads the intermediate: forward the y tiles (rows of TB elements sN apart), inverse the z lines
+    const View& mid = inv ? pz.in : py.in;
+    f.discard = inv ? (Z::Z_DISCARD && aligned128(mid.seg[0].base, mid.seg[0].sA0, mid.seg[0].sA1, 1 << LOG2N))
+                    : (Z::Y_DISCARD && aligned128(mid.seg[0].base, mid.seg[0].sA0, mid.seg[0].sA1, mid.sN));
+    auto kf = fft_zy_fused_kernel<T, LOG2N, false>;
+    auto ki = fft_zy_fused_kernel<T, LOG2N, true>;
+    static cudaError_t once = set_smem(kf, Z::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ki, Z::SMEM_BYTES);
+    if (once != cudaSuccess) return once;
+    // persistent: as many CTAs as fit at once (tickets hand out the work; fewer resident CTAs are fine as well)
+    static const int resident = [&] {
+        int dev = 0, sms = 0, per = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kf, Z::THREADS, Z::SMEM_BYTES) != cudaSuccess || per < 1) per = 1;
+        return sms * per;
+    }();
+    const long long total = f.order.total();
+    if (total <= 0) { *tickets = 0; return cudaSuccess; }
+    const unsigned grid = unsigned(total < resident ? total : resident);
+    if (inv) ki<<<grid, Z::THREADS, Z::SMEM_BYTES, stream>>>(pz, py, f);
+    else kf<<<grid, Z::THREADS, Z::SMEM_BYTES, stream>>>(pz, py, f);
+    const cudaError_t e = cudaGetLastError();
+    // every ticket below total() is drawn once, and every CTA draws one more, which tells it to stop
+    *tickets = e == cudaSuccess ? (unsigned long long)total + grid : 0;
+    return e;
+}
+
+template cudaError_t launch_zy_fused<DFFT_T, DFFT_LOG2N>(const FftParams&, const FftParams&, const ZyFused&, unsigned long long*, cudaStream_t);
+#endif
+
 }  // namespace dfft

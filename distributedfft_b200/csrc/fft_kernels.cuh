@@ -27,6 +27,7 @@
 #include <type_traits>
 
 #include "fft_core.cuh"
+#include "zy_order.hpp"
 
 namespace dfft {
 
@@ -284,6 +285,134 @@ struct TileCoord {
     }
 };
 
+// ---- global-memory access of a C2C tile ------------------------------------------------------------------
+// MemPlain: default caching, what every standalone pass uses.  MemHint: per-instruction L2 eviction priorities
+// (createpolicy.fractional policies), used by the fused z/y kernel to keep its intermediate in the L2.
+template <typename T>
+struct MemPlain {
+    __device__ __forceinline__ cx<T> ld(const cx<T>* p) const { return ld_elem<T>(p); }
+    __device__ __forceinline__ void st(cx<T>* p, cx<T> v) const { st_elem<T>(p, v); }
+};
+
+__device__ __forceinline__ unsigned long long l2_evict_first() {
+    unsigned long long pol;
+    asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ unsigned long long l2_evict_last() {
+    unsigned long long pol;
+    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ unsigned long long l2_evict_normal() {
+    unsigned long long pol;
+    asm("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+
+template <typename T>
+struct MemHint {
+    unsigned long long ld_pol, st_pol;
+    __device__ __forceinline__ cx<T> ld(const cx<T>* p) const {
+        cx<T> r;
+        if constexpr (sizeof(T) == 8)
+            asm volatile("ld.global.L2::cache_hint.v2.f64 {%0, %1}, [%2], %3;" : "=d"(r.x), "=d"(r.y) : "l"(p), "l"(ld_pol) : "memory");
+        else
+            asm volatile("ld.global.L2::cache_hint.v2.f32 {%0, %1}, [%2], %3;" : "=f"(r.x), "=f"(r.y) : "l"(p), "l"(ld_pol) : "memory");
+        return r;
+    }
+    __device__ __forceinline__ void st(cx<T>* p, cx<T> v) const {
+        if constexpr (sizeof(T) == 8)
+            asm volatile("st.global.L2::cache_hint.v2.f64 [%0], {%1, %2}, %3;" ::"l"(p), "d"(v.x), "d"(v.y), "l"(st_pol) : "memory");
+        else
+            asm volatile("st.global.L2::cache_hint.v2.f32 [%0], {%1, %2}, %3;" ::"l"(p), "f"(v.x), "f"(v.y), "l"(st_pol) : "memory");
+    }
+};
+
+// drop a 128-byte L2 line without writing it back (its contents become undefined)
+__device__ __forceinline__ void l2_discard(const void* p) { asm volatile("discard.global.L2 [%0], 128;" ::"l"(p) : "memory"); }
+
+// ---- one tile of a C2C pass: load, CtaFft::stages, store --------------------------------------------------
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, typename M>
+__device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<T>* sm, unsigned long long* tab_in, unsigned long long* tab_out,
+                                         bool multi, const M& mem) {
+    using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
+    using LA = LineAccess<T, C::LINES>;
+    using TC = TileCoord<C, TILED, TB>;
+    constexpr int E = C::E, TPL = C::TPL;
+    const TC tc(p, tile);
+    const int j = tc.j, t = tc.t;
+    if (multi) {
+        // TILED: one table per CTA (a0, a1 are CTA-uniform), filled by the first threads;
+        // CONTIG: one table per line, filled by that line's threads.
+        const int line = TILED ? 0 : t;
+        const int lane = TILED ? int(threadIdx.x) : j;
+        const int lanes = TILED ? C::THREADS : TPL;
+        LA::fill_table(p.in, tab_in, line, lane, lanes, tc.a0, tc.a1);
+        LA::fill_table(p.out, tab_out, line, lane, lanes, tc.a0, tc.a1);
+        __syncthreads();
+    }
+    const LA in(p.in, tab_in, TILED ? 0 : t, tc.a0, tc.a1, tc.b);
+    const LA out(p.out, tab_out, TILED ? 0 : t, tc.a0, tc.a1, tc.b);
+
+    cx<T> v[E];
+    if (tc.valid) {
+        if (!in.multi) {
+            if constexpr (!TILED) {
+                // contiguous line: sN == 1, immediate offsets
+                const cx<T>* q = in.p0 + j;
+#pragma unroll
+                for (int e = 0; e < E; ++e) v[e] = mem.ld(q + e * TPL);
+            } else {
+                const long long step = (long long)TPL * p.in.sN;
+                const cx<T>* q = in.p0 + (long long)j * p.in.sN;
+#pragma unroll
+                for (int e = 0; e < E; ++e) { v[e] = mem.ld(q); q += step; }
+            }
+        } else {
+#pragma unroll
+            for (int e = 0; e < E; ++e) v[e] = mem.ld(TILED ? in.at(j + e * TPL) : in.at1(j + e * TPL));
+        }
+        if constexpr (INV) {
+#pragma unroll
+            for (int e = 0; e < E; ++e) v[e] = cswap(v[e]);
+        }
+    } else {
+#pragma unroll
+        for (int e = 0; e < E; ++e) v[e] = cx<T>{T(0), T(0)};
+    }
+
+    C::template stages<0>(v, j, t, sm, reinterpret_cast<const cx<T>*>(p.tw));
+
+    if (tc.valid) {
+        if (!out.multi) {
+            if constexpr (!TILED) {
+                cx<T>* q = out.p0 + j;
+#pragma unroll
+                for (int e = 0; e < E; ++e) {
+                    const cx<T> x = v[C::Core::final_slot(e)];
+                    mem.st(q + e * TPL, INV ? cswap(x) : x);
+                }
+            } else {
+                const long long step = (long long)TPL * p.out.sN;
+                cx<T>* q = out.p0 + (long long)j * p.out.sN;
+#pragma unroll
+                for (int e = 0; e < E; ++e) {
+                    const cx<T> x = v[C::Core::final_slot(e)];
+                    mem.st(q, INV ? cswap(x) : x);
+                    q += step;
+                }
+            }
+        } else {
+#pragma unroll
+            for (int e = 0; e < E; ++e) {
+                const cx<T> x = v[C::Core::final_slot(e)];
+                mem.st(TILED ? out.at(j + e * TPL) : out.at1(j + e * TPL), INV ? cswap(x) : x);
+            }
+        }
+    }
+}
+
 // ---- C2C pass ------------------------------------------------------------------------------------------
 // Grid-stride over tiles: launched with one CTA per tile it is the plain kernel; launched with fewer CTAs
 // (FftParams::max_ctas) it is persistent and occupies only that many CTA slots, which is how the overlapped
@@ -292,9 +421,7 @@ template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV>
 __global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
 fft_c2c_kernel(const __grid_constant__ FftParams p) {
     using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
-    using LA = LineAccess<T, C::LINES>;
     using TC = TileCoord<C, TILED, TB>;
-    constexpr int E = C::E, TPL = C::TPL;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
     unsigned long long* tab_in = reinterpret_cast<unsigned long long*>(smem_raw + C::TILE_BYTES);
@@ -304,83 +431,170 @@ fft_c2c_kernel(const __grid_constant__ FftParams p) {
 
 #pragma unroll 1
     for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const TC tc(p, tile);
-        const int j = tc.j, t = tc.t;
-        if (multi) {
-            // TILED: one table per CTA (a0, a1 are CTA-uniform), filled by the first threads;
-            // CONTIG: one table per line, filled by that line's threads.
-            const int line = TILED ? 0 : t;
-            const int lane = TILED ? int(threadIdx.x) : j;
-            const int lanes = TILED ? C::THREADS : TPL;
-            LA::fill_table(p.in, tab_in, line, lane, lanes, tc.a0, tc.a1);
-            LA::fill_table(p.out, tab_out, line, lane, lanes, tc.a0, tc.a1);
-            __syncthreads();
-        }
-        const LA in(p.in, tab_in, TILED ? 0 : t, tc.a0, tc.a1, tc.b);
-        const LA out(p.out, tab_out, TILED ? 0 : t, tc.a0, tc.a1, tc.b);
-
-        cx<T> v[E];
-        if (tc.valid) {
-            if (!in.multi) {
-                if constexpr (!TILED) {
-                    // contiguous line: sN == 1, immediate offsets
-                    const cx<T>* q = in.p0 + j;
-#pragma unroll
-                    for (int e = 0; e < E; ++e) v[e] = ld_elem<T>(q + e * TPL);
-                } else {
-                    const long long step = (long long)TPL * p.in.sN;
-                    const cx<T>* q = in.p0 + (long long)j * p.in.sN;
-#pragma unroll
-                    for (int e = 0; e < E; ++e) { v[e] = ld_elem<T>(q); q += step; }
-                }
-            } else {
-#pragma unroll
-                for (int e = 0; e < E; ++e) v[e] = ld_elem<T>(TILED ? in.at(j + e * TPL) : in.at1(j + e * TPL));
-            }
-            if constexpr (INV) {
-#pragma unroll
-                for (int e = 0; e < E; ++e) v[e] = cswap(v[e]);
-            }
-        } else {
-#pragma unroll
-            for (int e = 0; e < E; ++e) v[e] = cx<T>{T(0), T(0)};
-        }
-
-        C::template stages<0>(v, j, t, sm, reinterpret_cast<const cx<T>*>(p.tw));
-
-        if (tc.valid) {
-            if (!out.multi) {
-                if constexpr (!TILED) {
-                    cx<T>* q = out.p0 + j;
-#pragma unroll
-                    for (int e = 0; e < E; ++e) {
-                        const cx<T> x = v[C::Core::final_slot(e)];
-                        st_elem<T>(q + e * TPL, INV ? cswap(x) : x);
-                    }
-                } else {
-                    const long long step = (long long)TPL * p.out.sN;
-                    cx<T>* q = out.p0 + (long long)j * p.out.sN;
-#pragma unroll
-                    for (int e = 0; e < E; ++e) {
-                        const cx<T> x = v[C::Core::final_slot(e)];
-                        st_elem<T>(q, INV ? cswap(x) : x);
-                        q += step;
-                    }
-                }
-            } else {
-#pragma unroll
-                for (int e = 0; e < E; ++e) {
-                    const cx<T> x = v[C::Core::final_slot(e)];
-                    st_elem<T>(TILED ? out.at(j + e * TPL) : out.at1(j + e * TPL), INV ? cswap(x) : x);
-                }
-            }
-        }
+        c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV>(p, tile, sm, tab_in, tab_out, multi, MemPlain<T>{});
+        const int t = TILED ? int(threadIdx.x) % TB : int(threadIdx.x) / C::TPL;
         if (tile + gridDim.x < ntiles) {
             // persistent use: the next tile's first scatter must not overtake this tile's last gather, and
             // the segment tables are rewritten
             if (multi) __syncthreads();
             else if constexpr (C::NST > 1) C::sync(t);
         }
+    }
+}
+
+// ---- fused z + y stage of one-rank slab transforms ---------------------------------------------------------
+// One persistent launch runs the z pass (CONTIG, `pz`) and the y pass (TILED, `py`) of the same x-planes, plane group
+// by plane group, so that the intermediate one pass writes is still in the L2 when the other reads it (ZyOrder in
+// zy_order.hpp).  Forward: phase A = z lines (caller's input -> intermediate slot), phase B = y tiles (slot -> blocked
+// hand-over of the x pass).  Inverse (INV): phase A = y tiles (blocked hand-over -> slot), phase B = z lines (slot ->
+// caller's output).  Both phases run the per-tile code of fft_c2c_kernel (c2c_tile), so every line is transformed by
+// exactly the arithmetic of the standalone passes; only the CTA shape is shared: TB y columns or TB z lines.
+//
+// L2 policy (per instruction only; no persisting-L2 carve-out, a device-wide setting):
+//   * streaming data — phase A's input, phase B's output — is loaded / stored with L2::evict_first;
+//   * phase A stores the intermediate with L2::evict_last;
+//   * a phase-B CTA discards (discard.global.L2) every 128-byte line of the intermediate it has read, once its tile is
+//     stored: the line is dead and is dropped without a write-back to HBM.  That needs every such line to
+//     be read by one CTA only — 128-byte y-tile rows (TB * sizeof(complex) a multiple of 128) and z lines of a multiple
+//     of 128 bytes, on 128-byte aligned views (ZyFused::discard, checked by the launcher).
+struct ZyFused {
+    unsigned long long* ctr;          // [0] ticket counter, [1 + g] finished phase-A items of group g; never reset
+    unsigned long long ticket_base;   // value of ctr[0] when this launch starts (every launch adds total() + grid)
+    unsigned long long epoch;         // launches of this step so far, this one included
+    int* err;                         // the plan's device error flag
+    long long timeout_cycles;         // clock64 cycles a dependency wait may take (0 = no limit)
+    ZyOrder order;
+    int discard;                      // phase B may discard the intermediate lines it has read
+};
+constexpr int ZY_ERR_TIMEOUT = 200;   // value of the error flag when a fused-stage dependency wait timed out
+
+template <typename T, int LOG2N>
+struct ZyShape {
+    using S = Shape<T, LOG2N>;
+    static constexpr int LOG2E = S::LOG2E, TB = S::TBT;
+    using CY = CtaFft<T, LOG2N, LOG2E, TB, true>;
+    using CZ = CtaFft<T, LOG2N, LOG2E, TB, false>;
+    static constexpr int THREADS = CY::THREADS;
+    static_assert(CZ::THREADS == THREADS, "one CTA shape for both phases");
+    static_assert(CY::NST >= 2 && CZ::NST >= 2, "the discard hook runs after the first exchange through shared memory");
+    static constexpr size_t TILE_BYTES = CY::TILE_BYTES > CZ::TILE_BYTES ? CY::TILE_BYTES : CZ::TILE_BYTES;
+    static constexpr size_t TABLE_BYTES = CY::TABLE_BYTES > CZ::TABLE_BYTES ? CY::TABLE_BYTES : CZ::TABLE_BYTES;
+    static constexpr size_t SMEM_BYTES = TILE_BYTES + TABLE_BYTES + 32;  // + the ticket broadcast
+    // 128-byte lines of the intermediate a phase-B tile owns entirely
+    static constexpr bool Y_DISCARD = (TB * sizeof(cx<T>)) % 128 == 0;
+    static constexpr bool Z_DISCARD = ((1 << LOG2N) * sizeof(cx<T>)) % 128 == 0;
+};
+
+// End of a work item of fft_zy_fused_kernel (all threads, after the tile is stored): a phase-A item counts itself done,
+// a phase-B item drops the intermediate lines it has read.  Kept out of line: the kernel runs at its 128-register limit
+// and this bookkeeping, inlined into the loop, made the register allocator spill the tile's points.
+template <typename T, int LOG2N, bool INV>
+__device__ __noinline__ void zy_item_done(const FftParams& pz, const FftParams& py, const ZyFused& f, long long ticket) {
+    using Z = ZyShape<T, LOG2N>;
+    constexpr int TB = Z::TB, N = 1 << LOG2N;
+    const ZyItem done = f.order.decode(ticket);
+    const int tid = threadIdx.x;
+    if (done.phase == 0) {
+        // release at gpu scope, after the barrier that ordered every thread's stores of the item before this thread
+        if (tid == 0) asm volatile("red.release.gpu.global.add.u64 [%0], 1;" ::"l"(f.ctr + 1 + done.group) : "memory");
+    } else if (f.discard) {
+        // Phase B: the intermediate this tile read is dead — drop its 128-byte lines without a write-back.  Done
+        // here, after the tile, rather than as soon as it is in registers: with the 16 points per thread live the
+        // extra addressing spilled registers, and a line survives the few microseconds of one tile.
+        if (INV) {  // phase B = z lines
+            if constexpr (Z::Z_DISCARD) {
+                constexpr int PER_LINE = int(N * sizeof(cx<T>)) / 128;  // TB lines of this tile
+                for (int k = tid; k < TB * PER_LINE; k += Z::THREADS) {
+                    const long long line = done.tile * TB + k / PER_LINE;
+                    const long long a1 = line % pz.A1, a0 = line / pz.A1;
+                    const char* q = reinterpret_cast<const char*>(reinterpret_cast<const cx<T>*>(pz.in.seg[0].base) + a0 * pz.in.seg[0].sA0 +
+                                                                  a1 * pz.in.seg[0].sA1);
+                    l2_discard(q + (k % PER_LINE) * 128);
+                }
+            }
+        } else {
+            if constexpr (Z::Y_DISCARD) {
+                constexpr int PER_ROW = int(TB * sizeof(cx<T>)) / 128;
+                int bt, a1, a0;
+                tiled_decode<TB>(py, done.tile, bt, a1, a0);
+                const cx<T>* b0 = reinterpret_cast<const cx<T>*>(py.in.seg[0].base) + a0 * py.in.seg[0].sA0 + a1 * py.in.seg[0].sA1 + bt * TB;
+                for (int k = tid; k < N * PER_ROW; k += Z::THREADS)
+                    l2_discard(reinterpret_cast<const char*>(b0 + (long long)(k / PER_ROW) * py.in.sN) + (k % PER_ROW) * 128);
+            }
+        }
+    }
+}
+
+template <typename T, int LOG2N, bool INV>
+__global__ void __launch_bounds__(ZyShape<T, LOG2N>::THREADS, min_ctas_per_sm<T, ZyShape<T, LOG2N>::LOG2E>(ZyShape<T, LOG2N>::THREADS))
+fft_zy_fused_kernel(const __grid_constant__ FftParams pz, const __grid_constant__ FftParams py, const __grid_constant__ ZyFused f) {
+    using Z = ZyShape<T, LOG2N>;
+    constexpr int TB = Z::TB;
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
+    unsigned long long* tab_in = reinterpret_cast<unsigned long long*>(smem_raw + Z::TILE_BYTES);
+    unsigned long long* tab_out = tab_in + (Z::TABLE_BYTES - 16) / 16;
+    volatile long long* bcast = reinterpret_cast<volatile long long*>(smem_raw + Z::TILE_BYTES + Z::TABLE_BYTES);
+    const int tid = threadIdx.x;
+    const long long total = f.order.total();
+
+    // bcast[par]: the current ticket; bcast[par ^ 1]: the next one, drawn while this item runs (the atomic's latency is
+    // hidden behind the tile's loads).  Values are re-read from shared memory where needed instead of being kept in
+    // registers through the tiles.  bcast[2]: give up.
+    int par = 0;
+    if (tid == 0) bcast[0] = (long long)(atomicAdd(f.ctr, 1ull) - f.ticket_base);
+#pragma unroll 1
+    for (;; par ^= 1) {
+        __syncthreads();
+        const long long ticket = bcast[par];
+        if (ticket >= total) break;
+        if (tid == 0) bcast[par ^ 1] = (long long)(atomicAdd(f.ctr, 1ull) - f.ticket_base);
+        const ZyItem it = f.order.decode(ticket);
+        if (it.phase == 1) {
+            // Wait until every phase-A item of this group has finished.  This cannot deadlock: tickets are handed out in
+            // increasing order and only to CTAs that are already running, and every item a ticket depends on has a lower
+            // ticket (zy_order.hpp).  So the lowest unfinished ticket is held by a resident CTA whose earlier item is
+            // finished, and all its dependencies are finished: it completes, and by induction so does every ticket —
+            // with any number of resident CTAs, also when other work on the GPU leaves this launch fewer CTAs than it
+            // asked for.  The wait is still bounded (the plan's rendezvous timeout): a logic error surfaces as an error
+            // code, not a hung GPU.
+            if (tid == 0) {
+                const unsigned long long target = f.epoch * (unsigned long long)f.order.a_items(it.group);
+                const unsigned long long* c = f.ctr + 1 + it.group;
+                unsigned long long v;
+                asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(c) : "memory");
+                long long bail = 0;
+                if (v < target) {
+                    const long long t0 = clock64();
+                    while (true) {
+                        __nanosleep(32);
+                        asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(c) : "memory");
+                        if (v >= target) break;
+                        if (f.timeout_cycles > 0 && clock64() - t0 > f.timeout_cycles) {
+                            atomicExch(f.err, ZY_ERR_TIMEOUT);
+                            bail = 1;
+                            break;
+                        }
+                    }
+                }
+                bcast[2] = bail;
+            }
+            __syncthreads();
+            if (bcast[2]) break;
+        }
+        const bool z_item = (it.phase == 0) == !INV;  // forward: phase A = z; inverse: phase A = y
+        const MemHint<T> mem_a{l2_evict_first(), l2_evict_last()};   // streaming input -> intermediate
+        const MemHint<T> mem_b{l2_evict_normal(), l2_evict_first()};  // intermediate -> streaming output
+        if (z_item) {
+            if (it.phase == 0) c2c_tile<T, LOG2N, Z::LOG2E, TB, false, INV>(pz, it.tile, sm, tab_in, tab_out, false, mem_a);
+            else c2c_tile<T, LOG2N, Z::LOG2E, TB, false, INV>(pz, it.tile, sm, tab_in, tab_out, false, mem_b);
+        } else {
+            if (it.phase == 0) c2c_tile<T, LOG2N, Z::LOG2E, TB, true, INV>(py, it.tile, sm, tab_in, tab_out, false, mem_a);
+            else c2c_tile<T, LOG2N, Z::LOG2E, TB, true, INV>(py, it.tile, sm, tab_in, tab_out, false, mem_b);
+        }
+        // the tile is stored and shared memory is free again before the item counts
+        __syncthreads();
+        zy_item_done<T, LOG2N, INV>(pz, py, f, bcast[par]);
     }
 }
 
@@ -715,6 +929,15 @@ cudaError_t launch_pass(PassKind kind, const FftParams& p, cudaStream_t stream);
 // launch_pass for a runtime size; returns cudaErrorInvalidValue for unsupported lengths.
 cudaError_t launch_pass_f64(int log2n, PassKind kind, const FftParams& p, cudaStream_t stream);
 cudaError_t launch_pass_f32(int log2n, PassKind kind, const FftParams& p, cudaStream_t stream);
+
+// fused z + y stage (fft_zy_fused_kernel), instantiated for the lengths zy_fused_length accepts.  pz: the z pass, py: the y
+// pass, f: counters and plane groups (f.order.na / nb are filled in here).  *tickets: how far the launch advances
+// f.ctr[0] (the next launch's f.ticket_base grows by it).
+template <typename T, int LOG2N>
+cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFused& f, unsigned long long* tickets, cudaStream_t stream);
+cudaError_t launch_zy_fused_f64(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, unsigned long long* tickets, cudaStream_t stream);
+cudaError_t launch_zy_fused_f32(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, unsigned long long* tickets, cudaStream_t stream);
+constexpr bool zy_fused_length(int log2n) { return log2n == 8 || log2n == 9; }
 
 constexpr int MAX_LOG2N = 13;
 
