@@ -228,7 +228,7 @@ struct Step {
     std::vector<int> waits;
     int record = -1;
     // fused z + y stage (fft_zy_fused_kernel): prm is the z pass, prm_y the y pass; zyf holds the counters, advanced by
-    // every launch
+    // every launch on the device
     bool zy = false;
     FftParams prm_y{};
     ZyFused zyf{};
@@ -237,6 +237,9 @@ struct Step {
 struct Schedule {
     std::vector<Step> steps;
     bool built = false;
+    // an eager exec has run this schedule: its tables, counters and kernel attributes are set up, so a stream capture
+    // may record it (dfft_plan_describe builds schedules without running them)
+    bool executed = false;
     bool overlapped = false;  // uses the plan's auxiliary streams
     int nevents = 0;
 };
@@ -1773,14 +1776,19 @@ static int plan_setup_flags(dfft_plan_s* p) {
 // =====================================================================================================
 // execution
 // =====================================================================================================
-static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in, cudaStream_t st) {
+// capture: `st` is capturing into a CUDA graph (one-rank plans only, see exec_common).  Then only the kernels are
+// enqueued: no timer or timeline events, and the plan's record of its last exec (launch count, stream, timer) stays
+// what the last eager exec left.
+static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in, cudaStream_t st, bool capture = false) {
     const int P = p->P, me = p->rank;
     const size_t es = p->esize;
-    p->epoch++;
-    p->last_stream = st;
+    if (!capture) {
+        p->epoch++;
+        p->last_stream = st;
+    }
     int launches = 0;
     int ev = 0;
-    const bool timing = p->timing;
+    const bool timing = p->timing && !capture;
     cudaStream_t const ax0 = p->aux[0], ax1 = p->aux[1];
     cudaStream_t streams[3] = {st, ax0, ax1};
     auto mark = [&](const char* name, int is_fft, const char* label = "") -> cudaError_t {
@@ -1836,11 +1844,7 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
             if (s.out_user == 2) prm.out.seg[0].base = (char*)out + (size_t)s.prm.out.seg[0].base;
             cudaError_t e;
             if (s.zy) {
-                ZyFused f = s.zyf;
-                f.epoch += 1;
-                unsigned long long tickets = 0;
-                e = p->prec == DFFT_F64 ? launch_zy_fused_f64(s.log2n, prm, s.prm_y, f, &tickets, ss) : launch_zy_fused_f32(s.log2n, prm, s.prm_y, f, &tickets, ss);
-                if (e == cudaSuccess) { s.zyf.epoch = f.epoch; s.zyf.ticket_base += tickets; }
+                e = p->prec == DFFT_F64 ? launch_zy_fused_f64(s.log2n, prm, s.prm_y, s.zyf, ss) : launch_zy_fused_f32(s.log2n, prm, s.prm_y, s.zyf, ss);
             } else {
                 e = p->prec == DFFT_F64 ? launch_pass_f64(s.log2n, s.kind, prm, ss) : launch_pass_f32(s.log2n, s.kind, prm, ss);
             }
@@ -1884,9 +1888,11 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
         }
     }
     CK_CUDA(mark("Run complete", -1));
+    if (capture) return DFFT_SUCCESS;
     if (timing) p->n_events_used = ev;
     p->last_launches = launches;
     p->execs++;
+    sc.executed = true;
     return DFFT_SUCCESS;
 }
 
@@ -1927,20 +1933,29 @@ static int exec_common(dfft_plan_t p, void* out, const void* in, int inverse, in
     if (d < 1 || d > 3) return fail(DFFT_ERR_INVALID, "d must be 1, 2 or 3");
     if (!out || !in) return fail(DFFT_ERR_INVALID, "null buffer");
     CK_CUDA(cudaSetDevice(p->comm->device));
+    cudaStream_t st = sync ? p->own_stream : (cudaStream_t)stream;
+    // A stream capture records the kernels into a graph without running them, so nothing may be set up on the way
+    // (allocations, table uploads, kernel attributes): the schedule must have run eagerly before.  Multi-rank plans take
+    // their rendezvous epochs from the host, which a replay would repeat.
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    if (!sync) CK_CUDA(cudaStreamIsCapturing(st, &cap));
+    const bool capture = cap != cudaStreamCaptureStatusNone;
+    if (capture && p->P > 1) return fail(DFFT_ERR_UNSUPPORTED, "capture of multi-rank plans is not supported yet");
+    if (capture && !p->sched[inverse ? 1 : 0][d - 1].executed)
+        return fail(DFFT_ERR_STATE, "run one exec of this direction before capturing it into a CUDA graph");
     Schedule* scp = nullptr;
     {
         int rc = get_schedule(p, inverse, d, &scp);
         if (rc) return rc;
     }
     Schedule& sc = *scp;
-    cudaStream_t st = sync ? p->own_stream : (cudaStream_t)stream;
     if (sync) {
         // explicit edge from the legacy default stream (belt and braces on top of the blocking-stream semantics; it
         // also covers callers whose own streams are blocking streams, which the legacy stream itself waits for)
         CK_CUDA(cudaEventRecord(p->entry_ev, cudaStreamLegacy));
         CK_CUDA(cudaStreamWaitEvent(st, p->entry_ev, 0));
     }
-    int rc = run_schedule(p, sc, out, in, st);
+    int rc = run_schedule(p, sc, out, in, st, capture);
     if (rc) return rc;
     if (!sync) return DFFT_SUCCESS;
     rc = dfft_plan_wait(p);

@@ -25,20 +25,20 @@ cudaError_t launch_pass_f32(int log2n, PassKind kind, const FftParams& p, cudaSt
 }
 
 #define DFFT_ZY_DECL(T, L) \
-    extern template cudaError_t launch_zy_fused<T, L>(const FftParams&, const FftParams&, const ZyFused&, unsigned long long*, cudaStream_t);
+    extern template cudaError_t launch_zy_fused<T, L>(const FftParams&, const FftParams&, const ZyFused&, cudaStream_t);
 DFFT_ZY_DECL(double, 8) DFFT_ZY_DECL(double, 9) DFFT_ZY_DECL(float, 8) DFFT_ZY_DECL(float, 9)
 
-cudaError_t launch_zy_fused_f64(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, unsigned long long* tickets, cudaStream_t stream) {
+cudaError_t launch_zy_fused_f64(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, cudaStream_t stream) {
     switch (log2n) {
-        case 8: return launch_zy_fused<double, 8>(pz, py, f, tickets, stream);
-        case 9: return launch_zy_fused<double, 9>(pz, py, f, tickets, stream);
+        case 8: return launch_zy_fused<double, 8>(pz, py, f, stream);
+        case 9: return launch_zy_fused<double, 9>(pz, py, f, stream);
         default: return cudaErrorInvalidValue;
     }
 }
-cudaError_t launch_zy_fused_f32(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, unsigned long long* tickets, cudaStream_t stream) {
+cudaError_t launch_zy_fused_f32(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, cudaStream_t stream) {
     switch (log2n) {
-        case 8: return launch_zy_fused<float, 8>(pz, py, f, tickets, stream);
-        case 9: return launch_zy_fused<float, 9>(pz, py, f, tickets, stream);
+        case 8: return launch_zy_fused<float, 8>(pz, py, f, stream);
+        case 9: return launch_zy_fused<float, 9>(pz, py, f, stream);
         default: return cudaErrorInvalidValue;
     }
 }

@@ -202,7 +202,7 @@ static bool aligned128(const void* base, long long elems_a, long long elems_b, l
 }
 
 template <typename T, int LOG2N>
-cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFused& f_in, unsigned long long* tickets, cudaStream_t stream) {
+cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFused& f_in, cudaStream_t stream) {
     static_assert(zy_fused_length(LOG2N), "fused z + y stage: length not instantiated");
     using Z = ZyShape<T, LOG2N>;
     constexpr int TB = Z::TB;
@@ -222,7 +222,8 @@ cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFu
     auto ki = fft_zy_fused_kernel<T, LOG2N, true>;
     static cudaError_t once = set_smem(kf, Z::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ki, Z::SMEM_BYTES);
     if (once != cudaSuccess) return once;
-    // persistent: as many CTAs as fit at once (tickets hand out the work; fewer resident CTAs are fine as well)
+    // persistent: as many CTAs as fit at once (tickets hand out the work; fewer resident CTAs are fine as well).  The
+    // grid depends on the work list only, so every launch of a step draws the same number of tickets (zy_launch_of).
     static const int resident = [&] {
         int dev = 0, sms = 0, per = 0;
         cudaGetDevice(&dev);
@@ -231,17 +232,14 @@ cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFu
         return sms * per;
     }();
     const long long total = f.order.total();
-    if (total <= 0) { *tickets = 0; return cudaSuccess; }
+    if (total <= 0) return cudaSuccess;
     const unsigned grid = unsigned(total < resident ? total : resident);
     if (inv) ki<<<grid, Z::THREADS, Z::SMEM_BYTES, stream>>>(pz, py, f);
     else kf<<<grid, Z::THREADS, Z::SMEM_BYTES, stream>>>(pz, py, f);
-    const cudaError_t e = cudaGetLastError();
-    // every ticket below total() is drawn once, and every CTA draws one more, which tells it to stop
-    *tickets = e == cudaSuccess ? (unsigned long long)total + grid : 0;
-    return e;
+    return cudaGetLastError();
 }
 
-template cudaError_t launch_zy_fused<DFFT_T, DFFT_LOG2N>(const FftParams&, const FftParams&, const ZyFused&, unsigned long long*, cudaStream_t);
+template cudaError_t launch_zy_fused<DFFT_T, DFFT_LOG2N>(const FftParams&, const FftParams&, const ZyFused&, cudaStream_t);
 #endif
 
 }  // namespace dfft

@@ -459,8 +459,6 @@ fft_c2c_kernel(const __grid_constant__ FftParams p) {
 //     of 128 bytes, on 128-byte aligned views (ZyFused::discard, checked by the launcher).
 struct ZyFused {
     unsigned long long* ctr;          // [0] ticket counter, [1 + g] finished phase-A items of group g; never reset
-    unsigned long long ticket_base;   // value of ctr[0] when this launch starts (every launch adds total() + grid)
-    unsigned long long epoch;         // launches of this step so far, this one included
     int* err;                         // the plan's device error flag
     long long timeout_cycles;         // clock64 cycles a dependency wait may take (0 = no limit)
     ZyOrder order;
@@ -479,7 +477,7 @@ struct ZyShape {
     static_assert(CY::NST >= 2 && CZ::NST >= 2, "the discard hook runs after the first exchange through shared memory");
     static constexpr size_t TILE_BYTES = CY::TILE_BYTES > CZ::TILE_BYTES ? CY::TILE_BYTES : CZ::TILE_BYTES;
     static constexpr size_t TABLE_BYTES = CY::TABLE_BYTES > CZ::TABLE_BYTES ? CY::TABLE_BYTES : CZ::TABLE_BYTES;
-    static constexpr size_t SMEM_BYTES = TILE_BYTES + TABLE_BYTES + 32;  // + the ticket broadcast
+    static constexpr size_t SMEM_BYTES = TILE_BYTES + TABLE_BYTES + 48;  // + the ticket broadcast
     // 128-byte lines of the intermediate a phase-B tile owns entirely
     static constexpr bool Y_DISCARD = (TB * sizeof(cx<T>)) % 128 == 0;
     static constexpr bool Z_DISCARD = ((1 << LOG2N) * sizeof(cx<T>)) % 128 == 0;
@@ -540,15 +538,22 @@ fft_zy_fused_kernel(const __grid_constant__ FftParams pz, const __grid_constant_
 
     // bcast[par]: the current ticket; bcast[par ^ 1]: the next one, drawn while this item runs (the atomic's latency is
     // hidden behind the tile's loads).  Values are re-read from shared memory where needed instead of being kept in
-    // registers through the tiles.  bcast[2]: give up.
+    // registers through the tiles.  bcast[2]: give up.  bcast[3], bcast[4]: this launch's counter base and epoch, fixed
+    // by the CTA's first draw (zy_launch_of) — the kernel takes no per-exec value from the host, so a graph can replay it.
     int par = 0;
-    if (tid == 0) bcast[0] = (long long)(atomicAdd(f.ctr, 1ull) - f.ticket_base);
+    if (tid == 0) {
+        const unsigned long long raw = atomicAdd(f.ctr, 1ull);
+        const ZyLaunch l = zy_launch_of(raw, f.order.draws(gridDim.x));
+        bcast[3] = (long long)l.base;
+        bcast[4] = (long long)l.epoch;
+        bcast[0] = (long long)(raw - l.base);
+    }
 #pragma unroll 1
     for (;; par ^= 1) {
         __syncthreads();
         const long long ticket = bcast[par];
         if (ticket >= total) break;
-        if (tid == 0) bcast[par ^ 1] = (long long)(atomicAdd(f.ctr, 1ull) - f.ticket_base);
+        if (tid == 0) bcast[par ^ 1] = (long long)(atomicAdd(f.ctr, 1ull) - (unsigned long long)bcast[3]);
         const ZyItem it = f.order.decode(ticket);
         if (it.phase == 1) {
             // Wait until every phase-A item of this group has finished.  This cannot deadlock: tickets are handed out in
@@ -559,7 +564,7 @@ fft_zy_fused_kernel(const __grid_constant__ FftParams pz, const __grid_constant_
             // asked for.  The wait is still bounded (the plan's rendezvous timeout): a logic error surfaces as an error
             // code, not a hung GPU.
             if (tid == 0) {
-                const unsigned long long target = f.epoch * (unsigned long long)f.order.a_items(it.group);
+                const unsigned long long target = (unsigned long long)bcast[4] * (unsigned long long)f.order.a_items(it.group);
                 const unsigned long long* c = f.ctr + 1 + it.group;
                 unsigned long long v;
                 asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(c) : "memory");
@@ -931,12 +936,12 @@ cudaError_t launch_pass_f64(int log2n, PassKind kind, const FftParams& p, cudaSt
 cudaError_t launch_pass_f32(int log2n, PassKind kind, const FftParams& p, cudaStream_t stream);
 
 // fused z + y stage (fft_zy_fused_kernel), instantiated for the lengths zy_fused_length accepts.  pz: the z pass, py: the y
-// pass, f: counters and plane groups (f.order.na / nb are filled in here).  *tickets: how far the launch advances
-// f.ctr[0] (the next launch's f.ticket_base grows by it).
+// pass, f: counters and plane groups (f.order.na / nb are filled in here).  Every launch of one step must use the same
+// counters and the same grid (zy_launch_of), which the launcher's fixed grid for a given work list provides.
 template <typename T, int LOG2N>
-cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFused& f, unsigned long long* tickets, cudaStream_t stream);
-cudaError_t launch_zy_fused_f64(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, unsigned long long* tickets, cudaStream_t stream);
-cudaError_t launch_zy_fused_f32(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, unsigned long long* tickets, cudaStream_t stream);
+cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFused& f, cudaStream_t stream);
+cudaError_t launch_zy_fused_f64(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, cudaStream_t stream);
+cudaError_t launch_zy_fused_f32(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, cudaStream_t stream);
 constexpr bool zy_fused_length(int log2n) { return log2n == 8 || log2n == 9; }
 
 constexpr int MAX_LOG2N = 13;

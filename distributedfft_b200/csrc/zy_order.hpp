@@ -71,6 +71,23 @@ struct ZyOrder {
         const long long tile = (n - L) * fb + t;
         return ZyItem{1, int(tile / fb), tile};
     }
+
+    // Tickets one launch of `grid` CTAs draws from the counter: every ticket below total() once, and one more per CTA,
+    // which tells it to stop.
+    DFFT_ZY_HD unsigned long long draws(unsigned grid) const { return (unsigned long long)total() + grid; }
 };
+
+// Which launch a raw counter value belongs to.  The counter is zeroed once and never reset, and every launch of a step
+// has the same grid, so launch e (from 1) draws exactly the values [(e - 1) * K, e * K) with K = draws(grid), once the
+// launches before it have ended (launches of one step are stream-ordered).  A CTA's first draw therefore fixes the
+// launch's base and epoch without any value from the host, which is what lets a captured graph replay the launch.
+struct ZyLaunch {
+    unsigned long long base;   // counter value of the launch's ticket 0
+    unsigned long long epoch;  // launches of this step so far, this one included
+};
+DFFT_ZY_HD ZyLaunch zy_launch_of(unsigned long long raw, unsigned long long draws_per_launch) {
+    const unsigned long long e = raw / draws_per_launch;
+    return ZyLaunch{e * draws_per_launch, e + 1};
+}
 
 }  // namespace dfft

@@ -140,6 +140,9 @@ class MPIcuFFT:
             raise RuntimeError("plan not initialised (call initFFT)")
 
     def execR2C(self, out, in_, d: int = 3, stream=None):
+        """Real-to-complex transform.  With `stream` the exec is only enqueued there (dfft_exec_r2c_async); such a call may
+        be captured into a CUDA graph (torch.cuda.graph) on one-rank plans once this direction has run eagerly
+        (INTEGRATION.md section 4)."""
         self._need()
         if stream is not None:
             if d != 3:
@@ -150,6 +153,7 @@ class MPIcuFFT:
         return check(lib().dfft_exec_r2c_partial(self._h, _ptr(out), _ptr(in_), d))
 
     def execC2R(self, out, in_, d: int = 3, stream=None):
+        """Complex-to-real transform; `stream` as for execR2C, capturable the same way."""
         self._need()
         if stream is not None:
             if d != 3:
@@ -160,7 +164,8 @@ class MPIcuFFT:
         return check(lib().dfft_exec_c2r_partial(self._h, _ptr(out), _ptr(in_), d))
 
     def execC2C(self, out, in_, direction: int = FORWARD, d: int = 3, stream=None):
-        """Complex transform (not in the reference; BASELINE configs 1-4 need it)."""
+        """Complex transform (not in the reference; BASELINE configs 1-4 need it).  `stream` as for execR2C, capturable
+        the same way."""
         self._need()
         if stream is not None:
             if d != 3:

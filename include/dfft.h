@@ -121,10 +121,24 @@ int dfft_exec_r2c_partial(dfft_plan_t plan, void* out, const void* in, int d);
 int dfft_exec_c2r_partial(dfft_plan_t plan, void* out, const void* in, int d);
 int dfft_exec_c2c_partial(dfft_plan_t plan, void* out, const void* in, int direction, int d);
 
+/* CUDA graphs: an _async call on a stream that is being captured (cudaStreamBeginCapture, torch.cuda.graph) records
+ * the transform's kernels into the graph instead of running them, for plans of one rank:
+ *   - the same direction must have run eagerly on this plan first (the first exec sets up tables and kernel
+ *     attributes, which a capture cannot do); otherwise DFFT_ERR_STATE and nothing is captured;
+ *   - multi-rank plans return DFFT_ERR_UNSUPPORTED and capture nothing;
+ *   - a captured exec records no timer events and leaves the launch count, the phase and step times and the stream
+ *     dfft_plan_wait waits for as the last eager exec left them;
+ *   - the graph replays the buffers it was captured with and stays valid until the plan is destroyed, re-tuned
+ *     (dfft_plan_tune) or given a new work area (dfft_set_work_area);
+ *   - execs of one plan, eager or replayed, must be ordered on the device with respect to each other (one stream, or
+ *     events), as for eager execs alone.
+ * The plain synchronous calls and dfft_plan_tune cannot be captured. */
 int dfft_exec_r2c_async(dfft_plan_t plan, void* out, const void* in, void* stream);
 int dfft_exec_c2r_async(dfft_plan_t plan, void* out, const void* in, void* stream);
 int dfft_exec_c2c_async(dfft_plan_t plan, void* out, const void* in, int direction, void* stream);
-/* Waits for the stream of the last _async call and reports a device-side rendezvous failure, if any. */
+/* Waits for the stream of the last eager _async call and reports a device-side failure (rendezvous or fused-stage
+ * timeout), if any.  After replaying a graph, synchronise the replay stream first; dfft_plan_wait then reports the
+ * errors the replayed kernels recorded. */
 int dfft_plan_wait(dfft_plan_t plan);
 
 /* ---- getters (mpicufft.hpp:65-78, mpicufft_slab.hpp:122-125, mpicufft_pencil.hpp:112-122) ---------- */
@@ -155,7 +169,8 @@ int dfft_layout(int decomp, int transform, size_t nx, size_t ny, size_t nz, size
  * benchmark sweeps (jobs/ ** /benchmarks_base.json).  dfft_plan_tune makes it once, at plan time, like FFTW_MEASURE:
  * it runs the transform on the caller's buffers with the sequential schedule and with overlapped schedules that give the
  * exchanging pass different numbers of CTAs, and keeps the fastest (slowest rank decides).  Collective; `out` is
- * overwritten, `in` is not.  Only plans with send_method Streams have alternatives.  Returns the candidate index. */
+ * overwritten, `in` is not.  Only plans with send_method Streams have alternatives.  Returns the candidate index.
+ * Not capturable: call it before capturing, never on a capturing stream. */
 int dfft_plan_tune(dfft_plan_t plan, void* out, const void* in, int inverse, int reps);
 const char* dfft_plan_tune_report(dfft_plan_t plan);
 
