@@ -46,6 +46,9 @@ SIGNATURES = {
     "dfft_comm_size": (C.c_int, [C.c_void_p]),
     "dfft_plan_create": (C.c_int, [C.c_void_p, C.POINTER(dfft_config), C.c_int, C.c_int, C.c_int, C.c_size_t, C.c_size_t,
                                    C.c_size_t, C.c_size_t, C.c_size_t, C.c_int, C.POINTER(C.c_void_p)]),
+    "dfft_plan_create_batched": (C.c_int, [C.c_void_p, C.POINTER(dfft_config), C.c_int, C.c_int, C.c_int, C.c_size_t, C.c_size_t,
+                                           C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int, C.POINTER(C.c_void_p)]),
+    "dfft_get_batch": (C.c_size_t, [C.c_void_p]),
     "dfft_plan_destroy": (C.c_int, [C.c_void_p]),
     "dfft_set_work_area": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "dfft_exec_r2c": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -232,11 +232,19 @@ struct Step {
     bool zy = false;
     FftParams prm_y{};
     ZyFused zyf{};
+    // batched small cubic fields (fft_batch_small_kernel): one launch for every field; prm.in / prm.out are the caller's
+    // buffers, bsf holds the counters
+    bool batch_small = false;
+    BatchSmall bsf{};
 };
 
 struct Schedule {
     std::vector<Step> steps;
     bool built = false;
+    // batched plans: the steps transform one field and run once per field, the caller's buffers shifted by field_in /
+    // field_out bytes each time — unless whole_batch, where they cover every field at once
+    bool whole_batch = false;
+    size_t field_in = 0, field_out = 0;
     // an eager exec has run this schedule: its tables, counters and kernel attributes are set up, so a stream capture
     // may record it (dfft_plan_describe builds schedules without running them)
     bool executed = false;
@@ -254,6 +262,7 @@ struct dfft_plan_s {
     int prec = DFFT_F64;
     size_t esize = 16;  // bytes per complex element
     int rank = 0, P = 1;
+    size_t batch = 1;         // fields per exec, back to back in every caller buffer (dfft_plan_create_batched)
     size_t domain_bytes = 0;  // this rank (getDomainSize)
     size_t slot_bytes = 0;    // uniform over ranks
     int nslots = 2;
@@ -419,6 +428,56 @@ static int fuse_zy(dfft_plan_s* p, Step zs, const Step& ys, const char* label, c
         if (cudaMemset(c, 0, bytes) != cudaSuccess) return fail(DFFT_ERR_CUDA, "fused z + y stage: counter initialisation failed");
         out.zyf.ctr = reinterpret_cast<unsigned long long*>(c);
     }
+    return DFFT_SUCCESS;
+}
+
+// Whether a batched exec runs as one launch of fft_batch_small_kernel: one-rank slab C2C plans of the full 3D transform
+// of cubic fields of an instantiated length (batch_small_length), from BATCH_SMALL_MIN fields on.  Decided from the
+// length, the precision and the batch only; every other batched plan runs its per-field schedule once per field.
+constexpr size_t BATCH_SMALL_MIN = 2;
+static bool batch_small(const dfft_plan_s* p, int d) {
+    const Geometry& g = p->g;
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3) return false;
+    if (g.nx != g.ny || g.ny != g.nz || !batch_small_length(ilog2_exact(g.nx))) return false;
+    return p->batch >= BATCH_SMALL_MIN && p->batch * g.nx <= 0x7fffffff;
+}
+
+static int build_batch_small(dfft_plan_s* p, int inverse, Schedule& sc) {
+    const size_t N = p->g.nx;
+    sc.steps.clear();
+    sc.whole_batch = true;
+    Step s;
+    s.type = STEP_PASS;
+    s.batch_small = true;
+    s.label = "batched pass";
+    s.phase = inverse ? "2D FFT Y-Z-Direction" : "1D FFT X-Direction";  // the exec's last section
+    s.kind = PASS_C2C_CONTIG;
+    s.log2n = ilog2_exact(N);
+    s.prm.inverse = inverse;
+    void* tw = nullptr;
+    if (p->tabs.get_tw(s.log2n, &tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
+    s.prm.tw = tw;
+    s.prm.in = single_view(nullptr, 0, 0, 1);
+    s.prm.out = single_view(nullptr, 0, 0, 1);
+    s.in_user = 1;
+    s.out_user = 2;
+    s.bsf.tw = tw;
+    s.bsf.err = p->err_d;
+    s.bsf.timeout_cycles = p->rendezvous_timeout_cycles;
+    // look-ahead in fields: phase A runs L fields ahead of phase B, L + 1 fields of intermediate in flight, a third of the
+    // L2 (the rule of the fused z + y stage, with a field in place of a plane)
+    const long long ahead = (long long)(p->l2_bytes / (3 * N * N * N * p->esize)) - 1;
+    s.bsf.order.ahead = int(ahead < 1 ? 1 : ahead);
+    if (!p->tabs.dry) {
+        const size_t bytes = sizeof(unsigned long long) * (1 + p->batch);
+        void* c = nullptr;
+        if (cudaMalloc(&c, bytes) != cudaSuccess) return fail(DFFT_ERR_CUDA, "batched stage: counter allocation failed");
+        p->tabs.bytes.push_back(c);  // freed with the schedules
+        if (cudaMemset(c, 0, bytes) != cudaSuccess) return fail(DFFT_ERR_CUDA, "batched stage: counter initialisation failed");
+        s.bsf.ctr = reinterpret_cast<unsigned long long*>(c);
+    }
+    sc.steps.push_back(s);
+    sc.built = true;
     return DFFT_SUCCESS;
 }
 
@@ -1779,7 +1838,8 @@ static int plan_setup_flags(dfft_plan_s* p) {
 // capture: `st` is capturing into a CUDA graph (one-rank plans only, see exec_common).  Then only the kernels are
 // enqueued: no timer or timeline events, and the plan's record of its last exec (launch count, stream, timer) stays
 // what the last eager exec left.
-static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in, cudaStream_t st, bool capture = false) {
+// nfields: fields of a batched plan to transform (0 = all of them; dfft_plan_tune measures field 0 only).
+static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in, cudaStream_t st, bool capture = false, size_t nfields = 0) {
     const int P = p->P, me = p->rank;
     const size_t es = p->esize;
     if (!capture) {
@@ -1807,15 +1867,28 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
         p->ev_labels[ev] = label;
         return cudaEventRecord(p->events[ev++], st);
     };
+    // overlapped schedules: the auxiliary streams fork from the caller's stream before a field and join it after
+    auto fork = [&]() -> cudaError_t {
+        cudaError_t e = cudaEventRecord(p->fork_ev, st);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(ax0, p->fork_ev, 0);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(ax1, p->fork_ev, 0);
+        return e;
+    };
+    auto join = [&]() -> cudaError_t {
+        cudaError_t e = cudaSuccess;
+        for (int a = 0; a < 2 && e == cudaSuccess; ++a) {
+            e = cudaEventRecord(p->join_ev[a], a == 0 ? ax0 : ax1);
+            if (e == cudaSuccess) e = cudaStreamWaitEvent(st, p->join_ev[a], 0);
+        }
+        return e;
+    };
     if (sc.overlapped) {
         while (int(p->sync_events.size()) < sc.nevents) {
             cudaEvent_t e;
             CK_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
             p->sync_events.push_back(e);
         }
-        CK_CUDA(cudaEventRecord(p->fork_ev, st));
-        CK_CUDA(cudaStreamWaitEvent(ax0, p->fork_ev, 0));
-        CK_CUDA(cudaStreamWaitEvent(ax1, p->fork_ev, 0));
+        CK_CUDA(fork());
     }
     CK_CUDA(mark("start", -1));
     int tl = 0;
@@ -1833,60 +1906,68 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
         p->tl_streams[tl] = stream_id;
         return cudaEventRecord(p->tl_events[tl++], ss_);
     };
-    for (Step& s : sc.steps) {
-        cudaStream_t ss = streams[s.stream];
-        for (int w : s.waits) CK_CUDA(cudaStreamWaitEvent(ss, p->sync_events[w], 0));
-        CK_CUDA(tl_mark(ss, s.label, s.stream));
-        if (s.type == STEP_PASS) {
-            FftParams prm = s.prm;
-            // views on the caller's buffers store a byte offset in seg[0].base
-            if (s.in_user == 1) prm.in.seg[0].base = (char*)const_cast<void*>(in) + (size_t)s.prm.in.seg[0].base;
-            if (s.out_user == 2) prm.out.seg[0].base = (char*)out + (size_t)s.prm.out.seg[0].base;
-            cudaError_t e;
-            if (s.zy) {
-                e = p->prec == DFFT_F64 ? launch_zy_fused_f64(s.log2n, prm, s.prm_y, s.zyf, ss) : launch_zy_fused_f32(s.log2n, prm, s.prm_y, s.zyf, ss);
-            } else {
-                e = p->prec == DFFT_F64 ? launch_pass_f64(s.log2n, s.kind, prm, ss) : launch_pass_f32(s.log2n, s.kind, prm, ss);
-            }
-            if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("FFT pass launch failed: ") + cudaGetErrorString(e));
-            ++launches;
-            CK_CUDA(mark(s.phase, 1, s.label));
-        } else if (s.type == STEP_RENDEZVOUS) {
-            const std::vector<int>& G = p->grp[s.group];
-            if (G.size() > 1) {
-                const unsigned long long ticket = ++p->ticket[s.phase_id];
-                rendezvous_kernel<<<1, 32 * int((G.size() + 31) / 32), 0, ss>>>(p->peer_flags_d, p->flags, p->groups_d + s.group * P, int(G.size()), me, P,
-                                                                              s.phase_id, ticket, p->err_d, p->rendezvous_timeout_cycles);
-                CK_CUDA(cudaGetLastError());
-                ++launches;
-            }
-            CK_CUDA(mark(s.phase, 0, s.label));
-        } else {
-            const std::vector<int>& G = p->grp[s.group];
-            char* sb = (char*)p->slot_ptr[s.send_slot][me];
-            char* rb = (char*)p->slot_ptr[s.recv_slot][me];
-            CK_NCCL(ncclGroupStart());
-            for (size_t q = 0; q < G.size(); ++q) {
-                if (G[q] == me) continue;
-                if (s.scount[q]) CK_NCCL(ncclSend(sb + s.soff[q] * es, s.scount[q] * es, ncclChar, G[q], p->comm->nccl, ss));
-                if (s.rcount[q]) CK_NCCL(ncclRecv(rb + s.roff[q] * es, s.rcount[q] * es, ncclChar, G[q], p->comm->nccl, ss));
-            }
-            CK_NCCL(ncclGroupEnd());
-            for (size_t q = 0; q < G.size(); ++q)
-                if (G[q] == me && s.scount[q])
-                    CK_CUDA(cudaMemcpyAsync(rb + s.roff[q] * es, sb + s.soff[q] * es, s.scount[q] * es, cudaMemcpyDeviceToDevice, ss));
-            CK_CUDA(mark(s.phase, 0, s.label));
+    const size_t fields = sc.whole_batch ? 1 : (nfields ? nfields : p->batch);
+    for (size_t f = 0; f < fields; ++f) {
+        // batched plans: the phase times mark the section ends of the last field; the step list covers every field
+        const bool last = f + 1 == fields;
+        if (f > 0 && sc.overlapped) {
+            CK_CUDA(join());
+            CK_CUDA(fork());
         }
-        CK_CUDA(tl_mark(ss, s.label, s.stream));
-        if (s.record >= 0) CK_CUDA(cudaEventRecord(p->sync_events[s.record], ss));
+        for (Step& s : sc.steps) {
+            cudaStream_t ss = streams[s.stream];
+            for (int w : s.waits) CK_CUDA(cudaStreamWaitEvent(ss, p->sync_events[w], 0));
+            CK_CUDA(tl_mark(ss, s.label, s.stream));
+            const char* phase = last ? s.phase : nullptr;
+            if (s.type == STEP_PASS) {
+                FftParams prm = s.prm;
+                // views on the caller's buffers store a byte offset in seg[0].base (field f starts f field sizes further)
+                if (s.in_user == 1) prm.in.seg[0].base = (char*)const_cast<void*>(in) + f * sc.field_in + (size_t)s.prm.in.seg[0].base;
+                if (s.out_user == 2) prm.out.seg[0].base = (char*)out + f * sc.field_out + (size_t)s.prm.out.seg[0].base;
+                cudaError_t e;
+                if (s.batch_small) {
+                    e = p->prec == DFFT_F64 ? launch_batch_small_f64(s.log2n, prm.in.seg[0].base, prm.out.seg[0].base, (long long)p->batch, s.prm.inverse, s.bsf, ss)
+                                            : launch_batch_small_f32(s.log2n, prm.in.seg[0].base, prm.out.seg[0].base, (long long)p->batch, s.prm.inverse, s.bsf, ss);
+                } else if (s.zy) {
+                    e = p->prec == DFFT_F64 ? launch_zy_fused_f64(s.log2n, prm, s.prm_y, s.zyf, ss) : launch_zy_fused_f32(s.log2n, prm, s.prm_y, s.zyf, ss);
+                } else {
+                    e = p->prec == DFFT_F64 ? launch_pass_f64(s.log2n, s.kind, prm, ss) : launch_pass_f32(s.log2n, s.kind, prm, ss);
+                }
+                if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("FFT pass launch failed: ") + cudaGetErrorString(e));
+                ++launches;
+                CK_CUDA(mark(phase, 1, s.label));
+            } else if (s.type == STEP_RENDEZVOUS) {
+                const std::vector<int>& G = p->grp[s.group];
+                if (G.size() > 1) {
+                    const unsigned long long ticket = ++p->ticket[s.phase_id];
+                    rendezvous_kernel<<<1, 32 * int((G.size() + 31) / 32), 0, ss>>>(p->peer_flags_d, p->flags, p->groups_d + s.group * P, int(G.size()), me, P,
+                                                                                  s.phase_id, ticket, p->err_d, p->rendezvous_timeout_cycles);
+                    CK_CUDA(cudaGetLastError());
+                    ++launches;
+                }
+                CK_CUDA(mark(phase, 0, s.label));
+            } else {
+                const std::vector<int>& G = p->grp[s.group];
+                char* sb = (char*)p->slot_ptr[s.send_slot][me];
+                char* rb = (char*)p->slot_ptr[s.recv_slot][me];
+                CK_NCCL(ncclGroupStart());
+                for (size_t q = 0; q < G.size(); ++q) {
+                    if (G[q] == me) continue;
+                    if (s.scount[q]) CK_NCCL(ncclSend(sb + s.soff[q] * es, s.scount[q] * es, ncclChar, G[q], p->comm->nccl, ss));
+                    if (s.rcount[q]) CK_NCCL(ncclRecv(rb + s.roff[q] * es, s.rcount[q] * es, ncclChar, G[q], p->comm->nccl, ss));
+                }
+                CK_NCCL(ncclGroupEnd());
+                for (size_t q = 0; q < G.size(); ++q)
+                    if (G[q] == me && s.scount[q])
+                        CK_CUDA(cudaMemcpyAsync(rb + s.roff[q] * es, sb + s.soff[q] * es, s.scount[q] * es, cudaMemcpyDeviceToDevice, ss));
+                CK_CUDA(mark(phase, 0, s.label));
+            }
+            CK_CUDA(tl_mark(ss, s.label, s.stream));
+            if (s.record >= 0) CK_CUDA(cudaEventRecord(p->sync_events[s.record], ss));
+        }
     }
     if (timing) p->tl_used = tl;
-    if (sc.overlapped) {
-        for (int a = 0; a < 2; ++a) {
-            CK_CUDA(cudaEventRecord(p->join_ev[a], a == 0 ? ax0 : ax1));
-            CK_CUDA(cudaStreamWaitEvent(st, p->join_ev[a], 0));
-        }
-    }
+    if (sc.overlapped) CK_CUDA(join());
     CK_CUDA(mark("Run complete", -1));
     if (capture) return DFFT_SUCCESS;
     if (timing) p->n_events_used = ev;
@@ -1894,6 +1975,19 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
     p->execs++;
     sc.executed = true;
     return DFFT_SUCCESS;
+}
+
+// Bytes of one field in the caller's `in` and `out` of an exec (direction, d): the product of that buffer's layout, in
+// reals for the real side of R2C / C2R.  No schedule touches a caller buffer beyond it (tests/test_batch.py checks every
+// step's accesses), so fields sit back to back at this distance.
+static void field_bytes(const dfft_plan_s* p, int inverse, int d, size_t* in_b, size_t* out_b) {
+    size_t s0[3], sd[3], o[3];
+    p->g.layout(p->rank, 0, s0, o);
+    p->g.layout(p->rank, d, sd, o);
+    const size_t real_es = p->g.transform == DFFT_C2C ? p->esize : p->esize / 2;
+    const size_t b0 = s0[0] * s0[1] * s0[2] * real_es, bd = sd[0] * sd[1] * sd[2] * p->esize;
+    *in_b = inverse ? bd : b0;
+    *out_b = inverse ? b0 : bd;
 }
 
 // The one place that decides which schedule a (direction, d) pair runs — used by exec and by dfft_plan_describe, so
@@ -1912,10 +2006,12 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
         const bool want_pencil_overlap = streams && d == 3 && p->g.decomp == DFFT_PENCIL && p->direct1 && p->direct2 && p->P > 1 && p->xchg_ctas >= 0 &&
                                          pencil_overlap_enabled() && !seq_won && ((both_multi && !inverse) || tuned || pencil_overlap_mode() == 2);
         int rc;
-        if (want_overlap) rc = build_overlapped_slab(p, inverse ? 1 : 0, sc);
+        if (batch_small(p, d)) rc = build_batch_small(p, inverse ? 1 : 0, sc);
+        else if (want_overlap) rc = build_overlapped_slab(p, inverse ? 1 : 0, sc);
         else if (want_pencil_overlap) rc = build_overlapped_pencil(p, inverse ? 1 : 0, sc);
         else rc = build_schedule(p, inverse ? 1 : 0, d, sc);
         if (rc) return rc;
+        field_bytes(p, inverse, d, &sc.field_in, &sc.field_out);
         if (g_view_error) return fail(DFFT_ERR_STATE, "internal: segments of one view disagree on the axis stride");
     }
     *out = &sc;
@@ -2130,7 +2226,13 @@ int dfft_layout(int decomp, int transform, size_t nx, size_t ny, size_t nz, size
 
 int dfft_plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
                      size_t nz, size_t p1, size_t p2, int allocate, dfft_plan_t* plan) {
+    return dfft_plan_create_batched(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, 1, allocate, plan);
+}
+
+int dfft_plan_create_batched(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
+                             size_t nz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan) {
     if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
+    if (batch == 0) return fail(DFFT_ERR_INVALID, "batch must be at least 1");
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
     if (transform != DFFT_R2C && transform != DFFT_C2C) return fail(DFFT_ERR_INVALID, "bad transform");
     const bool dry = comm->dry;
@@ -2164,6 +2266,20 @@ int dfft_plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, in
     if (g.sx.size.back() == 0 || g.sy.size.back() == 0 || g.sz.size.back() == 0 || g.oy.size.back() == 0) {
         delete p;
         return fail(DFFT_ERR_INVALID, "partition leaves a rank without data");
+    }
+    {   // the whole batch of every caller buffer (any direction, any partial d) must be addressable
+        size_t widest = 0;
+        for (int d = 1; d <= 3; ++d) {
+            size_t bi = 0, bo = 0;
+            field_bytes(p, 0, d, &bi, &bo);
+            widest = std::max(widest, std::max(bi, bo));
+        }
+        if (batch > SIZE_MAX / widest) {
+            delete p;
+            return fail(DFFT_ERR_INVALID, "batch of " + std::to_string(batch) + " fields of " + std::to_string(widest) +
+                                              " bytes overflows the address range (size_t)");
+        }
+        p->batch = batch;
     }
     // groups
     const int me = p->rank, P = p->P;
@@ -2359,6 +2475,9 @@ int dfft_plan_wait(dfft_plan_t p) {
         if (err == ZY_ERR_TIMEOUT)
             return fail(DFFT_ERR_TIMEOUT, "fused z + y stage: a wait for the other phase timed out (DFFT_RENDEZVOUS_TIMEOUT_S); results are "
                                           "invalid and the plan must be destroyed");
+        if (err == BATCH_ERR_TIMEOUT)
+            return fail(DFFT_ERR_TIMEOUT, "batched stage: a wait for the other phase timed out (DFFT_RENDEZVOUS_TIMEOUT_S); results are "
+                                          "invalid and the plan must be destroyed");
         if (err >= 100)
             return fail(DFFT_ERR_TIMEOUT, "a peer rank gave up waiting at a device rendezvous (phase " + std::to_string(err - 100) +
                                               "); results are invalid and the plan must be destroyed");
@@ -2391,6 +2510,7 @@ int dfft_get_partial_start(dfft_plan_t p, int d, size_t start[3]) {
     return layout_of(p, d, nullptr, start);
 }
 size_t dfft_get_domain_size(dfft_plan_t p) { return p ? p->domain_bytes : 0; }
+size_t dfft_get_batch(dfft_plan_t p) { return p ? p->batch : 0; }
 size_t dfft_get_work_size_device(dfft_plan_t p) { return p ? p->work_bytes : 0; }
 size_t dfft_get_work_size_host(dfft_plan_t) { return 0; }
 void* dfft_get_work_area_device(dfft_plan_t p) { return p ? p->work : nullptr; }
@@ -2557,7 +2677,7 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
         if (rc) continue;  // a candidate this geometry cannot build: skip it (every rank takes the same branch)
         for (int it = 0; it < reps + 1; ++it) {
             if (it == 1) CK_CUDA(cudaEventRecord(e0, p->own_stream));
-            rc = run_schedule(p, *sc, out, in, p->own_stream);
+            rc = run_schedule(p, *sc, out, in, p->own_stream, false, 1);  // batched plans: field 0
             if (rc) return rc;
         }
         CK_CUDA(cudaEventRecord(e1, p->own_stream));
@@ -2630,7 +2750,11 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
         if (rc) return rc;
     }
     Schedule& sc = *scp;
-    std::string o = "{\"rank\":" + std::to_string(p->rank) + ",\"esize\":" + std::to_string(p->esize) + ",\"slot_bytes\":" + std::to_string(p->slot_bytes) +
+    std::string o = "{\"rank\":" + std::to_string(p->rank) + ",\"esize\":" + std::to_string(p->esize) +
+                    (p->batch > 1 ? ",\"batch\":" + std::to_string(p->batch) + ",\"field_in\":" + std::to_string(sc.field_in) +
+                                        ",\"field_out\":" + std::to_string(sc.field_out)
+                                  : std::string()) +
+                    ",\"slot_bytes\":" + std::to_string(p->slot_bytes) +
                     ",\"nslots\":" + std::to_string(p->nslots) + ",\"overlapped\":" + (sc.overlapped ? "true" : "false") + ",\"slots\":[";
     for (int s_ = 0; s_ < p->nslots; ++s_) {
         if (s_) o += ",";
@@ -2654,11 +2778,77 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
         if (inv) { listed.push_back(y); listed.push_back(z); }
         else { listed.push_back(z); listed.push_back(y); }
     }
-    for (const Step& s_ : listed) {
+    // Batched plans: the batched stage is listed as its three single-segment views over all fields (in_user 2: it reads
+    // the caller's `out`); a per-field schedule is listed once per field, with the caller's buffers shifted to the field
+    // and the field in "field".  Between fields an overlapped schedule joins its streams into the caller's and forks
+    // them again: the last step of each stream records an event that the first step of every stream of the next field
+    // waits for.
+    std::vector<long long> field_of(listed.size(), 0);
+    if (sc.whole_batch) {
+        std::vector<Step> all;
+        for (const Step& s_ : listed) {
+            if (!s_.batch_small) { all.push_back(s_); continue; }
+            const long long N = (long long)p->g.nx, N2 = N * N, N3 = N2 * N, B = (long long)p->batch;
+            Step z = s_, y = s_, x = s_;
+            z.batch_small = y.batch_small = x.batch_small = false;
+            z.kind = PASS_C2C_CONTIG; z.label = "batched pass: z lines";
+            z.prm.A0 = int(B * N); z.prm.A1 = int(N); z.prm.B = 1;
+            z.prm.in = z.prm.out = single_view(nullptr, N2, N, 1);
+            y.kind = PASS_C2C_TILED; y.label = "batched pass: y lines";
+            y.prm.A0 = int(B * N); y.prm.A1 = 1; y.prm.B = int(N);
+            y.prm.in = y.prm.out = single_view(nullptr, N2, 0, N);
+            x.kind = PASS_C2C_TILED; x.label = "batched pass: x lines";
+            x.prm.A0 = int(B); x.prm.A1 = 1; x.prm.B = int(N2);
+            x.prm.in = x.prm.out = single_view(nullptr, N3, 0, N2);
+            const bool inv = s_.prm.inverse != 0;
+            Step* order[3] = {&z, &y, &x};
+            if (inv) std::swap(order[0], order[2]);
+            for (int k = 0; k < 3; ++k) {
+                order[k]->in_user = k == 0 ? 1 : 2;
+                order[k]->out_user = 2;
+                all.push_back(*order[k]);
+            }
+        }
+        listed.swap(all);
+        field_of.assign(listed.size(), -1);
+    } else if (p->batch > 1) {
+        const size_t per = listed.size();
+        std::vector<Step> all;
+        field_of.clear();
+        int join_ev[3] = {-1, -1, -1};
+        for (size_t f = 0; f < p->batch; ++f) {
+            bool seen[3] = {false, false, false};
+            for (size_t k = 0; k < per; ++k) {
+                Step s_ = listed[k];
+                if (s_.type == STEP_PASS) {
+                    if (s_.in_user == 1) s_.prm.in.seg[0].base = (char*)s_.prm.in.seg[0].base + f * sc.field_in;
+                    if (s_.out_user == 2) s_.prm.out.seg[0].base = (char*)s_.prm.out.seg[0].base + f * sc.field_out;
+                }
+                if (sc.overlapped && f > 0 && !seen[s_.stream])
+                    for (int e : join_ev) if (e >= 0) s_.waits.push_back(e);
+                seen[s_.stream] = true;
+                all.push_back(s_);
+                field_of.push_back((long long)f);
+            }
+            if (!sc.overlapped) continue;
+            for (int st_ = 0; st_ < 3; ++st_) {
+                join_ev[st_] = -1;
+                for (size_t k = all.size(); k-- > all.size() - per;) {
+                    if (all[k].stream != st_) continue;
+                    if (all[k].record < 0) all[k].record = sc.nevents + st_;
+                    join_ev[st_] = all[k].record;
+                    break;
+                }
+            }
+        }
+        listed.swap(all);
+    }
+    for (size_t i = 0; i < listed.size(); ++i) {
+        const Step& s_ = listed[i];
         if (!first) o += ",";
         first = false;
         o += "{\"type\":" + std::to_string(int(s_.type)) + ",\"label\":\"" + s_.label + "\",\"stream\":" + std::to_string(s_.stream) +
-             ",\"record\":" + std::to_string(s_.record) + ",\"waits\":[";
+             (p->batch > 1 ? ",\"field\":" + std::to_string(field_of[i]) : std::string()) + ",\"record\":" + std::to_string(s_.record) + ",\"waits\":[";
         for (size_t w = 0; w < s_.waits.size(); ++w) o += (w ? "," : "") + std::to_string(s_.waits[w]);
         o += "]";
         if (s_.type == STEP_PASS) {

@@ -43,4 +43,23 @@ cudaError_t launch_zy_fused_f32(int log2n, const FftParams& pz, const FftParams&
     }
 }
 
+#define DFFT_BATCH_DECL(T, L) \
+    extern template cudaError_t launch_batch_small<T, L>(const void*, void*, long long, int, const BatchSmall&, cudaStream_t);
+DFFT_BATCH_DECL(double, 5) DFFT_BATCH_DECL(double, 6) DFFT_BATCH_DECL(float, 5) DFFT_BATCH_DECL(float, 6)
+
+cudaError_t launch_batch_small_f64(int log2n, const void* in, void* out, long long batch, int inverse, const BatchSmall& f, cudaStream_t stream) {
+    switch (log2n) {
+        case 5: return launch_batch_small<double, 5>(in, out, batch, inverse, f, stream);
+        case 6: return launch_batch_small<double, 6>(in, out, batch, inverse, f, stream);
+        default: return cudaErrorInvalidValue;
+    }
+}
+cudaError_t launch_batch_small_f32(int log2n, const void* in, void* out, long long batch, int inverse, const BatchSmall& f, cudaStream_t stream) {
+    switch (log2n) {
+        case 5: return launch_batch_small<float, 5>(in, out, batch, inverse, f, stream);
+        case 6: return launch_batch_small<float, 6>(in, out, batch, inverse, f, stream);
+        default: return cudaErrorInvalidValue;
+    }
+}
+
 }  // namespace dfft

@@ -242,4 +242,52 @@ cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFu
 template cudaError_t launch_zy_fused<DFFT_T, DFFT_LOG2N>(const FftParams&, const FftParams&, const ZyFused&, cudaStream_t);
 #endif
 
+#if DFFT_LOG2N == 5 || DFFT_LOG2N == 6
+template <typename T, int LOG2N>
+cudaError_t launch_batch_small(const void* in, void* out, long long batch, int inverse, const BatchSmall& f_in, cudaStream_t stream) {
+    static_assert(batch_small_length(LOG2N), "batched small fields: length not instantiated");
+    using BS = BatchShape<T, LOG2N>;
+    constexpr long long N = BS::N, N2 = N * N, N3 = N2 * N;
+    if (batch < 1 || batch * N > 0x7fffffffLL || f_in.order.ahead < 1 || !f_in.ctr) return cudaErrorInvalidValue;
+    BatchSmall f = f_in;
+    const int items = int(N3 / BS::POINTS);  // plane items = slice items per field
+    f.order.nx = int(batch);
+    f.order.gpp = 1;
+    f.order.na = items;
+    f.order.nb = items;
+    f.plane_in = inverse ? out : in;
+    f.plane_out = out;
+    FftParams px{};
+    px.A0 = int(batch); px.A1 = 1; px.B = int(N2);
+    px.inverse = inverse;
+    px.tw = f.tw;
+    for (View* v : {&px.in, &px.out}) {
+        v->nseg = 1;
+        v->sN = N2;
+        v->seg[0].sA0 = N3;
+    }
+    px.in.seg[0].base = inverse ? const_cast<void*>(in) : out;
+    px.out.seg[0].base = out;
+    auto kf = fft_batch_small_kernel<T, LOG2N, false>;
+    auto ki = fft_batch_small_kernel<T, LOG2N, true>;
+    static cudaError_t once = set_smem(kf, BS::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ki, BS::SMEM_BYTES);
+    if (once != cudaSuccess) return once;
+    // persistent, as many CTAs as fit at once; the grid depends on the batch only (zy_launch_of)
+    static const int resident = [&] {
+        int dev = 0, sms = 0, per = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kf, BS::THREADS, BS::SMEM_BYTES) != cudaSuccess || per < 1) per = 1;
+        return sms * per;
+    }();
+    const long long total = f.order.total();
+    const unsigned grid = unsigned(total < resident ? total : resident);
+    if (inverse) ki<<<grid, BS::THREADS, BS::SMEM_BYTES, stream>>>(px, f);
+    else kf<<<grid, BS::THREADS, BS::SMEM_BYTES, stream>>>(px, f);
+    return cudaGetLastError();
+}
+
+template cudaError_t launch_batch_small<DFFT_T, DFFT_LOG2N>(const void*, void*, long long, int, const BatchSmall&, cudaStream_t);
+#endif
+
 }  // namespace dfft

@@ -603,6 +603,172 @@ fft_zy_fused_kernel(const __grid_constant__ FftParams pz, const __grid_constant_
     }
 }
 
+// ---- batches of small cubic fields: one persistent launch per exec ------------------------------------------
+// A batch of B fields of N^3 points (N = 32, 64), back to back, transformed in one launch as two phases per field:
+//   plane items: the z lines and the y columns of PPI consecutive x-planes (4096 points), staged through shared memory
+//                between the two axes;
+//   slice items: the x lines of TB consecutive (y, z) columns (4096 points, rows N^2 apart), fft_c2c_kernel's tile code.
+// Forward: phase A = plane items (caller's in -> caller's out), phase B = slice items (out -> out, in place).  Inverse, in
+// the order of the unbatched plan (x, then y, then z): phase A = slice items (in -> out), phase B = plane items (out -> out,
+// in place).  A phase-B item of field f needs every phase-A item of f; the work list is ZyOrder with one group per field,
+// so every dependency has a lower ticket (zy_order.hpp) and the wait below is the one of fft_zy_fused_kernel.  Each line
+// runs FftCore<T, LOG2N, Shape::LOG2E> with the plan's twiddle table, as in the standalone passes: bit-identical results.
+// L2 policy as in the fused z + y stage: phase A loads with evict_first and stores the intermediate with evict_last,
+// phase B stores with evict_first; a field is read from HBM once and written once.
+struct BatchSmall {
+    unsigned long long* ctr;   // [0] ticket counter, [1 + f] finished phase-A items of field f; zeroed once, never reset
+    int* err;                  // the plan's device error flag
+    long long timeout_cycles;  // clock64 cycles a dependency wait may take (0 = no limit)
+    ZyOrder order;             // nx = fields, gpp = 1, na / nb items per field (filled in by the launcher), look-ahead in fields
+    const void* plane_in;      // plane items read here and write plane_out
+    void* plane_out;
+    const void* tw;            // exp(-2 pi i m / N), the plan's table
+};
+constexpr int BATCH_ERR_TIMEOUT = 201;  // value of the error flag when a batched-stage dependency wait timed out
+
+template <typename T, int LOG2N>
+struct BatchShape {
+    static constexpr int LOG2E = Shape<T, LOG2N>::LOG2E, N = 1 << LOG2N, TPL = N >> LOG2E;
+    static constexpr int POINTS = 4096;            // points of one work item
+    static constexpr int THREADS = POINTS >> LOG2E;
+    static constexpr int PPI = POINTS / (N * N);   // x-planes of a plane item
+    static constexpr int TB = POINTS / N;          // z lines / y columns of a plane item, x columns of a slice item
+    using CZ = CtaFft<T, LOG2N, LOG2E, TB, false>;
+    using CY = CtaFft<T, LOG2N, LOG2E, TB, true>;
+    static_assert(CZ::THREADS == THREADS && CY::THREADS == THREADS, "one CTA shape for both items");
+    // staged planes: rows of N + TPL points, so that the z-line stores of the TPL threads of consecutive lines fall into
+    // distinct banks
+    static constexpr int RP = N + TPL;
+    static constexpr size_t STAGE_BYTES = size_t(PPI) * N * RP * sizeof(cx<T>);
+    static constexpr size_t TILE_BYTES = CZ::TILE_BYTES > CY::TILE_BYTES ? (CZ::TILE_BYTES > STAGE_BYTES ? CZ::TILE_BYTES : STAGE_BYTES)
+                                                                         : (CY::TILE_BYTES > STAGE_BYTES ? CY::TILE_BYTES : STAGE_BYTES);
+    static constexpr size_t SMEM_BYTES = TILE_BYTES + 48;  // + the ticket broadcast
+};
+constexpr bool batch_small_length(int log2n) { return log2n == 5 || log2n == 6; }
+
+// One plane item: the 4096 points at src (PPI x-planes, [p][y][z]) -> dst.  Forward z then y; inverse y then z.
+template <typename T, int LOG2N, bool INV, typename M>
+__device__ __forceinline__ void batch_plane_item(const cx<T>* src, cx<T>* dst, const cx<T>* tw, cx<T>* sm, const M& mem) {
+    using BS = BatchShape<T, LOG2N>;
+    constexpr int N = BS::N, TPL = BS::TPL, TB = BS::TB, RP = BS::RP, E = BS::CZ::E;
+    const int tid = threadIdx.x;
+    const int jz = tid % TPL, tz = tid / TPL;          // z lines: thread jz of line tz = (plane, y)
+    const int jy = tid / TB, ty = tid % TB;            // y columns: thread jy of column ty = (plane, z)
+    const int py = ty / N, zy = ty % N;
+    cx<T> v[E];
+    if constexpr (!INV) {
+        const cx<T>* q = src + tz * N + jz;
+#pragma unroll
+        for (int e = 0; e < E; ++e) v[e] = mem.ld(q + e * TPL);
+        BS::CZ::template stages<0>(v, jz, tz, sm, tw);
+        __syncthreads();  // every line's last gather is done: the exchange space becomes the staging buffer
+#pragma unroll
+        for (int e = 0; e < E; ++e) sm[tz * RP + jz + e * TPL] = v[BS::CZ::Core::final_slot(e)];
+        __syncthreads();
+#pragma unroll
+        for (int e = 0; e < E; ++e) v[e] = sm[(py * N + jy + e * TPL) * RP + zy];
+        __syncthreads();  // the staged planes are read before the first exchange overwrites them
+        BS::CY::template stages<0>(v, jy, ty, sm, tw);
+        cx<T>* o = dst + py * N * N + jy * N + zy;
+#pragma unroll
+        for (int e = 0; e < E; ++e) mem.st(o + e * TPL * N, v[BS::CY::Core::final_slot(e)]);
+    } else {
+        // re/im stay swapped between the two axes: the standalone passes swap on store and swap back on load
+        const cx<T>* q = src + py * N * N + jy * N + zy;
+#pragma unroll
+        for (int e = 0; e < E; ++e) v[e] = cswap(mem.ld(q + e * TPL * N));
+        BS::CY::template stages<0>(v, jy, ty, sm, tw);
+        __syncthreads();
+#pragma unroll
+        for (int e = 0; e < E; ++e) sm[(py * N + jy + e * TPL) * RP + zy] = v[BS::CY::Core::final_slot(e)];
+        __syncthreads();
+#pragma unroll
+        for (int e = 0; e < E; ++e) v[e] = sm[tz * RP + jz + e * TPL];
+        __syncthreads();
+        BS::CZ::template stages<0>(v, jz, tz, sm, tw);
+        cx<T>* o = dst + tz * N + jz;
+#pragma unroll
+        for (int e = 0; e < E; ++e) mem.st(o + e * TPL, cswap(v[BS::CZ::Core::final_slot(e)]));
+    }
+}
+
+// px: the slice items' view (A0 = fields, sA0 = N^3, n = x with sN = N^2, B = N^2; forward out -> out, inverse in -> out)
+template <typename T, int LOG2N, bool INV>
+__global__ void __launch_bounds__(BatchShape<T, LOG2N>::THREADS, min_ctas_per_sm<T, BatchShape<T, LOG2N>::LOG2E>(BatchShape<T, LOG2N>::THREADS))
+fft_batch_small_kernel(const __grid_constant__ FftParams px, const __grid_constant__ BatchSmall f) {
+    using BS = BatchShape<T, LOG2N>;
+    constexpr int TB = BS::TB;
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
+    unsigned long long* no_tab = reinterpret_cast<unsigned long long*>(smem_raw);  // single-segment views need no tables
+    volatile long long* bcast = reinterpret_cast<volatile long long*>(smem_raw + BS::TILE_BYTES);
+    const int tid = threadIdx.x;
+    const long long total = f.order.total();
+    const cx<T>* plane_in = reinterpret_cast<const cx<T>*>(f.plane_in);
+    cx<T>* plane_out = reinterpret_cast<cx<T>*>(f.plane_out);
+
+    // ticket broadcast as in fft_zy_fused_kernel: bcast[par] current ticket, bcast[par ^ 1] the next one, bcast[2] give
+    // up, bcast[3] / bcast[4] this launch's counter base and epoch (zy_launch_of)
+    int par = 0;
+    if (tid == 0) {
+        const unsigned long long raw = atomicAdd(f.ctr, 1ull);
+        const ZyLaunch l = zy_launch_of(raw, f.order.draws(gridDim.x));
+        bcast[3] = (long long)l.base;
+        bcast[4] = (long long)l.epoch;
+        bcast[0] = (long long)(raw - l.base);
+    }
+#pragma unroll 1
+    for (;; par ^= 1) {
+        __syncthreads();
+        const long long ticket = bcast[par];
+        if (ticket >= total) break;
+        if (tid == 0) bcast[par ^ 1] = (long long)(atomicAdd(f.ctr, 1ull) - (unsigned long long)bcast[3]);
+        const ZyItem it = f.order.decode(ticket);
+        if (it.phase == 1) {
+            // Wait until every phase-A item of this field has finished; deadlock-free for the reason given at the wait in
+            // fft_zy_fused_kernel (every dependency has a lower ticket), bounded so that a logic error becomes an error code.
+            if (tid == 0) {
+                const unsigned long long target = (unsigned long long)bcast[4] * (unsigned long long)f.order.a_items(it.group);
+                const unsigned long long* c = f.ctr + 1 + it.group;
+                unsigned long long v;
+                asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(c) : "memory");
+                long long bail = 0;
+                if (v < target) {
+                    const long long t0 = clock64();
+                    while (true) {
+                        __nanosleep(32);
+                        asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(c) : "memory");
+                        if (v >= target) break;
+                        if (f.timeout_cycles > 0 && clock64() - t0 > f.timeout_cycles) {
+                            atomicExch(f.err, BATCH_ERR_TIMEOUT);
+                            bail = 1;
+                            break;
+                        }
+                    }
+                }
+                bcast[2] = bail;
+            }
+            __syncthreads();
+            if (bcast[2]) break;
+        }
+        const bool slice = (it.phase == 0) == INV;
+        const MemHint<T> mem_a{l2_evict_first(), l2_evict_last()};   // streaming input -> intermediate
+        const MemHint<T> mem_b{l2_evict_normal(), l2_evict_first()};  // intermediate -> streaming output
+        if (slice) {
+            if (it.phase == 0) c2c_tile<T, LOG2N, BS::LOG2E, TB, true, INV>(px, it.tile, sm, no_tab, no_tab, false, mem_a);
+            else c2c_tile<T, LOG2N, BS::LOG2E, TB, true, INV>(px, it.tile, sm, no_tab, no_tab, false, mem_b);
+        } else {
+            const long long off = it.tile * BS::POINTS;
+            const cx<T>* tw = reinterpret_cast<const cx<T>*>(f.tw);
+            if (it.phase == 0) batch_plane_item<T, LOG2N, INV>(plane_in + off, plane_out + off, tw, sm, mem_a);
+            else batch_plane_item<T, LOG2N, INV>(plane_in + off, plane_out + off, tw, sm, mem_b);
+        }
+        // the item is stored and shared memory is free again before it counts
+        __syncthreads();
+        if (it.phase == 0 && tid == 0) asm volatile("red.release.gpu.global.add.u64 [%0], 1;" ::"l"(f.ctr + 1 + it.group) : "memory");
+    }
+}
+
 // ---- C2C TILED pass fed by TMA ----------------------------------------------------------------------------
 // Same tile, same stages, but the N x TB input tile is fetched by the TMA engine (cp.async.bulk.tensor, SASS UTMALDG)
 // straight into the tile buffer and announced through an mbarrier, instead of 16 LDG.128 per thread:
@@ -943,6 +1109,14 @@ cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFu
 cudaError_t launch_zy_fused_f64(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, cudaStream_t stream);
 cudaError_t launch_zy_fused_f32(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, cudaStream_t stream);
 constexpr bool zy_fused_length(int log2n) { return log2n == 8 || log2n == 9; }
+
+// batched small cubic fields (fft_batch_small_kernel), instantiated for the lengths batch_small_length accepts.  in / out:
+// the caller's buffers (fields back to back); f: counters, table and look-ahead (the work list is filled in here).  Every
+// launch of one step must use the same counters and the same batch, so that the grid and the draws per launch stay fixed.
+template <typename T, int LOG2N>
+cudaError_t launch_batch_small(const void* in, void* out, long long batch, int inverse, const BatchSmall& f, cudaStream_t stream);
+cudaError_t launch_batch_small_f64(int log2n, const void* in, void* out, long long batch, int inverse, const BatchSmall& f, cudaStream_t stream);
+cudaError_t launch_batch_small_f32(int log2n, const void* in, void* out, long long batch, int inverse, const BatchSmall& f, cudaStream_t stream);
 
 constexpr int MAX_LOG2N = 13;
 

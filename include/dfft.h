@@ -96,6 +96,26 @@ int dfft_comm_size(dfft_comm_t comm);
 int dfft_plan_create(dfft_comm_t comm, const dfft_config* config, int decomp /*dfft_decomp*/,
                      int precision /*dfft_prec*/, int transform /*dfft_transform*/, size_t nx, size_t ny,
                      size_t nz, size_t p1, size_t p2, int allocate, dfft_plan_t* plan);
+/* Batched plans (not in the reference): every exec transforms `batch` independent fields of the geometry above.
+ *   - Fields sit back to back in every caller buffer: field f of a buffer starts f times that buffer's per-field size
+ *     further, the product of its layout (dfft_get_in_size / dfft_get_out_size for full transforms,
+ *     dfft_get_partial_size(d) for partial ones; counted in reals on the real side of R2C / C2R).  This is a contiguous
+ *     [batch][X][Y][Z] array (torch tensor [B, X, Y, Z] or [B, X, Y, Z/2+1]).  No exec reads or writes a caller buffer
+ *     beyond the per-field size of its last field, so the per-field distance is never dfft_get_domain_size().
+ *   - The input of every field is left intact, as for one field.
+ *   - All exec, _async, partial, tune, timer and getter calls keep their signatures; the getters describe one field, and
+ *     the work area is that of one field (fields run one after another through it).
+ *   - dfft_plan_tune measures field 0 of the given buffers.
+ *   - dfft_get_last_launch_count, the step list and the timeline cover every launch of the exec; the phase times mark
+ *     the section ends of the last field.
+ *   - One-rank slab C2C plans of cubic 32^3 or 64^3 fields run a batch of two or more fields as one launch; every
+ *     other batched plan runs its one-field schedule once per field (multi-rank plans: each field with its own entry
+ *     rendezvous).  Both are capturable under the conditions of the _async calls below.
+ * batch == 1 is dfft_plan_create.  batch == 0, or a batch whose buffers would overflow size_t: DFFT_ERR_INVALID. */
+int dfft_plan_create_batched(dfft_comm_t comm, const dfft_config* config, int decomp /*dfft_decomp*/,
+                             int precision /*dfft_prec*/, int transform /*dfft_transform*/, size_t nx, size_t ny,
+                             size_t nz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan);
+size_t dfft_get_batch(dfft_plan_t plan); /* fields per exec (1 for dfft_plan_create), 0 for a null plan */
 int dfft_plan_destroy(dfft_plan_t plan);
 /* setWorkArea(device, host) — mpicufft_slab.cpp:236-281. device must hold dfft_get_work_size_device()
  * bytes; with comm_method Peer2Peer and more than one rank it must be the base of a cudaMalloc

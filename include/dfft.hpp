@@ -79,6 +79,13 @@ public:
     virtual ~MPIcuFFT() { if (plan) dfft_plan_destroy(plan); }
 
     virtual void initFFT(GlobalSize* global_size, Partition* partition, bool allocate = true) = 0;
+    // not in the reference: every exec transforms `batch` fields, back to back in each buffer (dfft_plan_create_batched)
+    void initFFT(GlobalSize* global_size, Partition* partition, bool allocate, size_t batch) {
+        struct Reset { size_t& b; ~Reset() { b = 1; } } reset{batch_};
+        batch_ = batch;
+        initFFT(global_size, partition, allocate);
+    }
+    size_t getBatch() const { return dfft_get_batch(plan); }
     virtual void setWorkArea(void* device = nullptr, void* host = nullptr) { DFFT_CALL(dfft_set_work_area(plan, device, host)); }
     virtual void execR2C(void* out, const void* in) = 0;
 
@@ -104,9 +111,14 @@ protected:
         c.benchmark_dir = config.benchmark_dir.empty() ? nullptr : config.benchmark_dir.c_str();
         c.comm_method2 = config.comm_method2; c.send_method2 = config.send_method2;
         if (plan) { dfft_plan_destroy(plan); plan = nullptr; }
-        DFFT_CALL(dfft_plan_create(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, p1, p2, allocate ? 1 : 0, &plan));
+        if (batch_ == 1)
+            DFFT_CALL(dfft_plan_create(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, p1, p2, allocate ? 1 : 0, &plan));
+        else
+            DFFT_CALL(dfft_plan_create_batched(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, p1, p2, batch_,
+                                               allocate ? 1 : 0, &plan));
         initialized = true;
     }
+    size_t batch_ = 1;  // fields of the plan initFFT is creating
     Configurations config;
     dfft_comm_t comm;
     int transform;
@@ -119,6 +131,7 @@ template <typename T>
 class MPIcuFFT_Slab : public MPIcuFFT<T> {
 public:
     using MPIcuFFT<T>::MPIcuFFT;
+    using MPIcuFFT<T>::initFFT;
     void initFFT(GlobalSize* global_size, Partition* /*partition*/, bool allocate = true) override {
         this->create(DFFT_SLAB_ZY_THEN_X, global_size, size_t(this->pcnt), 1, allocate);
     }
@@ -133,6 +146,7 @@ template <typename T>
 class MPIcuFFT_Slab_Z_Then_YX : public MPIcuFFT_Slab<T> {
 public:
     using MPIcuFFT_Slab<T>::MPIcuFFT_Slab;
+    using MPIcuFFT_Slab<T>::initFFT;
     void initFFT(GlobalSize* global_size, Partition* /*partition*/, bool allocate = true) override {
         this->create(DFFT_SLAB_Z_THEN_YX, global_size, size_t(this->pcnt), 1, allocate);
     }
@@ -144,6 +158,7 @@ template <typename T>
 class MPIcuFFT_Pencil : public MPIcuFFT<T> {
 public:
     using MPIcuFFT<T>::MPIcuFFT;
+    using MPIcuFFT<T>::initFFT;
     void initFFT(GlobalSize* global_size, Partition* partition, bool allocate = true) override {
         if (partition == nullptr || global_size == nullptr) throw std::runtime_error("GlobalSize or Partition not initialized!");
         if (partition->P1 * partition->P2 != size_t(this->pcnt)) throw std::runtime_error("Invalid Input Partition!");
