@@ -236,6 +236,9 @@ struct Step {
     // buffers, bsf holds the counters
     bool batch_small = false;
     BatchSmall bsf{};
+    // its stores are output values of the exec (the fused and batched stages: those of their last phase), so it runs the
+    // scaled twin of its kernel when the plan's output scale for the direction is not 1 (dfft_plan_set_scale)
+    bool final_store = false;
 };
 
 struct Schedule {
@@ -250,6 +253,7 @@ struct Schedule {
     bool executed = false;
     bool overlapped = false;  // uses the plan's auxiliary streams
     int nevents = 0;
+    int inverse = 0;          // direction (selects the plan's output scale)
 };
 
 }  // namespace dfft
@@ -263,6 +267,7 @@ struct dfft_plan_s {
     size_t esize = 16;  // bytes per complex element
     int rank = 0, P = 1;
     size_t batch = 1;         // fields per exec, back to back in every caller buffer (dfft_plan_create_batched)
+    double scale[2] = {1.0, 1.0};  // [fwd/inv] output scale (dfft_plan_set_scale), applied by the steps marked final_store
     size_t domain_bytes = 0;  // this rank (getDomainSize)
     size_t slot_bytes = 0;    // uniform over ranks
     int nslots = 2;
@@ -1921,17 +1926,18 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
             const char* phase = last ? s.phase : nullptr;
             if (s.type == STEP_PASS) {
                 FftParams prm = s.prm;
+                const double scale = s.final_store ? p->scale[sc.inverse] : 1.0;
                 // views on the caller's buffers store a byte offset in seg[0].base (field f starts f field sizes further)
                 if (s.in_user == 1) prm.in.seg[0].base = (char*)const_cast<void*>(in) + f * sc.field_in + (size_t)s.prm.in.seg[0].base;
                 if (s.out_user == 2) prm.out.seg[0].base = (char*)out + f * sc.field_out + (size_t)s.prm.out.seg[0].base;
                 cudaError_t e;
                 if (s.batch_small) {
-                    e = p->prec == DFFT_F64 ? launch_batch_small_f64(s.log2n, prm.in.seg[0].base, prm.out.seg[0].base, (long long)p->batch, s.prm.inverse, s.bsf, ss)
-                                            : launch_batch_small_f32(s.log2n, prm.in.seg[0].base, prm.out.seg[0].base, (long long)p->batch, s.prm.inverse, s.bsf, ss);
+                    e = p->prec == DFFT_F64 ? launch_batch_small_f64(s.log2n, prm.in.seg[0].base, prm.out.seg[0].base, (long long)p->batch, s.prm.inverse, s.bsf, scale, ss)
+                                            : launch_batch_small_f32(s.log2n, prm.in.seg[0].base, prm.out.seg[0].base, (long long)p->batch, s.prm.inverse, s.bsf, scale, ss);
                 } else if (s.zy) {
-                    e = p->prec == DFFT_F64 ? launch_zy_fused_f64(s.log2n, prm, s.prm_y, s.zyf, ss) : launch_zy_fused_f32(s.log2n, prm, s.prm_y, s.zyf, ss);
+                    e = p->prec == DFFT_F64 ? launch_zy_fused_f64(s.log2n, prm, s.prm_y, s.zyf, scale, ss) : launch_zy_fused_f32(s.log2n, prm, s.prm_y, s.zyf, scale, ss);
                 } else {
-                    e = p->prec == DFFT_F64 ? launch_pass_f64(s.log2n, s.kind, prm, ss) : launch_pass_f32(s.log2n, s.kind, prm, ss);
+                    e = p->prec == DFFT_F64 ? launch_pass_f64(s.log2n, s.kind, prm, scale, ss) : launch_pass_f32(s.log2n, s.kind, prm, scale, ss);
                 }
                 if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("FFT pass launch failed: ") + cudaGetErrorString(e));
                 ++launches;
@@ -2011,6 +2017,13 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
         else if (want_pencil_overlap) rc = build_overlapped_pencil(p, inverse ? 1 : 0, sc);
         else rc = build_schedule(p, inverse ? 1 : 0, d, sc);
         if (rc) return rc;
+        // No step reads the caller's `out` (views on it are only ever stored to), so every store into it is an output
+        // value of the exec: the steps that write `out` are exactly the ones that store final values.  This covers the tail
+        // launches of blocked hand-over layouts, every z chunk of overlapped x passes, the last pass of partial transforms
+        // and the fused and batched stages (whose earlier phase writes only the work area, or `out` inside the same launch).
+        // tests/test_scale.py replays every such schedule and checks that each output value is scaled exactly once.
+        for (Step& s : sc.steps) s.final_store = s.type == STEP_PASS && s.out_user == 2;
+        sc.inverse = inverse ? 1 : 0;
         field_bytes(p, inverse, d, &sc.field_in, &sc.field_out);
         if (g_view_error) return fail(DFFT_ERR_STATE, "internal: segments of one view disagree on the axis stride");
     }
@@ -2517,6 +2530,23 @@ void* dfft_get_work_area_device(dfft_plan_t p) { return p ? p->work : nullptr; }
 int dfft_get_rank(dfft_plan_t p) { return p ? p->rank : -1; }
 int dfft_get_world_size(dfft_plan_t p) { return p ? p->P : -1; }
 
+int dfft_plan_set_scale(dfft_plan_t p, double forward_scale, double inverse_scale) {
+    if (!p) return fail(DFFT_ERR_INVALID, "null plan");
+    if (!std::isfinite(forward_scale) || !std::isfinite(inverse_scale)) return fail(DFFT_ERR_INVALID, "scale must be finite");
+    p->scale[0] = forward_scale;
+    p->scale[1] = inverse_scale;
+    // the next exec of either direction may launch kernels that have not been set up yet: run it eagerly before a capture
+    for (auto& dir : p->sched)
+        for (Schedule& sc : dir) sc.executed = false;
+    return DFFT_SUCCESS;
+}
+int dfft_plan_get_scale(dfft_plan_t p, double* forward_scale, double* inverse_scale) {
+    if (!p) return fail(DFFT_ERR_INVALID, "null plan");
+    if (forward_scale) *forward_scale = p->scale[0];
+    if (inverse_scale) *inverse_scale = p->scale[1];
+    return DFFT_SUCCESS;
+}
+
 int dfft_timer_enable(dfft_plan_t p, int enable) {
     if (!p) return fail(DFFT_ERR_INVALID, "null plan");
     p->timing = enable != 0;
@@ -2772,6 +2802,7 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
         y.kind = PASS_C2C_TILED;
         y.prm = s_.prm_y;
         y.in_user = y.out_user = 0;
+        y.final_store = false;
         const bool inv = s_.prm.inverse != 0;
         z.label = inv ? "yz pass: z phase" : "zy pass: z phase";
         y.label = inv ? "yz pass: y phase" : "zy pass: y phase";
@@ -2806,6 +2837,7 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
             for (int k = 0; k < 3; ++k) {
                 order[k]->in_user = k == 0 ? 1 : 2;
                 order[k]->out_user = 2;
+                order[k]->final_store = k == 2;  // the last axis of phase B
                 all.push_back(*order[k]);
             }
         }
@@ -2858,6 +2890,13 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
             json_view(o, s_.prm.in, p->tabs);
             o += ",\"out\":";
             json_view(o, s_.prm.out, p->tabs);
+            // the scale as the kernels apply it (f32 plans: rounded to float)
+            const double scale = p->prec == DFFT_F32 ? double(float(p->scale[sc.inverse])) : p->scale[sc.inverse];
+            if (s_.final_store && p->scale[sc.inverse] != 1.0) {
+                char num[40];
+                snprintf(num, sizeof num, "%.17g", scale);
+                o += std::string(",\"scale\":") + num;
+            }
         } else if (s_.type == STEP_RENDEZVOUS) {
             o += ",\"group\":" + std::to_string(s_.group) + ",\"phase_id\":" + std::to_string(s_.phase_id) + ",\"members\":[";
             const std::vector<int>& G = p->grp[s_.group];
@@ -2931,7 +2970,7 @@ int dfft_fft1d_contig(int precision, int kind, int direction, size_t n, size_t l
     prm.in = single_view(const_cast<void*>(in), 0, ip, 1);
     prm.out = single_view(out, 0, op, 1);
     PassKind pk = kind == 0 ? PASS_C2C_CONTIG : (kind == 1 ? PASS_R2C : PASS_C2R);
-    cudaError_t e = precision == DFFT_F64 ? launch_pass_f64(l2, pk, prm, (cudaStream_t)stream) : launch_pass_f32(l2, pk, prm, (cudaStream_t)stream);
+    cudaError_t e = precision == DFFT_F64 ? launch_pass_f64(l2, pk, prm, 1.0, (cudaStream_t)stream) : launch_pass_f32(l2, pk, prm, 1.0, (cudaStream_t)stream);
     if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("launch failed: ") + cudaGetErrorString(e));
     return DFFT_SUCCESS;
 }
@@ -2949,8 +2988,8 @@ int dfft_fft1d_strided(int precision, int direction, size_t a, size_t n, size_t 
     prm.tw = tw;
     prm.in = single_view(const_cast<void*>(in), (long long)(n * b), 0, (long long)b);
     prm.out = single_view(out, (long long)(n * b), 0, (long long)b);
-    cudaError_t e = precision == DFFT_F64 ? launch_pass_f64(l2, PASS_C2C_TILED, prm, (cudaStream_t)stream)
-                                          : launch_pass_f32(l2, PASS_C2C_TILED, prm, (cudaStream_t)stream);
+    cudaError_t e = precision == DFFT_F64 ? launch_pass_f64(l2, PASS_C2C_TILED, prm, 1.0, (cudaStream_t)stream)
+                                          : launch_pass_f32(l2, PASS_C2C_TILED, prm, 1.0, (cudaStream_t)stream);
     if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("launch failed: ") + cudaGetErrorString(e));
     return DFFT_SUCCESS;
 }
@@ -2969,8 +3008,8 @@ int dfft_fft1d_general(int precision, int direction, size_t n, size_t a0, size_t
     prm.tw = tw;
     prm.in = single_view(const_cast<void*>(in), in_strides[0], in_strides[1], in_strides[2]);
     prm.out = single_view(out, out_strides[0], out_strides[1], out_strides[2]);
-    cudaError_t e = precision == DFFT_F64 ? launch_pass_f64(l2, PASS_C2C_TILED, prm, (cudaStream_t)stream)
-                                          : launch_pass_f32(l2, PASS_C2C_TILED, prm, (cudaStream_t)stream);
+    cudaError_t e = precision == DFFT_F64 ? launch_pass_f64(l2, PASS_C2C_TILED, prm, 1.0, (cudaStream_t)stream)
+                                          : launch_pass_f32(l2, PASS_C2C_TILED, prm, 1.0, (cudaStream_t)stream);
     if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("launch failed: ") + cudaGetErrorString(e));
     return DFFT_SUCCESS;
 }

@@ -61,13 +61,21 @@ static bool make_view_map(const View& v, int A0, int A1, int N, int B, int TB, C
                CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+// the parameters of a scaled twin (FftScaled): the pass' parameters and the output scale
+static FftScaled with_scale(const FftParams& p, double scale) {
+    FftScaled q;
+    static_cast<FftParams&>(q) = p;
+    q.scale = scale;
+    return q;
+}
+
 static int wide_tiles() {
     const char* e = getenv("DFFT_WIDE_TILES");
     return e ? atoi(e) : 0;
 }
 
 template <typename T, int LOG2N, int TB>
-static cudaError_t launch_tiled(const FftParams& p_in, cudaStream_t stream, long long lines) {
+static cudaError_t launch_tiled(const FftParams& p_in, double scale, cudaStream_t stream, long long lines) {
     FftParams p = p_in;
     {
         const int e = env_int("DFFT_TILE_SWZ", -1);  // experiment override of the tile-order blocking
@@ -80,11 +88,12 @@ static cudaError_t launch_tiled(const FftParams& p_in, cudaStream_t stream, long
     using S = Shape<T, LOG2N>;
     constexpr int LOG2E = S::LOG2E;
     using C = CtaFft<T, LOG2N, LOG2E, TB, true>;
-    auto kf = fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, false>;
-    auto ki = fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, true>;
+    auto kf = fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, false, false>;
+    auto ki = fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, true, false>;
     static cudaError_t once = set_smem(kf, C::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ki, C::SMEM_BYTES);
     if (once != cudaSuccess) return once;
     if (p.B <= 0) return cudaSuccess;
+    const bool scaled = scale != 1.0;
     const long long grid = lines * ((p.B + TB - 1) / TB);
     if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
     if constexpr (C::NST >= 2 && LOG2N >= 7) {
@@ -100,8 +109,8 @@ static cudaError_t launch_tiled(const FftParams& p_in, cudaStream_t stream, long
         const bool bulk_ok = p.bulk_out && p.out.sN == TB && p.B == TB;
         alignas(64) CUtensorMap tm;
         if (want && p.in.nseg == 1 && (!p.bulk_out || bulk_ok) && make_view_map<T>(p.in, p.A0, p.A1, C::N, p.B, TB, &tm)) {
-            auto tf = fft_c2c_tma_kernel<T, LOG2N, LOG2E, TB, false>;
-            auto ti = fft_c2c_tma_kernel<T, LOG2N, LOG2E, TB, true>;
+            auto tf = fft_c2c_tma_kernel<T, LOG2N, LOG2E, TB, false, false>;
+            auto ti = fft_c2c_tma_kernel<T, LOG2N, LOG2E, TB, true, false>;
             static cudaError_t oncet = set_smem(tf, C::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ti, C::SMEM_BYTES);
             if (oncet != cudaSuccess) return oncet;
             static int resident = [&] {
@@ -115,34 +124,63 @@ static cudaError_t launch_tiled(const FftParams& p_in, cudaStream_t stream, long
             if (p.max_ctas > 0 && g > p.max_ctas) g = p.max_ctas;
             FftParams q = p;
             q.bulk_out = bulk_ok ? 1 : 0;
+            if (scaled) {
+                auto tfs = fft_c2c_tma_kernel<T, LOG2N, LOG2E, TB, false, true>;
+                auto tis = fft_c2c_tma_kernel<T, LOG2N, LOG2E, TB, true, true>;
+                static cudaError_t onces = set_smem(tfs, C::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(tis, C::SMEM_BYTES);
+                if (onces != cudaSuccess) return onces;
+                const FftScaled qs = with_scale(q, scale);
+                if (p.inverse) tis<<<unsigned(g), C::THREADS, C::SMEM_BYTES, stream>>>(qs, tm);
+                else tfs<<<unsigned(g), C::THREADS, C::SMEM_BYTES, stream>>>(qs, tm);
+                return cudaGetLastError();
+            }
             if (p.inverse) ti<<<unsigned(g), C::THREADS, C::SMEM_BYTES, stream>>>(q, tm);
             else tf<<<unsigned(g), C::THREADS, C::SMEM_BYTES, stream>>>(q, tm);
             return cudaGetLastError();
         }
     }
     const unsigned g = unsigned((p.max_ctas > 0 && grid > p.max_ctas) ? p.max_ctas : grid);
+    if (scaled) {
+        auto kfs = fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, false, true>;
+        auto kis = fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, true, true>;
+        static cudaError_t onces = set_smem(kfs, C::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(kis, C::SMEM_BYTES);
+        if (onces != cudaSuccess) return onces;
+        if (p.inverse) kis<<<g, C::THREADS, C::SMEM_BYTES, stream>>>(with_scale(p, scale));
+        else kfs<<<g, C::THREADS, C::SMEM_BYTES, stream>>>(with_scale(p, scale));
+        return cudaGetLastError();
+    }
     if (p.inverse) ki<<<g, C::THREADS, C::SMEM_BYTES, stream>>>(p);
     else kf<<<g, C::THREADS, C::SMEM_BYTES, stream>>>(p);
     return cudaGetLastError();
 }
 
 template <typename T, int LOG2N>
-cudaError_t launch_pass(PassKind kind, const FftParams& p, cudaStream_t stream) {
+cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStream_t stream) {
     using S = Shape<T, LOG2N>;
     constexpr int LOG2E = S::LOG2E;
     const long long lines = (long long)p.A0 * p.A1;
     if (lines <= 0) return cudaSuccess;
     cudaError_t err = cudaSuccess;
+    const bool scaled = scale != 1.0;
     switch (kind) {
         case PASS_C2C_CONTIG: {
             using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
-            auto kf = fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, false>;
-            auto ki = fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, true>;
+            auto kf = fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, false, false>;
+            auto ki = fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, true, false>;
             static cudaError_t once = set_smem(kf, C::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ki, C::SMEM_BYTES);
             if (once != cudaSuccess) return once;
             if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
             const long long grid = (lines + S::TBC - 1) / S::TBC;
             if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+            if (scaled) {
+                auto kfs = fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, false, true>;
+                auto kis = fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, true, true>;
+                static cudaError_t onces = set_smem(kfs, C::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(kis, C::SMEM_BYTES);
+                if (onces != cudaSuccess) return onces;
+                if (p.inverse) kis<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(with_scale(p, scale));
+                else kfs<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(with_scale(p, scale));
+                break;
+            }
             if (p.inverse) ki<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(p);
             else kf<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(p);
             break;
@@ -161,29 +199,43 @@ cudaError_t launch_pass(PassKind kind, const FftParams& p, cudaStream_t stream) 
                 const bool wide = w > 0 || p.tile_pref == 2 || (w == 0 && p.tile_pref == 0 && LOG2N >= 10 && (far_rows || tma_auto));
                 // never a wide tile for a view that is only one narrow tile wide (blocked hand-over with CH = TBT): half of
                 // its columns would be empty
-                if (wide && w >= 0 && p.tile_pref != 1 && p.B > S::TBT) return launch_tiled<T, LOG2N, S::TBT_WIDE>(p, stream, lines);
+                if (wide && w >= 0 && p.tile_pref != 1 && p.B > S::TBT) return launch_tiled<T, LOG2N, S::TBT_WIDE>(p, scale, stream, lines);
             }
-            return launch_tiled<T, LOG2N, S::TBT>(p, stream, lines);
+            return launch_tiled<T, LOG2N, S::TBT>(p, scale, stream, lines);
         }
         case PASS_R2C: {
             using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
-            auto k = fft_r2c_kernel<T, LOG2N, LOG2E, S::TBC>;
+            auto k = fft_r2c_kernel<T, LOG2N, LOG2E, S::TBC, false>;
             static cudaError_t once = set_smem(k, C::SMEM_BYTES);
             if (once != cudaSuccess) return once;
             if (p.in.nseg != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
             const long long grid = (lines + S::TBC - 1) / S::TBC;
             if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+            if (scaled) {
+                auto ks = fft_r2c_kernel<T, LOG2N, LOG2E, S::TBC, true>;
+                static cudaError_t onces = set_smem(ks, C::SMEM_BYTES);
+                if (onces != cudaSuccess) return onces;
+                ks<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(with_scale(p, scale));
+                break;
+            }
             k<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(p);
             break;
         }
         case PASS_C2R: {
             using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
-            auto k = fft_c2r_kernel<T, LOG2N, LOG2E, S::TBC>;
+            auto k = fft_c2r_kernel<T, LOG2N, LOG2E, S::TBC, false>;
             static cudaError_t once = set_smem(k, C::SMEM_BYTES);
             if (once != cudaSuccess) return once;
             if (p.out.nseg != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
             const long long grid = (lines + S::TBC - 1) / S::TBC;
             if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+            if (scaled) {
+                auto ks = fft_c2r_kernel<T, LOG2N, LOG2E, S::TBC, true>;
+                static cudaError_t onces = set_smem(ks, C::SMEM_BYTES);
+                if (onces != cudaSuccess) return onces;
+                ks<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(with_scale(p, scale));
+                break;
+            }
             k<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(p);
             break;
         }
@@ -193,7 +245,7 @@ cudaError_t launch_pass(PassKind kind, const FftParams& p, cudaStream_t stream) 
     return err;
 }
 
-template cudaError_t launch_pass<DFFT_T, DFFT_LOG2N>(PassKind, const FftParams&, cudaStream_t);
+template cudaError_t launch_pass<DFFT_T, DFFT_LOG2N>(PassKind, const FftParams&, double, cudaStream_t);
 
 #if DFFT_LOG2N == 8 || DFFT_LOG2N == 9
 static bool aligned128(const void* base, long long elems_a, long long elems_b, long long elems_c) {
@@ -202,7 +254,7 @@ static bool aligned128(const void* base, long long elems_a, long long elems_b, l
 }
 
 template <typename T, int LOG2N>
-cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFused& f_in, cudaStream_t stream) {
+cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFused& f_in, double scale, cudaStream_t stream) {
     static_assert(zy_fused_length(LOG2N), "fused z + y stage: length not instantiated");
     using Z = ZyShape<T, LOG2N>;
     constexpr int TB = Z::TB;
@@ -210,6 +262,7 @@ cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFu
     if (pz.in.nseg != 1 || pz.out.nseg != 1 || py.in.nseg != 1 || py.out.nseg != 1 || pz.in.sN != 1 || pz.out.sN != 1) return cudaErrorInvalidValue;
     if (pz.inverse != py.inverse || py.tile_swz != 0 || pz.A0 != py.A0 || pz.A1 % TB || py.B % TB || f_in.order.nx != pz.A0 || f_in.order.gpp < 1 || f_in.order.ahead < 1)
         return cudaErrorInvalidValue;
+    if (scale != 1.0 && !inv) return cudaErrorInvalidValue;  // the forward stage stores the x pass' input
     ZyFused f = f_in;
     const int z_per_plane = pz.A1 / TB, y_per_plane = py.A1 * (py.B / TB);  // tiles = work items
     f.order.na = inv ? y_per_plane : z_per_plane;
@@ -218,8 +271,8 @@ cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFu
     const View& mid = inv ? pz.in : py.in;
     f.discard = inv ? (Z::Z_DISCARD && aligned128(mid.seg[0].base, mid.seg[0].sA0, mid.seg[0].sA1, 1 << LOG2N))
                     : (Z::Y_DISCARD && aligned128(mid.seg[0].base, mid.seg[0].sA0, mid.seg[0].sA1, mid.sN));
-    auto kf = fft_zy_fused_kernel<T, LOG2N, false>;
-    auto ki = fft_zy_fused_kernel<T, LOG2N, true>;
+    auto kf = fft_zy_fused_kernel<T, LOG2N, false, false>;
+    auto ki = fft_zy_fused_kernel<T, LOG2N, true, false>;
     static cudaError_t once = set_smem(kf, Z::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ki, Z::SMEM_BYTES);
     if (once != cudaSuccess) return once;
     // persistent: as many CTAs as fit at once (tickets hand out the work; fewer resident CTAs are fine as well).  The
@@ -234,17 +287,24 @@ cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFu
     const long long total = f.order.total();
     if (total <= 0) return cudaSuccess;
     const unsigned grid = unsigned(total < resident ? total : resident);
+    if (scale != 1.0) {
+        auto kis = fft_zy_fused_kernel<T, LOG2N, true, true>;
+        static cudaError_t onces = set_smem(kis, Z::SMEM_BYTES);
+        if (onces != cudaSuccess) return onces;
+        kis<<<grid, Z::THREADS, Z::SMEM_BYTES, stream>>>(with_scale(pz, scale), py, f);
+        return cudaGetLastError();
+    }
     if (inv) ki<<<grid, Z::THREADS, Z::SMEM_BYTES, stream>>>(pz, py, f);
     else kf<<<grid, Z::THREADS, Z::SMEM_BYTES, stream>>>(pz, py, f);
     return cudaGetLastError();
 }
 
-template cudaError_t launch_zy_fused<DFFT_T, DFFT_LOG2N>(const FftParams&, const FftParams&, const ZyFused&, cudaStream_t);
+template cudaError_t launch_zy_fused<DFFT_T, DFFT_LOG2N>(const FftParams&, const FftParams&, const ZyFused&, double, cudaStream_t);
 #endif
 
 #if DFFT_LOG2N == 5 || DFFT_LOG2N == 6
 template <typename T, int LOG2N>
-cudaError_t launch_batch_small(const void* in, void* out, long long batch, int inverse, const BatchSmall& f_in, cudaStream_t stream) {
+cudaError_t launch_batch_small(const void* in, void* out, long long batch, int inverse, const BatchSmall& f_in, double scale, cudaStream_t stream) {
     static_assert(batch_small_length(LOG2N), "batched small fields: length not instantiated");
     using BS = BatchShape<T, LOG2N>;
     constexpr long long N = BS::N, N2 = N * N, N3 = N2 * N;
@@ -268,8 +328,8 @@ cudaError_t launch_batch_small(const void* in, void* out, long long batch, int i
     }
     px.in.seg[0].base = inverse ? const_cast<void*>(in) : out;
     px.out.seg[0].base = out;
-    auto kf = fft_batch_small_kernel<T, LOG2N, false>;
-    auto ki = fft_batch_small_kernel<T, LOG2N, true>;
+    auto kf = fft_batch_small_kernel<T, LOG2N, false, false>;
+    auto ki = fft_batch_small_kernel<T, LOG2N, true, false>;
     static cudaError_t once = set_smem(kf, BS::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ki, BS::SMEM_BYTES);
     if (once != cudaSuccess) return once;
     // persistent, as many CTAs as fit at once; the grid depends on the batch only (zy_launch_of)
@@ -282,12 +342,21 @@ cudaError_t launch_batch_small(const void* in, void* out, long long batch, int i
     }();
     const long long total = f.order.total();
     const unsigned grid = unsigned(total < resident ? total : resident);
+    if (scale != 1.0) {
+        auto kfs = fft_batch_small_kernel<T, LOG2N, false, true>;
+        auto kis = fft_batch_small_kernel<T, LOG2N, true, true>;
+        static cudaError_t onces = set_smem(kfs, BS::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(kis, BS::SMEM_BYTES);
+        if (onces != cudaSuccess) return onces;
+        if (inverse) kis<<<grid, BS::THREADS, BS::SMEM_BYTES, stream>>>(with_scale(px, scale), f);
+        else kfs<<<grid, BS::THREADS, BS::SMEM_BYTES, stream>>>(with_scale(px, scale), f);
+        return cudaGetLastError();
+    }
     if (inverse) ki<<<grid, BS::THREADS, BS::SMEM_BYTES, stream>>>(px, f);
     else kf<<<grid, BS::THREADS, BS::SMEM_BYTES, stream>>>(px, f);
     return cudaGetLastError();
 }
 
-template cudaError_t launch_batch_small<DFFT_T, DFFT_LOG2N>(const void*, void*, long long, int, const BatchSmall&, cudaStream_t);
+template cudaError_t launch_batch_small<DFFT_T, DFFT_LOG2N>(const void*, void*, long long, int, const BatchSmall&, double, cudaStream_t);
 #endif
 
 }  // namespace dfft

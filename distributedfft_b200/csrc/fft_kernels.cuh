@@ -67,6 +67,15 @@ struct FftParams {
                       // (0 = plain order: b tiles fastest, then a1, then a0)
 };
 
+// Output scale (dfft_plan_set_scale).  Every kernel that stores final values has a scaled twin (template flag SCALED)
+// that takes FftScaled in place of FftParams and multiplies each finished value by the scale right before its store.
+// The unscaled instantiations keep their parameters and code exactly; the twin is launched only for a scale != 1.
+struct FftScaled : FftParams {
+    double scale;  // rounded to the kernel's precision once (f32: float(scale))
+};
+template <bool SCALED>
+using KParams = std::conditional_t<SCALED, FftScaled, FftParams>;
+
 enum PassKind { PASS_C2C_CONTIG = 0, PASS_C2C_TILED = 1, PASS_R2C = 2, PASS_C2R = 3 };
 
 // ---- tile shape choices (compile time) -----------------------------------------------------------
@@ -329,6 +338,23 @@ struct MemHint {
     }
 };
 
+// Real multiply of a finished value by the output scale.  __dmul_rn / __fmul_rn are never contracted into an FMA, so the
+// stored value is exactly the unscaled result times s, rounded once in the kernel's precision.
+template <typename T>
+__device__ __forceinline__ cx<T> cscale(cx<T> v, T s) {
+    if constexpr (sizeof(T) == 8) return cx<T>{__dmul_rn(v.x, s), __dmul_rn(v.y, s)};
+    else return cx<T>{__fmul_rn(v.x, s), __fmul_rn(v.y, s)};
+}
+
+// store policy of the scaled twins: the policy M, with every stored value scaled first
+template <typename T, typename M>
+struct MemScaled {
+    M m;
+    T s;
+    __device__ __forceinline__ cx<T> ld(const cx<T>* p) const { return m.ld(p); }
+    __device__ __forceinline__ void st(cx<T>* p, cx<T> v) const { m.st(p, cscale<T>(v, s)); }
+};
+
 // drop a 128-byte L2 line without writing it back (its contents become undefined)
 __device__ __forceinline__ void l2_discard(const void* p) { asm volatile("discard.global.L2 [%0], 128;" ::"l"(p) : "memory"); }
 
@@ -417,9 +443,9 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
 // Grid-stride over tiles: launched with one CTA per tile it is the plain kernel; launched with fewer CTAs
 // (FftParams::max_ctas) it is persistent and occupies only that many CTA slots, which is how the overlapped
 // schedule leaves the rest of the GPU to the other passes.
-template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV>
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, bool SCALED>
 __global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
-fft_c2c_kernel(const __grid_constant__ FftParams p) {
+fft_c2c_kernel(const __grid_constant__ KParams<SCALED> p) {
     using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
     using TC = TileCoord<C, TILED, TB>;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -431,7 +457,8 @@ fft_c2c_kernel(const __grid_constant__ FftParams p) {
 
 #pragma unroll 1
     for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV>(p, tile, sm, tab_in, tab_out, multi, MemPlain<T>{});
+        if constexpr (SCALED) c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV>(p, tile, sm, tab_in, tab_out, multi, MemScaled<T, MemPlain<T>>{{}, T(p.scale)});
+        else c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV>(p, tile, sm, tab_in, tab_out, multi, MemPlain<T>{});
         const int t = TILED ? int(threadIdx.x) % TB : int(threadIdx.x) / C::TPL;
         if (tile + gridDim.x < ntiles) {
             // persistent use: the next tile's first scatter must not overtake this tile's last gather, and
@@ -523,9 +550,11 @@ __device__ __noinline__ void zy_item_done(const FftParams& pz, const FftParams& 
     }
 }
 
-template <typename T, int LOG2N, bool INV>
+// SCALED (inverse only): phase B, the z lines that store the caller's output, scales its stores by pz.scale.
+template <typename T, int LOG2N, bool INV, bool SCALED>
 __global__ void __launch_bounds__(ZyShape<T, LOG2N>::THREADS, min_ctas_per_sm<T, ZyShape<T, LOG2N>::LOG2E>(ZyShape<T, LOG2N>::THREADS))
-fft_zy_fused_kernel(const __grid_constant__ FftParams pz, const __grid_constant__ FftParams py, const __grid_constant__ ZyFused f) {
+fft_zy_fused_kernel(const __grid_constant__ KParams<SCALED> pz, const __grid_constant__ FftParams py, const __grid_constant__ ZyFused f) {
+    static_assert(INV || !SCALED, "the forward fused stage stores the intermediate of the x pass only");
     using Z = ZyShape<T, LOG2N>;
     constexpr int TB = Z::TB;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -592,6 +621,7 @@ fft_zy_fused_kernel(const __grid_constant__ FftParams pz, const __grid_constant_
         const MemHint<T> mem_b{l2_evict_normal(), l2_evict_first()};  // intermediate -> streaming output
         if (z_item) {
             if (it.phase == 0) c2c_tile<T, LOG2N, Z::LOG2E, TB, false, INV>(pz, it.tile, sm, tab_in, tab_out, false, mem_a);
+            else if constexpr (SCALED) c2c_tile<T, LOG2N, Z::LOG2E, TB, false, INV>(pz, it.tile, sm, tab_in, tab_out, false, MemScaled<T, MemHint<T>>{mem_b, T(pz.scale)});
             else c2c_tile<T, LOG2N, Z::LOG2E, TB, false, INV>(pz, it.tile, sm, tab_in, tab_out, false, mem_b);
         } else {
             if (it.phase == 0) c2c_tile<T, LOG2N, Z::LOG2E, TB, true, INV>(py, it.tile, sm, tab_in, tab_out, false, mem_a);
@@ -693,9 +723,11 @@ __device__ __forceinline__ void batch_plane_item(const cx<T>* src, cx<T>* dst, c
 }
 
 // px: the slice items' view (A0 = fields, sA0 = N^3, n = x with sN = N^2, B = N^2; forward out -> out, inverse in -> out)
-template <typename T, int LOG2N, bool INV>
+// SCALED: phase B (forward the slice items, inverse the plane items) scales its stores by px.scale; phase A's stores into
+// the caller's output are intermediate and stay unscaled.
+template <typename T, int LOG2N, bool INV, bool SCALED>
 __global__ void __launch_bounds__(BatchShape<T, LOG2N>::THREADS, min_ctas_per_sm<T, BatchShape<T, LOG2N>::LOG2E>(BatchShape<T, LOG2N>::THREADS))
-fft_batch_small_kernel(const __grid_constant__ FftParams px, const __grid_constant__ BatchSmall f) {
+fft_batch_small_kernel(const __grid_constant__ KParams<SCALED> px, const __grid_constant__ BatchSmall f) {
     using BS = BatchShape<T, LOG2N>;
     constexpr int TB = BS::TB;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -756,11 +788,13 @@ fft_batch_small_kernel(const __grid_constant__ FftParams px, const __grid_consta
         const MemHint<T> mem_b{l2_evict_normal(), l2_evict_first()};  // intermediate -> streaming output
         if (slice) {
             if (it.phase == 0) c2c_tile<T, LOG2N, BS::LOG2E, TB, true, INV>(px, it.tile, sm, no_tab, no_tab, false, mem_a);
+            else if constexpr (SCALED) c2c_tile<T, LOG2N, BS::LOG2E, TB, true, INV>(px, it.tile, sm, no_tab, no_tab, false, MemScaled<T, MemHint<T>>{mem_b, T(px.scale)});
             else c2c_tile<T, LOG2N, BS::LOG2E, TB, true, INV>(px, it.tile, sm, no_tab, no_tab, false, mem_b);
         } else {
             const long long off = it.tile * BS::POINTS;
             const cx<T>* tw = reinterpret_cast<const cx<T>*>(f.tw);
             if (it.phase == 0) batch_plane_item<T, LOG2N, INV>(plane_in + off, plane_out + off, tw, sm, mem_a);
+            else if constexpr (SCALED) batch_plane_item<T, LOG2N, INV>(plane_in + off, plane_out + off, tw, sm, MemScaled<T, MemHint<T>>{mem_b, T(px.scale)});
             else batch_plane_item<T, LOG2N, INV>(plane_in + off, plane_out + off, tw, sm, mem_b);
         }
         // the item is stored and shared memory is free again before it counts
@@ -801,9 +835,10 @@ struct TmaBar {
     }
 };
 
-template <typename T, int LOG2N, int LOG2E, int TB, bool INV>
+// SCALED: every finished value is scaled by p.scale in registers, before the 16-byte stores or the staging for bulk_out.
+template <typename T, int LOG2N, int LOG2E, int TB, bool INV, bool SCALED>
 __global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
-fft_c2c_tma_kernel(const __grid_constant__ FftParams p, const __grid_constant__ CUtensorMap tm_in) {
+fft_c2c_tma_kernel(const __grid_constant__ KParams<SCALED> p, const __grid_constant__ CUtensorMap tm_in) {
     using C = CtaFft<T, LOG2N, LOG2E, TB, true>;
     using Core = typename C::Core;
     using L = typename C::L;
@@ -823,6 +858,11 @@ fft_c2c_tma_kernel(const __grid_constant__ FftParams p, const __grid_constant__ 
     const bool out_multi = p.out.nseg > 1;
     const bool bulk = p.bulk_out != 0;
     const int tid = threadIdx.x;
+    auto finish = [&](cx<T> x) {  // the stored form of a finished value
+        if constexpr (INV) x = cswap(x);
+        if constexpr (SCALED) x = cscale<T>(x, T(p.scale));
+        return x;
+    };
 
     auto request = [&](long long tile) {  // one thread: arm the barrier and ask the TMA engine for the tile
         const TC tc(p, tile);
@@ -900,26 +940,19 @@ fft_c2c_tma_kernel(const __grid_constant__ FftParams p, const __grid_constant__ 
                     cx<T>* q = out.p0 + (long long)j * p.out.sN;
 #pragma unroll
                     for (int e = 0; e < E; ++e) {
-                        const cx<T> x = v[Core::final_slot(e)];
-                        st_elem<T>(q, INV ? cswap(x) : x);
+                        st_elem<T>(q, finish(v[Core::final_slot(e)]));
                         q += step;
                     }
                 } else {
 #pragma unroll
-                    for (int e = 0; e < E; ++e) {
-                        const cx<T> x = v[Core::final_slot(e)];
-                        st_elem<T>(out.at(j + e * TPL), INV ? cswap(x) : x);
-                    }
+                    for (int e = 0; e < E; ++e) st_elem<T>(out.at(j + e * TPL), finish(v[Core::final_slot(e)]));
                 }
             }
             if (out_multi) __syncthreads();  // the segment table is rewritten by the next tile
         } else {
             __syncthreads();  // last gather finished everywhere: stage the finished tile, natural order [n][TB]
 #pragma unroll
-            for (int e = 0; e < E; ++e) {
-                const cx<T> x = v[Core::final_slot(e)];
-                sm[(j + e * TPL) * TB + t] = INV ? cswap(x) : x;
-            }
+            for (int e = 0; e < E; ++e) sm[(j + e * TPL) * TB + t] = finish(v[Core::final_slot(e)]);
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             __syncthreads();
             if (tid == 0) {
@@ -952,9 +985,9 @@ __device__ __forceinline__ cx<T> shfl_cx(cx<T> v, int src_lane) {
 // ---- R2C pass (CONTIG): real line of 2M points -> M+1 complex points ------------------------------------
 // The real line is read as M complex points z[m] = x[2m] + i x[2m+1], transformed with the length-M
 // core and split into even/odd spectra in shared memory:  X[k] = Xe[k] + W_2M^k Xo[k].
-template <typename T, int LOG2M, int LOG2E, int TB>
+template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED>
 __global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
-fft_r2c_kernel(const __grid_constant__ FftParams p) {
+fft_r2c_kernel(const __grid_constant__ KParams<SCALED> p) {
     using C = CtaFft<T, LOG2M, LOG2E, TB, false>;
     using LA = LineAccess<T, C::LINES>;
     constexpr int E = C::E, TPL = C::TPL, M = C::N, NST = C::NST;
@@ -1001,8 +1034,13 @@ fft_r2c_kernel(const __grid_constant__ FftParams p) {
         const cx<T> xo = cx<T>{T(0.5) * d.y, T(-0.5) * d.x};  // -i/2 * d
         const cx<T> tt = cmul(ld_tw(tw2, k), xo);
         if (valid) {
-            st_elem<T>(out.at1(k), cadd(xe, tt));
-            st_elem<T>(out.at1(M - k), cconj(csub(xe, tt)));
+            if constexpr (SCALED) {
+                st_elem<T>(out.at1(k), cscale<T>(cadd(xe, tt), T(p.scale)));
+                st_elem<T>(out.at1(M - k), cscale<T>(cconj(csub(xe, tt)), T(p.scale)));
+            } else {
+                st_elem<T>(out.at1(k), cadd(xe, tt));
+                st_elem<T>(out.at1(M - k), cconj(csub(xe, tt)));
+            }
         }
     };
 #pragma unroll
@@ -1011,9 +1049,9 @@ fft_r2c_kernel(const __grid_constant__ FftParams p) {
 }
 
 // ---- C2R pass (CONTIG): M+1 complex points -> real line of 2M points, unnormalised -----------------------
-template <typename T, int LOG2M, int LOG2E, int TB>
+template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED>
 __global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
-fft_c2r_kernel(const __grid_constant__ FftParams p) {
+fft_c2r_kernel(const __grid_constant__ KParams<SCALED> p) {
     using C = CtaFft<T, LOG2M, LOG2E, TB, false>;
     using LA = LineAccess<T, C::LINES>;
     constexpr int E = C::E, TPL = C::TPL, M = C::N;
@@ -1089,34 +1127,40 @@ fft_c2r_kernel(const __grid_constant__ FftParams p) {
     if (valid) {
         cx<T>* q = out.p0 + j;
 #pragma unroll
-        for (int e = 0; e < E; ++e) st_elem<T>(q + e * TPL, cswap(v[C::Core::final_slot(e)]));
+        for (int e = 0; e < E; ++e) {
+            if constexpr (SCALED) st_elem<T>(q + e * TPL, cscale<T>(cswap(v[C::Core::final_slot(e)]), T(p.scale)));
+            else st_elem<T>(q + e * TPL, cswap(v[C::Core::final_slot(e)]));
+        }
     }
 }
 
 // ---- host launchers (one explicit instantiation per precision and size, see fft_inst.cu) ----------------
+// scale: the output scale of the pass' stores; 1 launches the unscaled kernels, anything else their scaled twins.
 template <typename T, int LOG2N>
-cudaError_t launch_pass(PassKind kind, const FftParams& p, cudaStream_t stream);
+cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStream_t stream);
 
 // launch_pass for a runtime size; returns cudaErrorInvalidValue for unsupported lengths.
-cudaError_t launch_pass_f64(int log2n, PassKind kind, const FftParams& p, cudaStream_t stream);
-cudaError_t launch_pass_f32(int log2n, PassKind kind, const FftParams& p, cudaStream_t stream);
+cudaError_t launch_pass_f64(int log2n, PassKind kind, const FftParams& p, double scale, cudaStream_t stream);
+cudaError_t launch_pass_f32(int log2n, PassKind kind, const FftParams& p, double scale, cudaStream_t stream);
 
 // fused z + y stage (fft_zy_fused_kernel), instantiated for the lengths zy_fused_length accepts.  pz: the z pass, py: the y
 // pass, f: counters and plane groups (f.order.na / nb are filled in here).  Every launch of one step must use the same
-// counters and the same grid (zy_launch_of), which the launcher's fixed grid for a given work list provides.
+// counters and the same grid (zy_launch_of), which the launcher's fixed grid for a given work list provides.  scale: of the
+// last phase's stores, inverse only (the forward stage stores an intermediate).
 template <typename T, int LOG2N>
-cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFused& f, cudaStream_t stream);
-cudaError_t launch_zy_fused_f64(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, cudaStream_t stream);
-cudaError_t launch_zy_fused_f32(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, cudaStream_t stream);
+cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFused& f, double scale, cudaStream_t stream);
+cudaError_t launch_zy_fused_f64(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, double scale, cudaStream_t stream);
+cudaError_t launch_zy_fused_f32(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, double scale, cudaStream_t stream);
 constexpr bool zy_fused_length(int log2n) { return log2n == 8 || log2n == 9; }
 
 // batched small cubic fields (fft_batch_small_kernel), instantiated for the lengths batch_small_length accepts.  in / out:
 // the caller's buffers (fields back to back); f: counters, table and look-ahead (the work list is filled in here).  Every
 // launch of one step must use the same counters and the same batch, so that the grid and the draws per launch stay fixed.
+// scale: of phase B's stores.
 template <typename T, int LOG2N>
-cudaError_t launch_batch_small(const void* in, void* out, long long batch, int inverse, const BatchSmall& f, cudaStream_t stream);
-cudaError_t launch_batch_small_f64(int log2n, const void* in, void* out, long long batch, int inverse, const BatchSmall& f, cudaStream_t stream);
-cudaError_t launch_batch_small_f32(int log2n, const void* in, void* out, long long batch, int inverse, const BatchSmall& f, cudaStream_t stream);
+cudaError_t launch_batch_small(const void* in, void* out, long long batch, int inverse, const BatchSmall& f, double scale, cudaStream_t stream);
+cudaError_t launch_batch_small_f64(int log2n, const void* in, void* out, long long batch, int inverse, const BatchSmall& f, double scale, cudaStream_t stream);
+cudaError_t launch_batch_small_f32(int log2n, const void* in, void* out, long long batch, int inverse, const BatchSmall& f, double scale, cudaStream_t stream);
 
 constexpr int MAX_LOG2N = 13;
 

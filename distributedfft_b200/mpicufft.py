@@ -214,6 +214,20 @@ class MPIcuFFT:
     def getRank(self): return int(lib().dfft_get_rank(self._h))
     def getWorldSize(self): return int(lib().dfft_get_world_size(self._h))
 
+    # -- output scale (not in the reference) ------------------------------------------------------
+    def setScale(self, forward: float = 1.0, inverse: float = 1.0):
+        """Multiply every output value of forward / inverse execs by these scales, inside the kernel that stores them
+        (dfft_plan_set_scale).  With N the product of the transformed lengths: torch's norm="backward" is (1, 1/N),
+        "ortho" (1/sqrt(N), 1/sqrt(N)), "forward" (1/N, 1).  Local to this rank: set the same values on every rank.
+        A CUDA graph keeps the scale it was captured with; run each direction eagerly once before capturing again."""
+        check(lib().dfft_plan_set_scale(self._h, float(forward), float(inverse)))
+
+    def getScale(self):
+        """(forward, inverse) output scales."""
+        f, i = C.c_double(), C.c_double()
+        check(lib().dfft_plan_get_scale(self._h, C.byref(f), C.byref(i)))
+        return f.value, i.value
+
     # -- timer -----------------------------------------------------------------------------------
     def enableTimer(self, on: bool = True):
         check(lib().dfft_timer_enable(self._h, 1 if on else 0))

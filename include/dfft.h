@@ -156,6 +156,24 @@ int dfft_exec_c2c_partial(dfft_plan_t plan, void* out, const void* in, int direc
 int dfft_exec_r2c_async(dfft_plan_t plan, void* out, const void* in, void* stream);
 int dfft_exec_c2r_async(dfft_plan_t plan, void* out, const void* in, void* stream);
 int dfft_exec_c2c_async(dfft_plan_t plan, void* out, const void* in, int direction, void* stream);
+/* Output scale (not in the reference; cuFFT has none either).  Every exec of a direction multiplies each output value by
+ * that direction's scale: the real and imaginary parts of complex outputs, the real values of C2R outputs.  It applies to
+ * the plain and _async calls, R2C / C2R / C2C, partial transforms (the value is used as given), every field of a batched
+ * plan, and every decomposition.  The kernel that stores the final values multiplies them, in the plan's precision, as
+ * they leave the registers: no extra launch and no extra memory traffic.  The result equals the unscaled output times the
+ * scale computed in the same precision, bit for bit (f32 plans round the scale to float once).  Defaults (1, 1): the plan
+ * runs exactly its unscaled kernels.
+ * Normalisations, with N the product of the transformed lengths (Nx*Ny*Nz, or that of the first d for partial ones):
+ *   backward (torch / numpy default, cuFFT round trips)  (1, 1/N)
+ *   ortho                                                (1/sqrt(N), 1/sqrt(N))
+ *   forward                                              (1/N, 1)
+ * Local to the calling rank, not collective: set the same values on every rank of a multi-rank plan.  A null plan, or a
+ * NaN or infinite scale, returns DFFT_ERR_INVALID.  A CUDA graph replays the scale in effect when it was captured.
+ * dfft_plan_set_scale (even to the values already set) makes every direction run eagerly once more before it can be
+ * captured again (DFFT_ERR_STATE otherwise), as for the first exec. */
+int dfft_plan_set_scale(dfft_plan_t plan, double forward_scale, double inverse_scale);
+/* Either pointer may be NULL. */
+int dfft_plan_get_scale(dfft_plan_t plan, double* forward_scale, double* inverse_scale);
 /* Waits for the stream of the last eager _async call and reports a device-side failure (rendezvous or fused-stage
  * timeout), if any.  After replaying a graph, synchronise the replay stream first; dfft_plan_wait then reports the
  * errors the replayed kernels recorded. */

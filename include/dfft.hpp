@@ -86,6 +86,10 @@ public:
         initFFT(global_size, partition, allocate);
     }
     size_t getBatch() const { return dfft_get_batch(plan); }
+    // not in the reference: output scale of every forward / inverse exec (dfft_plan_set_scale; after initFFT).  For
+    // normalised round trips use setScale(1, 1.0 / (Nx * Ny * Nz)).
+    void setScale(double forward_scale, double inverse_scale) { DFFT_CALL(dfft_plan_set_scale(plan, forward_scale, inverse_scale)); }
+    void getScale(double& forward_scale, double& inverse_scale) const { DFFT_CALL(dfft_plan_get_scale(plan, &forward_scale, &inverse_scale)); }
     virtual void setWorkArea(void* device = nullptr, void* host = nullptr) { DFFT_CALL(dfft_set_work_area(plan, device, host)); }
     virtual void execR2C(void* out, const void* in) = 0;
 
