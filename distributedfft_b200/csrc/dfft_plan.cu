@@ -32,6 +32,7 @@
 #include <vector>
 
 #include "../../include/dfft.h"
+#include "bluestein.hpp"
 #include "fft_kernels.cuh"
 #include "geometry.hpp"
 
@@ -78,6 +79,32 @@ static cudaError_t make_table(size_t count, size_t denom, void** dev) {
     return cudaMemcpy(*dev, h.data(), count * sizeof(cx<T>), cudaMemcpyHostToDevice);
 }
 
+// Bluestein table of n-point lines: one allocation [K^ (M entries)][chirp (n entries)] (bluestein.hpp)
+template <typename T>
+static cudaError_t make_bluestein_table(size_t n, void** dev) {
+    const std::vector<cx<T>> h = bluestein_table<T>(n);
+    cudaError_t e = cudaMalloc(dev, h.size() * sizeof(cx<T>));
+    if (e != cudaSuccess) return e;
+    return cudaMemcpy(*dev, h.data(), h.size() * sizeof(cx<T>), cudaMemcpyHostToDevice);
+}
+
+// Lengths of C2C axes: powers of two in [2, 2^MAX_LOG2N] (the power-of-two kernels) and any length in [3, BLUESTEIN_MAX_N]
+// (the Bluestein pass)
+static bool bluestein_length(size_t n) { return ilog2_exact(n) < 0 && n >= 3 && n <= size_t(BLUESTEIN_MAX_N); }
+static bool c2c_length(size_t n) { return (ilog2_exact(n) >= 1 && ilog2_exact(n) <= MAX_LOG2N) || bluestein_length(n); }
+
+// A Bluestein pass: the pass' parameters (tw: the M-point table), its table and the output scale
+static cudaError_t launch_bluestein_pass(int prec, int log2m, PassKind kind, const FftParams& prm, size_t n, const void* table, double scale,
+                                         cudaStream_t stream) {
+    FftBluestein b;
+    static_cast<FftParams&>(b) = prm;
+    b.n = int(n);
+    b.kspec = table;
+    b.chirp = table ? static_cast<const char*>(table) + (size_t(1) << log2m) * (prec == DFFT_F64 ? 16 : 8) : nullptr;
+    b.scale = scale;
+    return prec == DFFT_F64 ? launch_bluestein_f64(log2m, kind, b, stream) : launch_bluestein_f32(log2m, kind, b, stream);
+}
+
 struct Tables {
     int prec = DFFT_F64;
     bool dry = false;  // geometry-only plans: no device allocations, segment tables live on the host
@@ -85,6 +112,7 @@ struct Tables {
     std::vector<std::vector<unsigned char>*> dry_store;
     std::map<int, void*> tw;   // log2n -> exp(-2 pi i m / n), m < n
     std::map<int, void*> tw2;  // log2m -> exp(-2 pi i k / 2m), k <= m/2
+    std::map<size_t, void*> blu;  // n -> Bluestein table of n-point lines
     std::vector<void*> bytes;  // seg_of_n tables
     cudaError_t get_tw(int log2n, void** out) {
         if (dry) { *out = nullptr; return cudaSuccess; }
@@ -108,6 +136,18 @@ struct Tables {
             cudaError_t e = prec == DFFT_F64 ? make_table<double>(m / 2 + 1, 2 * m, &d) : make_table<float>(m / 2 + 1, 2 * m, &d);
             if (e != cudaSuccess) return e;
             it = tw2.emplace(log2m, d).first;
+        }
+        *out = it->second;
+        return cudaSuccess;
+    }
+    cudaError_t get_blu(size_t n, void** out) {
+        if (dry) { *out = nullptr; return cudaSuccess; }
+        auto it = blu.find(n);
+        if (it == blu.end()) {
+            void* d = nullptr;
+            cudaError_t e = prec == DFFT_F64 ? make_bluestein_table<double>(n, &d) : make_bluestein_table<float>(n, &d);
+            if (e != cudaSuccess) return e;
+            it = blu.emplace(n, d).first;
         }
         *out = it->second;
         return cudaSuccess;
@@ -142,9 +182,10 @@ struct Tables {
     void release() {
         for (auto& kv : tw) cudaFree(kv.second);
         for (auto& kv : tw2) cudaFree(kv.second);
+        for (auto& kv : blu) cudaFree(kv.second);
         for (void* p : bytes) cudaFree(p);
         for (auto* v : dry_store) delete v;
-        tw.clear(); tw2.clear(); bytes.clear(); dry_store.clear(); host_tabs.clear();
+        tw.clear(); tw2.clear(); blu.clear(); bytes.clear(); dry_store.clear(); host_tabs.clear();
     }
 };
 
@@ -215,6 +256,11 @@ struct Step {
     // PASS
     PassKind kind = PASS_C2C_CONTIG;
     int log2n = 0;
+    // pass length (0: 2^log2n); when it is not 2^log2n the pass runs fft_bluestein_kernel with M = 2^log2n points and the
+    // table `blu`
+    size_t n = 0;
+    const void* blu = nullptr;
+    bool bluestein() const { return n != 0 && n != (size_t(1) << log2n); }
     FftParams prm{};
     int in_user = 0, out_user = 0;  // 1: patch seg[0].base with the caller's in, 2: with the caller's out
     // RENDEZVOUS
@@ -393,6 +439,10 @@ static SegN mkseg(void* base, long long sA0, long long sA1, long long sN, size_t
     return r;
 }
 
+// Whether every axis is a power of two.  Plans with another length run the sequential schedule only: the overlapped
+// schedules build their passes for power-of-two lengths.
+static bool pow2_axes(const dfft_plan_s* p) { return ilog2_exact(p->g.nx) > 0 && ilog2_exact(p->g.ny) > 0 && ilog2_exact(p->g.nz) > 0; }
+
 // Whether the z and y passes run as one fused launch (fft_zy_fused_kernel): one-rank slab C2C plans of the full 3D
 // transform with Ny == Nz of an instantiated length (zy_fused_length) whose array is larger than the L2 — below that the
 // three passes are L2-resident already and gain nothing.
@@ -502,6 +552,13 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         s.kind = kind;
         s.phase = phase;
         s.log2n = ilog2_exact(n);
+        s.n = n;
+        if ((kind == PASS_C2C_CONTIG || kind == PASS_C2C_TILED) && bluestein_length(n)) {
+            s.log2n = bluestein_log2m(n);  // the view mapping stays the kind's; the exec launches the Bluestein kernel
+            void* blu = nullptr;
+            if (T.get_blu(n, &blu) != cudaSuccess) return fail(DFFT_ERR_CUDA, "Bluestein table allocation failed");
+            s.blu = blu;
+        }
         if (s.log2n < 1 || s.log2n > MAX_LOG2N)
             return fail(DFFT_ERR_UNSUPPORTED, "axis length " + std::to_string(n) + " is not a supported power of two (2..8192)");
         s.prm.A0 = 1; s.prm.A1 = 1; s.prm.B = 1;
@@ -1936,6 +1993,8 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
                                             : launch_batch_small_f32(s.log2n, prm.in.seg[0].base, prm.out.seg[0].base, (long long)p->batch, s.prm.inverse, s.bsf, scale, ss);
                 } else if (s.zy) {
                     e = p->prec == DFFT_F64 ? launch_zy_fused_f64(s.log2n, prm, s.prm_y, s.zyf, scale, ss) : launch_zy_fused_f32(s.log2n, prm, s.prm_y, s.zyf, scale, ss);
+                } else if (s.bluestein()) {
+                    e = launch_bluestein_pass(p->prec, s.log2n, s.kind, prm, s.n, s.blu, scale, ss);
                 } else {
                     e = p->prec == DFFT_F64 ? launch_pass_f64(s.log2n, s.kind, prm, scale, ss) : launch_pass_f32(s.log2n, s.kind, prm, scale, ss);
                 }
@@ -2004,13 +2063,15 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
         g_view_error = false;
         const bool streams = p->cfg.send_method == DFFT_SEND_STREAMS || (p->g.decomp == DFFT_PENCIL && p->cfg.send_method2 == DFFT_SEND_STREAMS);
         const bool seq_won = p->tuned_seq[inverse ? 1 : 0] != 0;
-        const bool want_overlap = streams && d == 3 && p->P > 1 && p->g.decomp == DFFT_SLAB_ZY_THEN_X && p->direct2 && p->xchg_ctas >= 0 && !seq_won;
+        const bool want_overlap = streams && d == 3 && p->P > 1 && p->g.decomp == DFFT_SLAB_ZY_THEN_X && p->direct2 && p->xchg_ctas >= 0 && !seq_won &&
+                                  pow2_axes(p);
         // pencil: forward on a grid with two real transpositions by default; every other
         // combination (inverse, p1 or p2 == 1) only once dfft_plan_tune has measured it faster than the sequential schedule
         const bool both_multi = p->grp[1].size() > 1 && p->grp[2].size() > 1;
         const bool tuned = p->tuned_ctas[inverse ? 1 : 0] != -2;
         const bool want_pencil_overlap = streams && d == 3 && p->g.decomp == DFFT_PENCIL && p->direct1 && p->direct2 && p->P > 1 && p->xchg_ctas >= 0 &&
-                                         pencil_overlap_enabled() && !seq_won && ((both_multi && !inverse) || tuned || pencil_overlap_mode() == 2);
+                                         pencil_overlap_enabled() && !seq_won && ((both_multi && !inverse) || tuned || pencil_overlap_mode() == 2) &&
+                                         pow2_axes(p);
         int rc;
         if (batch_small(p, d)) rc = build_batch_small(p, inverse ? 1 : 0, sc);
         else if (want_overlap) rc = build_overlapped_slab(p, inverse ? 1 : 0, sc);
@@ -2270,8 +2331,13 @@ int dfft_plan_create_batched(dfft_comm_t comm, const dfft_config* config, int de
         return fail(DFFT_ERR_INVALID, "invalid partition: P1*P2 must equal the communicator size");
     }
     const Geometry& g = p->g;
-    if (ilog2_exact(nx) < 1 || ilog2_exact(ny) < 1 || ilog2_exact(nz) < 1 || ilog2_exact(nx) > MAX_LOG2N || ilog2_exact(ny) > MAX_LOG2N ||
-        ilog2_exact(nz) > MAX_LOG2N + (transform == DFFT_R2C ? 1 : 0) || (transform == DFFT_R2C && nz < 4)) {
+    if (transform == DFFT_C2C) {
+        if (!c2c_length(nx) || !c2c_length(ny) || !c2c_length(nz)) {
+            delete p;
+            return fail(DFFT_ERR_UNSUPPORTED, "Nx, Ny, Nz of C2C plans must be powers of two in [2, 8192] or any length in [3, 4096]");
+        }
+    } else if (ilog2_exact(nx) < 1 || ilog2_exact(ny) < 1 || ilog2_exact(nz) < 1 || ilog2_exact(nx) > MAX_LOG2N || ilog2_exact(ny) > MAX_LOG2N ||
+               ilog2_exact(nz) > MAX_LOG2N + 1 || nz < 4) {
         delete p;
         return fail(DFFT_ERR_UNSUPPORTED, "Nx, Ny, Nz must be powers of two in [2, 8192] (Nz >= 4 for R2C)");
     }
@@ -2647,7 +2713,7 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
     std::vector<Cand> cands;
     cands.push_back({1, 0, 0, 0});
     const bool streams = p->cfg.send_method == DFFT_SEND_STREAMS || (p->g.decomp == DFFT_PENCIL && p->cfg.send_method2 == DFFT_SEND_STREAMS);
-    const bool has_overlap = streams && p->P > 1 && p->xchg_ctas >= 0 &&
+    const bool has_overlap = streams && p->P > 1 && p->xchg_ctas >= 0 && pow2_axes(p) &&
                              ((p->g.decomp == DFFT_SLAB_ZY_THEN_X && p->direct2) ||
                               (p->g.decomp == DFFT_PENCIL && p->direct1 && p->direct2 && pencil_overlap_enabled()));
     const bool pencil_inv = inverse && p->g.decomp == DFFT_PENCIL;
@@ -2668,7 +2734,8 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
     }
     p->tune_report.clear();
     if (cands.size() == 1) {
-        p->tune_report = "sequential schedule (no alternatives for this plan)";
+        p->tune_report = pow2_axes(p) ? "sequential schedule (no alternatives for this plan)"
+                                      : "sequential schedule (no alternatives for this plan: an axis length is not a power of two)";
         return 0;
     }
     const bool was_timing = p->timing;
@@ -2884,7 +2951,8 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
         for (size_t w = 0; w < s_.waits.size(); ++w) o += (w ? "," : "") + std::to_string(s_.waits[w]);
         o += "]";
         if (s_.type == STEP_PASS) {
-            o += ",\"kind\":" + std::to_string(int(s_.kind)) + ",\"log2n\":" + std::to_string(s_.log2n) + ",\"A0\":" + std::to_string(s_.prm.A0) +
+            o += ",\"kind\":" + std::to_string(int(s_.kind)) + ",\"log2n\":" + std::to_string(s_.log2n) +
+                 (s_.bluestein() ? ",\"n\":" + std::to_string(s_.n) : std::string()) + ",\"A0\":" + std::to_string(s_.prm.A0) +
                  ",\"A1\":" + std::to_string(s_.prm.A1) + ",\"B\":" + std::to_string(s_.prm.B) + ",\"inverse\":" + std::to_string(s_.prm.inverse) +
                  ",\"in_user\":" + std::to_string(s_.in_user) + ",\"out_user\":" + std::to_string(s_.out_user) + ",\"in\":";
             json_view(o, s_.prm.in, p->tabs);
@@ -2948,10 +3016,44 @@ static int cached_table(bool second, int prec, int log2n, void** out) {
     return DFFT_SUCCESS;
 }
 
+static std::map<std::pair<int, size_t>, void*> g_blu_cache;  // (prec, n)
+
+// C2C lines of a length that is not a power of two: the Bluestein pass, with the (prec, device, n) table cached like
+// the twiddle tables
+static int fft1d_bluestein(int prec, PassKind kind, size_t n, const FftParams& prm_in, void* stream) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    const int l2 = bluestein_log2m(n);
+    const auto key = std::make_pair(prec * 64 + dev, n);
+    auto it = g_blu_cache.find(key);
+    if (it == g_blu_cache.end()) {
+        void* d = nullptr;
+        cudaError_t e = prec == DFFT_F64 ? make_bluestein_table<double>(n, &d) : make_bluestein_table<float>(n, &d);
+        if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, "Bluestein table allocation failed");
+        it = g_blu_cache.emplace(key, d).first;
+    }
+    FftParams prm = prm_in;
+    void* tw = nullptr;
+    int rc = cached_table(false, prec, l2, &tw);
+    if (rc) return rc;
+    prm.tw = tw;
+    cudaError_t e = launch_bluestein_pass(prec, l2, kind, prm, n, it->second, 1.0, (cudaStream_t)stream);
+    if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("launch failed: ") + cudaGetErrorString(e));
+    return DFFT_SUCCESS;
+}
+
 int dfft_fft1d_contig(int precision, int kind, int direction, size_t n, size_t lines, void* out, size_t out_pitch, const void* in,
                       size_t in_pitch, void* stream) {
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
     if (kind < 0 || kind > 2) return fail(DFFT_ERR_INVALID, "bad kind");
+    if (kind == 0 && bluestein_length(n)) {
+        FftParams prm{};
+        prm.A0 = 1; prm.A1 = int(lines); prm.B = 1;
+        prm.inverse = direction > 0 ? 1 : 0;
+        prm.in = single_view(const_cast<void*>(in), 0, (long long)in_pitch, 1);
+        prm.out = single_view(out, 0, (long long)out_pitch, 1);
+        return fft1d_bluestein(precision, PASS_C2C_CONTIG, n, prm, stream);
+    }
     const size_t len = kind == 0 ? n : n / 2;
     const int l2 = ilog2_exact(len);
     if (ilog2_exact(n) < 1 || l2 < 1 || l2 > MAX_LOG2N) return fail(DFFT_ERR_UNSUPPORTED, "length must be a power of two");
@@ -2978,10 +3080,15 @@ int dfft_fft1d_contig(int precision, int kind, int direction, size_t n, size_t l
 int dfft_fft1d_strided(int precision, int direction, size_t a, size_t n, size_t b, void* out, const void* in, void* stream) {
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
     const int l2 = ilog2_exact(n);
-    if (l2 < 1 || l2 > MAX_LOG2N) return fail(DFFT_ERR_UNSUPPORTED, "length must be a power of two");
+    if (!c2c_length(n)) return fail(DFFT_ERR_UNSUPPORTED, "length must be a power of two in [2, 8192] or any length in [3, 4096]");
     FftParams prm{};
     prm.A0 = int(a); prm.A1 = 1; prm.B = int(b);
     prm.inverse = direction > 0 ? 1 : 0;
+    if (bluestein_length(n)) {
+        prm.in = single_view(const_cast<void*>(in), (long long)(n * b), 0, (long long)b);
+        prm.out = single_view(out, (long long)(n * b), 0, (long long)b);
+        return fft1d_bluestein(precision, PASS_C2C_TILED, n, prm, stream);
+    }
     void* tw = nullptr;
     int rc = cached_table(false, precision, l2, &tw);
     if (rc) return rc;
@@ -2998,10 +3105,15 @@ int dfft_fft1d_general(int precision, int direction, size_t n, size_t a0, size_t
                        const void* in, const long long in_strides[3], void* stream) {
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
     const int l2 = ilog2_exact(n);
-    if (l2 < 1 || l2 > MAX_LOG2N) return fail(DFFT_ERR_UNSUPPORTED, "length must be a power of two");
+    if (!c2c_length(n)) return fail(DFFT_ERR_UNSUPPORTED, "length must be a power of two in [2, 8192] or any length in [3, 4096]");
     FftParams prm{};
     prm.A0 = int(a0); prm.A1 = int(a1); prm.B = int(b);
     prm.inverse = direction > 0 ? 1 : 0;
+    if (bluestein_length(n)) {
+        prm.in = single_view(const_cast<void*>(in), in_strides[0], in_strides[1], in_strides[2]);
+        prm.out = single_view(out, out_strides[0], out_strides[1], out_strides[2]);
+        return fft1d_bluestein(precision, PASS_C2C_TILED, n, prm, stream);
+    }
     void* tw = nullptr;
     int rc = cached_table(false, precision, l2, &tw);
     if (rc) return rc;

@@ -24,6 +24,27 @@ cudaError_t launch_pass_f32(int log2n, PassKind kind, const FftParams& p, double
     }
 }
 
+#define DFFT_BLU_DECL(T, L) extern template cudaError_t launch_bluestein<T, L>(PassKind, const FftBluestein&, cudaStream_t);
+#define DFFT_BLU_ALL(M, T) M(T, 3) M(T, 4) M(T, 5) M(T, 6) M(T, 7) M(T, 8) M(T, 9) M(T, 10) M(T, 11) M(T, 12) M(T, 13)
+DFFT_BLU_ALL(DFFT_BLU_DECL, double)
+DFFT_BLU_ALL(DFFT_BLU_DECL, float)
+
+#define DFFT_BLU_CASE(T, L) \
+    case L: return launch_bluestein<T, L>(kind, p, stream);
+
+cudaError_t launch_bluestein_f64(int log2m, PassKind kind, const FftBluestein& p, cudaStream_t stream) {
+    switch (log2m) {
+        DFFT_BLU_ALL(DFFT_BLU_CASE, double)
+        default: return cudaErrorInvalidValue;
+    }
+}
+cudaError_t launch_bluestein_f32(int log2m, PassKind kind, const FftBluestein& p, cudaStream_t stream) {
+    switch (log2m) {
+        DFFT_BLU_ALL(DFFT_BLU_CASE, float)
+        default: return cudaErrorInvalidValue;
+    }
+}
+
 #define DFFT_ZY_DECL(T, L) \
     extern template cudaError_t launch_zy_fused<T, L>(const FftParams&, const FftParams&, const ZyFused&, double, cudaStream_t);
 DFFT_ZY_DECL(double, 8) DFFT_ZY_DECL(double, 9) DFFT_ZY_DECL(float, 8) DFFT_ZY_DECL(float, 9)

@@ -247,6 +247,45 @@ cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStr
 
 template cudaError_t launch_pass<DFFT_T, DFFT_LOG2N>(PassKind, const FftParams&, double, cudaStream_t);
 
+#if DFFT_LOG2N >= 3
+template <typename T, int LOG2M, int TB, bool TILED>
+static cudaError_t launch_bluestein_tiles(const FftBluestein& p, long long grid, cudaStream_t stream) {
+    using C = CtaFft<T, LOG2M, Shape<T, LOG2M>::LOG2E, TB, TILED>;
+    auto kf = fft_bluestein_kernel<T, LOG2M, Shape<T, LOG2M>::LOG2E, TB, TILED, false>;
+    auto ki = fft_bluestein_kernel<T, LOG2M, Shape<T, LOG2M>::LOG2E, TB, TILED, true>;
+    static cudaError_t once = set_smem(kf, C::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ki, C::SMEM_BYTES);
+    if (once != cudaSuccess) return once;
+    if (grid <= 0) return cudaSuccess;
+    if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+    if (p.inverse) ki<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(p);
+    else kf<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(p);
+    return cudaGetLastError();
+}
+
+template <typename T, int LOG2M>
+cudaError_t launch_bluestein(PassKind kind, const FftBluestein& p_in, cudaStream_t stream) {
+    using S = Shape<T, LOG2M>;
+    if (p_in.n < 1 || 2 * (long long)p_in.n - 1 > (1LL << LOG2M) || !p_in.chirp || !p_in.kspec) return cudaErrorInvalidValue;
+    const long long lines = (long long)p_in.A0 * p_in.A1;
+    if (lines <= 0) return cudaSuccess;
+    FftBluestein p = p_in;
+    if (kind == PASS_C2C_CONTIG) {
+        if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
+        return launch_bluestein_tiles<T, LOG2M, S::TBC, false>(p, (lines + S::TBC - 1) / S::TBC, stream);
+    }
+    if (kind != PASS_C2C_TILED) return cudaErrorInvalidValue;
+    // the tile-order blocking of launch_tiled, where the batch extents allow it
+    if (p.tile_swz > 0) {
+        const int G = 1 << p.tile_swz;
+        if (p.tile_swz > 4 || p.A0 % G || p.A1 % G) p.tile_swz = 0;
+    } else p.tile_swz = 0;
+    if (p.B <= 0) return cudaSuccess;
+    return launch_bluestein_tiles<T, LOG2M, S::TBT, true>(p, lines * ((p.B + S::TBT - 1) / S::TBT), stream);
+}
+
+template cudaError_t launch_bluestein<DFFT_T, DFFT_LOG2N>(PassKind, const FftBluestein&, cudaStream_t);
+#endif
+
 #if DFFT_LOG2N == 8 || DFFT_LOG2N == 9
 static bool aligned128(const void* base, long long elems_a, long long elems_b, long long elems_c) {
     constexpr long long es = sizeof(cx<DFFT_T>);

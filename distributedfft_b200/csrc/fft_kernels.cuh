@@ -1134,6 +1134,79 @@ fft_c2r_kernel(const __grid_constant__ KParams<SCALED> p) {
     }
 }
 
+// ---- Bluestein pass: C2C lines of any length n through two transforms of length M = 2^LOG2M >= 2n - 1 ----------------
+// X_k = c_k * IDFT_M(DFT_M(y) * K^)_k with c_k = exp(-pi i k^2 / n), y_k = x_k c_k (k < n, 0 up to M), and K^ the M-point
+// spectrum of the conjugate chirp, divided by M (host tables, bluestein.hpp).  Both transforms are CtaFft's stages on the
+// tile of the power-of-two kernels; the inverse DFT_M is swap(DFT_M(swap(.))), and the inverse direction swaps re/im on
+// load and store as every kernel here does, so only forward tables exist.  One CTA per tile: every CTA reads all of its
+// points before it stores, and tiles are disjoint, so out == in works.  The parameters of the other kernels are unchanged.
+struct FftBluestein : FftParams {
+    int n;              // line length
+    const void* chirp;  // c_k, k < n
+    const void* kspec;  // K^_m, m < M
+    double scale;       // output scale, applied when != 1 (rounded to the kernel's precision once)
+};
+
+template <typename T, int LOG2M, int LOG2E, int TB, bool TILED, bool INV>
+__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
+fft_bluestein_kernel(const __grid_constant__ FftBluestein p) {
+    using C = CtaFft<T, LOG2M, LOG2E, TB, TILED>;
+    using LA = LineAccess<T, C::LINES>;
+    using TC = TileCoord<C, TILED, TB>;
+    constexpr int E = C::E, TPL = C::TPL;
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
+    unsigned long long* tab_in = reinterpret_cast<unsigned long long*>(smem_raw + C::TILE_BYTES);
+    unsigned long long* tab_out = tab_in + C::LINES * MAXSEG;
+    const TC tc(p, blockIdx.x);
+    const int j = tc.j, t = tc.t, n = p.n;
+    if (p.in.nseg > 1 || p.out.nseg > 1) {
+        const int line = TILED ? 0 : t;
+        const int lane = TILED ? int(threadIdx.x) : j;
+        const int lanes = TILED ? C::THREADS : TPL;
+        LA::fill_table(p.in, tab_in, line, lane, lanes, tc.a0, tc.a1);
+        LA::fill_table(p.out, tab_out, line, lane, lanes, tc.a0, tc.a1);
+        __syncthreads();
+    }
+    const LA in(p.in, tab_in, TILED ? 0 : t, tc.a0, tc.a1, tc.b);
+    const LA out(p.out, tab_out, TILED ? 0 : t, tc.a0, tc.a1, tc.b);
+    const cx<T>* chirp = reinterpret_cast<const cx<T>*>(p.chirp);
+    const cx<T>* kspec = reinterpret_cast<const cx<T>*>(p.kspec);
+    const cx<T>* tw = reinterpret_cast<const cx<T>*>(p.tw);
+
+    // y = x * c, zero-padded to M
+    cx<T> v[E];
+#pragma unroll
+    for (int e = 0; e < E; ++e) {
+        const int k = j + e * TPL;
+        v[e] = cx<T>{T(0), T(0)};
+        if (tc.valid && k < n) {
+            const cx<T> x = ld_elem<T>(TILED ? in.at(k) : in.at1(k));
+            v[e] = cmul(INV ? cswap(x) : x, ld_tw(chirp, k));
+        }
+    }
+    C::template stages<0>(v, j, t, sm, tw);
+    // Y[j + e*TPL] sits in slot final_slot(e); the second transform takes it in slot e, pre-swapped for the inverse DFT
+    cx<T> z[E];
+#pragma unroll
+    for (int e = 0; e < E; ++e) z[e] = cswap(cmul(v[C::Core::final_slot(e)], ld_tw(kspec, j + e * TPL)));
+    if constexpr (C::NST > 1) C::sync(t);  // the first transform's last gather is done before the second's first scatter
+    C::template stages<0>(z, j, t, sm, tw);
+
+    const bool scaled = p.scale != 1.0;
+    const T s = T(p.scale);
+#pragma unroll
+    for (int e = 0; e < E; ++e) {
+        const int k = j + e * TPL;
+        if (tc.valid && k < n) {
+            cx<T> x = cmul(ld_tw(chirp, k), cswap(z[C::Core::final_slot(e)]));
+            if (INV) x = cswap(x);
+            if (scaled) x = cscale<T>(x, s);
+            st_elem<T>(TILED ? out.at(k) : out.at1(k), x);
+        }
+    }
+}
+
 // ---- host launchers (one explicit instantiation per precision and size, see fft_inst.cu) ----------------
 // scale: the output scale of the pass' stores; 1 launches the unscaled kernels, anything else their scaled twins.
 template <typename T, int LOG2N>
@@ -1162,6 +1235,14 @@ cudaError_t launch_batch_small(const void* in, void* out, long long batch, int i
 cudaError_t launch_batch_small_f64(int log2n, const void* in, void* out, long long batch, int inverse, const BatchSmall& f, double scale, cudaStream_t stream);
 cudaError_t launch_batch_small_f32(int log2n, const void* in, void* out, long long batch, int inverse, const BatchSmall& f, double scale, cudaStream_t stream);
 
+// Bluestein pass (fft_bluestein_kernel) of p.n-point lines, M = 2^LOG2M >= 2 p.n - 1: kind PASS_C2C_CONTIG or PASS_C2C_TILED
+// (the view mapping of the power-of-two pass), one CTA per tile; p.scale scales the stores.  Instantiated for LOG2M 3..13.
+template <typename T, int LOG2M>
+cudaError_t launch_bluestein(PassKind kind, const FftBluestein& p, cudaStream_t stream);
+cudaError_t launch_bluestein_f64(int log2m, PassKind kind, const FftBluestein& p, cudaStream_t stream);
+cudaError_t launch_bluestein_f32(int log2m, PassKind kind, const FftBluestein& p, cudaStream_t stream);
+
 constexpr int MAX_LOG2N = 13;
+constexpr int BLUESTEIN_MAX_N = 4096;  // 2n - 1 <= 2^MAX_LOG2N
 
 }  // namespace dfft

@@ -92,7 +92,11 @@ int dfft_comm_size(dfft_comm_t comm);
 
 /* ---- plan = constructor + initFFT (mpicufft_slab.cpp:97-233, mpicufft_pencil.cpp:63-342) ---------- */
 /* p1,p2: Partition{P1,P2} (params.hpp:39-56); slab decompositions ignore them and use the communicator
- * size.  allocate != 0: the plan allocates (and owns) its device work area, like initFFT(.., true). */
+ * size.  allocate != 0: the plan allocates (and owns) its device work area, like initFFT(.., true).
+ * Axis lengths: C2C plans take, per axis, a power of two in [2, 8192] or any length in [3, 4096] (lengths that are not
+ * powers of two run a Bluestein pass: two FFTs of the next power of two >= 2n - 1 per line, slower than a power-of-two
+ * pass of similar size, and always the sequential schedule); R2C plans take powers of two in [2, 8192] (Nz in [4, 16384]).
+ * Other lengths: DFFT_ERR_UNSUPPORTED. */
 int dfft_plan_create(dfft_comm_t comm, const dfft_config* config, int decomp /*dfft_decomp*/,
                      int precision /*dfft_prec*/, int transform /*dfft_transform*/, size_t nx, size_t ny,
                      size_t nz, size_t p1, size_t p2, int allocate, dfft_plan_t* plan);
@@ -244,8 +248,10 @@ const char* dfft_last_error_string(void);
 int dfft_version(void);
 
 /* ---- single-axis building block (what one cufftExec* of the reference's plans computes) ------------
- * Batched 1D transform of `lines` contiguous lines of length n (power of two) on the current device.
- * kind: 0 C2C, 1 R2C (n real -> n/2+1 complex), 2 C2R.  Exposed for tests and micro-benchmarks. */
+ * Batched 1D transform of `lines` contiguous lines of length n on the current device.
+ * kind: 0 C2C, 1 R2C (n real -> n/2+1 complex), 2 C2R.  Exposed for tests and micro-benchmarks.
+ * Lengths: C2C (kind 0, dfft_fft1d_strided, dfft_fft1d_general) a power of two in [2, 8192] or any length in [3, 4096];
+ * R2C / C2R powers of two only.  Other lengths: DFFT_ERR_UNSUPPORTED.  out == in is allowed. */
 int dfft_fft1d_contig(int precision, int kind, int direction, size_t n, size_t lines, void* out,
                       size_t out_pitch, const void* in, size_t in_pitch, void* stream);
 /* Batched 1D C2C along the middle axis of a [a][n][b] array (b contiguous). */
