@@ -93,16 +93,20 @@ static cudaError_t make_bluestein_table(size_t n, void** dev) {
 static bool bluestein_length(size_t n) { return ilog2_exact(n) < 0 && n >= 3 && n <= size_t(BLUESTEIN_MAX_N); }
 static bool c2c_length(size_t n) { return (ilog2_exact(n) >= 1 && ilog2_exact(n) <= MAX_LOG2N) || bluestein_length(n); }
 
-// A Bluestein pass: the pass' parameters (tw: the M-point table), its table and the output scale
-static cudaError_t launch_bluestein_pass(int prec, int log2m, PassKind kind, const FftParams& prm, size_t n, const void* table, double scale,
-                                         cudaStream_t stream) {
+// One FFT pass of n-point lines (R2C / C2R: n complex points) over the views of prm, its stores scaled by `scale`: the
+// power-of-two kernels, or the Bluestein pass when n is not a power of two (prm.tw: the M-point table; blu: the Bluestein
+// table of n)
+static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftParams& prm, const void* blu, double scale, cudaStream_t stream) {
+    const int log2n = ilog2_exact(n);
+    if (log2n >= 0) return launch_pass(prec, log2n, kind, prm, scale, stream);
+    const int log2m = bluestein_log2m(n);
     FftBluestein b;
     static_cast<FftParams&>(b) = prm;
     b.n = int(n);
-    b.kspec = table;
-    b.chirp = table ? static_cast<const char*>(table) + (size_t(1) << log2m) * (prec == DFFT_F64 ? 16 : 8) : nullptr;
+    b.kspec = blu;
+    b.chirp = blu ? static_cast<const char*>(blu) + (size_t(1) << log2m) * (prec == DFFT_F64 ? 16 : 8) : nullptr;
     b.scale = scale;
-    return prec == DFFT_F64 ? launch_bluestein_f64(log2m, kind, b, stream) : launch_bluestein_f32(log2m, kind, b, stream);
+    return launch_bluestein(prec, log2m, kind, b, stream);
 }
 
 struct Tables {
@@ -248,12 +252,15 @@ struct dfft_comm_s {
 namespace dfft {
 
 enum StepType { STEP_PASS = 0, STEP_RENDEZVOUS = 1, STEP_A2A = 2 };
+// the kernel a PASS step launches: one FFT pass, the fused z + y stage or the batched stage of small cubic fields
+enum StepKernel { KERNEL_PASS = 0, KERNEL_ZY_FUSED = 1, KERNEL_BATCH_SMALL = 2 };
 
 struct Step {
     StepType type = STEP_PASS;
     const char* phase = nullptr;  // timer section recorded after this step
     const char* label = "";       // short name of the step ("z pass", "y pass", "rendezvous 2", ...)
     // PASS
+    StepKernel kernel = KERNEL_PASS;
     PassKind kind = PASS_C2C_CONTIG;
     int log2n = 0;
     // pass length (0: 2^log2n); when it is not 2^log2n the pass runs fft_bluestein_kernel with M = 2^log2n points and the
@@ -273,14 +280,12 @@ struct Step {
     int stream = 0;
     std::vector<int> waits;
     int record = -1;
-    // fused z + y stage (fft_zy_fused_kernel): prm is the z pass, prm_y the y pass; zyf holds the counters, advanced by
-    // every launch on the device
-    bool zy = false;
+    // fused z + y stage (KERNEL_ZY_FUSED): prm is the z pass, prm_y the y pass; zyf holds the counters, advanced by every
+    // launch on the device
     FftParams prm_y{};
     ZyFused zyf{};
-    // batched small cubic fields (fft_batch_small_kernel): one launch for every field; prm.in / prm.out are the caller's
+    // batched small cubic fields (KERNEL_BATCH_SMALL): one launch for every field; prm.in / prm.out are the caller's
     // buffers, bsf holds the counters
-    bool batch_small = false;
     BatchSmall bsf{};
     // its stores are output values of the exec (the fused and batched stages: those of their last phase), so it runs the
     // scaled twin of its kernel when the plan's output scale for the direction is not 1 (dfft_plan_set_scale)
@@ -459,7 +464,7 @@ static bool zy_fused(const dfft_plan_s* p, int inverse, int d) {
 static int fuse_zy(dfft_plan_s* p, Step zs, const Step& ys, const char* label, const char* phase, Step& out) {
     if (zs.log2n != ys.log2n) return fail(DFFT_ERR_STATE, "internal: fused z + y stage needs Ny == Nz");
     out = zs;
-    out.zy = true;
+    out.kernel = KERNEL_ZY_FUSED;
     out.label = label;
     out.phase = phase;
     out.prm_y = ys.prm;
@@ -503,7 +508,7 @@ static int build_batch_small(dfft_plan_s* p, int inverse, Schedule& sc) {
     sc.whole_batch = true;
     Step s;
     s.type = STEP_PASS;
-    s.batch_small = true;
+    s.kernel = KERNEL_BATCH_SMALL;
     s.label = "batched pass";
     s.phase = inverse ? "2D FFT Y-Z-Direction" : "1D FFT X-Direction";  // the exec's last section
     s.kind = PASS_C2C_CONTIG;
@@ -1987,16 +1992,13 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
                 // views on the caller's buffers store a byte offset in seg[0].base (field f starts f field sizes further)
                 if (s.in_user == 1) prm.in.seg[0].base = (char*)const_cast<void*>(in) + f * sc.field_in + (size_t)s.prm.in.seg[0].base;
                 if (s.out_user == 2) prm.out.seg[0].base = (char*)out + f * sc.field_out + (size_t)s.prm.out.seg[0].base;
-                cudaError_t e;
-                if (s.batch_small) {
-                    e = p->prec == DFFT_F64 ? launch_batch_small_f64(s.log2n, prm.in.seg[0].base, prm.out.seg[0].base, (long long)p->batch, s.prm.inverse, s.bsf, scale, ss)
-                                            : launch_batch_small_f32(s.log2n, prm.in.seg[0].base, prm.out.seg[0].base, (long long)p->batch, s.prm.inverse, s.bsf, scale, ss);
-                } else if (s.zy) {
-                    e = p->prec == DFFT_F64 ? launch_zy_fused_f64(s.log2n, prm, s.prm_y, s.zyf, scale, ss) : launch_zy_fused_f32(s.log2n, prm, s.prm_y, s.zyf, scale, ss);
-                } else if (s.bluestein()) {
-                    e = launch_bluestein_pass(p->prec, s.log2n, s.kind, prm, s.n, s.blu, scale, ss);
-                } else {
-                    e = p->prec == DFFT_F64 ? launch_pass_f64(s.log2n, s.kind, prm, scale, ss) : launch_pass_f32(s.log2n, s.kind, prm, scale, ss);
+                cudaError_t e = cudaErrorInvalidValue;
+                switch (s.kernel) {
+                    case KERNEL_PASS: e = launch_fft_pass(p->prec, s.kind, s.n ? s.n : size_t(1) << s.log2n, prm, s.blu, scale, ss); break;
+                    case KERNEL_ZY_FUSED: e = launch_zy_fused(p->prec, s.log2n, prm, s.prm_y, s.zyf, scale, ss); break;
+                    case KERNEL_BATCH_SMALL:
+                        e = launch_batch_small(p->prec, s.log2n, prm.in.seg[0].base, prm.out.seg[0].base, (long long)p->batch, s.prm.inverse, s.bsf, scale, ss);
+                        break;
                 }
                 if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("FFT pass launch failed: ") + cudaGetErrorString(e));
                 ++launches;
@@ -2863,9 +2865,9 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
     bool first = true;
     std::vector<Step> listed;  // the fused z + y stage is listed as its two phases, in the order they consume data
     for (const Step& s_ : sc.steps) {
-        if (!s_.zy) { listed.push_back(s_); continue; }
+        if (s_.kernel != KERNEL_ZY_FUSED) { listed.push_back(s_); continue; }
         Step z = s_, y = s_;
-        z.zy = y.zy = false;
+        z.kernel = y.kernel = KERNEL_PASS;
         y.kind = PASS_C2C_TILED;
         y.prm = s_.prm_y;
         y.in_user = y.out_user = 0;
@@ -2885,10 +2887,10 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
     if (sc.whole_batch) {
         std::vector<Step> all;
         for (const Step& s_ : listed) {
-            if (!s_.batch_small) { all.push_back(s_); continue; }
+            if (s_.kernel != KERNEL_BATCH_SMALL) { all.push_back(s_); continue; }
             const long long N = (long long)p->g.nx, N2 = N * N, N3 = N2 * N, B = (long long)p->batch;
             Step z = s_, y = s_, x = s_;
-            z.batch_small = y.batch_small = x.batch_small = false;
+            z.kernel = y.kernel = x.kernel = KERNEL_PASS;
             z.kind = PASS_C2C_CONTIG; z.label = "batched pass: z lines";
             z.prm.A0 = int(B * N); z.prm.A1 = int(N); z.prm.B = 1;
             z.prm.in = z.prm.out = single_view(nullptr, N2, N, 1);
@@ -2995,49 +2997,28 @@ int dfft_timer_gather(dfft_plan_t p) {
 const char* dfft_timer_csv_path(dfft_plan_t p) { return p ? p->csv_path.c_str() : nullptr; }
 
 // ---- single-axis building blocks -----------------------------------------------------------------------
-static std::map<std::pair<int, int>, void*> g_tw_cache, g_tw2_cache;  // (prec, log2n)
-
-static int cached_table(bool second, int prec, int log2n, void** out) {
+// Tables of the single-axis calls: one Tables per (precision, device), process-wide and never freed
+static Tables& fft1d_tables(int prec) {
+    static std::map<std::pair<int, int>, Tables> tabs;
     int dev = 0;
     cudaGetDevice(&dev);
-    auto& cache = second ? g_tw2_cache : g_tw_cache;
-    auto key = std::make_pair(prec * 64 + dev, log2n);
-    auto it = cache.find(key);
-    if (it == cache.end()) {
-        void* d = nullptr;
-        size_t n = size_t(1) << log2n;
-        cudaError_t e;
-        if (!second) e = prec == DFFT_F64 ? make_table<double>(n, n, &d) : make_table<float>(n, n, &d);
-        else e = prec == DFFT_F64 ? make_table<double>(n / 2 + 1, 2 * n, &d) : make_table<float>(n / 2 + 1, 2 * n, &d);
-        if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
-        it = cache.emplace(key, d).first;
-    }
-    *out = it->second;
-    return DFFT_SUCCESS;
+    Tables& T = tabs[std::make_pair(prec, dev)];
+    T.prec = prec;
+    return T;
 }
 
-static std::map<std::pair<int, size_t>, void*> g_blu_cache;  // (prec, n)
-
-// C2C lines of a length that is not a power of two: the Bluestein pass, with the (prec, device, n) table cached like
-// the twiddle tables
-static int fft1d_bluestein(int prec, PassKind kind, size_t n, const FftParams& prm_in, void* stream) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    const int l2 = bluestein_log2m(n);
-    const auto key = std::make_pair(prec * 64 + dev, n);
-    auto it = g_blu_cache.find(key);
-    if (it == g_blu_cache.end()) {
-        void* d = nullptr;
-        cudaError_t e = prec == DFFT_F64 ? make_bluestein_table<double>(n, &d) : make_bluestein_table<float>(n, &d);
-        if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, "Bluestein table allocation failed");
-        it = g_blu_cache.emplace(key, d).first;
-    }
-    FftParams prm = prm_in;
-    void* tw = nullptr;
-    int rc = cached_table(false, prec, l2, &tw);
-    if (rc) return rc;
-    prm.tw = tw;
-    cudaError_t e = launch_bluestein_pass(prec, l2, kind, prm, n, it->second, 1.0, (cudaStream_t)stream);
+// one pass of n-point lines over prm's views (R2C / C2R: n complex points), with the tables of its length
+static int fft1d_pass(int prec, PassKind kind, size_t n, FftParams prm, void* stream) {
+    Tables& T = fft1d_tables(prec);
+    const bool blu = bluestein_length(n);
+    const int l2 = blu ? bluestein_log2m(n) : ilog2_exact(n);
+    void *tw = nullptr, *tw2 = nullptr, *table = nullptr;
+    if (blu && T.get_blu(n, &table) != cudaSuccess) return fail(DFFT_ERR_CUDA, "Bluestein table allocation failed");
+    if (T.get_tw(l2, &tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
+    if ((kind == PASS_R2C || kind == PASS_C2R) && T.get_tw2(l2, &tw2) != cudaSuccess)
+        return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
+    prm.tw = tw; prm.tw2 = tw2;
+    cudaError_t e = launch_fft_pass(prec, kind, n, prm, table, 1.0, (cudaStream_t)stream);
     if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("launch failed: ") + cudaGetErrorString(e));
     return DFFT_SUCCESS;
 }
@@ -3046,84 +3027,42 @@ int dfft_fft1d_contig(int precision, int kind, int direction, size_t n, size_t l
                       size_t in_pitch, void* stream) {
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
     if (kind < 0 || kind > 2) return fail(DFFT_ERR_INVALID, "bad kind");
-    if (kind == 0 && bluestein_length(n)) {
-        FftParams prm{};
-        prm.A0 = 1; prm.A1 = int(lines); prm.B = 1;
-        prm.inverse = direction > 0 ? 1 : 0;
-        prm.in = single_view(const_cast<void*>(in), 0, (long long)in_pitch, 1);
-        prm.out = single_view(out, 0, (long long)out_pitch, 1);
-        return fft1d_bluestein(precision, PASS_C2C_CONTIG, n, prm, stream);
-    }
     const size_t len = kind == 0 ? n : n / 2;
     const int l2 = ilog2_exact(len);
-    if (ilog2_exact(n) < 1 || l2 < 1 || l2 > MAX_LOG2N) return fail(DFFT_ERR_UNSUPPORTED, "length must be a power of two");
+    if (kind == 0 ? !c2c_length(n) : (ilog2_exact(n) < 1 || l2 < 1 || l2 > MAX_LOG2N)) return fail(DFFT_ERR_UNSUPPORTED, "length must be a power of two");
     FftParams prm{};
     prm.A0 = 1; prm.A1 = int(lines); prm.B = 1;
     prm.inverse = (kind == 0 && direction > 0) ? 1 : 0;
-    void *tw = nullptr, *tw2 = nullptr;
-    int rc = cached_table(false, precision, l2, &tw);
-    if (rc) return rc;
-    if (kind != 0) { rc = cached_table(true, precision, l2, &tw2); if (rc) return rc; }
-    prm.tw = tw; prm.tw2 = tw2;
     // pitches are in elements of the respective array (reals for real arrays); views are in complex units
     long long ip = (long long)in_pitch, op = (long long)out_pitch;
     if (kind == 1) { if (in_pitch & 1) return fail(DFFT_ERR_INVALID, "real pitch must be even"); ip /= 2; }
     if (kind == 2) { if (out_pitch & 1) return fail(DFFT_ERR_INVALID, "real pitch must be even"); op /= 2; }
     prm.in = single_view(const_cast<void*>(in), 0, ip, 1);
     prm.out = single_view(out, 0, op, 1);
-    PassKind pk = kind == 0 ? PASS_C2C_CONTIG : (kind == 1 ? PASS_R2C : PASS_C2R);
-    cudaError_t e = precision == DFFT_F64 ? launch_pass_f64(l2, pk, prm, 1.0, (cudaStream_t)stream) : launch_pass_f32(l2, pk, prm, 1.0, (cudaStream_t)stream);
-    if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("launch failed: ") + cudaGetErrorString(e));
-    return DFFT_SUCCESS;
+    return fft1d_pass(precision, kind == 0 ? PASS_C2C_CONTIG : (kind == 1 ? PASS_R2C : PASS_C2R), len, prm, stream);
 }
 
 int dfft_fft1d_strided(int precision, int direction, size_t a, size_t n, size_t b, void* out, const void* in, void* stream) {
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
-    const int l2 = ilog2_exact(n);
     if (!c2c_length(n)) return fail(DFFT_ERR_UNSUPPORTED, "length must be a power of two in [2, 8192] or any length in [3, 4096]");
     FftParams prm{};
     prm.A0 = int(a); prm.A1 = 1; prm.B = int(b);
     prm.inverse = direction > 0 ? 1 : 0;
-    if (bluestein_length(n)) {
-        prm.in = single_view(const_cast<void*>(in), (long long)(n * b), 0, (long long)b);
-        prm.out = single_view(out, (long long)(n * b), 0, (long long)b);
-        return fft1d_bluestein(precision, PASS_C2C_TILED, n, prm, stream);
-    }
-    void* tw = nullptr;
-    int rc = cached_table(false, precision, l2, &tw);
-    if (rc) return rc;
-    prm.tw = tw;
     prm.in = single_view(const_cast<void*>(in), (long long)(n * b), 0, (long long)b);
     prm.out = single_view(out, (long long)(n * b), 0, (long long)b);
-    cudaError_t e = precision == DFFT_F64 ? launch_pass_f64(l2, PASS_C2C_TILED, prm, 1.0, (cudaStream_t)stream)
-                                          : launch_pass_f32(l2, PASS_C2C_TILED, prm, 1.0, (cudaStream_t)stream);
-    if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("launch failed: ") + cudaGetErrorString(e));
-    return DFFT_SUCCESS;
+    return fft1d_pass(precision, PASS_C2C_TILED, n, prm, stream);
 }
 
 int dfft_fft1d_general(int precision, int direction, size_t n, size_t a0, size_t a1, size_t b, void* out, const long long out_strides[3],
                        const void* in, const long long in_strides[3], void* stream) {
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
-    const int l2 = ilog2_exact(n);
     if (!c2c_length(n)) return fail(DFFT_ERR_UNSUPPORTED, "length must be a power of two in [2, 8192] or any length in [3, 4096]");
     FftParams prm{};
     prm.A0 = int(a0); prm.A1 = int(a1); prm.B = int(b);
     prm.inverse = direction > 0 ? 1 : 0;
-    if (bluestein_length(n)) {
-        prm.in = single_view(const_cast<void*>(in), in_strides[0], in_strides[1], in_strides[2]);
-        prm.out = single_view(out, out_strides[0], out_strides[1], out_strides[2]);
-        return fft1d_bluestein(precision, PASS_C2C_TILED, n, prm, stream);
-    }
-    void* tw = nullptr;
-    int rc = cached_table(false, precision, l2, &tw);
-    if (rc) return rc;
-    prm.tw = tw;
     prm.in = single_view(const_cast<void*>(in), in_strides[0], in_strides[1], in_strides[2]);
     prm.out = single_view(out, out_strides[0], out_strides[1], out_strides[2]);
-    cudaError_t e = precision == DFFT_F64 ? launch_pass_f64(l2, PASS_C2C_TILED, prm, 1.0, (cudaStream_t)stream)
-                                          : launch_pass_f32(l2, PASS_C2C_TILED, prm, 1.0, (cudaStream_t)stream);
-    if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("launch failed: ") + cudaGetErrorString(e));
-    return DFFT_SUCCESS;
+    return fft1d_pass(precision, PASS_C2C_TILED, n, prm, stream);
 }
 
 }  // extern "C"

@@ -69,6 +69,45 @@ static FftScaled with_scale(const FftParams& p, double scale) {
     return q;
 }
 
+// Launches one instantiation of a kernel template: KF / KI forward / inverse, KFS / KIS their scaled twins, picked by
+// p.inverse and scale != 1; `rest` follows the parameters.  Kernels without an inverse flag (R2C, C2R) pass their kernel as
+// both KF and KI, kernels without scaled twins nullptr (the Bluestein kernel scales by a runtime value of its parameters).
+// The shared-memory attribute of the unscaled pair is set on its first launch, that of the twins on their first launch.
+template <auto KF, auto KI, auto KFS, auto KIS, typename P, typename... R>
+static cudaError_t launch_kernel(const P& p, double scale, unsigned grid, int threads, size_t smem, cudaStream_t stream, const R&... rest) {
+    static const cudaError_t once = set_smem(KF, smem) == cudaSuccess ? set_smem(KI, smem) : cudaErrorInvalidValue;
+    if (once != cudaSuccess) return once;
+    if constexpr (!std::is_null_pointer_v<decltype(KIS)>) {
+        if (scale != 1.0) {
+            static const cudaError_t onces = set_smem(KFS, smem) == cudaSuccess ? set_smem(KIS, smem) : cudaErrorInvalidValue;
+            if (onces != cudaSuccess) return onces;
+            const FftScaled q = with_scale(p, scale);
+            if (p.inverse) KIS<<<grid, threads, smem, stream>>>(q, rest...);
+            else KFS<<<grid, threads, smem, stream>>>(q, rest...);
+            return cudaGetLastError();
+        }
+    }
+    if (p.inverse) KI<<<grid, threads, smem, stream>>>(p, rest...);
+    else KF<<<grid, threads, smem, stream>>>(p, rest...);
+    return cudaGetLastError();
+}
+
+// CTAs of a persistent kernel that fit on the device at once (callers keep the value in a static per instantiation)
+template <typename K>
+static int resident_ctas(K kernel, int threads, size_t smem) {
+    int dev = 0, sms = 0, per = 0;
+    set_smem(kernel, smem);  // the occupancy counts with the kernel's shared-memory limit
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kernel, threads, smem) != cudaSuccess || per < 1) per = 1;
+    return sms * per;
+}
+
+// the tile-order blocking log2 G where the batch extents allow it (G <= 16 divides A0 and A1), plain order otherwise
+static int tile_swz_for(int swz, int A0, int A1) {
+    return swz > 0 && swz <= 4 && A0 % (1 << swz) == 0 && A1 % (1 << swz) == 0 ? swz : 0;
+}
+
 static int wide_tiles() {
     const char* e = getenv("DFFT_WIDE_TILES");
     return e ? atoi(e) : 0;
@@ -77,23 +116,12 @@ static int wide_tiles() {
 template <typename T, int LOG2N, int TB>
 static cudaError_t launch_tiled(const FftParams& p_in, double scale, cudaStream_t stream, long long lines) {
     FftParams p = p_in;
-    {
-        const int e = env_int("DFFT_TILE_SWZ", -1);  // experiment override of the tile-order blocking
-        if (e >= 0) p.tile_swz = e;
-        if (p.tile_swz > 0) {
-            const int G = 1 << p.tile_swz;
-            if (p.tile_swz > 4 || p.A0 % G || p.A1 % G) p.tile_swz = 0;
-        } else p.tile_swz = 0;
-    }
+    const int swz = env_int("DFFT_TILE_SWZ", -1);  // experiment override of the tile-order blocking
+    p.tile_swz = tile_swz_for(swz >= 0 ? swz : p.tile_swz, p.A0, p.A1);
     using S = Shape<T, LOG2N>;
     constexpr int LOG2E = S::LOG2E;
     using C = CtaFft<T, LOG2N, LOG2E, TB, true>;
-    auto kf = fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, false, false>;
-    auto ki = fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, true, false>;
-    static cudaError_t once = set_smem(kf, C::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ki, C::SMEM_BYTES);
-    if (once != cudaSuccess) return once;
     if (p.B <= 0) return cudaSuccess;
-    const bool scaled = scale != 1.0;
     const long long grid = lines * ((p.B + TB - 1) / TB);
     if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
     if constexpr (C::NST >= 2 && LOG2N >= 7) {
@@ -109,82 +137,37 @@ static cudaError_t launch_tiled(const FftParams& p_in, double scale, cudaStream_
         const bool bulk_ok = p.bulk_out && p.out.sN == TB && p.B == TB;
         alignas(64) CUtensorMap tm;
         if (want && p.in.nseg == 1 && (!p.bulk_out || bulk_ok) && make_view_map<T>(p.in, p.A0, p.A1, C::N, p.B, TB, &tm)) {
-            auto tf = fft_c2c_tma_kernel<T, LOG2N, LOG2E, TB, false, false>;
-            auto ti = fft_c2c_tma_kernel<T, LOG2N, LOG2E, TB, true, false>;
-            static cudaError_t oncet = set_smem(tf, C::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ti, C::SMEM_BYTES);
-            if (oncet != cudaSuccess) return oncet;
-            static int resident = [&] {
-                int dev = 0, sms = 0, per = 0;
-                cudaGetDevice(&dev);
-                cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-                if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, tf, C::THREADS, C::SMEM_BYTES) != cudaSuccess || per < 1) per = 1;
-                return sms * per;
-            }();
+            constexpr auto tf = fft_c2c_tma_kernel<T, LOG2N, LOG2E, TB, false, false>;
+            static const int resident = resident_ctas(tf, C::THREADS, C::SMEM_BYTES);
             long long g = grid < resident ? grid : resident;
             if (p.max_ctas > 0 && g > p.max_ctas) g = p.max_ctas;
             FftParams q = p;
             q.bulk_out = bulk_ok ? 1 : 0;
-            if (scaled) {
-                auto tfs = fft_c2c_tma_kernel<T, LOG2N, LOG2E, TB, false, true>;
-                auto tis = fft_c2c_tma_kernel<T, LOG2N, LOG2E, TB, true, true>;
-                static cudaError_t onces = set_smem(tfs, C::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(tis, C::SMEM_BYTES);
-                if (onces != cudaSuccess) return onces;
-                const FftScaled qs = with_scale(q, scale);
-                if (p.inverse) tis<<<unsigned(g), C::THREADS, C::SMEM_BYTES, stream>>>(qs, tm);
-                else tfs<<<unsigned(g), C::THREADS, C::SMEM_BYTES, stream>>>(qs, tm);
-                return cudaGetLastError();
-            }
-            if (p.inverse) ti<<<unsigned(g), C::THREADS, C::SMEM_BYTES, stream>>>(q, tm);
-            else tf<<<unsigned(g), C::THREADS, C::SMEM_BYTES, stream>>>(q, tm);
-            return cudaGetLastError();
+            return launch_kernel<tf, fft_c2c_tma_kernel<T, LOG2N, LOG2E, TB, true, false>, fft_c2c_tma_kernel<T, LOG2N, LOG2E, TB, false, true>,
+                                 fft_c2c_tma_kernel<T, LOG2N, LOG2E, TB, true, true>>(q, scale, unsigned(g), C::THREADS, C::SMEM_BYTES, stream, tm);
         }
     }
     const unsigned g = unsigned((p.max_ctas > 0 && grid > p.max_ctas) ? p.max_ctas : grid);
-    if (scaled) {
-        auto kfs = fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, false, true>;
-        auto kis = fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, true, true>;
-        static cudaError_t onces = set_smem(kfs, C::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(kis, C::SMEM_BYTES);
-        if (onces != cudaSuccess) return onces;
-        if (p.inverse) kis<<<g, C::THREADS, C::SMEM_BYTES, stream>>>(with_scale(p, scale));
-        else kfs<<<g, C::THREADS, C::SMEM_BYTES, stream>>>(with_scale(p, scale));
-        return cudaGetLastError();
-    }
-    if (p.inverse) ki<<<g, C::THREADS, C::SMEM_BYTES, stream>>>(p);
-    else kf<<<g, C::THREADS, C::SMEM_BYTES, stream>>>(p);
-    return cudaGetLastError();
+    return launch_kernel<fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, false, false>, fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, true, false>,
+                         fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, false, true>, fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, true, true>>(
+        p, scale, g, C::THREADS, C::SMEM_BYTES, stream);
 }
 
 template <typename T, int LOG2N>
 cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStream_t stream) {
     using S = Shape<T, LOG2N>;
     constexpr int LOG2E = S::LOG2E;
+    using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
     const long long lines = (long long)p.A0 * p.A1;
     if (lines <= 0) return cudaSuccess;
-    cudaError_t err = cudaSuccess;
-    const bool scaled = scale != 1.0;
+    const long long grid = (lines + S::TBC - 1) / S::TBC;  // CONTIG, R2C and C2R
     switch (kind) {
-        case PASS_C2C_CONTIG: {
-            using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
-            auto kf = fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, false, false>;
-            auto ki = fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, true, false>;
-            static cudaError_t once = set_smem(kf, C::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ki, C::SMEM_BYTES);
-            if (once != cudaSuccess) return once;
+        case PASS_C2C_CONTIG:
             if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
-            const long long grid = (lines + S::TBC - 1) / S::TBC;
             if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            if (scaled) {
-                auto kfs = fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, false, true>;
-                auto kis = fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, true, true>;
-                static cudaError_t onces = set_smem(kfs, C::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(kis, C::SMEM_BYTES);
-                if (onces != cudaSuccess) return onces;
-                if (p.inverse) kis<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(with_scale(p, scale));
-                else kfs<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(with_scale(p, scale));
-                break;
-            }
-            if (p.inverse) ki<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(p);
-            else kf<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(p);
-            break;
-        }
+            return launch_kernel<fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, false, false>, fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, true, false>,
+                                 fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, false, true>, fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, true, true>>(
+                p, scale, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
         case PASS_C2C_TILED: {
             // Wide tiles (128-byte rows, one CTA per SM) are chosen when the rows of a tile sit in different 2 MB pages
             // (x passes with a row pitch >= 1 MiB), narrow ones otherwise (y passes); a choice still to be confirmed on
@@ -204,45 +187,21 @@ cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStr
             return launch_tiled<T, LOG2N, S::TBT>(p, scale, stream, lines);
         }
         case PASS_R2C: {
-            using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
-            auto k = fft_r2c_kernel<T, LOG2N, LOG2E, S::TBC, false>;
-            static cudaError_t once = set_smem(k, C::SMEM_BYTES);
-            if (once != cudaSuccess) return once;
             if (p.in.nseg != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
-            const long long grid = (lines + S::TBC - 1) / S::TBC;
             if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            if (scaled) {
-                auto ks = fft_r2c_kernel<T, LOG2N, LOG2E, S::TBC, true>;
-                static cudaError_t onces = set_smem(ks, C::SMEM_BYTES);
-                if (onces != cudaSuccess) return onces;
-                ks<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(with_scale(p, scale));
-                break;
-            }
-            k<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(p);
-            break;
+            constexpr auto k = fft_r2c_kernel<T, LOG2N, LOG2E, S::TBC, false>;
+            constexpr auto ks = fft_r2c_kernel<T, LOG2N, LOG2E, S::TBC, true>;
+            return launch_kernel<k, k, ks, ks>(p, scale, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
         }
         case PASS_C2R: {
-            using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
-            auto k = fft_c2r_kernel<T, LOG2N, LOG2E, S::TBC, false>;
-            static cudaError_t once = set_smem(k, C::SMEM_BYTES);
-            if (once != cudaSuccess) return once;
             if (p.out.nseg != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
-            const long long grid = (lines + S::TBC - 1) / S::TBC;
             if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            if (scaled) {
-                auto ks = fft_c2r_kernel<T, LOG2N, LOG2E, S::TBC, true>;
-                static cudaError_t onces = set_smem(ks, C::SMEM_BYTES);
-                if (onces != cudaSuccess) return onces;
-                ks<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(with_scale(p, scale));
-                break;
-            }
-            k<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(p);
-            break;
+            constexpr auto k = fft_c2r_kernel<T, LOG2N, LOG2E, S::TBC, false>;
+            constexpr auto ks = fft_c2r_kernel<T, LOG2N, LOG2E, S::TBC, true>;
+            return launch_kernel<k, k, ks, ks>(p, scale, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
         }
         default: return cudaErrorInvalidValue;
     }
-    err = cudaGetLastError();
-    return err;
 }
 
 template cudaError_t launch_pass<DFFT_T, DFFT_LOG2N>(PassKind, const FftParams&, double, cudaStream_t);
@@ -251,15 +210,11 @@ template cudaError_t launch_pass<DFFT_T, DFFT_LOG2N>(PassKind, const FftParams&,
 template <typename T, int LOG2M, int TB, bool TILED>
 static cudaError_t launch_bluestein_tiles(const FftBluestein& p, long long grid, cudaStream_t stream) {
     using C = CtaFft<T, LOG2M, Shape<T, LOG2M>::LOG2E, TB, TILED>;
-    auto kf = fft_bluestein_kernel<T, LOG2M, Shape<T, LOG2M>::LOG2E, TB, TILED, false>;
-    auto ki = fft_bluestein_kernel<T, LOG2M, Shape<T, LOG2M>::LOG2E, TB, TILED, true>;
-    static cudaError_t once = set_smem(kf, C::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ki, C::SMEM_BYTES);
-    if (once != cudaSuccess) return once;
     if (grid <= 0) return cudaSuccess;
     if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-    if (p.inverse) ki<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(p);
-    else kf<<<unsigned(grid), C::THREADS, C::SMEM_BYTES, stream>>>(p);
-    return cudaGetLastError();
+    return launch_kernel<fft_bluestein_kernel<T, LOG2M, Shape<T, LOG2M>::LOG2E, TB, TILED, false>,
+                         fft_bluestein_kernel<T, LOG2M, Shape<T, LOG2M>::LOG2E, TB, TILED, true>, nullptr, nullptr>(
+        p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
 }
 
 template <typename T, int LOG2M>
@@ -274,11 +229,7 @@ cudaError_t launch_bluestein(PassKind kind, const FftBluestein& p_in, cudaStream
         return launch_bluestein_tiles<T, LOG2M, S::TBC, false>(p, (lines + S::TBC - 1) / S::TBC, stream);
     }
     if (kind != PASS_C2C_TILED) return cudaErrorInvalidValue;
-    // the tile-order blocking of launch_tiled, where the batch extents allow it
-    if (p.tile_swz > 0) {
-        const int G = 1 << p.tile_swz;
-        if (p.tile_swz > 4 || p.A0 % G || p.A1 % G) p.tile_swz = 0;
-    } else p.tile_swz = 0;
+    p.tile_swz = tile_swz_for(p.tile_swz, p.A0, p.A1);  // the tile-order blocking of launch_tiled
     if (p.B <= 0) return cudaSuccess;
     return launch_bluestein_tiles<T, LOG2M, S::TBT, true>(p, lines * ((p.B + S::TBT - 1) / S::TBT), stream);
 }
@@ -310,32 +261,16 @@ cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFu
     const View& mid = inv ? pz.in : py.in;
     f.discard = inv ? (Z::Z_DISCARD && aligned128(mid.seg[0].base, mid.seg[0].sA0, mid.seg[0].sA1, 1 << LOG2N))
                     : (Z::Y_DISCARD && aligned128(mid.seg[0].base, mid.seg[0].sA0, mid.seg[0].sA1, mid.sN));
-    auto kf = fft_zy_fused_kernel<T, LOG2N, false, false>;
-    auto ki = fft_zy_fused_kernel<T, LOG2N, true, false>;
-    static cudaError_t once = set_smem(kf, Z::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ki, Z::SMEM_BYTES);
-    if (once != cudaSuccess) return once;
     // persistent: as many CTAs as fit at once (tickets hand out the work; fewer resident CTAs are fine as well).  The
     // grid depends on the work list only, so every launch of a step draws the same number of tickets (zy_launch_of).
-    static const int resident = [&] {
-        int dev = 0, sms = 0, per = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kf, Z::THREADS, Z::SMEM_BYTES) != cudaSuccess || per < 1) per = 1;
-        return sms * per;
-    }();
+    constexpr auto kf = fft_zy_fused_kernel<T, LOG2N, false, false>;
+    static const int resident = resident_ctas(kf, Z::THREADS, Z::SMEM_BYTES);
     const long long total = f.order.total();
     if (total <= 0) return cudaSuccess;
     const unsigned grid = unsigned(total < resident ? total : resident);
-    if (scale != 1.0) {
-        auto kis = fft_zy_fused_kernel<T, LOG2N, true, true>;
-        static cudaError_t onces = set_smem(kis, Z::SMEM_BYTES);
-        if (onces != cudaSuccess) return onces;
-        kis<<<grid, Z::THREADS, Z::SMEM_BYTES, stream>>>(with_scale(pz, scale), py, f);
-        return cudaGetLastError();
-    }
-    if (inv) ki<<<grid, Z::THREADS, Z::SMEM_BYTES, stream>>>(pz, py, f);
-    else kf<<<grid, Z::THREADS, Z::SMEM_BYTES, stream>>>(pz, py, f);
-    return cudaGetLastError();
+    // only the inverse stage has a scaled twin (a scaled forward stage is refused above)
+    constexpr auto kis = fft_zy_fused_kernel<T, LOG2N, true, true>;
+    return launch_kernel<kf, fft_zy_fused_kernel<T, LOG2N, true, false>, kis, kis>(pz, scale, grid, Z::THREADS, Z::SMEM_BYTES, stream, py, f);
 }
 
 template cudaError_t launch_zy_fused<DFFT_T, DFFT_LOG2N>(const FftParams&, const FftParams&, const ZyFused&, double, cudaStream_t);
@@ -367,32 +302,13 @@ cudaError_t launch_batch_small(const void* in, void* out, long long batch, int i
     }
     px.in.seg[0].base = inverse ? const_cast<void*>(in) : out;
     px.out.seg[0].base = out;
-    auto kf = fft_batch_small_kernel<T, LOG2N, false, false>;
-    auto ki = fft_batch_small_kernel<T, LOG2N, true, false>;
-    static cudaError_t once = set_smem(kf, BS::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(ki, BS::SMEM_BYTES);
-    if (once != cudaSuccess) return once;
     // persistent, as many CTAs as fit at once; the grid depends on the batch only (zy_launch_of)
-    static const int resident = [&] {
-        int dev = 0, sms = 0, per = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kf, BS::THREADS, BS::SMEM_BYTES) != cudaSuccess || per < 1) per = 1;
-        return sms * per;
-    }();
+    constexpr auto kf = fft_batch_small_kernel<T, LOG2N, false, false>;
+    static const int resident = resident_ctas(kf, BS::THREADS, BS::SMEM_BYTES);
     const long long total = f.order.total();
     const unsigned grid = unsigned(total < resident ? total : resident);
-    if (scale != 1.0) {
-        auto kfs = fft_batch_small_kernel<T, LOG2N, false, true>;
-        auto kis = fft_batch_small_kernel<T, LOG2N, true, true>;
-        static cudaError_t onces = set_smem(kfs, BS::SMEM_BYTES) != cudaSuccess ? cudaErrorInvalidValue : set_smem(kis, BS::SMEM_BYTES);
-        if (onces != cudaSuccess) return onces;
-        if (inverse) kis<<<grid, BS::THREADS, BS::SMEM_BYTES, stream>>>(with_scale(px, scale), f);
-        else kfs<<<grid, BS::THREADS, BS::SMEM_BYTES, stream>>>(with_scale(px, scale), f);
-        return cudaGetLastError();
-    }
-    if (inverse) ki<<<grid, BS::THREADS, BS::SMEM_BYTES, stream>>>(px, f);
-    else kf<<<grid, BS::THREADS, BS::SMEM_BYTES, stream>>>(px, f);
-    return cudaGetLastError();
+    return launch_kernel<kf, fft_batch_small_kernel<T, LOG2N, true, false>, fft_batch_small_kernel<T, LOG2N, false, true>,
+                         fft_batch_small_kernel<T, LOG2N, true, true>>(px, scale, grid, BS::THREADS, BS::SMEM_BYTES, stream, f);
 }
 
 template cudaError_t launch_batch_small<DFFT_T, DFFT_LOG2N>(const void*, void*, long long, int, const BatchSmall&, double, cudaStream_t);

@@ -484,14 +484,81 @@ fft_c2c_kernel(const __grid_constant__ KParams<SCALED> p) {
 //     stored: the line is dead and is dropped without a write-back to HBM.  That needs every such line to
 //     be read by one CTA only — 128-byte y-tile rows (TB * sizeof(complex) a multiple of 128) and z lines of a multiple
 //     of 128 bytes, on 128-byte aligned views (ZyFused::discard, checked by the launcher).
-struct ZyFused {
-    unsigned long long* ctr;          // [0] ticket counter, [1 + g] finished phase-A items of group g; never reset
-    int* err;                         // the plan's device error flag
-    long long timeout_cycles;         // clock64 cycles a dependency wait may take (0 = no limit)
+//
+// The parameters of the two persistent two-phase kernels (this one and fft_batch_small_kernel) begin with TicketWork, the
+// state of their common ticket loop (ticket_loop).
+struct TicketWork {
+    unsigned long long* ctr;   // [0] ticket counter, [1 + g] finished phase-A items of group g; zeroed once, never reset
+    int* err;                  // the plan's device error flag
+    long long timeout_cycles;  // clock64 cycles a dependency wait may take (0 = no limit)
     ZyOrder order;
-    int discard;                      // phase B may discard the intermediate lines it has read
+};
+struct ZyFused : TicketWork {
+    int discard;  // phase B may discard the intermediate lines it has read
 };
 constexpr int ZY_ERR_TIMEOUT = 200;   // value of the error flag when a fused-stage dependency wait timed out
+
+// The ticket loop of a persistent two-phase kernel: draws tickets until the work list is done, waits before each phase-B
+// item until every phase-A item of its group has finished, and runs item(it, slot) for every work item `it` (all threads;
+// *slot holds its ticket).  Shared memory `bcast`: bcast[par] the current ticket; bcast[par ^ 1] the next one, drawn while
+// this item runs (the atomic's latency is hidden behind the tile's loads).  Values are re-read from shared memory where
+// needed instead of being kept in registers through the tiles.  bcast[2]: give up.  bcast[3], bcast[4]: this launch's
+// counter base and epoch, fixed by the CTA's first draw (zy_launch_of) — the kernel takes no per-exec value from the host,
+// so a graph can replay it.  A timed-out wait sets the error flag to timeout_err and ends the loop.
+template <typename Item>
+__device__ __forceinline__ void ticket_loop(const TicketWork& f, volatile long long* bcast, int timeout_err, const Item& item) {
+    const int tid = threadIdx.x;
+    const long long total = f.order.total();
+    int par = 0;
+    if (tid == 0) {
+        const unsigned long long raw = atomicAdd(f.ctr, 1ull);
+        const ZyLaunch l = zy_launch_of(raw, f.order.draws(gridDim.x));
+        bcast[3] = (long long)l.base;
+        bcast[4] = (long long)l.epoch;
+        bcast[0] = (long long)(raw - l.base);
+    }
+#pragma unroll 1
+    for (;; par ^= 1) {
+        __syncthreads();
+        const long long ticket = bcast[par];
+        if (ticket >= total) break;
+        if (tid == 0) bcast[par ^ 1] = (long long)(atomicAdd(f.ctr, 1ull) - (unsigned long long)bcast[3]);
+        const ZyItem it = f.order.decode(ticket);
+        if (it.phase == 1) {
+            // Wait until every phase-A item of this group has finished.  This cannot deadlock: tickets are handed out in
+            // increasing order and only to CTAs that are already running, and every item a ticket depends on has a lower
+            // ticket (zy_order.hpp).  So the lowest unfinished ticket is held by a resident CTA whose earlier item is
+            // finished, and all its dependencies are finished: it completes, and by induction so does every ticket —
+            // with any number of resident CTAs, also when other work on the GPU leaves this launch fewer CTAs than it
+            // asked for.  The wait is still bounded (the plan's rendezvous timeout): a logic error surfaces as an error
+            // code, not a hung GPU.
+            if (tid == 0) {
+                const unsigned long long target = (unsigned long long)bcast[4] * (unsigned long long)f.order.a_items(it.group);
+                const unsigned long long* c = f.ctr + 1 + it.group;
+                unsigned long long v;
+                asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(c) : "memory");
+                long long bail = 0;
+                if (v < target) {
+                    const long long t0 = clock64();
+                    while (true) {
+                        __nanosleep(32);
+                        asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(c) : "memory");
+                        if (v >= target) break;
+                        if (f.timeout_cycles > 0 && clock64() - t0 > f.timeout_cycles) {
+                            atomicExch(f.err, timeout_err);
+                            bail = 1;
+                            break;
+                        }
+                    }
+                }
+                bcast[2] = bail;
+            }
+            __syncthreads();
+            if (bcast[2]) break;
+        }
+        item(it, bcast + par);
+    }
+}
 
 template <typename T, int LOG2N>
 struct ZyShape {
@@ -562,60 +629,7 @@ fft_zy_fused_kernel(const __grid_constant__ KParams<SCALED> pz, const __grid_con
     unsigned long long* tab_in = reinterpret_cast<unsigned long long*>(smem_raw + Z::TILE_BYTES);
     unsigned long long* tab_out = tab_in + (Z::TABLE_BYTES - 16) / 16;
     volatile long long* bcast = reinterpret_cast<volatile long long*>(smem_raw + Z::TILE_BYTES + Z::TABLE_BYTES);
-    const int tid = threadIdx.x;
-    const long long total = f.order.total();
-
-    // bcast[par]: the current ticket; bcast[par ^ 1]: the next one, drawn while this item runs (the atomic's latency is
-    // hidden behind the tile's loads).  Values are re-read from shared memory where needed instead of being kept in
-    // registers through the tiles.  bcast[2]: give up.  bcast[3], bcast[4]: this launch's counter base and epoch, fixed
-    // by the CTA's first draw (zy_launch_of) — the kernel takes no per-exec value from the host, so a graph can replay it.
-    int par = 0;
-    if (tid == 0) {
-        const unsigned long long raw = atomicAdd(f.ctr, 1ull);
-        const ZyLaunch l = zy_launch_of(raw, f.order.draws(gridDim.x));
-        bcast[3] = (long long)l.base;
-        bcast[4] = (long long)l.epoch;
-        bcast[0] = (long long)(raw - l.base);
-    }
-#pragma unroll 1
-    for (;; par ^= 1) {
-        __syncthreads();
-        const long long ticket = bcast[par];
-        if (ticket >= total) break;
-        if (tid == 0) bcast[par ^ 1] = (long long)(atomicAdd(f.ctr, 1ull) - (unsigned long long)bcast[3]);
-        const ZyItem it = f.order.decode(ticket);
-        if (it.phase == 1) {
-            // Wait until every phase-A item of this group has finished.  This cannot deadlock: tickets are handed out in
-            // increasing order and only to CTAs that are already running, and every item a ticket depends on has a lower
-            // ticket (zy_order.hpp).  So the lowest unfinished ticket is held by a resident CTA whose earlier item is
-            // finished, and all its dependencies are finished: it completes, and by induction so does every ticket —
-            // with any number of resident CTAs, also when other work on the GPU leaves this launch fewer CTAs than it
-            // asked for.  The wait is still bounded (the plan's rendezvous timeout): a logic error surfaces as an error
-            // code, not a hung GPU.
-            if (tid == 0) {
-                const unsigned long long target = (unsigned long long)bcast[4] * (unsigned long long)f.order.a_items(it.group);
-                const unsigned long long* c = f.ctr + 1 + it.group;
-                unsigned long long v;
-                asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(c) : "memory");
-                long long bail = 0;
-                if (v < target) {
-                    const long long t0 = clock64();
-                    while (true) {
-                        __nanosleep(32);
-                        asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(c) : "memory");
-                        if (v >= target) break;
-                        if (f.timeout_cycles > 0 && clock64() - t0 > f.timeout_cycles) {
-                            atomicExch(f.err, ZY_ERR_TIMEOUT);
-                            bail = 1;
-                            break;
-                        }
-                    }
-                }
-                bcast[2] = bail;
-            }
-            __syncthreads();
-            if (bcast[2]) break;
-        }
+    ticket_loop(f, bcast, ZY_ERR_TIMEOUT, [&](const ZyItem& it, const volatile long long* slot) {
         const bool z_item = (it.phase == 0) == !INV;  // forward: phase A = z; inverse: phase A = y
         const MemHint<T> mem_a{l2_evict_first(), l2_evict_last()};   // streaming input -> intermediate
         const MemHint<T> mem_b{l2_evict_normal(), l2_evict_first()};  // intermediate -> streaming output
@@ -629,8 +643,8 @@ fft_zy_fused_kernel(const __grid_constant__ KParams<SCALED> pz, const __grid_con
         }
         // the tile is stored and shared memory is free again before the item counts
         __syncthreads();
-        zy_item_done<T, LOG2N, INV>(pz, py, f, bcast[par]);
-    }
+        zy_item_done<T, LOG2N, INV>(pz, py, f, *slot);
+    });
 }
 
 // ---- batches of small cubic fields: one persistent launch per exec ------------------------------------------
@@ -641,15 +655,13 @@ fft_zy_fused_kernel(const __grid_constant__ KParams<SCALED> pz, const __grid_con
 // Forward: phase A = plane items (caller's in -> caller's out), phase B = slice items (out -> out, in place).  Inverse, in
 // the order of the unbatched plan (x, then y, then z): phase A = slice items (in -> out), phase B = plane items (out -> out,
 // in place).  A phase-B item of field f needs every phase-A item of f; the work list is ZyOrder with one group per field,
-// so every dependency has a lower ticket (zy_order.hpp) and the wait below is the one of fft_zy_fused_kernel.  Each line
+// so every dependency has a lower ticket (zy_order.hpp) and the kernel runs the ticket loop of fft_zy_fused_kernel.  Each line
 // runs FftCore<T, LOG2N, Shape::LOG2E> with the plan's twiddle table, as in the standalone passes: bit-identical results.
 // L2 policy as in the fused z + y stage: phase A loads with evict_first and stores the intermediate with evict_last,
 // phase B stores with evict_first; a field is read from HBM once and written once.
-struct BatchSmall {
-    unsigned long long* ctr;   // [0] ticket counter, [1 + f] finished phase-A items of field f; zeroed once, never reset
-    int* err;                  // the plan's device error flag
-    long long timeout_cycles;  // clock64 cycles a dependency wait may take (0 = no limit)
-    ZyOrder order;             // nx = fields, gpp = 1, na / nb items per field (filled in by the launcher), look-ahead in fields
+// TicketWork: one group per field (ctr[1 + f] counts field f), order.nx = fields, gpp = 1, na / nb items per field (filled in
+// by the launcher), look-ahead in fields.
+struct BatchSmall : TicketWork {
     const void* plane_in;      // plane items read here and write plane_out
     void* plane_out;
     const void* tw;            // exp(-2 pi i m / N), the plan's table
@@ -734,55 +746,10 @@ fft_batch_small_kernel(const __grid_constant__ KParams<SCALED> px, const __grid_
     cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
     unsigned long long* no_tab = reinterpret_cast<unsigned long long*>(smem_raw);  // single-segment views need no tables
     volatile long long* bcast = reinterpret_cast<volatile long long*>(smem_raw + BS::TILE_BYTES);
-    const int tid = threadIdx.x;
-    const long long total = f.order.total();
     const cx<T>* plane_in = reinterpret_cast<const cx<T>*>(f.plane_in);
     cx<T>* plane_out = reinterpret_cast<cx<T>*>(f.plane_out);
-
-    // ticket broadcast as in fft_zy_fused_kernel: bcast[par] current ticket, bcast[par ^ 1] the next one, bcast[2] give
-    // up, bcast[3] / bcast[4] this launch's counter base and epoch (zy_launch_of)
-    int par = 0;
-    if (tid == 0) {
-        const unsigned long long raw = atomicAdd(f.ctr, 1ull);
-        const ZyLaunch l = zy_launch_of(raw, f.order.draws(gridDim.x));
-        bcast[3] = (long long)l.base;
-        bcast[4] = (long long)l.epoch;
-        bcast[0] = (long long)(raw - l.base);
-    }
-#pragma unroll 1
-    for (;; par ^= 1) {
-        __syncthreads();
-        const long long ticket = bcast[par];
-        if (ticket >= total) break;
-        if (tid == 0) bcast[par ^ 1] = (long long)(atomicAdd(f.ctr, 1ull) - (unsigned long long)bcast[3]);
-        const ZyItem it = f.order.decode(ticket);
-        if (it.phase == 1) {
-            // Wait until every phase-A item of this field has finished; deadlock-free for the reason given at the wait in
-            // fft_zy_fused_kernel (every dependency has a lower ticket), bounded so that a logic error becomes an error code.
-            if (tid == 0) {
-                const unsigned long long target = (unsigned long long)bcast[4] * (unsigned long long)f.order.a_items(it.group);
-                const unsigned long long* c = f.ctr + 1 + it.group;
-                unsigned long long v;
-                asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(c) : "memory");
-                long long bail = 0;
-                if (v < target) {
-                    const long long t0 = clock64();
-                    while (true) {
-                        __nanosleep(32);
-                        asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(c) : "memory");
-                        if (v >= target) break;
-                        if (f.timeout_cycles > 0 && clock64() - t0 > f.timeout_cycles) {
-                            atomicExch(f.err, BATCH_ERR_TIMEOUT);
-                            bail = 1;
-                            break;
-                        }
-                    }
-                }
-                bcast[2] = bail;
-            }
-            __syncthreads();
-            if (bcast[2]) break;
-        }
+    // the ticket loop of fft_zy_fused_kernel, with one group per field
+    ticket_loop(f, bcast, BATCH_ERR_TIMEOUT, [&](const ZyItem& it, const volatile long long*) {
         const bool slice = (it.phase == 0) == INV;
         const MemHint<T> mem_a{l2_evict_first(), l2_evict_last()};   // streaming input -> intermediate
         const MemHint<T> mem_b{l2_evict_normal(), l2_evict_first()};  // intermediate -> streaming output
@@ -799,8 +766,8 @@ fft_batch_small_kernel(const __grid_constant__ KParams<SCALED> px, const __grid_
         }
         // the item is stored and shared memory is free again before it counts
         __syncthreads();
-        if (it.phase == 0 && tid == 0) asm volatile("red.release.gpu.global.add.u64 [%0], 1;" ::"l"(f.ctr + 1 + it.group) : "memory");
-    }
+        if (it.phase == 0 && threadIdx.x == 0) asm volatile("red.release.gpu.global.add.u64 [%0], 1;" ::"l"(f.ctr + 1 + it.group) : "memory");
+    });
 }
 
 // ---- C2C TILED pass fed by TMA ----------------------------------------------------------------------------
@@ -1212,9 +1179,9 @@ fft_bluestein_kernel(const __grid_constant__ FftBluestein p) {
 template <typename T, int LOG2N>
 cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStream_t stream);
 
-// launch_pass for a runtime size; returns cudaErrorInvalidValue for unsupported lengths.
-cudaError_t launch_pass_f64(int log2n, PassKind kind, const FftParams& p, double scale, cudaStream_t stream);
-cudaError_t launch_pass_f32(int log2n, PassKind kind, const FftParams& p, double scale, cudaStream_t stream);
+// Each launcher also has a runtime form (fft_dispatch.cu) that takes the precision (DFFT_F64 / DFFT_F32) and the log2 length
+// first; it returns cudaErrorInvalidValue for a length that is not instantiated.
+cudaError_t launch_pass(int prec, int log2n, PassKind kind, const FftParams& p, double scale, cudaStream_t stream);
 
 // fused z + y stage (fft_zy_fused_kernel), instantiated for the lengths zy_fused_length accepts.  pz: the z pass, py: the y
 // pass, f: counters and plane groups (f.order.na / nb are filled in here).  Every launch of one step must use the same
@@ -1222,8 +1189,7 @@ cudaError_t launch_pass_f32(int log2n, PassKind kind, const FftParams& p, double
 // last phase's stores, inverse only (the forward stage stores an intermediate).
 template <typename T, int LOG2N>
 cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFused& f, double scale, cudaStream_t stream);
-cudaError_t launch_zy_fused_f64(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, double scale, cudaStream_t stream);
-cudaError_t launch_zy_fused_f32(int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, double scale, cudaStream_t stream);
+cudaError_t launch_zy_fused(int prec, int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, double scale, cudaStream_t stream);
 constexpr bool zy_fused_length(int log2n) { return log2n == 8 || log2n == 9; }
 
 // batched small cubic fields (fft_batch_small_kernel), instantiated for the lengths batch_small_length accepts.  in / out:
@@ -1232,15 +1198,14 @@ constexpr bool zy_fused_length(int log2n) { return log2n == 8 || log2n == 9; }
 // scale: of phase B's stores.
 template <typename T, int LOG2N>
 cudaError_t launch_batch_small(const void* in, void* out, long long batch, int inverse, const BatchSmall& f, double scale, cudaStream_t stream);
-cudaError_t launch_batch_small_f64(int log2n, const void* in, void* out, long long batch, int inverse, const BatchSmall& f, double scale, cudaStream_t stream);
-cudaError_t launch_batch_small_f32(int log2n, const void* in, void* out, long long batch, int inverse, const BatchSmall& f, double scale, cudaStream_t stream);
+cudaError_t launch_batch_small(int prec, int log2n, const void* in, void* out, long long batch, int inverse, const BatchSmall& f, double scale,
+                               cudaStream_t stream);
 
 // Bluestein pass (fft_bluestein_kernel) of p.n-point lines, M = 2^LOG2M >= 2 p.n - 1: kind PASS_C2C_CONTIG or PASS_C2C_TILED
 // (the view mapping of the power-of-two pass), one CTA per tile; p.scale scales the stores.  Instantiated for LOG2M 3..13.
 template <typename T, int LOG2M>
 cudaError_t launch_bluestein(PassKind kind, const FftBluestein& p, cudaStream_t stream);
-cudaError_t launch_bluestein_f64(int log2m, PassKind kind, const FftBluestein& p, cudaStream_t stream);
-cudaError_t launch_bluestein_f32(int log2m, PassKind kind, const FftBluestein& p, cudaStream_t stream);
+cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluestein& p, cudaStream_t stream);
 
 constexpr int MAX_LOG2N = 13;
 constexpr int BLUESTEIN_MAX_N = 4096;  // 2n - 1 <= 2^MAX_LOG2N

@@ -11,7 +11,7 @@
 // what B(g+L) will read.  The look-ahead is what keeps a B item from waiting: the items of A(g) are drawn L groups of
 // work before the first item of B(g), so with L * gpp * (na + nb) above the number of resident CTAs they have finished
 // by then.  Every B item of group g depends on all A items of group g, whose tickets are all lower than any ticket of
-// B(g) — the property the deadlock argument at the wait in fft_zy_fused_kernel rests on.
+// B(g) — the property the deadlock argument at the wait in ticket_loop (fft_kernels.cuh) rests on.
 //
 // Host-compiled as well (tests/zy_order_test.cpp checks the list).
 #pragma once
