@@ -283,6 +283,7 @@ struct Step {
     // fused z + y stage (KERNEL_ZY_FUSED): prm is the z pass, prm_y the y pass; zyf holds the counters, advanced by every
     // launch on the device
     FftParams prm_y{};
+    int y_in_user = 0, y_out_user = 0;  // in_user / out_user of prm_y (in-place plans: its view on the caller's buffer)
     ZyFused zyf{};
     // batched small cubic fields (KERNEL_BATCH_SMALL): one launch for every field; prm.in / prm.out are the caller's
     // buffers, bsf holds the counters
@@ -319,6 +320,9 @@ struct dfft_plan_s {
     int rank = 0, P = 1;
     size_t batch = 1;         // fields per exec, back to back in every caller buffer (dfft_plan_create_batched)
     double scale[2] = {1.0, 1.0};  // [fwd/inv] output scale (dfft_plan_set_scale), applied by the steps marked final_store
+    // dfft_plan_create_inplace: every exec has out == in, fields domain_bytes apart, real rows of R2C / C2R padded to Nzc
+    // complex units.  buf_slot: one rank — the schedules' first slot (D1) is the caller's buffer and is not allocated.
+    bool inplace = false, buf_slot = false;
     size_t domain_bytes = 0;  // this rank (getDomainSize)
     size_t slot_bytes = 0;    // uniform over ranks
     int nslots = 2;
@@ -447,6 +451,14 @@ static SegN mkseg(void* base, long long sA0, long long sA1, long long sN, size_t
 // Whether every axis is a power of two.  Plans with another length run the sequential schedule only: the overlapped
 // schedules build their passes for power-of-two lengths.
 static bool pow2_axes(const dfft_plan_s* p) { return ilog2_exact(p->g.nx) > 0 && ilog2_exact(p->g.ny) > 0 && ilog2_exact(p->g.nz) > 0; }
+
+// Row pitch, in complex units, of the z-contiguous side of the caller's buffers that holds Nz points per row: the input
+// of forward passes, the output of inverse ones.  Real rows of R2C / C2R plans are Nz reals (Nz/2 units) apart, or, in
+// place, Nzc units apart (the padded layout of FFTW and cuFFT: the last one or two reals of a row are never touched).
+static long long z_row_pitch(const dfft_plan_s* p) {
+    const Geometry& g = p->g;
+    return (long long)(g.transform == DFFT_C2C || p->inplace ? g.nzc : g.nz / 2);
+}
 
 // Whether the z and y passes run as one fused launch (fft_zy_fused_kernel): one-rank slab C2C plans of the full 3D
 // transform with Ny == Nz of an instantiated length (zy_fused_length) whose array is larger than the L2 — below that the
@@ -600,7 +612,12 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     if (dir1) D1 = nxt++;
     if (dir2) D2 = nxt++;
     if (!dir1 || !dir2) { SS = nxt++; SR = nxt++; }
-    auto slotp = [&](int s, int r) -> void* { return p->slot_ptr[s][r]; };
+    // in-place plans of one rank: D1 is the caller's buffer — its views hold byte offsets (from a null base), which
+    // relocate_buffer_views turns into views on the buffer; the other slots move down by one
+    auto slotp = [&](int s, int r) -> void* {
+        if (p->buf_slot) return s == D1 ? nullptr : p->slot_ptr[s - 1][r];
+        return p->slot_ptr[s][r];
+    };
 
     if (p->any_direct) rendezvous(0, 0, nullptr);  // everyone has left the previous exec: slots are free
 
@@ -647,8 +664,8 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         rc = new_pass(c2c ? PASS_C2C_CONTIG : PASS_R2C, c2c ? g.nz : g.nz / 2, zyx || g.decomp == DFFT_PENCIL ? "1D FFT Z-Direction" : nullptr, s1);
         if (rc) return rc;
         s1.prm.A0 = int(nx_i); s1.prm.A1 = int(ny_j);
-        {   // input: caller's buffer; real lines of nz reals = nz/2 complex
-            const long long pitch = c2c ? (long long)g.nz : (long long)(g.nz / 2);
+        {   // input: caller's buffer; real lines of nz reals = nz/2 complex (in place: padded rows)
+            const long long pitch = z_row_pitch(p);
             s1.prm.in = single_view(nullptr, pitch * (long long)ny_j, pitch, 1);
             s1.in_user = 1;
         }
@@ -846,7 +863,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     // Reverse order: x, transposition 2', y, transposition 1', z.  Partial d: only the last d of them.
     const PassKind zkind = c2c ? PASS_C2C_CONTIG : PASS_C2R;
     const size_t zlen = c2c ? g.nz : g.nz / 2;
-    const long long zpitch_out = c2c ? (long long)g.nz : (long long)(g.nz / 2);  // output line pitch in complex units
+    const long long zpitch_out = z_row_pitch(p);  // output line pitch in complex units
 
     if (d == 1) {
         Step s;
@@ -1189,7 +1206,7 @@ static int build_overlapped_slab(dfft_plan_s* p, int inverse, Schedule& sc) {
             rc = new_pass(c2c ? PASS_C2C_CONTIG : PASS_R2C, c2c ? g.nz : g.nz / 2, c2c ? "z pass" : "z pass (R2C)", s);
             if (rc) return rc;
             const size_t pl0 = groups.start[gi], npl = groups.size[gi];
-            const long long pitch = c2c ? (long long)g.nz : (long long)(g.nz / 2);
+            const long long pitch = z_row_pitch(p);
             s.prm.A0 = int(npl); s.prm.A1 = int(ny);
             s.prm.in = single_view((void*)(size_t)(pl0 * ny * pitch * es), pitch * (long long)ny, pitch, 1);
             s.in_user = 1;
@@ -1363,7 +1380,7 @@ static int build_overlapped_slab(dfft_plan_s* p, int inverse, Schedule& sc) {
         }
         Step s;
         const PassKind zkind = c2c ? PASS_C2C_CONTIG : PASS_C2R;
-        const long long zpitch = c2c ? (long long)g.nz : (long long)(g.nz / 2);
+        const long long zpitch = z_row_pitch(p);
         rc = new_pass(zkind, c2c ? g.nz : g.nz / 2, c2c ? "z pass" : "z pass (C2R)", s);
         if (rc) return rc;
         s.prm.A0 = int(nx_p); s.prm.A1 = int(ny);
@@ -1536,7 +1553,7 @@ static int build_overlapped_pencil_inverse(dfft_plan_s* p, Schedule& sc, size_t 
         }
     }
     const PassKind zkind = c2c ? PASS_C2C_CONTIG : PASS_C2R;
-    const long long zpitch = c2c ? (long long)g.nz : (long long)(g.nz / 2);  // output line pitch in complex units
+    const long long zpitch = z_row_pitch(p);  // output line pitch in complex units
     for (size_t gi = 0; gi < NG; ++gi) {
         const size_t pl0 = groups.start[gi], npl = groups.size[gi];
         Step r = rendezvous(1, 2);  // all row peers have delivered plane group gi
@@ -1654,7 +1671,7 @@ static int build_overlapped_pencil(dfft_plan_s* p, int inverse, Schedule& sc) {
         rc = new_pass(c2c ? PASS_C2C_CONTIG : PASS_R2C, c2c ? g.nz : g.nz / 2, c2c ? "z pass" : "z pass (R2C)", s);
         if (rc) return rc;
         const size_t pl0 = groups.start[gi], npl = groups.size[gi];
-        const long long pitch = c2c ? (long long)g.nz : (long long)(g.nz / 2);
+        const long long pitch = z_row_pitch(p);
         s.prm.A0 = int(npl); s.prm.A1 = int(ny_j);
         s.prm.in = single_view((void*)(size_t)(pl0 * ny_j * pitch * es), pitch * (long long)ny_j, pitch, 1);
         s.in_user = 1;
@@ -1989,13 +2006,21 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
             if (s.type == STEP_PASS) {
                 FftParams prm = s.prm;
                 const double scale = s.final_store ? p->scale[sc.inverse] : 1.0;
-                // views on the caller's buffers store a byte offset in seg[0].base (field f starts f field sizes further)
-                if (s.in_user == 1) prm.in.seg[0].base = (char*)const_cast<void*>(in) + f * sc.field_in + (size_t)s.prm.in.seg[0].base;
-                if (s.out_user == 2) prm.out.seg[0].base = (char*)out + f * sc.field_out + (size_t)s.prm.out.seg[0].base;
+                // views on the caller's buffers store a byte offset in seg[0].base (field f starts f field sizes further);
+                // in_user 2: a view that reads `out` (in-place plans)
+                auto user = [&](View& v, int which) {
+                    if (which == 1) v.seg[0].base = (char*)const_cast<void*>(in) + f * sc.field_in + (size_t)v.seg[0].base;
+                    if (which == 2) v.seg[0].base = (char*)out + f * sc.field_out + (size_t)v.seg[0].base;
+                };
+                user(prm.in, s.in_user);
+                user(prm.out, s.out_user);
+                FftParams prm_y = s.prm_y;
+                user(prm_y.in, s.y_in_user);
+                user(prm_y.out, s.y_out_user);
                 cudaError_t e = cudaErrorInvalidValue;
                 switch (s.kernel) {
                     case KERNEL_PASS: e = launch_fft_pass(p->prec, s.kind, s.n ? s.n : size_t(1) << s.log2n, prm, s.blu, scale, ss); break;
-                    case KERNEL_ZY_FUSED: e = launch_zy_fused(p->prec, s.log2n, prm, s.prm_y, s.zyf, scale, ss); break;
+                    case KERNEL_ZY_FUSED: e = launch_zy_fused(p->prec, s.log2n, prm, prm_y, s.zyf, scale, ss); break;
                     case KERNEL_BATCH_SMALL:
                         e = launch_batch_small(p->prec, s.log2n, prm.in.seg[0].base, prm.out.seg[0].base, (long long)p->batch, s.prm.inverse, s.bsf, scale, ss);
                         break;
@@ -2047,7 +2072,12 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
 // Bytes of one field in the caller's `in` and `out` of an exec (direction, d): the product of that buffer's layout, in
 // reals for the real side of R2C / C2R.  No schedule touches a caller buffer beyond it (tests/test_batch.py checks every
 // step's accesses), so fields sit back to back at this distance.
+// In-place plans: one buffer, so one distance, dfft_get_domain_size(), which covers every layout (Geometry::domain_elems).
 static void field_bytes(const dfft_plan_s* p, int inverse, int d, size_t* in_b, size_t* out_b) {
+    if (p->inplace) {
+        *in_b = *out_b = p->domain_bytes;
+        return;
+    }
     size_t s0[3], sd[3], o[3];
     p->g.layout(p->rank, 0, s0, o);
     p->g.layout(p->rank, d, sd, o);
@@ -2055,6 +2085,26 @@ static void field_bytes(const dfft_plan_s* p, int inverse, int d, size_t* in_b, 
     const size_t b0 = s0[0] * s0[1] * s0[2] * real_es, bd = sd[0] * sd[1] * sd[2] * p->esize;
     *in_b = inverse ? bd : b0;
     *out_b = inverse ? b0 : bd;
+}
+
+// In-place plans of one rank: build_schedule gave the views on slot D1 byte offsets from a null base; they address the
+// caller's buffer, like the views on `out` (in_user / out_user 2, the same pointer as `in`).  Every other view without
+// a user flag lies in the plan's one allocated slot.
+static void relocate_buffer_views(const dfft_plan_s* p, Schedule& sc) {
+    const char* slot = static_cast<const char*>(p->slot_ptr[0][p->rank]);
+    auto relocate = [&](const View& v, int& user) {
+        const char* b = static_cast<const char*>(v.seg[0].base);
+        if (user == 0 && !(b >= slot && b < slot + p->slot_bytes)) user = 2;
+    };
+    for (Step& s : sc.steps) {
+        if (s.type != STEP_PASS) continue;
+        relocate(s.prm.in, s.in_user);
+        relocate(s.prm.out, s.out_user);
+        if (s.kernel == KERNEL_ZY_FUSED) {
+            relocate(s.prm_y.in, s.y_in_user);
+            relocate(s.prm_y.out, s.y_out_user);
+        }
+    }
 }
 
 // The one place that decides which schedule a (direction, d) pair runs — used by exec and by dfft_plan_describe, so
@@ -2086,6 +2136,9 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
         // and the fused and batched stages (whose earlier phase writes only the work area, or `out` inside the same launch).
         // tests/test_scale.py replays every such schedule and checks that each output value is scaled exactly once.
         for (Step& s : sc.steps) s.final_store = s.type == STEP_PASS && s.out_user == 2;
+        // In place the buffer also holds intermediates: its views from slot D1 are marked after the final stores.
+        // tests/test_inplace.py replays these schedules on one address range.
+        if (p->buf_slot) relocate_buffer_views(p, sc);
         sc.inverse = inverse ? 1 : 0;
         field_bytes(p, inverse, d, &sc.field_in, &sc.field_out);
         if (g_view_error) return fail(DFFT_ERR_STATE, "internal: segments of one view disagree on the axis stride");
@@ -2104,6 +2157,7 @@ static int exec_common(dfft_plan_t p, void* out, const void* in, int inverse, in
     if (p->g.transform != need_transform) return fail(DFFT_ERR_INVALID, need_transform == DFFT_C2C ? "plan was created for R2C/C2R" : "plan was created for C2C");
     if (d < 1 || d > 3) return fail(DFFT_ERR_INVALID, "d must be 1, 2 or 3");
     if (!out || !in) return fail(DFFT_ERR_INVALID, "null buffer");
+    if (p->inplace && out != in) return fail(DFFT_ERR_INVALID, "in-place plan: out must equal in");
     CK_CUDA(cudaSetDevice(p->comm->device));
     cudaStream_t st = sync ? p->own_stream : (cudaStream_t)stream;
     // A stream capture records the kernels into a graph without running them, so nothing may be set up on the way
@@ -2305,8 +2359,10 @@ int dfft_plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, in
     return dfft_plan_create_batched(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, 1, allocate, plan);
 }
 
-int dfft_plan_create_batched(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
-                             size_t nz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan) {
+}  // extern "C"
+
+static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
+                       size_t nz, size_t p1, size_t p2, size_t batch, bool inplace, int allocate, dfft_plan_t* plan) {
     if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
     if (batch == 0) return fail(DFFT_ERR_INVALID, "batch must be at least 1");
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
@@ -2348,6 +2404,10 @@ int dfft_plan_create_batched(dfft_comm_t comm, const dfft_config* config, int de
         delete p;
         return fail(DFFT_ERR_INVALID, "partition leaves a rank without data");
     }
+    p->inplace = inplace;
+    // the largest stage array of this rank; it also covers the padded real input of in-place R2C plans, which has the
+    // extent of the layout after d = 1
+    p->domain_bytes = g.domain_elems(p->rank) * p->esize;
     {   // the whole batch of every caller buffer (any direction, any partial d) must be addressable
         size_t widest = 0;
         for (int d = 1; d <= 3; ++d) {
@@ -2385,9 +2445,11 @@ int dfft_plan_create_batched(dfft_comm_t comm, const dfft_config* config, int de
     p->any_direct = (p->direct1 && p->grp[1].size() > 1) || (p->direct2 && p->grp[2].size() > 1);
     p->nslots = (d1 ? 1 : 0) + (d2 ? 1 : 0) + ((!d1 || !d2) ? 2 : 0);
     if (p->nslots < 2) p->nslots = 2;
+    // in place on one rank the caller's buffer is the schedules' first slot (D1; both transpositions are local there)
+    p->buf_slot = inplace && P == 1;
+    if (p->buf_slot) p->nslots = 1;
     size_t dom = 0;
     for (int r = 0; r < P; ++r) dom = std::max(dom, g.domain_elems(r));
-    p->domain_bytes = g.domain_elems(me) * p->esize;
     p->slot_bytes = ((dom * p->esize + 255) / 256) * 256;
     p->work_bytes = p->slot_bytes * p->nslots;
     {
@@ -2490,6 +2552,20 @@ int dfft_plan_create_batched(dfft_comm_t comm, const dfft_config* config, int de
     *plan = p;
     return DFFT_SUCCESS;
 }
+
+extern "C" {
+
+int dfft_plan_create_batched(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
+                             size_t nz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan) {
+    return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, false, allocate, plan);
+}
+
+int dfft_plan_create_inplace(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
+                             size_t nz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan) {
+    return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, true, allocate, plan);
+}
+
+int dfft_plan_is_inplace(dfft_plan_t p) { return p && p->inplace ? 1 : 0; }
 
 int dfft_plan_destroy(dfft_plan_t p) {
     if (!p) return DFFT_SUCCESS;
@@ -2704,6 +2780,7 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
     if (!p) return fail(DFFT_ERR_INVALID, "null plan");
     if (p->comm->dry) return fail(DFFT_ERR_STATE, "geometry-only plan");
     if (!p->work || !out || !in) return fail(DFFT_ERR_INVALID, "plan needs its work area and both buffers");
+    if (p->inplace && out != in) return fail(DFFT_ERR_INVALID, "in-place plan: out must equal in");
     CK_CUDA(cudaSetDevice(p->comm->device));
     const int dir = inverse ? 1 : 0;
     if (reps < 1) reps = 3;
@@ -2849,7 +2926,7 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
         if (rc) return rc;
     }
     Schedule& sc = *scp;
-    std::string o = "{\"rank\":" + std::to_string(p->rank) + ",\"esize\":" + std::to_string(p->esize) +
+    std::string o = "{\"rank\":" + std::to_string(p->rank) + ",\"esize\":" + std::to_string(p->esize) + (p->inplace ? ",\"inplace\":true" : "") +
                     (p->batch > 1 ? ",\"batch\":" + std::to_string(p->batch) + ",\"field_in\":" + std::to_string(sc.field_in) +
                                         ",\"field_out\":" + std::to_string(sc.field_out)
                                   : std::string()) +
@@ -2870,7 +2947,8 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
         z.kernel = y.kernel = KERNEL_PASS;
         y.kind = PASS_C2C_TILED;
         y.prm = s_.prm_y;
-        y.in_user = y.out_user = 0;
+        y.in_user = s_.y_in_user;
+        y.out_user = s_.y_out_user;
         y.final_store = false;
         const bool inv = s_.prm.inverse != 0;
         z.label = inv ? "yz pass: z phase" : "zy pass: z phase";
@@ -2922,7 +3000,7 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
             for (size_t k = 0; k < per; ++k) {
                 Step s_ = listed[k];
                 if (s_.type == STEP_PASS) {
-                    if (s_.in_user == 1) s_.prm.in.seg[0].base = (char*)s_.prm.in.seg[0].base + f * sc.field_in;
+                    if (s_.in_user) s_.prm.in.seg[0].base = (char*)s_.prm.in.seg[0].base + f * (s_.in_user == 1 ? sc.field_in : sc.field_out);
                     if (s_.out_user == 2) s_.prm.out.seg[0].base = (char*)s_.prm.out.seg[0].base + f * sc.field_out;
                 }
                 if (sc.overlapped && f > 0 && !seen[s_.stream])

@@ -257,10 +257,13 @@ cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFu
     const int z_per_plane = pz.A1 / TB, y_per_plane = py.A1 * (py.B / TB);  // tiles = work items
     f.order.na = inv ? y_per_plane : z_per_plane;
     f.order.nb = inv ? z_per_plane : y_per_plane;
-    // phase B reads the intermediate: forward the y tiles (rows of TB elements sN apart), inverse the z lines
+    // phase B reads the intermediate: forward the y tiles (rows of TB elements sN apart), inverse the z lines.  A phase B
+    // that stores where it reads (in place, as the inverse of an in-place plan does) would drop its own results: no
+    // discard then.
     const View& mid = inv ? pz.in : py.in;
-    f.discard = inv ? (Z::Z_DISCARD && aligned128(mid.seg[0].base, mid.seg[0].sA0, mid.seg[0].sA1, 1 << LOG2N))
-                    : (Z::Y_DISCARD && aligned128(mid.seg[0].base, mid.seg[0].sA0, mid.seg[0].sA1, mid.sN));
+    const bool in_place = mid.seg[0].base == (inv ? pz.out : py.out).seg[0].base;
+    f.discard = !in_place && (inv ? (Z::Z_DISCARD && aligned128(mid.seg[0].base, mid.seg[0].sA0, mid.seg[0].sA1, 1 << LOG2N))
+                                  : (Z::Y_DISCARD && aligned128(mid.seg[0].base, mid.seg[0].sA0, mid.seg[0].sA1, mid.sN)));
     // persistent: as many CTAs as fit at once (tickets hand out the work; fewer resident CTAs are fine as well).  The
     // grid depends on the work list only, so every launch of a step draws the same number of tickets (zy_launch_of).
     constexpr auto kf = fft_zy_fused_kernel<T, LOG2N, false, false>;

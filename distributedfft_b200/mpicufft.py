@@ -108,9 +108,13 @@ class MPIcuFFT:
         self.initialized = False
 
     # -- plan ------------------------------------------------------------------------------------
-    def initFFT(self, global_size: GlobalSize, partition: Optional[Partition] = None, allocate: bool = True, batch: int = 1):
+    def initFFT(self, global_size: GlobalSize, partition: Optional[Partition] = None, allocate: bool = True, batch: int = 1,
+                inplace: bool = False):
         """`batch` (not in the reference): every exec transforms that many fields, back to back in each buffer — a
-        contiguous [batch, X, Y, Z] tensor; the getters describe one field (dfft_plan_create_batched)."""
+        contiguous [batch, X, Y, Z] tensor; the getters describe one field (dfft_plan_create_batched).
+        `inplace` (dfft_plan_create_inplace): every exec gets the same buffer twice and overwrites its input; fields are
+        getDomainSize() bytes apart.  R2C / C2R use padded real rows: with buf a complex [X, Y, Nz/2+1] tensor, pass
+        torch.view_as_real(buf).view(X, Y, Nz + 2) as the real side."""
         if global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         cfg = _lib.dfft_config(int(self.config.cuda_aware), int(self.config.warmup_rounds), int(self.config.comm_method),
@@ -122,7 +126,12 @@ class MPIcuFFT:
         if self._decomp == PENCIL and partition is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         h = C.c_void_p()
-        if batch == 1:
+        if inplace:
+            if batch < 0:
+                raise ValueError("batch must be at least 1")
+            check(lib().dfft_plan_create_inplace(self.comm._h, C.byref(cfg), self._decomp, self.precision, self.transform, global_size.Nx,
+                                                 global_size.Ny, global_size.Nz, p1, p2, batch, 1 if allocate else 0, C.byref(h)))
+        elif batch == 1:
             check(lib().dfft_plan_create(self.comm._h, C.byref(cfg), self._decomp, self.precision, self.transform,
                                          global_size.Nx, global_size.Ny, global_size.Nz, p1, p2, 1 if allocate else 0, C.byref(h)))
         else:
@@ -207,6 +216,7 @@ class MPIcuFFT:
     def getPartialStart(self, d): return self._triple(lib().dfft_get_partial_start, d)
     def getDomainSize(self): return int(lib().dfft_get_domain_size(self._h))
     def getBatch(self): return int(lib().dfft_get_batch(self._h))
+    def isInPlace(self): return bool(lib().dfft_plan_is_inplace(self._h))
     def getWorkSizeDevice(self): return int(lib().dfft_get_work_size_device(self._h))
     def getWorkSizeHost(self): return int(lib().dfft_get_work_size_host(self._h))
     def getWorkAreaDevice(self): return lib().dfft_get_work_area_device(self._h)
@@ -275,13 +285,13 @@ class MPIcuFFT_Pencil(MPIcuFFT):
     """z FFT -> transpose -> y FFT -> transpose -> x FFT on a P1 x P2 grid. include/mpicufft_pencil.hpp."""
     _decomp = PENCIL
 
-    def initFFT(self, global_size, partition=None, allocate=True, batch=1):
+    def initFFT(self, global_size, partition=None, allocate=True, batch=1, inplace=False):
         if partition is None or global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         if partition.P1 * partition.P2 != self.comm.size:
             raise RuntimeError("Invalid Input Partition!")
         self.partition = partition
-        super().initFFT(global_size, partition, allocate, batch)
+        super().initFFT(global_size, partition, allocate, batch, inplace)
 
     def getPartitionDimensions(self):
         """(input_dim, transposed_dim, output_dim), each a dict with size_x/y/z and start_x/y/z lists

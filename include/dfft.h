@@ -120,6 +120,25 @@ int dfft_plan_create_batched(dfft_comm_t comm, const dfft_config* config, int de
                              int precision /*dfft_prec*/, int transform /*dfft_transform*/, size_t nx, size_t ny,
                              size_t nz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan);
 size_t dfft_get_batch(dfft_plan_t plan); /* fields per exec (1 for dfft_plan_create), 0 for a null plan */
+/* In-place plans (cuFFT and FFTW offer the same): the exec writes its output over its input, so a transform needs one
+ * caller buffer instead of two.  Same arguments and validation as dfft_plan_create_batched.
+ *   - Every exec (plain, _async, partial) and dfft_plan_tune require out == in; another `out` returns DFFT_ERR_INVALID.
+ *     The input is consumed.  dfft_plan_tune runs the transform on the buffer, so it overwrites it as well.
+ *   - The buffer holds dfft_get_domain_size() bytes per field, and field f starts f * dfft_get_domain_size() bytes in, on
+ *     both sides (one distance for input and output).
+ *   - R2C / C2R use the padded real layout of FFTW and cuFFT in-place transforms: real rows are 2 * (Nz/2 + 1) reals apart,
+ *     and the last two reals of each row (Nz is even) are padding that is neither read nor written.  The sizes
+ *     the getters report stay the logical ones (Nz reals).  In torch terms: the real view of a complex [X][Y][Nz/2+1]
+ *     tensor, torch.view_as_real(buf).view(X, Y, Nz + 2), of which the first Nz columns are the data.
+ *   - One rank: the work area is one slot (dfft_get_work_size_device() is half that of the out-of-place plan); the
+ *     caller's buffer holds the first intermediate.  Several ranks keep their work area and schedules and save the
+ *     caller's second buffer.
+ *   - Output scale, partial transforms, batches, dfft_plan_tune and CUDA graph capture work as for other plans.
+ * Out-of-place plans are unchanged; out == in on them is not supported (it needs an in-place plan). */
+int dfft_plan_create_inplace(dfft_comm_t comm, const dfft_config* config, int decomp /*dfft_decomp*/,
+                             int precision /*dfft_prec*/, int transform /*dfft_transform*/, size_t nx, size_t ny,
+                             size_t nz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan);
+int dfft_plan_is_inplace(dfft_plan_t plan); /* 1 for plans of dfft_plan_create_inplace, 0 otherwise (and for a null plan) */
 int dfft_plan_destroy(dfft_plan_t plan);
 /* setWorkArea(device, host) — mpicufft_slab.cpp:236-281. device must hold dfft_get_work_size_device()
  * bytes; with comm_method Peer2Peer and more than one rank it must be the base of a cudaMalloc
@@ -132,6 +151,7 @@ int dfft_set_work_area(dfft_plan_t plan, void* device, void* host);
  *   real/complex input  [in_size[0]][in_size[1]][in_size[2]]     (dfft_get_in_size)
  *   complex output      [out_size[0]][out_size[1]][out_size[2]]  (dfft_get_out_size)
  * `out` of exec_r2c / `in` of exec_c2r must hold dfft_get_domain_size() bytes.
+ * out == in needs a plan of dfft_plan_create_inplace (see there); other plans take two distinct buffers.
  * The plain calls return after the device has finished (the reference's cudaDeviceSynchronize);
  * the _async calls enqueue on `stream` (a cudaStream_t) and return. */
 int dfft_exec_r2c(dfft_plan_t plan, void* out, const void* in);
@@ -211,7 +231,8 @@ int dfft_layout(int decomp, int transform, size_t nx, size_t ny, size_t nz, size
  * benchmark sweeps (jobs/ ** /benchmarks_base.json).  dfft_plan_tune makes it once, at plan time, like FFTW_MEASURE:
  * it runs the transform on the caller's buffers with the sequential schedule and with overlapped schedules that give the
  * exchanging pass different numbers of CTAs, and keeps the fastest (slowest rank decides).  Collective; `out` is
- * overwritten, `in` is not.  Only plans with send_method Streams have alternatives.  Returns the candidate index.
+ * overwritten, `in` is not — except on in-place plans, where out == in and the buffer is overwritten.  Only plans with
+ * send_method Streams have alternatives.  Returns the candidate index.
  * Not capturable: call it before capturing, never on a capturing stream. */
 int dfft_plan_tune(dfft_plan_t plan, void* out, const void* in, int inverse, int reps);
 const char* dfft_plan_tune_report(dfft_plan_t plan);

@@ -85,7 +85,15 @@ public:
         batch_ = batch;
         initFFT(global_size, partition, allocate);
     }
+    // not in the reference: an in-place plan (dfft_plan_create_inplace): every exec takes out == in and overwrites its
+    // input; R2C / C2R use padded real rows of 2 * (Nz/2 + 1) reals
+    void initFFT(GlobalSize* global_size, Partition* partition, bool allocate, size_t batch, bool inplace) {
+        struct Reset { bool& i; ~Reset() { i = false; } } reset{inplace_};
+        inplace_ = inplace;
+        initFFT(global_size, partition, allocate, batch);
+    }
     size_t getBatch() const { return dfft_get_batch(plan); }
+    bool isInPlace() const { return dfft_plan_is_inplace(plan) != 0; }
     // not in the reference: output scale of every forward / inverse exec (dfft_plan_set_scale; after initFFT).  For
     // normalised round trips use setScale(1, 1.0 / (Nx * Ny * Nz)).
     void setScale(double forward_scale, double inverse_scale) { DFFT_CALL(dfft_plan_set_scale(plan, forward_scale, inverse_scale)); }
@@ -115,14 +123,18 @@ protected:
         c.benchmark_dir = config.benchmark_dir.empty() ? nullptr : config.benchmark_dir.c_str();
         c.comm_method2 = config.comm_method2; c.send_method2 = config.send_method2;
         if (plan) { dfft_plan_destroy(plan); plan = nullptr; }
-        if (batch_ == 1)
+        if (inplace_)
+            DFFT_CALL(dfft_plan_create_inplace(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, p1, p2, batch_,
+                                               allocate ? 1 : 0, &plan));
+        else if (batch_ == 1)
             DFFT_CALL(dfft_plan_create(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, p1, p2, allocate ? 1 : 0, &plan));
         else
             DFFT_CALL(dfft_plan_create_batched(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, p1, p2, batch_,
                                                allocate ? 1 : 0, &plan));
         initialized = true;
     }
-    size_t batch_ = 1;  // fields of the plan initFFT is creating
+    size_t batch_ = 1;       // fields of the plan initFFT is creating
+    bool inplace_ = false;   // whether initFFT is creating an in-place plan
     Configurations config;
     dfft_comm_t comm;
     int transform;
