@@ -65,6 +65,9 @@ SIGNATURES = {
     "dfft_exec_r2c_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dfft_exec_c2r_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dfft_exec_c2c_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "dfft_exec_r2r": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "dfft_exec_r2r_partial": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
+    "dfft_exec_r2r_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "dfft_plan_wait": (C.c_int, [C.c_void_p]),
     "dfft_get_in_size": (C.c_int, [C.c_void_p, C.POINTER(C.c_size_t)]),
     "dfft_get_in_start": (C.c_int, [C.c_void_p, C.POINTER(C.c_size_t)]),
@@ -105,6 +108,7 @@ SIGNATURES = {
     "dfft_fft1d_general": (C.c_int, [C.c_int, C.c_int, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.POINTER(C.c_longlong),
                                      C.c_void_p, C.POINTER(C.c_longlong), C.c_void_p]),
     "dfft_fft1d_strided": (C.c_int, [C.c_int, C.c_int, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dfft_fft1d_r2r": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 

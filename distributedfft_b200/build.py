@@ -61,7 +61,7 @@ def build(verbose: bool = False, force: bool = False, defines=(), out: str = LIB
     out=".../libdfft_t128.so", objdir=".../build_t128"); select at run time with DFFT_LIB=<path>)."""
     OBJ_ = objdir
     os.makedirs(OBJ_, exist_ok=True)
-    headers = [os.path.join(CSRC, h) for h in ("fft_core.cuh", "fft_kernels.cuh", "zy_order.hpp", "geometry.hpp", "bluestein.hpp")]
+    headers = [os.path.join(CSRC, h) for h in ("fft_core.cuh", "fft_kernels.cuh", "zy_order.hpp", "geometry.hpp", "bluestein.hpp", "r2r.hpp")]
     headers.append(os.path.join(HERE, "..", "include", "dfft.h"))
     jobs = []
     inst = os.path.join(CSRC, "fft_inst.cu")

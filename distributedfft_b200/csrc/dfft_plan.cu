@@ -92,12 +92,24 @@ static cudaError_t make_bluestein_table(size_t n, void** dev) {
 // (the Bluestein pass)
 static bool bluestein_length(size_t n) { return ilog2_exact(n) < 0 && n >= 3 && n <= size_t(BLUESTEIN_MAX_N); }
 static bool c2c_length(size_t n) { return (ilog2_exact(n) >= 1 && ilog2_exact(n) <= MAX_LOG2N) || bluestein_length(n); }
+// Real-to-real plans (DCT / DST): powers of two in [2, 2^MAX_LOG2N]
+static bool is_r2r(int transform) { return transform == DFFT_DCT || transform == DFFT_DST; }
+static bool r2r_length(size_t n) { return ilog2_exact(n) >= 1 && ilog2_exact(n) <= MAX_LOG2N; }
 
 // One FFT pass of n-point lines (R2C / C2R: n complex points) over the views of prm, its stores scaled by `scale`: the
 // power-of-two kernels, or the Bluestein pass when n is not a power of two (prm.tw: the M-point table; blu: the Bluestein
-// table of n)
-static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftParams& prm, const void* blu, double scale, cudaStream_t stream) {
+// table of n).  PASS_R2R_*: the R2R kernel, DST when dst != 0 (prm.tw2: its w_k table).
+static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftParams& prm, const void* blu, double scale, cudaStream_t stream,
+                                   int dst = 0) {
     const int log2n = ilog2_exact(n);
+    if (kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED) {
+        FftR2r r;
+        static_cast<FftParams&>(r) = prm;
+        r.w = prm.tw2;
+        r.dst = dst;
+        r.scale = scale;
+        return launch_r2r(prec, log2n, kind, r, stream);
+    }
     if (log2n >= 0) return launch_pass(prec, log2n, kind, prm, scale, stream);
     const int log2m = bluestein_log2m(n);
     FftBluestein b;
@@ -452,12 +464,12 @@ static SegN mkseg(void* base, long long sA0, long long sA1, long long sN, size_t
 // schedules build their passes for power-of-two lengths.
 static bool pow2_axes(const dfft_plan_s* p) { return ilog2_exact(p->g.nx) > 0 && ilog2_exact(p->g.ny) > 0 && ilog2_exact(p->g.nz) > 0; }
 
-// Row pitch, in complex units, of the z-contiguous side of the caller's buffers that holds Nz points per row: the input
-// of forward passes, the output of inverse ones.  Real rows of R2C / C2R plans are Nz reals (Nz/2 units) apart, or, in
+// Row pitch, in elements (complex units; reals for DCT / DST plans), of the z-contiguous side of the caller's buffers that
+// holds Nz points per row: the input of forward passes, the output of inverse ones.  Real rows of R2C / C2R plans are Nz reals (Nz/2 units) apart, or, in
 // place, Nzc units apart (the padded layout of FFTW and cuFFT: the last one or two reals of a row are never touched).
 static long long z_row_pitch(const dfft_plan_s* p) {
     const Geometry& g = p->g;
-    return (long long)(g.transform == DFFT_C2C || p->inplace ? g.nzc : g.nz / 2);
+    return (long long)(g.transform != DFFT_R2C || p->inplace ? g.nzc : g.nz / 2);
 }
 
 // Whether the z and y passes run as one fused launch (fft_zy_fused_kernel): one-rank slab C2C plans of the full 3D
@@ -558,7 +570,9 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     const int me = p->rank, P = p->P;
     const int pi = g.pi(me), pj = g.pj(me);
     const size_t es = p->esize;
-    const bool c2c = g.transform == DFFT_C2C;
+    // DCT / DST plans run the C2C builders over reals; new_pass turns their C2C kinds into R2R ones
+    const bool c2c = g.transform != DFFT_R2C;
+    const bool r2r = is_r2r(g.transform);
     Tables& T = p->tabs;
     sc.steps.clear();
 
@@ -566,6 +580,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         s = Step();
         s.type = STEP_PASS;
         s.label = (kind == PASS_C2C_TILED) ? "strided pass" : (kind == PASS_R2C ? "z pass (R2C)" : (kind == PASS_C2R ? "z pass (C2R)" : "z pass"));
+        if (r2r) kind = kind == PASS_C2C_TILED ? PASS_R2R_TILED : PASS_R2R_CONTIG;
         s.kind = kind;
         s.phase = phase;
         s.log2n = ilog2_exact(n);
@@ -584,9 +599,10 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         if (T.get_tw(s.log2n, &tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
         s.prm.tw = tw;
         s.prm.tw2 = nullptr;
-        if (kind == PASS_R2C || kind == PASS_C2R) {
+        if (kind == PASS_R2C || kind == PASS_C2R || r2r) {
+            // R2R: w_k = exp(-i pi k / 2N), k <= N, the R2C table of length 2N
             void* tw2 = nullptr;
-            if (T.get_tw2(s.log2n, &tw2) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
+            if (T.get_tw2(s.log2n + (r2r ? 1 : 0), &tw2) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
             s.prm.tw2 = tw2;
         }
         return DFFT_SUCCESS;
@@ -2019,7 +2035,9 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
                 user(prm_y.out, s.y_out_user);
                 cudaError_t e = cudaErrorInvalidValue;
                 switch (s.kernel) {
-                    case KERNEL_PASS: e = launch_fft_pass(p->prec, s.kind, s.n ? s.n : size_t(1) << s.log2n, prm, s.blu, scale, ss); break;
+                    case KERNEL_PASS:
+                        e = launch_fft_pass(p->prec, s.kind, s.n ? s.n : size_t(1) << s.log2n, prm, s.blu, scale, ss, p->g.transform == DFFT_DST);
+                        break;
                     case KERNEL_ZY_FUSED: e = launch_zy_fused(p->prec, s.log2n, prm, prm_y, s.zyf, scale, ss); break;
                     case KERNEL_BATCH_SMALL:
                         e = launch_batch_small(p->prec, s.log2n, prm.in.seg[0].base, prm.out.seg[0].base, (long long)p->batch, s.prm.inverse, s.bsf, scale, ss);
@@ -2070,7 +2088,7 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
 }
 
 // Bytes of one field in the caller's `in` and `out` of an exec (direction, d): the product of that buffer's layout, in
-// reals for the real side of R2C / C2R.  No schedule touches a caller buffer beyond it (tests/test_batch.py checks every
+// reals for the real side of R2C / C2R and for DCT / DST plans (whose elements are reals).  No schedule touches a caller buffer beyond it (tests/test_batch.py checks every
 // step's accesses), so fields sit back to back at this distance.
 // In-place plans: one buffer, so one distance, dfft_get_domain_size(), which covers every layout (Geometry::domain_elems).
 static void field_bytes(const dfft_plan_s* p, int inverse, int d, size_t* in_b, size_t* out_b) {
@@ -2081,7 +2099,7 @@ static void field_bytes(const dfft_plan_s* p, int inverse, int d, size_t* in_b, 
     size_t s0[3], sd[3], o[3];
     p->g.layout(p->rank, 0, s0, o);
     p->g.layout(p->rank, d, sd, o);
-    const size_t real_es = p->g.transform == DFFT_C2C ? p->esize : p->esize / 2;
+    const size_t real_es = p->g.transform == DFFT_R2C ? p->esize / 2 : p->esize;
     const size_t b0 = s0[0] * s0[1] * s0[2] * real_es, bd = sd[0] * sd[1] * sd[2] * p->esize;
     *in_b = inverse ? bd : b0;
     *out_b = inverse ? b0 : bd;
@@ -2116,14 +2134,14 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
         const bool streams = p->cfg.send_method == DFFT_SEND_STREAMS || (p->g.decomp == DFFT_PENCIL && p->cfg.send_method2 == DFFT_SEND_STREAMS);
         const bool seq_won = p->tuned_seq[inverse ? 1 : 0] != 0;
         const bool want_overlap = streams && d == 3 && p->P > 1 && p->g.decomp == DFFT_SLAB_ZY_THEN_X && p->direct2 && p->xchg_ctas >= 0 && !seq_won &&
-                                  pow2_axes(p);
+                                  pow2_axes(p) && !is_r2r(p->g.transform);
         // pencil: forward on a grid with two real transpositions by default; every other
         // combination (inverse, p1 or p2 == 1) only once dfft_plan_tune has measured it faster than the sequential schedule
         const bool both_multi = p->grp[1].size() > 1 && p->grp[2].size() > 1;
         const bool tuned = p->tuned_ctas[inverse ? 1 : 0] != -2;
         const bool want_pencil_overlap = streams && d == 3 && p->g.decomp == DFFT_PENCIL && p->direct1 && p->direct2 && p->P > 1 && p->xchg_ctas >= 0 &&
                                          pencil_overlap_enabled() && !seq_won && ((both_multi && !inverse) || tuned || pencil_overlap_mode() == 2) &&
-                                         pow2_axes(p);
+                                         pow2_axes(p) && !is_r2r(p->g.transform);
         int rc;
         if (batch_small(p, d)) rc = build_batch_small(p, inverse ? 1 : 0, sc);
         else if (want_overlap) rc = build_overlapped_slab(p, inverse ? 1 : 0, sc);
@@ -2148,13 +2166,17 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
 }
 
 static int timer_gather(dfft_plan_s* p);
+static const char* transform_name(int t) { return t == DFFT_C2C ? "C2C" : t == DFFT_DCT ? "DCT" : t == DFFT_DST ? "DST" : "R2C/C2R"; }
+// need_transform: DFFT_R2C, DFFT_C2C, or EXEC_R2R for the execs of DCT and DST plans
+constexpr int EXEC_R2R = -1;
 static int exec_common(dfft_plan_t p, void* out, const void* in, int inverse, int d, int need_transform, void* stream, bool sync) {
     // sync == true: the plain calls run on the plan's own stream; _async calls use exactly the stream given
     // (NULL = the CUDA default stream)
     if (!p) return fail(DFFT_ERR_INVALID, "null plan");
     if (p->comm->dry) return fail(DFFT_ERR_STATE, "geometry-only plan (dfft_comm_create_dry) cannot execute");
     if (!p->work) return fail(DFFT_ERR_STATE, "plan has no work area (call dfft_set_work_area)");
-    if (p->g.transform != need_transform) return fail(DFFT_ERR_INVALID, need_transform == DFFT_C2C ? "plan was created for R2C/C2R" : "plan was created for C2C");
+    if (need_transform == EXEC_R2R ? !is_r2r(p->g.transform) : p->g.transform != need_transform)
+        return fail(DFFT_ERR_INVALID, std::string("plan was created for ") + transform_name(p->g.transform));
     if (d < 1 || d > 3) return fail(DFFT_ERR_INVALID, "d must be 1, 2 or 3");
     if (!out || !in) return fail(DFFT_ERR_INVALID, "null buffer");
     if (p->inplace && out != in) return fail(DFFT_ERR_INVALID, "in-place plan: out must equal in");
@@ -2366,7 +2388,7 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
     if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
     if (batch == 0) return fail(DFFT_ERR_INVALID, "batch must be at least 1");
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
-    if (transform != DFFT_R2C && transform != DFFT_C2C) return fail(DFFT_ERR_INVALID, "bad transform");
+    if (transform != DFFT_R2C && transform != DFFT_C2C && !is_r2r(transform)) return fail(DFFT_ERR_INVALID, "bad transform");
     const bool dry = comm->dry;
     if (!dry) CK_CUDA(cudaSetDevice(comm->device));
     const auto t_init0 = std::chrono::steady_clock::now();
@@ -2381,7 +2403,7 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
     }
     p->rank = comm->rank; p->P = comm->nranks;
     p->prec = precision;
-    p->esize = precision == DFFT_F64 ? 16 : 8;
+    p->esize = (precision == DFFT_F64 ? 16 : 8) / (is_r2r(transform) ? 2 : 1);  // DCT / DST: real elements
     p->tabs.prec = precision;
     p->tabs.dry = dry;
     if (!p->g.init(decomp, transform, nx, ny, nz, p1, p2, p->P)) {
@@ -2393,6 +2415,11 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
         if (!c2c_length(nx) || !c2c_length(ny) || !c2c_length(nz)) {
             delete p;
             return fail(DFFT_ERR_UNSUPPORTED, "Nx, Ny, Nz of C2C plans must be powers of two in [2, 8192] or any length in [3, 4096]");
+        }
+    } else if (is_r2r(transform)) {
+        if (!r2r_length(nx) || !r2r_length(ny) || !r2r_length(nz)) {
+            delete p;
+            return fail(DFFT_ERR_UNSUPPORTED, "Nx, Ny, Nz of DCT / DST plans must be powers of two in [2, 8192]");
         }
     } else if (ilog2_exact(nx) < 1 || ilog2_exact(ny) < 1 || ilog2_exact(nz) < 1 || ilog2_exact(nx) > MAX_LOG2N || ilog2_exact(ny) > MAX_LOG2N ||
                ilog2_exact(nz) > MAX_LOG2N + 1 || nz < 4) {
@@ -2488,6 +2515,8 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
             return w < lo ? lo : (w > 32 ? size_t(32) : w);
         };
         int ch = int(std::max<size_t>(8, std::max(tile_cols(ny), tile_cols(nx))));
+        // DCT / DST: the R2R tile holds that many column pairs, so the block is twice as many reals wide
+        if (is_r2r(transform)) ch = int(2 * std::max(tile_cols(ny), tile_cols(nx)));
         if (eb) ch = atoi(eb);
         size_t min_nz = g.nzc;  // smallest z extent any rank holds between the y and x passes
         if (decomp == DFFT_PENCIL)
@@ -2620,6 +2649,16 @@ int dfft_exec_r2c_async(dfft_plan_t p, void* out, const void* in, void* stream) 
 int dfft_exec_c2r_async(dfft_plan_t p, void* out, const void* in, void* stream) { return exec_common(p, out, in, 1, 3, DFFT_R2C, stream, false); }
 int dfft_exec_c2c_async(dfft_plan_t p, void* out, const void* in, int direction, void* stream) {
     return exec_common(p, out, in, direction > 0 ? 1 : 0, 3, DFFT_C2C, stream, false);
+}
+
+int dfft_exec_r2r(dfft_plan_t p, void* out, const void* in, int direction) {
+    return exec_common(p, out, in, direction > 0 ? 1 : 0, 3, EXEC_R2R, nullptr, true);
+}
+int dfft_exec_r2r_partial(dfft_plan_t p, void* out, const void* in, int direction, int d) {
+    return exec_common(p, out, in, direction > 0 ? 1 : 0, d, EXEC_R2R, nullptr, true);
+}
+int dfft_exec_r2r_async(dfft_plan_t p, void* out, const void* in, int direction, void* stream) {
+    return exec_common(p, out, in, direction > 0 ? 1 : 0, 3, EXEC_R2R, stream, false);
 }
 
 int dfft_plan_wait(dfft_plan_t p) {
@@ -2792,7 +2831,7 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
     std::vector<Cand> cands;
     cands.push_back({1, 0, 0, 0});
     const bool streams = p->cfg.send_method == DFFT_SEND_STREAMS || (p->g.decomp == DFFT_PENCIL && p->cfg.send_method2 == DFFT_SEND_STREAMS);
-    const bool has_overlap = streams && p->P > 1 && p->xchg_ctas >= 0 && pow2_axes(p) &&
+    const bool has_overlap = streams && p->P > 1 && p->xchg_ctas >= 0 && pow2_axes(p) && !is_r2r(p->g.transform) &&
                              ((p->g.decomp == DFFT_SLAB_ZY_THEN_X && p->direct2) ||
                               (p->g.decomp == DFFT_PENCIL && p->direct1 && p->direct2 && pencil_overlap_enabled()));
     const bool pencil_inv = inverse && p->g.decomp == DFFT_PENCIL;
@@ -2813,8 +2852,9 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
     }
     p->tune_report.clear();
     if (cands.size() == 1) {
-        p->tune_report = pow2_axes(p) ? "sequential schedule (no alternatives for this plan)"
-                                      : "sequential schedule (no alternatives for this plan: an axis length is not a power of two)";
+        p->tune_report = is_r2r(p->g.transform) ? "sequential schedule (no alternatives for this plan: DCT / DST plans run the sequential schedule)"
+                         : pow2_axes(p)         ? "sequential schedule (no alternatives for this plan)"
+                                                : "sequential schedule (no alternatives for this plan: an axis length is not a power of two)";
         return 0;
     }
     const bool was_timing = p->timing;
@@ -2927,6 +2967,7 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
     }
     Schedule& sc = *scp;
     std::string o = "{\"rank\":" + std::to_string(p->rank) + ",\"esize\":" + std::to_string(p->esize) + (p->inplace ? ",\"inplace\":true" : "") +
+                    (is_r2r(p->g.transform) ? std::string(",\"r2r\":\"") + (p->g.transform == DFFT_DST ? "dst" : "dct") + "\"" : std::string()) +
                     (p->batch > 1 ? ",\"batch\":" + std::to_string(p->batch) + ",\"field_in\":" + std::to_string(sc.field_in) +
                                         ",\"field_out\":" + std::to_string(sc.field_out)
                                   : std::string()) +
@@ -3085,18 +3126,20 @@ static Tables& fft1d_tables(int prec) {
     return T;
 }
 
-// one pass of n-point lines over prm's views (R2C / C2R: n complex points), with the tables of its length
-static int fft1d_pass(int prec, PassKind kind, size_t n, FftParams prm, void* stream) {
+// one pass of n-point lines over prm's views (R2C / C2R: n complex points), with the tables of its length; dst: of R2R
+// passes
+static int fft1d_pass(int prec, PassKind kind, size_t n, FftParams prm, void* stream, int dst = 0) {
     Tables& T = fft1d_tables(prec);
     const bool blu = bluestein_length(n);
+    const bool r2r = kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED;
     const int l2 = blu ? bluestein_log2m(n) : ilog2_exact(n);
     void *tw = nullptr, *tw2 = nullptr, *table = nullptr;
     if (blu && T.get_blu(n, &table) != cudaSuccess) return fail(DFFT_ERR_CUDA, "Bluestein table allocation failed");
     if (T.get_tw(l2, &tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
-    if ((kind == PASS_R2C || kind == PASS_C2R) && T.get_tw2(l2, &tw2) != cudaSuccess)
+    if ((kind == PASS_R2C || kind == PASS_C2R || r2r) && T.get_tw2(l2 + (r2r ? 1 : 0), &tw2) != cudaSuccess)
         return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
     prm.tw = tw; prm.tw2 = tw2;
-    cudaError_t e = launch_fft_pass(prec, kind, n, prm, table, 1.0, (cudaStream_t)stream);
+    cudaError_t e = launch_fft_pass(prec, kind, n, prm, table, 1.0, (cudaStream_t)stream, dst);
     if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("launch failed: ") + cudaGetErrorString(e));
     return DFFT_SUCCESS;
 }
@@ -3129,6 +3172,26 @@ int dfft_fft1d_strided(int precision, int direction, size_t a, size_t n, size_t 
     prm.in = single_view(const_cast<void*>(in), (long long)(n * b), 0, (long long)b);
     prm.out = single_view(out, (long long)(n * b), 0, (long long)b);
     return fft1d_pass(precision, PASS_C2C_TILED, n, prm, stream);
+}
+
+int dfft_fft1d_r2r(int precision, int transform, int direction, size_t n, size_t a, size_t b, void* out, const void* in, void* stream) {
+    if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
+    if (!is_r2r(transform)) return fail(DFFT_ERR_INVALID, "transform must be DFFT_DCT or DFFT_DST");
+    if (!r2r_length(n)) return fail(DFFT_ERR_UNSUPPORTED, "length must be a power of two in [2, 8192]");
+    if (a == 0 || b == 0) return DFFT_SUCCESS;
+    if (a * b > size_t(0x7fffffff) || n * b > size_t(1) << 62) return fail(DFFT_ERR_INVALID, "array too large");
+    FftParams prm{};
+    prm.inverse = direction > 0 ? 1 : 0;
+    if (b == 1) {  // CONTIG: a lines of n reals
+        prm.A0 = 1; prm.A1 = int(a); prm.B = 1;
+        prm.in = single_view(const_cast<void*>(in), 0, (long long)n, 1);
+        prm.out = single_view(out, 0, (long long)n, 1);
+    } else {       // TILED: [a][n][b], b contiguous
+        prm.A0 = int(a); prm.A1 = 1; prm.B = int(b);
+        prm.in = single_view(const_cast<void*>(in), (long long)(n * b), 0, (long long)b);
+        prm.out = single_view(out, (long long)(n * b), 0, (long long)b);
+    }
+    return fft1d_pass(precision, b == 1 ? PASS_R2R_CONTIG : PASS_R2R_TILED, n, prm, stream, transform == DFFT_DST);
 }
 
 int dfft_fft1d_general(int precision, int direction, size_t n, size_t a0, size_t a1, size_t b, void* out, const long long out_strides[3],

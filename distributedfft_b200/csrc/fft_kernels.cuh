@@ -27,6 +27,7 @@
 #include <type_traits>
 
 #include "fft_core.cuh"
+#include "r2r.hpp"
 #include "zy_order.hpp"
 
 namespace dfft {
@@ -76,7 +77,8 @@ struct FftScaled : FftParams {
 template <bool SCALED>
 using KParams = std::conditional_t<SCALED, FftScaled, FftParams>;
 
-enum PassKind { PASS_C2C_CONTIG = 0, PASS_C2C_TILED = 1, PASS_R2C = 2, PASS_C2R = 3 };
+// PASS_R2R_*: the view mapping of PASS_C2C_* over real elements (fft_r2r_kernel)
+enum PassKind { PASS_C2C_CONTIG = 0, PASS_C2C_TILED = 1, PASS_R2C = 2, PASS_C2R = 3, PASS_R2R_CONTIG = 4, PASS_R2R_TILED = 5 };
 
 // ---- tile shape choices (compile time) -----------------------------------------------------------
 template <typename T, int LOG2N>
@@ -151,12 +153,13 @@ __device__ __forceinline__ void st_elem(cx<T>* p, cx<T> v) {
 }
 
 // ---- per-thread access to one line of a view ----------------------------------------------------------
-// LINES = lines per CTA that need their own segment table (TB for CONTIG, 1 for TILED).
-template <typename T, int LINES>
+// LINES = lines per CTA that need their own segment table (TB for CONTIG, 1 for TILED).  EL: the element the view counts in
+// (complex, or T for the real views of R2R passes).
+template <typename T, int LINES, typename EL = cx<T>>
 struct LineAccess {
     static constexpr int TABLE_ELEMS = LINES * MAXSEG;  // unsigned long long entries in shared memory
     const View& v;
-    cx<T>* p0;                  // single segment: element n = 0 of this thread's line (b included)
+    EL* p0;                     // single segment: element n = 0 of this thread's line (b included)
     const unsigned long long* tab;  // multi segment: tab[s] = address of element n = 0 of segment s (b excluded)
     long long boff;             // multi segment: + b (elements)
     bool multi;
@@ -167,7 +170,7 @@ struct LineAccess {
         if (v.nseg <= 1) return;
         for (int s = lane_in_line; s < v.nseg; s += lanes_per_line) {
             const Seg& g = v.seg[s];
-            cx<T>* p = reinterpret_cast<cx<T>*>(g.base) + (a0 * g.sA0 + a1 * g.sA1 - (long long)g.n0 * v.sN);
+            EL* p = reinterpret_cast<EL*>(g.base) + (a0 * g.sA0 + a1 * g.sA1 - (long long)g.n0 * v.sN);
             table[line_in_cta * MAXSEG + s] = reinterpret_cast<unsigned long long>(p);
         }
     }
@@ -175,20 +178,20 @@ struct LineAccess {
         : v(v_) {
         multi = v.nseg > 1;
         const Seg& g = v.seg[0];
-        p0 = reinterpret_cast<cx<T>*>(g.base) + (a0 * g.sA0 + a1 * g.sA1 - (long long)g.n0 * v.sN + b);
+        p0 = reinterpret_cast<EL*>(g.base) + (a0 * g.sA0 + a1 * g.sA1 - (long long)g.n0 * v.sN + b);
         tab = table + line_in_cta * MAXSEG;
         boff = b;
     }
-    __device__ __forceinline__ cx<T>* at(int n) const {
+    __device__ __forceinline__ EL* at(int n) const {
         if (!multi) return p0 + (long long)n * v.sN;
         const int s = v.seg_of_n[n];
-        return reinterpret_cast<cx<T>*>(tab[s]) + ((long long)n * v.sN + boff);
+        return reinterpret_cast<EL*>(tab[s]) + ((long long)n * v.sN + boff);
     }
     // unit stride along n (every CONTIG view): no multiply
-    __device__ __forceinline__ cx<T>* at1(int n) const {
+    __device__ __forceinline__ EL* at1(int n) const {
         if (!multi) return p0 + n;
         const int s = v.seg_of_n[n];
-        return reinterpret_cast<cx<T>*>(tab[s]) + (n + boff);
+        return reinterpret_cast<EL*>(tab[s]) + (n + boff);
     }
 };
 
@@ -1174,6 +1177,175 @@ fft_bluestein_kernel(const __grid_constant__ FftBluestein p) {
     }
 }
 
+// ---- real-to-real pass: DCT-II / DCT-III and DST-II / DST-III of real N-point lines ------------------------------------
+// Two real lines a, b are packed into one complex N-point line (r2r.hpp) and transformed by CtaFft's stages on the tile of
+// the power-of-two kernels; no half-length core.  The views count in reals (LineAccess<T, ., T>).
+//   CONTIG: the pair (2L, 2L+1) of the flattened (a0, a1) line order takes line slot L of the tile, TB slots per CTA.
+//   TILED:  the columns (2c, 2c+1) of the contiguous dimension take column c of the tile: a tile is N x 2 TB reals.
+// An odd count gives the last line or column a zero partner, whose results are not stored.
+// Forward: the permuted loads reach their reals straight from global memory (the two halves of a sector are read by two
+// instructions of the same warp, the second from L1); after the stages Z goes through shared memory once, so that point k
+// meets Z[N-k].  Inverse: X[k] and X[N-k] are both loaded from global memory and Z is built in registers; the stores are
+// permuted.  One CTA per tile and every load before any store, so out == in works.  A scale != 1 multiplies the final
+// stores (__dmul_rn / __fmul_rn: the scaled output is the unscaled one times s, bit for bit).
+struct FftR2r : FftParams {
+    const void* w;  // w_k = exp(-i pi k / 2N), k <= N (the R2C table of length 2N: Tables::get_tw2(log2 N + 1))
+    int dst;        // 0 DCT, 1 DST
+    double scale;   // output scale, applied when != 1 (rounded to the kernel's precision once)
+};
+
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED>
+struct R2rShape {
+    using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
+    static constexpr int LINES = TILED ? 1 : 2 * TB;  // real lines with their own segment table
+    static constexpr size_t SMEM_BYTES = C::TILE_BYTES + size_t(2) * LINES * MAXSEG * sizeof(unsigned long long);
+    static_assert(SMEM_BYTES <= 227 * 1024, "R2R tile does not fit the shared memory of a CTA");
+};
+
+template <typename T>
+__device__ __forceinline__ T rscale(T v, T s) {
+    if constexpr (sizeof(T) == 8) return __dmul_rn(v, s);
+    else return __fmul_rn(v, s);
+}
+
+// reals q[0] and (second) q[1]: one 2-element access when q is aligned to it, two scalar ones otherwise (odd strides)
+template <typename T>
+__device__ __forceinline__ void ld_pair(const T* q, bool second, T& a, T& b) {
+    if (second && (reinterpret_cast<unsigned long long>(q) & (2 * sizeof(T) - 1)) == 0) {
+        const cx<T> r = ld_elem<T>(reinterpret_cast<const cx<T>*>(q));
+        a = r.x; b = r.y;
+    } else {
+        a = q[0];
+        b = second ? q[1] : T(0);
+    }
+}
+template <typename T>
+__device__ __forceinline__ void st_pair(T* q, bool second, T a, T b) {
+    if (second && (reinterpret_cast<unsigned long long>(q) & (2 * sizeof(T) - 1)) == 0) {
+        st_elem<T>(reinterpret_cast<cx<T>*>(q), cx<T>{a, b});
+    } else {
+        q[0] = a;
+        if (second) q[1] = b;
+    }
+}
+
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV>
+__global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
+fft_r2r_kernel(const __grid_constant__ FftR2r p) {
+    using RS = R2rShape<T, LOG2N, LOG2E, TB, TILED>;
+    using C = typename RS::C;
+    using LA = LineAccess<T, RS::LINES, T>;
+    constexpr int E = C::E, TPL = C::TPL, N = C::N;
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
+    unsigned long long* tab_in = reinterpret_cast<unsigned long long*>(smem_raw + C::TILE_BYTES);
+    unsigned long long* tab_out = tab_in + RS::LINES * MAXSEG;
+    const int tid = threadIdx.x;
+    // line a and its partner b: (a0, a1) of each and whether it exists; TILED: b is column `col` + 1 of the same row
+    int j, t, a0a, a1a, a0b, a1b, col = 0;
+    bool va, vb;
+    if constexpr (TILED) {
+        t = tid % TB; j = tid / TB;
+        const int nbt = ((p.B + 1) / 2 + TB - 1) / TB;  // tiles of TB column pairs
+        const int bt = int(blockIdx.x % unsigned(nbt)), a = int(blockIdx.x / unsigned(nbt));
+        a1a = a1b = a % p.A1;
+        a0a = a0b = a / p.A1;
+        col = 2 * (bt * TB + t);
+        va = col < p.B;
+        vb = col + 1 < p.B;
+    } else {
+        j = tid % TPL; t = tid / TPL;
+        const long long lines = (long long)p.A0 * p.A1;
+        const long long la = 2 * ((long long)blockIdx.x * TB + t), lb = la + 1;
+        va = la < lines;
+        vb = lb < lines;
+        a1a = int(la % p.A1); a0a = int(la / p.A1);
+        a1b = int(lb % p.A1); a0b = int(lb / p.A1);
+    }
+    if (p.in.nseg > 1 || p.out.nseg > 1) {
+        if constexpr (TILED) {
+            LA::fill_table(p.in, tab_in, 0, tid, C::THREADS, a0a, a1a);
+            LA::fill_table(p.out, tab_out, 0, tid, C::THREADS, a0a, a1a);
+        } else {
+            LA::fill_table(p.in, tab_in, 2 * t, j, TPL, a0a, a1a);
+            LA::fill_table(p.in, tab_in, 2 * t + 1, j, TPL, a0b, a1b);
+            LA::fill_table(p.out, tab_out, 2 * t, j, TPL, a0a, a1a);
+            LA::fill_table(p.out, tab_out, 2 * t + 1, j, TPL, a0b, a1b);
+        }
+        __syncthreads();
+    }
+    // TILED: line b is the next real of line a's row, so one access object serves both
+    const LA ina(p.in, tab_in, TILED ? 0 : 2 * t, a0a, a1a, col), outa(p.out, tab_out, TILED ? 0 : 2 * t, a0a, a1a, col);
+    const LA inb(p.in, tab_in, TILED ? 0 : 2 * t + 1, a0b, a1b, 0), outb(p.out, tab_out, TILED ? 0 : 2 * t + 1, a0b, a1b, 0);
+    const cx<T>* w = reinterpret_cast<const cx<T>*>(p.w);
+    const cx<T>* tw = reinterpret_cast<const cx<T>*>(p.tw);
+    const int dst = p.dst;
+    const bool scaled = p.scale != 1.0;
+    const T s = T(p.scale);
+    // reals m of both lines (0 for a missing line)
+    auto load2 = [&](int m, T& a, T& b) {
+        a = T(0); b = T(0);
+        if constexpr (TILED) {
+            if (va) ld_pair<T>(ina.at(m), vb, a, b);
+        } else {
+            if (va) a = *ina.at1(m);
+            if (vb) b = *inb.at1(m);
+        }
+    };
+    auto store2 = [&](int m, T a, T b) {
+        if (scaled) { a = rscale<T>(a, s); b = rscale<T>(b, s); }
+        if constexpr (TILED) {
+            if (va) st_pair<T>(outa.at(m), vb, a, b);
+        } else {
+            if (va) *outa.at1(m) = a;
+            if (vb) *outb.at1(m) = b;
+        }
+    };
+
+    cx<T> v[E];
+    if constexpr (!INV) {
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            const int m = r2r_perm(j + e * TPL, N);
+            const T sg = r2r_sign<T>(m, dst);
+            T a, b;
+            load2(m, a, b);
+            v[e] = cx<T>{sg * a, sg * b};
+        }
+        C::template stages<0>(v, j, t, sm, tw);
+        // Z in natural order -> shared memory, then point k with Z[N-k]
+        if constexpr (C::NST > 1) C::sync(t);
+#pragma unroll
+        for (int e = 0; e < E; ++e) sm[C::sidx(j + e * TPL, t)] = v[C::Core::final_slot(e)];
+        C::sync(t);
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            const int k = j + e * TPL;
+            const cx<T> x = r2r_split<T>(sm[C::sidx(k, t)], sm[C::sidx((N - k) & (N - 1), t)], ld_tw(w, k));
+            store2(r2r_out_index(k, N, dst), x.x, x.y);
+        }
+    } else {
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            const int k = j + e * TPL;
+            const int nk = r2r_in_nk(k, N, dst);
+            T ak, bk, am = T(0), bm = T(0);
+            load2(r2r_in_k(k, N, dst), ak, bk);
+            if (nk >= 0) load2(nk, am, bm);
+            // stored with re/im swapped: the inverse transform is run as swap(fwd(swap(.)))
+            v[e] = cswap(r2r_build<T>(ak, am, bk, bm, ld_tw(w, k)));
+        }
+        C::template stages<0>(v, j, t, sm, tw);
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            const cx<T> z = cswap(v[C::Core::final_slot(e)]);
+            const int m = r2r_perm(j + e * TPL, N);
+            const T sg = r2r_sign<T>(m, dst);
+            store2(m, sg * z.x, sg * z.y);
+        }
+    }
+}
+
 // ---- host launchers (one explicit instantiation per precision and size, see fft_inst.cu) ----------------
 // scale: the output scale of the pass' stores; 1 launches the unscaled kernels, anything else their scaled twins.
 template <typename T, int LOG2N>
@@ -1206,6 +1378,12 @@ cudaError_t launch_batch_small(int prec, int log2n, const void* in, void* out, l
 template <typename T, int LOG2M>
 cudaError_t launch_bluestein(PassKind kind, const FftBluestein& p, cudaStream_t stream);
 cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluestein& p, cudaStream_t stream);
+
+// R2R pass (fft_r2r_kernel) of 2^LOG2N-point real lines: kind PASS_R2R_CONTIG (sN == 1, line pairs) or PASS_R2R_TILED
+// (column pairs), views in reals, one CTA per tile; p.scale scales the stores.  Instantiated for LOG2N 1..13.
+template <typename T, int LOG2N>
+cudaError_t launch_r2r(PassKind kind, const FftR2r& p, cudaStream_t stream);
+cudaError_t launch_r2r(int prec, int log2n, PassKind kind, const FftR2r& p, cudaStream_t stream);
 
 constexpr int MAX_LOG2N = 13;
 constexpr int BLUESTEIN_MAX_N = 4096;  // 2n - 1 <= 2^MAX_LOG2N

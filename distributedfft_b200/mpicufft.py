@@ -16,7 +16,7 @@ from .params import CommunicationMethod, Configurations, GlobalSize, Partition, 
 
 SLAB_ZY_THEN_X, SLAB_Z_THEN_YX, PENCIL = 0, 1, 2
 F32, F64 = 0, 1
-R2C, C2C = 0, 1
+R2C, C2C, DCT, DST = 0, 1, 2, 3
 FORWARD, INVERSE = -1, 1
 
 
@@ -84,7 +84,8 @@ class Comm:
 
 class MPIcuFFT:
     """Abstract plan (include/mpicufft.hpp:55-105). `precision`: 'double' | 'float' replaces the C++
-    template argument; `transform`: 'r2c' (the reference's) or 'c2c'."""
+    template argument; `transform`: 'r2c' (the reference's), 'c2c', or the real-to-real 'dct' / 'dst' (type II forward, type III
+    inverse, on all three axes; execR2R)."""
 
     _decomp = SLAB_ZY_THEN_X
 
@@ -102,8 +103,12 @@ class MPIcuFFT:
             self.transform = R2C
         elif transform in ("c2c", "C2C"):
             self.transform = C2C
+        elif transform in ("dct", "DCT"):
+            self.transform = DCT
+        elif transform in ("dst", "DST"):
+            self.transform = DST
         else:
-            raise ValueError(f"transform must be 'r2c' or 'c2c', got {transform!r}")
+            raise ValueError(f"transform must be 'r2c', 'c2c', 'dct' or 'dst', got {transform!r}")
         self._h = None
         self.initialized = False
 
@@ -191,6 +196,19 @@ class MPIcuFFT:
         if d == 3:
             return check(lib().dfft_exec_c2c(self._h, _ptr(out), _ptr(in_), direction))
         return check(lib().dfft_exec_c2c_partial(self._h, _ptr(out), _ptr(in_), direction, d))
+
+    def execR2R(self, out, in_, direction: int = FORWARD, d: int = 3, stream=None):
+        """Real-to-real transform of a 'dct' / 'dst' plan (not in the reference): FORWARD is type II, INVERSE type III, both
+        unnormalised like scipy.fft.dct / dst(norm=None).  Real [x][y][z] buffers.  `stream` as for execR2C, capturable the
+        same way."""
+        self._need()
+        if stream is not None:
+            if d != 3:
+                raise ValueError("async partial transforms are not exposed")
+            return check(lib().dfft_exec_r2r_async(self._h, _ptr(out), _ptr(in_), direction, _stream_ptr(stream)))
+        if d == 3:
+            return check(lib().dfft_exec_r2r(self._h, _ptr(out), _ptr(in_), direction))
+        return check(lib().dfft_exec_r2r_partial(self._h, _ptr(out), _ptr(in_), direction, d))
 
     def wait(self):
         return check(lib().dfft_plan_wait(self._h))
@@ -298,7 +316,7 @@ class MPIcuFFT_Pencil(MPIcuFFT):
         (Partition_Dimensions, params.hpp:58-81; mpicufft_pencil.hpp:112-116)."""
         from .params import partition_sizes
         g, p = self.global_size, self.partition
-        nzc = g.Nz if self.transform == C2C else g.Nz // 2 + 1
+        nzc = g.Nz // 2 + 1 if self.transform == R2C else g.Nz
 
         def dims(nx_parts, ny_parts, nz_parts, nz):
             d = {}
@@ -330,6 +348,12 @@ def fft1d_contig(precision: int, kind: int, direction: int, n: int, lines: int, 
 
 def fft1d_strided(precision: int, direction: int, a: int, n: int, b: int, out, in_, stream=None):
     check(lib().dfft_fft1d_strided(precision, direction, a, n, b, _ptr(out), _ptr(in_), _stream_ptr(stream)))
+
+
+def fft1d_r2r(precision: int, transform: int, direction: int, n: int, a: int, b: int, out, in_, stream=None):
+    """DCT / DST (transform DCT or DST; FORWARD type II, INVERSE type III) along the middle axis of a dense real [a][n][b]
+    array, b contiguous; out may be in_."""
+    check(lib().dfft_fft1d_r2r(precision, transform, direction, n, a, b, _ptr(out), _ptr(in_), _stream_ptr(stream)))
 
 
 def fft1d_general(precision: int, direction: int, n: int, a0: int, a1: int, b: int, out, out_strides, in_, in_strides, stream=None):

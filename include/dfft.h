@@ -77,7 +77,23 @@ typedef enum { DFFT_F32 = 0, DFFT_F64 = 1 } dfft_prec; /* cuFFT<float> / cuFFT<d
 /* The reference only offers real<->complex (execR2C/execC2R).  DFFT_C2C plans add the complex
  * transform the benchmark configurations name; the z extent of every complex array is then Nz instead
  * of Nz/2+1. */
-typedef enum { DFFT_R2C = 0, DFFT_C2C = 1 } dfft_transform;
+typedef enum { DFFT_R2C = 0, DFFT_C2C = 1, DFFT_DCT = 2, DFFT_DST = 3 } dfft_transform;
+/* DFFT_DCT / DFFT_DST plans (not in the reference; cuFFT has neither, FFTW calls them REDFT10 / REDFT01 and RODFT10 /
+ * RODFT01): real-to-real transforms, the same kind along all three axes, for spectral solvers with Neumann (DCT) or
+ * Dirichlet (DST) boundaries.  With N the axis length:
+ *   forward, type II:   DCT  y_k = 2 sum_n x_n cos(pi k (2n+1) / 2N)      DST  y_k = 2 sum_n x_n sin(pi (k+1)(2n+1) / 2N)
+ *   inverse, type III:  DCT  y_k = x_0 + 2 sum_{n>=1} x_n cos(pi n (2k+1) / 2N)
+ *                       DST  y_k = (-1)^k x_{N-1} + 2 sum_{n<N-1} x_n sin(pi (n+1)(2k+1) / 2N)
+ * exactly scipy.fft.dct / dst(type=2 | 3, norm=None).  Both directions are unnormalised: a round trip scales by
+ * 8 Nx Ny Nz (partial transforms: 2^d times the product of the first d lengths).
+ *   - Buffers are real [x][y][z], z contiguous, with the partition and the getters of a C2C plan (the z extent is Nz
+ *     everywhere); dfft_get_domain_size counts bytes of reals.
+ *   - Lengths: powers of two in [2, 8192] per axis; others return DFFT_ERR_UNSUPPORTED.
+ *   - Every decomposition with Peer2Peer and All2All, partial d, batches, in-place plans, dfft_plan_set_scale, graph
+ *     capture of one-rank _async execs, the timer and dfft_plan_describe work as for C2C plans.
+ *   - Execs: dfft_exec_r2r*; the R2C / C2R / C2C execs return DFFT_ERR_INVALID on these plans, and dfft_exec_r2r* on
+ *     others.
+ *   - The sequential schedule always runs, also with send_method Streams (dfft_plan_tune has one candidate). */
 
 typedef struct dfft_comm_s* dfft_comm_t;
 typedef struct dfft_plan_s* dfft_plan_t;
@@ -160,10 +176,13 @@ int dfft_exec_c2r(dfft_plan_t plan, void* out, const void* in);
 #define DFFT_FORWARD (-1)
 #define DFFT_INVERSE (1)
 int dfft_exec_c2c(dfft_plan_t plan, void* out, const void* in, int direction);
+/* DFFT_DCT / DFFT_DST plans: direction DFFT_FORWARD runs type II, DFFT_INVERSE type III. */
+int dfft_exec_r2r(dfft_plan_t plan, void* out, const void* in, int direction);
 /* pencil execR2C(out,in,d)/execC2R(out,in,d): transform only the first d dimensions (z; z,y; z,y,x). */
 int dfft_exec_r2c_partial(dfft_plan_t plan, void* out, const void* in, int d);
 int dfft_exec_c2r_partial(dfft_plan_t plan, void* out, const void* in, int d);
 int dfft_exec_c2c_partial(dfft_plan_t plan, void* out, const void* in, int direction, int d);
+int dfft_exec_r2r_partial(dfft_plan_t plan, void* out, const void* in, int direction, int d);
 
 /* CUDA graphs: an _async call on a stream that is being captured (cudaStreamBeginCapture, torch.cuda.graph) records
  * the transform's kernels into the graph instead of running them, for plans of one rank:
@@ -180,6 +199,7 @@ int dfft_exec_c2c_partial(dfft_plan_t plan, void* out, const void* in, int direc
 int dfft_exec_r2c_async(dfft_plan_t plan, void* out, const void* in, void* stream);
 int dfft_exec_c2r_async(dfft_plan_t plan, void* out, const void* in, void* stream);
 int dfft_exec_c2c_async(dfft_plan_t plan, void* out, const void* in, int direction, void* stream);
+int dfft_exec_r2r_async(dfft_plan_t plan, void* out, const void* in, int direction, void* stream);
 /* Output scale (not in the reference; cuFFT has none either).  Every exec of a direction multiplies each output value by
  * that direction's scale: the real and imaginary parts of complex outputs, the real values of C2R outputs.  It applies to
  * the plain and _async calls, R2C / C2R / C2C, partial transforms (the value is used as given), every field of a batched
@@ -278,6 +298,11 @@ int dfft_fft1d_contig(int precision, int kind, int direction, size_t n, size_t l
 /* Batched 1D C2C along the middle axis of a [a][n][b] array (b contiguous). */
 int dfft_fft1d_strided(int precision, int direction, size_t a, size_t n, size_t b, void* out, const void* in,
                        void* stream);
+
+/* DCT / DST (transform DFFT_DCT or DFFT_DST; forward type II, inverse type III, unnormalised) along the middle axis of
+ * a dense real [a][n][b] array, b contiguous; n a power of two in [2, 8192].  out == in is allowed. */
+int dfft_fft1d_r2r(int precision, int transform, int direction, size_t n, size_t a, size_t b, void* out, const void* in,
+                   void* stream);
 
 /* ---- test hooks -----------------------------------------------------------------------------------------
  * Geometry-only communicator: plans created on it never touch CUDA or NCCL (slot addresses are synthetic,

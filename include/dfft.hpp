@@ -100,6 +100,11 @@ public:
     void getScale(double& forward_scale, double& inverse_scale) const { DFFT_CALL(dfft_plan_get_scale(plan, &forward_scale, &inverse_scale)); }
     virtual void setWorkArea(void* device = nullptr, void* host = nullptr) { DFFT_CALL(dfft_set_work_area(plan, device, host)); }
     virtual void execR2C(void* out, const void* in) = 0;
+    // not in the reference: real-to-real transform of a plan constructed with transform_ = DFFT_DCT or DFFT_DST (forward
+    // type II, inverse type III, unnormalised); d < 3 transforms only the first d dimensions
+    void execR2R(void* out, const void* in, int direction, int d = 3) {
+        DFFT_CALL(d == 3 ? dfft_exec_r2r(plan, out, in, direction) : dfft_exec_r2r_partial(plan, out, in, direction, d));
+    }
 
     virtual void getInSize(size_t* isize) { DFFT_CALL(dfft_get_in_size(plan, isize)); }
     virtual void getInStart(size_t* istart) { DFFT_CALL(dfft_get_in_start(plan, istart)); }
@@ -194,7 +199,7 @@ public:
     virtual void execC2C(void* out, const void* in, int direction, int d = 3) { DFFT_CALL(dfft_exec_c2c_partial(this->plan, out, in, direction, d)); }
     // getPartitionDimensions(input_dim, transposed_dim, output_dim) — mpicufft_pencil.hpp:112-116
     void getPartitionDimensions(Partition_Dimensions& in_, Partition_Dimensions& tr_, Partition_Dimensions& out_) {
-        const size_t nzc = this->transform == DFFT_C2C ? gs_.Nz : gs_.Nz / 2 + 1;
+        const size_t nzc = this->transform == DFFT_R2C ? gs_.Nz / 2 + 1 : gs_.Nz;
         auto fill = [](std::vector<size_t>& size, std::vector<size_t>& start, size_t n, size_t parts) {
             size.resize(parts); start.resize(parts);
             dfft_partition(n, parts, size.data(), start.data());
