@@ -92,23 +92,25 @@ static cudaError_t make_bluestein_table(size_t n, void** dev) {
 // (the Bluestein pass)
 static bool bluestein_length(size_t n) { return ilog2_exact(n) < 0 && n >= 3 && n <= size_t(BLUESTEIN_MAX_N); }
 static bool c2c_length(size_t n) { return (ilog2_exact(n) >= 1 && ilog2_exact(n) <= MAX_LOG2N) || bluestein_length(n); }
-// Real-to-real plans (DCT / DST): powers of two in [2, 2^MAX_LOG2N]
-static bool is_r2r(int transform) { return transform == DFFT_DCT || transform == DFFT_DST; }
+// Real-to-real plans: powers of two in [2, 2^MAX_LOG2N].  The transform of a plan from dfft_plan_create_r2r is DFFT_DCT or
+// DFFT_DST when all three kinds are that one, DFFT_R2HC for any other combination (its kinds are in dfft_plan_s::kinds).
+static bool is_r2r(int transform) { return transform == DFFT_DCT || transform == DFFT_DST || transform == DFFT_R2HC; }
+static const char* r2r_name(int k) { return k == DFFT_DST ? "dst" : k == DFFT_R2HC ? "r2hc" : "dct"; }
 static bool r2r_length(size_t n) { return ilog2_exact(n) >= 1 && ilog2_exact(n) <= MAX_LOG2N; }
 
 // One FFT pass of n-point lines (R2C / C2R: n complex points) over the views of prm, its stores scaled by `scale`: the
 // power-of-two kernels, or the Bluestein pass when n is not a power of two (prm.tw: the M-point table; blu: the Bluestein
-// table of n).  PASS_R2R_*: the R2R kernel, DST when dst != 0 (prm.tw2: its w_k table).
+// table of n).  PASS_R2R_*: the R2R kernel of kind r2r (DFFT_DCT, DFFT_DST with prm.tw2 its w_k table, or DFFT_R2HC).
 static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftParams& prm, const void* blu, double scale, cudaStream_t stream,
-                                   int dst = 0) {
+                                   int r2r = DFFT_DCT) {
     const int log2n = ilog2_exact(n);
     if (kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED) {
         FftR2r r;
         static_cast<FftParams&>(r) = prm;
         r.w = prm.tw2;
-        r.dst = dst;
+        r.dst = r2r == DFFT_DST;
         r.scale = scale;
-        return launch_r2r(prec, log2n, kind, r, stream);
+        return launch_r2r(prec, log2n, kind, r, r2r == DFFT_R2HC, stream);
     }
     if (log2n >= 0) return launch_pass(prec, log2n, kind, prm, scale, stream);
     const int log2m = bluestein_log2m(n);
@@ -280,6 +282,7 @@ struct Step {
     size_t n = 0;
     const void* blu = nullptr;
     bool bluestein() const { return n != 0 && n != (size_t(1) << log2n); }
+    int r2r = 0;  // PASS_R2R_*: the kind of the axis it transforms (DFFT_DCT, DFFT_DST or DFFT_R2HC)
     FftParams prm{};
     int in_user = 0, out_user = 0;  // 1: patch seg[0].base with the caller's in, 2: with the caller's out
     // RENDEZVOUS
@@ -330,6 +333,7 @@ struct dfft_plan_s {
     int prec = DFFT_F64;
     size_t esize = 16;  // bytes per complex element
     int rank = 0, P = 1;
+    int kinds[3] = {0, 0, 0};  // real-to-real plans: the kind of the x, y and z axis
     size_t batch = 1;         // fields per exec, back to back in every caller buffer (dfft_plan_create_batched)
     double scale[2] = {1.0, 1.0};  // [fwd/inv] output scale (dfft_plan_set_scale), applied by the steps marked final_store
     // dfft_plan_create_inplace: every exec has out == in, fields domain_bytes apart, real rows of R2C / C2R padded to Nzc
@@ -576,11 +580,15 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     Tables& T = p->tabs;
     sc.steps.clear();
 
-    auto new_pass = [&](PassKind kind, size_t n, const char* phase, Step& s) -> int {
+    // axis: 0 x, 1 y, 2 z — R2R passes take their kind from it
+    auto new_pass = [&](PassKind kind, size_t n, int axis, const char* phase, Step& s) -> int {
         s = Step();
         s.type = STEP_PASS;
         s.label = (kind == PASS_C2C_TILED) ? "strided pass" : (kind == PASS_R2C ? "z pass (R2C)" : (kind == PASS_C2R ? "z pass (C2R)" : "z pass"));
-        if (r2r) kind = kind == PASS_C2C_TILED ? PASS_R2R_TILED : PASS_R2R_CONTIG;
+        if (r2r) {
+            kind = kind == PASS_C2C_TILED ? PASS_R2R_TILED : PASS_R2R_CONTIG;
+            s.r2r = p->kinds[axis];
+        }
         s.kind = kind;
         s.phase = phase;
         s.log2n = ilog2_exact(n);
@@ -599,8 +607,8 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         if (T.get_tw(s.log2n, &tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
         s.prm.tw = tw;
         s.prm.tw2 = nullptr;
-        if (kind == PASS_R2C || kind == PASS_C2R || r2r) {
-            // R2R: w_k = exp(-i pi k / 2N), k <= N, the R2C table of length 2N
+        if (kind == PASS_R2C || kind == PASS_C2R || (r2r && s.r2r != DFFT_R2HC)) {
+            // DCT / DST: w_k = exp(-i pi k / 2N), k <= N, the R2C table of length 2N
             void* tw2 = nullptr;
             if (T.get_tw2(s.log2n + (r2r ? 1 : 0), &tw2) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
             s.prm.tw2 = tw2;
@@ -677,7 +685,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         // ------------------------------------------------------------------ forward
         // pass 1: z (contiguous), lines (x in nx_i, y in ny_j)
         Step s1;
-        rc = new_pass(c2c ? PASS_C2C_CONTIG : PASS_R2C, c2c ? g.nz : g.nz / 2, zyx || g.decomp == DFFT_PENCIL ? "1D FFT Z-Direction" : nullptr, s1);
+        rc = new_pass(c2c ? PASS_C2C_CONTIG : PASS_R2C, c2c ? g.nz : g.nz / 2, 2, zyx || g.decomp == DFFT_PENCIL ? "1D FFT Z-Direction" : nullptr, s1);
         if (rc) return rc;
         s1.prm.A0 = int(nx_i); s1.prm.A1 = int(ny_j);
         {   // input: caller's buffer; real lines of nz reals = nz/2 complex (in place: padded rows)
@@ -732,7 +740,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         // pass 2: y (tiled): a0 = x, n = y, b = z in nz_j
         Step s2;
         const size_t nx2 = zyx ? g.nx : nx_i;  // x extent held after transposition 1
-        rc = new_pass(PASS_C2C_TILED, g.ny, g.decomp == DFFT_SLAB_ZY_THEN_X ? "2D FFT Y-Z-Direction" : (zyx ? nullptr : "1D FFT Y-Direction"), s2);
+        rc = new_pass(PASS_C2C_TILED, g.ny, 1, g.decomp == DFFT_SLAB_ZY_THEN_X ? "2D FFT Y-Z-Direction" : (zyx ? nullptr : "1D FFT Y-Direction"), s2);
         if (rc) return rc;
         s2.label = "y pass";
         s2.prm.A0 = int(nx2); s2.prm.A1 = 1; s2.prm.B = int(nz_j);
@@ -758,7 +766,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
             if (s2.prm.in.nseg != 1) return fail(DFFT_ERR_STATE, "internal: z_then_yx gather view");
             sc.steps.push_back(s2);
             Step s3;
-            rc = new_pass(PASS_C2C_TILED, g.nx, "2D FFT Y-X-Direction", s3);
+            rc = new_pass(PASS_C2C_TILED, g.nx, 0, "2D FFT Y-X-Direction", s3);
             if (rc) return rc;
             s3.label = "x pass";
             s3.prm.A0 = 1; s3.prm.A1 = 1; s3.prm.B = int(g.ny * nz_j);
@@ -842,7 +850,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
 
         // pass 3: x (tiled): n = x, b = (y in oy_i, z in nz_j); received blocks are x-major => contiguous
         Step s3;
-        rc = new_pass(PASS_C2C_TILED, g.nx, "1D FFT X-Direction", s3);
+        rc = new_pass(PASS_C2C_TILED, g.nx, 0, "1D FFT X-Direction", s3);
         if (rc) return rc;
         s3.label = "x pass";
         if (CH) {
@@ -883,7 +891,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
 
     if (d == 1) {
         Step s;
-        rc = new_pass(zkind, zlen, "1D FFT Z-Direction", s);
+        rc = new_pass(zkind, zlen, 2, "1D FFT Z-Direction", s);
         if (rc) return rc;
         s.prm.A0 = int(nx_i); s.prm.A1 = int(ny_j);
         s.prm.in = single_view(nullptr, (long long)(ny_j * nzc), (long long)nzc, 1);
@@ -899,7 +907,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         // input [nx][ny][nz_me]: y pass (to a slot), x pass scattering along x to the owners of x,
         // then z inverse on [nx_me][ny][nzc].
         Step sy_;
-        rc = new_pass(PASS_C2C_TILED, g.ny, nullptr, sy_);
+        rc = new_pass(PASS_C2C_TILED, g.ny, 1, nullptr, sy_);
         if (rc) return rc;
         sy_.label = "y pass";
         const int W = dir1 ? D2 : SR;  // a local scratch slot that is not the transposition target
@@ -909,7 +917,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         sy_.prm.out = single_view(slotp(W, me), (long long)(g.ny * nz_j), 0, (long long)nz_j);
         sc.steps.push_back(sy_);
         Step sx_;
-        rc = new_pass(PASS_C2C_TILED, g.nx, "2D FFT Y-X-Direction", sx_);
+        rc = new_pass(PASS_C2C_TILED, g.nx, 0, "2D FFT Y-X-Direction", sx_);
         if (rc) return rc;
         sx_.label = "x pass";
         sx_.prm.A0 = 1; sx_.prm.A1 = int(g.ny); sx_.prm.B = int(nz_j);
@@ -929,7 +937,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         if (!dir1) { xa.phase = "Transpose (Finished All2All)"; xa.group = 1; sc.steps.push_back(xa); }
         else if (G1.size() > 1) rendezvous(1, 1, "Transpose (Finished Receive)");
         Step sz_;
-        rc = new_pass(zkind, zlen, "1D FFT Z-Direction", sz_);
+        rc = new_pass(zkind, zlen, 2, "1D FFT Z-Direction", sz_);
         if (rc) return rc;
         sz_.prm.A0 = int(nx_i); sz_.prm.A1 = int(g.ny);
         if (dir1) sz_.prm.in = single_view(slotp(D1, me), (long long)(g.ny * nzc), (long long)nzc, 1);
@@ -960,7 +968,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         else any_rem = rem != 0;
         // x pass: in = caller's [nx][oy_i][nz_j]; tile = (y_loc, z block); n = x
         Step s3;
-        rc = new_pass(PASS_C2C_TILED, g.nx, "1D FFT X-Direction", s3);
+        rc = new_pass(PASS_C2C_TILED, g.nx, 0, "1D FFT X-Direction", s3);
         if (rc) return rc;
         s3.label = "x pass";
         s3.prm.A0 = int(oy_i); s3.prm.A1 = int(nzm / CH); s3.prm.B = int(CH);
@@ -993,7 +1001,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         if (G2.size() > 1) rendezvous(2, 2, slab ? "Transpose (Finished Receive)" : "Second Transpose (Finished Receive)");
         // y pass: in = my slot, blocked [nz_j/CH][ny][nx_i][CH]; tile = (x_loc, z block); n = y
         Step s2;
-        rc = new_pass(PASS_C2C_TILED, g.ny, slab ? nullptr : "1D FFT Y-Direction", s2);
+        rc = new_pass(PASS_C2C_TILED, g.ny, 1, slab ? nullptr : "1D FFT Y-Direction", s2);
         if (rc) return rc;
         s2.label = "y pass";
         s2.prm.A0 = int(nx_i); s2.prm.A1 = int(nzm / CH); s2.prm.B = int(CH);
@@ -1022,7 +1030,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         }
         if (G1.size() > 1) rendezvous(1, 1, "First Transpose (Finished Receive)");
         Step s1;
-        rc = new_pass(zkind, zlen, slab ? "2D FFT Y-Z-Direction" : "1D FFT Z-Direction", s1);
+        rc = new_pass(zkind, zlen, 2, slab ? "2D FFT Y-Z-Direction" : "1D FFT Z-Direction", s1);
         if (rc) return rc;
         s1.prm.A0 = int(nx_i); s1.prm.A1 = int(ny_j);
         s1.prm.in = single_view(slotp(D1, me), (long long)(ny_j * nzc), (long long)nzc, 1);
@@ -1044,7 +1052,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     bool have_in_slot = false;  // whether the y pass input is in a slot (d == 3) or the caller's buffer (d == 2)
     if (d == 3) {
         Step s3;
-        rc = new_pass(PASS_C2C_TILED, g.nx, "1D FFT X-Direction", s3);
+        rc = new_pass(PASS_C2C_TILED, g.nx, 0, "1D FFT X-Direction", s3);
         if (rc) return rc;
         s3.label = "x pass";
         s3.prm.A0 = 1; s3.prm.A1 = 1; s3.prm.B = int(oy_i * nz_j);
@@ -1069,7 +1077,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     }
     // y pass on [nx_i][ny][nz_j]
     Step s2;
-    rc = new_pass(PASS_C2C_TILED, g.ny, slab ? nullptr : "1D FFT Y-Direction", s2);
+    rc = new_pass(PASS_C2C_TILED, g.ny, 1, slab ? nullptr : "1D FFT Y-Direction", s2);
     if (rc) return rc;
     s2.label = "y pass";
     s2.prm.A0 = int(nx_i); s2.prm.A1 = 1; s2.prm.B = int(nz_j);
@@ -1104,7 +1112,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     else if (G1.size() > 1) rendezvous(1, 1, "First Transpose (Finished Receive)");
     // z pass on [nx_i][ny_j][nzc]
     Step s1;
-    rc = new_pass(zkind, zlen, slab ? "2D FFT Y-Z-Direction" : "1D FFT Z-Direction", s1);
+    rc = new_pass(zkind, zlen, 2, slab ? "2D FFT Y-Z-Direction" : "1D FFT Z-Direction", s1);
     if (rc) return rc;
     s1.prm.A0 = int(nx_i); s1.prm.A1 = int(ny_j);
     if (dir1) s1.prm.in = single_view(slotp(D1, me), (long long)(ny_j * nzc), (long long)nzc, 1);
@@ -2036,7 +2044,7 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
                 cudaError_t e = cudaErrorInvalidValue;
                 switch (s.kernel) {
                     case KERNEL_PASS:
-                        e = launch_fft_pass(p->prec, s.kind, s.n ? s.n : size_t(1) << s.log2n, prm, s.blu, scale, ss, p->g.transform == DFFT_DST);
+                        e = launch_fft_pass(p->prec, s.kind, s.n ? s.n : size_t(1) << s.log2n, prm, s.blu, scale, ss, s.r2r);
                         break;
                     case KERNEL_ZY_FUSED: e = launch_zy_fused(p->prec, s.log2n, prm, prm_y, s.zyf, scale, ss); break;
                     case KERNEL_BATCH_SMALL:
@@ -2166,8 +2174,10 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
 }
 
 static int timer_gather(dfft_plan_s* p);
-static const char* transform_name(int t) { return t == DFFT_C2C ? "C2C" : t == DFFT_DCT ? "DCT" : t == DFFT_DST ? "DST" : "R2C/C2R"; }
-// need_transform: DFFT_R2C, DFFT_C2C, or EXEC_R2R for the execs of DCT and DST plans
+static const char* transform_name(int t) {
+    return t == DFFT_C2C ? "C2C" : t == DFFT_DCT ? "DCT" : t == DFFT_DST ? "DST" : t == DFFT_R2HC ? "per-axis R2R" : "R2C/C2R";
+}
+// need_transform: DFFT_R2C, DFFT_C2C, or EXEC_R2R for the execs of real-to-real plans
 constexpr int EXEC_R2R = -1;
 static int exec_common(dfft_plan_t p, void* out, const void* in, int inverse, int d, int need_transform, void* stream, bool sync) {
     // sync == true: the plain calls run on the plan's own stream; _async calls use exactly the stream given
@@ -2383,12 +2393,15 @@ int dfft_plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, in
 
 }  // extern "C"
 
+// kinds: of the plans of dfft_plan_create_r2r (their transform is DFFT_DCT, DFFT_DST or DFFT_R2HC), nullptr otherwise
 static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
-                       size_t nz, size_t p1, size_t p2, size_t batch, bool inplace, int allocate, dfft_plan_t* plan) {
+                       size_t nz, size_t p1, size_t p2, size_t batch, bool inplace, int allocate, dfft_plan_t* plan,
+                       const int* kinds = nullptr) {
     if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
     if (batch == 0) return fail(DFFT_ERR_INVALID, "batch must be at least 1");
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
     if (transform != DFFT_R2C && transform != DFFT_C2C && !is_r2r(transform)) return fail(DFFT_ERR_INVALID, "bad transform");
+    if (transform == DFFT_R2HC && !kinds) return fail(DFFT_ERR_INVALID, "bad transform (per-axis kinds: dfft_plan_create_r2r)");
     const bool dry = comm->dry;
     if (!dry) CK_CUDA(cudaSetDevice(comm->device));
     const auto t_init0 = std::chrono::steady_clock::now();
@@ -2403,6 +2416,7 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
     }
     p->rank = comm->rank; p->P = comm->nranks;
     p->prec = precision;
+    for (int a = 0; a < 3; ++a) p->kinds[a] = kinds ? kinds[a] : is_r2r(transform) ? transform : 0;
     p->esize = (precision == DFFT_F64 ? 16 : 8) / (is_r2r(transform) ? 2 : 1);  // DCT / DST: real elements
     p->tabs.prec = precision;
     p->tabs.dry = dry;
@@ -2595,6 +2609,24 @@ int dfft_plan_create_inplace(dfft_comm_t comm, const dfft_config* config, int de
 }
 
 int dfft_plan_is_inplace(dfft_plan_t p) { return p && p->inplace ? 1 : 0; }
+
+int dfft_plan_create_r2r(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, const int kinds[3], size_t nx, size_t ny,
+                         size_t nz, size_t p1, size_t p2, size_t batch, int inplace, int allocate, dfft_plan_t* plan) {
+    if (!kinds) return fail(DFFT_ERR_INVALID, "null kinds");
+    for (int a = 0; a < 3; ++a)
+        if (!is_r2r(kinds[a])) return fail(DFFT_ERR_INVALID, "kinds must be DFFT_DCT, DFFT_DST or DFFT_R2HC");
+    // three DCT (DST) axes make exactly the DCT (DST) plan
+    const bool uniform = kinds[0] == kinds[1] && kinds[1] == kinds[2] && kinds[0] != DFFT_R2HC;
+    return plan_create(comm, config, decomp, precision, uniform ? kinds[0] : DFFT_R2HC, nx, ny, nz, p1, p2, batch, inplace != 0, allocate, plan,
+                       kinds);
+}
+
+int dfft_plan_get_r2r_kinds(dfft_plan_t p, int kinds[3]) {
+    if (!p || !kinds) return fail(DFFT_ERR_INVALID, "null plan / kinds");
+    if (!is_r2r(p->g.transform)) return fail(DFFT_ERR_INVALID, std::string("plan was created for ") + transform_name(p->g.transform));
+    for (int a = 0; a < 3; ++a) kinds[a] = p->kinds[a];
+    return DFFT_SUCCESS;
+}
 
 int dfft_plan_destroy(dfft_plan_t p) {
     if (!p) return DFFT_SUCCESS;
@@ -2966,8 +2998,14 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
         if (rc) return rc;
     }
     Schedule& sc = *scp;
+    const bool per_axis = p->g.transform == DFFT_R2HC;
+    const bool uniform = p->kinds[0] == p->kinds[1] && p->kinds[1] == p->kinds[2];
     std::string o = "{\"rank\":" + std::to_string(p->rank) + ",\"esize\":" + std::to_string(p->esize) + (p->inplace ? ",\"inplace\":true" : "") +
-                    (is_r2r(p->g.transform) ? std::string(",\"r2r\":\"") + (p->g.transform == DFFT_DST ? "dst" : "dct") + "\"" : std::string()) +
+                    // "mixed" when the axes differ; per-axis plans also list the kinds, and each R2R pass its own below
+                    (is_r2r(p->g.transform) ? std::string(",\"r2r\":\"") + (uniform ? r2r_name(p->kinds[0]) : "mixed") + "\"" : std::string()) +
+                    (per_axis ? std::string(",\"r2r_kinds\":[\"") + r2r_name(p->kinds[0]) + "\",\"" + r2r_name(p->kinds[1]) + "\",\"" +
+                                    r2r_name(p->kinds[2]) + "\"]"
+                              : std::string()) +
                     (p->batch > 1 ? ",\"batch\":" + std::to_string(p->batch) + ",\"field_in\":" + std::to_string(sc.field_in) +
                                         ",\"field_out\":" + std::to_string(sc.field_out)
                                   : std::string()) +
@@ -3072,7 +3110,8 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
         for (size_t w = 0; w < s_.waits.size(); ++w) o += (w ? "," : "") + std::to_string(s_.waits[w]);
         o += "]";
         if (s_.type == STEP_PASS) {
-            o += ",\"kind\":" + std::to_string(int(s_.kind)) + ",\"log2n\":" + std::to_string(s_.log2n) +
+            o += ",\"kind\":" + std::to_string(int(s_.kind)) + (per_axis ? std::string(",\"r2r\":\"") + r2r_name(s_.r2r) + "\"" : std::string()) +
+                 ",\"log2n\":" + std::to_string(s_.log2n) +
                  (s_.bluestein() ? ",\"n\":" + std::to_string(s_.n) : std::string()) + ",\"A0\":" + std::to_string(s_.prm.A0) +
                  ",\"A1\":" + std::to_string(s_.prm.A1) + ",\"B\":" + std::to_string(s_.prm.B) + ",\"inverse\":" + std::to_string(s_.prm.inverse) +
                  ",\"in_user\":" + std::to_string(s_.in_user) + ",\"out_user\":" + std::to_string(s_.out_user) + ",\"in\":";
@@ -3126,12 +3165,12 @@ static Tables& fft1d_tables(int prec) {
     return T;
 }
 
-// one pass of n-point lines over prm's views (R2C / C2R: n complex points), with the tables of its length; dst: of R2R
-// passes
-static int fft1d_pass(int prec, PassKind kind, size_t n, FftParams prm, void* stream, int dst = 0) {
+// one pass of n-point lines over prm's views (R2C / C2R: n complex points), with the tables of its length; r2r: the kind of
+// R2R passes
+static int fft1d_pass(int prec, PassKind kind, size_t n, FftParams prm, void* stream, int r2r_k = DFFT_DCT) {
     Tables& T = fft1d_tables(prec);
     const bool blu = bluestein_length(n);
-    const bool r2r = kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED;
+    const bool r2r = (kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED) && r2r_k != DFFT_R2HC;  // with a w_k table
     const int l2 = blu ? bluestein_log2m(n) : ilog2_exact(n);
     void *tw = nullptr, *tw2 = nullptr, *table = nullptr;
     if (blu && T.get_blu(n, &table) != cudaSuccess) return fail(DFFT_ERR_CUDA, "Bluestein table allocation failed");
@@ -3139,7 +3178,7 @@ static int fft1d_pass(int prec, PassKind kind, size_t n, FftParams prm, void* st
     if ((kind == PASS_R2C || kind == PASS_C2R || r2r) && T.get_tw2(l2 + (r2r ? 1 : 0), &tw2) != cudaSuccess)
         return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
     prm.tw = tw; prm.tw2 = tw2;
-    cudaError_t e = launch_fft_pass(prec, kind, n, prm, table, 1.0, (cudaStream_t)stream, dst);
+    cudaError_t e = launch_fft_pass(prec, kind, n, prm, table, 1.0, (cudaStream_t)stream, r2r_k);
     if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("launch failed: ") + cudaGetErrorString(e));
     return DFFT_SUCCESS;
 }
@@ -3176,7 +3215,7 @@ int dfft_fft1d_strided(int precision, int direction, size_t a, size_t n, size_t 
 
 int dfft_fft1d_r2r(int precision, int transform, int direction, size_t n, size_t a, size_t b, void* out, const void* in, void* stream) {
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
-    if (!is_r2r(transform)) return fail(DFFT_ERR_INVALID, "transform must be DFFT_DCT or DFFT_DST");
+    if (!is_r2r(transform)) return fail(DFFT_ERR_INVALID, "transform must be DFFT_DCT, DFFT_DST or DFFT_R2HC");
     if (!r2r_length(n)) return fail(DFFT_ERR_UNSUPPORTED, "length must be a power of two in [2, 8192]");
     if (a == 0 || b == 0) return DFFT_SUCCESS;
     if (a * b > size_t(0x7fffffff) || n * b > size_t(1) << 62) return fail(DFFT_ERR_INVALID, "array too large");
@@ -3191,7 +3230,7 @@ int dfft_fft1d_r2r(int precision, int transform, int direction, size_t n, size_t
         prm.in = single_view(const_cast<void*>(in), (long long)(n * b), 0, (long long)b);
         prm.out = single_view(out, (long long)(n * b), 0, (long long)b);
     }
-    return fft1d_pass(precision, b == 1 ? PASS_R2R_CONTIG : PASS_R2R_TILED, n, prm, stream, transform == DFFT_DST);
+    return fft1d_pass(precision, b == 1 ? PASS_R2R_CONTIG : PASS_R2R_TILED, n, prm, stream, transform);
 }
 
 int dfft_fft1d_general(int precision, int direction, size_t n, size_t a0, size_t a1, size_t b, void* out, const long long out_strides[3],

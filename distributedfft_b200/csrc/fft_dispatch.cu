@@ -31,8 +31,8 @@ cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluest
     return dispatch<3, MAX_LOG2N>(prec, log2m, [&](auto t, auto l) { return launch_bluestein<decltype(t), decltype(l)::value>(kind, p, stream); });
 }
 
-cudaError_t launch_r2r(int prec, int log2n, PassKind kind, const FftR2r& p, cudaStream_t stream) {
-    return dispatch<1, MAX_LOG2N>(prec, log2n, [&](auto t, auto l) { return launch_r2r<decltype(t), decltype(l)::value>(kind, p, stream); });
+cudaError_t launch_r2r(int prec, int log2n, PassKind kind, const FftR2r& p, bool hc, cudaStream_t stream) {
+    return dispatch<1, MAX_LOG2N>(prec, log2n, [&](auto t, auto l) { return launch_r2r<decltype(t), decltype(l)::value>(kind, p, hc, stream); });
 }
 
 cudaError_t launch_zy_fused(int prec, int log2n, const FftParams& pz, const FftParams& py, const ZyFused& f, double scale, cudaStream_t stream) {

@@ -238,34 +238,37 @@ template cudaError_t launch_bluestein<DFFT_T, DFFT_LOG2N>(PassKind, const FftBlu
 #endif
 
 template <typename T, int LOG2N, int TB, bool TILED>
-static cudaError_t launch_r2r_tiles(const FftR2r& p, long long grid, cudaStream_t stream) {
+static cudaError_t launch_r2r_tiles(const FftR2r& p, bool hc, long long grid, cudaStream_t stream) {
     using RS = R2rShape<T, LOG2N, Shape<T, LOG2N>::LOG2E, TB, TILED>;
+    constexpr int LOG2E = Shape<T, LOG2N>::LOG2E;
     if (grid <= 0) return cudaSuccess;
     if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-    return launch_kernel<fft_r2r_kernel<T, LOG2N, Shape<T, LOG2N>::LOG2E, TB, TILED, false>,
-                         fft_r2r_kernel<T, LOG2N, Shape<T, LOG2N>::LOG2E, TB, TILED, true>, nullptr, nullptr>(
+    if (hc)
+        return launch_kernel<fft_r2hc_kernel<T, LOG2N, LOG2E, TB, TILED, false>, fft_r2hc_kernel<T, LOG2N, LOG2E, TB, TILED, true>, nullptr, nullptr>(
+            p, 1.0, unsigned(grid), RS::C::THREADS, RS::SMEM_BYTES, stream);
+    return launch_kernel<fft_r2r_kernel<T, LOG2N, LOG2E, TB, TILED, false>, fft_r2r_kernel<T, LOG2N, LOG2E, TB, TILED, true>, nullptr, nullptr>(
         p, 1.0, unsigned(grid), RS::C::THREADS, RS::SMEM_BYTES, stream);
 }
 
 // CONTIG: TBC line pairs per CTA; TILED: the tile of the C2C pass, TBT column pairs wide (2 TBT reals: the blocked
 // hand-over width of R2R plans)
 template <typename T, int LOG2N>
-cudaError_t launch_r2r(PassKind kind, const FftR2r& p, cudaStream_t stream) {
+cudaError_t launch_r2r(PassKind kind, const FftR2r& p, bool hc, cudaStream_t stream) {
     using S = Shape<T, LOG2N>;
-    if (!p.w || !p.tw) return cudaErrorInvalidValue;
+    if ((!hc && !p.w) || !p.tw) return cudaErrorInvalidValue;
     const long long lines = (long long)p.A0 * p.A1;
     if (lines <= 0) return cudaSuccess;
     if (kind == PASS_R2R_CONTIG) {
         if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
-        return launch_r2r_tiles<T, LOG2N, S::TBC, false>(p, ((lines + 1) / 2 + S::TBC - 1) / S::TBC, stream);
+        return launch_r2r_tiles<T, LOG2N, S::TBC, false>(p, hc, ((lines + 1) / 2 + S::TBC - 1) / S::TBC, stream);
     }
     if (kind != PASS_R2R_TILED) return cudaErrorInvalidValue;
     if (p.B <= 0) return cudaSuccess;
     const long long pairs = ((long long)p.B + 1) / 2;
-    return launch_r2r_tiles<T, LOG2N, S::TBT, true>(p, lines * ((pairs + S::TBT - 1) / S::TBT), stream);
+    return launch_r2r_tiles<T, LOG2N, S::TBT, true>(p, hc, lines * ((pairs + S::TBT - 1) / S::TBT), stream);
 }
 
-template cudaError_t launch_r2r<DFFT_T, DFFT_LOG2N>(PassKind, const FftR2r&, cudaStream_t);
+template cudaError_t launch_r2r<DFFT_T, DFFT_LOG2N>(PassKind, const FftR2r&, bool, cudaStream_t);
 
 #if DFFT_LOG2N == 8 || DFFT_LOG2N == 9
 static bool aligned128(const void* base, long long elems_a, long long elems_b, long long elems_c) {

@@ -1177,7 +1177,7 @@ fft_bluestein_kernel(const __grid_constant__ FftBluestein p) {
     }
 }
 
-// ---- real-to-real pass: DCT-II / DCT-III and DST-II / DST-III of real N-point lines ------------------------------------
+// ---- real-to-real pass: DCT-II / DCT-III, DST-II / DST-III and R2HC / HC2R of real N-point lines ------------------------
 // Two real lines a, b are packed into one complex N-point line (r2r.hpp) and transformed by CtaFft's stages on the tile of
 // the power-of-two kernels; no half-length core.  The views count in reals (LineAccess<T, ., T>).
 //   CONTIG: the pair (2L, 2L+1) of the flattened (a0, a1) line order takes line slot L of the tile, TB slots per CTA.
@@ -1229,9 +1229,10 @@ __device__ __forceinline__ void st_pair(T* q, bool second, T a, T b) {
     }
 }
 
-template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV>
-__global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
-fft_r2r_kernel(const __grid_constant__ FftR2r p) {
+// The body of both R2R kernels.  HC: R2HC / HC2R (r2r.hpp) — natural order, no w_k and no sign flips; p.w and p.dst are
+// not read.  A compile-time mode keeps the R2HC branches out of the DCT / DST instantiations (and their registers).
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, bool HC>
+__device__ __forceinline__ void r2r_pass(const FftR2r& p) {
     using RS = R2rShape<T, LOG2N, LOG2E, TB, TILED>;
     using C = typename RS::C;
     using LA = LineAccess<T, RS::LINES, T>;
@@ -1303,7 +1304,41 @@ fft_r2r_kernel(const __grid_constant__ FftR2r p) {
     };
 
     cx<T> v[E];
-    if constexpr (!INV) {
+    if constexpr (HC && !INV) {
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            T a, b;
+            load2(j + e * TPL, a, b);
+            v[e] = cx<T>{a, b};
+        }
+        C::template stages<0>(v, j, t, sm, tw);
+        if constexpr (C::NST > 1) C::sync(t);
+#pragma unroll
+        for (int e = 0; e < E; ++e) sm[C::sidx(j + e * TPL, t)] = v[C::Core::final_slot(e)];
+        C::sync(t);
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            const int k = j + e * TPL;
+            const cx<T> x = r2hc_split<T>(sm[C::sidx(k, t)], sm[C::sidx((N - k) & (N - 1), t)], k, N);
+            store2(k, x.x, x.y);
+        }
+    } else if constexpr (HC) {
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            const int k = j + e * TPL;
+            const int nk = r2hc_in_nk(k, N);
+            T ak, bk, am = T(0), bm = T(0);
+            load2(k, ak, bk);
+            if (nk >= 0) load2(nk, am, bm);
+            v[e] = cswap(r2hc_build<T>(ak, am, bk, bm, k, N));
+        }
+        C::template stages<0>(v, j, t, sm, tw);
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            const cx<T> z = cswap(v[C::Core::final_slot(e)]);
+            store2(j + e * TPL, z.x, z.y);
+        }
+    } else if constexpr (!INV) {
 #pragma unroll
         for (int e = 0; e < E; ++e) {
             const int m = r2r_perm(j + e * TPL, N);
@@ -1346,6 +1381,19 @@ fft_r2r_kernel(const __grid_constant__ FftR2r p) {
     }
 }
 
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV>
+__global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
+fft_r2r_kernel(const __grid_constant__ FftR2r p) {
+    r2r_pass<T, LOG2N, LOG2E, TB, TILED, INV, false>(p);
+}
+
+// R2HC forward, HC2R inverse: the DCT / DST kernel's tile, pairing, views and scale
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV>
+__global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
+fft_r2hc_kernel(const __grid_constant__ FftR2r p) {
+    r2r_pass<T, LOG2N, LOG2E, TB, TILED, INV, true>(p);
+}
+
 // ---- host launchers (one explicit instantiation per precision and size, see fft_inst.cu) ----------------
 // scale: the output scale of the pass' stores; 1 launches the unscaled kernels, anything else their scaled twins.
 template <typename T, int LOG2N>
@@ -1379,11 +1427,12 @@ template <typename T, int LOG2M>
 cudaError_t launch_bluestein(PassKind kind, const FftBluestein& p, cudaStream_t stream);
 cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluestein& p, cudaStream_t stream);
 
-// R2R pass (fft_r2r_kernel) of 2^LOG2N-point real lines: kind PASS_R2R_CONTIG (sN == 1, line pairs) or PASS_R2R_TILED
-// (column pairs), views in reals, one CTA per tile; p.scale scales the stores.  Instantiated for LOG2N 1..13.
+// R2R pass of 2^LOG2N-point real lines: kind PASS_R2R_CONTIG (sN == 1, line pairs) or PASS_R2R_TILED (column pairs), views
+// in reals, one CTA per tile; p.scale scales the stores.  hc: R2HC / HC2R (fft_r2hc_kernel), otherwise DCT / DST
+// (fft_r2r_kernel, p.dst).  Instantiated for LOG2N 1..13.
 template <typename T, int LOG2N>
-cudaError_t launch_r2r(PassKind kind, const FftR2r& p, cudaStream_t stream);
-cudaError_t launch_r2r(int prec, int log2n, PassKind kind, const FftR2r& p, cudaStream_t stream);
+cudaError_t launch_r2r(PassKind kind, const FftR2r& p, bool hc, cudaStream_t stream);
+cudaError_t launch_r2r(int prec, int log2n, PassKind kind, const FftR2r& p, bool hc, cudaStream_t stream);
 
 constexpr int MAX_LOG2N = 13;
 constexpr int BLUESTEIN_MAX_N = 4096;  // 2n - 1 <= 2^MAX_LOG2N

@@ -26,7 +26,7 @@ struct Split {
 
 struct Geometry {
     int decomp = 0, transform = 0;
-    size_t nx = 0, ny = 0, nz = 0, nzc = 0;  // nzc: z extent of every complex array (DCT / DST: of every real array, Nz)
+    size_t nx = 0, ny = 0, nz = 0, nzc = 0;  // nzc: z extent of every complex array (real-to-real: of every real array, Nz)
     int P = 1, P1 = 1, P2 = 1;
     // x split of the input (over P1, or over P for both slab sequences)
     Split sx;
@@ -39,7 +39,7 @@ struct Geometry {
     bool init(int decomp_, int transform_, size_t nx_, size_t ny_, size_t nz_, size_t p1, size_t p2, int nranks) {
         decomp = decomp_; transform = transform_;
         nx = nx_; ny = ny_; nz = nz_;
-        nzc = (transform == DFFT_C2C || transform == DFFT_DCT || transform == DFFT_DST) ? nz : nz / 2 + 1;
+        nzc = (transform == DFFT_C2C || transform == DFFT_DCT || transform == DFFT_DST || transform == DFFT_R2HC) ? nz : nz / 2 + 1;
         P = nranks;
         if (decomp == DFFT_SLAB_ZY_THEN_X) { P1 = P; P2 = 1; }
         else if (decomp == DFFT_SLAB_Z_THEN_YX) { P1 = P; P2 = 1; }  // P1 only used for the x split

@@ -1,4 +1,5 @@
-// r2r.hpp — per-point arithmetic of the real-to-real pass (fft_r2r_kernel), shared with tests/emu_r2r.cpp.
+// r2r.hpp — per-point arithmetic of the real-to-real passes (fft_r2r_kernel, fft_r2hc_kernel), shared with
+// tests/emu_r2r.cpp and tests/emu_r2hc.cpp.
 //
 // Two real N-point lines a and b are transformed through one complex N-point FFT (CtaFft's stages):
 //   perm:     v[n] = x[2n],  v[N-1-n] = x[2n+1]  (n < N/2);  z = v_a + i v_b
@@ -41,6 +42,33 @@ DFFT_HD cx<T> r2r_build(T ak, T am, T bk, T bm, cx<T> w) {
     const cx<T> wc = cconj(w);
     const cx<T> va = cmul(wc, cx<T>{ak, -am}), vb = cmul(wc, cx<T>{bk, -bm});
     return cx<T>{va.x - vb.y, va.y + vb.x};
+}
+
+// ---- R2HC / HC2R (fft_r2hc_kernel): the same pairing without permutation or w_k ----------------------------------------
+// Halfcomplex line of X = DFT_N(x) (FFTW's R2HC format): hc[k] = Re X[k] for k <= N/2, hc[N-k] = Im X[k] for 0 < k < N/2.
+//   R2HC:  z = a + i b in natural order,  Z = DFT_N(z);  with m = -k mod N, A = (Z[k] + conj Z[m]) / 2 = X_a[k] and
+//          B = (Z[k] - conj Z[m]) / 2i = X_b[k], so hc_a[k] = Re A (k <= N/2) or Im A[m] (k > N/2), and likewise hc_b.
+//   HC2R:  Z[k] = X_a[k] + i X_b[k], the full spectra rebuilt from hc[k] and hc[N-k];  z = unnormalised inverse DFT_N(Z),
+//          a = Re z, b = Im z.
+// Unnormalised like FFTW's R2HC / HC2R: HC2R(R2HC(x)) = N x.
+
+// forward: halfcomplex point k of both lines from Z[k] and Z[-k mod N] (the halving is exact)
+template <typename T>
+DFFT_HD cx<T> r2hc_split(cx<T> zk, cx<T> zm, int k, int N) {
+    if (2 * k <= N) return cx<T>{T(0.5) * (zk.x + zm.x), T(0.5) * (zk.y + zm.y)};
+    return cx<T>{T(0.5) * (zm.y - zk.y), T(0.5) * (zk.x - zm.x)};  // {hc_a[k], hc_b[k]}
+}
+
+// inverse: position in the input line of hc[N-k], the other half of X[k]; -1 when X[k] is real (k = 0 and k = N/2)
+DFFT_HD int r2hc_in_nk(int k, int N) { return k == 0 || 2 * k == N ? -1 : N - k; }
+
+// inverse: Z[k] = X_a[k] + i X_b[k] from hc[k] (ak, bk) and hc[N-k] (am, bm; 0 when X[k] is real)
+template <typename T>
+DFFT_HD cx<T> r2hc_build(T ak, T am, T bk, T bm, int k, int N) {
+    // X[k] = hc[k] + i hc[N-k] for k <= N/2, conj X[N-k] = hc[N-k] - i hc[k] above
+    const bool lo = 2 * k <= N;
+    const cx<T> xa = lo ? cx<T>{ak, am} : cx<T>{am, -ak}, xb = lo ? cx<T>{bk, bm} : cx<T>{bm, -bk};
+    return cx<T>{xa.x - xb.y, xa.y + xb.x};
 }
 
 }  // namespace dfft

@@ -16,7 +16,8 @@ from .params import CommunicationMethod, Configurations, GlobalSize, Partition, 
 
 SLAB_ZY_THEN_X, SLAB_Z_THEN_YX, PENCIL = 0, 1, 2
 F32, F64 = 0, 1
-R2C, C2C, DCT, DST = 0, 1, 2, 3
+R2C, C2C, DCT, DST, R2HC = 0, 1, 2, 3, 4
+_R2R_KINDS = {"dct": DCT, "dst": DST, "r2hc": R2HC}
 FORWARD, INVERSE = -1, 1
 
 
@@ -85,7 +86,8 @@ class Comm:
 class MPIcuFFT:
     """Abstract plan (include/mpicufft.hpp:55-105). `precision`: 'double' | 'float' replaces the C++
     template argument; `transform`: 'r2c' (the reference's), 'c2c', or the real-to-real 'dct' / 'dst' (type II forward, type III
-    inverse, on all three axes; execR2R)."""
+    inverse, on all three axes; execR2R).  A tuple of three names from 'dct', 'dst', 'r2hc', in (x, y, z) order, gives a
+    real-to-real plan with a kind per axis (dfft_plan_create_r2r; 'r2hc': FFTW's R2HC forward, HC2R inverse)."""
 
     _decomp = SLAB_ZY_THEN_X
 
@@ -99,7 +101,15 @@ class MPIcuFFT:
             self.precision = F32
         else:
             raise ValueError(f"precision must be 'double' or 'float', got {precision!r}")
-        if transform in ("r2c", "R2C"):
+        self.kinds = None
+        if isinstance(transform, tuple):
+            if len(transform) != 3 or not all(isinstance(k, str) and k.lower() in _R2R_KINDS for k in transform):
+                raise ValueError(f"a per-axis transform is three of 'dct', 'dst', 'r2hc', got {transform!r}")
+            self.kinds = tuple(_R2R_KINDS[k.lower()] for k in transform)
+            # as the library records it: three DCT (DST) axes are the DCT (DST) plan
+            uniform = len(set(self.kinds)) == 1 and self.kinds[0] != R2HC
+            self.transform = self.kinds[0] if uniform else R2HC
+        elif transform in ("r2c", "R2C"):
             self.transform = R2C
         elif transform in ("c2c", "C2C"):
             self.transform = C2C
@@ -131,7 +141,13 @@ class MPIcuFFT:
         if self._decomp == PENCIL and partition is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         h = C.c_void_p()
-        if inplace:
+        if self.kinds is not None:
+            if batch < 0:
+                raise ValueError("batch must be at least 1")
+            check(lib().dfft_plan_create_r2r(self.comm._h, C.byref(cfg), self._decomp, self.precision, (C.c_int * 3)(*self.kinds),
+                                             global_size.Nx, global_size.Ny, global_size.Nz, p1, p2, batch, 1 if inplace else 0,
+                                             1 if allocate else 0, C.byref(h)))
+        elif inplace:
             if batch < 0:
                 raise ValueError("batch must be at least 1")
             check(lib().dfft_plan_create_inplace(self.comm._h, C.byref(cfg), self._decomp, self.precision, self.transform, global_size.Nx,
@@ -198,8 +214,8 @@ class MPIcuFFT:
         return check(lib().dfft_exec_c2c_partial(self._h, _ptr(out), _ptr(in_), direction, d))
 
     def execR2R(self, out, in_, direction: int = FORWARD, d: int = 3, stream=None):
-        """Real-to-real transform of a 'dct' / 'dst' plan (not in the reference): FORWARD is type II, INVERSE type III, both
-        unnormalised like scipy.fft.dct / dst(norm=None).  Real [x][y][z] buffers.  `stream` as for execR2C, capturable the
+        """Real-to-real transform of a 'dct' / 'dst' or per-axis plan (not in the reference): FORWARD is type II (R2HC on
+        'r2hc' axes), INVERSE type III (HC2R), all unnormalised like scipy.fft.dct / dst(norm=None).  Real [x][y][z] buffers.  `stream` as for execR2C, capturable the
         same way."""
         self._need()
         if stream is not None:
@@ -209,6 +225,13 @@ class MPIcuFFT:
         if d == 3:
             return check(lib().dfft_exec_r2r(self._h, _ptr(out), _ptr(in_), direction))
         return check(lib().dfft_exec_r2r_partial(self._h, _ptr(out), _ptr(in_), direction, d))
+
+    def getR2RKinds(self):
+        """(x, y, z) kinds of a real-to-real plan: DCT, DST or R2HC each (dfft_plan_get_r2r_kinds)."""
+        self._need()
+        k = (C.c_int * 3)()
+        check(lib().dfft_plan_get_r2r_kinds(self._h, k))
+        return tuple(k)
 
     def wait(self):
         return check(lib().dfft_plan_wait(self._h))
@@ -351,8 +374,8 @@ def fft1d_strided(precision: int, direction: int, a: int, n: int, b: int, out, i
 
 
 def fft1d_r2r(precision: int, transform: int, direction: int, n: int, a: int, b: int, out, in_, stream=None):
-    """DCT / DST (transform DCT or DST; FORWARD type II, INVERSE type III) along the middle axis of a dense real [a][n][b]
-    array, b contiguous; out may be in_."""
+    """DCT / DST / R2HC (transform DCT, DST or R2HC; FORWARD type II or R2HC, INVERSE type III or HC2R) along the middle
+    axis of a dense real [a][n][b] array, b contiguous; out may be in_."""
     check(lib().dfft_fft1d_r2r(precision, transform, direction, n, a, b, _ptr(out), _ptr(in_), _stream_ptr(stream)))
 
 

@@ -77,7 +77,7 @@ typedef enum { DFFT_F32 = 0, DFFT_F64 = 1 } dfft_prec; /* cuFFT<float> / cuFFT<d
 /* The reference only offers real<->complex (execR2C/execC2R).  DFFT_C2C plans add the complex
  * transform the benchmark configurations name; the z extent of every complex array is then Nz instead
  * of Nz/2+1. */
-typedef enum { DFFT_R2C = 0, DFFT_C2C = 1, DFFT_DCT = 2, DFFT_DST = 3 } dfft_transform;
+typedef enum { DFFT_R2C = 0, DFFT_C2C = 1, DFFT_DCT = 2, DFFT_DST = 3, DFFT_R2HC = 4 } dfft_transform;
 /* DFFT_DCT / DFFT_DST plans (not in the reference; cuFFT has neither, FFTW calls them REDFT10 / REDFT01 and RODFT10 /
  * RODFT01): real-to-real transforms, the same kind along all three axes, for spectral solvers with Neumann (DCT) or
  * Dirichlet (DST) boundaries.  With N the axis length:
@@ -94,6 +94,13 @@ typedef enum { DFFT_R2C = 0, DFFT_C2C = 1, DFFT_DCT = 2, DFFT_DST = 3 } dfft_tra
  *   - Execs: dfft_exec_r2r*; the R2C / C2R / C2C execs return DFFT_ERR_INVALID on these plans, and dfft_exec_r2r* on
  *     others.
  *   - The sequential schedule always runs, also with send_method Streams (dfft_plan_tune has one candidate). */
+/* DFFT_R2HC (not in the reference; FFTW's R2HC / HC2R): the real DFT of a periodic axis in FFTW's halfcomplex format, a
+ * kind only for dfft_plan_create_r2r and dfft_fft1d_r2r (dfft_plan_create* return DFFT_ERR_INVALID for transform 4).
+ * Forward (R2HC) of N reals x, with X = DFT_N(x) = sum_n x_n exp(-2 pi i k n / N):
+ *   hc = r_0, r_1, ..., r_{N/2}, i_{N/2-1}, ..., i_1    (r_k = Re X_k, i_k = Im X_k; N is even)
+ * i.e. hc[k] = Re X_k for k <= N/2 and hc[N-k] = Im X_k for 0 < k < N/2 (numpy: X = rfft(x),
+ * hc = concatenate([X.real[:N/2+1], X.imag[N/2-1:0:-1]]); scipy.fftpack.rfft interleaves the parts and is another format).
+ * Inverse (HC2R) is the unnormalised inverse: HC2R(R2HC(x)) = N x. */
 
 typedef struct dfft_comm_s* dfft_comm_t;
 typedef struct dfft_plan_s* dfft_plan_t;
@@ -155,6 +162,22 @@ int dfft_plan_create_inplace(dfft_comm_t comm, const dfft_config* config, int de
                              int precision /*dfft_prec*/, int transform /*dfft_transform*/, size_t nx, size_t ny,
                              size_t nz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan);
 int dfft_plan_is_inplace(dfft_plan_t plan); /* 1 for plans of dfft_plan_create_inplace, 0 otherwise (and for a null plan) */
+/* Real-to-real plans with a kind per axis (FFTW's fftw_plan_r2r with one kind per dimension): kinds[0], [1], [2] are the
+ * kinds of the x, y and z axis, each DFFT_DCT (Neumann), DFFT_DST (Dirichlet) or DFFT_R2HC (periodic).  Everything said of
+ * DFFT_DCT / DFFT_DST plans above holds: real [x][y][z] buffers, powers of two in [2, 8192] (others:
+ * DFFT_ERR_UNSUPPORTED), dfft_exec_r2r* (forward: DCT-II, DST-II or R2HC on each axis; inverse: DCT-III, DST-III or
+ * HC2R), partial d over the first d axes in z, y, x order, each with its own kind, and dfft_layout with DFFT_DCT.
+ * `batch` and `inplace` (!= 0) mean what they mean for dfft_plan_create_batched / dfft_plan_create_inplace.
+ *   - A round trip scales by the product over the transformed axes of N (R2HC) or 2N (DCT, DST).
+ *   - Three DFFT_DCT (DFFT_DST) kinds make the DFFT_DCT (DFFT_DST) plan: the same steps, description and output.  Other
+ *     combinations: dfft_plan_describe reports "r2r_kinds" and, per R2R pass, "r2r" (the kind of its axis).
+ *   - A null kinds or a kind outside {DFFT_DCT, DFFT_DST, DFFT_R2HC}: DFFT_ERR_INVALID. */
+int dfft_plan_create_r2r(dfft_comm_t comm, const dfft_config* config, int decomp /*dfft_decomp*/, int precision /*dfft_prec*/,
+                         const int kinds[3], size_t nx, size_t ny, size_t nz, size_t p1, size_t p2, size_t batch, int inplace,
+                         int allocate, dfft_plan_t* plan);
+/* kinds[0..2] of the x, y and z axis of a real-to-real plan (also of DFFT_DCT / DFFT_DST plans); DFFT_ERR_INVALID for
+ * R2C / C2C plans. */
+int dfft_plan_get_r2r_kinds(dfft_plan_t plan, int kinds[3]);
 int dfft_plan_destroy(dfft_plan_t plan);
 /* setWorkArea(device, host) — mpicufft_slab.cpp:236-281. device must hold dfft_get_work_size_device()
  * bytes; with comm_method Peer2Peer and more than one rank it must be the base of a cudaMalloc
@@ -176,7 +199,7 @@ int dfft_exec_c2r(dfft_plan_t plan, void* out, const void* in);
 #define DFFT_FORWARD (-1)
 #define DFFT_INVERSE (1)
 int dfft_exec_c2c(dfft_plan_t plan, void* out, const void* in, int direction);
-/* DFFT_DCT / DFFT_DST plans: direction DFFT_FORWARD runs type II, DFFT_INVERSE type III. */
+/* Real-to-real plans: direction DFFT_FORWARD runs DCT-II / DST-II / R2HC, DFFT_INVERSE DCT-III / DST-III / HC2R. */
 int dfft_exec_r2r(dfft_plan_t plan, void* out, const void* in, int direction);
 /* pencil execR2C(out,in,d)/execC2R(out,in,d): transform only the first d dimensions (z; z,y; z,y,x). */
 int dfft_exec_r2c_partial(dfft_plan_t plan, void* out, const void* in, int d);
@@ -299,8 +322,9 @@ int dfft_fft1d_contig(int precision, int kind, int direction, size_t n, size_t l
 int dfft_fft1d_strided(int precision, int direction, size_t a, size_t n, size_t b, void* out, const void* in,
                        void* stream);
 
-/* DCT / DST (transform DFFT_DCT or DFFT_DST; forward type II, inverse type III, unnormalised) along the middle axis of
- * a dense real [a][n][b] array, b contiguous; n a power of two in [2, 8192].  out == in is allowed. */
+/* DCT / DST / R2HC (transform DFFT_DCT, DFFT_DST or DFFT_R2HC; forward type II or R2HC, inverse type III or HC2R,
+ * unnormalised) along the middle axis of a dense real [a][n][b] array, b contiguous; n a power of two in [2, 8192].
+ * out == in is allowed. */
 int dfft_fft1d_r2r(int precision, int transform, int direction, size_t n, size_t a, size_t b, void* out, const void* in,
                    void* stream);
 

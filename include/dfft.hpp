@@ -76,6 +76,13 @@ public:
         pidx = dfft_comm_rank(comm);
         pcnt = dfft_comm_size(comm);
     }
+    // not in the reference: a real-to-real plan with a kind per axis — kinds_[0..2] of x, y, z, each DFFT_DCT, DFFT_DST or
+    // DFFT_R2HC; initFFT creates it with dfft_plan_create_r2r and execR2R runs it
+    MPIcuFFT(Configurations config_, dfft_comm_t comm_, int max_world_size, const int (&kinds_)[3])
+        : MPIcuFFT(config_, comm_, max_world_size, DFFT_R2HC) {
+        per_axis = true;
+        for (int a = 0; a < 3; ++a) kinds[a] = kinds_[a];
+    }
     virtual ~MPIcuFFT() { if (plan) dfft_plan_destroy(plan); }
 
     virtual void initFFT(GlobalSize* global_size, Partition* partition, bool allocate = true) = 0;
@@ -100,8 +107,9 @@ public:
     void getScale(double& forward_scale, double& inverse_scale) const { DFFT_CALL(dfft_plan_get_scale(plan, &forward_scale, &inverse_scale)); }
     virtual void setWorkArea(void* device = nullptr, void* host = nullptr) { DFFT_CALL(dfft_set_work_area(plan, device, host)); }
     virtual void execR2C(void* out, const void* in) = 0;
-    // not in the reference: real-to-real transform of a plan constructed with transform_ = DFFT_DCT or DFFT_DST (forward
-    // type II, inverse type III, unnormalised); d < 3 transforms only the first d dimensions
+    // not in the reference: real-to-real transform of a plan constructed with transform_ = DFFT_DCT or DFFT_DST, or with
+    // per-axis kinds (forward type II / R2HC, inverse type III / HC2R, unnormalised); d < 3 transforms only the first d
+    // dimensions
     void execR2R(void* out, const void* in, int direction, int d = 3) {
         DFFT_CALL(d == 3 ? dfft_exec_r2r(plan, out, in, direction) : dfft_exec_r2r_partial(plan, out, in, direction, d));
     }
@@ -128,7 +136,10 @@ protected:
         c.benchmark_dir = config.benchmark_dir.empty() ? nullptr : config.benchmark_dir.c_str();
         c.comm_method2 = config.comm_method2; c.send_method2 = config.send_method2;
         if (plan) { dfft_plan_destroy(plan); plan = nullptr; }
-        if (inplace_)
+        if (per_axis)
+            DFFT_CALL(dfft_plan_create_r2r(comm, &c, decomp, dfft_shim::prec<T>::value, kinds, gs->Nx, gs->Ny, gs->Nz, p1, p2, batch_,
+                                           inplace_ ? 1 : 0, allocate ? 1 : 0, &plan));
+        else if (inplace_)
             DFFT_CALL(dfft_plan_create_inplace(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, p1, p2, batch_,
                                                allocate ? 1 : 0, &plan));
         else if (batch_ == 1)
@@ -143,6 +154,8 @@ protected:
     Configurations config;
     dfft_comm_t comm;
     int transform;
+    bool per_axis = false;  // constructed with per-axis kinds
+    int kinds[3] = {0, 0, 0};
     int pidx = 0, pcnt = 1;
     dfft_plan_t plan = nullptr;
     bool initialized = false;
