@@ -20,6 +20,7 @@
 
 #include <sys/stat.h>
 
+#include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <fstream>
@@ -121,6 +122,18 @@ static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftP
     b.chirp = blu ? static_cast<const char*>(blu) + (size_t(1) << log2m) * (prec == DFFT_F64 ? 16 : 8) : nullptr;
     b.scale = scale;
     return launch_bluestein(prec, log2m, kind, b, stream);
+}
+
+// Passes over an axis the plan keeps (dfft_plan_set_transform_axes): the views of the FFT pass they replace, no transform
+static bool is_copy(PassKind kind) { return kind == PASS_COPY_CONTIG || kind == PASS_COPY_TILED; }
+// one copy pass of n-point lines over the views of prm; real: the real elements of R2R plans
+static cudaError_t launch_copy_pass(int prec, bool real, PassKind kind, size_t n, const FftParams& prm, double scale, cudaStream_t stream) {
+    FftCopy c;
+    static_cast<FftParams&>(c) = prm;
+    c.n = int(n);
+    c.ltpl = 0;
+    c.scale = scale;
+    return launch_copy(prec, real, kind, c, stream);
 }
 
 struct Tables {
@@ -281,8 +294,9 @@ struct Step {
     // table `blu`
     size_t n = 0;
     const void* blu = nullptr;
-    bool bluestein() const { return n != 0 && n != (size_t(1) << log2n); }
+    bool bluestein() const { return !is_copy(kind) && n != 0 && n != (size_t(1) << log2n); }
     int r2r = 0;  // PASS_R2R_*: the kind of the axis it transforms (DFFT_DCT, DFFT_DST or DFFT_R2HC)
+    int axis = 0;  // the axis of the pass: 0 x, 1 y, 2 z (PASS_COPY_*: n is its length, log2n 0)
     FftParams prm{};
     int in_user = 0, out_user = 0;  // 1: patch seg[0].base with the caller's in, 2: with the caller's out
     // RENDEZVOUS
@@ -306,6 +320,9 @@ struct Step {
     // its stores are output values of the exec (the fused and batched stages: those of their last phase), so it runs the
     // scaled twin of its kernel when the plan's output scale for the direction is not 1 (dfft_plan_set_scale)
     bool final_store = false;
+    // a copy whose input and output views are the same elements, kept because it stores final values: it only has work to
+    // do when the output scale is not 1, and is not launched otherwise (drop_identity_copies)
+    bool identity = false;
 };
 
 struct Schedule {
@@ -334,6 +351,8 @@ struct dfft_plan_s {
     size_t esize = 16;  // bytes per complex element
     int rank = 0, P = 1;
     int kinds[3] = {0, 0, 0};  // real-to-real plans: the kind of the x, y and z axis
+    int taxes[3] = {1, 1, 1};  // dfft_plan_set_transform_axes: 1 transforms the x, y, z axis, 0 keeps it (copy passes)
+    bool axes_fixed = false;   // a schedule was built or tuned for taxes: the setter refuses from then on
     size_t batch = 1;         // fields per exec, back to back in every caller buffer (dfft_plan_create_batched)
     double scale[2] = {1.0, 1.0};  // [fwd/inv] output scale (dfft_plan_set_scale), applied by the steps marked final_store
     // dfft_plan_create_inplace: every exec has out == in, fields domain_bytes apart, real rows of R2C / C2R padded to Nzc
@@ -467,6 +486,9 @@ static SegN mkseg(void* base, long long sA0, long long sA1, long long sN, size_t
 // Whether every axis is a power of two.  Plans with another length run the sequential schedule only: the overlapped
 // schedules build their passes for power-of-two lengths.
 static bool pow2_axes(const dfft_plan_s* p) { return ilog2_exact(p->g.nx) > 0 && ilog2_exact(p->g.ny) > 0 && ilog2_exact(p->g.nz) > 0; }
+// Whether every axis is transformed.  Plans with a kept axis (dfft_plan_set_transform_axes) run the sequential schedule
+// only: the overlapped schedules, the fused z + y stage and the batched stage transform every axis they touch.
+static bool all_axes(const dfft_plan_s* p) { return p->taxes[0] && p->taxes[1] && p->taxes[2]; }
 
 // Row pitch, in elements (complex units; reals for DCT / DST plans), of the z-contiguous side of the caller's buffers that
 // holds Nz points per row: the input of forward passes, the output of inverse ones.  Real rows of R2C / C2R plans are Nz reals (Nz/2 units) apart, or, in
@@ -481,7 +503,7 @@ static long long z_row_pitch(const dfft_plan_s* p) {
 // three passes are L2-resident already and gain nothing.
 static bool zy_fused(const dfft_plan_s* p, int inverse, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3) return false;
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p)) return false;
     if (g.ny != g.nz || !zy_fused_length(ilog2_exact(g.ny))) return false;
     // the fused stage reads and writes the blocked hand-over layout of the x pass
     if (p->blocked_ch <= 0 || g.nz % size_t(p->blocked_ch) || (inverse && !p->blocked_inv)) return false;
@@ -525,7 +547,7 @@ static int fuse_zy(dfft_plan_s* p, Step zs, const Step& ys, const char* label, c
 constexpr size_t BATCH_SMALL_MIN = 2;
 static bool batch_small(const dfft_plan_s* p, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3) return false;
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p)) return false;
     if (g.nx != g.ny || g.ny != g.nz || !batch_small_length(ilog2_exact(g.nx))) return false;
     return p->batch >= BATCH_SMALL_MIN && p->batch * g.nx <= 0x7fffffff;
 }
@@ -585,6 +607,16 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         s = Step();
         s.type = STEP_PASS;
         s.label = (kind == PASS_C2C_TILED) ? "strided pass" : (kind == PASS_R2C ? "z pass (R2C)" : (kind == PASS_C2R ? "z pass (C2R)" : "z pass"));
+        s.axis = axis;
+        if (!p->taxes[axis]) {
+            // a kept axis: this pass's views, moved by the copy kernel without tables (labels: name_copies)
+            s.kind = kind == PASS_C2C_TILED ? PASS_COPY_TILED : PASS_COPY_CONTIG;
+            s.phase = phase;
+            s.n = n;
+            s.prm.A0 = 1; s.prm.A1 = 1; s.prm.B = 1;
+            s.prm.inverse = inverse;
+            return DFFT_SUCCESS;
+        }
         if (r2r) {
             kind = kind == PASS_C2C_TILED ? PASS_R2R_TILED : PASS_R2R_CONTIG;
             s.r2r = p->kinds[axis];
@@ -911,10 +943,13 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         if (rc) return rc;
         sy_.label = "y pass";
         const int W = dir1 ? D2 : SR;  // a local scratch slot that is not the transposition target
+        // one rank with x kept: the y pass leaves [nx][ny][nzc] in D1, where the z pass reads it, and no x copy runs (the
+        // other decompositions run their d = 2 steps instead, get_schedule)
+        const bool no_x = P == 1 && !p->taxes[0];
         sy_.prm.A0 = int(g.nx); sy_.prm.B = int(nz_j);
         sy_.prm.in = single_view(nullptr, (long long)(g.ny * nz_j), 0, (long long)nz_j);
         sy_.in_user = 1;
-        sy_.prm.out = single_view(slotp(W, me), (long long)(g.ny * nz_j), 0, (long long)nz_j);
+        sy_.prm.out = single_view(slotp(no_x ? D1 : W, me), (long long)(g.ny * nz_j), 0, (long long)nz_j);
         sc.steps.push_back(sy_);
         Step sx_;
         rc = new_pass(PASS_C2C_TILED, g.nx, 0, "2D FFT Y-X-Direction", sx_);
@@ -933,7 +968,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
                 return mkseg(eptr(slotp(SS, me), xa.soff[q], es), 0, (long long)nz_j, (long long)(g.ny * nz_j), g.sx.start[q]);
             });
         }
-        sc.steps.push_back(sx_);
+        if (!no_x) sc.steps.push_back(sx_);
         if (!dir1) { xa.phase = "Transpose (Finished All2All)"; xa.group = 1; sc.steps.push_back(xa); }
         else if (G1.size() > 1) rendezvous(1, 1, "Transpose (Finished Receive)");
         Step sz_;
@@ -2027,7 +2062,9 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
             for (int w : s.waits) CK_CUDA(cudaStreamWaitEvent(ss, p->sync_events[w], 0));
             CK_CUDA(tl_mark(ss, s.label, s.stream));
             const char* phase = last ? s.phase : nullptr;
-            if (s.type == STEP_PASS) {
+            if (s.type == STEP_PASS && s.identity && p->scale[sc.inverse] == 1.0) {
+                CK_CUDA(mark(phase, 1, s.label));  // an in-place copy onto itself with nothing to scale: no launch
+            } else if (s.type == STEP_PASS) {
                 FftParams prm = s.prm;
                 const double scale = s.final_store ? p->scale[sc.inverse] : 1.0;
                 // views on the caller's buffers store a byte offset in seg[0].base (field f starts f field sizes further);
@@ -2044,7 +2081,8 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
                 cudaError_t e = cudaErrorInvalidValue;
                 switch (s.kernel) {
                     case KERNEL_PASS:
-                        e = launch_fft_pass(p->prec, s.kind, s.n ? s.n : size_t(1) << s.log2n, prm, s.blu, scale, ss, s.r2r);
+                        e = is_copy(s.kind) ? launch_copy_pass(p->prec, is_r2r(p->g.transform), s.kind, s.n, prm, scale, ss)
+                                            : launch_fft_pass(p->prec, s.kind, s.n ? s.n : size_t(1) << s.log2n, prm, s.blu, scale, ss, s.r2r);
                         break;
                     case KERNEL_ZY_FUSED: e = launch_zy_fused(p->prec, s.log2n, prm, prm_y, s.zyf, scale, ss); break;
                     case KERNEL_BATCH_SMALL:
@@ -2133,29 +2171,131 @@ static void relocate_buffer_views(const dfft_plan_s* p, Schedule& sc) {
     }
 }
 
+// ---- kept axes (DESIGN.md section 3.12) ------------------------------------------------------------------------------
+// The builders label passes by their role ("y pass", "x pass (tail)"); copy passes are named after their axis instead.
+static void name_copies(Schedule& sc) {
+    static const char* const names[3][2] = {{"x copy", "x copy (tail)"}, {"y copy", "y copy (tail)"}, {"z copy", "z copy (tail)"}};
+    for (Step& s : sc.steps)
+        if (s.type == STEP_PASS && is_copy(s.kind)) s.label = names[s.axis][std::strstr(s.label, "(tail)") ? 1 : 0];
+}
+
+// A kept z whose copy is local and keeps element order — both views one segment with the same strides, the input the
+// caller's `in` (forward) or the output the caller's `out` (inverse), the other side a slot of this rank — is dropped
+// whenever another pass follows it (forward) or precedes it (inverse).  Forward: the passes that read the slot region it
+// fills read the caller's `in` at the same offsets instead, up to the first pass that writes into that region.  Inverse:
+// the passes that fill the region it reads write the caller's `out` instead (out_user 2, so the output scale lands on
+// them).  This holds for slab ZY_Then_X on any rank count and for every decomposition on one rank; elsewhere the z pass
+// scatters across ranks.  A single z copy (d = 1) stays: it is the exec.
+static void drop_z_copy(const dfft_plan_s* p, Schedule& sc, int inverse) {
+    if (p->taxes[2]) return;
+    std::vector<size_t> passes;
+    for (size_t k = 0; k < sc.steps.size(); ++k)
+        if (sc.steps[k].type == STEP_PASS) passes.push_back(k);
+    if (passes.size() < 2) return;
+    const size_t iz = inverse ? passes.back() : passes.front();
+    const Step z = sc.steps[iz];
+    if (!is_copy(z.kind) || z.axis != 2 || z.prm.in.nseg != 1 || z.prm.out.nseg != 1) return;
+    const Seg &a = z.prm.in.seg[0], &b = z.prm.out.seg[0];
+    if (a.sA0 != b.sA0 || a.sA1 != b.sA1 || z.prm.in.sN != z.prm.out.sN) return;
+    if (inverse ? (z.in_user != 0 || z.out_user != 2) : (z.in_user != 1 || z.out_user != 0)) return;
+    // the slot region the copy fills (forward) or drains (inverse), and the shift that takes it to the caller's buffer
+    const View& sv = inverse ? z.prm.in : z.prm.out;
+    const long long A0 = std::max(z.prm.A0, 1), A1 = std::max(z.prm.A1, 1);
+    const long long last = (A0 - 1) * sv.seg[0].sA0 + (A1 - 1) * sv.seg[0].sA1 + (long long)(z.n - 1) * sv.sN;
+    const char* lo = static_cast<const char*>(sv.seg[0].base);
+    const char* hi = lo + size_t(last + 1) * p->esize;
+    const long long shift = static_cast<const char*>(inverse ? b.base : a.base) - lo;
+    auto inside = [&](const View& v, int user) {
+        const char* base = static_cast<const char*>(v.seg[0].base);
+        return user == 0 && v.nseg == 1 && base >= lo && base < hi;
+    };
+    auto move = [&](View& v) { v.seg[0].base = const_cast<char*>(static_cast<const char*>(v.seg[0].base)) + shift; };
+    // local: the pass next to it (no rendezvous or all-to-all between them) reads (forward) or fills (inverse) the region —
+    // with a rendezvous between them, peers deliver into the region (the Z_Then_YX inverse) and it must stay
+    const Step& nb = sc.steps[inverse ? iz - 1 : iz + 1];
+    if (nb.type != STEP_PASS || !(inverse ? inside(nb.prm.out, nb.out_user) : inside(nb.prm.in, nb.in_user))) return;
+    if (!inverse) {
+        for (size_t k = iz + 1; k < sc.steps.size(); ++k) {
+            Step& s = sc.steps[k];
+            if (s.type != STEP_PASS) continue;
+            const bool overwrites = inside(s.prm.out, s.out_user);
+            if (inside(s.prm.in, s.in_user)) { move(s.prm.in); s.in_user = 1; }
+            if (overwrites) break;
+        }
+    } else {
+        for (size_t k = iz; k-- > 0;) {
+            Step& s = sc.steps[k];
+            if (s.type != STEP_PASS) continue;
+            if (inside(s.prm.in, s.in_user)) break;
+            if (inside(s.prm.out, s.out_user)) { move(s.prm.out); s.out_user = 2; }
+        }
+    }
+    sc.steps.erase(sc.steps.begin() + long(iz));
+    // the inverse's last timer section moves to the pass that now ends the exec
+    if (inverse && z.phase && !sc.steps[iz - 1].phase) sc.steps[iz - 1].phase = z.phase;
+}
+
+// the same elements of the same buffer (in place, the caller's `in` and `out` are one buffer)
+static bool same_view(const View& a, int ua, const View& b, int ub, bool inplace) {
+    auto buf = [&](int u) { return u == 0 ? 0 : inplace ? 1 : u; };
+    if (buf(ua) != buf(ub) || a.nseg != b.nseg || a.sN != b.sN || (a.nseg > 1 && a.seg_of_n != b.seg_of_n)) return false;
+    for (int i = 0; i < a.nseg; ++i)
+        if (a.seg[i].base != b.seg[i].base || a.seg[i].sA0 != b.seg[i].sA0 || a.seg[i].sA1 != b.seg[i].sA1 || a.seg[i].n0 != b.seg[i].n0)
+            return false;
+    return true;
+}
+
+// A copy whose input and output views are identical moves nothing (the in-place y pass of Z_Then_YX, the in-place z
+// pass of one rank) and is not emitted — unless it stores final values, where the output scale still has to be applied
+// (in-place execs that end in a kept axis on the caller's buffer, e.g. d = 1 with z kept).
+static void drop_identity_copies(const dfft_plan_s* p, Schedule& sc) {
+    for (size_t k = 0; k < sc.steps.size();) {
+        Step& s = sc.steps[k];
+        if (s.type == STEP_PASS && is_copy(s.kind) && same_view(s.prm.in, s.in_user, s.prm.out, s.out_user, p->inplace)) {
+            // the scale may change after the schedule is built: a final store stays in the list and run_schedule skips it
+            // while the scale is 1
+            if (s.final_store) {
+                s.identity = true;
+            } else {
+                if (s.phase && k > 0 && !sc.steps[k - 1].phase) sc.steps[k - 1].phase = s.phase;
+                sc.steps.erase(sc.steps.begin() + long(k));
+                continue;
+            }
+        }
+        ++k;
+    }
+}
+
 // The one place that decides which schedule a (direction, d) pair runs — used by exec and by dfft_plan_describe, so
 // the CPU schedule emulation always validates exactly what executes.
 static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
     Schedule& sc = p->sched[inverse ? 1 : 0][d - 1];
+    p->axes_fixed = true;
     if (!sc.built) {
         g_view_error = false;
         const bool streams = p->cfg.send_method == DFFT_SEND_STREAMS || (p->g.decomp == DFFT_PENCIL && p->cfg.send_method2 == DFFT_SEND_STREAMS);
         const bool seq_won = p->tuned_seq[inverse ? 1 : 0] != 0;
         const bool want_overlap = streams && d == 3 && p->P > 1 && p->g.decomp == DFFT_SLAB_ZY_THEN_X && p->direct2 && p->xchg_ctas >= 0 && !seq_won &&
-                                  pow2_axes(p) && !is_r2r(p->g.transform);
+                                  pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p);
         // pencil: forward on a grid with two real transpositions by default; every other
         // combination (inverse, p1 or p2 == 1) only once dfft_plan_tune has measured it faster than the sequential schedule
         const bool both_multi = p->grp[1].size() > 1 && p->grp[2].size() > 1;
         const bool tuned = p->tuned_ctas[inverse ? 1 : 0] != -2;
         const bool want_pencil_overlap = streams && d == 3 && p->g.decomp == DFFT_PENCIL && p->direct1 && p->direct2 && p->P > 1 && p->xchg_ctas >= 0 &&
                                          pencil_overlap_enabled() && !seq_won && ((both_multi && !inverse) || tuned || pencil_overlap_mode() == 2) &&
-                                         pow2_axes(p) && !is_r2r(p->g.transform);
+                                         pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p);
+        // one rank with x kept: the layout after d = 2 is the output layout, so d = 3 runs the d = 2 steps (no x copy)
+        const int db = p->P == 1 && !p->taxes[0] && d == 3 ? 2 : d;
         int rc;
         if (batch_small(p, d)) rc = build_batch_small(p, inverse ? 1 : 0, sc);
         else if (want_overlap) rc = build_overlapped_slab(p, inverse ? 1 : 0, sc);
         else if (want_pencil_overlap) rc = build_overlapped_pencil(p, inverse ? 1 : 0, sc);
-        else rc = build_schedule(p, inverse ? 1 : 0, d, sc);
+        else rc = build_schedule(p, inverse ? 1 : 0, db, sc);
         if (rc) return rc;
+        if (!all_axes(p)) {
+            name_copies(sc);
+            drop_z_copy(p, sc, inverse ? 1 : 0);
+        }
         // No step reads the caller's `out` (views on it are only ever stored to), so every store into it is an output
         // value of the exec: the steps that write `out` are exactly the ones that store final values.  This covers the tail
         // launches of blocked hand-over layouts, every z chunk of overlapped x passes, the last pass of partial transforms
@@ -2165,6 +2305,7 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
         // In place the buffer also holds intermediates: its views from slot D1 are marked after the final stores.
         // tests/test_inplace.py replays these schedules on one address range.
         if (p->buf_slot) relocate_buffer_views(p, sc);
+        if (!all_axes(p)) drop_identity_copies(p, sc);
         sc.inverse = inverse ? 1 : 0;
         field_bytes(p, inverse, d, &sc.field_in, &sc.field_out);
         if (g_view_error) return fail(DFFT_ERR_STATE, "internal: segments of one view disagree on the axis stride");
@@ -2755,6 +2896,21 @@ int dfft_plan_set_scale(dfft_plan_t p, double forward_scale, double inverse_scal
         for (Schedule& sc : dir) sc.executed = false;
     return DFFT_SUCCESS;
 }
+int dfft_plan_set_transform_axes(dfft_plan_t p, const int transform[3]) {
+    if (!p || !transform) return fail(DFFT_ERR_INVALID, "null plan / transform");
+    for (int a = 0; a < 3; ++a)
+        if (transform[a] != 0 && transform[a] != 1) return fail(DFFT_ERR_INVALID, "transform axes must be 0 (keep) or 1 (transform)");
+    if (p->g.transform == DFFT_R2C && !transform[2]) return fail(DFFT_ERR_INVALID, "R2C / C2R plans transform z (it turns reals into complex)");
+    // schedules, tuned choices and captured graphs are built for the axes of their time
+    if (p->axes_fixed) return fail(DFFT_ERR_STATE, "set the transform axes before the first exec, dfft_plan_tune or dfft_plan_describe");
+    for (int a = 0; a < 3; ++a) p->taxes[a] = transform[a];
+    return DFFT_SUCCESS;
+}
+int dfft_plan_get_transform_axes(dfft_plan_t p, int transform[3]) {
+    if (!p || !transform) return fail(DFFT_ERR_INVALID, "null plan / transform");
+    for (int a = 0; a < 3; ++a) transform[a] = p->taxes[a];
+    return DFFT_SUCCESS;
+}
 int dfft_plan_get_scale(dfft_plan_t p, double* forward_scale, double* inverse_scale) {
     if (!p) return fail(DFFT_ERR_INVALID, "null plan");
     if (forward_scale) *forward_scale = p->scale[0];
@@ -2853,6 +3009,7 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
     if (!p->work || !out || !in) return fail(DFFT_ERR_INVALID, "plan needs its work area and both buffers");
     if (p->inplace && out != in) return fail(DFFT_ERR_INVALID, "in-place plan: out must equal in");
     CK_CUDA(cudaSetDevice(p->comm->device));
+    p->axes_fixed = true;
     const int dir = inverse ? 1 : 0;
     if (reps < 1) reps = 3;
     int sms = 0;
@@ -2863,7 +3020,7 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
     std::vector<Cand> cands;
     cands.push_back({1, 0, 0, 0});
     const bool streams = p->cfg.send_method == DFFT_SEND_STREAMS || (p->g.decomp == DFFT_PENCIL && p->cfg.send_method2 == DFFT_SEND_STREAMS);
-    const bool has_overlap = streams && p->P > 1 && p->xchg_ctas >= 0 && pow2_axes(p) && !is_r2r(p->g.transform) &&
+    const bool has_overlap = streams && p->P > 1 && p->xchg_ctas >= 0 && pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p) &&
                              ((p->g.decomp == DFFT_SLAB_ZY_THEN_X && p->direct2) ||
                               (p->g.decomp == DFFT_PENCIL && p->direct1 && p->direct2 && pencil_overlap_enabled()));
     const bool pencil_inv = inverse && p->g.decomp == DFFT_PENCIL;
@@ -2885,6 +3042,7 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
     p->tune_report.clear();
     if (cands.size() == 1) {
         p->tune_report = is_r2r(p->g.transform) ? "sequential schedule (no alternatives for this plan: DCT / DST plans run the sequential schedule)"
+                         : !all_axes(p)         ? "sequential schedule (no alternatives for this plan: plans with a kept axis run the sequential schedule)"
                          : pow2_axes(p)         ? "sequential schedule (no alternatives for this plan)"
                                                 : "sequential schedule (no alternatives for this plan: an axis length is not a power of two)";
         return 0;
@@ -3006,6 +3164,9 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
                     (per_axis ? std::string(",\"r2r_kinds\":[\"") + r2r_name(p->kinds[0]) + "\",\"" + r2r_name(p->kinds[1]) + "\",\"" +
                                     r2r_name(p->kinds[2]) + "\"]"
                               : std::string()) +
+                    (all_axes(p) ? std::string()
+                                 : ",\"transform_axes\":[" + std::to_string(p->taxes[0]) + "," + std::to_string(p->taxes[1]) + "," +
+                                       std::to_string(p->taxes[2]) + "]") +
                     (p->batch > 1 ? ",\"batch\":" + std::to_string(p->batch) + ",\"field_in\":" + std::to_string(sc.field_in) +
                                         ",\"field_out\":" + std::to_string(sc.field_out)
                                   : std::string()) +
@@ -3110,9 +3271,12 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
         for (size_t w = 0; w < s_.waits.size(); ++w) o += (w ? "," : "") + std::to_string(s_.waits[w]);
         o += "]";
         if (s_.type == STEP_PASS) {
-            o += ",\"kind\":" + std::to_string(int(s_.kind)) + (per_axis ? std::string(",\"r2r\":\"") + r2r_name(s_.r2r) + "\"" : std::string()) +
+            // copy passes (kinds 6 / 7): "n" is the length of the kept axis, "log2n" 0, no "r2r"
+            const bool copy = is_copy(s_.kind);
+            o += ",\"kind\":" + std::to_string(int(s_.kind)) +
+                 (per_axis && !copy ? std::string(",\"r2r\":\"") + r2r_name(s_.r2r) + "\"" : std::string()) +
                  ",\"log2n\":" + std::to_string(s_.log2n) +
-                 (s_.bluestein() ? ",\"n\":" + std::to_string(s_.n) : std::string()) + ",\"A0\":" + std::to_string(s_.prm.A0) +
+                 (s_.bluestein() || copy ? ",\"n\":" + std::to_string(s_.n) : std::string()) + ",\"A0\":" + std::to_string(s_.prm.A0) +
                  ",\"A1\":" + std::to_string(s_.prm.A1) + ",\"B\":" + std::to_string(s_.prm.B) + ",\"inverse\":" + std::to_string(s_.prm.inverse) +
                  ",\"in_user\":" + std::to_string(s_.in_user) + ",\"out_user\":" + std::to_string(s_.out_user) + ",\"in\":";
             json_view(o, s_.prm.in, p->tabs);

@@ -270,6 +270,37 @@ cudaError_t launch_r2r(PassKind kind, const FftR2r& p, bool hc, cudaStream_t str
 
 template cudaError_t launch_r2r<DFFT_T, DFFT_LOG2N>(PassKind, const FftR2r&, bool, cudaStream_t);
 
+#if DFFT_LOG2N == 1
+// CONTIG: lines of up to COPY_THREADS threads (the power of two >= n), COPY_THREADS / that many lines per CTA; TILED: rows
+// as wide as the power of two >= B, up to 32 elements (a 512-byte row of cx<double>), the CTA's other threads on further n
+template <typename E>
+cudaError_t launch_copy(PassKind kind, const FftCopy& p_in, cudaStream_t stream) {
+    FftCopy p = p_in;
+    const long long lines = (long long)p.A0 * p.A1;
+    if (lines <= 0 || p.n <= 0) return cudaSuccess;
+    const bool tiled = kind == PASS_COPY_TILED;
+    if (!tiled && kind != PASS_COPY_CONTIG) return cudaErrorInvalidValue;
+    if (tiled && p.B <= 0) return cudaSuccess;
+    // TILED: G x G blocks of (a0, a1) tiles, the largest G <= 2^DFFT_COPY_SWZ that divides both extents
+    p.tile_swz = 0;
+    if (tiled) {
+        p.tile_swz = env_int("DFFT_COPY_SWZ", COPY_SWZ);
+        while (p.tile_swz > 0 && (p.A0 % (1 << p.tile_swz) || p.A1 % (1 << p.tile_swz))) --p.tile_swz;
+    }
+    const int span = tiled ? (p.B < 32 ? p.B : 32) : (p.n < COPY_THREADS ? p.n : COPY_THREADS);
+    p.ltpl = 0;
+    while ((1 << p.ltpl) < span) ++p.ltpl;
+    const long long grid = tiled ? lines * ((p.B + (1 << p.ltpl) - 1) >> p.ltpl) : (lines + (COPY_THREADS >> p.ltpl) - 1) / (COPY_THREADS >> p.ltpl);
+    if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+    if (tiled) fft_copy_kernel<E, true><<<unsigned(grid), COPY_THREADS, 0, stream>>>(p);
+    else fft_copy_kernel<E, false><<<unsigned(grid), COPY_THREADS, 0, stream>>>(p);
+    return cudaGetLastError();
+}
+
+template cudaError_t launch_copy<DFFT_T>(PassKind, const FftCopy&, cudaStream_t);
+template cudaError_t launch_copy<cx<DFFT_T>>(PassKind, const FftCopy&, cudaStream_t);
+#endif
+
 #if DFFT_LOG2N == 8 || DFFT_LOG2N == 9
 static bool aligned128(const void* base, long long elems_a, long long elems_b, long long elems_c) {
     constexpr long long es = sizeof(cx<DFFT_T>);

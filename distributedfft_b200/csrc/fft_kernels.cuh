@@ -77,8 +77,12 @@ struct FftScaled : FftParams {
 template <bool SCALED>
 using KParams = std::conditional_t<SCALED, FftScaled, FftParams>;
 
-// PASS_R2R_*: the view mapping of PASS_C2C_* over real elements (fft_r2r_kernel)
-enum PassKind { PASS_C2C_CONTIG = 0, PASS_C2C_TILED = 1, PASS_R2C = 2, PASS_C2R = 3, PASS_R2R_CONTIG = 4, PASS_R2R_TILED = 5 };
+// PASS_R2R_*: the view mapping of PASS_C2C_* over real elements (fft_r2r_kernel).  PASS_COPY_*: the views of a C2C or R2R
+// pass over an axis the plan keeps, moved without a transform (fft_copy_kernel)
+enum PassKind {
+    PASS_C2C_CONTIG = 0, PASS_C2C_TILED = 1, PASS_R2C = 2, PASS_C2R = 3, PASS_R2R_CONTIG = 4, PASS_R2R_TILED = 5,
+    PASS_COPY_CONTIG = 6, PASS_COPY_TILED = 7
+};
 
 // ---- tile shape choices (compile time) -----------------------------------------------------------
 template <typename T, int LOG2N>
@@ -251,12 +255,9 @@ struct CtaFft {
     }
 };
 
-// linear tile number -> (b tile, a1, a0) of a TILED pass
-template <int TB>
-__device__ __forceinline__ void tiled_decode(const FftParams& p, long long tile, int& bt, int& a1, int& a0) {
-    const int nbt = (p.B + TB - 1) / TB;
-    bt = int(tile % nbt);
-    const int a = int(tile / nbt);
+// linear (a0, a1) tile number -> (a1, a0): plain order (a1 fastest), or G x G blocks of (a0, a1) numbered consecutively
+// when p.tile_swz = log2 G > 0
+__device__ __forceinline__ void tile_order(const FftParams& p, int a, int& a1, int& a0) {
     if (p.tile_swz > 0) {
         const int lg = p.tile_swz, G = 1 << lg;
         const int lo = a & (G * G - 1), hi = a >> (2 * lg);
@@ -267,6 +268,14 @@ __device__ __forceinline__ void tiled_decode(const FftParams& p, long long tile,
         a1 = a % p.A1;
         a0 = a / p.A1;
     }
+}
+
+// linear tile number -> (b tile, a1, a0) of a TILED pass
+template <int TB>
+__device__ __forceinline__ void tiled_decode(const FftParams& p, long long tile, int& bt, int& a1, int& a0) {
+    const int nbt = (p.B + TB - 1) / TB;
+    bt = int(tile % nbt);
+    tile_order(p, int(tile / nbt), a1, a0);
 }
 
 // common prologue: thread -> (j, t), tile -> (a0, a1, b), segment tables
@@ -1394,6 +1403,107 @@ fft_r2hc_kernel(const __grid_constant__ FftR2r p) {
     r2r_pass<T, LOG2N, LOG2E, TB, TILED, INV, true>(p);
 }
 
+// ---- copy pass: an axis the plan keeps (dfft_plan_set_transform_axes) ------------------------------------------------
+// Moves element (a0, a1, n, b) of p.in to the same index of p.out for any line length p.n, through the segmented views of
+// the FFT pass it replaces (scatters into peer slots, gathers from receive slots, blocked layouts and tails unchanged).
+//   CONTIG: a CTA holds `lpc` lines of `tpl` threads each (tpl = 2^ltpl), threads run along n: coalesced over n.
+//   TILED:  a CTA holds one (a0, a1) and `tpl` consecutive b (tpl = 2^ltpl), its rows blockDim / tpl apart along n:
+//           threads run along the contiguous b, so every row is one coalesced run.  The (a0, a1) tiles run in G x G
+//           blocks (p.tile_swz = log2 G, tile_order), so that CTAs running at the same time read and write neighbouring
+//           rows on both sides when a0 is near on one side and a1 on the other (the blocked hand-over layouts).
+// Each thread loads COPY_ILP elements before it stores them; an element is read by the same thread that writes it, before
+// it writes it.  A scale != 1 multiplies each real value with __dmul_rn / __fmul_rn, so a scaled copy is the unscaled
+// one times s, bit for bit.  E: float, double (the real views of R2R plans), cx<float> or cx<double>.
+struct FftCopy : FftParams {
+    int n;         // line length
+    int ltpl;      // log2 of the threads per line (CONTIG) or per row (TILED)
+    double scale;  // output scale, applied when != 1 (rounded to the element's precision once)
+};
+constexpr int COPY_THREADS = 512;
+// elements in flight per thread (experiment knob -DDFFT_COPY_ILP=<n>)
+#ifndef DFFT_COPY_ILP
+#define DFFT_COPY_ILP 8
+#endif
+constexpr int COPY_ILP = DFFT_COPY_ILP;
+constexpr int COPY_SWZ = 1;  // log2 G of the TILED tile blocking (DFFT_COPY_SWZ overrides it per launch, 0 = plain order)
+
+template <typename E>
+struct CopyElem {
+    using R = E;
+    static __device__ __forceinline__ E ld(const E* p) { return *p; }
+    static __device__ __forceinline__ void st(E* p, E v) { *p = v; }
+    static __device__ __forceinline__ E mul(E v, R s) { return rscale<R>(v, s); }
+};
+template <typename T>
+struct CopyElem<cx<T>> {
+    using R = T;
+    static __device__ __forceinline__ cx<T> ld(const cx<T>* p) { return ld_elem<T>(p); }
+    static __device__ __forceinline__ void st(cx<T>* p, cx<T> v) { st_elem<T>(p, v); }
+    static __device__ __forceinline__ cx<T> mul(cx<T> v, T s) { return cx<T>{rscale<T>(v.x, s), rscale<T>(v.y, s)}; }
+};
+
+// element (a0, a1, n, b) of a view: p0 + n sN for a single-segment view (p0: element n = 0 of the line), through the
+// segment of n otherwise
+template <typename E>
+struct CopyLine {
+    E* p0;
+    long long sN;
+    bool multi;
+    __device__ __forceinline__ CopyLine(const View& v, int a0, int a1, int b) {
+        const Seg& g = v.seg[0];
+        p0 = reinterpret_cast<E*>(g.base) + (a0 * g.sA0 + a1 * g.sA1 - (long long)g.n0 * v.sN + b);
+        sN = v.sN;
+        multi = v.nseg > 1;
+    }
+    __device__ __forceinline__ E* at(const View& v, int a0, int a1, int n, int b) const {
+        if (!multi) return p0 + n * sN;
+        const Seg& g = v.seg[v.seg_of_n[n]];
+        return reinterpret_cast<E*>(g.base) + (a0 * g.sA0 + a1 * g.sA1 + (long long)(n - g.n0) * sN + b);
+    }
+};
+
+template <typename E, bool TILED>
+__global__ void __launch_bounds__(COPY_THREADS) fft_copy_kernel(const __grid_constant__ FftCopy p) {
+    using CE = CopyElem<E>;
+    const int tid = threadIdx.x, tpl = 1 << p.ltpl;
+    int a0, a1, b, j, step;
+    bool valid;
+    if constexpr (TILED) {
+        const int nbt = (p.B + tpl - 1) >> p.ltpl;
+        const int bt = int(blockIdx.x % unsigned(nbt));
+        tile_order(p, int(blockIdx.x / unsigned(nbt)), a1, a0);
+        b = (bt << p.ltpl) + (tid & (tpl - 1));
+        j = tid >> p.ltpl;
+        step = COPY_THREADS >> p.ltpl;
+        valid = b < p.B;
+    } else {
+        const long long line = (long long)blockIdx.x * (COPY_THREADS >> p.ltpl) + (tid >> p.ltpl);
+        a1 = int(line % p.A1);
+        a0 = int(line / p.A1);
+        b = 0;
+        j = tid & (tpl - 1);
+        step = tpl;
+        valid = line < (long long)p.A0 * p.A1;
+    }
+    if (!valid) return;
+    const bool scaled = p.scale != 1.0;
+    const typename CE::R s = typename CE::R(p.scale);
+    const CopyLine<E> in(p.in, a0, a1, b), out(p.out, a0, a1, b);
+    for (int n0 = j; n0 < p.n; n0 += COPY_ILP * step) {
+        E v[COPY_ILP];
+#pragma unroll
+        for (int u = 0; u < COPY_ILP; ++u) {
+            const int n = n0 + u * step;
+            if (n < p.n) v[u] = CE::ld(in.at(p.in, a0, a1, n, b));
+        }
+#pragma unroll
+        for (int u = 0; u < COPY_ILP; ++u) {
+            const int n = n0 + u * step;
+            if (n < p.n) CE::st(out.at(p.out, a0, a1, n, b), scaled ? CE::mul(v[u], s) : v[u]);
+        }
+    }
+}
+
 // ---- host launchers (one explicit instantiation per precision and size, see fft_inst.cu) ----------------
 // scale: the output scale of the pass' stores; 1 launches the unscaled kernels, anything else their scaled twins.
 template <typename T, int LOG2N>
@@ -1433,6 +1543,13 @@ cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluest
 template <typename T, int LOG2N>
 cudaError_t launch_r2r(PassKind kind, const FftR2r& p, bool hc, cudaStream_t stream);
 cudaError_t launch_r2r(int prec, int log2n, PassKind kind, const FftR2r& p, bool hc, cudaStream_t stream);
+
+// copy pass of p.n-point lines (fft_copy_kernel): kind PASS_COPY_CONTIG or PASS_COPY_TILED, p.ltpl is filled in here.
+// Instantiated for E = T and cx<T> in the LOG2N = 1 unit of each precision; the runtime form takes real != 0 for the
+// real elements of R2R plans.
+template <typename E>
+cudaError_t launch_copy(PassKind kind, const FftCopy& p, cudaStream_t stream);
+cudaError_t launch_copy(int prec, bool real, PassKind kind, const FftCopy& p, cudaStream_t stream);
 
 constexpr int MAX_LOG2N = 13;
 constexpr int BLUESTEIN_MAX_N = 4096;  // 2n - 1 <= 2^MAX_LOG2N

@@ -124,12 +124,13 @@ class MPIcuFFT:
 
     # -- plan ------------------------------------------------------------------------------------
     def initFFT(self, global_size: GlobalSize, partition: Optional[Partition] = None, allocate: bool = True, batch: int = 1,
-                inplace: bool = False):
+                inplace: bool = False, transform_axes: Optional[Sequence[bool]] = None):
         """`batch` (not in the reference): every exec transforms that many fields, back to back in each buffer — a
         contiguous [batch, X, Y, Z] tensor; the getters describe one field (dfft_plan_create_batched).
         `inplace` (dfft_plan_create_inplace): every exec gets the same buffer twice and overwrites its input; fields are
         getDomainSize() bytes apart.  R2C / C2R use padded real rows: with buf a complex [X, Y, Nz/2+1] tensor, pass
-        torch.view_as_real(buf).view(X, Y, Nz + 2) as the real side."""
+        torch.view_as_real(buf).view(X, Y, Nz + 2) as the real side.
+        `transform_axes` (x, y, z): setTransformAxes right after creation, e.g. (False, True, True) keeps x."""
         if global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         cfg = _lib.dfft_config(int(self.config.cuda_aware), int(self.config.warmup_rounds), int(self.config.comm_method),
@@ -163,6 +164,28 @@ class MPIcuFFT:
         self._h = h
         self.global_size = global_size
         self.initialized = True
+        if transform_axes is not None:
+            try:
+                self.setTransformAxes(*transform_axes)
+            except Exception:
+                self.destroy()
+                self.initialized = False
+                raise
+
+    def setTransformAxes(self, x: bool = True, y: bool = True, z: bool = True):
+        """Transform (True) or keep (False) each axis (dfft_plan_set_transform_axes).  A kept axis is redistributed as a
+        transformed one would be but its values are not transformed: (False, True, True) transforms z and y and returns
+        x whole on every rank, in the output layout, for a solve along x.  Only before the first exec, tune or describe;
+        local to this rank (set the same values on every rank).  R2C plans must transform z."""
+        self._need()
+        check(lib().dfft_plan_set_transform_axes(self._h, (C.c_int * 3)(int(bool(x)), int(bool(y)), int(bool(z)))))
+
+    def getTransformAxes(self):
+        """(x, y, z): True where the axis is transformed."""
+        self._need()
+        t = (C.c_int * 3)()
+        check(lib().dfft_plan_get_transform_axes(self._h, t))
+        return tuple(bool(v) for v in t)
 
     def setWorkArea(self, device=None, host=None):
         check(lib().dfft_set_work_area(self._h, _ptr(device), _ptr(host)))
@@ -326,13 +349,13 @@ class MPIcuFFT_Pencil(MPIcuFFT):
     """z FFT -> transpose -> y FFT -> transpose -> x FFT on a P1 x P2 grid. include/mpicufft_pencil.hpp."""
     _decomp = PENCIL
 
-    def initFFT(self, global_size, partition=None, allocate=True, batch=1, inplace=False):
+    def initFFT(self, global_size, partition=None, allocate=True, batch=1, inplace=False, transform_axes=None):
         if partition is None or global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         if partition.P1 * partition.P2 != self.comm.size:
             raise RuntimeError("Invalid Input Partition!")
         self.partition = partition
-        super().initFFT(global_size, partition, allocate, batch, inplace)
+        super().initFFT(global_size, partition, allocate, batch, inplace, transform_axes)
 
     def getPartitionDimensions(self):
         """(input_dim, transposed_dim, output_dim), each a dict with size_x/y/z and start_x/y/z lists

@@ -241,6 +241,25 @@ int dfft_exec_r2r_async(dfft_plan_t plan, void* out, const void* in, int directi
 int dfft_plan_set_scale(dfft_plan_t plan, double forward_scale, double inverse_scale);
 /* Either pointer may be NULL. */
 int dfft_plan_get_scale(dfft_plan_t plan, double* forward_scale, double* inverse_scale);
+/* Untransformed axes (not in the reference; FFTW's guru "howmany" dimensions, 2DECOMP&FFT's standalone transposes).
+ * transform[0], [1], [2] belong to the x, y and z axis, the order of dfft_plan_create_r2r's kinds: 1 transforms that axis,
+ * 0 keeps it.  A kept axis is redistributed exactly as a transformed one would be, but its values are not transformed: an
+ * exec with x kept transforms z and y and delivers the output distribution (x whole on every rank), the layout a
+ * tridiagonal or banded solve along x needs.  All three kept: a distributed transpose.  Default {1, 1, 1}.
+ *   - Layouts, getters, dfft_get_domain_size and work sizes do not change.  A kept axis still needs a length its plan's
+ *     transform accepts.  R2R kinds of kept axes are ignored (dfft_plan_get_r2r_kinds still reports them).
+ *   - Partial d keeps its meaning: the first d stages in z, y, x order, each transformed or kept.  A round trip scales by
+ *     the product over the transformed axes among them of N (C2C, R2C, R2HC) or 2N (DCT, DST).
+ *   - A kept axis is one copy pass where a transform would run, none where the copy would only move memory on one rank
+ *     (DESIGN.md section 3.12).  These plans run the sequential schedule (dfft_plan_tune has one candidate).  Scale,
+ *     batches, in-place plans, every decomposition, Peer2Peer and All2All and graph capture work as for other plans.
+ *   - dfft_plan_describe: copy steps have kind 6 (contiguous) or 7 (strided) and "n"; plans with a kept axis report
+ *     "transform_axes".
+ * A null plan or array, an entry that is not 0 or 1, or an R2C / C2R plan with z kept: DFFT_ERR_INVALID.  Once the plan
+ * has built a schedule (its first exec, dfft_plan_tune or dfft_plan_describe): DFFT_ERR_STATE — set it once, right after
+ * creation.  Local to the calling rank: set the same values on every rank. */
+int dfft_plan_set_transform_axes(dfft_plan_t plan, const int transform[3]);
+int dfft_plan_get_transform_axes(dfft_plan_t plan, int transform[3]);
 /* Waits for the stream of the last eager _async call and reports a device-side failure (rendezvous or fused-stage
  * timeout), if any.  After replaying a graph, synchronise the replay stream first; dfft_plan_wait then reports the
  * errors the replayed kernels recorded. */

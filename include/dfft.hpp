@@ -105,6 +105,12 @@ public:
     // normalised round trips use setScale(1, 1.0 / (Nx * Ny * Nz)).
     void setScale(double forward_scale, double inverse_scale) { DFFT_CALL(dfft_plan_set_scale(plan, forward_scale, inverse_scale)); }
     void getScale(double& forward_scale, double& inverse_scale) const { DFFT_CALL(dfft_plan_get_scale(plan, &forward_scale, &inverse_scale)); }
+    // not in the reference: transform (true) or keep (false) the x, y, z axis (dfft_plan_set_transform_axes; after
+    // initFFT, before the first exec).  setTransformAxes(false, true, true) leaves x untransformed and whole on every rank.
+    void setTransformAxes(bool x, bool y, bool z) {
+        const int t[3] = {x ? 1 : 0, y ? 1 : 0, z ? 1 : 0};
+        DFFT_CALL(dfft_plan_set_transform_axes(plan, t));
+    }
     virtual void setWorkArea(void* device = nullptr, void* host = nullptr) { DFFT_CALL(dfft_set_work_area(plan, device, host)); }
     virtual void execR2C(void* out, const void* in) = 0;
     // not in the reference: real-to-real transform of a plan constructed with transform_ = DFFT_DCT or DFFT_DST, or with
