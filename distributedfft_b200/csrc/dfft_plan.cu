@@ -526,6 +526,7 @@ static int fuse_zy(dfft_plan_s* p, Step zs, const Step& ys, const char* label, c
     {
         const long long ahead = (long long)(p->l2_bytes / (3 * p->g.ny * p->g.nz * p->esize)) - 1;
         out.zyf.order.ahead = int(ahead < 1 ? 1 : ahead);
+        if (const char* e = getenv("DFFT_ZY_AHEAD")) out.zyf.order.ahead = std::max(1, atoi(e));  // look-ahead sweeps
     }
     out.zyf.err = p->err_d;
     out.zyf.timeout_cycles = p->rendezvous_timeout_cycles;
@@ -537,6 +538,15 @@ static int fuse_zy(dfft_plan_s* p, Step zs, const Step& ys, const char* label, c
         p->tabs.bytes.push_back(c);  // freed with the schedules
         if (cudaMemset(c, 0, bytes) != cudaSuccess) return fail(DFFT_ERR_CUDA, "fused z + y stage: counter initialisation failed");
         out.zyf.ctr = reinterpret_cast<unsigned long long*>(c);
+#ifdef DFFT_ZY_TRACE
+        // trace build: ZY_TRACE_SLOTS stamps per work item (4096 points each, both phases), rewritten by every launch
+        const size_t tbytes = sizeof(unsigned long long) * ZY_TRACE_SLOTS * 2 * size_t(p->g.nx) * (p->g.ny * p->g.nz / 4096);
+        void* t = nullptr;
+        if (cudaMalloc(&t, tbytes) != cudaSuccess) return fail(DFFT_ERR_CUDA, "fused z + y stage: trace allocation failed");
+        p->tabs.bytes.push_back(t);
+        if (cudaMemset(t, 0, tbytes) != cudaSuccess) return fail(DFFT_ERR_CUDA, "fused z + y stage: trace initialisation failed");
+        out.zyf.trace = reinterpret_cast<unsigned long long*>(t);
+#endif
     }
     return DFFT_SUCCESS;
 }
@@ -2911,6 +2921,23 @@ int dfft_plan_get_transform_axes(dfft_plan_t p, int transform[3]) {
     for (int a = 0; a < 3; ++a) transform[a] = p->taxes[a];
     return DFFT_SUCCESS;
 }
+#ifdef DFFT_ZY_TRACE
+// Trace build only (not part of include/dfft.h): copies the fused z + y stage's stamps of the last 3D exec in one direction
+// (fft_kernels.cuh, ZyStamp) to host memory; returns the number of work items, or a negative dfft_status.
+int dfft_zy_trace_copy(dfft_plan_t p, int inverse, void* host, size_t bytes) {
+    if (!p || !host) return DFFT_ERR_INVALID;
+    for (const Step& s : p->sched[inverse ? 1 : 0][2].steps) {
+        if (s.kernel != KERNEL_ZY_FUSED || !s.zyf.trace) continue;
+        const size_t items = 2 * size_t(p->g.nx) * (p->g.ny * p->g.nz / 4096);
+        const size_t need = items * ZY_TRACE_SLOTS * sizeof(unsigned long long);
+        if (bytes < need) return DFFT_ERR_INVALID;
+        if (cudaMemcpy(host, s.zyf.trace, need, cudaMemcpyDeviceToHost) != cudaSuccess) return DFFT_ERR_CUDA;
+        return int(items);
+    }
+    return DFFT_ERR_STATE;
+}
+#endif
+
 int dfft_plan_get_scale(dfft_plan_t p, double* forward_scale, double* inverse_scale) {
     if (!p) return fail(DFFT_ERR_INVALID, "null plan");
     if (forward_scale) *forward_scale = p->scale[0];

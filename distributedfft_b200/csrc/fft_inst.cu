@@ -329,15 +329,40 @@ cudaError_t launch_zy_fused(const FftParams& pz, const FftParams& py, const ZyFu
     f.discard = !in_place && (inv ? (Z::Z_DISCARD && aligned128(mid.seg[0].base, mid.seg[0].sA0, mid.seg[0].sA1, 1 << LOG2N))
                                   : (Z::Y_DISCARD && aligned128(mid.seg[0].base, mid.seg[0].sA0, mid.seg[0].sA1, mid.sN)));
     // persistent: as many CTAs as fit at once (tickets hand out the work; fewer resident CTAs are fine as well).  The
-    // grid depends on the work list only, so every launch of a step draws the same number of tickets (zy_launch_of).
-    constexpr auto kf = fft_zy_fused_kernel<T, LOG2N, false, false>;
-    static const int resident = resident_ctas(kf, Z::THREADS, Z::SMEM_BYTES);
+    // grid depends on the work list only, so every launch of a step draws the same number of tickets (zy_launch_of) —
+    // also when one exec runs the fed kernel and the next the register-fed one: the grid is the smaller residency of both.
+    constexpr auto kf_reg = fft_zy_fused_kernel<T, LOG2N, false, false>;
+    constexpr auto kis_reg = fft_zy_fused_kernel<T, LOG2N, true, true>;
+    static const int resident_reg = resident_ctas(kf_reg, Z::THREADS, Z::SMEM_BYTES);
+    int resident = resident_reg;
     const long long total = f.order.total();
     if (total <= 0) return cudaSuccess;
+    if constexpr (sizeof(T) == 8) {
+        // f64: inputs by asynchronous copies wherever the views are 16-byte aligned — z lines (pz.in) by bulk copies, y tiles
+        // by a tensor map of py.in, encoded here per exec because py.in may be the caller's buffer (inverse).  An aligned
+        // view whose map cannot be encoded is an error, not a quiet switch to the register-fed kernel.  DFFT_ZY_FEED=0
+        // forces the register-fed kernel (comparison of the two).  f32 keeps the register-fed kernel: fed, its
+        // 64-register budget spills and the inverse stage was slower (DESIGN.md section 3.4).
+        constexpr auto kf = fft_zy_fed_kernel<T, LOG2N, false, false>;
+        static const int resident_fed = resident_ctas(kf, Z::THREADS, Z::SMEM_BYTES);
+        if (resident_fed < resident) resident = resident_fed;
+        const unsigned grid = unsigned(total < resident ? total : resident);
+        constexpr unsigned long long es = sizeof(cx<T>);
+        const auto a16 = [](unsigned long long v) { return v % 16 == 0; };
+        const Seg& gz = pz.in.seg[0];
+        const Seg& gy = py.in.seg[0];
+        const bool aligned = a16(reinterpret_cast<unsigned long long>(gz.base)) && a16(gz.sA0 * es) && a16(gz.sA1 * es) &&
+                             a16(reinterpret_cast<unsigned long long>(gy.base)) && a16(gy.sA0 * es) && a16(gy.sA1 * es) && a16(py.in.sN * es);
+        if (env_int("DFFT_ZY_FEED", 1) != 0 && aligned) {
+            alignas(64) CUtensorMap tm;
+            if (!make_view_map<T>(py.in, py.A0, py.A1, 1 << LOG2N, py.B, TB, &tm)) return cudaErrorNotSupported;
+            // only the inverse stage has a scaled twin (a scaled forward stage is refused above)
+            constexpr auto kis = fft_zy_fed_kernel<T, LOG2N, true, true>;
+            return launch_kernel<kf, fft_zy_fed_kernel<T, LOG2N, true, false>, kis, kis>(pz, scale, grid, Z::THREADS, Z::SMEM_BYTES, stream, py, f, tm);
+        }
+    }
     const unsigned grid = unsigned(total < resident ? total : resident);
-    // only the inverse stage has a scaled twin (a scaled forward stage is refused above)
-    constexpr auto kis = fft_zy_fused_kernel<T, LOG2N, true, true>;
-    return launch_kernel<kf, fft_zy_fused_kernel<T, LOG2N, true, false>, kis, kis>(pz, scale, grid, Z::THREADS, Z::SMEM_BYTES, stream, py, f);
+    return launch_kernel<kf_reg, fft_zy_fused_kernel<T, LOG2N, true, false>, kis_reg, kis_reg>(pz, scale, grid, Z::THREADS, Z::SMEM_BYTES, stream, py, f);
 }
 
 template cudaError_t launch_zy_fused<DFFT_T, DFFT_LOG2N>(const FftParams&, const FftParams&, const ZyFused&, double, cudaStream_t);

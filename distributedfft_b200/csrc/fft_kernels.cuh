@@ -200,6 +200,11 @@ struct LineAccess {
 };
 
 // ---- the in-CTA transform ---------------------------------------------------------------------------
+struct NoGatherHook {
+    template <int ST>
+    __device__ __forceinline__ void operator()(std::integral_constant<int, ST>) const {}
+};
+
 template <typename T, int LOG2N, int LOG2E, int TB, bool TILED>
 struct CtaFft {
     using Core = FftCore<T, LOG2N, LOG2E>;
@@ -240,8 +245,11 @@ struct CtaFft {
         }
     }
 
-    template <int ST>
-    static __device__ __forceinline__ void stages(cx<T> (&v)[E], int j, int t, cx<T>* sm, const cx<T>* tw) {
+    // after_gather(std::integral_constant<int, ST>): called by every thread once the gather that follows stage ST has left
+    // shared memory; after ST = NST - 2 the buffer is free for this thread (the caller synchronises the CTA before it
+    // reuses it)
+    template <int ST, typename Hook = NoGatherHook>
+    static __device__ __forceinline__ void stages(cx<T> (&v)[E], int j, int t, cx<T>* sm, const cx<T>* tw, const Hook& after_gather = {}) {
         Core::template stage_compute<ST>(v, j, tw);
         if constexpr (ST + 1 < NST) {
             if constexpr (ST > 0) sync(t);
@@ -250,7 +258,8 @@ struct CtaFft {
             for (int e = 0; e < E; ++e) p[L::off(Core::template scatter_off<ST>(e))] = v[e];
             sync(t);
             gather(v, sm, j, t);
-            stages<ST + 1>(v, j, t, sm, tw);
+            after_gather(std::integral_constant<int, ST>{});
+            stages<ST + 1>(v, j, t, sm, tw, after_gather);
         }
     }
 };
@@ -371,9 +380,9 @@ struct MemScaled {
 __device__ __forceinline__ void l2_discard(const void* p) { asm volatile("discard.global.L2 [%0], 128;" ::"l"(p) : "memory"); }
 
 // ---- one tile of a C2C pass: load, CtaFft::stages, store --------------------------------------------------
-template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, typename M>
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, typename M, typename Hook = NoGatherHook>
 __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<T>* sm, unsigned long long* tab_in, unsigned long long* tab_out,
-                                         bool multi, const M& mem) {
+                                         bool multi, const M& mem, const Hook& after_gather = {}) {
     using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
     using LA = LineAccess<T, C::LINES>;
     using TC = TileCoord<C, TILED, TB>;
@@ -420,7 +429,7 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
         for (int e = 0; e < E; ++e) v[e] = cx<T>{T(0), T(0)};
     }
 
-    C::template stages<0>(v, j, t, sm, reinterpret_cast<const cx<T>*>(p.tw));
+    C::template stages<0>(v, j, t, sm, reinterpret_cast<const cx<T>*>(p.tw), after_gather);
 
     if (tc.valid) {
         if (!out.multi) {
@@ -481,6 +490,38 @@ fft_c2c_kernel(const __grid_constant__ KParams<SCALED> p) {
     }
 }
 
+// ---- mbarrier of an asynchronous tile copy (fft_c2c_tma_kernel, fft_zy_fused_kernel) ------------------------------
+struct TmaBar {
+    static __device__ __forceinline__ void init(unsigned long long* bar, unsigned count) {
+        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(unsigned(__cvta_generic_to_shared(bar))), "r"(count) : "memory");
+    }
+    static __device__ __forceinline__ void expect(unsigned long long* bar, unsigned bytes) {
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(unsigned(__cvta_generic_to_shared(bar))), "r"(bytes) : "memory");
+    }
+    static __device__ __forceinline__ bool try_wait(unsigned a, unsigned parity) {
+        unsigned ok;
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+            : "=r"(ok) : "r"(a), "r"(parity) : "memory");
+        return ok != 0;
+    }
+    // bounded wait: a lost transaction must not hang the GPU (returns false after ~2 s)
+    static __device__ __forceinline__ bool wait(unsigned long long* bar, unsigned parity) {
+        const unsigned a = unsigned(__cvta_generic_to_shared(bar));
+        for (long long spin = 0; spin < (1ll << 26); ++spin)
+            if (try_wait(a, parity)) return true;
+        return false;
+    }
+    // wait of at most `cycles` clock64 cycles (0 = no limit); false when they ran out
+    static __device__ __forceinline__ bool wait_for(unsigned long long* bar, unsigned parity, long long cycles) {
+        const unsigned a = unsigned(__cvta_generic_to_shared(bar));
+        const long long t0 = clock64();
+        while (!try_wait(a, parity))
+            if (cycles > 0 && clock64() - t0 > cycles) return false;
+        return true;
+    }
+};
+
 // ---- fused z + y stage of one-rank slab transforms ---------------------------------------------------------
 // One persistent launch runs the z pass (CONTIG, `pz`) and the y pass (TILED, `py`) of the same x-planes, plane group
 // by plane group, so that the intermediate one pass writes is still in the L2 when the other reads it (ZyOrder in
@@ -497,6 +538,12 @@ fft_c2c_kernel(const __grid_constant__ KParams<SCALED> p) {
 //     be read by one CTA only — 128-byte y-tile rows (TB * sizeof(complex) a multiple of 128) and z lines of a multiple
 //     of 128 bytes, on 128-byte aligned views (ZyFused::discard, checked by the launcher).
 //
+// Fed by asynchronous copies (FED, the default where the views allow it): every item's N x TB input points arrive by
+// cp.async.bulk (z lines) or cp.async.bulk.tensor (y tiles) in shared memory, announced by an mbarrier, and the next
+// item's copy is requested as soon as the current item's last gather has left the buffer (fft_zy_fed_kernel).  The
+// register-fed form (fft_zy_fused_kernel, c2c_tile) stays for f32 and for views the copies cannot address (16-byte
+// alignment); launch_zy_fused chooses.
+//
 // The parameters of the two persistent two-phase kernels (this one and fft_batch_small_kernel) begin with TicketWork, the
 // state of their common ticket loop (ticket_loop).
 struct TicketWork {
@@ -504,11 +551,49 @@ struct TicketWork {
     int* err;                  // the plan's device error flag
     long long timeout_cycles;  // clock64 cycles a dependency wait may take (0 = no limit)
     ZyOrder order;
+#ifdef DFFT_ZY_TRACE
+    unsigned long long* trace;  // trace build: ZY_TRACE_SLOTS stamps per ticket of the last launch (null: none)
+#endif
 };
+
+// Trace build (-DDFFT_ZY_TRACE, tools/zy_trace.py): thread 0 of a CTA writes %globaltimer stamps per work item into
+// TicketWork::trace[ticket * ZY_TRACE_SLOTS + k].  The default build compiles none of it.
+constexpr int ZY_TRACE_SLOTS = 8;
+enum ZyStamp {
+    ZY_TICKET = 0,      // ticket read from the broadcast slot
+    ZY_DEP_MET = 1,     // dependencies met (phase A: at once)
+    ZY_INPUTS = 2,      // fed kernel: the item's copy has landed
+    ZY_EXCHANGED = 3,   // first exchange through shared memory done (register-fed kernel: its loads have arrived)
+    ZY_LAST_GATHER = 4, // last gather done: the buffer is free
+    ZY_STORED = 5,      // every store of the item issued (thread 0)
+    ZY_DONE = 6,        // counted done / discards issued
+    ZY_WHERE = 7        // (smid << 32) | (CTA << 1) | phase
+};
+#ifdef DFFT_ZY_TRACE
+__device__ __forceinline__ void zy_stamp(const TicketWork& f, long long ticket, int k) {
+    if (f.trace && threadIdx.x == 0) {
+        unsigned long long t;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+        f.trace[ticket * ZY_TRACE_SLOTS + k] = t;
+    }
+}
+__device__ __forceinline__ void zy_stamp_where(const TicketWork& f, long long ticket, int phase) {
+    if (f.trace && threadIdx.x == 0) {
+        unsigned smid;
+        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+        f.trace[ticket * ZY_TRACE_SLOTS + ZY_WHERE] = ((unsigned long long)smid << 32) | ((unsigned long long)blockIdx.x << 1) | unsigned(phase);
+    }
+}
+#define ZY_STAMP(f, ticket, k) zy_stamp(f, ticket, k)
+#define ZY_STAMP_WHERE(f, ticket, phase) zy_stamp_where(f, ticket, phase)
+#else
+#define ZY_STAMP(f, ticket, k) ((void)0)  // the arguments (volatile shared reads among them) are not evaluated
+#define ZY_STAMP_WHERE(f, ticket, phase) ((void)0)
+#endif
 struct ZyFused : TicketWork {
     int discard;  // phase B may discard the intermediate lines it has read
 };
-constexpr int ZY_ERR_TIMEOUT = 200;   // value of the error flag when a fused-stage dependency wait timed out
+constexpr int ZY_ERR_TIMEOUT = 200;   // value of the error flag when a fused-stage wait (dependency or input copy) timed out
 
 // The ticket loop of a persistent two-phase kernel: draws tickets until the work list is done, waits before each phase-B
 // item until every phase-A item of its group has finished, and runs item(it, slot) for every work item `it` (all threads;
@@ -517,8 +602,14 @@ constexpr int ZY_ERR_TIMEOUT = 200;   // value of the error flag when a fused-st
 // needed instead of being kept in registers through the tiles.  bcast[2]: give up.  bcast[3], bcast[4]: this launch's
 // counter base and epoch, fixed by the CTA's first draw (zy_launch_of) — the kernel takes no per-exec value from the host,
 // so a graph can replay it.  A timed-out wait sets the error flag to timeout_err and ends the loop.
-template <typename Item>
-__device__ __forceinline__ void ticket_loop(const TicketWork& f, volatile long long* bcast, int timeout_err, const Item& item) {
+// ready(it, ticket): thread 0, once the item's dependencies are met and before the item runs (the fused stage requests the
+// item's input there unless it did so earlier).  An item that returns a bool ends the loop by returning false (the same
+// value in every thread).
+struct NoFeed {
+    __device__ __forceinline__ void operator()(const ZyItem&, long long) const {}
+};
+template <typename Item, typename Ready = NoFeed>
+__device__ __forceinline__ void ticket_loop(const TicketWork& f, volatile long long* bcast, int timeout_err, const Item& item, const Ready& ready = {}) {
     const int tid = threadIdx.x;
     const long long total = f.order.total();
     int par = 0;
@@ -534,6 +625,7 @@ __device__ __forceinline__ void ticket_loop(const TicketWork& f, volatile long l
         __syncthreads();
         const long long ticket = bcast[par];
         if (ticket >= total) break;
+        ZY_STAMP(f, ticket, ZY_TICKET);
         if (tid == 0) bcast[par ^ 1] = (long long)(atomicAdd(f.ctr, 1ull) - (unsigned long long)bcast[3]);
         const ZyItem it = f.order.decode(ticket);
         if (it.phase == 1) {
@@ -564,11 +656,20 @@ __device__ __forceinline__ void ticket_loop(const TicketWork& f, volatile long l
                     }
                 }
                 bcast[2] = bail;
+                if (!bail) ready(it, ticket);
             }
             __syncthreads();
             if (bcast[2]) break;
+        } else if (tid == 0) {
+            ready(it, ticket);
         }
-        item(it, bcast + par);
+        ZY_STAMP(f, ticket, ZY_DEP_MET);
+        ZY_STAMP_WHERE(f, ticket, it.phase);
+        if constexpr (std::is_same_v<decltype(item(it, bcast + par)), bool>) {
+            if (!item(it, bcast + par)) break;
+        } else {
+            item(it, bcast + par);
+        }
     }
 }
 
@@ -590,9 +691,10 @@ struct ZyShape {
 };
 
 // End of a work item of fft_zy_fused_kernel (all threads, after the tile is stored): a phase-A item counts itself done,
-// a phase-B item drops the intermediate lines it has read.  Kept out of line: the kernel runs at its 128-register limit
-// and this bookkeeping, inlined into the loop, made the register allocator spill the tile's points.
-template <typename T, int LOG2N, bool INV>
+// a phase-B item of the register-fed kernel (DISCARD) drops the intermediate lines it has read.  Kept out of line: the
+// kernel runs at its 128-register limit and this bookkeeping, inlined into the loop, made the register allocator spill the
+// tile's points.
+template <typename T, int LOG2N, bool INV, bool DISCARD>
 __device__ __noinline__ void zy_item_done(const FftParams& pz, const FftParams& py, const ZyFused& f, long long ticket) {
     using Z = ZyShape<T, LOG2N>;
     constexpr int TB = Z::TB, N = 1 << LOG2N;
@@ -601,10 +703,11 @@ __device__ __noinline__ void zy_item_done(const FftParams& pz, const FftParams& 
     if (done.phase == 0) {
         // release at gpu scope, after the barrier that ordered every thread's stores of the item before this thread
         if (tid == 0) asm volatile("red.release.gpu.global.add.u64 [%0], 1;" ::"l"(f.ctr + 1 + done.group) : "memory");
-    } else if (f.discard) {
-        // Phase B: the intermediate this tile read is dead — drop its 128-byte lines without a write-back.  Done
-        // here, after the tile, rather than as soon as it is in registers: with the 16 points per thread live the
-        // extra addressing spilled registers, and a line survives the few microseconds of one tile.
+    } else if (DISCARD && f.discard) {
+        // Phase B: the intermediate this tile read is dead — drop its 128-byte lines without a write-back.  The
+        // register-fed kernel does it here, after the tile, rather than as soon as it is in registers: with the 16
+        // points per thread live the extra addressing spilled registers, and a line survives the few microseconds of
+        // one tile.  The fed kernel calls this with the item's bytes in shared memory and nothing live.
         if (INV) {  // phase B = z lines
             if constexpr (Z::Z_DISCARD) {
                 constexpr int PER_LINE = int(N * sizeof(cx<T>)) / 128;  // TB lines of this tile
@@ -629,7 +732,54 @@ __device__ __noinline__ void zy_item_done(const FftParams& pz, const FftParams& 
     }
 }
 
+// One work item of the fed stage (all threads): its N x TB points are in shared memory as the copies wrote them — TB dense
+// z lines [t][n], or a dense y tile [n][TB].  One gather into registers, then the buffer becomes the padded exchange space
+// of CtaFft::stages; from there on the arithmetic is c2c_tile's, so the results are bit-identical.  `ok`: this thread's
+// wait for the copy succeeded; false in any thread ends the item in every thread (returns false).
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, typename M, typename Hook>
+__device__ __forceinline__ bool zy_fed_tile(const FftParams& p, long long tile, cx<T>* sm, const M& mem, bool ok, const Hook& after_gather) {
+    using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
+    constexpr int E = C::E, TPL = C::TPL, N = C::N;
+    const TileCoord<C, TILED, TB> tc(p, tile);
+    const int j = tc.j, t = tc.t;
+    cx<T> v[E];
+#pragma unroll
+    for (int e = 0; e < E; ++e) {
+        const cx<T> x = TILED ? sm[(j + e * TPL) * TB + t] : sm[t * N + j + e * TPL];
+        v[e] = INV ? cswap(x) : x;
+    }
+    if (__syncthreads_or(!ok)) return false;
+    C::template stages<0>(v, j, t, sm, reinterpret_cast<const cx<T>*>(p.tw), after_gather);
+    if (tc.valid) {
+        const Seg& g = p.out.seg[0];
+        cx<T>* q = reinterpret_cast<cx<T>*>(g.base) + (tc.a0 * g.sA0 + tc.a1 * g.sA1 - (long long)g.n0 * p.out.sN + tc.b) + (long long)j * p.out.sN;
+        const long long step = (long long)TPL * p.out.sN;
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            const cx<T> x = v[C::Core::final_slot(e)];
+            if constexpr (TILED) {
+                mem.st(q, INV ? cswap(x) : x);
+                q += step;
+            } else {
+                mem.st(q + e * TPL, INV ? cswap(x) : x);  // contiguous line: sN == 1
+            }
+        }
+    }
+    return true;
+}
+
+// global -> shared copies of the fed stage, completing on the mbarrier at shared address mb, with an L2 policy
+__device__ __forceinline__ void bulk_load(unsigned dst, const void* src, unsigned bytes, unsigned mb, unsigned long long pol) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(dst), "l"(src), "r"(bytes), "r"(mb), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void tensor_load4(unsigned dst, const CUtensorMap* tm, int c0, int c1, int c2, int c3, unsigned mb, unsigned long long pol) {
+    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5, %6}], [%2], %7;"
+                 ::"r"(dst), "l"(tm), "r"(mb), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(pol) : "memory");
+}
+
 // SCALED (inverse only): phase B, the z lines that store the caller's output, scales its stores by pz.scale.
+// Register-fed form: every item's inputs by 16-byte loads into registers (c2c_tile).
 template <typename T, int LOG2N, bool INV, bool SCALED>
 __global__ void __launch_bounds__(ZyShape<T, LOG2N>::THREADS, min_ctas_per_sm<T, ZyShape<T, LOG2N>::LOG2E>(ZyShape<T, LOG2N>::THREADS))
 fft_zy_fused_kernel(const __grid_constant__ KParams<SCALED> pz, const __grid_constant__ FftParams py, const __grid_constant__ ZyFused f) {
@@ -645,18 +795,146 @@ fft_zy_fused_kernel(const __grid_constant__ KParams<SCALED> pz, const __grid_con
         const bool z_item = (it.phase == 0) == !INV;  // forward: phase A = z; inverse: phase A = y
         const MemHint<T> mem_a{l2_evict_first(), l2_evict_last()};   // streaming input -> intermediate
         const MemHint<T> mem_b{l2_evict_normal(), l2_evict_first()};  // intermediate -> streaming output
+        // trace build: the first exchange and the last gather (nothing in the default build)
+        auto stamp = [&](auto st) {
+            constexpr int ST = decltype(st)::value, NST = CtaFft<T, LOG2N, Z::LOG2E, TB, false>::NST;
+            if constexpr (ST == 0) ZY_STAMP(f, *slot, ZY_EXCHANGED);
+            if constexpr (ST + 2 == NST) ZY_STAMP(f, *slot, ZY_LAST_GATHER);
+        };
         if (z_item) {
-            if (it.phase == 0) c2c_tile<T, LOG2N, Z::LOG2E, TB, false, INV>(pz, it.tile, sm, tab_in, tab_out, false, mem_a);
-            else if constexpr (SCALED) c2c_tile<T, LOG2N, Z::LOG2E, TB, false, INV>(pz, it.tile, sm, tab_in, tab_out, false, MemScaled<T, MemHint<T>>{mem_b, T(pz.scale)});
-            else c2c_tile<T, LOG2N, Z::LOG2E, TB, false, INV>(pz, it.tile, sm, tab_in, tab_out, false, mem_b);
+            if (it.phase == 0) c2c_tile<T, LOG2N, Z::LOG2E, TB, false, INV>(pz, it.tile, sm, tab_in, tab_out, false, mem_a, stamp);
+            else if constexpr (SCALED) c2c_tile<T, LOG2N, Z::LOG2E, TB, false, INV>(pz, it.tile, sm, tab_in, tab_out, false, MemScaled<T, MemHint<T>>{mem_b, T(pz.scale)}, stamp);
+            else c2c_tile<T, LOG2N, Z::LOG2E, TB, false, INV>(pz, it.tile, sm, tab_in, tab_out, false, mem_b, stamp);
         } else {
-            if (it.phase == 0) c2c_tile<T, LOG2N, Z::LOG2E, TB, true, INV>(py, it.tile, sm, tab_in, tab_out, false, mem_a);
-            else c2c_tile<T, LOG2N, Z::LOG2E, TB, true, INV>(py, it.tile, sm, tab_in, tab_out, false, mem_b);
+            if (it.phase == 0) c2c_tile<T, LOG2N, Z::LOG2E, TB, true, INV>(py, it.tile, sm, tab_in, tab_out, false, mem_a, stamp);
+            else c2c_tile<T, LOG2N, Z::LOG2E, TB, true, INV>(py, it.tile, sm, tab_in, tab_out, false, mem_b, stamp);
         }
+        ZY_STAMP(f, *slot, ZY_STORED);
         // the tile is stored and shared memory is free again before the item counts
         __syncthreads();
-        zy_item_done<T, LOG2N, INV>(pz, py, f, *slot);
+        zy_item_done<T, LOG2N, INV, true>(pz, py, f, *slot);
+        ZY_STAMP(f, *slot, ZY_DONE);
     });
+}
+
+// Fed form (complex-double): inputs by asynchronous copies.  tm_y: rank-4 map (b, n, a1, a0) of py.in, box TB x min(N, 256).
+template <typename T, int LOG2N, bool INV, bool SCALED>
+__global__ void __launch_bounds__(ZyShape<T, LOG2N>::THREADS, min_ctas_per_sm<T, ZyShape<T, LOG2N>::LOG2E>(ZyShape<T, LOG2N>::THREADS))
+fft_zy_fed_kernel(const __grid_constant__ KParams<SCALED> pz, const __grid_constant__ FftParams py, const __grid_constant__ ZyFused f,
+                  const __grid_constant__ CUtensorMap tm_y) {
+    static_assert(INV || !SCALED, "the forward fused stage stores the intermediate of the x pass only");
+    using Z = ZyShape<T, LOG2N>;
+    constexpr int TB = Z::TB, N = 1 << LOG2N, NST = CtaFft<T, LOG2N, Z::LOG2E, TB, false>::NST;
+    constexpr unsigned TILE_TX = unsigned(N) * TB * unsigned(sizeof(cx<T>));  // bytes of one item, either kind
+    constexpr int D0 = sizeof(T) == 8 ? 2 : 1;                                // 8-byte map units per complex element
+    static_assert(TILE_TX <= Z::TILE_BYTES, "an item's dense landing fits the tile buffer");
+    static_assert(NST == CtaFft<T, LOG2N, Z::LOG2E, TB, true>::NST, "one stage count for both phases");
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
+    unsigned long long* bar = reinterpret_cast<unsigned long long*>(smem_raw + Z::TILE_BYTES + Z::TABLE_BYTES - 16);  // tables unused
+    volatile long long* bcast = reinterpret_cast<volatile long long*>(smem_raw + Z::TILE_BYTES + Z::TABLE_BYTES);
+    const int tid = threadIdx.x;
+    const long long total = f.order.total();
+    long long requested = -1;  // thread 0: the last ticket whose input copy was issued
+    unsigned parity = 0;
+    if (tid == 0) {
+        TmaBar::init(bar, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }  // the ticket loop's first barrier orders the init before any use
+
+    // thread 0: arm the barrier and issue the copies of item n (phase A input: evict_first, as the register-fed loads)
+    auto request = [&](const ZyItem& n, long long ticket) {
+        requested = ticket;
+        const unsigned dst = unsigned(__cvta_generic_to_shared(sm));
+        const unsigned mb = unsigned(__cvta_generic_to_shared(bar));
+        const unsigned long long pol = n.phase == 0 ? l2_evict_first() : l2_evict_normal();
+        TmaBar::expect(bar, TILE_TX);
+        if ((n.phase == 0) == !INV) {
+            // TB consecutive z lines of one a0 (A1 % TB == 0): one range when adjacent, else one copy per line
+            const long long line = n.tile * TB;
+            const Seg& g = pz.in.seg[0];
+            const cx<T>* src = reinterpret_cast<const cx<T>*>(g.base) + ((line / pz.A1) * g.sA0 + (line % pz.A1) * g.sA1 - g.n0);
+            if (g.sA1 == N) {
+                bulk_load(dst, src, TILE_TX, mb, pol);
+            } else {
+#pragma unroll 1
+                for (int t = 0; t < TB; ++t) bulk_load(dst + t * unsigned(N * sizeof(cx<T>)), src + t * g.sA1, unsigned(N * sizeof(cx<T>)), mb, pol);
+            }
+        } else {
+            int bt, a1, a0;
+            tiled_decode<TB>(py, n.tile, bt, a1, a0);
+#pragma unroll
+            for (int r = 0; r < N; r += 256)
+                tensor_load4(dst + unsigned(r) * TB * unsigned(sizeof(cx<T>)), &tm_y, bt * TB * D0, r, a1, a0, mb, pol);
+        }
+    };
+    // ticket loop, thread 0, dependencies met: the item's copy, unless it was issued early.  A phase-B item reads what
+    // other CTAs stored through the generic proxy (acquired by the counter wait); the proxy fence orders those stores
+    // before this thread's async-proxy read.
+    auto ready = [&](const ZyItem& it, long long ticket) {
+        if (requested == ticket) return;
+        if (it.phase == 1) asm volatile("fence.proxy.async.global;" ::: "memory");
+        request(it, ticket);
+    };
+    ticket_loop(f, bcast, ZY_ERR_TIMEOUT, [&](const ZyItem& it, const volatile long long* slot) -> bool {
+        // A timed-out wait (the plan's timeout, seconds) sets the error flag and ends the loop in every thread.  The copy
+        // it waited for may then still be in flight into this CTA's shared memory after the CTA has exited; as after a
+        // timed-out dependency wait, the plan's device state is undefined once the flag is set (dfft_plan_wait reports it).
+        const bool ok = TmaBar::wait_for(bar, parity, f.timeout_cycles);
+        parity ^= 1;
+        ZY_STAMP(f, *slot, ZY_INPUTS);
+        if (!ok) atomicExch(f.err, ZY_ERR_TIMEOUT);
+        else if (it.phase == 1) zy_item_done<T, LOG2N, INV, true>(pz, py, f, *slot);  // its intermediate is dead: discard
+        // Early request of the next item, once the last gather of this one has left the buffer (every thread, between
+        // the last gather and the last stage).  A phase-A item is requested at once.  A phase-B item is requested only
+        // if its group counter has reached the target at the first look: thread 0 never waits here while this item is
+        // unfinished, otherwise the request waits for the top of the loop, after this item has counted itself done.
+        // So ticket_loop's argument holds word for word: the lowest unfinished ticket is held by a resident CTA whose
+        // earlier item is finished, all its dependencies are finished, and nothing it waits for depends on later work.
+        const volatile long long* next_slot = bcast + ((slot - bcast) ^ 1);
+        auto after_gather = [&](auto st) {
+            constexpr int ST = decltype(st)::value;
+            if constexpr (ST == 0) ZY_STAMP(f, *slot, ZY_EXCHANGED);
+            if constexpr (ST + 2 == NST) {
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic reads of the buffer before the async write
+                __syncthreads();
+                ZY_STAMP(f, *slot, ZY_LAST_GATHER);
+                if (tid == 0) {
+                    const long long next = *next_slot;
+                    if (next < total) {
+                        const ZyItem n = f.order.decode(next);
+                        bool go = n.phase == 0;
+                        if (!go) {
+                            const unsigned long long target = (unsigned long long)bcast[4] * (unsigned long long)f.order.a_items(n.group);
+                            unsigned long long v;
+                            asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(f.ctr + 1 + n.group) : "memory");
+                            go = v >= target;
+                            if (go) asm volatile("fence.proxy.async.global;" ::: "memory");
+                        }
+                        if (go) request(n, next);
+                    }
+                }
+            }
+        };
+        const bool z_item = (it.phase == 0) == !INV;
+        const MemHint<T> mem_a{0, l2_evict_last()};    // -> intermediate
+        const MemHint<T> mem_b{0, l2_evict_first()};   // -> streaming output
+        bool done;
+        if (z_item) {
+            if (it.phase == 0) done = zy_fed_tile<T, LOG2N, Z::LOG2E, TB, false, INV>(pz, it.tile, sm, mem_a, ok, after_gather);
+            else if constexpr (SCALED) done = zy_fed_tile<T, LOG2N, Z::LOG2E, TB, false, INV>(pz, it.tile, sm, MemScaled<T, MemHint<T>>{mem_b, T(pz.scale)}, ok, after_gather);
+            else done = zy_fed_tile<T, LOG2N, Z::LOG2E, TB, false, INV>(pz, it.tile, sm, mem_b, ok, after_gather);
+        } else {
+            if (it.phase == 0) done = zy_fed_tile<T, LOG2N, Z::LOG2E, TB, true, INV>(py, it.tile, sm, mem_a, ok, after_gather);
+            else done = zy_fed_tile<T, LOG2N, Z::LOG2E, TB, true, INV>(py, it.tile, sm, mem_b, ok, after_gather);
+        }
+        if (!done) return false;
+        ZY_STAMP(f, *slot, ZY_STORED);
+        __syncthreads();  // every store of the item is issued before it counts
+        zy_item_done<T, LOG2N, INV, false>(pz, py, f, *slot);
+        ZY_STAMP(f, *slot, ZY_DONE);
+        return true;
+    }, ready);
 }
 
 // ---- batches of small cubic fields: one persistent launch per exec ------------------------------------------
@@ -793,26 +1071,7 @@ fft_batch_small_kernel(const __grid_constant__ KParams<SCALED> px, const __grid_
 // Input view: single segment; described by a rank-4 tensor map (b, n, a1, a0) built by the launcher, box TB x 256.
 // Output: either 16-byte stores from registers through any (segmented) view, or — `bulk_out`, blocked hand-over
 // layouts whose rows per destination are adjacent — one cp.async.bulk (UBLKCP) per destination from the buffer.
-struct TmaBar {
-    static __device__ __forceinline__ void init(unsigned long long* bar, unsigned count) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(unsigned(__cvta_generic_to_shared(bar))), "r"(count) : "memory");
-    }
-    static __device__ __forceinline__ void expect(unsigned long long* bar, unsigned bytes) {
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(unsigned(__cvta_generic_to_shared(bar))), "r"(bytes) : "memory");
-    }
-    // bounded wait: a lost transaction must not hang the GPU (returns false after ~2 s)
-    static __device__ __forceinline__ bool wait(unsigned long long* bar, unsigned parity) {
-        const unsigned a = unsigned(__cvta_generic_to_shared(bar));
-        for (long long spin = 0; spin < (1ll << 26); ++spin) {
-            unsigned ok;
-            asm volatile(
-                "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                : "=r"(ok) : "r"(a), "r"(parity) : "memory");
-            if (ok) return true;
-        }
-        return false;
-    }
-};
+// (TmaBar: above, with the fused z + y stage.)
 
 // SCALED: every finished value is scaled by p.scale in registers, before the 16-byte stores or the staging for bulk_out.
 template <typename T, int LOG2N, int LOG2E, int TB, bool INV, bool SCALED>
