@@ -110,6 +110,8 @@ SIGNATURES = {
                                     C.c_size_t, C.c_void_p]),
     "dfft_comm_create_dry": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     "dfft_plan_describe": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "dfft_debug_run_step": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_size_t, C.c_int, C.POINTER(C.c_void_p), C.c_size_t, C.c_void_p,
+                                      C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     "dfft_fft1d_general": (C.c_int, [C.c_int, C.c_int, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.POINTER(C.c_longlong),
                                      C.c_void_p, C.POINTER(C.c_longlong), C.c_void_p]),
     "dfft_fft1d_strided": (C.c_int, [C.c_int, C.c_int, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),

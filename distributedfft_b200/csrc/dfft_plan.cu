@@ -220,6 +220,26 @@ struct Tables {
     }
 };
 
+// The power-of-two length a pass of n-point lines runs (R2C / C2R: n complex points): log2 n, or log2 M of the Bluestein
+// pass for C2C lengths that are not powers of two; -1 for lengths nothing runs
+static int pass_log2(PassKind kind, size_t n) {
+    return (kind == PASS_C2C_CONTIG || kind == PASS_C2C_TILED) && bluestein_length(n) ? bluestein_log2m(n) : ilog2_exact(n);
+}
+
+// The tables such a pass reads, from T: tw of its power-of-two length, tw2 for R2C / C2R and DCT / DST passes (r2r: the kind
+// of R2R passes; DCT / DST take w_k = exp(-i pi k / 2N), k <= N, the R2C table of length 2N), blu for Bluestein lengths.
+// One rule for plans and for the single-axis calls.
+static int pass_tables(Tables& T, PassKind kind, size_t n, int r2r, void** tw, void** tw2, void** blu) {
+    const int l2 = pass_log2(kind, n);
+    const bool with_w = (kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED) && r2r != DFFT_R2HC;
+    *tw = *tw2 = *blu = nullptr;
+    if (l2 != ilog2_exact(n) && T.get_blu(n, blu) != cudaSuccess) return fail(DFFT_ERR_CUDA, "Bluestein table allocation failed");
+    if (T.get_tw(l2, tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
+    if ((kind == PASS_R2C || kind == PASS_C2R || with_w) && T.get_tw2(l2 + (with_w ? 1 : 0), tw2) != cudaSuccess)
+        return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
+    return DFFT_SUCCESS;
+}
+
 // ---- device rendezvous ---------------------------------------------------------------------------------
 // flags layout (uint64): [phase][rank], NPHASE phases.  Thread i handles group member i: publishes my
 // epoch in the peer's flag row, then waits for the peer's epoch in mine.
@@ -633,29 +653,18 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         }
         s.kind = kind;
         s.phase = phase;
-        s.log2n = ilog2_exact(n);
+        s.log2n = pass_log2(kind, n);  // Bluestein lengths: the view mapping stays the kind's; the exec launches the Bluestein kernel
         s.n = n;
-        if ((kind == PASS_C2C_CONTIG || kind == PASS_C2C_TILED) && bluestein_length(n)) {
-            s.log2n = bluestein_log2m(n);  // the view mapping stays the kind's; the exec launches the Bluestein kernel
-            void* blu = nullptr;
-            if (T.get_blu(n, &blu) != cudaSuccess) return fail(DFFT_ERR_CUDA, "Bluestein table allocation failed");
-            s.blu = blu;
-        }
         if (s.log2n < 1 || s.log2n > MAX_LOG2N)
             return fail(DFFT_ERR_UNSUPPORTED, "axis length " + std::to_string(n) + " is not a supported power of two (2..8192)");
         s.prm.A0 = 1; s.prm.A1 = 1; s.prm.B = 1;
         s.prm.inverse = inverse;
-        void* tw = nullptr;
-        if (T.get_tw(s.log2n, &tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
+        void *tw = nullptr, *tw2 = nullptr, *blu = nullptr;
+        const int rc = pass_tables(T, kind, n, s.r2r, &tw, &tw2, &blu);
         s.prm.tw = tw;
-        s.prm.tw2 = nullptr;
-        if (kind == PASS_R2C || kind == PASS_C2R || (r2r && s.r2r != DFFT_R2HC)) {
-            // DCT / DST: w_k = exp(-i pi k / 2N), k <= N, the R2C table of length 2N
-            void* tw2 = nullptr;
-            if (T.get_tw2(s.log2n + (r2r ? 1 : 0), &tw2) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
-            s.prm.tw2 = tw2;
-        }
-        return DFFT_SUCCESS;
+        s.prm.tw2 = tw2;
+        s.blu = blu;
+        return rc;
     };
     auto rendezvous = [&](int group, int phase_id, const char* phase) {
         Step s;
@@ -1988,6 +1997,41 @@ static int plan_setup_flags(dfft_plan_s* p) {
 // =====================================================================================================
 // execution
 // =====================================================================================================
+// Views on the caller's buffers store a byte offset in seg[0].base; field f of a batched plan starts f field sizes further.
+// which: the step's in_user / out_user (1: `in`, 2: `out` — in_user 2 is a view that reads `out`, in-place plans).
+static void user_view(View& v, int which, const Schedule& sc, size_t f, void* out, const void* in) {
+    if (which == 1) v.seg[0].base = (char*)const_cast<void*>(in) + f * sc.field_in + (size_t)v.seg[0].base;
+    if (which == 2) v.seg[0].base = (char*)out + f * sc.field_out + (size_t)v.seg[0].base;
+}
+
+// Enqueues PASS step s of sc for field f on ss: the copy, FFT, fused or batched kernel over its views, its stores scaled by
+// the direction's output scale when they are final values.  An in-place copy onto itself with nothing to scale is not
+// launched (*launched = false).
+static cudaError_t run_pass_step(const dfft_plan_s* p, const Schedule& sc, const Step& s, size_t f, void* out, const void* in, cudaStream_t ss,
+                                 bool* launched) {
+    *launched = false;
+    if (s.identity && p->scale[sc.inverse] == 1.0) return cudaSuccess;
+    const double scale = s.final_store ? p->scale[sc.inverse] : 1.0;
+    FftParams prm = s.prm, prm_y = s.prm_y;
+    user_view(prm.in, s.in_user, sc, f, out, in);
+    user_view(prm.out, s.out_user, sc, f, out, in);
+    user_view(prm_y.in, s.y_in_user, sc, f, out, in);
+    user_view(prm_y.out, s.y_out_user, sc, f, out, in);
+    cudaError_t e = cudaErrorInvalidValue;
+    switch (s.kernel) {
+        case KERNEL_PASS:
+            e = is_copy(s.kind) ? launch_copy_pass(p->prec, is_r2r(p->g.transform), s.kind, s.n, prm, scale, ss)
+                                : launch_fft_pass(p->prec, s.kind, s.n ? s.n : size_t(1) << s.log2n, prm, s.blu, scale, ss, s.r2r);
+            break;
+        case KERNEL_ZY_FUSED: e = launch_zy_fused(p->prec, s.log2n, prm, prm_y, s.zyf, scale, ss); break;
+        case KERNEL_BATCH_SMALL:
+            e = launch_batch_small(p->prec, s.log2n, prm.in.seg[0].base, prm.out.seg[0].base, (long long)p->batch, s.prm.inverse, s.bsf, scale, ss);
+            break;
+    }
+    *launched = e == cudaSuccess;
+    return e;
+}
+
 // capture: `st` is capturing into a CUDA graph (one-rank plans only, see exec_common).  Then only the kernels are
 // enqueued: no timer or timeline events, and the plan's record of its last exec (launch count, stream, timer) stays
 // what the last eager exec left.
@@ -2072,35 +2116,11 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
             for (int w : s.waits) CK_CUDA(cudaStreamWaitEvent(ss, p->sync_events[w], 0));
             CK_CUDA(tl_mark(ss, s.label, s.stream));
             const char* phase = last ? s.phase : nullptr;
-            if (s.type == STEP_PASS && s.identity && p->scale[sc.inverse] == 1.0) {
-                CK_CUDA(mark(phase, 1, s.label));  // an in-place copy onto itself with nothing to scale: no launch
-            } else if (s.type == STEP_PASS) {
-                FftParams prm = s.prm;
-                const double scale = s.final_store ? p->scale[sc.inverse] : 1.0;
-                // views on the caller's buffers store a byte offset in seg[0].base (field f starts f field sizes further);
-                // in_user 2: a view that reads `out` (in-place plans)
-                auto user = [&](View& v, int which) {
-                    if (which == 1) v.seg[0].base = (char*)const_cast<void*>(in) + f * sc.field_in + (size_t)v.seg[0].base;
-                    if (which == 2) v.seg[0].base = (char*)out + f * sc.field_out + (size_t)v.seg[0].base;
-                };
-                user(prm.in, s.in_user);
-                user(prm.out, s.out_user);
-                FftParams prm_y = s.prm_y;
-                user(prm_y.in, s.y_in_user);
-                user(prm_y.out, s.y_out_user);
-                cudaError_t e = cudaErrorInvalidValue;
-                switch (s.kernel) {
-                    case KERNEL_PASS:
-                        e = is_copy(s.kind) ? launch_copy_pass(p->prec, is_r2r(p->g.transform), s.kind, s.n, prm, scale, ss)
-                                            : launch_fft_pass(p->prec, s.kind, s.n ? s.n : size_t(1) << s.log2n, prm, s.blu, scale, ss, s.r2r);
-                        break;
-                    case KERNEL_ZY_FUSED: e = launch_zy_fused(p->prec, s.log2n, prm, prm_y, s.zyf, scale, ss); break;
-                    case KERNEL_BATCH_SMALL:
-                        e = launch_batch_small(p->prec, s.log2n, prm.in.seg[0].base, prm.out.seg[0].base, (long long)p->batch, s.prm.inverse, s.bsf, scale, ss);
-                        break;
-                }
+            if (s.type == STEP_PASS) {
+                bool launched = false;
+                const cudaError_t e = run_pass_step(p, sc, s, f, out, in, ss, &launched);
                 if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("FFT pass launch failed: ") + cudaGetErrorString(e));
-                ++launches;
+                if (launched) ++launches;
                 CK_CUDA(mark(phase, 1, s.label));
             } else if (s.type == STEP_RENDEZVOUS) {
                 const std::vector<int>& G = p->grp[s.group];
@@ -3359,15 +3379,9 @@ static Tables& fft1d_tables(int prec) {
 // one pass of n-point lines over prm's views (R2C / C2R: n complex points), with the tables of its length; r2r: the kind of
 // R2R passes
 static int fft1d_pass(int prec, PassKind kind, size_t n, FftParams prm, void* stream, int r2r_k = DFFT_DCT) {
-    Tables& T = fft1d_tables(prec);
-    const bool blu = bluestein_length(n);
-    const bool r2r = (kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED) && r2r_k != DFFT_R2HC;  // with a w_k table
-    const int l2 = blu ? bluestein_log2m(n) : ilog2_exact(n);
     void *tw = nullptr, *tw2 = nullptr, *table = nullptr;
-    if (blu && T.get_blu(n, &table) != cudaSuccess) return fail(DFFT_ERR_CUDA, "Bluestein table allocation failed");
-    if (T.get_tw(l2, &tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
-    if ((kind == PASS_R2C || kind == PASS_C2R || r2r) && T.get_tw2(l2 + (r2r ? 1 : 0), &tw2) != cudaSuccess)
-        return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
+    const int rc = pass_tables(fft1d_tables(prec), kind, n, r2r_k, &tw, &tw2, &table);
+    if (rc) return rc;
     prm.tw = tw; prm.tw2 = tw2;
     cudaError_t e = launch_fft_pass(prec, kind, n, prm, table, 1.0, (cudaStream_t)stream, r2r_k);
     if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("launch failed: ") + cudaGetErrorString(e));
@@ -3434,6 +3448,100 @@ int dfft_fft1d_general(int precision, int direction, size_t n, size_t a0, size_t
     prm.in = single_view(const_cast<void*>(in), in_strides[0], in_strides[1], in_strides[2]);
     prm.out = single_view(out, out_strides[0], out_strides[1], out_strides[2]);
     return fft1d_pass(precision, PASS_C2C_TILED, n, prm, stream);
+}
+
+// One pass step of a geometry-only plan on the current device, for replaying every rank's schedule on one GPU.  Slot
+// addresses ((r+1) << 44) + off become work[r] + off, the caller's views are offsets into in / out as in an exec.  Every
+// segment's element range is checked against the buffer it lands in before anything is launched.
+int dfft_debug_run_step(dfft_plan_t p, int inverse, int d, size_t field, int step, void* const* work, size_t work_bytes, void* out,
+                        size_t out_bytes, const void* in, size_t in_bytes, void* stream) {
+    if (!p || d < 1 || d > 3 || !work) return fail(DFFT_ERR_INVALID, "bad arguments");
+    if (!p->comm->dry) return fail(DFFT_ERR_STATE, "only geometry-only plans (dfft_comm_create_dry) run single steps");
+    Schedule* scp = nullptr;
+    {
+        int rc = get_schedule(p, inverse, d, &scp);
+        if (rc) return rc;
+    }
+    const Schedule& sc = *scp;
+    if (step < 0 || size_t(step) >= sc.steps.size() || field >= (sc.whole_batch ? 1 : p->batch)) return fail(DFFT_ERR_INVALID, "no such step or field");
+    Step s = sc.steps[size_t(step)];
+    if (s.type != STEP_PASS || s.kernel != KERNEL_PASS) return fail(DFFT_ERR_UNSUPPORTED, "only single pass steps run on their own");
+    const size_t len = s.n ? s.n : size_t(1) << s.log2n;  // points per line (R2C / C2R: complex points of the real side)
+    if (!is_copy(s.kind)) {
+        void *tw = nullptr, *tw2 = nullptr, *blu = nullptr;
+        const int rc = pass_tables(fft1d_tables(p->prec), s.kind, len, s.r2r, &tw, &tw2, &blu);
+        if (rc) return rc;
+        s.prm.tw = tw;
+        s.prm.tw2 = tw2;
+        s.blu = blu;
+    }
+    // the views as the kernel sees them: slot addresses on the work areas, the caller's on in / out; each segment's range
+    struct Range { const char *lo, *hi, *buf; size_t bytes; };
+    std::vector<Range> ranges;
+    std::vector<std::pair<View*, const std::vector<unsigned char>*>> tables;
+    auto resolve = [&](View& v, int user, size_t n_len, View& launched) -> int {
+        if (v.nseg < 1 || v.nseg > MAXSEG || (user && v.nseg != 1)) return fail(DFFT_ERR_STATE, "internal: view segments");
+        const std::vector<unsigned char>* tab = nullptr;
+        if (v.nseg > 1) {
+            auto it = p->tabs.host_tabs.find(v.seg_of_n);
+            if (it == p->tabs.host_tabs.end() || it->second.size() < n_len) return fail(DFFT_ERR_STATE, "internal: segment table");
+            tab = &it->second;
+            tables.emplace_back(&launched, tab);
+        }
+        launched = v;
+        if (user) user_view(launched, user, sc, field, out, in);
+        for (int g = 0; g < v.nseg; ++g) {
+            Seg& sg = launched.seg[g];
+            const char* buf = user == 1 ? static_cast<const char*>(in) : static_cast<const char*>(out);
+            size_t bytes = user == 1 ? in_bytes : out_bytes;
+            if (!user) {
+                const unsigned long long a = (unsigned long long)v.seg[g].base, r = (a >> 44) - 1;
+                if ((a >> 44) == 0 || r >= (unsigned long long)p->P || !work[r]) return fail(DFFT_ERR_INVALID, "a view lies in no rank's work area");
+                buf = static_cast<const char*>(work[r]);
+                bytes = work_bytes;
+                sg.base = const_cast<char*>(buf) + (a & ((1ull << 44) - 1));
+            }
+            // n of this segment, then the lowest and highest element offset over (a0, a1, n, b)
+            long long n_lo = -1, n_hi = -1;
+            for (size_t n = 0; n < n_len; ++n)
+                if (v.nseg == 1 || (*tab)[n] == g) { if (n_lo < 0) n_lo = (long long)n; n_hi = (long long)n; }
+            if (n_lo < 0 || s.prm.A0 <= 0 || s.prm.A1 <= 0 || s.prm.B <= 0) continue;  // the segment holds no element
+            long long lo = 0, hi = s.prm.B - 1;
+            for (const long long t : {(long long)(s.prm.A0 - 1) * sg.sA0, (long long)(s.prm.A1 - 1) * sg.sA1}) { lo += std::min(0ll, t); hi += std::max(0ll, t); }
+            const long long t0 = (n_lo - sg.n0) * v.sN, t1 = (n_hi - sg.n0) * v.sN;
+            lo += std::min(t0, t1);
+            hi += std::max(t0, t1);
+            const char* b = static_cast<const char*>(sg.base);
+            ranges.push_back({b + lo * (long long)p->esize, b + (hi + 1) * (long long)p->esize, buf, bytes});
+        }
+        return DFFT_SUCCESS;
+    };
+    const size_t in_len = len + (s.kind == PASS_C2R ? 1 : 0), out_len = len + (s.kind == PASS_R2C ? 1 : 0);
+    Step t = s;  // the step with resolved views: its user flags are cleared, so run_pass_step leaves them as they are
+    t.in_user = t.out_user = 0;
+    int rc = resolve(s.prm.in, s.in_user, in_len, t.prm.in);
+    if (!rc) rc = resolve(s.prm.out, s.out_user, out_len, t.prm.out);
+    if (rc) return rc;
+    for (const Range& r : ranges)
+        if (!r.buf || r.lo < r.buf || r.hi > r.buf + r.bytes)
+            return fail(DFFT_ERR_INVALID, "a view reaches outside the buffer it lies in");
+    // segment tables of multi-segment views: uploaded for this call
+    std::vector<void*> dev;
+    auto release = [&]() { for (void* q : dev) cudaFree(q); };
+    for (auto& vt : tables) {
+        void* q = nullptr;
+        cudaError_t e = cudaMalloc(&q, vt.second->size());
+        if (e == cudaSuccess) dev.push_back(q);
+        if (e == cudaSuccess) e = cudaMemcpy(q, vt.second->data(), vt.second->size(), cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) { release(); return fail(DFFT_ERR_CUDA, std::string("segment table upload: ") + cudaGetErrorString(e)); }
+        vt.first->seg_of_n = static_cast<const unsigned char*>(q);
+    }
+    bool launched = false;
+    cudaError_t e = run_pass_step(p, sc, t, field, out, in, (cudaStream_t)stream, &launched);
+    if (e == cudaSuccess) e = cudaStreamSynchronize((cudaStream_t)stream);
+    release();
+    if (e != cudaSuccess) return fail(DFFT_ERR_CUDA, std::string("pass step: ") + cudaGetErrorString(e));
+    return DFFT_SUCCESS;
 }
 
 }  // extern "C"

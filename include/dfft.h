@@ -354,6 +354,19 @@ int dfft_fft1d_r2r(int precision, int transform, int direction, size_t n, size_t
  * the data movement of any rank count with numpy (tests/test_schedule_emulation.py). */
 int dfft_comm_create_dry(int rank, int nranks, dfft_comm_t* comm);
 int dfft_plan_describe(dfft_plan_t plan, int inverse, int d, char* buf, size_t capacity, size_t* needed);
+/* Runs one pass step of a geometry-only plan's schedule on the current device, with the kernels and parameters an exec
+ * launches for it (tables, tile choice, CTA limit, output scale), then synchronises `stream`.  With the steps of every rank
+ * run in lock step and the all-to-all steps done as copies, one GPU replays a multi-rank exec
+ * (tests/test_gpu_schedule_replay.py).
+ *   - step indexes the schedule of (inverse, d), field the field of a per-field batched plan: item i of
+ *     dfft_plan_describe's list is (field i / steps, step i % steps).
+ *   - work[r] is rank r's work area of work_bytes bytes (P entries): a slot address ((r+1) << 44) + off maps to
+ *     work[r] + off.  Views on the caller's buffers are offsets into in / out (in_bytes / out_bytes), as in an exec.
+ *   - Every element of both views must lie inside the buffer it maps to; otherwise DFFT_ERR_INVALID and nothing runs.
+ *   - Rendezvous and all-to-all steps, the fused z + y stage and the batched stage: DFFT_ERR_UNSUPPORTED.  A plan not made
+ *     on dfft_comm_create_dry: DFFT_ERR_STATE. */
+int dfft_debug_run_step(dfft_plan_t plan, int inverse, int d, size_t field, int step, void* const* work, size_t work_bytes,
+                        void* out, size_t out_bytes, const void* in, size_t in_bytes, void* stream);
 
 /* Batched 1D C2C along n of element (i0, i1, n, ib) at  i0*strides[0] + i1*strides[1] + n*strides[2] + ib
  * (elements; ib contiguous, extents a0 x a1 x n x b) — the general strided view the plan's passes use. */
