@@ -55,6 +55,10 @@ SIGNATURES = {
     "dfft_plan_create_r2r": (C.c_int, [C.c_void_p, C.POINTER(dfft_config), C.c_int, C.c_int, C.POINTER(C.c_int), C.c_size_t, C.c_size_t,
                                        C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     "dfft_plan_get_r2r_kinds": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
+    "dfft_plan_create_padded": (C.c_int, [C.c_void_p, C.POINTER(dfft_config), C.c_int, C.c_int, C.c_int, C.c_size_t, C.c_size_t,
+                                          C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                          C.c_int, C.POINTER(C.c_void_p)]),
+    "dfft_plan_get_spectral_size": (C.c_int, [C.c_void_p, C.POINTER(C.c_size_t)]),
     "dfft_plan_set_scale": (C.c_int, [C.c_void_p, C.c_double, C.c_double]),
     "dfft_plan_get_scale": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "dfft_plan_destroy": (C.c_int, [C.c_void_p]),

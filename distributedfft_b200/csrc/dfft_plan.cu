@@ -102,9 +102,19 @@ static bool r2r_length(size_t n) { return ilog2_exact(n) >= 1 && ilog2_exact(n) 
 // One FFT pass of n-point lines (R2C / C2R: n complex points) over the views of prm, its stores scaled by `scale`: the
 // power-of-two kernels, or the Bluestein pass when n is not a power of two (prm.tw: the M-point table; blu: the Bluestein
 // table of n).  PASS_R2R_*: the R2R kernel of kind r2r (DFFT_DCT, DFFT_DST with prm.tw2 its w_k table, or DFFT_R2HC).
+// hole: passes of padded plans that keep part of their spectral side, the hole [hole[0], hole[1]) of their lines
+// (pass_hole); the padded twin of the power-of-two kernel runs then.
 static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftParams& prm, const void* blu, double scale, cudaStream_t stream,
-                                   int r2r = DFFT_DCT) {
+                                   int r2r = DFFT_DCT, const int* hole = nullptr) {
     const int log2n = ilog2_exact(n);
+    if (hole && log2n >= 0) {
+        FftPadded q;
+        static_cast<FftParams&>(q) = prm;
+        q.scale = scale;
+        q.lo = hole[0];
+        q.hi = hole[1];
+        return launch_padded(prec, log2n, kind, q, stream);
+    }
     if (kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED) {
         FftR2r r;
         static_cast<FftParams&>(r) = prm;
@@ -122,6 +132,16 @@ static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftP
     b.chirp = blu ? static_cast<const char*>(blu) + (size_t(1) << log2m) * (prec == DFFT_F64 ? 16 : 8) : nullptr;
     b.scale = scale;
     return launch_bluestein(prec, log2m, kind, b, stream);
+}
+
+// The hole of a pass of n-point lines (R2C / C2R: n complex points, n + 1 spectral ones) that keeps `keep` points of its
+// spectral side (0: all of them).  C2C: frequencies 0 .. ceil(K/2) - 1 and the K - ceil(K/2) negative ones, at the end of
+// the line (numpy's fftfreq(K) * K mod N); R2C / C2R: k = 0 .. keep - 1.
+static void pass_hole(PassKind kind, size_t n, size_t keep, int hole[2]) {
+    const bool half = kind == PASS_R2C || kind == PASS_C2R;
+    const size_t full = half ? n + 1 : n, k = keep ? keep : full;
+    hole[0] = int(half ? k : (k + 1) / 2);
+    hole[1] = int(hole[0] + full - k);
 }
 
 // Passes over an axis the plan keeps (dfft_plan_set_transform_axes): the views of the FFT pass they replace, no transform
@@ -317,6 +337,9 @@ struct Step {
     bool bluestein() const { return !is_copy(kind) && n != 0 && n != (size_t(1) << log2n); }
     int r2r = 0;  // PASS_R2R_*: the kind of the axis it transforms (DFFT_DCT, DFFT_DST or DFFT_R2HC)
     int axis = 0;  // the axis of the pass: 0 x, 1 y, 2 z (PASS_COPY_*: n is its length, log2n 0)
+    // padded plans: the points its spectral side keeps of each line (Kx, Ky, Kz; R2C / C2R: Kz/2 + 1 of the Nz/2 + 1), the
+    // rest is the hole (fft_kernels.cuh, FftPadded); 0: the whole line
+    size_t keep = 0;
     FftParams prm{};
     int in_user = 0, out_user = 0;  // 1: patch seg[0].base with the caller's in, 2: with the caller's out
     // RENDEZVOUS
@@ -509,6 +532,10 @@ static bool pow2_axes(const dfft_plan_s* p) { return ilog2_exact(p->g.nx) > 0 &&
 // Whether every axis is transformed.  Plans with a kept axis (dfft_plan_set_transform_axes) run the sequential schedule
 // only: the overlapped schedules, the fused z + y stage and the batched stage transform every axis they touch.
 static bool all_axes(const dfft_plan_s* p) { return p->taxes[0] && p->taxes[1] && p->taxes[2]; }
+// Whether the schedules may take another form than the sequential one: the overlapped schedules, the fused z + y stage and
+// the batched stage build their passes for power-of-two lengths, every axis transformed and no padding (their kernels have
+// no padded twins, FftPadded).
+static bool alt_schedules(const dfft_plan_s* p) { return pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p) && !p->g.padded(); }
 
 // Row pitch, in elements (complex units; reals for DCT / DST plans), of the z-contiguous side of the caller's buffers that
 // holds Nz points per row: the input of forward passes, the output of inverse ones.  Real rows of R2C / C2R plans are Nz reals (Nz/2 units) apart, or, in
@@ -523,7 +550,7 @@ static long long z_row_pitch(const dfft_plan_s* p) {
 // three passes are L2-resident already and gain nothing.
 static bool zy_fused(const dfft_plan_s* p, int inverse, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p)) return false;
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded()) return false;
     if (g.ny != g.nz || !zy_fused_length(ilog2_exact(g.ny))) return false;
     // the fused stage reads and writes the blocked hand-over layout of the x pass
     if (p->blocked_ch <= 0 || g.nz % size_t(p->blocked_ch) || (inverse && !p->blocked_inv)) return false;
@@ -577,7 +604,7 @@ static int fuse_zy(dfft_plan_s* p, Step zs, const Step& ys, const char* label, c
 constexpr size_t BATCH_SMALL_MIN = 2;
 static bool batch_small(const dfft_plan_s* p, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p)) return false;
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded()) return false;
     if (g.nx != g.ny || g.ny != g.nz || !batch_small_length(ilog2_exact(g.nx))) return false;
     return p->batch >= BATCH_SMALL_MIN && p->batch * g.nx <= 0x7fffffff;
 }
@@ -655,6 +682,10 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         s.phase = phase;
         s.log2n = pass_log2(kind, n);  // Bluestein lengths: the view mapping stays the kind's; the exec launches the Bluestein kernel
         s.n = n;
+        {   // padded plans: the spectral extent of the axis
+            const size_t k = axis == 0 ? g.kx : axis == 1 ? g.ky : g.kzc, full = axis == 0 ? g.nx : axis == 1 ? g.ny : g.nzc;
+            if (k != full) s.keep = k;
+        }
         if (s.log2n < 1 || s.log2n > MAX_LOG2N)
             return fail(DFFT_ERR_UNSUPPORTED, "axis length " + std::to_string(n) + " is not a supported power of two (2..8192)");
         s.prm.A0 = 1; s.prm.A1 = 1; s.prm.B = 1;
@@ -696,7 +727,8 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
 
     if (p->any_direct) rendezvous(0, 0, nullptr);  // everyone has left the previous exec: slots are free
 
-    const size_t nzc = g.nzc;
+    // spectral extents (padded plans: K; the pass lengths stay the physical N)
+    const size_t kzc = g.kzc, ky = g.ky, kx = g.kx;
     const bool zyx = g.decomp == DFFT_SLAB_Z_THEN_YX;
     const bool zy = zy_fused(p, inverse, d);  // one fused launch for the z and y passes
     int rc;
@@ -705,7 +737,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     const size_t nx_i = g.sx.size[pi], x0_i = g.sx.start[pi];
     const size_t ny_j = zyx ? g.ny : g.sy.size[pj], y0_j = zyx ? 0 : g.sy.start[pj];
     const size_t nz_j = zyx ? g.sz.size[me] : g.sz.size[pj], z0_j = zyx ? g.sz.start[me] : g.sz.start[pj];
-    const size_t oy_i = zyx ? g.ny : g.oy.size[pi], oy0_i = zyx ? 0 : g.oy.start[pi];
+    const size_t oy_i = zyx ? ky : g.oy.size[pi], oy0_i = zyx ? 0 : g.oy.start[pi];
     (void)x0_i; (void)y0_j; (void)z0_j; (void)oy0_i;
 
     const unsigned char *tab_z = nullptr, *tab_y_in = nullptr, *tab_y_out = nullptr, *tab_x = nullptr;
@@ -745,7 +777,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
             s1.in_user = 1;
         }
         if (d == 1) {
-            s1.prm.out = single_view(nullptr, (long long)(ny_j * nzc), (long long)nzc, 1);
+            s1.prm.out = single_view(nullptr, (long long)(ny_j * kzc), (long long)kzc, 1);
             s1.out_user = 2;
             sc.steps.push_back(s1);
             sc.built = true;
@@ -806,13 +838,14 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         }
         if (d == 2 || zyx) {
             if (d == 2) {
-                s2.prm.out = single_view(nullptr, (long long)(g.ny * nz_j), 0, (long long)nz_j);
+                s2.prm.out = single_view(nullptr, (long long)(ky * nz_j), 0, (long long)nz_j);
                 s2.out_user = 2;
                 sc.steps.push_back(s2);
                 sc.built = true;
                 return DFFT_SUCCESS;
             }
-            // z_then_yx: y pass in place, then x pass into the caller's out
+            // z_then_yx: y pass in place (padded: its Ky output rows keep the input's strides, the first Ky * nz_j elements of
+            // every x plane), then x pass into the caller's out
             s2.prm.out = s2.prm.in;
             if (s2.prm.in.nseg != 1) return fail(DFFT_ERR_STATE, "internal: z_then_yx gather view");
             sc.steps.push_back(s2);
@@ -820,9 +853,9 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
             rc = new_pass(PASS_C2C_TILED, g.nx, 0, "2D FFT Y-X-Direction", s3);
             if (rc) return rc;
             s3.label = "x pass";
-            s3.prm.A0 = 1; s3.prm.A1 = 1; s3.prm.B = int(g.ny * nz_j);
+            s3.prm.A0 = 1; s3.prm.A1 = 1; s3.prm.B = int(ky * nz_j);
             s3.prm.in = single_view(s2.prm.in.seg[0].base, 0, 0, (long long)(g.ny * nz_j));
-            s3.prm.out = single_view(nullptr, 0, 0, (long long)(g.ny * nz_j));
+            s3.prm.out = single_view(nullptr, 0, 0, (long long)(ky * nz_j));
             s3.out_user = 2;
             sc.steps.push_back(s3);
             sc.built = true;
@@ -843,7 +876,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         Step s2t;
         bool have_tail = false;
         if (dir2 && CH) {
-            // blocked hand-over: receiver q holds [nzc/CH][nx][ny_q][CH] — the rows a y-pass tile sends to one
+            // blocked hand-over: receiver q holds [kzc/CH][nx][ny_q][CH] — the rows a y-pass tile sends to one
             // destination (consecutive y) are adjacent, so every warp store is 512 contiguous bytes
             s2.prm.A1 = int(nzm / CH); s2.prm.B = int(CH);
             s2.prm.in.seg[0].sA1 = (long long)CH;
@@ -860,7 +893,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
                     return mkseg(eptr(slotp(D2, r), x0_i * nyq * CH, es), (long long)(nyq * CH), (long long)(g.nx * nyq * CH), (long long)CH, g.oy.start[q]);
                 });
             }
-            if (any_rem) {  // leftover columns z in [nzm, nzc): plain layout [nx][ny_q][rem] behind the blocked part
+            if (any_rem) {  // leftover columns z in [nzm, kzc): plain layout [nx][ny_q][rem] behind the blocked part
                 s2t = s2;
                 have_tail = true;
                 s2t.label = "y pass (tail)";
@@ -905,7 +938,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         if (rc) return rc;
         s3.label = "x pass";
         if (CH) {
-            // in: [nzc/CH][nx][oy_i][CH]: a0 = y_loc, a1 = z chunk, n = x
+            // in: [kzc/CH][nx][oy_i][CH]: a0 = y_loc, a1 = z chunk, n = x
             s3.prm.A0 = int(oy_i); s3.prm.A1 = int(nzm / CH); s3.prm.B = int(CH);
             if (G2.size() == 1 && p->single_rank_layout)
                 s3.prm.in = single_view(slotp(D2, me), (long long)((nzm / CH) * g.nx * CH), (long long)(g.nx * CH), (long long)CH);
@@ -945,7 +978,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         rc = new_pass(zkind, zlen, 2, "1D FFT Z-Direction", s);
         if (rc) return rc;
         s.prm.A0 = int(nx_i); s.prm.A1 = int(ny_j);
-        s.prm.in = single_view(nullptr, (long long)(ny_j * nzc), (long long)nzc, 1);
+        s.prm.in = single_view(nullptr, (long long)(ny_j * kzc), (long long)kzc, 1);
         s.in_user = 1;
         s.prm.out = single_view(nullptr, zpitch_out * (long long)ny_j, zpitch_out, 1);
         s.out_user = 2;
@@ -956,17 +989,17 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
 
     if (zyx) {
         // input [nx][ny][nz_me]: y pass (to a slot), x pass scattering along x to the owners of x,
-        // then z inverse on [nx_me][ny][nzc].
+        // then z inverse on [nx_me][ny][kzc].
         Step sy_;
         rc = new_pass(PASS_C2C_TILED, g.ny, 1, nullptr, sy_);
         if (rc) return rc;
         sy_.label = "y pass";
         const int W = dir1 ? D2 : SR;  // a local scratch slot that is not the transposition target
-        // one rank with x kept: the y pass leaves [nx][ny][nzc] in D1, where the z pass reads it, and no x copy runs (the
+        // one rank with x kept: the y pass leaves [nx][ny][kzc] in D1, where the z pass reads it, and no x copy runs (the
         // other decompositions run their d = 2 steps instead, get_schedule)
         const bool no_x = P == 1 && !p->taxes[0];
-        sy_.prm.A0 = int(g.nx); sy_.prm.B = int(nz_j);
-        sy_.prm.in = single_view(nullptr, (long long)(g.ny * nz_j), 0, (long long)nz_j);
+        sy_.prm.A0 = int(kx); sy_.prm.B = int(nz_j);
+        sy_.prm.in = single_view(nullptr, (long long)(ky * nz_j), 0, (long long)nz_j);
         sy_.in_user = 1;
         sy_.prm.out = single_view(slotp(no_x ? D1 : W, me), (long long)(g.ny * nz_j), 0, (long long)nz_j);
         sc.steps.push_back(sy_);
@@ -979,7 +1012,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         Step xa;
         if (dir1) {
             seg_view(sx_.prm.out, tab_x, G1, [&](int q, int r) {
-                return mkseg(eptr(slotp(D1, r), z0_j, es), 0, (long long)nzc, (long long)(g.ny * nzc), g.sx.start[q]);
+                return mkseg(eptr(slotp(D1, r), z0_j, es), 0, (long long)kzc, (long long)(g.ny * kzc), g.sx.start[q]);
             });
         } else {
             a2a_counts(xa, G1, [&](int q) { return g.sx.size[q] * g.ny * nz_j; }, [&](int q) { return nx_i * g.ny * g.sz.size[q]; });
@@ -994,7 +1027,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         rc = new_pass(zkind, zlen, 2, "1D FFT Z-Direction", sz_);
         if (rc) return rc;
         sz_.prm.A0 = int(nx_i); sz_.prm.A1 = int(g.ny);
-        if (dir1) sz_.prm.in = single_view(slotp(D1, me), (long long)(g.ny * nzc), (long long)nzc, 1);
+        if (dir1) sz_.prm.in = single_view(slotp(D1, me), (long long)(g.ny * kzc), (long long)kzc, 1);
         else
             seg_view(sz_.prm.in, tab_z, G1, [&](int q, int) {
                 const size_t nzq = g.sz.size[q];
@@ -1032,7 +1065,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         s3.prm.bulk_out = G2.size() > 1 ? p->bulk_store : 0;
         seg_view(s3.prm.out, tab_x, G2, [&](int q, int r) {
             const size_t nxq = g.sx.size[q];
-            return mkseg(eptr(slotp(D2, r), oy0_i * nxq * CH, es), (long long)(nxq * CH), (long long)(g.ny * nxq * CH), (long long)CH, g.sx.start[q]);
+            return mkseg(eptr(slotp(D2, r), oy0_i * nxq * CH, es), (long long)(nxq * CH), (long long)(ky * nxq * CH), (long long)CH, g.sx.start[q]);
         });
         Step s3t;
         if (any_rem) {  // leftover columns: plain [nx_q][ny][rem] behind the blocked part
@@ -1044,7 +1077,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
             s3t.prm.in = single_view((void*)(size_t)(nzm * es), (long long)nz_j, 0, (long long)(oy_i * nz_j));
             seg_view(s3t.prm.out, tab_x, G2, [&](int q, int r) {
                 const size_t nxq = g.sx.size[q];
-                return mkseg(eptr(slotp(D2, r), g.ny * nxq * nzm + oy0_i * rem, es), (long long)rem, 0, (long long)(g.ny * rem), g.sx.start[q]);
+                return mkseg(eptr(slotp(D2, r), ky * nxq * nzm + oy0_i * rem, es), (long long)rem, 0, (long long)(ky * rem), g.sx.start[q]);
             });
             const char* ph = s3.phase; s3.phase = nullptr; s3t.phase = ph;
             sc.steps.push_back(s3);
@@ -1059,22 +1092,22 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         if (rc) return rc;
         s2.label = "y pass";
         s2.prm.A0 = int(nx_i); s2.prm.A1 = int(nzm / CH); s2.prm.B = int(CH);
-        s2.prm.in = single_view(slotp(D2, me), (long long)CH, (long long)(g.ny * nx_i * CH), (long long)(nx_i * CH));
+        s2.prm.in = single_view(slotp(D2, me), (long long)CH, (long long)(ky * nx_i * CH), (long long)(nx_i * CH));
         if (G1.size() > 1) s2.prm.tile_pref = p->xchg_tile_pref;
         else s2.prm.tile_pref = 1;
         seg_view(s2.prm.out, tab_y_in, G1, [&](int q, int r) {
             const size_t nyq = g.sy.size[q];
-            return mkseg(eptr(slotp(D1, r), z0_j, es), (long long)(nyq * nzc), (long long)CH, (long long)nzc, g.sy.start[q]);
+            return mkseg(eptr(slotp(D1, r), z0_j, es), (long long)(nyq * kzc), (long long)CH, (long long)kzc, g.sy.start[q]);
         });
         if (any_rem) {
             Step s2t = s2;
             s2t.label = "y pass (tail)";
             s2t.phase = nullptr;
             s2t.prm.A0 = int(nx_i); s2t.prm.A1 = 1; s2t.prm.B = int(rem);
-            s2t.prm.in = single_view(eptr(slotp(D2, me), g.ny * nx_i * nzm, es), (long long)(g.ny * rem), 0, (long long)rem);
+            s2t.prm.in = single_view(eptr(slotp(D2, me), ky * nx_i * nzm, es), (long long)(ky * rem), 0, (long long)rem);
             seg_view(s2t.prm.out, tab_y_in, G1, [&](int q, int r) {
                 const size_t nyq = g.sy.size[q];
-                return mkseg(eptr(slotp(D1, r), z0_j + nzm, es), (long long)(nyq * nzc), 0, (long long)nzc, g.sy.start[q]);
+                return mkseg(eptr(slotp(D1, r), z0_j + nzm, es), (long long)(nyq * kzc), 0, (long long)kzc, g.sy.start[q]);
             });
             const char* ph = s2.phase; s2.phase = nullptr; s2t.phase = ph;
             sc.steps.push_back(s2);
@@ -1087,7 +1120,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         rc = new_pass(zkind, zlen, 2, slab ? "2D FFT Y-Z-Direction" : "1D FFT Z-Direction", s1);
         if (rc) return rc;
         s1.prm.A0 = int(nx_i); s1.prm.A1 = int(ny_j);
-        s1.prm.in = single_view(slotp(D1, me), (long long)(ny_j * nzc), (long long)nzc, 1);
+        s1.prm.in = single_view(slotp(D1, me), (long long)(ny_j * kzc), (long long)kzc, 1);
         s1.prm.out = single_view(nullptr, zpitch_out * (long long)ny_j, zpitch_out, 1);
         s1.out_user = 2;
         if (zy) {
@@ -1114,9 +1147,9 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         s3.in_user = 1;
         if (dir2 && G2.size() > 1) s3.prm.tile_pref = p->xchg_tile_pref;
         if (dir2) {
-            // dest (q,j) holds [nx_q][ny][nz_j]; my rows y in [oy0_i, +oy_i)
+            // dest (q,j) holds [nx_q][ky][nz_j]; my rows y in [oy0_i, +oy_i)
             seg_view(s3.prm.out, tab_x, G2, [&](int q, int r) {
-                return mkseg(eptr(slotp(D2, r), oy0_i * nz_j, es), 0, 0, (long long)(g.ny * nz_j), g.sx.start[q]);
+                return mkseg(eptr(slotp(D2, r), oy0_i * nz_j, es), 0, 0, (long long)(ky * nz_j), g.sx.start[q]);
             });
         } else {
             a2a_counts(x2, G2, [&](int q) { return g.sx.size[q] * oy_i * nz_j; }, [&](int q) { return nx_i * g.oy.size[q] * nz_j; });
@@ -1129,17 +1162,17 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         else if (G2.size() > 1) rendezvous(2, 2, slab ? "Transpose (Finished Receive)" : "Second Transpose (Finished Receive)");
         have_in_slot = true;
     }
-    // y pass on [nx_i][ny][nz_j]
+    // y pass on [nx_i][ky][nz_j]
     Step s2;
     rc = new_pass(PASS_C2C_TILED, g.ny, 1, slab ? nullptr : "1D FFT Y-Direction", s2);
     if (rc) return rc;
     s2.label = "y pass";
     s2.prm.A0 = int(nx_i); s2.prm.A1 = 1; s2.prm.B = int(nz_j);
     if (!have_in_slot) {
-        s2.prm.in = single_view(nullptr, (long long)(g.ny * nz_j), 0, (long long)nz_j);
+        s2.prm.in = single_view(nullptr, (long long)(ky * nz_j), 0, (long long)nz_j);
         s2.in_user = 1;
     } else if (dir2) {
-        s2.prm.in = single_view(slotp(D2, me), (long long)(g.ny * nz_j), 0, (long long)nz_j);
+        s2.prm.in = single_view(slotp(D2, me), (long long)(ky * nz_j), 0, (long long)nz_j);
     } else {
         seg_view(s2.prm.in, tab_y_out, G2, [&](int q, int) {
             const size_t nyq = g.oy.size[q];
@@ -1149,10 +1182,10 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     Step x1;
     if (dir1 && G1.size() > 1) s2.prm.tile_pref = p->xchg_tile_pref;
     if (dir1) {
-        // dest (i,q) holds [nx_i][ny_q][nzc]; my columns z in [z0_j, +nz_j)
+        // dest (i,q) holds [nx_i][ny_q][kzc]; my columns z in [z0_j, +nz_j)
         seg_view(s2.prm.out, tab_y_in, G1, [&](int q, int r) {
             const size_t nyq = g.sy.size[q];
-            return mkseg(eptr(slotp(D1, r), z0_j, es), (long long)(nyq * nzc), 0, (long long)nzc, g.sy.start[q]);
+            return mkseg(eptr(slotp(D1, r), z0_j, es), (long long)(nyq * kzc), 0, (long long)kzc, g.sy.start[q]);
         });
     } else {
         a2a_counts(x1, G1, [&](int q) { return nx_i * g.sy.size[q] * nz_j; }, [&](int q) { return nx_i * ny_j * g.sz.size[q]; });
@@ -1164,12 +1197,12 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     sc.steps.push_back(s2);
     if (!dir1) { x1.phase = "First Transpose (Finished All2All)"; x1.group = 1; sc.steps.push_back(x1); }
     else if (G1.size() > 1) rendezvous(1, 1, "First Transpose (Finished Receive)");
-    // z pass on [nx_i][ny_j][nzc]
+    // z pass on [nx_i][ny_j][kzc]
     Step s1;
     rc = new_pass(zkind, zlen, 2, slab ? "2D FFT Y-Z-Direction" : "1D FFT Z-Direction", s1);
     if (rc) return rc;
     s1.prm.A0 = int(nx_i); s1.prm.A1 = int(ny_j);
-    if (dir1) s1.prm.in = single_view(slotp(D1, me), (long long)(ny_j * nzc), (long long)nzc, 1);
+    if (dir1) s1.prm.in = single_view(slotp(D1, me), (long long)(ny_j * kzc), (long long)kzc, 1);
     else
         seg_view(s1.prm.in, tab_z, G1, [&](int q, int) {
             const size_t nzq = g.sz.size[q];
@@ -2020,8 +2053,14 @@ static cudaError_t run_pass_step(const dfft_plan_s* p, const Schedule& sc, const
     cudaError_t e = cudaErrorInvalidValue;
     switch (s.kernel) {
         case KERNEL_PASS:
-            e = is_copy(s.kind) ? launch_copy_pass(p->prec, is_r2r(p->g.transform), s.kind, s.n, prm, scale, ss)
-                                : launch_fft_pass(p->prec, s.kind, s.n ? s.n : size_t(1) << s.log2n, prm, s.blu, scale, ss, s.r2r);
+            if (is_copy(s.kind)) {
+                e = launch_copy_pass(p->prec, is_r2r(p->g.transform), s.kind, s.n, prm, scale, ss);
+            } else {
+                const size_t n = s.n ? s.n : size_t(1) << s.log2n;
+                int hole[2];
+                pass_hole(s.kind, n, s.keep, hole);
+                e = launch_fft_pass(p->prec, s.kind, n, prm, s.blu, scale, ss, s.r2r, s.keep ? hole : nullptr);
+            }
             break;
         case KERNEL_ZY_FUSED: e = launch_zy_fused(p->prec, s.log2n, prm, prm_y, s.zyf, scale, ss); break;
         case KERNEL_BATCH_SMALL:
@@ -2306,14 +2345,14 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
         const bool streams = p->cfg.send_method == DFFT_SEND_STREAMS || (p->g.decomp == DFFT_PENCIL && p->cfg.send_method2 == DFFT_SEND_STREAMS);
         const bool seq_won = p->tuned_seq[inverse ? 1 : 0] != 0;
         const bool want_overlap = streams && d == 3 && p->P > 1 && p->g.decomp == DFFT_SLAB_ZY_THEN_X && p->direct2 && p->xchg_ctas >= 0 && !seq_won &&
-                                  pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p);
+                                  alt_schedules(p);
         // pencil: forward on a grid with two real transpositions by default; every other
         // combination (inverse, p1 or p2 == 1) only once dfft_plan_tune has measured it faster than the sequential schedule
         const bool both_multi = p->grp[1].size() > 1 && p->grp[2].size() > 1;
         const bool tuned = p->tuned_ctas[inverse ? 1 : 0] != -2;
         const bool want_pencil_overlap = streams && d == 3 && p->g.decomp == DFFT_PENCIL && p->direct1 && p->direct2 && p->P > 1 && p->xchg_ctas >= 0 &&
                                          pencil_overlap_enabled() && !seq_won && ((both_multi && !inverse) || tuned || pencil_overlap_mode() == 2) &&
-                                         pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p);
+                                         alt_schedules(p);
         // one rank with x kept: the layout after d = 2 is the output layout, so d = 3 runs the d = 2 steps (no x copy)
         const int db = p->P == 1 && !p->taxes[0] && d == 3 ? 2 : d;
         int rc;
@@ -2564,10 +2603,11 @@ int dfft_plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, in
 
 }  // extern "C"
 
-// kinds: of the plans of dfft_plan_create_r2r (their transform is DFFT_DCT, DFFT_DST or DFFT_R2HC), nullptr otherwise
+// kinds: of the plans of dfft_plan_create_r2r (their transform is DFFT_DCT, DFFT_DST or DFFT_R2HC), nullptr otherwise.
+// spectral: Kx, Ky, Kz of the plans of dfft_plan_create_padded (checked there), nullptr otherwise.
 static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
                        size_t nz, size_t p1, size_t p2, size_t batch, bool inplace, int allocate, dfft_plan_t* plan,
-                       const int* kinds = nullptr) {
+                       const int* kinds = nullptr, const size_t* spectral = nullptr) {
     if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
     if (batch == 0) return fail(DFFT_ERR_INVALID, "batch must be at least 1");
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
@@ -2591,7 +2631,7 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
     p->esize = (precision == DFFT_F64 ? 16 : 8) / (is_r2r(transform) ? 2 : 1);  // DCT / DST: real elements
     p->tabs.prec = precision;
     p->tabs.dry = dry;
-    if (!p->g.init(decomp, transform, nx, ny, nz, p1, p2, p->P)) {
+    if (!p->g.init(decomp, transform, nx, ny, nz, p1, p2, p->P, spectral ? spectral[0] : 0, spectral ? spectral[1] : 0, spectral ? spectral[2] : 0)) {
         delete p;
         return fail(DFFT_ERR_INVALID, "invalid partition: P1*P2 must equal the communicator size");
     }
@@ -2703,7 +2743,7 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
         // DCT / DST: the R2R tile holds that many column pairs, so the block is twice as many reals wide
         if (is_r2r(transform)) ch = int(2 * std::max(tile_cols(ny), tile_cols(nx)));
         if (eb) ch = atoi(eb);
-        size_t min_nz = g.nzc;  // smallest z extent any rank holds between the y and x passes
+        size_t min_nz = g.kzc;  // smallest z extent any rank holds between the y and x passes
         if (decomp == DFFT_PENCIL)
             for (size_t v : g.sz.size) min_nz = std::min(min_nz, v);
         p->blocked_ch = ((decomp == DFFT_SLAB_ZY_THEN_X || decomp == DFFT_PENCIL) && ch > 0 && min_nz >= size_t(4 * ch)) ? ch : 0;
@@ -2780,6 +2820,27 @@ int dfft_plan_create_inplace(dfft_comm_t comm, const dfft_config* config, int de
 }
 
 int dfft_plan_is_inplace(dfft_plan_t p) { return p && p->inplace ? 1 : 0; }
+
+int dfft_plan_create_padded(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
+                            size_t nz, size_t kx, size_t ky, size_t kz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan) {
+    if (transform == DFFT_DCT || transform == DFFT_DST) return fail(DFFT_ERR_UNSUPPORTED, "padded plans are C2C or R2C / C2R");
+    if (transform != DFFT_C2C && transform != DFFT_R2C) return fail(DFFT_ERR_INVALID, "bad transform");
+    const size_t n[3] = {nx, ny, nz}, k[3] = {kx, ky, kz};
+    for (int a = 0; a < 3; ++a) {
+        if (k[a] == 0 || k[a] > n[a])
+            return fail(DFFT_ERR_INVALID, "spectral size " + std::to_string(k[a]) + " of axis " + "xyz"[a] + " must be in [1, " + std::to_string(n[a]) + "]");
+        if (k[a] < n[a] && ilog2_exact(n[a]) < 0)
+            return fail(DFFT_ERR_UNSUPPORTED, std::string("axis ") + "xyz"[a] + " of length " + std::to_string(n[a]) +
+                                                  " is not a power of two: its spectral size must be its length");
+    }
+    return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, false, allocate, plan, nullptr, k);
+}
+
+int dfft_plan_get_spectral_size(dfft_plan_t p, size_t k[3]) {
+    if (!p || !k) return fail(DFFT_ERR_INVALID, "null plan / size");
+    k[0] = p->g.kx; k[1] = p->g.ky; k[2] = p->g.kz;
+    return DFFT_SUCCESS;
+}
 
 int dfft_plan_create_r2r(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, const int kinds[3], size_t nx, size_t ny,
                          size_t nz, size_t p1, size_t p2, size_t batch, int inplace, int allocate, dfft_plan_t* plan) {
@@ -2931,6 +2992,8 @@ int dfft_plan_set_transform_axes(dfft_plan_t p, const int transform[3]) {
     for (int a = 0; a < 3; ++a)
         if (transform[a] != 0 && transform[a] != 1) return fail(DFFT_ERR_INVALID, "transform axes must be 0 (keep) or 1 (transform)");
     if (p->g.transform == DFFT_R2C && !transform[2]) return fail(DFFT_ERR_INVALID, "R2C / C2R plans transform z (it turns reals into complex)");
+    if (p->g.padded() && !(transform[0] && transform[1] && transform[2]))
+        return fail(DFFT_ERR_UNSUPPORTED, "padded plans transform every axis");
     // schedules, tuned choices and captured graphs are built for the axes of their time
     if (p->axes_fixed) return fail(DFFT_ERR_STATE, "set the transform axes before the first exec, dfft_plan_tune or dfft_plan_describe");
     for (int a = 0; a < 3; ++a) p->taxes[a] = transform[a];
@@ -3067,7 +3130,7 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
     std::vector<Cand> cands;
     cands.push_back({1, 0, 0, 0});
     const bool streams = p->cfg.send_method == DFFT_SEND_STREAMS || (p->g.decomp == DFFT_PENCIL && p->cfg.send_method2 == DFFT_SEND_STREAMS);
-    const bool has_overlap = streams && p->P > 1 && p->xchg_ctas >= 0 && pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p) &&
+    const bool has_overlap = streams && p->P > 1 && p->xchg_ctas >= 0 && alt_schedules(p) &&
                              ((p->g.decomp == DFFT_SLAB_ZY_THEN_X && p->direct2) ||
                               (p->g.decomp == DFFT_PENCIL && p->direct1 && p->direct2 && pencil_overlap_enabled()));
     const bool pencil_inv = inverse && p->g.decomp == DFFT_PENCIL;
@@ -3090,6 +3153,7 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
     if (cands.size() == 1) {
         p->tune_report = is_r2r(p->g.transform) ? "sequential schedule (no alternatives for this plan: DCT / DST plans run the sequential schedule)"
                          : !all_axes(p)         ? "sequential schedule (no alternatives for this plan: plans with a kept axis run the sequential schedule)"
+                         : p->g.padded()        ? "sequential schedule (no alternatives for this plan: padded plans run the sequential schedule)"
                          : pow2_axes(p)         ? "sequential schedule (no alternatives for this plan)"
                                                 : "sequential schedule (no alternatives for this plan: an axis length is not a power of two)";
         return 0;
@@ -3214,6 +3278,8 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
                     (all_axes(p) ? std::string()
                                  : ",\"transform_axes\":[" + std::to_string(p->taxes[0]) + "," + std::to_string(p->taxes[1]) + "," +
                                        std::to_string(p->taxes[2]) + "]") +
+                    (p->g.padded() ? ",\"spectral\":[" + std::to_string(p->g.kx) + "," + std::to_string(p->g.ky) + "," + std::to_string(p->g.kz) + "]"
+                                   : std::string()) +
                     (p->batch > 1 ? ",\"batch\":" + std::to_string(p->batch) + ",\"field_in\":" + std::to_string(sc.field_in) +
                                         ",\"field_out\":" + std::to_string(sc.field_out)
                                   : std::string()) +
@@ -3323,7 +3389,8 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
             o += ",\"kind\":" + std::to_string(int(s_.kind)) +
                  (per_axis && !copy ? std::string(",\"r2r\":\"") + r2r_name(s_.r2r) + "\"" : std::string()) +
                  ",\"log2n\":" + std::to_string(s_.log2n) +
-                 (s_.bluestein() || copy ? ",\"n\":" + std::to_string(s_.n) : std::string()) + ",\"A0\":" + std::to_string(s_.prm.A0) +
+                 (s_.bluestein() || copy ? ",\"n\":" + std::to_string(s_.n) : std::string()) +
+                 (s_.keep ? ",\"keep\":" + std::to_string(s_.keep) : std::string()) + ",\"A0\":" + std::to_string(s_.prm.A0) +
                  ",\"A1\":" + std::to_string(s_.prm.A1) + ",\"B\":" + std::to_string(s_.prm.B) + ",\"inverse\":" + std::to_string(s_.prm.inverse) +
                  ",\"in_user\":" + std::to_string(s_.in_user) + ",\"out_user\":" + std::to_string(s_.out_user) + ",\"in\":";
             json_view(o, s_.prm.in, p->tabs);
@@ -3516,7 +3583,9 @@ int dfft_debug_run_step(dfft_plan_t p, int inverse, int d, size_t field, int ste
         }
         return DFFT_SUCCESS;
     };
-    const size_t in_len = len + (s.kind == PASS_C2R ? 1 : 0), out_len = len + (s.kind == PASS_R2C ? 1 : 0);
+    // points along n of each view: padded passes hold `keep` on their spectral side (out forward, in inverse)
+    const size_t in_len = s.keep && s.prm.inverse ? s.keep : len + (s.kind == PASS_C2R ? 1 : 0);
+    const size_t out_len = s.keep && !s.prm.inverse ? s.keep : len + (s.kind == PASS_R2C ? 1 : 0);
     Step t = s;  // the step with resolved views: its user flags are cleared, so run_pass_step leaves them as they are
     t.in_user = t.out_user = 0;
     int rc = resolve(s.prm.in, s.in_user, in_len, t.prm.in);

@@ -27,6 +27,10 @@ cudaError_t launch_pass(int prec, int log2n, PassKind kind, const FftParams& p, 
     return dispatch<1, MAX_LOG2N>(prec, log2n, [&](auto t, auto l) { return launch_pass<decltype(t), decltype(l)::value>(kind, p, scale, stream); });
 }
 
+cudaError_t launch_padded(int prec, int log2n, PassKind kind, const FftPadded& p, cudaStream_t stream) {
+    return dispatch<1, MAX_LOG2N>(prec, log2n, [&](auto t, auto l) { return launch_padded<decltype(t), decltype(l)::value>(kind, p, stream); });
+}
+
 cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluestein& p, cudaStream_t stream) {
     return dispatch<3, MAX_LOG2N>(prec, log2m, [&](auto t, auto l) { return launch_bluestein<decltype(t), decltype(l)::value>(kind, p, stream); });
 }

@@ -206,6 +206,66 @@ cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStr
 
 template cudaError_t launch_pass<DFFT_T, DFFT_LOG2N>(PassKind, const FftParams&, double, cudaStream_t);
 
+template <typename T, int LOG2N, int TB>
+static cudaError_t launch_padded_tiled(const FftPadded& p, long long lines, cudaStream_t stream) {
+    using C = CtaFft<T, LOG2N, Shape<T, LOG2N>::LOG2E, TB, true>;
+    FftPadded q = p;
+    q.tile_swz = tile_swz_for(p.tile_swz, p.A0, p.A1);
+    const long long g = lines * ((p.B + TB - 1) / TB);
+    if (g > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+    return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, Shape<T, LOG2N>::LOG2E, TB, true, false>, fft_c2c_padded_kernel<T, LOG2N, Shape<T, LOG2N>::LOG2E, TB, true, true>,
+                         nullptr, nullptr>(q, 1.0, unsigned(g), C::THREADS, C::SMEM_BYTES, stream);
+}
+
+// the padded twins (fft_c2c_padded_kernel, fft_r2c_padded_kernel, fft_c2r_padded_kernel): the tiles of launch_pass (TILED:
+// narrow or wide by its rule), one CTA per tile, the register-fed kernel only
+template <typename T, int LOG2N>
+cudaError_t launch_padded(PassKind kind, const FftPadded& p, cudaStream_t stream) {
+    using S = Shape<T, LOG2N>;
+    constexpr int LOG2E = S::LOG2E;
+    const long long lines = (long long)p.A0 * p.A1;
+    if (lines <= 0) return cudaSuccess;
+    const int points = (1 << LOG2N) + (kind == PASS_R2C || kind == PASS_C2R ? 1 : 0);  // of the spectral side's line
+    if (p.lo < 0 || p.hi < p.lo || p.hi > points) return cudaErrorInvalidValue;
+    const long long grid = (lines + S::TBC - 1) / S::TBC;  // CONTIG, R2C and C2R
+    switch (kind) {
+        case PASS_C2C_CONTIG: {
+            using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
+            if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
+            if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+            return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, false, false>, fft_c2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, false, true>,
+                                 nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+        }
+        case PASS_C2C_TILED: {
+            if (p.B <= 0) return cudaSuccess;
+            if constexpr (S::TBT_WIDE != S::TBT) {
+                // the wide-tile rule of launch_pass, without the TMA-fed kernel
+                const int w = wide_tiles();
+                const bool far_rows = (unsigned long long)p.in.sN * sizeof(cx<T>) >= (1ull << 20) ||
+                                      (unsigned long long)p.out.sN * sizeof(cx<T>) >= (1ull << 20);
+                const bool wide = w > 0 || p.tile_pref == 2 || (w == 0 && p.tile_pref == 0 && LOG2N >= 10 && far_rows);
+                if (wide && w >= 0 && p.tile_pref != 1 && p.B > S::TBT) return launch_padded_tiled<T, LOG2N, S::TBT_WIDE>(p, lines, stream);
+            }
+            return launch_padded_tiled<T, LOG2N, S::TBT>(p, lines, stream);
+        }
+        case PASS_R2C:
+        case PASS_C2R: {
+            using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
+            if ((kind == PASS_R2C ? p.in.nseg : p.out.nseg) != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
+            if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+            if (kind == PASS_R2C) {
+                constexpr auto k = fft_r2c_padded_kernel<T, LOG2N, LOG2E, S::TBC>;
+                return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+            }
+            constexpr auto k = fft_c2r_padded_kernel<T, LOG2N, LOG2E, S::TBC>;
+            return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+        }
+        default: return cudaErrorInvalidValue;
+    }
+}
+
+template cudaError_t launch_padded<DFFT_T, DFFT_LOG2N>(PassKind, const FftPadded&, cudaStream_t);
+
 #if DFFT_LOG2N >= 3
 template <typename T, int LOG2M, int TB, bool TILED>
 static cudaError_t launch_bluestein_tiles(const FftBluestein& p, long long grid, cudaStream_t stream) {

@@ -376,13 +376,34 @@ struct MemScaled {
     __device__ __forceinline__ void st(cx<T>* p, cx<T> v) const { m.st(p, cscale<T>(v, s)); }
 };
 
+// ---- padded passes (dfft_plan_create_padded) ----------------------------------------------------------------
+// A padded pass transforms N-point lines whose spectral side keeps K of the N points: the forward pass never stores the
+// hole [lo, hi) of the line and the inverse pass reads it as zero without a load.  Position p outside the hole is element
+// m = p (p < lo) or p - (hi - lo) of the spectral view, so the spectral view and its segment table are those of a K-point
+// axis.  The padded twins take the scale at run time (one instantiation per precision and length).
+struct FftPadded : FftScaled {
+    int lo, hi;  // hole of the N-point line (C2C: [ceil(K/2), ceil(K/2) + N - K); R2C / C2R: [K/2 + 1, N/2 + 1))
+};
+// spectral index of line position n, -1 in the hole
+__device__ __forceinline__ int keep_index(int n, int lo, int hi) { return n < lo ? n : (n < hi ? -1 : n - (hi - lo)); }
+
+// store policy of the padded twins: plain stores, scaled when s != 1 (a runtime value)
+template <typename T>
+struct MemRtScaled {
+    bool on;
+    T s;
+    __device__ __forceinline__ cx<T> ld(const cx<T>* p) const { return ld_elem<T>(p); }
+    __device__ __forceinline__ void st(cx<T>* p, cx<T> v) const { st_elem<T>(p, on ? cscale<T>(v, s) : v); }
+};
+
 // drop a 128-byte L2 line without writing it back (its contents become undefined)
 __device__ __forceinline__ void l2_discard(const void* p) { asm volatile("discard.global.L2 [%0], 128;" ::"l"(p) : "memory"); }
 
 // ---- one tile of a C2C pass: load, CtaFft::stages, store --------------------------------------------------
-template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, typename M, typename Hook = NoGatherHook>
+// PADDED: the spectral side (out forward, in inverse) keeps the line positions outside the hole [lo, hi) (FftPadded).
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, typename M, typename Hook = NoGatherHook, bool PADDED = false>
 __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<T>* sm, unsigned long long* tab_in, unsigned long long* tab_out,
-                                         bool multi, const M& mem, const Hook& after_gather = {}) {
+                                         bool multi, const M& mem, const Hook& after_gather = {}, int lo = 0, int hi = 0) {
     using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
     using LA = LineAccess<T, C::LINES>;
     using TC = TileCoord<C, TILED, TB>;
@@ -404,7 +425,13 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
 
     cx<T> v[E];
     if (tc.valid) {
-        if (!in.multi) {
+        if constexpr (PADDED && INV) {
+#pragma unroll
+            for (int e = 0; e < E; ++e) {
+                const int m = keep_index(j + e * TPL, lo, hi);
+                v[e] = m < 0 ? cx<T>{T(0), T(0)} : mem.ld(TILED ? in.at(m) : in.at1(m));
+            }
+        } else if (!in.multi) {
             if constexpr (!TILED) {
                 // contiguous line: sN == 1, immediate offsets
                 const cx<T>* q = in.p0 + j;
@@ -432,7 +459,13 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
     C::template stages<0>(v, j, t, sm, reinterpret_cast<const cx<T>*>(p.tw), after_gather);
 
     if (tc.valid) {
-        if (!out.multi) {
+        if constexpr (PADDED && !INV) {
+#pragma unroll
+            for (int e = 0; e < E; ++e) {
+                const int m = keep_index(j + e * TPL, lo, hi);
+                if (m >= 0) mem.st(TILED ? out.at(m) : out.at1(m), v[C::Core::final_slot(e)]);
+            }
+        } else if (!out.multi) {
             if constexpr (!TILED) {
                 cx<T>* q = out.p0 + j;
 #pragma unroll
@@ -488,6 +521,20 @@ fft_c2c_kernel(const __grid_constant__ KParams<SCALED> p) {
             else if constexpr (C::NST > 1) C::sync(t);
         }
     }
+}
+
+// padded twin of fft_c2c_kernel (FftPadded): one CTA per tile
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV>
+__global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
+fft_c2c_padded_kernel(const __grid_constant__ FftPadded p) {
+    using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
+    unsigned long long* tab_in = reinterpret_cast<unsigned long long*>(smem_raw + C::TILE_BYTES);
+    unsigned long long* tab_out = tab_in + C::LINES * MAXSEG;
+    const bool multi = p.in.nseg > 1 || p.out.nseg > 1;
+    c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV, MemRtScaled<T>, NoGatherHook, true>(p, blockIdx.x, sm, tab_in, tab_out, multi,
+                                                                                 MemRtScaled<T>{p.scale != 1.0, T(p.scale)}, {}, p.lo, p.hi);
 }
 
 // ---- mbarrier of an asynchronous tile copy (fft_c2c_tma_kernel, fft_zy_fused_kernel) ------------------------------
@@ -1223,9 +1270,9 @@ __device__ __forceinline__ cx<T> shfl_cx(cx<T> v, int src_lane) {
 // ---- R2C pass (CONTIG): real line of 2M points -> M+1 complex points ------------------------------------
 // The real line is read as M complex points z[m] = x[2m] + i x[2m+1], transformed with the length-M
 // core and split into even/odd spectra in shared memory:  X[k] = Xe[k] + W_2M^k Xo[k].
-template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED>
-__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
-fft_r2c_kernel(const __grid_constant__ KParams<SCALED> p) {
+// PADDED (P = FftPadded): the points k >= p.lo are not stored; the scale is p.scale at run time.
+template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED, bool PADDED, typename P>
+__device__ __forceinline__ void r2c_lines(const P& p) {
     using C = CtaFft<T, LOG2M, LOG2E, TB, false>;
     using LA = LineAccess<T, C::LINES>;
     constexpr int E = C::E, TPL = C::TPL, M = C::N, NST = C::NST;
@@ -1272,7 +1319,11 @@ fft_r2c_kernel(const __grid_constant__ KParams<SCALED> p) {
         const cx<T> xo = cx<T>{T(0.5) * d.y, T(-0.5) * d.x};  // -i/2 * d
         const cx<T> tt = cmul(ld_tw(tw2, k), xo);
         if (valid) {
-            if constexpr (SCALED) {
+            if constexpr (PADDED) {
+                const MemRtScaled<T> mem{p.scale != 1.0, T(p.scale)};
+                if (k < p.lo) mem.st(out.at1(k), cadd(xe, tt));
+                if (M - k < p.lo) mem.st(out.at1(M - k), cconj(csub(xe, tt)));
+            } else if constexpr (SCALED) {
                 st_elem<T>(out.at1(k), cscale<T>(cadd(xe, tt), T(p.scale)));
                 st_elem<T>(out.at1(M - k), cscale<T>(cconj(csub(xe, tt)), T(p.scale)));
             } else {
@@ -1286,10 +1337,24 @@ fft_r2c_kernel(const __grid_constant__ KParams<SCALED> p) {
     if (j == 0) emit(M / 2);
 }
 
-// ---- C2R pass (CONTIG): M+1 complex points -> real line of 2M points, unnormalised -----------------------
 template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED>
 __global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
-fft_c2r_kernel(const __grid_constant__ KParams<SCALED> p) {
+fft_r2c_kernel(const __grid_constant__ KParams<SCALED> p) {
+    r2c_lines<T, LOG2M, LOG2E, TB, SCALED, false>(p);
+}
+
+// padded twin of fft_r2c_kernel: keeps the points k < p.lo (p.hi = M + 1)
+template <typename T, int LOG2M, int LOG2E, int TB>
+__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
+fft_r2c_padded_kernel(const __grid_constant__ FftPadded p) {
+    r2c_lines<T, LOG2M, LOG2E, TB, false, true>(p);
+}
+
+// ---- C2R pass (CONTIG): M+1 complex points -> real line of 2M points, unnormalised -----------------------
+// PADDED (P = FftPadded): the points k >= p.lo read as zero, their partner loads X[M - k] as well; the scale is p.scale at
+// run time.
+template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED, bool PADDED, typename P>
+__device__ __forceinline__ void c2r_lines(const P& p) {
     using C = CtaFft<T, LOG2M, LOG2E, TB, false>;
     using LA = LineAccess<T, C::LINES>;
     constexpr int E = C::E, TPL = C::TPL, M = C::N;
@@ -1317,9 +1382,15 @@ fft_c2r_kernel(const __grid_constant__ KParams<SCALED> p) {
         cx<T> xk[E];
         cx<T> xM{T(0), T(0)};
         if (valid) {
+            if constexpr (PADDED) {
 #pragma unroll
-            for (int e = 0; e < E; ++e) xk[e] = ld_elem<T>(in.at1(j + e * TPL));
-            if (j == 0) xM = ld_elem<T>(in.at1(M));
+                for (int e = 0; e < E; ++e) xk[e] = j + e * TPL < p.lo ? ld_elem<T>(in.at1(j + e * TPL)) : cx<T>{T(0), T(0)};
+                if (j == 0 && M < p.lo) xM = ld_elem<T>(in.at1(M));
+            } else {
+#pragma unroll
+                for (int e = 0; e < E; ++e) xk[e] = ld_elem<T>(in.at1(j + e * TPL));
+                if (j == 0) xM = ld_elem<T>(in.at1(M));
+            }
         } else {
 #pragma unroll
             for (int e = 0; e < E; ++e) xk[e] = cx<T>{T(0), T(0)};
@@ -1345,8 +1416,13 @@ fft_c2r_kernel(const __grid_constant__ KParams<SCALED> p) {
     auto build = [&](int k) {
         cx<T> xk{T(0), T(0)}, xm{T(0), T(0)};
         if (valid) {
-            xk = ld_elem<T>(in.at1(k));
-            xm = cconj(ld_elem<T>(in.at1(M - k)));
+            if constexpr (PADDED) {
+                if (k < p.lo) xk = ld_elem<T>(in.at1(k));
+                if (M - k < p.lo) xm = cconj(ld_elem<T>(in.at1(M - k)));
+            } else {
+                xk = ld_elem<T>(in.at1(k));
+                xm = cconj(ld_elem<T>(in.at1(M - k)));
+            }
         }
         const cx<T> xe = cadd(xk, xm);
         const cx<T> xo = cmul(cconj(ld_tw(tw2, k)), csub(xk, xm));
@@ -1366,10 +1442,24 @@ fft_c2r_kernel(const __grid_constant__ KParams<SCALED> p) {
         cx<T>* q = out.p0 + j;
 #pragma unroll
         for (int e = 0; e < E; ++e) {
-            if constexpr (SCALED) st_elem<T>(q + e * TPL, cscale<T>(cswap(v[C::Core::final_slot(e)]), T(p.scale)));
+            if constexpr (PADDED) MemRtScaled<T>{p.scale != 1.0, T(p.scale)}.st(q + e * TPL, cswap(v[C::Core::final_slot(e)]));
+            else if constexpr (SCALED) st_elem<T>(q + e * TPL, cscale<T>(cswap(v[C::Core::final_slot(e)]), T(p.scale)));
             else st_elem<T>(q + e * TPL, cswap(v[C::Core::final_slot(e)]));
         }
     }
+}
+
+template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED>
+__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
+fft_c2r_kernel(const __grid_constant__ KParams<SCALED> p) {
+    c2r_lines<T, LOG2M, LOG2E, TB, SCALED, false>(p);
+}
+
+// padded twin of fft_c2r_kernel: the points k >= p.lo are zero (p.hi = M + 1)
+template <typename T, int LOG2M, int LOG2E, int TB>
+__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
+fft_c2r_padded_kernel(const __grid_constant__ FftPadded p) {
+    c2r_lines<T, LOG2M, LOG2E, TB, false, true>(p);
 }
 
 // ---- Bluestein pass: C2C lines of any length n through two transforms of length M = 2^LOG2M >= 2n - 1 ----------------
@@ -1771,6 +1861,12 @@ cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStr
 // Each launcher also has a runtime form (fft_dispatch.cu) that takes the precision (DFFT_F64 / DFFT_F32) and the log2 length
 // first; it returns cudaErrorInvalidValue for a length that is not instantiated.
 cudaError_t launch_pass(int prec, int log2n, PassKind kind, const FftParams& p, double scale, cudaStream_t stream);
+
+// padded pass (FftPadded): kind PASS_C2C_CONTIG, PASS_C2C_TILED, PASS_R2C or PASS_C2R over the views of launch_pass, the
+// hole [p.lo, p.hi) of each line on its spectral side (out forward, in inverse); p.scale scales the stores.
+template <typename T, int LOG2N>
+cudaError_t launch_padded(PassKind kind, const FftPadded& p, cudaStream_t stream);
+cudaError_t launch_padded(int prec, int log2n, PassKind kind, const FftPadded& p, cudaStream_t stream);
 
 // fused z + y stage (fft_zy_fused_kernel), instantiated for the lengths zy_fused_length accepts.  pz: the z pass, py: the y
 // pass, f: counters and plane groups (f.order.na / nb are filled in here).  Every launch of one step must use the same

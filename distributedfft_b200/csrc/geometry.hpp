@@ -27,6 +27,10 @@ struct Split {
 struct Geometry {
     int decomp = 0, transform = 0;
     size_t nx = 0, ny = 0, nz = 0, nzc = 0;  // nzc: z extent of every complex array (real-to-real: of every real array, Nz)
+    // spectral extents (dfft_plan_create_padded): Kx, Ky and the z extent of the spectrum (R2C: Kz/2 + 1); nx, ny, nzc for
+    // every other plan.  An axis is padded by the pass that transforms it: the layout after d stages has K on the first d
+    // axes in z, y, x order.
+    size_t kx = 0, ky = 0, kz = 0, kzc = 0;
     int P = 1, P1 = 1, P2 = 1;
     // x split of the input (over P1, or over P for both slab sequences)
     Split sx;
@@ -35,11 +39,17 @@ struct Geometry {
     // y split of the output over P1 (slab zy_x: over P)
     Split oy;
 
-    // returns false on an invalid partition
-    bool init(int decomp_, int transform_, size_t nx_, size_t ny_, size_t nz_, size_t p1, size_t p2, int nranks) {
+    // returns false on an invalid partition.  kx_, ky_, kz_: the spectral grid (0: the physical one)
+    bool init(int decomp_, int transform_, size_t nx_, size_t ny_, size_t nz_, size_t p1, size_t p2, int nranks, size_t kx_ = 0, size_t ky_ = 0,
+              size_t kz_ = 0) {
         decomp = decomp_; transform = transform_;
         nx = nx_; ny = ny_; nz = nz_;
-        nzc = (transform == DFFT_C2C || transform == DFFT_DCT || transform == DFFT_DST || transform == DFFT_R2HC) ? nz : nz / 2 + 1;
+        const bool real_z = !(transform == DFFT_C2C || transform == DFFT_DCT || transform == DFFT_DST || transform == DFFT_R2HC);
+        nzc = real_z ? nz / 2 + 1 : nz;
+        kx = kx_ ? kx_ : nx;
+        ky = ky_ ? ky_ : ny;
+        kz = kz_ ? kz_ : nz;
+        kzc = real_z ? kz / 2 + 1 : kz;
         P = nranks;
         if (decomp == DFFT_SLAB_ZY_THEN_X) { P1 = P; P2 = 1; }
         else if (decomp == DFFT_SLAB_Z_THEN_YX) { P1 = P; P2 = 1; }  // P1 only used for the x split
@@ -50,15 +60,16 @@ struct Geometry {
         sx.make(nx, P1);
         if (decomp == DFFT_SLAB_Z_THEN_YX) {
             sy.make(ny, 1);
-            sz.make(nzc, P);
-            oy.make(ny, 1);
+            sz.make(kzc, P);
+            oy.make(ky, 1);
         } else {
             sy.make(ny, P2);
-            sz.make(nzc, P2);
-            oy.make(ny, P1);
+            sz.make(kzc, P2);
+            oy.make(ky, P1);
         }
         return true;
     }
+    bool padded() const { return kx != nx || ky != ny || kz != nz; }
     int pi(int rank) const { return decomp == DFFT_PENCIL ? rank / P2 : rank; }
     int pj(int rank) const { return decomp == DFFT_PENCIL ? rank % P2 : 0; }
 
@@ -67,10 +78,10 @@ struct Geometry {
         const int i = pi(rank), j = pj(rank);
         if (decomp == DFFT_SLAB_Z_THEN_YX) {
             if (which <= 1) {
-                size[0] = sx.size[i]; size[1] = ny; size[2] = which == 0 ? nz : nzc;
+                size[0] = sx.size[i]; size[1] = ny; size[2] = which == 0 ? nz : kzc;
                 start[0] = sx.start[i]; start[1] = 0; start[2] = 0;
             } else {
-                size[0] = nx; size[1] = ny; size[2] = sz.size[rank];
+                size[0] = which == 2 ? nx : kx; size[1] = ky; size[2] = sz.size[rank];
                 start[0] = 0; start[1] = 0; start[2] = sz.start[rank];
             }
             return;
@@ -78,21 +89,22 @@ struct Geometry {
         switch (which) {
             case 0:
             case 1:
-                size[0] = sx.size[i]; size[1] = sy.size[j]; size[2] = which == 0 ? nz : nzc;
+                size[0] = sx.size[i]; size[1] = sy.size[j]; size[2] = which == 0 ? nz : kzc;
                 start[0] = sx.start[i]; start[1] = sy.start[j]; start[2] = 0;
                 break;
             case 2:
-                size[0] = sx.size[i]; size[1] = ny; size[2] = sz.size[j];
+                size[0] = sx.size[i]; size[1] = ky; size[2] = sz.size[j];
                 start[0] = sx.start[i]; start[1] = 0; start[2] = sz.start[j];
                 break;
             default:
-                size[0] = nx; size[1] = oy.size[i]; size[2] = sz.size[j];
+                size[0] = kx; size[1] = oy.size[i]; size[2] = sz.size[j];
                 start[0] = 0; start[1] = oy.start[i]; start[2] = sz.start[j];
                 break;
         }
     }
     // complex elements of the largest per-rank stage array (the reference's domainsize / sizeof(C_t),
-    // mpicufft_slab.cpp:132)
+    // mpicufft_slab.cpp:132).  Padded plans have two more: the y pass' physical side [x_i][Ny][z_j] and the x pass' physical
+    // side (Z_Then_YX: [Nx][Ny][z_r]; otherwise [Nx][y_i][z_j], y spectral); in every other plan they are layouts 2 and 3.
     size_t domain_elems(int rank) const {
         size_t m = 0;
         for (int w = 1; w <= 3; ++w) {
@@ -100,7 +112,10 @@ struct Geometry {
             layout(rank, w, s, o);
             m = std::max(m, s[0] * s[1] * s[2]);
         }
-        return m;
+        const size_t zr = decomp == DFFT_SLAB_Z_THEN_YX ? sz.size[rank] : sz.size[pj(rank)];
+        const size_t xr = decomp == DFFT_SLAB_Z_THEN_YX ? nx : sx.size[pi(rank)];
+        const size_t yr = decomp == DFFT_SLAB_Z_THEN_YX ? ny : oy.size[pi(rank)];
+        return std::max(m, std::max(xr * ny * zr, nx * yr * zr));
     }
 };
 

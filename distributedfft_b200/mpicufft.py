@@ -124,13 +124,15 @@ class MPIcuFFT:
 
     # -- plan ------------------------------------------------------------------------------------
     def initFFT(self, global_size: GlobalSize, partition: Optional[Partition] = None, allocate: bool = True, batch: int = 1,
-                inplace: bool = False, transform_axes: Optional[Sequence[bool]] = None):
+                inplace: bool = False, transform_axes: Optional[Sequence[bool]] = None, spectral: Optional[Sequence[int]] = None):
         """`batch` (not in the reference): every exec transforms that many fields, back to back in each buffer — a
         contiguous [batch, X, Y, Z] tensor; the getters describe one field (dfft_plan_create_batched).
         `inplace` (dfft_plan_create_inplace): every exec gets the same buffer twice and overwrites its input; fields are
         getDomainSize() bytes apart.  R2C / C2R use padded real rows: with buf a complex [X, Y, Nz/2+1] tensor, pass
         torch.view_as_real(buf).view(X, Y, Nz + 2) as the real side.
-        `transform_axes` (x, y, z): setTransformAxes right after creation, e.g. (False, True, True) keeps x."""
+        `transform_axes` (x, y, z): setTransformAxes right after creation, e.g. (False, True, True) keeps x.
+        `spectral` (kx, ky, kz) (dfft_plan_create_padded): a padded plan, global_size the physical grid and (kx, ky, kz) the
+        spectrum it keeps — the forward stores only those modes, the inverse zero-pads them (the 3/2 dealiasing rule)."""
         if global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         cfg = _lib.dfft_config(int(self.config.cuda_aware), int(self.config.warmup_rounds), int(self.config.comm_method),
@@ -142,7 +144,15 @@ class MPIcuFFT:
         if self._decomp == PENCIL and partition is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         h = C.c_void_p()
-        if self.kinds is not None:
+        if spectral is not None:
+            if inplace or self.kinds is not None:
+                raise ValueError("padded plans are out of place and C2C or R2C")
+            if batch < 1:
+                raise ValueError("batch must be at least 1")
+            kx, ky, kz = (int(k) for k in spectral)
+            check(lib().dfft_plan_create_padded(self.comm._h, C.byref(cfg), self._decomp, self.precision, self.transform, global_size.Nx,
+                                                global_size.Ny, global_size.Nz, kx, ky, kz, p1, p2, batch, 1 if allocate else 0, C.byref(h)))
+        elif self.kinds is not None:
             if batch < 0:
                 raise ValueError("batch must be at least 1")
             check(lib().dfft_plan_create_r2r(self.comm._h, C.byref(cfg), self._decomp, self.precision, (C.c_int * 3)(*self.kinds),
@@ -279,6 +289,7 @@ class MPIcuFFT:
     def getPartialSize(self, d): return self._triple(lib().dfft_get_partial_size, d)
     def getPartialStart(self, d): return self._triple(lib().dfft_get_partial_start, d)
     def getDomainSize(self): return int(lib().dfft_get_domain_size(self._h))
+    def getSpectralSize(self): return self._triple(lib().dfft_plan_get_spectral_size)
     def getBatch(self): return int(lib().dfft_get_batch(self._h))
     def isInPlace(self): return bool(lib().dfft_plan_is_inplace(self._h))
     def getWorkSizeDevice(self): return int(lib().dfft_get_work_size_device(self._h))
@@ -349,13 +360,13 @@ class MPIcuFFT_Pencil(MPIcuFFT):
     """z FFT -> transpose -> y FFT -> transpose -> x FFT on a P1 x P2 grid. include/mpicufft_pencil.hpp."""
     _decomp = PENCIL
 
-    def initFFT(self, global_size, partition=None, allocate=True, batch=1, inplace=False, transform_axes=None):
+    def initFFT(self, global_size, partition=None, allocate=True, batch=1, inplace=False, transform_axes=None, spectral=None):
         if partition is None or global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         if partition.P1 * partition.P2 != self.comm.size:
             raise RuntimeError("Invalid Input Partition!")
         self.partition = partition
-        super().initFFT(global_size, partition, allocate, batch, inplace, transform_axes)
+        super().initFFT(global_size, partition, allocate, batch, inplace, transform_axes, spectral)
 
     def getPartitionDimensions(self):
         """(input_dim, transposed_dim, output_dim), each a dict with size_x/y/z and start_x/y/z lists

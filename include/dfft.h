@@ -178,6 +178,27 @@ int dfft_plan_create_r2r(dfft_comm_t comm, const dfft_config* config, int decomp
 /* kinds[0..2] of the x, y and z axis of a real-to-real plan (also of DFFT_DCT / DFFT_DST plans); DFFT_ERR_INVALID for
  * R2C / C2C plans. */
 int dfft_plan_get_r2r_kinds(dfft_plan_t plan, int kinds[3]);
+/* Padded plans (mpi4py-fft's `padding`, for the 3/2 dealiasing rule of pseudo-spectral solvers): a physical grid of
+ * nx x ny x nz points and a spectrum of kx x ky x kz modes, 1 <= k <= n per axis.  The spectral side of the plan is that of
+ * an ordinary kx x ky x kz plan on the same ranks, the physical side that of the nx x ny x nz plan.
+ *   - C2C axis: spectral index m in [0, K) is frequency numpy.fft.fftfreq(K)[m] * K, at position m (m < ceil(K/2)) or
+ *     m + N - K of the N-point line.  R2C z axis: the modes k = 0 .. Kz/2, a spectral z extent of Kz/2 + 1.
+ *   - Forward: the N-point transform, then only the kept modes are stored.  Inverse: the unnormalised inverse of the
+ *     zero-embedded spectrum; the missing modes are never read.  inverse(forward(x)) = Nx*Ny*Nz times the low-pass
+ *     projection of x, forward(inverse(X)) = Nx*Ny*Nz*X.
+ *   - Partial d: each axis is truncated (padded) by the pass that transforms it, so the layout after d stages has K on
+ *     the first d axes in z, y, x order.  The getters, batch distances and dfft_get_work_size_device follow.
+ *   - Batch, output scale, Peer2Peer / All2All, dfft_plan_describe ("spectral", and "keep" on every pass with a hole) and
+ *     graph capture work as for other plans; padded plans run the sequential schedule (dfft_plan_tune has no alternative).
+ *   - kx = nx, ky = ny, kz = nz makes the plan of dfft_plan_create_batched: the same steps, description and output.
+ *   - DFFT_DCT / DFFT_DST, or K < N on an axis whose length is not a power of two: DFFT_ERR_UNSUPPORTED.  A K of 0 or
+ *     above N, transform 4, or a spectral split that leaves a rank without data: DFFT_ERR_INVALID.
+ *   - No in-place form; dfft_plan_set_transform_axes other than {1, 1, 1} on a plan with some K < N: DFFT_ERR_UNSUPPORTED. */
+int dfft_plan_create_padded(dfft_comm_t comm, const dfft_config* config, int decomp /*dfft_decomp*/, int precision /*dfft_prec*/,
+                            int transform /*dfft_transform*/, size_t nx, size_t ny, size_t nz, size_t kx, size_t ky, size_t kz,
+                            size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan);
+/* k[0..2] = kx, ky, kz of a padded plan; nx, ny, nz for every other plan. */
+int dfft_plan_get_spectral_size(dfft_plan_t plan, size_t k[3]);
 int dfft_plan_destroy(dfft_plan_t plan);
 /* setWorkArea(device, host) — mpicufft_slab.cpp:236-281. device must hold dfft_get_work_size_device()
  * bytes; with comm_method Peer2Peer and more than one rank it must be the base of a cudaMalloc

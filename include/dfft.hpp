@@ -99,6 +99,15 @@ public:
         inplace_ = inplace;
         initFFT(global_size, partition, allocate, batch);
     }
+    // not in the reference: a padded plan (dfft_plan_create_padded): global_size is the physical grid, spectral the
+    // Kx x Ky x Kz spectrum it keeps (the forward truncates to it, the inverse zero-pads it), 1 <= K <= N per axis
+    void initFFT(GlobalSize* global_size, GlobalSize* spectral, Partition* partition, bool allocate = true, size_t batch = 1) {
+        struct Reset { GlobalSize*& s; ~Reset() { s = nullptr; } } reset{spectral_};
+        spectral_ = spectral;
+        initFFT(global_size, partition, allocate, batch);
+    }
+    // kx, ky, kz of a padded plan; Nx, Ny, Nz of every other plan
+    void getSpectralSize(size_t* k) const { DFFT_CALL(dfft_plan_get_spectral_size(plan, k)); }
     size_t getBatch() const { return dfft_get_batch(plan); }
     bool isInPlace() const { return dfft_plan_is_inplace(plan) != 0; }
     // not in the reference: output scale of every forward / inverse exec (dfft_plan_set_scale; after initFFT).  For
@@ -142,7 +151,10 @@ protected:
         c.benchmark_dir = config.benchmark_dir.empty() ? nullptr : config.benchmark_dir.c_str();
         c.comm_method2 = config.comm_method2; c.send_method2 = config.send_method2;
         if (plan) { dfft_plan_destroy(plan); plan = nullptr; }
-        if (per_axis)
+        if (spectral_)
+            DFFT_CALL(dfft_plan_create_padded(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, spectral_->Nx, spectral_->Ny,
+                                              spectral_->Nz, p1, p2, batch_, allocate ? 1 : 0, &plan));
+        else if (per_axis)
             DFFT_CALL(dfft_plan_create_r2r(comm, &c, decomp, dfft_shim::prec<T>::value, kinds, gs->Nx, gs->Ny, gs->Nz, p1, p2, batch_,
                                            inplace_ ? 1 : 0, allocate ? 1 : 0, &plan));
         else if (inplace_)
@@ -157,6 +169,7 @@ protected:
     }
     size_t batch_ = 1;       // fields of the plan initFFT is creating
     bool inplace_ = false;   // whether initFFT is creating an in-place plan
+    GlobalSize* spectral_ = nullptr;  // the spectrum of the padded plan initFFT is creating
     Configurations config;
     dfft_comm_t comm;
     int transform;
