@@ -397,6 +397,7 @@ struct dfft_plan_s {
     int taxes[3] = {1, 1, 1};  // dfft_plan_set_transform_axes: 1 transforms the x, y, z axis, 0 keeps it (copy passes)
     bool axes_fixed = false;   // a schedule was built or tuned for taxes: the setter refuses from then on
     size_t batch = 1;         // fields per exec, back to back in every caller buffer (dfft_plan_create_batched)
+    size_t comps = 1;         // values per grid point, interleaved (dfft_plan_create_interleaved); esize stays one value's
     double scale[2] = {1.0, 1.0};  // [fwd/inv] output scale (dfft_plan_set_scale), applied by the steps marked final_store
     // dfft_plan_create_inplace: every exec has out == in, fields domain_bytes apart, real rows of R2C / C2R padded to Nzc
     // complex units.  buf_slot: one rank — the schedules' first slot (D1) is the caller's buffer and is not allocated.
@@ -535,7 +536,8 @@ static bool all_axes(const dfft_plan_s* p) { return p->taxes[0] && p->taxes[1] &
 // Whether the schedules may take another form than the sequential one: the overlapped schedules, the fused z + y stage and
 // the batched stage build their passes for power-of-two lengths, every axis transformed and no padding (their kernels have
 // no padded twins, FftPadded).
-static bool alt_schedules(const dfft_plan_s* p) { return pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p) && !p->g.padded(); }
+// Interleaved plans (C > 1 values per point) run it too: those kernels address one value per point.
+static bool alt_schedules(const dfft_plan_s* p) { return pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p) && !p->g.padded() && p->comps == 1; }
 
 // Row pitch, in elements (complex units; reals for DCT / DST plans), of the z-contiguous side of the caller's buffers that
 // holds Nz points per row: the input of forward passes, the output of inverse ones.  Real rows of R2C / C2R plans are Nz reals (Nz/2 units) apart, or, in
@@ -550,7 +552,7 @@ static long long z_row_pitch(const dfft_plan_s* p) {
 // three passes are L2-resident already and gain nothing.
 static bool zy_fused(const dfft_plan_s* p, int inverse, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded()) return false;
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || p->comps > 1) return false;
     if (g.ny != g.nz || !zy_fused_length(ilog2_exact(g.ny))) return false;
     // the fused stage reads and writes the blocked hand-over layout of the x pass
     if (p->blocked_ch <= 0 || g.nz % size_t(p->blocked_ch) || (inverse && !p->blocked_inv)) return false;
@@ -604,7 +606,7 @@ static int fuse_zy(dfft_plan_s* p, Step zs, const Step& ys, const char* label, c
 constexpr size_t BATCH_SMALL_MIN = 2;
 static bool batch_small(const dfft_plan_s* p, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded()) return false;
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || p->comps > 1) return false;
     if (g.nx != g.ny || g.ny != g.nz || !batch_small_length(ilog2_exact(g.nx))) return false;
     return p->batch >= BATCH_SMALL_MIN && p->batch * g.nx <= 0x7fffffff;
 }
@@ -652,7 +654,8 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     const Geometry& g = p->g;
     const int me = p->rank, P = p->P;
     const int pi = g.pi(me), pj = g.pj(me);
-    const size_t es = p->esize;
+    // bytes per grid point: the views below count points; interleaved plans widen them to values afterwards (widen_views)
+    const size_t es = p->esize * p->comps;
     // DCT / DST plans run the C2C builders over reals; new_pass turns their C2C kinds into R2R ones
     const bool c2c = g.transform != DFFT_R2C;
     const bool r2r = is_r2r(g.transform);
@@ -2214,8 +2217,9 @@ static void field_bytes(const dfft_plan_s* p, int inverse, int d, size_t* in_b, 
     size_t s0[3], sd[3], o[3];
     p->g.layout(p->rank, 0, s0, o);
     p->g.layout(p->rank, d, sd, o);
-    const size_t real_es = p->g.transform == DFFT_R2C ? p->esize / 2 : p->esize;
-    const size_t b0 = s0[0] * s0[1] * s0[2] * real_es, bd = sd[0] * sd[1] * sd[2] * p->esize;
+    const size_t es = p->esize * p->comps;  // bytes per point
+    const size_t real_es = p->g.transform == DFFT_R2C ? es / 2 : es;
+    const size_t b0 = s0[0] * s0[1] * s0[2] * real_es, bd = sd[0] * sd[1] * sd[2] * es;
     *in_b = inverse ? bd : b0;
     *out_b = inverse ? b0 : bd;
 }
@@ -2335,6 +2339,43 @@ static void drop_identity_copies(const dfft_plan_s* p, Schedule& sc) {
     }
 }
 
+// Interleaved plans: build_schedule lays out points of C values (its byte offsets count C * esize); the kernels address
+// single values.  So every stride scales by C, a pass whose contiguous dimension is z sees C columns per z point, the z
+// pass runs lines C apart with b the component (PASS_C2C_ILV: B = C, sN = C), and all-to-all counts are in values.  The
+// R2C / C2R z pass becomes the paired pass of Nz-point lines (PASS_R2C_ILV / PASS_C2R_ILV) with the Nz-point twiddle table;
+// its real side, built in complex units of Nz / 2 per row, is counted in reals (element (a0, a1, n, c) at
+// base + a0 sA0 + a1 sA1 + n C + c).
+static int widen_views(dfft_plan_s* p, Schedule& sc) {
+    const long long C = (long long)p->comps;
+    if (C == 1) return DFFT_SUCCESS;
+    auto widen = [&](View& v, long long f) {
+        v.sN *= C;
+        for (int i = 0; i < v.nseg; ++i) { v.seg[i].sA0 *= C * f; v.seg[i].sA1 *= C * f; }
+    };
+    for (Step& s : sc.steps) {
+        if (s.type == STEP_A2A)
+            for (std::vector<size_t>* v : {&s.scount, &s.soff, &s.rcount, &s.roff})
+                for (size_t& x : *v) x *= size_t(C);
+        if (s.type != STEP_PASS) continue;
+        const bool r2c = s.kind == PASS_R2C, c2r = s.kind == PASS_C2R;
+        widen(s.prm.in, r2c ? 2 : 1);
+        widen(s.prm.out, c2r ? 2 : 1);
+        s.prm.B = s.kind == PASS_C2C_TILED ? s.prm.B * int(C) : int(C);
+        if (s.kind == PASS_C2C_CONTIG) s.kind = PASS_C2C_ILV;
+        if (r2c || c2r) {
+            s.kind = r2c ? PASS_R2C_ILV : PASS_C2R_ILV;
+            s.n = 2 * (s.n ? s.n : size_t(1) << s.log2n);
+            s.log2n = ilog2_exact(s.n);
+            void *tw = nullptr, *tw2 = nullptr, *blu = nullptr;
+            const int rc = pass_tables(p->tabs, s.kind, s.n, 0, &tw, &tw2, &blu);
+            if (rc) return rc;
+            s.prm.tw = tw;
+            s.prm.tw2 = nullptr;
+        }
+    }
+    return DFFT_SUCCESS;
+}
+
 // The one place that decides which schedule a (direction, d) pair runs — used by exec and by dfft_plan_describe, so
 // the CPU schedule emulation always validates exactly what executes.
 static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
@@ -2360,6 +2401,8 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
         else if (want_overlap) rc = build_overlapped_slab(p, inverse ? 1 : 0, sc);
         else if (want_pencil_overlap) rc = build_overlapped_pencil(p, inverse ? 1 : 0, sc);
         else rc = build_schedule(p, inverse ? 1 : 0, db, sc);
+        if (rc) return rc;
+        rc = widen_views(p, sc);
         if (rc) return rc;
         if (!all_axes(p)) {
             name_copies(sc);
@@ -2607,7 +2650,7 @@ int dfft_plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, in
 // spectral: Kx, Ky, Kz of the plans of dfft_plan_create_padded (checked there), nullptr otherwise.
 static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
                        size_t nz, size_t p1, size_t p2, size_t batch, bool inplace, int allocate, dfft_plan_t* plan,
-                       const int* kinds = nullptr, const size_t* spectral = nullptr) {
+                       const int* kinds = nullptr, const size_t* spectral = nullptr, size_t comps = 1) {
     if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
     if (batch == 0) return fail(DFFT_ERR_INVALID, "batch must be at least 1");
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
@@ -2629,6 +2672,7 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
     p->prec = precision;
     for (int a = 0; a < 3; ++a) p->kinds[a] = kinds ? kinds[a] : is_r2r(transform) ? transform : 0;
     p->esize = (precision == DFFT_F64 ? 16 : 8) / (is_r2r(transform) ? 2 : 1);  // DCT / DST: real elements
+    p->comps = comps;
     p->tabs.prec = precision;
     p->tabs.dry = dry;
     if (!p->g.init(decomp, transform, nx, ny, nz, p1, p2, p->P, spectral ? spectral[0] : 0, spectral ? spectral[1] : 0, spectral ? spectral[2] : 0)) {
@@ -2659,7 +2703,7 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
     p->inplace = inplace;
     // the largest stage array of this rank; it also covers the padded real input of in-place R2C plans, which has the
     // extent of the layout after d = 1
-    p->domain_bytes = g.domain_elems(p->rank) * p->esize;
+    p->domain_bytes = g.domain_elems(p->rank) * p->esize * comps;
     {   // the whole batch of every caller buffer (any direction, any partial d) must be addressable
         size_t widest = 0;
         for (int d = 1; d <= 3; ++d) {
@@ -2702,7 +2746,7 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
     if (p->buf_slot) p->nslots = 1;
     size_t dom = 0;
     for (int r = 0; r < P; ++r) dom = std::max(dom, g.domain_elems(r));
-    p->slot_bytes = ((dom * p->esize + 255) / 256) * 256;
+    p->slot_bytes = ((dom * p->esize * comps + 255) / 256) * 256;
     p->work_bytes = p->slot_bytes * p->nslots;
     {
         const char* e = getenv("DFFT_XCHG_CTAS");
@@ -2835,6 +2879,26 @@ int dfft_plan_create_padded(dfft_comm_t comm, const dfft_config* config, int dec
     }
     return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, false, allocate, plan, nullptr, k);
 }
+
+// C values per point: the C = 1 plan with every element widened to C consecutive values (DESIGN.md section 3.14).  The
+// z pass of C > 1 runs interleaved lines (PASS_C2C_ILV) or paired R2C / C2R lines of Nz points (PASS_R2C_ILV /
+// PASS_C2R_ILV), which exist for a power-of-two Nz (R2C: up to 8192).
+constexpr size_t MAX_COMPONENTS = 64;
+int dfft_plan_create_interleaved(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
+                                 size_t nz, size_t p1, size_t p2, size_t components, size_t batch, int allocate, dfft_plan_t* plan) {
+    if (components == 0) return fail(DFFT_ERR_INVALID, "components must be at least 1");
+    if (components > MAX_COMPONENTS) return fail(DFFT_ERR_UNSUPPORTED, "at most " + std::to_string(MAX_COMPONENTS) + " components per point");
+    if (components > 1) {
+        if (transform != DFFT_C2C && transform != DFFT_R2C && !is_r2r(transform)) return fail(DFFT_ERR_INVALID, "bad transform");
+        if (is_r2r(transform)) return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans with more than one component are C2C or R2C / C2R");
+        if (ilog2_exact(nz) < 1) return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans need a power-of-two Nz (x and y may have any C2C length)");
+        // the paired R2C / C2R z pass runs Nz-point complex lines
+        if (transform == DFFT_R2C && ilog2_exact(nz) > MAX_LOG2N)
+            return fail(DFFT_ERR_UNSUPPORTED, "interleaved R2C / C2R plans need Nz <= " + std::to_string(1 << MAX_LOG2N));
+    }
+    return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, false, allocate, plan, nullptr, nullptr, components);
+}
+size_t dfft_get_components(dfft_plan_t p) { return p ? p->comps : 0; }
 
 int dfft_plan_get_spectral_size(dfft_plan_t p, size_t k[3]) {
     if (!p || !k) return fail(DFFT_ERR_INVALID, "null plan / size");
@@ -2994,6 +3058,8 @@ int dfft_plan_set_transform_axes(dfft_plan_t p, const int transform[3]) {
     if (p->g.transform == DFFT_R2C && !transform[2]) return fail(DFFT_ERR_INVALID, "R2C / C2R plans transform z (it turns reals into complex)");
     if (p->g.padded() && !(transform[0] && transform[1] && transform[2]))
         return fail(DFFT_ERR_UNSUPPORTED, "padded plans transform every axis");
+    if (p->comps > 1 && !(transform[0] && transform[1] && transform[2]))
+        return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans transform every axis");
     // schedules, tuned choices and captured graphs are built for the axes of their time
     if (p->axes_fixed) return fail(DFFT_ERR_STATE, "set the transform axes before the first exec, dfft_plan_tune or dfft_plan_describe");
     for (int a = 0; a < 3; ++a) p->taxes[a] = transform[a];
@@ -3154,6 +3220,7 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
         p->tune_report = is_r2r(p->g.transform) ? "sequential schedule (no alternatives for this plan: DCT / DST plans run the sequential schedule)"
                          : !all_axes(p)         ? "sequential schedule (no alternatives for this plan: plans with a kept axis run the sequential schedule)"
                          : p->g.padded()        ? "sequential schedule (no alternatives for this plan: padded plans run the sequential schedule)"
+                         : p->comps > 1         ? "sequential schedule (no alternatives for this plan: interleaved plans run the sequential schedule)"
                          : pow2_axes(p)         ? "sequential schedule (no alternatives for this plan)"
                                                 : "sequential schedule (no alternatives for this plan: an axis length is not a power of two)";
         return 0;
@@ -3280,6 +3347,7 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
                                        std::to_string(p->taxes[2]) + "]") +
                     (p->g.padded() ? ",\"spectral\":[" + std::to_string(p->g.kx) + "," + std::to_string(p->g.ky) + "," + std::to_string(p->g.kz) + "]"
                                    : std::string()) +
+                    (p->comps > 1 ? ",\"components\":" + std::to_string(p->comps) : std::string()) +
                     (p->batch > 1 ? ",\"batch\":" + std::to_string(p->batch) + ",\"field_in\":" + std::to_string(sc.field_in) +
                                         ",\"field_out\":" + std::to_string(sc.field_out)
                                   : std::string()) +
@@ -3546,7 +3614,8 @@ int dfft_debug_run_step(dfft_plan_t p, int inverse, int d, size_t field, int ste
     struct Range { const char *lo, *hi, *buf; size_t bytes; };
     std::vector<Range> ranges;
     std::vector<std::pair<View*, const std::vector<unsigned char>*>> tables;
-    auto resolve = [&](View& v, int user, size_t n_len, View& launched) -> int {
+    // bytes per view element: reals on the real side of the paired R2C / C2R pass of interleaved plans
+    auto resolve = [&](View& v, int user, size_t n_len, View& launched, size_t ebytes) -> int {
         if (v.nseg < 1 || v.nseg > MAXSEG || (user && v.nseg != 1)) return fail(DFFT_ERR_STATE, "internal: view segments");
         const std::vector<unsigned char>* tab = nullptr;
         if (v.nseg > 1) {
@@ -3579,17 +3648,21 @@ int dfft_debug_run_step(dfft_plan_t p, int inverse, int d, size_t field, int ste
             lo += std::min(t0, t1);
             hi += std::max(t0, t1);
             const char* b = static_cast<const char*>(sg.base);
-            ranges.push_back({b + lo * (long long)p->esize, b + (hi + 1) * (long long)p->esize, buf, bytes});
+            ranges.push_back({b + lo * (long long)ebytes, b + (hi + 1) * (long long)ebytes, buf, bytes});
         }
         return DFFT_SUCCESS;
     };
     // points along n of each view: padded passes hold `keep` on their spectral side (out forward, in inverse)
-    const size_t in_len = s.keep && s.prm.inverse ? s.keep : len + (s.kind == PASS_C2R ? 1 : 0);
-    const size_t out_len = s.keep && !s.prm.inverse ? s.keep : len + (s.kind == PASS_R2C ? 1 : 0);
+    // (the paired R2C / C2R pass: Nz reals, Nz / 2 + 1 complex points)
+    size_t in_len = s.keep && s.prm.inverse ? s.keep : len + (s.kind == PASS_C2R ? 1 : 0);
+    size_t out_len = s.keep && !s.prm.inverse ? s.keep : len + (s.kind == PASS_R2C ? 1 : 0);
+    if (s.kind == PASS_R2C_ILV) out_len = len / 2 + 1;
+    if (s.kind == PASS_C2R_ILV) in_len = len / 2 + 1;
+    const size_t es = p->esize;
     Step t = s;  // the step with resolved views: its user flags are cleared, so run_pass_step leaves them as they are
     t.in_user = t.out_user = 0;
-    int rc = resolve(s.prm.in, s.in_user, in_len, t.prm.in);
-    if (!rc) rc = resolve(s.prm.out, s.out_user, out_len, t.prm.out);
+    int rc = resolve(s.prm.in, s.in_user, in_len, t.prm.in, s.kind == PASS_R2C_ILV ? es / 2 : es);
+    if (!rc) rc = resolve(s.prm.out, s.out_user, out_len, t.prm.out, s.kind == PASS_C2R_ILV ? es / 2 : es);
     if (rc) return rc;
     for (const Range& r : ranges)
         if (!r.buf || r.lo < r.buf || r.hi > r.buf + r.bytes)

@@ -186,6 +186,35 @@ cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStr
             }
             return launch_tiled<T, LOG2N, S::TBT>(p, scale, stream, lines);
         }
+        case PASS_C2C_ILV: {
+            // C = B components per point, lines C apart along n.  From the tile width on, the TILED kernel's tiles are full
+            // rows of components; below it the interleaved kernel keeps every thread busy.
+            if (p.B < 1 || p.in.sN != p.B || p.out.sN != p.B) return cudaErrorInvalidValue;
+            if (p.B >= S::TBT) return launch_tiled<T, LOG2N, S::TBT>(p, scale, stream, lines);
+            const long long g = (lines * p.B + S::TBC - 1) / S::TBC;
+            if (g > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+            const unsigned grid_ilv = unsigned((p.max_ctas > 0 && g > p.max_ctas) ? p.max_ctas : g);
+            return launch_kernel<fft_c2c_ilv_kernel<T, LOG2N, LOG2E, S::TBC, false, false>, fft_c2c_ilv_kernel<T, LOG2N, LOG2E, S::TBC, true, false>,
+                                 fft_c2c_ilv_kernel<T, LOG2N, LOG2E, S::TBC, false, true>, fft_c2c_ilv_kernel<T, LOG2N, LOG2E, S::TBC, true, true>>(
+                p, scale, grid_ilv, C::THREADS, C::SMEM_BYTES, stream);
+        }
+        case PASS_R2C_ILV:
+        case PASS_C2R_ILV: {
+            // C = B components, (C + 1) / 2 paired lines per row; the real side is one segment
+            const bool c2r = kind == PASS_C2R_ILV;
+            if (p.B < 1 || (c2r ? p.out.nseg : p.in.nseg) != 1) return cudaErrorInvalidValue;
+            const long long g = (lines * ((p.B + 1) / 2) + S::TBC - 1) / S::TBC;
+            if (g > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+            const unsigned grid_rc = unsigned((p.max_ctas > 0 && g > p.max_ctas) ? p.max_ctas : g);
+            if (c2r) {
+                constexpr auto k = fft_rc_ilv_kernel<T, LOG2N, LOG2E, S::TBC, true, false>;
+                constexpr auto ks = fft_rc_ilv_kernel<T, LOG2N, LOG2E, S::TBC, true, true>;
+                return launch_kernel<k, k, ks, ks>(p, scale, grid_rc, C::THREADS, C::SMEM_BYTES, stream);
+            }
+            constexpr auto k = fft_rc_ilv_kernel<T, LOG2N, LOG2E, S::TBC, false, false>;
+            constexpr auto ks = fft_rc_ilv_kernel<T, LOG2N, LOG2E, S::TBC, false, true>;
+            return launch_kernel<k, k, ks, ks>(p, scale, grid_rc, C::THREADS, C::SMEM_BYTES, stream);
+        }
         case PASS_R2C: {
             if (p.in.nseg != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
             if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;

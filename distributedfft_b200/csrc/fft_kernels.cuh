@@ -79,9 +79,12 @@ using KParams = std::conditional_t<SCALED, FftScaled, FftParams>;
 
 // PASS_R2R_*: the view mapping of PASS_C2C_* over real elements (fft_r2r_kernel).  PASS_COPY_*: the views of a C2C or R2R
 // pass over an axis the plan keeps, moved without a transform (fft_copy_kernel)
+// PASS_C2C_ILV: the z pass of an interleaved plan (dfft_plan_create_interleaved), the view mapping of PASS_C2C_TILED with
+// b = the component (B = C, sN = C): fft_c2c_ilv_kernel, or the TILED kernel once C fills its tile.  PASS_R2C_ILV /
+// PASS_C2R_ILV: its R2C / C2R z pass of Nz-point paired lines (fft_rc_ilv_kernel), the real side counted in reals
 enum PassKind {
     PASS_C2C_CONTIG = 0, PASS_C2C_TILED = 1, PASS_R2C = 2, PASS_C2R = 3, PASS_R2R_CONTIG = 4, PASS_R2R_TILED = 5,
-    PASS_COPY_CONTIG = 6, PASS_COPY_TILED = 7
+    PASS_COPY_CONTIG = 6, PASS_COPY_TILED = 7, PASS_C2C_ILV = 8, PASS_R2C_ILV = 9, PASS_C2R_ILV = 10
 };
 
 // ---- tile shape choices (compile time) -----------------------------------------------------------
@@ -287,8 +290,9 @@ __device__ __forceinline__ void tiled_decode(const FftParams& p, long long tile,
     tile_order(p, int(tile / nbt), a1, a0);
 }
 
-// common prologue: thread -> (j, t), tile -> (a0, a1, b), segment tables
-template <typename C, bool TILED, int TB>
+// common prologue: thread -> (j, t), tile -> (a0, a1, b), segment tables.  ILV (CONTIG mapping only): the lines are the
+// (a0, a1, b) triples with b fastest — the B interleaved components of a row are neighbouring lines of one CTA
+template <typename C, bool TILED, int TB, bool ILV = false>
 struct TileCoord {
     int j, t, a0, a1, b;
     bool valid;
@@ -301,6 +305,13 @@ struct TileCoord {
             tiled_decode<TB>(p, tile, bt, a1, a0);
             b = bt * TB + t;
             valid = b < p.B;
+        } else if constexpr (ILV) {
+            const long long line = tile * TB + t;
+            valid = line < (long long)p.A0 * p.A1 * p.B;
+            b = int(line % p.B);
+            const long long row = line / p.B;
+            a1 = int(row % p.A1);
+            a0 = int(row / p.A1);
         } else {
             const long long line = tile * TB + t;
             valid = line < (long long)p.A0 * p.A1;
@@ -311,6 +322,7 @@ struct TileCoord {
     }
     static __device__ __forceinline__ long long num_tiles(const FftParams& p) {
         if constexpr (TILED) return (long long)p.A0 * p.A1 * ((p.B + TB - 1) / TB);
+        else if constexpr (ILV) return ((long long)p.A0 * p.A1 * p.B + TB - 1) / TB;
         else return ((long long)p.A0 * p.A1 + TB - 1) / TB;
     }
 };
@@ -401,12 +413,15 @@ __device__ __forceinline__ void l2_discard(const void* p) { asm volatile("discar
 
 // ---- one tile of a C2C pass: load, CtaFft::stages, store --------------------------------------------------
 // PADDED: the spectral side (out forward, in inverse) keeps the line positions outside the hole [lo, hi) (FftPadded).
-template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, typename M, typename Hook = NoGatherHook, bool PADDED = false>
+// ILV (CONTIG mapping): lines of an interleaved z pass, strided by sN along n (TileCoord)
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, typename M, typename Hook = NoGatherHook, bool PADDED = false,
+          bool ILV = false>
 __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<T>* sm, unsigned long long* tab_in, unsigned long long* tab_out,
                                          bool multi, const M& mem, const Hook& after_gather = {}, int lo = 0, int hi = 0) {
     using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
     using LA = LineAccess<T, C::LINES>;
-    using TC = TileCoord<C, TILED, TB>;
+    using TC = TileCoord<C, TILED, TB, ILV>;
+    constexpr bool STRIDED = TILED || ILV;
     constexpr int E = C::E, TPL = C::TPL;
     const TC tc(p, tile);
     const int j = tc.j, t = tc.t;
@@ -429,10 +444,10 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
 #pragma unroll
             for (int e = 0; e < E; ++e) {
                 const int m = keep_index(j + e * TPL, lo, hi);
-                v[e] = m < 0 ? cx<T>{T(0), T(0)} : mem.ld(TILED ? in.at(m) : in.at1(m));
+                v[e] = m < 0 ? cx<T>{T(0), T(0)} : mem.ld(STRIDED ? in.at(m) : in.at1(m));
             }
         } else if (!in.multi) {
-            if constexpr (!TILED) {
+            if constexpr (!STRIDED) {
                 // contiguous line: sN == 1, immediate offsets
                 const cx<T>* q = in.p0 + j;
 #pragma unroll
@@ -445,7 +460,7 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
             }
         } else {
 #pragma unroll
-            for (int e = 0; e < E; ++e) v[e] = mem.ld(TILED ? in.at(j + e * TPL) : in.at1(j + e * TPL));
+            for (int e = 0; e < E; ++e) v[e] = mem.ld(STRIDED ? in.at(j + e * TPL) : in.at1(j + e * TPL));
         }
         if constexpr (INV) {
 #pragma unroll
@@ -463,10 +478,10 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
 #pragma unroll
             for (int e = 0; e < E; ++e) {
                 const int m = keep_index(j + e * TPL, lo, hi);
-                if (m >= 0) mem.st(TILED ? out.at(m) : out.at1(m), v[C::Core::final_slot(e)]);
+                if (m >= 0) mem.st(STRIDED ? out.at(m) : out.at1(m), v[C::Core::final_slot(e)]);
             }
         } else if (!out.multi) {
-            if constexpr (!TILED) {
+            if constexpr (!STRIDED) {
                 cx<T>* q = out.p0 + j;
 #pragma unroll
                 for (int e = 0; e < E; ++e) {
@@ -487,7 +502,7 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
 #pragma unroll
             for (int e = 0; e < E; ++e) {
                 const cx<T> x = v[C::Core::final_slot(e)];
-                mem.st(TILED ? out.at(j + e * TPL) : out.at1(j + e * TPL), INV ? cswap(x) : x);
+                mem.st(STRIDED ? out.at(j + e * TPL) : out.at1(j + e * TPL), INV ? cswap(x) : x);
             }
         }
     }
@@ -519,6 +534,129 @@ fft_c2c_kernel(const __grid_constant__ KParams<SCALED> p) {
             // the segment tables are rewritten
             if (multi) __syncthreads();
             else if constexpr (C::NST > 1) C::sync(t);
+        }
+    }
+}
+
+// Interleaved z pass (PASS_C2C_ILV, C = p.B components per point, below the TILED tile width): the CONTIG shape with its
+// TB lines taken as consecutive (row, component) pairs, so a CTA's lines cover whole runs of [row][N][C] and the strided
+// accesses of one component are served by the same sectors as its neighbours'.  Same core, stage plan and tables as the
+// CONTIG kernel: bit-identical lines.  Grid-stride like fft_c2c_kernel (max_ctas).
+template <typename T, int LOG2N, int LOG2E, int TB, bool INV, bool SCALED>
+__global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
+fft_c2c_ilv_kernel(const __grid_constant__ KParams<SCALED> p) {
+    using C = CtaFft<T, LOG2N, LOG2E, TB, false>;
+    using TC = TileCoord<C, false, TB, true>;
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
+    unsigned long long* tab_in = reinterpret_cast<unsigned long long*>(smem_raw + C::TILE_BYTES);
+    unsigned long long* tab_out = tab_in + C::LINES * MAXSEG;
+    const bool multi = p.in.nseg > 1 || p.out.nseg > 1;
+    const long long ntiles = TC::num_tiles(p);
+
+#pragma unroll 1
+    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        if constexpr (SCALED)
+            c2c_tile<T, LOG2N, LOG2E, TB, false, INV, MemScaled<T, MemPlain<T>>, NoGatherHook, false, true>(p, tile, sm, tab_in, tab_out, multi,
+                                                                                                       MemScaled<T, MemPlain<T>>{{}, T(p.scale)});
+        else c2c_tile<T, LOG2N, LOG2E, TB, false, INV, MemPlain<T>, NoGatherHook, false, true>(p, tile, sm, tab_in, tab_out, multi, MemPlain<T>{});
+        if (tile + gridDim.x < ntiles) {
+            if (multi) __syncthreads();
+            else if constexpr (C::NST > 1) C::sync(int(threadIdx.x) / C::TPL);
+        }
+    }
+}
+
+// Paired R2C / C2R z pass of interleaved plans (PASS_R2C_ILV / PASS_C2R_ILV, C = p.B components per point, r2r.hpp): the
+// CONTIG shape with its TB lines taken as consecutive (row, component pair) items; components c, c + 1 ride one complex
+// N-point line (N = Nz), an odd C gives the last one a zero partner that stores nothing.  The real side is one segment
+// counted in reals (element (a0, a1, n, c) at base + a0 sA0 + a1 sA1 + n sN + c), the complex side a view with b the
+// component (segment tables along z for scatters and gathers).  R2C: after the stages Z goes through the line's shared
+// memory once, each thread splits its k <= N/2 with Z[N - k].  C2R: each thread builds Z[k] from X[k] or conj X[N - k] of both
+// components, straight from global memory.  Reals are loaded and stored one by one, so every C works (a pair is only
+// aligned for an even C).  Grid-stride like fft_c2c_kernel (max_ctas).
+template <typename T, int LOG2N, int LOG2E, int TB, bool C2R, bool SCALED>
+__global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
+fft_rc_ilv_kernel(const __grid_constant__ KParams<SCALED> p) {
+    using Cf = CtaFft<T, LOG2N, LOG2E, TB, false>;
+    using LA = LineAccess<T, TB>;
+    constexpr int E = Cf::E, TPL = Cf::TPL, N = Cf::N;
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
+    unsigned long long* tab = reinterpret_cast<unsigned long long*>(smem_raw + Cf::TILE_BYTES);
+    const View& rv = C2R ? p.out : p.in;
+    const View& cv = C2R ? p.in : p.out;
+    const bool multi = cv.nseg > 1;
+    const int C = p.B, pairs = (p.B + 1) / 2;
+    const long long nlines = (long long)p.A0 * p.A1 * pairs;
+    const long long ntiles = (nlines + TB - 1) / TB;
+    const int j = int(threadIdx.x) % TPL, t = int(threadIdx.x) / TPL;
+    T s = T(1);
+    if constexpr (SCALED) s = T(p.scale);
+    const cx<T>* tw = reinterpret_cast<const cx<T>*>(p.tw);
+
+#pragma unroll 1
+    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const long long line = tile * TB + t;
+        const bool valid = line < nlines;
+        const int ca = int(line % pairs) * 2;
+        const long long row = line / pairs;
+        const int a1 = int(row % p.A1), a0 = int(row / p.A1);
+        const bool hasb = ca + 1 < C;
+        if (multi) {
+            LA::fill_table(cv, tab, t, j, TPL, a0, a1);
+            __syncthreads();
+        }
+        const LA xa(cv, tab, t, a0, a1, ca), xb(cv, tab, t, a0, a1, ca + 1);
+        T* r0 = reinterpret_cast<T*>(rv.seg[0].base) + ((long long)a0 * rv.seg[0].sA0 + (long long)a1 * rv.seg[0].sA1 + ca);
+        cx<T> v[E];
+        if constexpr (!C2R) {
+#pragma unroll
+            for (int e = 0; e < E; ++e) {
+                const long long o = (long long)(j + e * TPL) * rv.sN;
+                v[e] = valid ? cx<T>{r0[o], hasb ? r0[o + 1] : T(0)} : cx<T>{T(0), T(0)};
+            }
+            Cf::template stages<0>(v, j, t, sm, tw);
+            Cf::sync(t);  // the line's last gather has left shared memory
+#pragma unroll
+            for (int e = 0; e < E; ++e) sm[Cf::sidx(j + e * TPL, t)] = v[Cf::Core::final_slot(e)];
+            Cf::sync(t);
+            if (valid) {
+#pragma unroll
+                for (int e = 0; e < E; ++e) {
+                    const int k = j + e * TPL;
+                    if (2 * k > N) continue;
+                    cx<T> ya, yb;
+                    rc_pair_split<T>(sm[Cf::sidx(k, t)], sm[Cf::sidx((N - k) & (N - 1), t)], ya, yb);
+                    if constexpr (SCALED) { ya = cscale<T>(ya, s); yb = cscale<T>(yb, s); }
+                    st_elem<T>(xa.at(k), ya);
+                    if (hasb) st_elem<T>(xb.at(k), yb);
+                }
+            }
+        } else {
+#pragma unroll
+            for (int e = 0; e < E; ++e) {
+                const int k = j + e * TPL, m = rc_pair_in_k(k, N);
+                cx<T> z{T(0), T(0)};
+                if (valid) z = rc_pair_build<T>(ld_elem<T>(xa.at(m)), hasb ? ld_elem<T>(xb.at(m)) : cx<T>{T(0), T(0)}, k, N);
+                v[e] = cswap(z);
+            }
+            Cf::template stages<0>(v, j, t, sm, tw);
+            if (valid) {
+#pragma unroll
+                for (int e = 0; e < E; ++e) {
+                    cx<T> z = cswap(v[Cf::Core::final_slot(e)]);
+                    if constexpr (SCALED) z = cscale<T>(z, s);
+                    const long long o = (long long)(j + e * TPL) * rv.sN;
+                    r0[o] = z.x;
+                    if (hasb) r0[o + 1] = z.y;
+                }
+            }
+        }
+        if (tile + gridDim.x < ntiles) {
+            // the next tile's first scatter (and, multi-segment, its tables) must not overtake this tile's shared-memory reads
+            if (multi) __syncthreads();
+            else Cf::sync(t);
         }
     }
 }

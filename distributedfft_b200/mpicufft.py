@@ -124,7 +124,8 @@ class MPIcuFFT:
 
     # -- plan ------------------------------------------------------------------------------------
     def initFFT(self, global_size: GlobalSize, partition: Optional[Partition] = None, allocate: bool = True, batch: int = 1,
-                inplace: bool = False, transform_axes: Optional[Sequence[bool]] = None, spectral: Optional[Sequence[int]] = None):
+                inplace: bool = False, transform_axes: Optional[Sequence[bool]] = None, spectral: Optional[Sequence[int]] = None,
+                components: int = 1):
         """`batch` (not in the reference): every exec transforms that many fields, back to back in each buffer — a
         contiguous [batch, X, Y, Z] tensor; the getters describe one field (dfft_plan_create_batched).
         `inplace` (dfft_plan_create_inplace): every exec gets the same buffer twice and overwrites its input; fields are
@@ -132,7 +133,10 @@ class MPIcuFFT:
         torch.view_as_real(buf).view(X, Y, Nz + 2) as the real side.
         `transform_axes` (x, y, z): setTransformAxes right after creation, e.g. (False, True, True) keeps x.
         `spectral` (kx, ky, kz) (dfft_plan_create_padded): a padded plan, global_size the physical grid and (kx, ky, kz) the
-        spectrum it keeps — the forward stores only those modes, the inverse zero-pads them (the 3/2 dealiasing rule)."""
+        spectrum it keeps — the forward stores only those modes, the inverse zero-pads them (the 3/2 dealiasing rule).
+        `components` C (dfft_plan_create_interleaved): every grid point holds C consecutive values, each component
+        transformed on its own — buffers are [X, Y, Z, C] tensors ([B, X, Y, Z, C] with a batch), reals on the real side
+        of R2C / C2R; C > 1 plans are C2C or R2C / C2R, out of place and not padded."""
         if global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         cfg = _lib.dfft_config(int(self.config.cuda_aware), int(self.config.warmup_rounds), int(self.config.comm_method),
@@ -144,7 +148,15 @@ class MPIcuFFT:
         if self._decomp == PENCIL and partition is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         h = C.c_void_p()
-        if spectral is not None:
+        if components != 1:
+            if spectral is not None or inplace or self.kinds is not None:
+                raise ValueError("interleaved plans are out of place and not padded")
+            if batch < 1:
+                raise ValueError("batch must be at least 1")
+            check(lib().dfft_plan_create_interleaved(self.comm._h, C.byref(cfg), self._decomp, self.precision, self.transform,
+                                                     global_size.Nx, global_size.Ny, global_size.Nz, p1, p2, int(components), batch,
+                                                     1 if allocate else 0, C.byref(h)))
+        elif spectral is not None:
             if inplace or self.kinds is not None:
                 raise ValueError("padded plans are out of place and C2C or R2C")
             if batch < 1:
@@ -291,6 +303,7 @@ class MPIcuFFT:
     def getDomainSize(self): return int(lib().dfft_get_domain_size(self._h))
     def getSpectralSize(self): return self._triple(lib().dfft_plan_get_spectral_size)
     def getBatch(self): return int(lib().dfft_get_batch(self._h))
+    def getComponents(self): return int(lib().dfft_get_components(self._h))
     def isInPlace(self): return bool(lib().dfft_plan_is_inplace(self._h))
     def getWorkSizeDevice(self): return int(lib().dfft_get_work_size_device(self._h))
     def getWorkSizeHost(self): return int(lib().dfft_get_work_size_host(self._h))
@@ -360,13 +373,13 @@ class MPIcuFFT_Pencil(MPIcuFFT):
     """z FFT -> transpose -> y FFT -> transpose -> x FFT on a P1 x P2 grid. include/mpicufft_pencil.hpp."""
     _decomp = PENCIL
 
-    def initFFT(self, global_size, partition=None, allocate=True, batch=1, inplace=False, transform_axes=None, spectral=None):
+    def initFFT(self, global_size, partition=None, allocate=True, batch=1, inplace=False, transform_axes=None, spectral=None, components=1):
         if partition is None or global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         if partition.P1 * partition.P2 != self.comm.size:
             raise RuntimeError("Invalid Input Partition!")
         self.partition = partition
-        super().initFFT(global_size, partition, allocate, batch, inplace, transform_axes, spectral)
+        super().initFFT(global_size, partition, allocate, batch, inplace, transform_axes, spectral, components)
 
     def getPartitionDimensions(self):
         """(input_dim, transposed_dim, output_dim), each a dict with size_x/y/z and start_x/y/z lists

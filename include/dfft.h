@@ -199,6 +199,30 @@ int dfft_plan_create_padded(dfft_comm_t comm, const dfft_config* config, int dec
                             size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan);
 /* k[0..2] = kx, ky, kz of a padded plan; nx, ny, nz for every other plan. */
 int dfft_plan_get_spectral_size(dfft_plan_t plan, size_t k[3]);
+/* Interleaved multi-component plans (FFTW-MPI's `howmany`): every grid point holds `components` consecutive values,
+ * and each component is transformed on its own.
+ *   - Every caller layout is that of the components = 1 plan with each element widened to C = components consecutive
+ *     values: input [in_size[0]][in_size[1]][in_size[2]][C], output [out_size[0]][out_size[1]][out_size[2]][C], partial d
+ *     likewise (torch tensors [X, Y, Z, C], with a batch [B, X, Y, Z, C]).  Component c of the output is the
+ *     components = 1 transform of component c of the input.
+ *   - The getters and dfft_layout describe the 3-D extents of one component; dfft_get_domain_size and
+ *     dfft_get_work_size_device count all C.  `batch` fields of C components each sit back to back.
+ *   - components = 1 makes the plan of dfft_plan_create_batched: the same steps, description and output.
+ *   - Peer2Peer / All2All, every decomposition, partial d, uneven splits, batches, the output scale, graph capture of
+ *     one-rank _async execs, the timer and dfft_debug_run_step work as for other plans.  C > 1 plans run the sequential
+ *     schedule (dfft_plan_tune has one candidate); dfft_plan_describe adds "components" and lists the C2C z pass as
+ *     kind 8, a TILED view mapping with b = the component, and the R2C / C2R z pass as kind 9 / 10, Nz-point lines whose
+ *     real side is counted in reals.
+ *   - C2C and R2C / C2R.  R2C / C2R pair components c, c + 1 as one complex Nz-point line in the z pass, so their
+ *     output matches the batched plan's within rounding; C2C output equals it bit for bit.
+ *   - components = 0, or a batch x components whose buffers overflow size_t: DFFT_ERR_INVALID; components > 64:
+ *     DFFT_ERR_UNSUPPORTED.  With components > 1, R2R transforms, a z length that is not a power of two, an R2C / C2R Nz
+ *     of 16384 (the paired z pass runs Nz-point lines) and dfft_plan_set_transform_axes other than {1, 1, 1}:
+ *     DFFT_ERR_UNSUPPORTED.  No in-place or padded form. */
+int dfft_plan_create_interleaved(dfft_comm_t comm, const dfft_config* config, int decomp /*dfft_decomp*/, int precision /*dfft_prec*/,
+                                 int transform /*dfft_transform*/, size_t nx, size_t ny, size_t nz, size_t p1, size_t p2,
+                                 size_t components, size_t batch, int allocate, dfft_plan_t* plan);
+size_t dfft_get_components(dfft_plan_t plan); /* 1 for every other plan, 0 for a null plan */
 int dfft_plan_destroy(dfft_plan_t plan);
 /* setWorkArea(device, host) — mpicufft_slab.cpp:236-281. device must hold dfft_get_work_size_device()
  * bytes; with comm_method Peer2Peer and more than one rank it must be the base of a cudaMalloc

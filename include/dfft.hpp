@@ -106,6 +106,15 @@ public:
         spectral_ = spectral;
         initFFT(global_size, partition, allocate, batch);
     }
+    // not in the reference: an interleaved plan (dfft_plan_create_interleaved): every grid point holds `components`
+    // consecutive values, each component transformed on its own ([x][y][z][C] buffers).  A named method, so that it cannot
+    // be mistaken for the (batch, inplace) overload.
+    void initFFTInterleaved(GlobalSize* global_size, Partition* partition, size_t components, bool allocate = true, size_t batch = 1) {
+        struct Reset { size_t& c; ~Reset() { c = 1; } } reset{components_};
+        components_ = components;
+        initFFT(global_size, partition, allocate, batch);
+    }
+    size_t getComponents() const { return dfft_get_components(plan); }
     // kx, ky, kz of a padded plan; Nx, Ny, Nz of every other plan
     void getSpectralSize(size_t* k) const { DFFT_CALL(dfft_plan_get_spectral_size(plan, k)); }
     size_t getBatch() const { return dfft_get_batch(plan); }
@@ -151,7 +160,10 @@ protected:
         c.benchmark_dir = config.benchmark_dir.empty() ? nullptr : config.benchmark_dir.c_str();
         c.comm_method2 = config.comm_method2; c.send_method2 = config.send_method2;
         if (plan) { dfft_plan_destroy(plan); plan = nullptr; }
-        if (spectral_)
+        if (components_ != 1)
+            DFFT_CALL(dfft_plan_create_interleaved(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, p1, p2,
+                                                   components_, batch_, allocate ? 1 : 0, &plan));
+        else if (spectral_)
             DFFT_CALL(dfft_plan_create_padded(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, spectral_->Nx, spectral_->Ny,
                                               spectral_->Nz, p1, p2, batch_, allocate ? 1 : 0, &plan));
         else if (per_axis)
@@ -170,6 +182,7 @@ protected:
     size_t batch_ = 1;       // fields of the plan initFFT is creating
     bool inplace_ = false;   // whether initFFT is creating an in-place plan
     GlobalSize* spectral_ = nullptr;  // the spectrum of the padded plan initFFT is creating
+    size_t components_ = 1;  // values per point of the interleaved plan initFFTInterleaved is creating
     Configurations config;
     dfft_comm_t comm;
     int transform;
