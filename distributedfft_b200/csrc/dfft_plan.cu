@@ -2342,7 +2342,8 @@ static void drop_identity_copies(const dfft_plan_s* p, Schedule& sc) {
 // Interleaved plans: build_schedule lays out points of C values (its byte offsets count C * esize); the kernels address
 // single values.  So every stride scales by C, a pass whose contiguous dimension is z sees C columns per z point, the z
 // pass runs lines C apart with b the component (PASS_C2C_ILV: B = C, sN = C), and all-to-all counts are in values.  The
-// R2C / C2R z pass becomes the paired pass of Nz-point lines (PASS_R2C_ILV / PASS_C2R_ILV) with the Nz-point twiddle table;
+// R2C / C2R z pass becomes the pass of Nz-point lines, one per component (PASS_R2C_ILV / PASS_C2R_ILV), with the Nz-point
+// twiddle table;
 // its real side, built in complex units of Nz / 2 per row, is counted in reals (element (a0, a1, n, c) at
 // base + a0 sA0 + a1 sA1 + n C + c).
 static int widen_views(dfft_plan_s* p, Schedule& sc) {
@@ -2881,7 +2882,7 @@ int dfft_plan_create_padded(dfft_comm_t comm, const dfft_config* config, int dec
 }
 
 // C values per point: the C = 1 plan with every element widened to C consecutive values (DESIGN.md section 3.14).  The
-// z pass of C > 1 runs interleaved lines (PASS_C2C_ILV) or paired R2C / C2R lines of Nz points (PASS_R2C_ILV /
+// z pass of C > 1 runs interleaved lines (PASS_C2C_ILV) or R2C / C2R lines of Nz points, one per component (PASS_R2C_ILV /
 // PASS_C2R_ILV), which exist for a power-of-two Nz (R2C: up to 8192).
 constexpr size_t MAX_COMPONENTS = 64;
 int dfft_plan_create_interleaved(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
@@ -2892,7 +2893,7 @@ int dfft_plan_create_interleaved(dfft_comm_t comm, const dfft_config* config, in
         if (transform != DFFT_C2C && transform != DFFT_R2C && !is_r2r(transform)) return fail(DFFT_ERR_INVALID, "bad transform");
         if (is_r2r(transform)) return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans with more than one component are C2C or R2C / C2R");
         if (ilog2_exact(nz) < 1) return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans need a power-of-two Nz (x and y may have any C2C length)");
-        // the paired R2C / C2R z pass runs Nz-point complex lines
+        // the interleaved R2C / C2R z pass runs Nz-point complex lines
         if (transform == DFFT_R2C && ilog2_exact(nz) > MAX_LOG2N)
             return fail(DFFT_ERR_UNSUPPORTED, "interleaved R2C / C2R plans need Nz <= " + std::to_string(1 << MAX_LOG2N));
     }
@@ -3614,7 +3615,7 @@ int dfft_debug_run_step(dfft_plan_t p, int inverse, int d, size_t field, int ste
     struct Range { const char *lo, *hi, *buf; size_t bytes; };
     std::vector<Range> ranges;
     std::vector<std::pair<View*, const std::vector<unsigned char>*>> tables;
-    // bytes per view element: reals on the real side of the paired R2C / C2R pass of interleaved plans
+    // bytes per view element: reals on the real side of the R2C / C2R pass of interleaved plans
     auto resolve = [&](View& v, int user, size_t n_len, View& launched, size_t ebytes) -> int {
         if (v.nseg < 1 || v.nseg > MAXSEG || (user && v.nseg != 1)) return fail(DFFT_ERR_STATE, "internal: view segments");
         const std::vector<unsigned char>* tab = nullptr;
@@ -3653,7 +3654,7 @@ int dfft_debug_run_step(dfft_plan_t p, int inverse, int d, size_t field, int ste
         return DFFT_SUCCESS;
     };
     // points along n of each view: padded passes hold `keep` on their spectral side (out forward, in inverse)
-    // (the paired R2C / C2R pass: Nz reals, Nz / 2 + 1 complex points)
+    // (the interleaved R2C / C2R pass: Nz reals, Nz / 2 + 1 complex points)
     size_t in_len = s.keep && s.prm.inverse ? s.keep : len + (s.kind == PASS_C2R ? 1 : 0);
     size_t out_len = s.keep && !s.prm.inverse ? s.keep : len + (s.kind == PASS_R2C ? 1 : 0);
     if (s.kind == PASS_R2C_ILV) out_len = len / 2 + 1;

@@ -200,10 +200,10 @@ cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStr
         }
         case PASS_R2C_ILV:
         case PASS_C2R_ILV: {
-            // C = B components, (C + 1) / 2 paired lines per row; the real side is one segment
+            // C = B components, one line per component; the real side is one segment
             const bool c2r = kind == PASS_C2R_ILV;
             if (p.B < 1 || (c2r ? p.out.nseg : p.in.nseg) != 1) return cudaErrorInvalidValue;
-            const long long g = (lines * ((p.B + 1) / 2) + S::TBC - 1) / S::TBC;
+            const long long g = (lines * p.B + S::TBC - 1) / S::TBC;
             if (g > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
             const unsigned grid_rc = unsigned((p.max_ctas > 0 && g > p.max_ctas) ? p.max_ctas : g);
             if (c2r) {

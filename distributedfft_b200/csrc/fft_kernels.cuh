@@ -81,7 +81,7 @@ using KParams = std::conditional_t<SCALED, FftScaled, FftParams>;
 // pass over an axis the plan keeps, moved without a transform (fft_copy_kernel)
 // PASS_C2C_ILV: the z pass of an interleaved plan (dfft_plan_create_interleaved), the view mapping of PASS_C2C_TILED with
 // b = the component (B = C, sN = C): fft_c2c_ilv_kernel, or the TILED kernel once C fills its tile.  PASS_R2C_ILV /
-// PASS_C2R_ILV: its R2C / C2R z pass of Nz-point paired lines (fft_rc_ilv_kernel), the real side counted in reals
+// PASS_C2R_ILV: its R2C / C2R z pass of Nz-point lines, one per component (fft_rc_ilv_kernel), the real side counted in reals
 enum PassKind {
     PASS_C2C_CONTIG = 0, PASS_C2C_TILED = 1, PASS_R2C = 2, PASS_C2R = 3, PASS_R2R_CONTIG = 4, PASS_R2R_TILED = 5,
     PASS_COPY_CONTIG = 6, PASS_COPY_TILED = 7, PASS_C2C_ILV = 8, PASS_R2C_ILV = 9, PASS_C2R_ILV = 10
@@ -567,14 +567,13 @@ fft_c2c_ilv_kernel(const __grid_constant__ KParams<SCALED> p) {
     }
 }
 
-// Paired R2C / C2R z pass of interleaved plans (PASS_R2C_ILV / PASS_C2R_ILV, C = p.B components per point, r2r.hpp): the
-// CONTIG shape with its TB lines taken as consecutive (row, component pair) items; components c, c + 1 ride one complex
-// N-point line (N = Nz), an odd C gives the last one a zero partner that stores nothing.  The real side is one segment
-// counted in reals (element (a0, a1, n, c) at base + a0 sA0 + a1 sA1 + n sN + c), the complex side a view with b the
+// R2C / C2R z pass of interleaved plans (PASS_R2C_ILV / PASS_C2R_ILV, C = p.B components per point, r2r.hpp): the CONTIG
+// shape with its TB lines taken as consecutive (row, component) items; every component runs its own complex N-point line
+// (N = Nz) with a zero imaginary part, so each component's result depends on that component alone.  The real side is one
+// segment counted in reals (element (a0, a1, n, c) at base + a0 sA0 + a1 sA1 + n sN + c), the complex side a view with b the
 // component (segment tables along z for scatters and gathers).  R2C: after the stages Z goes through the line's shared
-// memory once, each thread splits its k <= N/2 with Z[N - k].  C2R: each thread builds Z[k] from X[k] or conj X[N - k] of both
-// components, straight from global memory.  Reals are loaded and stored one by one, so every C works (a pair is only
-// aligned for an even C).  Grid-stride like fft_c2c_kernel (max_ctas).
+// memory once, each thread splits its k <= N/2 with Z[N - k].  C2R: each thread builds Z[k] from X[k] or conj X[N - k],
+// straight from global memory.  Grid-stride like fft_c2c_kernel (max_ctas).
 template <typename T, int LOG2N, int LOG2E, int TB, bool C2R, bool SCALED>
 __global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
 fft_rc_ilv_kernel(const __grid_constant__ KParams<SCALED> p) {
@@ -587,8 +586,8 @@ fft_rc_ilv_kernel(const __grid_constant__ KParams<SCALED> p) {
     const View& rv = C2R ? p.out : p.in;
     const View& cv = C2R ? p.in : p.out;
     const bool multi = cv.nseg > 1;
-    const int C = p.B, pairs = (p.B + 1) / 2;
-    const long long nlines = (long long)p.A0 * p.A1 * pairs;
+    const int C = p.B;
+    const long long nlines = (long long)p.A0 * p.A1 * C;
     const long long ntiles = (nlines + TB - 1) / TB;
     const int j = int(threadIdx.x) % TPL, t = int(threadIdx.x) / TPL;
     T s = T(1);
@@ -599,22 +598,21 @@ fft_rc_ilv_kernel(const __grid_constant__ KParams<SCALED> p) {
     for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const long long line = tile * TB + t;
         const bool valid = line < nlines;
-        const int ca = int(line % pairs) * 2;
-        const long long row = line / pairs;
+        const int c = int(line % C);
+        const long long row = line / C;
         const int a1 = int(row % p.A1), a0 = int(row / p.A1);
-        const bool hasb = ca + 1 < C;
         if (multi) {
             LA::fill_table(cv, tab, t, j, TPL, a0, a1);
             __syncthreads();
         }
-        const LA xa(cv, tab, t, a0, a1, ca), xb(cv, tab, t, a0, a1, ca + 1);
-        T* r0 = reinterpret_cast<T*>(rv.seg[0].base) + ((long long)a0 * rv.seg[0].sA0 + (long long)a1 * rv.seg[0].sA1 + ca);
+        const LA x(cv, tab, t, a0, a1, c);
+        T* r0 = reinterpret_cast<T*>(rv.seg[0].base) + ((long long)a0 * rv.seg[0].sA0 + (long long)a1 * rv.seg[0].sA1 + c);
         cx<T> v[E];
         if constexpr (!C2R) {
 #pragma unroll
             for (int e = 0; e < E; ++e) {
                 const long long o = (long long)(j + e * TPL) * rv.sN;
-                v[e] = valid ? cx<T>{r0[o], hasb ? r0[o + 1] : T(0)} : cx<T>{T(0), T(0)};
+                v[e] = cx<T>{valid ? r0[o] : T(0), T(0)};
             }
             Cf::template stages<0>(v, j, t, sm, tw);
             Cf::sync(t);  // the line's last gather has left shared memory
@@ -626,30 +624,26 @@ fft_rc_ilv_kernel(const __grid_constant__ KParams<SCALED> p) {
                 for (int e = 0; e < E; ++e) {
                     const int k = j + e * TPL;
                     if (2 * k > N) continue;
-                    cx<T> ya, yb;
-                    rc_pair_split<T>(sm[Cf::sidx(k, t)], sm[Cf::sidx((N - k) & (N - 1), t)], ya, yb);
-                    if constexpr (SCALED) { ya = cscale<T>(ya, s); yb = cscale<T>(yb, s); }
-                    st_elem<T>(xa.at(k), ya);
-                    if (hasb) st_elem<T>(xb.at(k), yb);
+                    cx<T> y = rc_line_split<T>(sm[Cf::sidx(k, t)], sm[Cf::sidx((N - k) & (N - 1), t)]);
+                    if constexpr (SCALED) y = cscale<T>(y, s);
+                    st_elem<T>(x.at(k), y);
                 }
             }
         } else {
 #pragma unroll
             for (int e = 0; e < E; ++e) {
-                const int k = j + e * TPL, m = rc_pair_in_k(k, N);
+                const int k = j + e * TPL;
                 cx<T> z{T(0), T(0)};
-                if (valid) z = rc_pair_build<T>(ld_elem<T>(xa.at(m)), hasb ? ld_elem<T>(xb.at(m)) : cx<T>{T(0), T(0)}, k, N);
+                if (valid) z = rc_line_build<T>(ld_elem<T>(x.at(rc_line_in_k(k, N))), k, N);
                 v[e] = cswap(z);
             }
             Cf::template stages<0>(v, j, t, sm, tw);
             if (valid) {
 #pragma unroll
                 for (int e = 0; e < E; ++e) {
-                    cx<T> z = cswap(v[Cf::Core::final_slot(e)]);
-                    if constexpr (SCALED) z = cscale<T>(z, s);
-                    const long long o = (long long)(j + e * TPL) * rv.sN;
-                    r0[o] = z.x;
-                    if (hasb) r0[o + 1] = z.y;
+                    T z = cswap(v[Cf::Core::final_slot(e)]).x;
+                    if constexpr (SCALED) z *= s;
+                    r0[(long long)(j + e * TPL) * rv.sN] = z;
                 }
             }
         }

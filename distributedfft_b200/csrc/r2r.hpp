@@ -71,29 +71,28 @@ DFFT_HD cx<T> r2hc_build(T ak, T am, T bk, T bm, int k, int N) {
     return cx<T>{xa.x - xb.y, xa.y + xb.x};
 }
 
-// ---- paired R2C / C2R z pass of interleaved plans (fft_rc_ilv_kernel) -------------------------------------------------------
-// Components a = c and b = c + 1 of one point ride one complex Nz-point line z = x_a + i x_b (an odd C gives the last
-// component a zero partner whose results are not stored).  Z = DFT_N(z), m = -k mod N:
-//   R2C, k = 0 .. N/2:  X_a[k] = (Z[k] + conj Z[m]) / 2,  X_b[k] = (Z[k] - conj Z[m]) / 2i
-//   C2R:  Z[k] = X_a[k] + i X_b[k], with X[k] = conj X[N-k] above N/2 and the imaginary parts of X[0], X[N/2] dropped (as
-//         numpy's irfft does);  z = unnormalised inverse DFT_N(Z),  x_a = Re z,  x_b = Im z.
+// ---- R2C / C2R z pass of interleaved plans (fft_rc_ilv_kernel) ---------------------------------------------------------------
+// Every component runs its own complex Nz-point line z = x + 0i.  (Two components sharing one line as z = x_a + i x_b would
+// halve the arithmetic, but the split then leaves X_b with an error of u |x_a| rather than u |x_b|: components are
+// independent fields, so a small one next to a large one would lose its digits.)  Z = DFT_N(z), m = -k mod N:
+//   R2C, k = 0 .. N/2:  X[k] = (Z[k] + conj Z[m]) / 2  (the real part of z's spectrum, Hermitian by construction)
+//   C2R:  Z[k] = X[k], with X[k] = conj X[N-k] above N/2 and the imaginary parts of X[0], X[N/2] dropped (as numpy's irfft
+//         does);  z = unnormalised inverse DFT_N(Z),  x = Re z.
 // Unnormalised like cuFFT: C2R(R2C(x)) = N x.
 
-// forward: X_a[k] and X_b[k] from Z[k] and Z[-k mod N] (the halving is exact)
+// forward: X[k] from Z[k] and Z[-k mod N] (the halving is exact)
 template <typename T>
-DFFT_HD void rc_pair_split(cx<T> zk, cx<T> zm, cx<T>& xa, cx<T>& xb) {
-    xa = cx<T>{T(0.5) * (zk.x + zm.x), T(0.5) * (zk.y - zm.y)};
-    xb = cx<T>{T(0.5) * (zk.y + zm.y), T(0.5) * (zm.x - zk.x)};
+DFFT_HD cx<T> rc_line_split(cx<T> zk, cx<T> zm) {
+    return cx<T>{T(0.5) * (zk.x + zm.x), T(0.5) * (zk.y - zm.y)};
 }
 
-// inverse: Z[k] for k in [0, N) from the stored half spectra: xa, xb = X_a[k], X_b[k] for k <= N/2 (load at k), else
-// X_a[N-k], X_b[N-k] (load at N - k)
-DFFT_HD int rc_pair_in_k(int k, int N) { return 2 * k <= N ? k : N - k; }
+// inverse: Z[k] for k in [0, N) from the stored half spectrum: x = X[k] for k <= N/2 (load at k), else X[N-k] (load at N - k)
+DFFT_HD int rc_line_in_k(int k, int N) { return 2 * k <= N ? k : N - k; }
 template <typename T>
-DFFT_HD cx<T> rc_pair_build(cx<T> xa, cx<T> xb, int k, int N) {
-    if (k == 0 || 2 * k == N) { xa.y = T(0); xb.y = T(0); }
-    else if (2 * k > N) { xa.y = -xa.y; xb.y = -xb.y; }
-    return cx<T>{xa.x - xb.y, xa.y + xb.x};
+DFFT_HD cx<T> rc_line_build(cx<T> x, int k, int N) {
+    if (k == 0 || 2 * k == N) x.y = T(0);
+    else if (2 * k > N) x.y = -x.y;
+    return x;
 }
 
 }  // namespace dfft

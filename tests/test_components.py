@@ -55,7 +55,7 @@ def describe_ilv(rank, P, decomp, transform, shape, p1, p2, comps, batch, comm_m
 
 def run_interleaved(P, decomp, shape, p1, p2, comm_method, inverse, d, comps, batch=1, scale=1.0, transform=dfft.C2C):
     """Replays an interleaved exec on every rank; returns the worst rel-L2 error over fields, components and ranks.  R2C /
-    C2R: the z pass is the paired pass (kinds 9 / 10) whose real side is counted in reals."""
+    C2R: the z pass is the interleaved R2C / C2R pass (kinds 9 / 10) whose real side is counted in reals."""
     nx, ny, nz = shape
     c2c = transform == dfft.C2C
     scheds = [describe_ilv(r, P, decomp, transform, shape, p1, p2, comps, batch, comm_method, inverse, d, scale) for r in range(P)]
@@ -212,7 +212,7 @@ def test_interleaved_partial_schedules(d, inverse, comm):
 
 
 R2C_CASES = [
-    # P, decomp, shape, p1, p2, comm, C — odd and even C (zero partner), multi-segment z scatter / gather, blocked tails
+    # P, decomp, shape, p1, p2, comm, C — odd and even C, multi-segment z scatter / gather, blocked tails
     (1, SL, (8, 16, 64), 1, 1, P2P, 3),
     (1, PE, (8, 8, 16), 1, 1, P2P, 2),
     (2, SL, (8, 8, 128), 2, 1, P2P, 5),
@@ -228,7 +228,7 @@ R2C_CASES = [
 @pytest.mark.parametrize("P,decomp,shape,p1,p2,comm,comps", R2C_CASES)
 @pytest.mark.parametrize("inverse", [0, 1])
 def test_interleaved_r2c_schedules(P, decomp, shape, p1, p2, comm, comps, inverse):
-    """the paired R2C / C2R z pass and the complex passes behind it"""
+    """the interleaved R2C / C2R z pass and the complex passes behind it"""
     assert run_interleaved(P, decomp, shape, p1, p2, comm, inverse, 3, comps, transform=dfft.R2C) < 1e-12
 
 
@@ -240,9 +240,9 @@ def test_interleaved_r2c_partial_batch_scale(d, inverse):
     assert run_interleaved(4, SL, (8, 8, 32), 4, 1, P2P, inverse, 3, 5, batch=2, scale=1.5, transform=dfft.R2C) < 1e-12
 
 
-def test_paired_split_matches_naive():
-    """tests/emu_rc_pair.cpp: the paired R2C / C2R per-line steps against a long-double DFT, Nz = 4..8192, with a partner and
-    with a zero partner (odd C); rel-L2 <= 1e-15 (f64) / 1e-6 (f32)"""
+def test_rc_line_matches_naive():
+    """tests/emu_rc_pair.cpp: the R2C / C2R per-line steps of the interleaved z pass (one component per line) against a
+    long-double DFT, Nz = 4..8192; rel-L2 <= 1e-15 (f64) / 1e-6 (f32)"""
     with tempfile.TemporaryDirectory() as td:
         exe = os.path.join(td, "emu")
         subprocess.run(["g++", "-O2", "-std=c++17", "-o", exe, os.path.join(HERE, "emu_rc_pair.cpp")], check=True)

@@ -11,6 +11,7 @@ import distributedfft_b200 as dfft
 from distributedfft_b200 import _lib
 from distributedfft_b200._lib import check, lib
 from test_components import describe_ilv
+from test_gpu_accuracy import check_units, ld, spec as unit_spec, unit_scales
 from test_schedule_emulation import A2A, P2P, PE, SL, SYNC, ZY
 
 torch = pytest.importorskip("torch")
@@ -97,7 +98,7 @@ def test_bit_identical_to_the_batched_plan(shape, comps, f64):
 @pytest.mark.parametrize("shape,comps,decomp", [((256, 256, 256), 3, SL), ((64, 64, 64), 2, SL), ((128, 64, 256), 7, SL),
                                                 ((32, 64, 16), 5, ZY), ((64, 32, 32), 4, PE), ((16, 16, 8192), 3, SL)])
 def test_r2c_against_numpy(shape, comps, decomp, f64):
-    """the paired R2C / C2R z pass: forward against numpy's rfftn, inverse against irfftn, round trip, scale bit for bit"""
+    """the interleaved R2C / C2R z pass: forward against numpy's rfftn, inverse against irfftn, round trip, scale bit for bit"""
     plan = make(shape, comps, decomp, f64, transform="r2c")
     x = torch.randn(shape + (comps,), dtype=torch.float64 if f64 else torch.float32, device="cuda",
                     generator=torch.Generator(device="cuda").manual_seed(5))
@@ -193,7 +194,8 @@ def test_multi_rank_replay_r2c(P, decomp, shape, p1, p2, comm, comps, inverse):
 
 
 def replay_case(P, decomp, shape, p1, p2, comm, comps, inverse, transform):
-    """every rank's steps in lock step with the real kernels; against numpy and, bit for bit, the one-rank plan"""
+    """every rank's steps in lock step with the real kernels; against numpy (R2C / C2R: each component against long double
+    on its own norm) and, bit for bit, the one-rank plan"""
     d = 3
     c2c = transform == dfft.C2C
     plans, comms, scheds = dry_plans(P, decomp, shape, p1, p2, comm, comps, inverse, d, transform)
@@ -206,7 +208,10 @@ def replay_case(P, decomp, shape, p1, p2, comm, comps, inverse, transform):
         spec = exec_(one, x)
         src, want = (spec, exec_(one, spec, dfft.INVERSE)) if inverse else (x, spec)
     else:
+        # components of mixed magnitude (1, 2^20, 2^-20, 0, ...): each is held to the per-component long-double bound
+        sc = unit_scales(comps)
         x = torch.randn(shape + (comps,), dtype=torch.float64, device="cuda", generator=torch.Generator(device="cuda").manual_seed(4))
+        x = x * torch.from_numpy(sc).cuda()
         spec = r2c(one, x)
         src, want = (spec, c2r(one, spec)) if inverse else (x, spec)
     lay = lambda r, w: dfft.layout(decomp, transform, *shape, p1, p2, r, w)
@@ -236,6 +241,7 @@ def replay_case(P, decomp, shape, p1, p2, comm, comps, inverse, transform):
                                            ins[r].numel(), torch.cuda.current_stream().cuda_stream)
             assert rc == 0, (lib().dfft_last_error_string() or b"").decode()
     torch.cuda.synchronize()
+    full = np.zeros(tuple(want.shape), dtype=want.cpu().numpy().dtype)
     for r in range(P):
         osz, ost = lay(r, 0 if inverse else d)
         got = outs[r].view(want.dtype).reshape(*osz, comps)
@@ -243,10 +249,12 @@ def replay_case(P, decomp, shape, p1, p2, comm, comps, inverse, transform):
             assert torch.equal(got, blk(want, ost, osz)), f"rank {r}"
         if c2c:
             ref = np.fft.ifftn(spec.cpu().numpy(), axes=(0, 1, 2)) * np.prod(shape) if inverse else np.fft.fftn(x.cpu().numpy(), axes=(0, 1, 2))
-        else:
-            ref = (np.fft.irfftn(spec.cpu().numpy(), s=shape, axes=(0, 1, 2)) * np.prod(shape) if inverse
-                   else np.fft.rfftn(x.cpu().numpy(), axes=(0, 1, 2)))
-        assert rel(got.cpu().numpy(), blk(ref, ost, osz)) < 1e-10
+            assert rel(got.cpu().numpy(), blk(ref, ost, osz)) < 1e-10
+        blk(full, ost, osz)[...] = got.cpu().numpy()
+    if not c2c:
+        ref = (np.fft.irfftn(ld(spec.cpu().numpy()), s=shape, axes=(0, 1, 2)) * np.prod(shape) if inverse
+               else np.fft.rfftn(ld(x.cpu().numpy()), axes=(0, 1, 2)))
+        check_units("replay R2C/C2R", unit_spec(dfft.F64, shape), full, ref, 3, sc, f"P={P} {'inv' if inverse else 'fwd'}")
     for p, c in zip(plans, comms):
         lib().dfft_plan_destroy(p)
         lib().dfft_comm_destroy(c)

@@ -10,7 +10,7 @@ the 3.35 TB/s HBM bound of the H100 SXM data sheet (one read and one write of th
 16 bytes per value).  The card's name, power limit and maximum SM clock are read in the same run.  A report, not a gate: one JSON
 line per case.
 
-    python tools/components_bench.py [--reps 10] [--windows 5] [--out components_bench.json]
+    python tools/components_bench.py [--reps 10] [--windows 5] [--precision double|float] [--transform c2c|r2c] [--out components_bench.json]
 """
 from __future__ import annotations
 
@@ -39,6 +39,8 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--reps", type=int, default=10, help="execs per timed window")
     ap.add_argument("--windows", type=int, default=5, help="alternating windows per variant")
+    ap.add_argument("--precision", choices=["double", "float"], default="double")
+    ap.add_argument("--transform", choices=["c2c", "r2c"], default=None, help="only the workloads of this transform")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
 
@@ -50,18 +52,23 @@ def main():
         sys.exit("components_bench needs a GPU")
     gpu = card()
     lines = []
+    f64 = args.precision == "double"
+    cdt, rdt = (torch.complex128, torch.float64) if f64 else (torch.complex64, torch.float32)
     for shape, comps, transform in WORKLOADS:
+        if args.transform and transform != args.transform:
+            continue
+
         def plan(c, b):
-            p = dfft.MPIcuFFT_Slab(dfft.Configurations(), dfft.Comm(), precision="double", transform=transform)
+            p = dfft.MPIcuFFT_Slab(dfft.Configurations(), dfft.Comm(), precision=args.precision, transform=transform)
             p.initFFT(dfft.GlobalSize(*shape), None, True, batch=b, components=c)
             return p
 
         c2c = transform == "c2c"
         ilv, bat = plan(comps, 1), plan(1, comps)
         spec = shape if c2c else shape[:2] + (shape[2] // 2 + 1,)
-        xr = torch.randn(shape + (comps,), dtype=torch.complex128 if c2c else torch.float64, device="cuda")
+        xr = torch.randn(shape + (comps,), dtype=cdt if c2c else rdt, device="cuda")
         # inverse input: a spectrum of real fields for C2R (X[0] and X[Nz/2] real along z)
-        Xs = torch.randn(spec + (comps,), dtype=torch.complex128, device="cuda") if c2c else torch.fft.rfftn(xr, dim=(0, 1, 2)).contiguous()
+        Xs = torch.randn(spec + (comps,), dtype=cdt, device="cuda") if c2c else torch.fft.rfftn(xr, dim=(0, 1, 2)).contiguous()
         s = torch.cuda.current_stream()
 
         def run(p, out, inp, direction, d=3, stream=s):
@@ -125,7 +132,7 @@ def main():
             c()
             torch.cuda.synchronize()
             ok = bool(torch.equal(ya.permute(3, 0, 1, 2), yc)) if c2c else float((ya.permute(3, 0, 1, 2) - yc).abs().max() / yc.abs().max())
-            line = {"gpu": gpu, "shape": list(shape), "components": comps, "transform": transform, "direction": name,
+            line = {"gpu": gpu, "precision": args.precision, "shape": list(shape), "components": comps, "transform": transform, "direction": name,
                     "best_ms": {k: round(min(v), 4) for k, v in times.items()}, "all_ms": {k: [round(t, 4) for t in v] for k, v in times.items()},
                     "z_pass": steps, "a_vs_c": ok}
             print(json.dumps(line), flush=True)
