@@ -96,12 +96,26 @@ static bool c2c_length(size_t n) { return (ilog2_exact(n) >= 1 && ilog2_exact(n)
 // Real-to-real plans: powers of two in [2, 2^MAX_LOG2N].  The transform of a plan from dfft_plan_create_r2r is DFFT_DCT or
 // DFFT_DST when all three kinds are that one, DFFT_R2HC for any other combination (its kinds are in dfft_plan_s::kinds).
 static bool is_r2r(int transform) { return transform == DFFT_DCT || transform == DFFT_DST || transform == DFFT_R2HC; }
-static const char* r2r_name(int k) { return k == DFFT_DST ? "dst" : k == DFFT_R2HC ? "r2hc" : "dct"; }
+static const char* r2r_name(int k) {
+    return k == DFFT_DST ? "dst" : k == DFFT_R2HC ? "r2hc" : k == DFFT_DCT1 ? "dct1" : k == DFFT_DST1 ? "dst1" : "dct";
+}
 static bool r2r_length(size_t n) { return ilog2_exact(n) >= 1 && ilog2_exact(n) <= MAX_LOG2N; }
+// Type-I kinds (DFFT_DCT1, DFFT_DST1): axis kinds of per-axis plans (transform DFFT_R2HC) and of dfft_fft1d_r2r only.  An
+// axis of L points runs N-point complex lines: L = N + 1 (DCT-I, N in [2, 8192]) or L = N - 1 (DST-I, N in [4, 8192]).
+static bool is_type1(int kind) { return kind == DFFT_DCT1 || kind == DFFT_DST1; }
+static bool is_r2r_kind(int kind) { return is_r2r(kind) || is_type1(kind); }
+// log2 N of a type-I axis of L points, -1 for a length the kind does not take
+static int type1_log2(int kind, size_t L) {
+    const int l2 = kind == DFFT_DCT1 ? (L >= 3 ? ilog2_exact(L - 1) : -1) : ilog2_exact(L + 1);
+    return l2 >= (kind == DFFT_DCT1 ? 1 : 2) && l2 <= MAX_LOG2N ? l2 : -1;
+}
+// the lengths an axis of R2R kind `kind` takes
+static bool r2r_kind_length(int kind, size_t n) { return is_type1(kind) ? type1_log2(kind, n) > 0 : r2r_length(n); }
 
 // One FFT pass of n-point lines (R2C / C2R: n complex points) over the views of prm, its stores scaled by `scale`: the
 // power-of-two kernels, or the Bluestein pass when n is not a power of two (prm.tw: the M-point table; blu: the Bluestein
-// table of n).  PASS_R2R_*: the R2R kernel of kind r2r (DFFT_DCT, DFFT_DST with prm.tw2 its w_k table, or DFFT_R2HC).
+// table of n).  PASS_R2R_*: the R2R kernel of kind r2r (DFFT_DCT, DFFT_DST with prm.tw2 its w_k table, or DFFT_R2HC), or
+// the type-I kernel (DFFT_DCT1, DFFT_DST1: n = N +- 1 reals, prm.tw2 the 2N-point table).
 // hole: passes of padded plans that keep part of their spectral side, the hole [hole[0], hole[1]) of their lines
 // (pass_hole); the padded twin of the power-of-two kernel runs then.
 static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftParams& prm, const void* blu, double scale, cudaStream_t stream,
@@ -119,8 +133,9 @@ static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftP
         FftR2r r;
         static_cast<FftParams&>(r) = prm;
         r.w = prm.tw2;
-        r.dst = r2r == DFFT_DST;
+        r.dst = r2r == DFFT_DST || r2r == DFFT_DST1;
         r.scale = scale;
+        if (is_type1(r2r)) return launch_r2r1(prec, type1_log2(r2r, n), kind, r, stream);
         return launch_r2r(prec, log2n, kind, r, r2r == DFFT_R2HC, stream);
     }
     if (log2n >= 0) return launch_pass(prec, log2n, kind, prm, scale, stream);
@@ -241,21 +256,26 @@ struct Tables {
 };
 
 // The power-of-two length a pass of n-point lines runs (R2C / C2R: n complex points): log2 n, or log2 M of the Bluestein
-// pass for C2C lengths that are not powers of two; -1 for lengths nothing runs
-static int pass_log2(PassKind kind, size_t n) {
+// pass for C2C lengths that are not powers of two, log2 N of type-I R2R passes (r2r: the kind of R2R passes); -1 for lengths
+// nothing runs
+static int pass_log2(PassKind kind, size_t n, int r2r = 0) {
+    if ((kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED) && is_type1(r2r)) return type1_log2(r2r, n);
     return (kind == PASS_C2C_CONTIG || kind == PASS_C2C_TILED) && bluestein_length(n) ? bluestein_log2m(n) : ilog2_exact(n);
 }
 
 // The tables such a pass reads, from T: tw of its power-of-two length, tw2 for R2C / C2R and DCT / DST passes (r2r: the kind
 // of R2R passes; DCT / DST take w_k = exp(-i pi k / 2N), k <= N, the R2C table of length 2N), blu for Bluestein lengths.
-// One rule for plans and for the single-axis calls.
+// Type-I passes take tw and tw2 of log2 N (W^k = exp(-i pi k / N), k <= N/2).  One rule for plans and for the single-axis
+// calls.
 static int pass_tables(Tables& T, PassKind kind, size_t n, int r2r, void** tw, void** tw2, void** blu) {
-    const int l2 = pass_log2(kind, n);
-    const bool with_w = (kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED) && r2r != DFFT_R2HC;
+    const bool rr = kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED;
+    const bool type1 = rr && is_type1(r2r);
+    const int l2 = pass_log2(kind, n, rr ? r2r : 0);
+    const bool with_w = rr && r2r != DFFT_R2HC && !type1;
     *tw = *tw2 = *blu = nullptr;
-    if (l2 != ilog2_exact(n) && T.get_blu(n, blu) != cudaSuccess) return fail(DFFT_ERR_CUDA, "Bluestein table allocation failed");
+    if (!type1 && l2 != ilog2_exact(n) && T.get_blu(n, blu) != cudaSuccess) return fail(DFFT_ERR_CUDA, "Bluestein table allocation failed");
     if (T.get_tw(l2, tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
-    if ((kind == PASS_R2C || kind == PASS_C2R || with_w) && T.get_tw2(l2 + (with_w ? 1 : 0), tw2) != cudaSuccess)
+    if ((kind == PASS_R2C || kind == PASS_C2R || with_w || type1) && T.get_tw2(l2 + (with_w ? 1 : 0), tw2) != cudaSuccess)
         return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
     return DFFT_SUCCESS;
 }
@@ -335,7 +355,9 @@ struct Step {
     size_t n = 0;
     const void* blu = nullptr;
     bool bluestein() const { return !is_copy(kind) && n != 0 && n != (size_t(1) << log2n); }
-    int r2r = 0;  // PASS_R2R_*: the kind of the axis it transforms (DFFT_DCT, DFFT_DST or DFFT_R2HC)
+    // PASS_R2R_*: the kind of the axis it transforms (DFFT_DCT, DFFT_DST, DFFT_R2HC, DFFT_DCT1 or DFFT_DST1; type-I passes
+    // have n = L reals per line and log2n = log2 N)
+    int r2r = 0;
     int axis = 0;  // the axis of the pass: 0 x, 1 y, 2 z (PASS_COPY_*: n is its length, log2n 0)
     // padded plans: the points its spectral side keeps of each line (Kx, Ky, Kz; R2C / C2R: Kz/2 + 1 of the Nz/2 + 1), the
     // rest is the hole (fft_kernels.cuh, FftPadded); 0: the whole line
@@ -683,7 +705,9 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         }
         s.kind = kind;
         s.phase = phase;
-        s.log2n = pass_log2(kind, n);  // Bluestein lengths: the view mapping stays the kind's; the exec launches the Bluestein kernel
+        // Bluestein lengths: the view mapping stays the kind's; the exec launches the Bluestein kernel.  Type-I R2R passes:
+        // log2 N of their N +- 1 reals per line
+        s.log2n = pass_log2(kind, n, s.r2r);
         s.n = n;
         {   // padded plans: the spectral extent of the axis
             const size_t k = axis == 0 ? g.kx : axis == 1 ? g.ky : g.kzc, full = axis == 0 ? g.nx : axis == 1 ? g.ny : g.nzc;
@@ -2687,9 +2711,14 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
             return fail(DFFT_ERR_UNSUPPORTED, "Nx, Ny, Nz of C2C plans must be powers of two in [2, 8192] or any length in [3, 4096]");
         }
     } else if (is_r2r(transform)) {
-        if (!r2r_length(nx) || !r2r_length(ny) || !r2r_length(nz)) {
+        const size_t n[3] = {nx, ny, nz};
+        for (int a = 0; a < 3; ++a) {
+            if (r2r_kind_length(p->kinds[a], n[a])) continue;
+            const std::string what = p->kinds[a] == DFFT_DCT1   ? "DCT-I axes must have 2^k + 1 points in [3, 8193]"
+                                     : p->kinds[a] == DFFT_DST1 ? "DST-I axes must have 2^k - 1 points in [3, 8191]"
+                                                                : "Nx, Ny, Nz of DCT / DST plans must be powers of two in [2, 8192]";
             delete p;
-            return fail(DFFT_ERR_UNSUPPORTED, "Nx, Ny, Nz of DCT / DST plans must be powers of two in [2, 8192]");
+            return fail(DFFT_ERR_UNSUPPORTED, what);
         }
     } else if (ilog2_exact(nx) < 1 || ilog2_exact(ny) < 1 || ilog2_exact(nz) < 1 || ilog2_exact(nx) > MAX_LOG2N || ilog2_exact(ny) > MAX_LOG2N ||
                ilog2_exact(nz) > MAX_LOG2N + 1 || nz < 4) {
@@ -2911,9 +2940,9 @@ int dfft_plan_create_r2r(dfft_comm_t comm, const dfft_config* config, int decomp
                          size_t nz, size_t p1, size_t p2, size_t batch, int inplace, int allocate, dfft_plan_t* plan) {
     if (!kinds) return fail(DFFT_ERR_INVALID, "null kinds");
     for (int a = 0; a < 3; ++a)
-        if (!is_r2r(kinds[a])) return fail(DFFT_ERR_INVALID, "kinds must be DFFT_DCT, DFFT_DST or DFFT_R2HC");
-    // three DCT (DST) axes make exactly the DCT (DST) plan
-    const bool uniform = kinds[0] == kinds[1] && kinds[1] == kinds[2] && kinds[0] != DFFT_R2HC;
+        if (!is_r2r_kind(kinds[a])) return fail(DFFT_ERR_INVALID, "kinds must be DFFT_DCT, DFFT_DST, DFFT_R2HC, DFFT_DCT1 or DFFT_DST1");
+    // three DCT (DST) axes make exactly the DCT (DST) plan; type-I kinds, like R2HC, make a per-axis plan
+    const bool uniform = kinds[0] == kinds[1] && kinds[1] == kinds[2] && (kinds[0] == DFFT_DCT || kinds[0] == DFFT_DST);
     return plan_create(comm, config, decomp, precision, uniform ? kinds[0] : DFFT_R2HC, nx, ny, nz, p1, p2, batch, inplace != 0, allocate, plan,
                        kinds);
 }
@@ -3556,8 +3585,11 @@ int dfft_fft1d_strided(int precision, int direction, size_t a, size_t n, size_t 
 
 int dfft_fft1d_r2r(int precision, int transform, int direction, size_t n, size_t a, size_t b, void* out, const void* in, void* stream) {
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
-    if (!is_r2r(transform)) return fail(DFFT_ERR_INVALID, "transform must be DFFT_DCT, DFFT_DST or DFFT_R2HC");
-    if (!r2r_length(n)) return fail(DFFT_ERR_UNSUPPORTED, "length must be a power of two in [2, 8192]");
+    if (!is_r2r_kind(transform)) return fail(DFFT_ERR_INVALID, "transform must be DFFT_DCT, DFFT_DST, DFFT_R2HC, DFFT_DCT1 or DFFT_DST1");
+    if (!r2r_kind_length(transform, n))
+        return fail(DFFT_ERR_UNSUPPORTED, transform == DFFT_DCT1   ? "DCT-I length must be 2^k + 1 in [3, 8193]"
+                                          : transform == DFFT_DST1 ? "DST-I length must be 2^k - 1 in [3, 8191]"
+                                                                   : "length must be a power of two in [2, 8192]");
     if (a == 0 || b == 0) return DFFT_SUCCESS;
     if (a * b > size_t(0x7fffffff) || n * b > size_t(1) << 62) return fail(DFFT_ERR_INVALID, "array too large");
     FftParams prm{};

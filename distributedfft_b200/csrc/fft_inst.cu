@@ -359,6 +359,38 @@ cudaError_t launch_r2r(PassKind kind, const FftR2r& p, bool hc, cudaStream_t str
 
 template cudaError_t launch_r2r<DFFT_T, DFFT_LOG2N>(PassKind, const FftR2r&, bool, cudaStream_t);
 
+// CONTIG: TBC lines per CTA.  TILED: one real per tile column, so the wide tile of the length (2 TBT columns where it fits
+// 128 KB and 1024 threads) gives rows of 2 TBT reals, the row width of the paired R2R tile (>= 64 bytes); lengths whose
+// wide tile does not fit keep TBT columns.  The tile order is the C2C pass's (tile_swz_for).
+template <typename T, int LOG2N>
+cudaError_t launch_r2r1(PassKind kind, const FftR2r& p_in, cudaStream_t stream) {
+    using S = Shape<T, LOG2N>;
+    constexpr int LOG2E = S::LOG2E;
+    if (!p_in.w || !p_in.tw) return cudaErrorInvalidValue;
+    const long long lines = (long long)p_in.A0 * p_in.A1;
+    if (lines <= 0) return cudaSuccess;
+    FftR2r p = p_in;
+    p.tile_swz = tile_swz_for(p.tile_swz, p.A0, p.A1);
+    if (kind == PASS_R2R_CONTIG) {
+        using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
+        if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
+        const long long grid = (lines + S::TBC - 1) / S::TBC;
+        if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+        constexpr auto k = fft_r2r1_kernel<T, LOG2N, LOG2E, S::TBC, false>;
+        return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+    }
+    if (kind != PASS_R2R_TILED) return cudaErrorInvalidValue;
+    if (p.B <= 0) return cudaSuccess;
+    constexpr int TB = S::TBT_WIDE;
+    using C = CtaFft<T, LOG2N, LOG2E, TB, true>;
+    const long long grid = lines * ((p.B + TB - 1) / TB);
+    if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+    constexpr auto k = fft_r2r1_kernel<T, LOG2N, LOG2E, TB, true>;
+    return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+}
+
+template cudaError_t launch_r2r1<DFFT_T, DFFT_LOG2N>(PassKind, const FftR2r&, cudaStream_t);
+
 #if DFFT_LOG2N == 1
 // CONTIG: lines of up to COPY_THREADS threads (the power of two >= n), COPY_THREADS / that many lines per CTA; TILED: rows
 // as wide as the power of two >= B, up to 32 elements (a 512-byte row of cx<double>), the CTA's other threads on further n

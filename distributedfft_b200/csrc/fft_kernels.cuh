@@ -1884,6 +1884,83 @@ fft_r2hc_kernel(const __grid_constant__ FftR2r p) {
     r2r_pass<T, LOG2N, LOG2E, TB, TILED, INV, true>(p);
 }
 
+// ---- type-I real-to-real pass: DCT-I (L = N + 1 reals per line) and DST-I (L = N - 1) -------------------------------------
+// One real line per complex N-point line of the tile (r2r.hpp): point m loads e_{2m} and e_{2m+1} of the line's 2N-point
+// extension, CtaFft's stages transform z, and the R2C split with the 2N-point table (FftR2r::w = W^k = exp(-i pi k / N),
+// k <= N/2: Tables::get_tw2(log2 N)) gives E_k, of which y takes the real part (DCT-I) or minus the imaginary part (DST-I).
+// p.dst picks the kind, p.inverse is not read: the transform is its own inverse.  The views count in reals.
+//   CONTIG: TB real lines per CTA, one per line slot.
+//   TILED:  one real column per tile column (TB columns: the wide tile of the length where shared memory allows it).
+// The mirrored loads reach their reals straight from global memory, as the DCT-II pass's permuted loads do; the second
+// read of a sector is meant to hit L1 (a design choice, not a measurement).  After the stages Z goes through shared memory
+// once; the thread of point k <= N/2 splits Z[k] with Z[N-k] and stores the outputs of E_k and E_{N-k}.  One CTA per tile
+// and every load before any store, so out == in works.  A scale != 1 multiplies the stores (__dmul_rn / __fmul_rn: the
+// scaled output is the unscaled one times s, bit for bit).
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED>
+__global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
+fft_r2r1_kernel(const __grid_constant__ FftR2r p) {
+    using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
+    using LA = LineAccess<T, C::LINES, T>;
+    constexpr int E = C::E, TPL = C::TPL, N = C::N;
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
+    unsigned long long* tab_in = reinterpret_cast<unsigned long long*>(smem_raw + C::TILE_BYTES);
+    unsigned long long* tab_out = tab_in + C::LINES * MAXSEG;
+    const TileCoord<C, TILED, TB> tc(p);
+    const int j = tc.j, t = tc.t;
+    if (p.in.nseg > 1 || p.out.nseg > 1) {
+        // TILED: one table per CTA, CONTIG: one per line (as in c2c_tile)
+        const int line = TILED ? 0 : t, lane = TILED ? int(threadIdx.x) : j, lanes = TILED ? C::THREADS : TPL;
+        LA::fill_table(p.in, tab_in, line, lane, lanes, tc.a0, tc.a1);
+        LA::fill_table(p.out, tab_out, line, lane, lanes, tc.a0, tc.a1);
+        __syncthreads();
+    }
+    const LA in(p.in, tab_in, TILED ? 0 : t, tc.a0, tc.a1, tc.b), out(p.out, tab_out, TILED ? 0 : t, tc.a0, tc.a1, tc.b);
+    const int dst = p.dst;
+    auto ext = [&](int i) -> T {  // e_i
+        bool neg;
+        const int m = r2r1_ext(i, N, dst, neg);
+        if (m < 0) return T(0);
+        T x;
+        if constexpr (TILED) x = *in.at(m);
+        else x = *in.at1(m);
+        return neg ? -x : x;
+    };
+    cx<T> v[E];
+#pragma unroll
+    for (int e = 0; e < E; ++e) {
+        const int m = j + e * TPL;
+        v[e] = tc.valid ? cx<T>{ext(2 * m), ext(2 * m + 1)} : cx<T>{T(0), T(0)};
+    }
+    C::template stages<0>(v, j, t, sm, reinterpret_cast<const cx<T>*>(p.tw));
+    // Z in natural order -> shared memory, then point k with Z[N-k]
+    if constexpr (C::NST > 1) C::sync(t);
+#pragma unroll
+    for (int e = 0; e < E; ++e) sm[C::sidx(j + e * TPL, t)] = v[C::Core::final_slot(e)];
+    C::sync(t);
+    if (!tc.valid) return;
+    const cx<T>* w = reinterpret_cast<const cx<T>*>(p.w);
+    const bool scaled = p.scale != 1.0;
+    const T s = T(p.scale);
+    auto store = [&](int k, cx<T> ek) {
+        const int o = r2r1_out_index(k, N, dst);
+        if (o < 0) return;
+        T y = r2r1_value<T>(ek, dst);
+        if (scaled) y = rscale<T>(y, s);
+        if constexpr (TILED) *out.at(o) = y;
+        else *out.at1(o) = y;
+    };
+    auto emit = [&](int k) {
+        cx<T> ek, enk;
+        r2r1_split<T>(sm[C::sidx(k, t)], sm[C::sidx((N - k) & (N - 1), t)], ld_tw(w, k), ek, enk);
+        store(k, ek);
+        if (2 * k != N) store(N - k, enk);
+    };
+#pragma unroll
+    for (int e = 0; e < E / 2; ++e) emit(j + e * TPL);
+    if (j == 0) emit(N / 2);
+}
+
 // ---- copy pass: an axis the plan keeps (dfft_plan_set_transform_axes) ------------------------------------------------
 // Moves element (a0, a1, n, b) of p.in to the same index of p.out for any line length p.n, through the segmented views of
 // the FFT pass it replaces (scatters into peer slots, gathers from receive slots, blocked layouts and tails unchanged).
@@ -2030,6 +2107,13 @@ cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluest
 template <typename T, int LOG2N>
 cudaError_t launch_r2r(PassKind kind, const FftR2r& p, bool hc, cudaStream_t stream);
 cudaError_t launch_r2r(int prec, int log2n, PassKind kind, const FftR2r& p, bool hc, cudaStream_t stream);
+
+// DCT-I / DST-I pass (fft_r2r1_kernel, p.dst) of real lines of 2^LOG2N + 1 or 2^LOG2N - 1 points: kind PASS_R2R_CONTIG
+// (sN == 1, TBC lines per CTA) or PASS_R2R_TILED (one real column per tile column), views in reals, one CTA per tile;
+// p.w = Tables::get_tw2(LOG2N), p.scale scales the stores.  Instantiated for LOG2N 1..13.
+template <typename T, int LOG2N>
+cudaError_t launch_r2r1(PassKind kind, const FftR2r& p, cudaStream_t stream);
+cudaError_t launch_r2r1(int prec, int log2n, PassKind kind, const FftR2r& p, cudaStream_t stream);
 
 // copy pass of p.n-point lines (fft_copy_kernel): kind PASS_COPY_CONTIG or PASS_COPY_TILED, p.ltpl is filled in here.
 // Instantiated for E = T and cx<T> in the LOG2N = 1 unit of each precision; the runtime form takes real != 0 for the

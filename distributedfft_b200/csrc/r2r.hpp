@@ -71,7 +71,42 @@ DFFT_HD cx<T> r2hc_build(T ak, T am, T bk, T bm, int k, int N) {
     return cx<T>{xa.x - xb.y, xa.y + xb.x};
 }
 
-// ---- R2C / C2R z pass of interleaved plans (fft_rc_ilv_kernel) ---------------------------------------------------------------
+// ---- DCT-I / DST-I (fft_r2r1_kernel): one real line per complex N-point FFT ------------------------------------------------
+// FFTW's REDFT00 (L = N + 1 points) and RODFT00 (L = N - 1) are DFTs of the line's 2N-point extension e:
+//   DCT-I, even:  e = x_0 .. x_N, x_{N-1} .. x_1          DST-I, odd:  e = 0, x_0 .. x_{N-2}, 0, -x_{N-2} .. -x_0
+// e is read as N complex points z_m = e_{2m} + i e_{2m+1}, Z = DFT_N(z), and split as the R2C pass does, W = exp(-i pi / N):
+//   E_k = (Z_k + conj Z_{N-k}) / 2 - i W^k (Z_k - conj Z_{N-k}) / 2,   k = 0 .. N,  Z_N := Z_0
+//   DCT-I:  y_k = Re E_k (k = 0 .. N)          DST-I:  y_k = -Im E_{k+1} (k = 0 .. N - 2)
+// (E = DFT_2N(e).)  One line per FFT: pairing two lines as z = e_a + i e_b would need a 2N-point FFT per pair and would tie
+// each line's error to its partner's norm.  Unnormalised like scipy's dct / dst with type=1: each is its own inverse up to 2N.
+
+// x index feeding point i < 2N of the extension, -1 where e_i is zero; neg: e_i = -x
+DFFT_HD int r2r1_ext(int i, int N, int dst, bool& neg) {
+    neg = false;
+    if (!dst) return i <= N ? i : 2 * N - i;
+    if (i == 0 || i == N) return -1;
+    if (i < N) return i - 1;
+    neg = true;
+    return 2 * N - 1 - i;
+}
+
+// E_k and E_{N-k} from Z[k], Z[-k mod N] and w = W^k (W^{N-k} = -conj W^k, so one twiddle of k <= N/2 serves both)
+template <typename T>
+DFFT_HD void r2r1_split(cx<T> zk, cx<T> zm, cx<T> w, cx<T>& ek, cx<T>& enk) {
+    const cx<T> c = cconj(zm);
+    const cx<T> xe{T(0.5) * (zk.x + c.x), T(0.5) * (zk.y + c.y)};
+    const cx<T> d = csub(zk, c);
+    const cx<T> tt = cmul(w, cx<T>{T(0.5) * d.y, T(-0.5) * d.x});  // W^k (-i/2) d
+    ek = cadd(xe, tt);
+    enk = cconj(csub(xe, tt));
+}
+
+// position of E_k's output in the line: k (DCT-I), k - 1 (DST-I), -1 for E_0 and E_N of the DST-I
+DFFT_HD int r2r1_out_index(int k, int N, int dst) { return !dst ? k : (k == 0 || k == N ? -1 : k - 1); }
+template <typename T>
+DFFT_HD T r2r1_value(cx<T> e, int dst) { return dst ? -e.y : e.x; }
+
+// ---- R2C / C2R z pass of interleaved plans (fft_rc_ilv_kernel)---------------------------------------------------------------
 // Every component runs its own complex Nz-point line z = x + 0i.  (Two components sharing one line as z = x_a + i x_b would
 // halve the arithmetic, but the split then leaves X_b with an error of u |x_a| rather than u |x_b|: components are
 // independent fields, so a small one next to a large one would lose its digits.)  Z = DFT_N(z), m = -k mod N:

@@ -101,6 +101,16 @@ typedef enum { DFFT_R2C = 0, DFFT_C2C = 1, DFFT_DCT = 2, DFFT_DST = 3, DFFT_R2HC
  * i.e. hc[k] = Re X_k for k <= N/2 and hc[N-k] = Im X_k for 0 < k < N/2 (numpy: X = rfft(x),
  * hc = concatenate([X.real[:N/2+1], X.imag[N/2-1:0:-1]]); scipy.fftpack.rfft interleaves the parts and is another format).
  * Inverse (HC2R) is the unnormalised inverse: HC2R(R2HC(x)) = N x. */
+/* DFFT_DCT1 / DFFT_DST1 (not in the reference; FFTW's REDFT00 / RODFT00, scipy.fft.dct / dst with type=1, norm=None): the
+ * type-I transforms of vertex-centred grids (the boundary nodes are grid points) and of Chebyshev-Gauss-Lobatto axes
+ * (x_j = cos(pi j / N), j = 0..N, whose Chebyshev transform is a DCT-I of N + 1 points).  Kinds only, like DFFT_R2HC: for
+ * dfft_plan_create_r2r and dfft_fft1d_r2r; dfft_plan_create* return DFFT_ERR_INVALID for transforms 16 and 17.  With N a
+ * power of two:
+ *   DCT-I, L = N + 1 points, N in [2, 8192]:  y_k = x_0 + (-1)^k x_N + 2 sum_{n=1}^{N-1} x_n cos(pi n k / N)
+ *   DST-I, L = N - 1 points, N in [4, 8192]:  y_k = 2 sum_{n=0}^{N-2} x_n sin(pi (n+1)(k+1) / N)
+ * so an axis takes L = 3, 5, 9, ..., 8193 (DCT-I) or 3, 7, 15, ..., 8191 (DST-I); any other length DFFT_ERR_UNSUPPORTED.
+ * Each is its own inverse up to 2N: forward and inverse execs run the same transform on such an axis. */
+enum { DFFT_DCT1 = 16, DFFT_DST1 = 17 };
 
 typedef struct dfft_comm_s* dfft_comm_t;
 typedef struct dfft_plan_s* dfft_plan_t;
@@ -163,15 +173,19 @@ int dfft_plan_create_inplace(dfft_comm_t comm, const dfft_config* config, int de
                              size_t nz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan);
 int dfft_plan_is_inplace(dfft_plan_t plan); /* 1 for plans of dfft_plan_create_inplace, 0 otherwise (and for a null plan) */
 /* Real-to-real plans with a kind per axis (FFTW's fftw_plan_r2r with one kind per dimension): kinds[0], [1], [2] are the
- * kinds of the x, y and z axis, each DFFT_DCT (Neumann), DFFT_DST (Dirichlet) or DFFT_R2HC (periodic).  Everything said of
- * DFFT_DCT / DFFT_DST plans above holds: real [x][y][z] buffers, powers of two in [2, 8192] (others:
+ * kinds of the x, y and z axis, each DFFT_DCT (Neumann), DFFT_DST (Dirichlet), DFFT_R2HC (periodic), or DFFT_DCT1 /
+ * DFFT_DST1 (Neumann / Dirichlet on vertex-centred or Chebyshev axes).  Everything said of DFFT_DCT / DFFT_DST plans above
+ * holds: real [x][y][z] buffers, powers of two in [2, 8192] (type-I axes: the lengths of DFFT_DCT1 / DFFT_DST1; others:
  * DFFT_ERR_UNSUPPORTED), dfft_exec_r2r* (forward: DCT-II, DST-II or R2HC on each axis; inverse: DCT-III, DST-III or
- * HC2R), partial d over the first d axes in z, y, x order, each with its own kind, and dfft_layout with DFFT_DCT.
+ * HC2R; DCT-I and DST-I both ways), partial d over the first d axes in z, y, x order, each with its own kind, and
+ * dfft_layout with DFFT_DCT.
  * `batch` and `inplace` (!= 0) mean what they mean for dfft_plan_create_batched / dfft_plan_create_inplace.
- *   - A round trip scales by the product over the transformed axes of N (R2HC) or 2N (DCT, DST).
+ *   - A round trip scales by the product over the transformed axes of N (R2HC) or 2N (DCT, DST, and DCT-I / DST-I with
+ *     their N = L - 1 / L + 1).
  *   - Three DFFT_DCT (DFFT_DST) kinds make the DFFT_DCT (DFFT_DST) plan: the same steps, description and output.  Other
- *     combinations: dfft_plan_describe reports "r2r_kinds" and, per R2R pass, "r2r" (the kind of its axis).
- *   - A null kinds or a kind outside {DFFT_DCT, DFFT_DST, DFFT_R2HC}: DFFT_ERR_INVALID. */
+ *     combinations, type-I kinds included: dfft_plan_describe reports "r2r_kinds" and, per R2R pass, "r2r" (the kind of its
+ *     axis: "dct", "dst", "r2hc", "dct1" or "dst1").
+ *   - A null kinds or a kind outside {DFFT_DCT, DFFT_DST, DFFT_R2HC, DFFT_DCT1, DFFT_DST1}: DFFT_ERR_INVALID. */
 int dfft_plan_create_r2r(dfft_comm_t comm, const dfft_config* config, int decomp /*dfft_decomp*/, int precision /*dfft_prec*/,
                          const int kinds[3], size_t nx, size_t ny, size_t nz, size_t p1, size_t p2, size_t batch, int inplace,
                          int allocate, dfft_plan_t* plan);
@@ -388,7 +402,7 @@ int dfft_fft1d_strided(int precision, int direction, size_t a, size_t n, size_t 
 
 /* DCT / DST / R2HC (transform DFFT_DCT, DFFT_DST or DFFT_R2HC; forward type II or R2HC, inverse type III or HC2R,
  * unnormalised) along the middle axis of a dense real [a][n][b] array, b contiguous; n a power of two in [2, 8192].
- * out == in is allowed. */
+ * DFFT_DCT1 / DFFT_DST1: DCT-I / DST-I in both directions, n one of the lengths of that kind.  out == in is allowed. */
 int dfft_fft1d_r2r(int precision, int transform, int direction, size_t n, size_t a, size_t b, void* out, const void* in,
                    void* stream);
 
