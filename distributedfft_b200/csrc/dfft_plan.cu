@@ -510,8 +510,9 @@ static View single_view(void* base, long long sA0, long long sA1, long long sN) 
 namespace dfft {
 
 static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc);
-static int build_overlapped_slab(dfft_plan_s* p, int inverse, Schedule& sc);
-static int build_overlapped_pencil(dfft_plan_s* p, int inverse, Schedule& sc);
+static int build_overlapped_forward(dfft_plan_s* p, Schedule& sc);
+static int build_overlapped_slab_inverse(dfft_plan_s* p, Schedule& sc);
+static int build_overlapped_pencil_inverse(dfft_plan_s* p, Schedule& sc);
 static bool pencil_overlap_enabled();
 
 }  // namespace dfft
@@ -672,6 +673,175 @@ static int build_batch_small(dfft_plan_s* p, int inverse, Schedule& sc) {
     return DFFT_SUCCESS;
 }
 
+// One pass step of n-point lines along `axis` (0 x, 1 y, 2 z), with the tables of its length (pass_tables), recording the
+// timer section `phase`; the builders set its views and dims.  DCT / DST plans run the C2C builders over reals: their C2C
+// kinds become R2R ones, of the axis's kind.
+static int new_pass(dfft_plan_s* p, int inverse, PassKind kind, size_t n, int axis, const char* phase, Step& s) {
+    const Geometry& g = p->g;
+    s = Step();
+    s.type = STEP_PASS;
+    s.label = (kind == PASS_C2C_TILED) ? "strided pass" : (kind == PASS_R2C ? "z pass (R2C)" : (kind == PASS_C2R ? "z pass (C2R)" : "z pass"));
+    s.axis = axis;
+    s.phase = phase;
+    s.n = n;
+    s.prm.A0 = 1; s.prm.A1 = 1; s.prm.B = 1;
+    s.prm.inverse = inverse;
+    if (!p->taxes[axis]) {
+        // a kept axis: this pass's views, moved by the copy kernel without tables (labels: name_copies)
+        s.kind = kind == PASS_C2C_TILED ? PASS_COPY_TILED : PASS_COPY_CONTIG;
+        return DFFT_SUCCESS;
+    }
+    if (is_r2r(g.transform)) {
+        kind = kind == PASS_C2C_TILED ? PASS_R2R_TILED : PASS_R2R_CONTIG;
+        s.r2r = p->kinds[axis];
+    }
+    s.kind = kind;
+    // Bluestein lengths: the view mapping stays the kind's; the exec launches the Bluestein kernel.  Type-I R2R passes:
+    // log2 N of their N +- 1 reals per line
+    s.log2n = pass_log2(kind, n, s.r2r);
+    {   // padded plans: the spectral extent of the axis
+        const size_t k = axis == 0 ? g.kx : axis == 1 ? g.ky : g.kzc, full = axis == 0 ? g.nx : axis == 1 ? g.ny : g.nzc;
+        if (k != full) s.keep = k;
+    }
+    if (s.log2n < 1 || s.log2n > MAX_LOG2N)
+        return fail(DFFT_ERR_UNSUPPORTED, "axis length " + std::to_string(n) + " is not a supported power of two (2..8192)");
+    void *tw = nullptr, *tw2 = nullptr, *blu = nullptr;
+    const int rc = pass_tables(p->tabs, kind, n, s.r2r, &tw, &tw2, &blu);
+    s.prm.tw = tw;
+    s.prm.tw2 = tw2;
+    s.blu = blu;
+    return rc;
+}
+
+// A rendezvous of `group` (0 all ranks, 1 first transposition group, 2 second) on plan stream `stream`
+static Step new_rendezvous(int group, int phase_id, const char* phase, int stream) {
+    Step s;
+    s.type = STEP_RENDEZVOUS;
+    s.label = group == 0 ? "entry rendezvous" : (group == 1 ? "rendezvous 1" : "rendezvous 2");
+    s.group = group;
+    s.phase_id = phase_id;
+    s.phase = phase;
+    s.stream = stream;
+    return s;
+}
+
+// The blocked hand-over of the second transposition: the scattering pass (forward the y pass, inverse the x pass) stores
+// into the slots of its G2 members, the gathering pass (forward x, inverse y) reads its own.  A receiver's nz columns of z
+// are laid out as
+//   forward  [nzm/CH][nx][ny_q][CH] + tail [nx][ny_q][rem]      (ny_q: the receiver's y rows)
+//   inverse  [nzm/CH][ky][nx_q][CH] + tail [nx_q][ky][rem]      (nx_q: the receiver's x planes)
+// with rem = nz % CH leftover columns and nzm = nz - rem, so the rows a tile of the scattering pass sends to one receiver
+// are adjacent (one contiguous run per receiver: what NVLink stores need), and the gathering pass reads rows CH apart.
+// The tail is the plain layout of the leftover columns, run by one extra launch of each pass.  The other side of both
+// passes is plain, z innermost.  One rank, forward (x_inner): [ky][nzm/CH][nx][CH], so that every x-pass tile is one
+// contiguous block.  A pass covers planes [a, +npl) of its a0 axis and the z columns [z0, +zc), whole blocks.
+struct HandOver {
+    size_t CH = 0, rem = 0, nzm = 0;
+    bool any_rem = false;  // some rank of the grid has leftover columns: every rank runs the tail steps (B = 0 on the others)
+    bool fwd = true, x_inner = false;
+    int me = 0;
+    size_t es = 0, nz = 0;
+    size_t L = 0;            // extent of the scattering pass's a0 axis at the receivers (forward nx, inverse ky)
+    size_t M_me = 0;         // this rank's extent of its n axis (forward its y rows, inverse its x planes)
+    const Split* recv = nullptr;  // the receivers' extents along it (forward oy, inverse sx)
+    const std::vector<int>* G = nullptr;
+    const unsigned char* tab = nullptr;  // segment table of recv (scattering views over more than one receiver)
+    std::vector<void*> slot;             // the hand-over slot of every rank
+
+    // blocked: both transpositions are peer stores and both passes run (d = 3); sequential: the schedule of build_schedule,
+    // the only one that takes the x-innermost layout of one rank
+    HandOver(const dfft_plan_s* p, int inverse, bool blocked, bool sequential, const unsigned char* tab_, std::vector<void*> slot_) {
+        const Geometry& g = p->g;
+        me = p->rank;
+        fwd = !inverse;
+        es = p->esize * p->comps;
+        nz = g.sz.size[g.pj(me)];
+        L = fwd ? g.nx : g.ky;
+        recv = fwd ? &g.oy : &g.sx;
+        M_me = recv->size[g.pi(me)];
+        G = &p->grp[2];
+        tab = tab_;
+        slot = std::move(slot_);
+        CH = blocked && (fwd || p->blocked_inv) ? size_t(p->blocked_ch) : 0;
+        if (!CH) return;
+        rem = nz % CH;
+        nzm = nz - rem;
+        for (size_t v : g.sz.size) any_rem = any_rem || v % CH != 0;
+        x_inner = fwd && sequential && G->size() == 1 && p->single_rank_layout;
+    }
+    // The z chunks of the overlapped passes: ns ranges, of whole blocks when blocked (at most nzm / CH of them; the
+    // leftover columns go with the last one)
+    Split chunks(size_t ns) const {
+        Split c;
+        if (!CH) { c.make(nz, ns); return c; }
+        c.make(nzm / CH, std::min(ns, nzm / CH));
+        for (size_t k = 0; k < c.size.size(); ++k) { c.size[k] *= CH; c.start[k] *= CH; }
+        return c;
+    }
+    // The scattering pass: input `plain` (the whole z extent from its base), stores into every receiver
+    void scatter(Step& s, View plain, size_t a, size_t npl, size_t z0, size_t zc) const {
+        dims(s, npl, zc);
+        s.prm.in = columns(plain, z0, CH);
+        seg_view(s.prm.out, tab, *G, [&](int q, int r) { return blocks(slot[r], recv->size[q], a, z0, true, recv->start[q]); });
+    }
+    Step scatter_tail(const Step& s, View plain, size_t a) const {
+        Step t = tail(s);
+        t.prm.in = columns(plain, nzm, 0);
+        seg_view(t.prm.out, tab, *G, [&](int q, int r) { return leftover(slot[r], recv->size[q], a, true, recv->start[q]); });
+        return t;
+    }
+    // The gathering pass: reads its own slot, stores into `plain`
+    void gather(Step& s, View plain, size_t a, size_t npl, size_t z0, size_t zc) const {
+        dims(s, npl, zc);
+        s.prm.in = own(blocks(slot[me], M_me, a, z0, false, 0));
+        s.prm.out = columns(plain, z0, CH);
+    }
+    Step gather_tail(const Step& s, View plain, size_t a) const {
+        Step t = tail(s);
+        t.prm.in = own(leftover(slot[me], M_me, a, false, 0));
+        t.prm.out = columns(plain, nzm, 0);
+        return t;
+    }
+
+  private:
+    void dims(Step& s, size_t npl, size_t zc) const {
+        s.prm.A0 = int(npl); s.prm.A1 = int(zc / CH); s.prm.B = int(CH);
+    }
+    // the pass of the leftover columns: a copy of s, on the same stream, that waits for nothing and records nothing
+    Step tail(const Step& s) const {
+        Step t = s;
+        t.label = s.axis == 1 ? "y pass (tail)" : "x pass (tail)";
+        t.phase = nullptr;
+        t.prm.bulk_out = 0;
+        t.waits.clear();
+        t.record = -1;
+        t.prm.A1 = 1; t.prm.B = int(rem);
+        return t;
+    }
+    // the plain side from column z0 on: rows CH apart within a pass of blocks (sA1 = CH), one row per line in the tail
+    View columns(View v, size_t z0, size_t sA1) const {
+        for (int i = 0; i < v.nseg; ++i) {
+            v.seg[i].base = eptr(v.seg[i].base, z0, es);
+            v.seg[i].sA1 = (long long)sA1;
+        }
+        return v;
+    }
+    static View own(const SegN& sn) { return single_view(sn.s.base, sn.s.sA0, sn.s.sA1, sn.sN); }
+    // the blocked part in the slot `base` of a receiver holding m along the scattering pass's n axis: writer, a0 runs over
+    // L (from a) and n over m; reader, a0 runs over m (from a) and n over L
+    SegN blocks(void* base, size_t m, size_t a, size_t z0, bool writer, size_t n0) const {
+        const size_t sl = x_inner ? CH : m * CH, sm = x_inner ? nzm * L : CH, blk = x_inner ? L * CH : L * m * CH;
+        const size_t sa = writer ? sl : sm, sn = writer ? sm : sl;
+        return mkseg(eptr(base, (z0 / CH) * blk + a * sa, es), (long long)sa, (long long)blk, (long long)sn, n0);
+    }
+    // the tail behind it: x outermost (forward [L][m][rem], inverse [m][L][rem])
+    SegN leftover(void* base, size_t m, size_t a, bool writer, size_t n0) const {
+        const size_t sl = fwd ? m * rem : rem, sm = fwd ? rem : L * rem;
+        const size_t sa = writer ? sl : sm, sn = writer ? sm : sl;
+        return mkseg(eptr(base, L * m * nzm + a * sa, es), (long long)sa, 0, (long long)sn, n0);
+    }
+};
+
 static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     const Geometry& g = p->g;
     const int me = p->rank, P = p->P;
@@ -680,59 +850,8 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     const size_t es = p->esize * p->comps;
     // DCT / DST plans run the C2C builders over reals; new_pass turns their C2C kinds into R2R ones
     const bool c2c = g.transform != DFFT_R2C;
-    const bool r2r = is_r2r(g.transform);
     Tables& T = p->tabs;
     sc.steps.clear();
-
-    // axis: 0 x, 1 y, 2 z — R2R passes take their kind from it
-    auto new_pass = [&](PassKind kind, size_t n, int axis, const char* phase, Step& s) -> int {
-        s = Step();
-        s.type = STEP_PASS;
-        s.label = (kind == PASS_C2C_TILED) ? "strided pass" : (kind == PASS_R2C ? "z pass (R2C)" : (kind == PASS_C2R ? "z pass (C2R)" : "z pass"));
-        s.axis = axis;
-        if (!p->taxes[axis]) {
-            // a kept axis: this pass's views, moved by the copy kernel without tables (labels: name_copies)
-            s.kind = kind == PASS_C2C_TILED ? PASS_COPY_TILED : PASS_COPY_CONTIG;
-            s.phase = phase;
-            s.n = n;
-            s.prm.A0 = 1; s.prm.A1 = 1; s.prm.B = 1;
-            s.prm.inverse = inverse;
-            return DFFT_SUCCESS;
-        }
-        if (r2r) {
-            kind = kind == PASS_C2C_TILED ? PASS_R2R_TILED : PASS_R2R_CONTIG;
-            s.r2r = p->kinds[axis];
-        }
-        s.kind = kind;
-        s.phase = phase;
-        // Bluestein lengths: the view mapping stays the kind's; the exec launches the Bluestein kernel.  Type-I R2R passes:
-        // log2 N of their N +- 1 reals per line
-        s.log2n = pass_log2(kind, n, s.r2r);
-        s.n = n;
-        {   // padded plans: the spectral extent of the axis
-            const size_t k = axis == 0 ? g.kx : axis == 1 ? g.ky : g.kzc, full = axis == 0 ? g.nx : axis == 1 ? g.ny : g.nzc;
-            if (k != full) s.keep = k;
-        }
-        if (s.log2n < 1 || s.log2n > MAX_LOG2N)
-            return fail(DFFT_ERR_UNSUPPORTED, "axis length " + std::to_string(n) + " is not a supported power of two (2..8192)");
-        s.prm.A0 = 1; s.prm.A1 = 1; s.prm.B = 1;
-        s.prm.inverse = inverse;
-        void *tw = nullptr, *tw2 = nullptr, *blu = nullptr;
-        const int rc = pass_tables(T, kind, n, s.r2r, &tw, &tw2, &blu);
-        s.prm.tw = tw;
-        s.prm.tw2 = tw2;
-        s.blu = blu;
-        return rc;
-    };
-    auto rendezvous = [&](int group, int phase_id, const char* phase) {
-        Step s;
-        s.type = STEP_RENDEZVOUS;
-        s.label = group == 0 ? "entry rendezvous" : (group == 1 ? "rendezvous 1" : "rendezvous 2");
-        s.group = group;
-        s.phase_id = phase_id;
-        s.phase = phase;
-        sc.steps.push_back(s);
-    };
 
     // groups: transposition 1 / 2 member lists (positions along the split axis)
     const std::vector<int>& G1 = p->grp[1];
@@ -751,8 +870,14 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         if (p->buf_slot) return s == D1 ? nullptr : p->slot_ptr[s - 1][r];
         return p->slot_ptr[s][r];
     };
+    // the second transposition's hand-over in slot D2 (tab: the segment table of the scattering pass's receivers)
+    auto hand_over = [&](bool blocked, const unsigned char* tab) {
+        std::vector<void*> d2(P, nullptr);
+        if (blocked) for (int r = 0; r < P; ++r) d2[r] = slotp(D2, r);
+        return HandOver(p, inverse, blocked, true, tab, d2);
+    };
 
-    if (p->any_direct) rendezvous(0, 0, nullptr);  // everyone has left the previous exec: slots are free
+    if (p->any_direct) sc.steps.push_back(new_rendezvous(0, 0, nullptr, 0));  // everyone has left the previous exec: slots are free
 
     // spectral extents (padded plans: K; the pass lengths stay the physical N)
     const size_t kzc = g.kzc, ky = g.ky, kx = g.kx;
@@ -765,7 +890,6 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     const size_t ny_j = zyx ? g.ny : g.sy.size[pj], y0_j = zyx ? 0 : g.sy.start[pj];
     const size_t nz_j = zyx ? g.sz.size[me] : g.sz.size[pj], z0_j = zyx ? g.sz.start[me] : g.sz.start[pj];
     const size_t oy_i = zyx ? ky : g.oy.size[pi], oy0_i = zyx ? 0 : g.oy.start[pi];
-    (void)x0_i; (void)y0_j; (void)z0_j; (void)oy0_i;
 
     const unsigned char *tab_z = nullptr, *tab_y_in = nullptr, *tab_y_out = nullptr, *tab_x = nullptr;
     if (G1.size() > 1) {
@@ -795,7 +919,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         // ------------------------------------------------------------------ forward
         // pass 1: z (contiguous), lines (x in nx_i, y in ny_j)
         Step s1;
-        rc = new_pass(c2c ? PASS_C2C_CONTIG : PASS_R2C, c2c ? g.nz : g.nz / 2, 2, zyx || g.decomp == DFFT_PENCIL ? "1D FFT Z-Direction" : nullptr, s1);
+        rc = new_pass(p, inverse, c2c ? PASS_C2C_CONTIG : PASS_R2C, c2c ? g.nz : g.nz / 2, 2, zyx || g.decomp == DFFT_PENCIL ? "1D FFT Z-Direction" : nullptr, s1);
         if (rc) return rc;
         s1.prm.A0 = int(nx_i); s1.prm.A1 = int(ny_j);
         {   // input: caller's buffer; real lines of nz reals = nz/2 complex (in place: padded rows)
@@ -845,12 +969,12 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         if (g.decomp == DFFT_SLAB_ZY_THEN_X) s1.phase = nullptr;
         if (!zy) sc.steps.push_back(s1);
         if (t1_a2a) { x1.phase = zyx ? "Transpose (Finished All2All)" : "First Transpose (Finished All2All)"; x1.group = 1; sc.steps.push_back(x1); }
-        else if (G1.size() > 1) rendezvous(1, 1, zyx ? "Transpose (Finished Receive)" : "First Transpose (Finished Receive)");
+        else if (G1.size() > 1) sc.steps.push_back(new_rendezvous(1, 1, zyx ? "Transpose (Finished Receive)" : "First Transpose (Finished Receive)", 0));
 
         // pass 2: y (tiled): a0 = x, n = y, b = z in nz_j
         Step s2;
         const size_t nx2 = zyx ? g.nx : nx_i;  // x extent held after transposition 1
-        rc = new_pass(PASS_C2C_TILED, g.ny, 1, g.decomp == DFFT_SLAB_ZY_THEN_X ? "2D FFT Y-Z-Direction" : (zyx ? nullptr : "1D FFT Y-Direction"), s2);
+        rc = new_pass(p, inverse, PASS_C2C_TILED, g.ny, 1, g.decomp == DFFT_SLAB_ZY_THEN_X ? "2D FFT Y-Z-Direction" : (zyx ? nullptr : "1D FFT Y-Direction"), s2);
         if (rc) return rc;
         s2.label = "y pass";
         s2.prm.A0 = int(nx2); s2.prm.A1 = 1; s2.prm.B = int(nz_j);
@@ -877,7 +1001,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
             if (s2.prm.in.nseg != 1) return fail(DFFT_ERR_STATE, "internal: z_then_yx gather view");
             sc.steps.push_back(s2);
             Step s3;
-            rc = new_pass(PASS_C2C_TILED, g.nx, 0, "2D FFT Y-X-Direction", s3);
+            rc = new_pass(p, inverse, PASS_C2C_TILED, g.nx, 0, "2D FFT Y-X-Direction", s3);
             if (rc) return rc;
             s3.label = "x pass";
             s3.prm.A0 = 1; s3.prm.A1 = 1; s3.prm.B = int(ky * nz_j);
@@ -891,49 +1015,16 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         // transposition 2: scatter along y over G2 (column of the grid, or all ranks for the slab)
         Step x2;
         const bool t2_a2a = !dir2;
-        const size_t CH = (dir2 && !t1_a2a) ? size_t(p->blocked_ch) : 0;  // slab and pencil (second transposition)
-        const size_t rem = CH ? nz_j % CH : 0, nzm = nz_j - rem;
-        // every rank emits the same step list: when any rank of the grid has leftover columns the others run the
-        // tail steps as empty passes (B = 0)
-        bool any_rem = false;
-        if (CH) {
-            if (g.decomp == DFFT_PENCIL) { for (size_t v : g.sz.size) any_rem = any_rem || (v % CH != 0); }
-            else any_rem = rem != 0;
-        }
+        const HandOver ho = hand_over(dir1 && dir2, tab_y_out);
         Step s2t;
-        bool have_tail = false;
-        if (dir2 && CH) {
-            // blocked hand-over: receiver q holds [kzc/CH][nx][ny_q][CH] — the rows a y-pass tile sends to one
-            // destination (consecutive y) are adjacent, so every warp store is 512 contiguous bytes
-            s2.prm.A1 = int(nzm / CH); s2.prm.B = int(CH);
-            s2.prm.in.seg[0].sA1 = (long long)CH;
+        if (ho.CH) {
             // rows are only adjacent when the tile is CH wide: with remote peers take the wide tile (TB = CH = 8 for
             // the 1024-point f64 pass: 128-byte instead of 64-byte rows per NVLink write), locally the faster narrow one
             s2.prm.tile_pref = G2.size() > 1 ? p->xchg_tile_pref : 1;
             s2.prm.bulk_out = G2.size() > 1 ? p->bulk_store : 0;
-            if (G2.size() == 1 && p->single_rank_layout) {
-                // one rank: keep x innermost, [ny][nzm/CH][nx][CH] — every x-pass tile is one contiguous block
-                s2.prm.out = single_view(slotp(D2, me), (long long)CH, (long long)(g.nx * CH), (long long)((nzm / CH) * g.nx * CH));
-            } else {
-                seg_view(s2.prm.out, tab_y_out, G2, [&](int q, int r) {
-                    const size_t nyq = g.oy.size[q];
-                    return mkseg(eptr(slotp(D2, r), x0_i * nyq * CH, es), (long long)(nyq * CH), (long long)(g.nx * nyq * CH), (long long)CH, g.oy.start[q]);
-                });
-            }
-            if (any_rem) {  // leftover columns z in [nzm, kzc): plain layout [nx][ny_q][rem] behind the blocked part
-                s2t = s2;
-                have_tail = true;
-                s2t.label = "y pass (tail)";
-                s2t.prm.bulk_out = 0;
-                s2t.phase = nullptr;
-                s2t.prm.A1 = 1; s2t.prm.B = int(rem);
-                s2t.prm.in.seg[0].base = eptr(s2.prm.in.seg[0].base, nzm, es);
-                s2t.prm.in.seg[0].sA1 = 0;
-                seg_view(s2t.prm.out, tab_y_out, G2, [&](int q, int r) {
-                    const size_t nyq = g.oy.size[q];
-                    return mkseg(eptr(slotp(D2, r), g.nx * nyq * nzm + x0_i * nyq * rem, es), (long long)(nyq * rem), 0, (long long)rem, g.oy.start[q]);
-                });
-            }
+            const View in = s2.prm.in;
+            ho.scatter(s2, in, x0_i, nx_i, 0, ho.nzm);
+            if (ho.any_rem) s2t = ho.scatter_tail(s2, in, x0_i);
         } else if (dir2) {
             if (G2.size() > 1) s2.prm.tile_pref = p->xchg_tile_pref;
             seg_view(s2.prm.out, tab_y_out, G2, [&](int q, int r) {
@@ -948,38 +1039,29 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
             });
         }
         if (zy) {
-            if (have_tail || t1_a2a || t2_a2a || G1.size() > 1 || G2.size() > 1) return fail(DFFT_ERR_STATE, "internal: fused z + y stage");
+            if (ho.any_rem || t1_a2a || t2_a2a || G1.size() > 1 || G2.size() > 1) return fail(DFFT_ERR_STATE, "internal: fused z + y stage");
             Step f;
             rc = fuse_zy(p, s1, s2, "zy pass", s2.phase, f);
             if (rc) return rc;
             sc.steps.push_back(f);
-        } else if (have_tail) { const char* ph = s2.phase; s2.phase = nullptr; sc.steps.push_back(s2); s2t.phase = ph; sc.steps.push_back(s2t); }
+        } else if (ho.any_rem) { const char* ph = s2.phase; s2.phase = nullptr; sc.steps.push_back(s2); s2t.phase = ph; sc.steps.push_back(s2t); }
         else sc.steps.push_back(s2);
         const bool slab = g.decomp == DFFT_SLAB_ZY_THEN_X;
         if (t2_a2a) { x2.phase = slab ? "Transpose (Finished All2All)" : "Second Transpose (Finished All2All)"; x2.group = 2; sc.steps.push_back(x2); }
-        else if (G2.size() > 1) rendezvous(2, 2, slab ? "Transpose (Finished Receive)" : "Second Transpose (Finished Receive)");
+        else if (G2.size() > 1) sc.steps.push_back(new_rendezvous(2, 2, slab ? "Transpose (Finished Receive)" : "Second Transpose (Finished Receive)", 0));
 
         // pass 3: x (tiled): n = x, b = (y in oy_i, z in nz_j); received blocks are x-major => contiguous
         Step s3;
-        rc = new_pass(PASS_C2C_TILED, g.nx, 0, "1D FFT X-Direction", s3);
+        rc = new_pass(p, inverse, PASS_C2C_TILED, g.nx, 0, "1D FFT X-Direction", s3);
         if (rc) return rc;
         s3.label = "x pass";
-        if (CH) {
-            // in: [kzc/CH][nx][oy_i][CH]: a0 = y_loc, a1 = z chunk, n = x
-            s3.prm.A0 = int(oy_i); s3.prm.A1 = int(nzm / CH); s3.prm.B = int(CH);
-            if (G2.size() == 1 && p->single_rank_layout)
-                s3.prm.in = single_view(slotp(D2, me), (long long)((nzm / CH) * g.nx * CH), (long long)(g.nx * CH), (long long)CH);
-            else
-                s3.prm.in = single_view(slotp(D2, me), (long long)CH, (long long)(g.nx * oy_i * CH), (long long)(oy_i * CH));
-            s3.prm.out = single_view(nullptr, (long long)nz_j, (long long)CH, (long long)(oy_i * nz_j));
+        if (ho.CH) {
+            // a0 = y_loc, a1 = z block, n = x
+            const View out = single_view(nullptr, (long long)nz_j, 0, (long long)(oy_i * nz_j));
+            ho.gather(s3, out, 0, oy_i, 0, ho.nzm);
             s3.prm.tile_swz = p->x_swz;
-            if (any_rem) {
-                Step s3t = s3;
-                s3t.label = "x pass (tail)";
-                s3t.phase = nullptr;
-                s3t.prm.A0 = int(oy_i); s3t.prm.A1 = 1; s3t.prm.B = int(rem);
-                s3t.prm.in = single_view(eptr(slotp(D2, me), g.nx * oy_i * nzm, es), (long long)rem, 0, (long long)(oy_i * rem));
-                s3t.prm.out = single_view((void*)(size_t)(nzm * es), (long long)nz_j, 0, (long long)(oy_i * nz_j));
+            if (ho.any_rem) {
+                Step s3t = ho.gather_tail(s3, out, 0);
                 s3t.out_user = 2;
                 sc.steps.push_back(s3t);
             }
@@ -1002,7 +1084,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
 
     if (d == 1) {
         Step s;
-        rc = new_pass(zkind, zlen, 2, "1D FFT Z-Direction", s);
+        rc = new_pass(p, inverse, zkind, zlen, 2, "1D FFT Z-Direction", s);
         if (rc) return rc;
         s.prm.A0 = int(nx_i); s.prm.A1 = int(ny_j);
         s.prm.in = single_view(nullptr, (long long)(ny_j * kzc), (long long)kzc, 1);
@@ -1018,7 +1100,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         // input [nx][ny][nz_me]: y pass (to a slot), x pass scattering along x to the owners of x,
         // then z inverse on [nx_me][ny][kzc].
         Step sy_;
-        rc = new_pass(PASS_C2C_TILED, g.ny, 1, nullptr, sy_);
+        rc = new_pass(p, inverse, PASS_C2C_TILED, g.ny, 1, nullptr, sy_);
         if (rc) return rc;
         sy_.label = "y pass";
         const int W = dir1 ? D2 : SR;  // a local scratch slot that is not the transposition target
@@ -1031,7 +1113,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         sy_.prm.out = single_view(slotp(no_x ? D1 : W, me), (long long)(g.ny * nz_j), 0, (long long)nz_j);
         sc.steps.push_back(sy_);
         Step sx_;
-        rc = new_pass(PASS_C2C_TILED, g.nx, 0, "2D FFT Y-X-Direction", sx_);
+        rc = new_pass(p, inverse, PASS_C2C_TILED, g.nx, 0, "2D FFT Y-X-Direction", sx_);
         if (rc) return rc;
         sx_.label = "x pass";
         sx_.prm.A0 = 1; sx_.prm.A1 = int(g.ny); sx_.prm.B = int(nz_j);
@@ -1049,9 +1131,9 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         }
         if (!no_x) sc.steps.push_back(sx_);
         if (!dir1) { xa.phase = "Transpose (Finished All2All)"; xa.group = 1; sc.steps.push_back(xa); }
-        else if (G1.size() > 1) rendezvous(1, 1, "Transpose (Finished Receive)");
+        else if (G1.size() > 1) sc.steps.push_back(new_rendezvous(1, 1, "Transpose (Finished Receive)", 0));
         Step sz_;
-        rc = new_pass(zkind, zlen, 2, "1D FFT Z-Direction", sz_);
+        rc = new_pass(p, inverse, zkind, zlen, 2, "1D FFT Z-Direction", sz_);
         if (rc) return rc;
         sz_.prm.A0 = int(nx_i); sz_.prm.A1 = int(g.ny);
         if (dir1) sz_.prm.in = single_view(slotp(D1, me), (long long)(g.ny * kzc), (long long)kzc, 1);
@@ -1069,89 +1151,59 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
 
     // pencil / slab zy_x inverse
     const bool slab = g.decomp == DFFT_SLAB_ZY_THEN_X;
-    // Blocked hand-over for the inverse as well (mirror of the forward one): the x pass stores into the receivers as
-    // [nz_j/CH][ny][nx_q][CH] (+ a plain tail of nz_j % CH columns), so the rows a tile sends to one destination —
-    // consecutive x — are adjacent (one contiguous run per destination), and the y pass reads rows nx_i*CH apart
-    // instead of one row per (y, z) plane.  DFFT_BLOCKED_INV=0 keeps the plain layout.
-    const size_t CHI = (d == 3 && dir2 && dir1 && p->blocked_inv) ? size_t(p->blocked_ch) : 0;
-    if (CHI) {
-        const size_t CH = CHI;
-        const size_t rem = nz_j % CH, nzm = nz_j - rem;
-        bool any_rem = false;
-        if (g.decomp == DFFT_PENCIL) { for (size_t v : g.sz.size) any_rem = any_rem || (v % CH != 0); }
-        else any_rem = rem != 0;
+    // Blocked hand-over for the inverse as well (HandOver; DFFT_BLOCKED_INV=0 keeps the plain layout): the y pass reads rows
+    // nx_i*CH apart instead of one row per (y, z) plane
+    const HandOver ho = hand_over(d == 3 && dir2 && dir1, tab_x);
+    if (ho.CH) {
         // x pass: in = caller's [nx][oy_i][nz_j]; tile = (y_loc, z block); n = x
         Step s3;
-        rc = new_pass(PASS_C2C_TILED, g.nx, 0, "1D FFT X-Direction", s3);
+        rc = new_pass(p, inverse, PASS_C2C_TILED, g.nx, 0, "1D FFT X-Direction", s3);
         if (rc) return rc;
         s3.label = "x pass";
-        s3.prm.A0 = int(oy_i); s3.prm.A1 = int(nzm / CH); s3.prm.B = int(CH);
-        s3.prm.in = single_view(nullptr, (long long)nz_j, (long long)CH, (long long)(oy_i * nz_j));
         s3.in_user = 1;
         s3.prm.tile_pref = G2.size() > 1 ? p->xchg_tile_pref : 1;
         s3.prm.bulk_out = G2.size() > 1 ? p->bulk_store : 0;
-        seg_view(s3.prm.out, tab_x, G2, [&](int q, int r) {
-            const size_t nxq = g.sx.size[q];
-            return mkseg(eptr(slotp(D2, r), oy0_i * nxq * CH, es), (long long)(nxq * CH), (long long)(ky * nxq * CH), (long long)CH, g.sx.start[q]);
-        });
-        Step s3t;
-        if (any_rem) {  // leftover columns: plain [nx_q][ny][rem] behind the blocked part
-            s3t = s3;
-            s3t.label = "x pass (tail)";
-            s3t.phase = nullptr;
-            s3t.prm.bulk_out = 0;
-            s3t.prm.A0 = int(oy_i); s3t.prm.A1 = 1; s3t.prm.B = int(rem);
-            s3t.prm.in = single_view((void*)(size_t)(nzm * es), (long long)nz_j, 0, (long long)(oy_i * nz_j));
-            seg_view(s3t.prm.out, tab_x, G2, [&](int q, int r) {
-                const size_t nxq = g.sx.size[q];
-                return mkseg(eptr(slotp(D2, r), ky * nxq * nzm + oy0_i * rem, es), (long long)rem, 0, (long long)(ky * rem), g.sx.start[q]);
-            });
-            const char* ph = s3.phase; s3.phase = nullptr; s3t.phase = ph;
+        const View in = single_view(nullptr, (long long)nz_j, 0, (long long)(oy_i * nz_j));
+        ho.scatter(s3, in, oy0_i, oy_i, 0, ho.nzm);
+        if (ho.any_rem) {
+            Step s3t = ho.scatter_tail(s3, in, oy0_i);
+            std::swap(s3.phase, s3t.phase);
             sc.steps.push_back(s3);
             sc.steps.push_back(s3t);
         } else {
             sc.steps.push_back(s3);
         }
-        if (G2.size() > 1) rendezvous(2, 2, slab ? "Transpose (Finished Receive)" : "Second Transpose (Finished Receive)");
-        // y pass: in = my slot, blocked [nz_j/CH][ny][nx_i][CH]; tile = (x_loc, z block); n = y
+        if (G2.size() > 1) sc.steps.push_back(new_rendezvous(2, 2, slab ? "Transpose (Finished Receive)" : "Second Transpose (Finished Receive)", 0));
+        // y pass: tile = (x_loc, z block); n = y; dest (i, q) holds [nx_i][ny_q][kzc], my columns z in [z0_j, +nz_j)
         Step s2;
-        rc = new_pass(PASS_C2C_TILED, g.ny, 1, slab ? nullptr : "1D FFT Y-Direction", s2);
+        rc = new_pass(p, inverse, PASS_C2C_TILED, g.ny, 1, slab ? nullptr : "1D FFT Y-Direction", s2);
         if (rc) return rc;
         s2.label = "y pass";
-        s2.prm.A0 = int(nx_i); s2.prm.A1 = int(nzm / CH); s2.prm.B = int(CH);
-        s2.prm.in = single_view(slotp(D2, me), (long long)CH, (long long)(ky * nx_i * CH), (long long)(nx_i * CH));
-        if (G1.size() > 1) s2.prm.tile_pref = p->xchg_tile_pref;
-        else s2.prm.tile_pref = 1;
-        seg_view(s2.prm.out, tab_y_in, G1, [&](int q, int r) {
+        s2.prm.tile_pref = G1.size() > 1 ? p->xchg_tile_pref : 1;
+        View out{};
+        seg_view(out, tab_y_in, G1, [&](int q, int r) {
             const size_t nyq = g.sy.size[q];
-            return mkseg(eptr(slotp(D1, r), z0_j, es), (long long)(nyq * kzc), (long long)CH, (long long)kzc, g.sy.start[q]);
+            return mkseg(eptr(slotp(D1, r), z0_j, es), (long long)(nyq * kzc), 0, (long long)kzc, g.sy.start[q]);
         });
-        if (any_rem) {
-            Step s2t = s2;
-            s2t.label = "y pass (tail)";
-            s2t.phase = nullptr;
-            s2t.prm.A0 = int(nx_i); s2t.prm.A1 = 1; s2t.prm.B = int(rem);
-            s2t.prm.in = single_view(eptr(slotp(D2, me), ky * nx_i * nzm, es), (long long)(ky * rem), 0, (long long)rem);
-            seg_view(s2t.prm.out, tab_y_in, G1, [&](int q, int r) {
-                const size_t nyq = g.sy.size[q];
-                return mkseg(eptr(slotp(D1, r), z0_j + nzm, es), (long long)(nyq * kzc), 0, (long long)kzc, g.sy.start[q]);
-            });
-            const char* ph = s2.phase; s2.phase = nullptr; s2t.phase = ph;
+        ho.gather(s2, out, 0, nx_i, 0, ho.nzm);
+        if (ho.any_rem) {
+            Step s2t = ho.gather_tail(s2, out, 0);
+            std::swap(s2.phase, s2t.phase);
             sc.steps.push_back(s2);
             sc.steps.push_back(s2t);
         } else if (!zy) {
             sc.steps.push_back(s2);
         }
-        if (G1.size() > 1) rendezvous(1, 1, "First Transpose (Finished Receive)");
+        if (G1.size() > 1) sc.steps.push_back(new_rendezvous(1, 1, "First Transpose (Finished Receive)", 0));
         Step s1;
-        rc = new_pass(zkind, zlen, 2, slab ? "2D FFT Y-Z-Direction" : "1D FFT Z-Direction", s1);
+        rc = new_pass(p, inverse, zkind, zlen, 2, slab ? "2D FFT Y-Z-Direction" : "1D FFT Z-Direction", s1);
         if (rc) return rc;
         s1.prm.A0 = int(nx_i); s1.prm.A1 = int(ny_j);
         s1.prm.in = single_view(slotp(D1, me), (long long)(ny_j * kzc), (long long)kzc, 1);
         s1.prm.out = single_view(nullptr, zpitch_out * (long long)ny_j, zpitch_out, 1);
         s1.out_user = 2;
         if (zy) {
-            if (any_rem || G1.size() > 1 || G2.size() > 1) return fail(DFFT_ERR_STATE, "internal: fused z + y stage");
+            if (ho.any_rem || G1.size() > 1 || G2.size() > 1) return fail(DFFT_ERR_STATE, "internal: fused z + y stage");
             Step f;
             rc = fuse_zy(p, s1, s2, "yz pass", s1.phase, f);
             if (rc) return rc;
@@ -1166,7 +1218,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     bool have_in_slot = false;  // whether the y pass input is in a slot (d == 3) or the caller's buffer (d == 2)
     if (d == 3) {
         Step s3;
-        rc = new_pass(PASS_C2C_TILED, g.nx, 0, "1D FFT X-Direction", s3);
+        rc = new_pass(p, inverse, PASS_C2C_TILED, g.nx, 0, "1D FFT X-Direction", s3);
         if (rc) return rc;
         s3.label = "x pass";
         s3.prm.A0 = 1; s3.prm.A1 = 1; s3.prm.B = int(oy_i * nz_j);
@@ -1186,12 +1238,12 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         }
         sc.steps.push_back(s3);
         if (!dir2) { x2.phase = slab ? "Transpose (Finished All2All)" : "Second Transpose (Finished All2All)"; x2.group = 2; sc.steps.push_back(x2); }
-        else if (G2.size() > 1) rendezvous(2, 2, slab ? "Transpose (Finished Receive)" : "Second Transpose (Finished Receive)");
+        else if (G2.size() > 1) sc.steps.push_back(new_rendezvous(2, 2, slab ? "Transpose (Finished Receive)" : "Second Transpose (Finished Receive)", 0));
         have_in_slot = true;
     }
     // y pass on [nx_i][ky][nz_j]
     Step s2;
-    rc = new_pass(PASS_C2C_TILED, g.ny, 1, slab ? nullptr : "1D FFT Y-Direction", s2);
+    rc = new_pass(p, inverse, PASS_C2C_TILED, g.ny, 1, slab ? nullptr : "1D FFT Y-Direction", s2);
     if (rc) return rc;
     s2.label = "y pass";
     s2.prm.A0 = int(nx_i); s2.prm.A1 = 1; s2.prm.B = int(nz_j);
@@ -1223,10 +1275,10 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     }
     sc.steps.push_back(s2);
     if (!dir1) { x1.phase = "First Transpose (Finished All2All)"; x1.group = 1; sc.steps.push_back(x1); }
-    else if (G1.size() > 1) rendezvous(1, 1, "First Transpose (Finished Receive)");
+    else if (G1.size() > 1) sc.steps.push_back(new_rendezvous(1, 1, "First Transpose (Finished Receive)", 0));
     // z pass on [nx_i][ny_j][kzc]
     Step s1;
-    rc = new_pass(zkind, zlen, 2, slab ? "2D FFT Y-Z-Direction" : "1D FFT Z-Direction", s1);
+    rc = new_pass(p, inverse, zkind, zlen, 2, slab ? "2D FFT Y-Z-Direction" : "1D FFT Z-Direction", s1);
     if (rc) return rc;
     s1.prm.A0 = int(nx_i); s1.prm.A1 = int(ny_j);
     if (dir1) s1.prm.in = single_view(slotp(D1, me), (long long)(ny_j * kzc), (long long)kzc, 1);
@@ -1239,7 +1291,6 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     s1.out_user = 2;
     sc.steps.push_back(s1);
     sc.built = true;
-    (void)P;
     return DFFT_SUCCESS;
 }
 
@@ -1247,23 +1298,180 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
 
 namespace dfft {
 
-// Overlapped slab (ZY_Then_X) schedule, Peer2Peer, SendMethod Streams.
+// Overlapped schedules, Peer2Peer on every transposition (send_method Streams): slab ZY_Then_X and pencil.
 //
-// The reference's Streams variant overlaps pack(q+1) with send(q) (mpicufft_slab.cpp:398-415).  Here the
-// exchange is the y pass itself (NVLink-bound), so the overlap is between whole FFT passes:
-//   stream 0 (caller) : z pass, plane group by plane group                       (HBM-bound)
-//   stream 1 (exchange, high priority): y pass per (plane group, z chunk), persistent on `xchg_ctas`
-//                       SMs, storing straight into the peers' slots              (NVLink-bound)
-//   stream 2 (follow-up): per z chunk: rendezvous with the peers, then the x pass of that chunk (HBM-bound)
-// The y pass of chunk c+1 runs while the x pass consumes chunk c, and while later plane groups are still in
-// the z pass.  Inverse: x pass per z chunk scatters (stream 1), y pass per chunk follows (stream 2), the z
-// pass runs last on the caller's stream.
+// The reference's Streams variant overlaps pack(q+1) with send(q) (mpicufft_slab.cpp:398-415).  Here the exchanges are
+// FFT passes that store straight into the peers' slots, so the overlap is between whole FFT passes.  Forward, one builder
+// for both: a slab is the pencil grid with one-member row groups (G1 = {me}), whose z pass stores into my own slot A and
+// whose y pass waits for it without a rendezvous:
+//   stream 0: z pass per plane group, scattering along z into the row peers' slot A             (HBM / NVLink-bound)
+//   stream 1: per plane group: meet the row peers; then the y pass per (plane group, z chunk), persistent on
+//             `xchg_ctas` CTAs, scattering along y into the column peers' slot B                 (NVLink-bound)
+//   stream 2: per z chunk: meet the column peers, x pass of that chunk                           (HBM-bound)
+// The y pass of chunk c+1 runs while the x pass consumes chunk c, and while later plane groups are still in the z pass.
+// On a pencil grid only the x pass can hide behind an exchange (both scatters share the NVLink ports).
+// Slab inverse: x pass per z chunk scatters (stream 1), y pass per chunk follows (stream 2), the z pass runs last on the
+// caller's stream.  Pencil inverse: it mirrors the forward one — again only the local pass, now the z pass, can hide:
+//   stream 0: x pass, scattering along x into the column peers' slot B; meet the column peers   (NVLink-bound)
+//   stream 1: y pass per plane group on a capped grid, scattering along y into the row peers' slot A  (NVLink-bound)
+//   stream 2: per plane group: meet the row peers, z pass of that group into the caller's buffer  (HBM-bound)
 static int exchange_ctas(const dfft_plan_s* p, int inverse) {
     const int t = p->tuned_ctas[inverse ? 1 : 0];
     return t != -2 ? t : p->xchg_ctas;
 }
 
-static int build_overlapped_slab(dfft_plan_s* p, int inverse, Schedule& sc) {
+// Plane groups of the overlapped z / y passes and z chunks of their y / x passes: every rank must build the same number
+// of steps, so both derive from global minima
+static size_t plane_groups(const dfft_plan_s* p, int inverse) {
+    size_t min_nx = p->g.nx;
+    for (size_t v : p->g.sx.size) min_nx = std::min(min_nx, v);
+    return std::min<size_t>(size_t(inverse && p->tuned_groups_inv > 0 ? p->tuned_groups_inv : p->ovl_groups), min_nx);
+}
+static size_t z_chunk_count(const dfft_plan_s* p, int inverse) {
+    size_t min_nz = p->g.nzc;
+    for (size_t v : p->g.sz.size) min_nz = std::min(min_nz, v);
+    const int t = p->tuned_chunks[inverse ? 1 : 0];
+    const size_t want = size_t(t > 0 ? t : p->ovl_chunks);
+    return min_nz >= 32 * want ? want : (min_nz >= 32 ? 2 : 1);
+}
+
+// the overlapped schedules' hand-over in slot B (tab: the segment table of the scattering pass's receivers)
+static HandOver overlapped_hand_over(const dfft_plan_s* p, int inverse, const unsigned char* tab) {
+    return HandOver(p, inverse, true, false, tab, p->slot_ptr[1]);
+}
+
+static int build_overlapped_forward(dfft_plan_s* p, Schedule& sc) {
+    const Geometry& g = p->g;
+    const int me = p->rank;
+    const int pi = g.pi(me), pj = g.pj(me);
+    const size_t es = p->esize;
+    const bool c2c = g.transform == DFFT_C2C;
+    Tables& T = p->tabs;
+    sc.steps.clear();
+    sc.overlapped = true;
+    const size_t ny = g.ny;
+    const size_t nx_i = g.sx.size[pi], x0_i = g.sx.start[pi];
+    const size_t ny_j = g.sy.size[pj], y0_j = g.sy.start[pj];
+    const size_t nz_j = g.sz.size[pj];
+    const size_t oy_i = g.oy.size[pi];
+    const std::vector<int>& G1 = p->grp[1];
+    const std::vector<int>& G2 = p->grp[2];
+    const int D1 = 0, D2 = 1;
+    auto slotp = [&](int s_, int r) -> void* { return p->slot_ptr[s_][r]; };
+    int nev = 0;
+
+    const size_t NG = plane_groups(p, 0), NS = z_chunk_count(p, 0);
+    Split groups;
+    groups.make(nx_i, NG);
+    // a slab has no first transposition: its z pass stores into my own slot A
+    const bool pencil = g.decomp == DFFT_PENCIL;
+    const unsigned char *tab_z = nullptr, *tab_y = nullptr;
+    if ((pencil && T.seg_table(g.sz, &tab_z) != cudaSuccess) || T.seg_table(g.oy, &tab_y) != cudaSuccess)
+        return fail(DFFT_ERR_CUDA, "segment table");
+    const HandOver ho = overlapped_hand_over(p, 0, tab_y);
+    const Split chunks = ho.chunks(NS);
+    // the ranks of a pencil grid hold different z extents: a chunk count clamped to one rank's blocks could differ
+    // between them
+    if (pencil && chunks.size.size() != NS) return fail(DFFT_ERR_STATE, "internal: blocked z chunks");
+    const size_t NSc = chunks.size.size();
+
+    sc.steps.push_back(new_rendezvous(0, 0, nullptr, 0));  // everyone has left the previous exec
+    // the auxiliary streams fork from the caller's stream at the start of run_schedule, i.e. BEFORE the
+    // entry rendezvous: make them wait for it explicitly
+    const int ev_entry = nev++;
+    sc.steps.back().record = ev_entry;
+    int rc;
+    std::vector<int> ev_z(NG), ev_y(NSc);
+    for (size_t gi = 0; gi < NG; ++gi) {
+        Step s;
+        rc = new_pass(p, 0, c2c ? PASS_C2C_CONTIG : PASS_R2C, c2c ? g.nz : g.nz / 2, 2, nullptr, s);
+        if (rc) return rc;
+        const size_t pl0 = groups.start[gi], npl = groups.size[gi];
+        const long long pitch = z_row_pitch(p);
+        s.prm.A0 = int(npl); s.prm.A1 = int(ny_j);
+        s.prm.in = single_view((void*)(size_t)(pl0 * ny_j * pitch * es), pitch * (long long)ny_j, pitch, 1);
+        s.in_user = 1;
+        seg_view(s.prm.out, tab_z, G1, [&](int q, int r) {
+            const size_t nzq = g.sz.size[q];
+            return mkseg(eptr(slotp(D1, r), (pl0 * ny + y0_j) * nzq, es), (long long)(ny * nzq), (long long)nzq, 1, g.sz.start[q]);
+        });
+        s.record = ev_z[gi] = nev++;
+        sc.steps.push_back(s);
+    }
+    for (size_t c = 0; c < NSc; ++c) {
+        const size_t z0 = chunks.start[c], zc = chunks.size[c];
+        for (size_t gi = 0; gi < NG; ++gi) {
+            const size_t pl0 = groups.start[gi], npl = groups.size[gi];
+            Step s;
+            rc = new_pass(p, 0, PASS_C2C_TILED, ny, 1, nullptr, s);
+            if (rc) return rc;
+            s.label = "y pass";
+            if (c == 0) {
+                // plane group gi has arrived: at a rendezvous with the row peers, or (slab) straight from my own z pass
+                std::vector<int> w{ev_z[gi]};
+                if (gi == 0) w.push_back(ev_entry);
+                if (pencil) {
+                    Step r = new_rendezvous(1, 1, nullptr, 1);
+                    r.waits = w;
+                    sc.steps.push_back(r);
+                } else {
+                    s.waits = w;
+                }
+            }
+            const View in = single_view(eptr(slotp(D1, me), pl0 * ny * nz_j, es), (long long)(ny * nz_j), 0, (long long)nz_j);
+            if (ho.CH) {
+                s.prm.bulk_out = G2.size() > 1 ? p->bulk_store : 0;
+                ho.scatter(s, in, x0_i + pl0, npl, z0, zc);
+            } else {
+                s.prm.A0 = int(npl); s.prm.A1 = 1; s.prm.B = int(zc);
+                s.prm.in = single_view(eptr(slotp(D1, me), pl0 * ny * nz_j + z0, es), (long long)(ny * nz_j), 0, (long long)nz_j);
+                seg_view(s.prm.out, tab_y, G2, [&](int q, int r) {
+                    const size_t nyq = g.oy.size[q];
+                    return mkseg(eptr(slotp(D2, r), (x0_i + pl0) * nyq * nz_j + z0, es), (long long)(nyq * nz_j), 0, (long long)nz_j, g.oy.start[q]);
+                });
+            }
+            s.prm.max_ctas = exchange_ctas(p, 0);
+            s.prm.tile_pref = G2.size() > 1 ? p->xchg_tile_pref : 0;
+            s.stream = 1;
+            const bool tail_here = ho.any_rem && c + 1 == NSc;
+            if (gi + 1 == NG && !tail_here) s.record = ev_y[c] = nev++;
+            sc.steps.push_back(s);
+            if (tail_here) {
+                Step t = ho.scatter_tail(s, in, x0_i + pl0);
+                if (gi + 1 == NG) t.record = ev_y[c] = nev++;
+                sc.steps.push_back(t);
+            }
+        }
+    }
+    const View out = single_view(nullptr, (long long)nz_j, 0, (long long)(oy_i * nz_j));
+    for (size_t c = 0; c < NSc; ++c) {
+        const size_t z0 = chunks.start[c], zc = chunks.size[c];
+        Step r = new_rendezvous(2, 2, nullptr, 2);
+        r.waits.push_back(ev_y[c]);
+        sc.steps.push_back(r);
+        Step s;
+        rc = new_pass(p, 0, PASS_C2C_TILED, g.nx, 0, nullptr, s);
+        if (rc) return rc;
+        s.label = "x pass";
+        if (ho.CH) {
+            ho.gather(s, out, 0, oy_i, z0, zc);
+            s.prm.tile_swz = p->x_swz;
+        } else {
+            s.prm.A0 = 1; s.prm.A1 = int(oy_i); s.prm.B = int(zc);
+            s.prm.in = single_view(eptr(slotp(D2, me), z0, es), 0, (long long)nz_j, (long long)(oy_i * nz_j));
+            s.prm.out = single_view((void*)(size_t)(z0 * es), 0, (long long)nz_j, (long long)(oy_i * nz_j));
+        }
+        s.out_user = 2;
+        s.stream = 2;
+        sc.steps.push_back(s);
+        if (ho.any_rem && c + 1 == NSc) sc.steps.push_back(ho.gather_tail(s, out, 0));
+    }
+    sc.nevents = nev;
+    sc.built = true;
+    return DFFT_SUCCESS;
+}
+
+static int build_overlapped_slab_inverse(dfft_plan_s* p, Schedule& sc) {
     const Geometry& g = p->g;
     const int me = p->rank;
     const size_t es = p->esize;
@@ -1271,264 +1479,97 @@ static int build_overlapped_slab(dfft_plan_s* p, int inverse, Schedule& sc) {
     Tables& T = p->tabs;
     sc.steps.clear();
     sc.overlapped = true;
-    const size_t nzc = g.nzc, ny = g.ny, nx = g.nx;
-    const size_t nx_p = g.sx.size[me], x0 = g.sx.start[me];
+    const size_t nzc = g.nzc, ny = g.ny;
+    const size_t nx_p = g.sx.size[me];
     const size_t oy_me = g.oy.size[me], oy0_me = g.oy.start[me];
     const std::vector<int>& G2 = p->grp[2];
     const int D1 = 0, D2 = 1;
     auto slotp = [&](int s_, int r) -> void* { return p->slot_ptr[s_][r]; };
     int nev = 0;
 
-    auto new_pass = [&](PassKind kind, size_t n, const char* label, Step& s) -> int {
-        s = Step();
-        s.type = STEP_PASS;
-        s.kind = kind;
-        s.label = label;
-        s.log2n = ilog2_exact(n);
-        if (s.log2n < 1 || s.log2n > MAX_LOG2N) return fail(DFFT_ERR_UNSUPPORTED, "unsupported axis length");
-        s.prm.A0 = 1; s.prm.A1 = 1; s.prm.B = 1;
-        s.prm.inverse = inverse;
-        void* tw = nullptr;
-        if (T.get_tw(s.log2n, &tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
-        s.prm.tw = tw;
-        if (kind == PASS_R2C || kind == PASS_C2R) {
-            void* tw2 = nullptr;
-            if (T.get_tw2(s.log2n, &tw2) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
-            s.prm.tw2 = tw2;
-        }
-        return DFFT_SUCCESS;
-    };
-    auto rendezvous = [&](int group, int phase_id, int stream) {
-        Step s;
-        s.type = STEP_RENDEZVOUS;
-        s.label = group == 0 ? "entry rendezvous" : "rendezvous 2";
-        s.group = group;
-        s.phase_id = phase_id;
-        s.stream = stream;
-        return s;
-    };
-
-    // plane groups (of my x planes) and z chunks
-    Split groups, chunks;
-    size_t min_nx = nx;  // the same number of plane groups (and steps) on every rank, also for uneven splits of x
-    for (size_t v : g.sx.size) min_nx = std::min(min_nx, v);
-    const size_t NG = std::min<size_t>(size_t(p->ovl_groups), std::max<size_t>(min_nx, 1));
-    const size_t want_chunks = size_t(p->tuned_chunks[inverse ? 1 : 0] > 0 ? p->tuned_chunks[inverse ? 1 : 0] : p->ovl_chunks);
-    const size_t NS = nzc >= 32 * want_chunks ? want_chunks : (nzc >= 32 ? 2 : 1);
-    groups.make(nx_p, NG);
-    const size_t CH = (inverse && !p->blocked_inv) ? 0 : size_t(p->blocked_ch);  // blocked hand-over, both directions
-    const size_t rem = CH ? nzc % CH : 0, nzm = nzc - rem;
-    if (CH) {  // z chunks are whole multiples of the block width; the Nzc % CH leftover columns ride with the last chunk
-        Split u;
-        u.make(nzm / CH, std::min<size_t>(NS, nzm / CH));
-        chunks.size.clear(); chunks.start.clear();
-        for (size_t c = 0; c < u.size.size(); ++c) { chunks.size.push_back(u.size[c] * CH); chunks.start.push_back(u.start[c] * CH); }
-    } else {
-        chunks.make(nzc, NS);
-    }
+    const unsigned char* tab_x = nullptr;
+    if (T.seg_table(g.sx, &tab_x) != cudaSuccess) return fail(DFFT_ERR_CUDA, "segment table");
+    const HandOver ho = overlapped_hand_over(p, 1, tab_x);
+    const Split chunks = ho.chunks(z_chunk_count(p, 1));
     const size_t NSc = chunks.size.size();
-    const unsigned char *tab_y = nullptr, *tab_x = nullptr;
-    if (T.seg_table(g.oy, &tab_y) != cudaSuccess || T.seg_table(g.sx, &tab_x) != cudaSuccess) return fail(DFFT_ERR_CUDA, "segment table");
 
-    sc.steps.push_back(rendezvous(0, 0, 0));  // everyone has left the previous exec
-    // the auxiliary streams fork from the caller's stream at the start of run_schedule, i.e. BEFORE the
-    // entry rendezvous: make them wait for it explicitly
-    const int ev_entry = nev++;
+    sc.steps.push_back(new_rendezvous(0, 0, nullptr, 0));  // everyone has left the previous exec
+    const int ev_entry = nev++;  // which the auxiliary streams wait for (build_overlapped_forward)
     sc.steps.back().record = ev_entry;
     int rc;
-
-    if (!inverse) {
-        std::vector<int> ev_z(NG), ev_y(NSc);
-        for (size_t gi = 0; gi < NG; ++gi) {
-            Step s;
-            rc = new_pass(c2c ? PASS_C2C_CONTIG : PASS_R2C, c2c ? g.nz : g.nz / 2, c2c ? "z pass" : "z pass (R2C)", s);
-            if (rc) return rc;
-            const size_t pl0 = groups.start[gi], npl = groups.size[gi];
-            const long long pitch = z_row_pitch(p);
-            s.prm.A0 = int(npl); s.prm.A1 = int(ny);
-            s.prm.in = single_view((void*)(size_t)(pl0 * ny * pitch * es), pitch * (long long)ny, pitch, 1);
-            s.in_user = 1;
-            s.prm.out = single_view(eptr(slotp(D1, me), pl0 * ny * nzc, es), (long long)(ny * nzc), (long long)nzc, 1);
-            s.stream = 0;
-            s.record = ev_z[gi] = nev++;
-            sc.steps.push_back(s);
-        }
-        for (size_t c = 0; c < NSc; ++c) {
-            const size_t z0 = chunks.start[c], zc = chunks.size[c];
-            for (size_t gi = 0; gi < NG; ++gi) {
-                Step s;
-                rc = new_pass(PASS_C2C_TILED, ny, "y pass", s);
-                if (rc) return rc;
-                const size_t pl0 = groups.start[gi], npl = groups.size[gi];
-                if (CH) {
-                    s.prm.A0 = int(npl); s.prm.A1 = int(zc / CH); s.prm.B = int(CH);
-                    s.prm.in = single_view(eptr(slotp(D1, me), pl0 * ny * nzc + z0, es), (long long)(ny * nzc), (long long)CH, (long long)nzc);
-                    s.prm.tile_pref = p->xchg_tile_pref;
-                    s.prm.bulk_out = p->bulk_store;
-                    seg_view(s.prm.out, tab_y, G2, [&](int q, int r) {
-                        const size_t nyq = g.oy.size[q];
-                        return mkseg(eptr(slotp(D2, r), ((z0 / CH) * nx + x0 + pl0) * nyq * CH, es), (long long)(nyq * CH), (long long)(nx * nyq * CH),
-                                     (long long)CH, g.oy.start[q]);
-                    });
-                } else {
-                s.prm.A0 = int(npl); s.prm.A1 = 1; s.prm.B = int(zc);
-                s.prm.tile_pref = p->xchg_tile_pref;
-                s.prm.in = single_view(eptr(slotp(D1, me), pl0 * ny * nzc + z0, es), (long long)(ny * nzc), 0, (long long)nzc);
-                seg_view(s.prm.out, tab_y, G2, [&](int q, int r) {
-                    const size_t nyq = g.oy.size[q];
-                    return mkseg(eptr(slotp(D2, r), (x0 + pl0) * nyq * nzc + z0, es), (long long)(nyq * nzc), 0, (long long)nzc, g.oy.start[q]);
-                });
-                }
-                s.prm.max_ctas = exchange_ctas(p, inverse);
-                s.stream = 1;
-                if (c == 0) s.waits.push_back(ev_z[gi]);
-                if (c == 0 && gi == 0) s.waits.push_back(ev_entry);
-                const bool tail_here = CH && rem && c + 1 == NSc;
-                if (gi + 1 == NG && !tail_here) s.record = ev_y[c] = nev++;
-                sc.steps.push_back(s);
-                if (tail_here) {
-                    Step t = s;
-                    t.label = "y pass (tail)";
-                    t.prm.bulk_out = 0;
-                    t.waits.clear();
-                    t.record = -1;
-                    t.prm.A0 = int(npl); t.prm.A1 = 1; t.prm.B = int(rem);
-                    t.prm.in = single_view(eptr(slotp(D1, me), pl0 * ny * nzc + nzm, es), (long long)(ny * nzc), 0, (long long)nzc);
-                    seg_view(t.prm.out, tab_y, G2, [&](int q, int r) {
-                        const size_t nyq = g.oy.size[q];
-                        return mkseg(eptr(slotp(D2, r), nx * nyq * nzm + (x0 + pl0) * nyq * rem, es), (long long)(nyq * rem), 0, (long long)rem, g.oy.start[q]);
-                    });
-                    if (gi + 1 == NG) t.record = ev_y[c] = nev++;
-                    sc.steps.push_back(t);
-                }
-            }
-        }
-        for (size_t c = 0; c < NSc; ++c) {
-            const size_t z0 = chunks.start[c], zc = chunks.size[c];
-            Step r = rendezvous(2, 2, 2);
-            r.waits.push_back(ev_y[c]);
-            sc.steps.push_back(r);
-            Step s;
-            rc = new_pass(PASS_C2C_TILED, nx, "x pass", s);
-            if (rc) return rc;
-            if (CH) {
-                // in: [nzc/CH][nx][oy_me][CH]; a0 = y_loc, a1 = z chunk within this z range, n = x
-                s.prm.A0 = int(oy_me); s.prm.A1 = int(zc / CH); s.prm.B = int(CH);
-                s.prm.in = single_view(eptr(slotp(D2, me), (z0 / CH) * nx * oy_me * CH, es), (long long)CH, (long long)(nx * oy_me * CH), (long long)(oy_me * CH));
-                s.prm.out = single_view((void*)(size_t)(z0 * es), (long long)nzc, (long long)CH, (long long)(oy_me * nzc));
-                s.prm.tile_swz = p->x_swz;
-            } else {
+    std::vector<int> ev_x(NSc), ev_yi(NSc);
+    const View in = single_view(nullptr, (long long)nzc, 0, (long long)(oy_me * nzc));
+    for (size_t c = 0; c < NSc; ++c) {
+        const size_t z0 = chunks.start[c], zc = chunks.size[c];
+        Step s;
+        rc = new_pass(p, 1, PASS_C2C_TILED, g.nx, 0, nullptr, s);
+        if (rc) return rc;
+        s.label = "x pass";
+        s.in_user = 1;
+        if (ho.CH) {
+            s.prm.bulk_out = p->bulk_store;
+            ho.scatter(s, in, oy0_me, oy_me, z0, zc);
+        } else {
             s.prm.A0 = 1; s.prm.A1 = int(oy_me); s.prm.B = int(zc);
-            s.prm.in = single_view(eptr(slotp(D2, me), z0, es), 0, (long long)nzc, (long long)(oy_me * nzc));
-            s.prm.out = single_view((void*)(size_t)(z0 * es), 0, (long long)nzc, (long long)(oy_me * nzc));
-            }
-            s.out_user = 2;
-            s.stream = 2;
-            sc.steps.push_back(s);
-            if (CH && rem && c + 1 == NSc) {
-                Step t = s;
-                t.label = "x pass (tail)";
-                t.prm.A0 = int(oy_me); t.prm.A1 = 1; t.prm.B = int(rem);
-                t.prm.in = single_view(eptr(slotp(D2, me), nx * oy_me * nzm, es), (long long)rem, 0, (long long)(oy_me * rem));
-                t.prm.out = single_view((void*)(size_t)(nzm * es), (long long)nzc, 0, (long long)(oy_me * nzc));
-                sc.steps.push_back(t);
-            }
+            s.prm.in = single_view((void*)(size_t)(z0 * es), 0, (long long)nzc, (long long)(oy_me * nzc));
+            // dest q holds [nx_q][ny][nzc]; my rows y in [oy0_me, +oy_me)
+            seg_view(s.prm.out, tab_x, G2, [&](int q, int r) {
+                return mkseg(eptr(slotp(D2, r), oy0_me * nzc + z0, es), 0, (long long)nzc, (long long)(ny * nzc), g.sx.start[q]);
+            });
         }
-    } else {
-        std::vector<int> ev_x(NSc), ev_yi(NSc);
-        for (size_t c = 0; c < NSc; ++c) {
-            const size_t z0 = chunks.start[c], zc = chunks.size[c];
-            Step s;
-            rc = new_pass(PASS_C2C_TILED, nx, "x pass", s);
-            if (rc) return rc;
-            s.in_user = 1;
-            if (CH) {
-                // dest q holds [nzc/CH][ny][nx_q][CH]: the rows a tile sends to one destination (consecutive x) are adjacent
-                s.prm.A0 = int(oy_me); s.prm.A1 = int(zc / CH); s.prm.B = int(CH);
-                s.prm.in = single_view((void*)(size_t)(z0 * es), (long long)nzc, (long long)CH, (long long)(oy_me * nzc));
-                s.prm.bulk_out = p->bulk_store;
-                seg_view(s.prm.out, tab_x, G2, [&](int q, int r) {
-                    const size_t nxq = g.sx.size[q];
-                    return mkseg(eptr(slotp(D2, r), ((z0 / CH) * ny + oy0_me) * nxq * CH, es), (long long)(nxq * CH), (long long)(ny * nxq * CH), (long long)CH,
-                                 g.sx.start[q]);
-                });
-            } else {
-                s.prm.A0 = 1; s.prm.A1 = int(oy_me); s.prm.B = int(zc);
-                s.prm.in = single_view((void*)(size_t)(z0 * es), 0, (long long)nzc, (long long)(oy_me * nzc));
-                // dest q holds [nx_q][ny][nzc]; my rows y in [oy0_me, +oy_me)
-                seg_view(s.prm.out, tab_x, G2, [&](int q, int r) {
-                    return mkseg(eptr(slotp(D2, r), oy0_me * nzc + z0, es), 0, (long long)nzc, (long long)(ny * nzc), g.sx.start[q]);
-                });
-            }
-            s.prm.max_ctas = exchange_ctas(p, inverse);
-            s.prm.tile_pref = p->xchg_tile_pref;
-            s.stream = 1;
-            if (c == 0) s.waits.push_back(ev_entry);
-            const bool tail_here = CH && rem && c + 1 == NSc;
-            if (!tail_here) s.record = ev_x[c] = nev++;
+        s.prm.max_ctas = exchange_ctas(p, 1);
+        s.prm.tile_pref = p->xchg_tile_pref;
+        s.stream = 1;
+        if (c == 0) s.waits.push_back(ev_entry);
+        const bool tail_here = ho.any_rem && c + 1 == NSc;
+        if (!tail_here) s.record = ev_x[c] = nev++;
+        sc.steps.push_back(s);
+        if (tail_here) {
+            Step t = ho.scatter_tail(s, in, oy0_me);
+            t.record = ev_x[c] = nev++;
+            sc.steps.push_back(t);
+        }
+    }
+    const View out = single_view(slotp(D1, me), (long long)(ny * nzc), 0, (long long)nzc);
+    for (size_t c = 0; c < NSc; ++c) {
+        const size_t z0 = chunks.start[c], zc = chunks.size[c];
+        Step r = new_rendezvous(2, 2, nullptr, 2);
+        r.waits.push_back(ev_x[c]);
+        sc.steps.push_back(r);
+        Step s;
+        rc = new_pass(p, 1, PASS_C2C_TILED, ny, 1, nullptr, s);
+        if (rc) return rc;
+        s.label = "y pass";
+        s.stream = 2;
+        if (ho.CH) {
+            s.prm.tile_pref = 1;
+            ho.gather(s, out, 0, nx_p, z0, zc);
+            const bool tail_here = ho.any_rem && c + 1 == NSc;
+            if (!tail_here) s.record = ev_yi[c] = nev++;
             sc.steps.push_back(s);
             if (tail_here) {
-                Step t = s;
-                t.label = "x pass (tail)";
-                t.prm.bulk_out = 0;
-                t.waits.clear();
-                t.prm.A0 = int(oy_me); t.prm.A1 = 1; t.prm.B = int(rem);
-                t.prm.in = single_view((void*)(size_t)(nzm * es), (long long)nzc, 0, (long long)(oy_me * nzc));
-                seg_view(t.prm.out, tab_x, G2, [&](int q, int r) {
-                    const size_t nxq = g.sx.size[q];
-                    return mkseg(eptr(slotp(D2, r), ny * nxq * nzm + oy0_me * rem, es), (long long)rem, 0, (long long)(ny * rem), g.sx.start[q]);
-                });
-                t.record = ev_x[c] = nev++;
+                Step t = ho.gather_tail(s, out, 0);
+                t.record = ev_yi[c] = nev++;
                 sc.steps.push_back(t);
             }
+        } else {
+            s.prm.A0 = int(nx_p); s.prm.A1 = 1; s.prm.B = int(zc);
+            s.prm.in = single_view(eptr(slotp(D2, me), z0, es), (long long)(ny * nzc), 0, (long long)nzc);
+            s.prm.out = s.prm.in;  // in place
+            s.record = ev_yi[c] = nev++;
+            sc.steps.push_back(s);
         }
-        for (size_t c = 0; c < NSc; ++c) {
-            const size_t z0 = chunks.start[c], zc = chunks.size[c];
-            Step r = rendezvous(2, 2, 2);
-            r.waits.push_back(ev_x[c]);
-            sc.steps.push_back(r);
-            Step s;
-            rc = new_pass(PASS_C2C_TILED, ny, "y pass", s);
-            if (rc) return rc;
-            s.stream = 2;
-            if (CH) {
-                s.prm.A0 = int(nx_p); s.prm.A1 = int(zc / CH); s.prm.B = int(CH);
-                s.prm.tile_pref = 1;
-                s.prm.in = single_view(eptr(slotp(D2, me), (z0 / CH) * ny * nx_p * CH, es), (long long)CH, (long long)(ny * nx_p * CH), (long long)(nx_p * CH));
-                s.prm.out = single_view(eptr(slotp(D1, me), z0, es), (long long)(ny * nzc), (long long)CH, (long long)nzc);
-                const bool tail_here = rem && c + 1 == NSc;
-                if (!tail_here) s.record = ev_yi[c] = nev++;
-                sc.steps.push_back(s);
-                if (tail_here) {
-                    Step t = s;
-                    t.label = "y pass (tail)";
-                    t.prm.A0 = int(nx_p); t.prm.A1 = 1; t.prm.B = int(rem);
-                    t.prm.in = single_view(eptr(slotp(D2, me), ny * nx_p * nzm, es), (long long)(ny * rem), 0, (long long)rem);
-                    t.prm.out = single_view(eptr(slotp(D1, me), nzm, es), (long long)(ny * nzc), 0, (long long)nzc);
-                    t.record = ev_yi[c] = nev++;
-                    sc.steps.push_back(t);
-                }
-            } else {
-                s.prm.A0 = int(nx_p); s.prm.A1 = 1; s.prm.B = int(zc);
-                s.prm.in = single_view(eptr(slotp(D2, me), z0, es), (long long)(ny * nzc), 0, (long long)nzc);
-                s.prm.out = s.prm.in;  // in place
-                s.record = ev_yi[c] = nev++;
-                sc.steps.push_back(s);
-            }
-        }
-        Step s;
-        const PassKind zkind = c2c ? PASS_C2C_CONTIG : PASS_C2R;
-        const long long zpitch = z_row_pitch(p);
-        rc = new_pass(zkind, c2c ? g.nz : g.nz / 2, c2c ? "z pass" : "z pass (C2R)", s);
-        if (rc) return rc;
-        s.prm.A0 = int(nx_p); s.prm.A1 = int(ny);
-        s.prm.in = single_view(slotp(CH ? D1 : D2, me), (long long)(ny * nzc), (long long)nzc, 1);
-        s.prm.out = single_view(nullptr, zpitch * (long long)ny, zpitch, 1);
-        s.out_user = 2;
-        s.stream = 0;
-        for (size_t c = 0; c < NSc; ++c) s.waits.push_back(ev_yi[c]);
-        sc.steps.push_back(s);
     }
+    Step s;
+    const long long zpitch = z_row_pitch(p);
+    rc = new_pass(p, 1, c2c ? PASS_C2C_CONTIG : PASS_C2R, c2c ? g.nz : g.nz / 2, 2, nullptr, s);
+    if (rc) return rc;
+    s.prm.A0 = int(nx_p); s.prm.A1 = int(ny);
+    s.prm.in = single_view(slotp(ho.CH ? D1 : D2, me), (long long)(ny * nzc), (long long)nzc, 1);
+    s.prm.out = single_view(nullptr, zpitch * (long long)ny, zpitch, 1);
+    s.out_user = 2;
+    for (size_t c = 0; c < NSc; ++c) s.waits.push_back(ev_yi[c]);
+    sc.steps.push_back(s);
     sc.nevents = nev;
     sc.built = true;
     return DFFT_SUCCESS;
@@ -1547,14 +1588,15 @@ static int pencil_overlap_mode() {
 }
 static bool pencil_overlap_enabled() { return pencil_overlap_mode() != 0; }
 
-// inverse half of build_overlapped_pencil (see the comment there); NG plane groups, the same on every rank
-static int build_overlapped_pencil_inverse(dfft_plan_s* p, Schedule& sc, size_t NG) {
+static int build_overlapped_pencil_inverse(dfft_plan_s* p, Schedule& sc) {
     const Geometry& g = p->g;
     const int me = p->rank;
     const int pi = g.pi(me), pj = g.pj(me);
     const size_t es = p->esize;
     const bool c2c = g.transform == DFFT_C2C;
     Tables& T = p->tabs;
+    sc.steps.clear();
+    sc.overlapped = true;
     const size_t ny = g.ny, nx = g.nx, nzc = g.nzc;
     const size_t nx_i = g.sx.size[pi];
     const size_t ny_j = g.sy.size[pj];
@@ -1565,74 +1607,29 @@ static int build_overlapped_pencil_inverse(dfft_plan_s* p, Schedule& sc, size_t 
     const int D1 = 0, D2 = 1;
     auto slotp = [&](int s_, int r) -> void* { return p->slot_ptr[s_][r]; };
     int nev = 0;
-    auto new_pass = [&](PassKind kind, size_t n, const char* label, Step& s) -> int {
-        s = Step();
-        s.type = STEP_PASS;
-        s.kind = kind;
-        s.label = label;
-        s.log2n = ilog2_exact(n);
-        if (s.log2n < 1 || s.log2n > MAX_LOG2N) return fail(DFFT_ERR_UNSUPPORTED, "unsupported axis length");
-        s.prm.A0 = 1; s.prm.A1 = 1; s.prm.B = 1;
-        s.prm.inverse = 1;
-        void* tw = nullptr;
-        if (T.get_tw(s.log2n, &tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
-        s.prm.tw = tw;
-        if (kind == PASS_C2R) {
-            void* tw2 = nullptr;
-            if (T.get_tw2(s.log2n, &tw2) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
-            s.prm.tw2 = tw2;
-        }
-        return DFFT_SUCCESS;
-    };
-    auto rendezvous = [&](int group, int stream) {
-        Step s;
-        s.type = STEP_RENDEZVOUS;
-        s.label = group == 0 ? "entry rendezvous" : (group == 1 ? "rendezvous 1" : "rendezvous 2");
-        s.group = group;
-        s.phase_id = group;
-        s.stream = stream;
-        return s;
-    };
+    const size_t NG = plane_groups(p, 1);
     Split groups;
     groups.make(nx_i, NG);
-    // hand-over of the x -> y transposition: blocked [nz_j/CH][ny][nx_q][CH] + plain tail [nx_q][ny][rem] (build_schedule)
-    const size_t CH = p->blocked_inv ? size_t(p->blocked_ch) : 0;
-    const size_t rem = CH ? nz_j % CH : 0, nzm = nz_j - rem;
-    bool any_rem = false;  // ranks without leftover columns run the tail steps as empty passes: same step list everywhere
-    if (CH) for (size_t v : g.sz.size) any_rem = any_rem || (v % CH != 0);
     const unsigned char *tab_x = nullptr, *tab_y_in = nullptr;
     if (T.seg_table(g.sx, &tab_x) != cudaSuccess || T.seg_table(g.sy, &tab_y_in) != cudaSuccess) return fail(DFFT_ERR_CUDA, "segment table");
+    const HandOver ho = overlapped_hand_over(p, 1, tab_x);
     int rc;
 
-    sc.steps.push_back(rendezvous(0, 0));  // everyone has left the previous exec
+    sc.steps.push_back(new_rendezvous(0, 0, nullptr, 0));  // everyone has left the previous exec
     // x pass on the caller's [nx][oy_i][nz_j], whole, uncapped: nothing local can run beside it yet
     {
         Step s;
-        rc = new_pass(PASS_C2C_TILED, nx, "x pass", s);
+        rc = new_pass(p, 1, PASS_C2C_TILED, nx, 0, nullptr, s);
         if (rc) return rc;
+        s.label = "x pass";
         s.in_user = 1;
         s.prm.tile_pref = G2.size() > 1 ? p->xchg_tile_pref : 1;
-        if (CH) {
-            s.prm.A0 = int(oy_i); s.prm.A1 = int(nzm / CH); s.prm.B = int(CH);
-            s.prm.in = single_view(nullptr, (long long)nz_j, (long long)CH, (long long)(oy_i * nz_j));
+        if (ho.CH) {
             s.prm.bulk_out = G2.size() > 1 ? p->bulk_store : 0;
-            seg_view(s.prm.out, tab_x, G2, [&](int q, int r) {
-                const size_t nxq = g.sx.size[q];
-                return mkseg(eptr(slotp(D2, r), oy0_i * nxq * CH, es), (long long)(nxq * CH), (long long)(ny * nxq * CH), (long long)CH, g.sx.start[q]);
-            });
+            const View in = single_view(nullptr, (long long)nz_j, 0, (long long)(oy_i * nz_j));
+            ho.scatter(s, in, oy0_i, oy_i, 0, ho.nzm);
             sc.steps.push_back(s);
-            if (any_rem) {
-                Step t = s;
-                t.label = "x pass (tail)";
-                t.prm.bulk_out = 0;
-                t.prm.A0 = int(oy_i); t.prm.A1 = 1; t.prm.B = int(rem);
-                t.prm.in = single_view((void*)(size_t)(nzm * es), (long long)nz_j, 0, (long long)(oy_i * nz_j));
-                seg_view(t.prm.out, tab_x, G2, [&](int q, int r) {
-                    const size_t nxq = g.sx.size[q];
-                    return mkseg(eptr(slotp(D2, r), ny * nxq * nzm + oy0_i * rem, es), (long long)rem, 0, (long long)(ny * rem), g.sx.start[q]);
-                });
-                sc.steps.push_back(t);
-            }
+            if (ho.any_rem) sc.steps.push_back(ho.scatter_tail(s, in, oy0_i));
         } else {
             s.prm.A0 = 1; s.prm.A1 = 1; s.prm.B = int(oy_i * nz_j);
             s.prm.in = single_view(nullptr, 0, 0, (long long)(oy_i * nz_j));
@@ -1643,49 +1640,39 @@ static int build_overlapped_pencil_inverse(dfft_plan_s* p, Schedule& sc, size_t 
             sc.steps.push_back(s);
         }
     }
-    sc.steps.push_back(rendezvous(2, 0));  // all column peers have delivered their rows
+    sc.steps.push_back(new_rendezvous(2, 2, nullptr, 0));  // all column peers have delivered their rows
     const int ev_x = nev++;
     sc.steps.back().record = ev_x;
     std::vector<int> ev_y(NG);
     for (size_t gi = 0; gi < NG; ++gi) {
         const size_t pl0 = groups.start[gi], npl = groups.size[gi];
         Step s;
-        rc = new_pass(PASS_C2C_TILED, ny, "y pass", s);
+        rc = new_pass(p, 1, PASS_C2C_TILED, ny, 1, nullptr, s);
         if (rc) return rc;
+        s.label = "y pass";
         s.stream = 1;
         if (gi == 0) s.waits.push_back(ev_x);
         s.prm.max_ctas = exchange_ctas(p, 1);
         s.prm.tile_pref = G1.size() > 1 ? p->xchg_tile_pref : 1;
-        if (CH) {
-            // in = my slot, blocked [nz_j/CH][ny][nx_i][CH]; tile = (x_loc, z block); dest (i, q) holds [nx_i][ny_q][nzc]
-            s.prm.A0 = int(npl); s.prm.A1 = int(nzm / CH); s.prm.B = int(CH);
-            s.prm.in = single_view(eptr(slotp(D2, me), pl0 * CH, es), (long long)CH, (long long)(ny * nx_i * CH), (long long)(nx_i * CH));
-            seg_view(s.prm.out, tab_y_in, G1, [&](int q, int r) {
-                const size_t nyq = g.sy.size[q];
-                return mkseg(eptr(slotp(D1, r), pl0 * nyq * nzc + z0_j, es), (long long)(nyq * nzc), (long long)CH, (long long)nzc, g.sy.start[q]);
-            });
-            if (!any_rem) s.record = ev_y[gi] = nev++;
+        // dest (i, q) holds [nx_i][ny_q][nzc]; my columns z in [z0_j, +nz_j)
+        View out{};
+        seg_view(out, tab_y_in, G1, [&](int q, int r) {
+            const size_t nyq = g.sy.size[q];
+            return mkseg(eptr(slotp(D1, r), pl0 * nyq * nzc + z0_j, es), (long long)(nyq * nzc), 0, (long long)nzc, g.sy.start[q]);
+        });
+        if (ho.CH) {
+            ho.gather(s, out, pl0, npl, 0, ho.nzm);
+            if (!ho.any_rem) s.record = ev_y[gi] = nev++;
             sc.steps.push_back(s);
-            if (any_rem) {
-                Step t = s;
-                t.label = "y pass (tail)";
-                t.waits.clear();
-                t.prm.A0 = int(npl); t.prm.A1 = 1; t.prm.B = int(rem);
-                t.prm.in = single_view(eptr(slotp(D2, me), ny * nx_i * nzm + pl0 * ny * rem, es), (long long)(ny * rem), 0, (long long)rem);
-                seg_view(t.prm.out, tab_y_in, G1, [&](int q, int r) {
-                    const size_t nyq = g.sy.size[q];
-                    return mkseg(eptr(slotp(D1, r), pl0 * nyq * nzc + z0_j + nzm, es), (long long)(nyq * nzc), 0, (long long)nzc, g.sy.start[q]);
-                });
+            if (ho.any_rem) {
+                Step t = ho.gather_tail(s, out, pl0);
                 t.record = ev_y[gi] = nev++;
                 sc.steps.push_back(t);
             }
         } else {
             s.prm.A0 = int(npl); s.prm.A1 = 1; s.prm.B = int(nz_j);
             s.prm.in = single_view(eptr(slotp(D2, me), pl0 * ny * nz_j, es), (long long)(ny * nz_j), 0, (long long)nz_j);
-            seg_view(s.prm.out, tab_y_in, G1, [&](int q, int r) {
-                const size_t nyq = g.sy.size[q];
-                return mkseg(eptr(slotp(D1, r), pl0 * nyq * nzc + z0_j, es), (long long)(nyq * nzc), 0, (long long)nzc, g.sy.start[q]);
-            });
+            s.prm.out = out;
             s.record = ev_y[gi] = nev++;
             sc.steps.push_back(s);
         }
@@ -1694,11 +1681,11 @@ static int build_overlapped_pencil_inverse(dfft_plan_s* p, Schedule& sc, size_t 
     const long long zpitch = z_row_pitch(p);  // output line pitch in complex units
     for (size_t gi = 0; gi < NG; ++gi) {
         const size_t pl0 = groups.start[gi], npl = groups.size[gi];
-        Step r = rendezvous(1, 2);  // all row peers have delivered plane group gi
+        Step r = new_rendezvous(1, 1, nullptr, 2);  // all row peers have delivered plane group gi
         r.waits.push_back(ev_y[gi]);
         sc.steps.push_back(r);
         Step s;
-        rc = new_pass(zkind, c2c ? g.nz : g.nz / 2, c2c ? "z pass" : "z pass (C2R)", s);
+        rc = new_pass(p, 1, zkind, c2c ? g.nz : g.nz / 2, 2, nullptr, s);
         if (rc) return rc;
         s.prm.A0 = int(npl); s.prm.A1 = int(ny_j);
         s.prm.in = single_view(eptr(slotp(D1, me), pl0 * ny_j * nzc, es), (long long)(ny_j * nzc), (long long)nzc, 1);
@@ -1712,205 +1699,7 @@ static int build_overlapped_pencil_inverse(dfft_plan_s* p, Schedule& sc, size_t 
     return DFFT_SUCCESS;
 }
 
-// Overlapped pencil schedules, Peer2Peer on both transpositions (send_method Streams).  Forward:
-//   stream 0: z pass per plane group, scattering along z into the row peers' slot A            (NVLink-bound)
-//   stream 1: per plane group: meet the row peers; then the y pass per (plane group, z chunk), persistent on
-//             `xchg_ctas` CTAs, scattering along y into the column peers' slot B                 (NVLink-bound)
-//   stream 2: per z chunk: meet the column peers, x pass of that chunk                           (HBM-bound)
-// Only the x pass can hide behind an exchange (both scatters share the NVLink ports).  The inverse mirrors it — again
-// only the local pass, now the z pass, can hide:
-//   stream 0: x pass, scattering along x into the column peers' slot B; meet the column peers   (NVLink-bound)
-//   stream 1: y pass per plane group on a capped grid, scattering along y into the row peers' slot A  (NVLink-bound)
-//   stream 2: per plane group: meet the row peers, z pass of that group into the caller's buffer  (HBM-bound)
-static int build_overlapped_pencil(dfft_plan_s* p, int inverse, Schedule& sc) {
-    const Geometry& g = p->g;
-    const int me = p->rank;
-    const int pi = g.pi(me), pj = g.pj(me);
-    const size_t es = p->esize;
-    const bool c2c = g.transform == DFFT_C2C;
-    Tables& T = p->tabs;
-    sc.steps.clear();
-    sc.overlapped = true;
-    const size_t ny = g.ny, nx = g.nx;
-    const size_t nx_i = g.sx.size[pi], x0_i = g.sx.start[pi];
-    const size_t ny_j = g.sy.size[pj], y0_j = g.sy.start[pj];
-    const size_t nz_j = g.sz.size[pj];
-    const size_t oy_i = g.oy.size[pi];
-    const std::vector<int>& G1 = p->grp[1];
-    const std::vector<int>& G2 = p->grp[2];
-    const int D1 = 0, D2 = 1;
-    auto slotp = [&](int s_, int r) -> void* { return p->slot_ptr[s_][r]; };
-    int nev = 0;
-
-    auto new_pass = [&](PassKind kind, size_t n, const char* label, Step& s) -> int {
-        s = Step();
-        s.type = STEP_PASS;
-        s.kind = kind;
-        s.label = label;
-        s.log2n = ilog2_exact(n);
-        if (s.log2n < 1 || s.log2n > MAX_LOG2N) return fail(DFFT_ERR_UNSUPPORTED, "unsupported axis length");
-        s.prm.A0 = 1; s.prm.A1 = 1; s.prm.B = 1;
-        s.prm.inverse = inverse;
-        void* tw = nullptr;
-        if (T.get_tw(s.log2n, &tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
-        s.prm.tw = tw;
-        if (kind == PASS_R2C || kind == PASS_C2R) {
-            void* tw2 = nullptr;
-            if (T.get_tw2(s.log2n, &tw2) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
-            s.prm.tw2 = tw2;
-        }
-        return DFFT_SUCCESS;
-    };
-    auto rendezvous = [&](int group, int stream) {
-        Step s;
-        s.type = STEP_RENDEZVOUS;
-        s.label = group == 0 ? "entry rendezvous" : (group == 1 ? "rendezvous 1" : "rendezvous 2");
-        s.group = group;
-        s.phase_id = group;
-        s.stream = stream;
-        return s;
-    };
-
-    // every rank must build the same number of steps: derive the group / chunk counts from global minima
-    size_t min_nx = nx, min_nz = g.nzc;
-    for (size_t v : g.sx.size) min_nx = std::min(min_nx, v);
-    for (size_t v : g.sz.size) min_nz = std::min(min_nz, v);
-    const size_t NG = std::min<size_t>(size_t(inverse && p->tuned_groups_inv > 0 ? p->tuned_groups_inv : p->ovl_groups), min_nx);
-    if (inverse) return build_overlapped_pencil_inverse(p, sc, NG);
-    const size_t want_chunks = size_t(p->tuned_chunks[0] > 0 ? p->tuned_chunks[0] : p->ovl_chunks);
-    const size_t NS = min_nz >= 32 * want_chunks ? want_chunks : (min_nz >= 32 ? 2 : 1);
-    Split groups, chunks;
-    groups.make(nx_i, NG);
-    // blocked hand-over of the second transposition: receiver (q, j) holds [nz_j/CH][nx][ny_q][CH] (+ a plain-layout
-    // tail of nz_j % CH columns), see build_schedule
-    const size_t CH = size_t(p->blocked_ch);
-    const size_t rem = CH ? nz_j % CH : 0, nzm = nz_j - rem;
-    bool any_rem = false;  // ranks without leftover columns run the tail steps as empty passes: same step list everywhere
-    if (CH) for (size_t v : g.sz.size) any_rem = any_rem || (v % CH != 0);
-    if (CH) {
-        Split u;
-        u.make(nzm / CH, std::min<size_t>(NS, nzm / CH));
-        if (u.size.size() != NS) return fail(DFFT_ERR_STATE, "internal: blocked z chunks");
-        chunks.size.clear(); chunks.start.clear();
-        for (size_t c = 0; c < u.size.size(); ++c) { chunks.size.push_back(u.size[c] * CH); chunks.start.push_back(u.start[c] * CH); }
-    } else {
-        chunks.make(nz_j, NS);
-    }
-    const unsigned char *tab_z = nullptr, *tab_y = nullptr;
-    if (T.seg_table(g.sz, &tab_z) != cudaSuccess || T.seg_table(g.oy, &tab_y) != cudaSuccess) return fail(DFFT_ERR_CUDA, "segment table");
-
-    sc.steps.push_back(rendezvous(0, 0));
-    const int ev_entry = nev++;
-    sc.steps.back().record = ev_entry;
-    int rc;
-    std::vector<int> ev_z(NG), ev_y(NS);
-    for (size_t gi = 0; gi < NG; ++gi) {
-        Step s;
-        rc = new_pass(c2c ? PASS_C2C_CONTIG : PASS_R2C, c2c ? g.nz : g.nz / 2, c2c ? "z pass" : "z pass (R2C)", s);
-        if (rc) return rc;
-        const size_t pl0 = groups.start[gi], npl = groups.size[gi];
-        const long long pitch = z_row_pitch(p);
-        s.prm.A0 = int(npl); s.prm.A1 = int(ny_j);
-        s.prm.in = single_view((void*)(size_t)(pl0 * ny_j * pitch * es), pitch * (long long)ny_j, pitch, 1);
-        s.in_user = 1;
-        seg_view(s.prm.out, tab_z, G1, [&](int q, int r) {
-            const size_t nzq = g.sz.size[q];
-            return mkseg(eptr(slotp(D1, r), (pl0 * ny + y0_j) * nzq, es), (long long)(ny * nzq), (long long)nzq, 1, g.sz.start[q]);
-        });
-        s.stream = 0;
-        s.record = ev_z[gi] = nev++;
-        sc.steps.push_back(s);
-    }
-    for (size_t c = 0; c < NS; ++c) {
-        const size_t z0 = chunks.start[c], zc = chunks.size[c];
-        for (size_t gi = 0; gi < NG; ++gi) {
-            const size_t pl0 = groups.start[gi], npl = groups.size[gi];
-            if (c == 0) {
-                Step r = rendezvous(1, 1);  // all row peers have delivered plane group gi
-                r.waits.push_back(ev_z[gi]);
-                if (gi == 0) r.waits.push_back(ev_entry);
-                sc.steps.push_back(r);
-            }
-            Step s;
-            rc = new_pass(PASS_C2C_TILED, ny, "y pass", s);
-            if (rc) return rc;
-            if (CH) {
-                s.prm.A0 = int(npl); s.prm.A1 = int(zc / CH); s.prm.B = int(CH);
-                s.prm.in = single_view(eptr(slotp(D1, me), pl0 * ny * nz_j + z0, es), (long long)(ny * nz_j), (long long)CH, (long long)nz_j);
-                s.prm.bulk_out = G2.size() > 1 ? p->bulk_store : 0;
-                seg_view(s.prm.out, tab_y, G2, [&](int q, int r) {
-                    const size_t nyq = g.oy.size[q];
-                    return mkseg(eptr(slotp(D2, r), ((z0 / CH) * nx + x0_i + pl0) * nyq * CH, es), (long long)(nyq * CH), (long long)(nx * nyq * CH),
-                                 (long long)CH, g.oy.start[q]);
-                });
-            } else {
-                s.prm.A0 = int(npl); s.prm.A1 = 1; s.prm.B = int(zc);
-                s.prm.in = single_view(eptr(slotp(D1, me), pl0 * ny * nz_j + z0, es), (long long)(ny * nz_j), 0, (long long)nz_j);
-                seg_view(s.prm.out, tab_y, G2, [&](int q, int r) {
-                    const size_t nyq = g.oy.size[q];
-                    return mkseg(eptr(slotp(D2, r), (x0_i + pl0) * nyq * nz_j + z0, es), (long long)(nyq * nz_j), 0, (long long)nz_j, g.oy.start[q]);
-                });
-            }
-            s.prm.max_ctas = exchange_ctas(p, 0);
-            s.prm.tile_pref = G2.size() > 1 ? p->xchg_tile_pref : 0;
-            s.stream = 1;
-            const bool tail_here = CH && any_rem && c + 1 == NS;
-            if (gi + 1 == NG && !tail_here) s.record = ev_y[c] = nev++;
-            sc.steps.push_back(s);
-            if (tail_here) {
-                Step t = s;
-                t.label = "y pass (tail)";
-                t.prm.bulk_out = 0;
-                t.waits.clear();
-                t.record = -1;
-                t.prm.A0 = int(npl); t.prm.A1 = 1; t.prm.B = int(rem);
-                t.prm.in = single_view(eptr(slotp(D1, me), pl0 * ny * nz_j + nzm, es), (long long)(ny * nz_j), 0, (long long)nz_j);
-                seg_view(t.prm.out, tab_y, G2, [&](int q, int r) {
-                    const size_t nyq = g.oy.size[q];
-                    return mkseg(eptr(slotp(D2, r), nx * nyq * nzm + (x0_i + pl0) * nyq * rem, es), (long long)(nyq * rem), 0, (long long)rem, g.oy.start[q]);
-                });
-                if (gi + 1 == NG) t.record = ev_y[c] = nev++;
-                sc.steps.push_back(t);
-            }
-        }
-    }
-    for (size_t c = 0; c < NS; ++c) {
-        const size_t z0 = chunks.start[c], zc = chunks.size[c];
-        Step r = rendezvous(2, 2);
-        r.waits.push_back(ev_y[c]);
-        sc.steps.push_back(r);
-        Step s;
-        rc = new_pass(PASS_C2C_TILED, nx, "x pass", s);
-        if (rc) return rc;
-        if (CH) {
-            s.prm.A0 = int(oy_i); s.prm.A1 = int(zc / CH); s.prm.B = int(CH);
-            s.prm.in = single_view(eptr(slotp(D2, me), (z0 / CH) * nx * oy_i * CH, es), (long long)CH, (long long)(nx * oy_i * CH), (long long)(oy_i * CH));
-            s.prm.out = single_view((void*)(size_t)(z0 * es), (long long)nz_j, (long long)CH, (long long)(oy_i * nz_j));
-            s.prm.tile_swz = p->x_swz;
-        } else {
-            s.prm.A0 = 1; s.prm.A1 = int(oy_i); s.prm.B = int(zc);
-            s.prm.in = single_view(eptr(slotp(D2, me), z0, es), 0, (long long)nz_j, (long long)(oy_i * nz_j));
-            s.prm.out = single_view((void*)(size_t)(z0 * es), 0, (long long)nz_j, (long long)(oy_i * nz_j));
-        }
-        s.out_user = 2;
-        s.stream = 2;
-        sc.steps.push_back(s);
-        if (CH && any_rem && c + 1 == NS) {
-            Step t = s;
-            t.label = "x pass (tail)";
-            t.prm.A0 = int(oy_i); t.prm.A1 = 1; t.prm.B = int(rem);
-            t.prm.in = single_view(eptr(slotp(D2, me), nx * oy_i * nzm, es), (long long)rem, 0, (long long)(oy_i * rem));
-            t.prm.out = single_view((void*)(size_t)(nzm * es), (long long)nz_j, 0, (long long)(oy_i * nz_j));
-            sc.steps.push_back(t);
-        }
-    }
-    sc.nevents = nev;
-    sc.built = true;
-    return DFFT_SUCCESS;
-}
-
 }  // namespace dfft
-
 
 // =====================================================================================================
 // memory / peer mapping
@@ -2423,8 +2212,10 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
         const int db = p->P == 1 && !p->taxes[0] && d == 3 ? 2 : d;
         int rc;
         if (batch_small(p, d)) rc = build_batch_small(p, inverse ? 1 : 0, sc);
-        else if (want_overlap) rc = build_overlapped_slab(p, inverse ? 1 : 0, sc);
-        else if (want_pencil_overlap) rc = build_overlapped_pencil(p, inverse ? 1 : 0, sc);
+        // the overlapped slab and pencil schedules share their forward builder; their inverses run different pipelines
+        else if ((want_overlap || want_pencil_overlap) && !inverse) rc = build_overlapped_forward(p, sc);
+        else if (want_overlap) rc = build_overlapped_slab_inverse(p, sc);
+        else if (want_pencil_overlap) rc = build_overlapped_pencil_inverse(p, sc);
         else rc = build_schedule(p, inverse ? 1 : 0, db, sc);
         if (rc) return rc;
         rc = widen_views(p, sc);
