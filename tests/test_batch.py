@@ -1,210 +1,55 @@
 """Batched plans (dfft_plan_create_batched) without a GPU: argument checks, the batch = 1 identity, the selection of the
 one-launch batched stage, its work list, and CPU replays of batched schedules.
 
-The replay runs the step lists dfft_plan_describe returns for every rank of a batched plan, with the numpy machinery of
-test_schedule_emulation.py (memory model, views, happens-before check), on distinct inputs per field.  Every field's
-block must match the oracle, and every step may only touch the caller's memory of its own field (the per-field distance
-is the product of the buffer's layout, never the domain size)."""
-import ctypes as C
+The replay runs the step lists dfft_plan_describe returns for every rank of a batched plan through step_replay.py, on
+distinct inputs per field.  Every field's block must match the oracle, and every step may only touch the caller's memory of
+its own field (the per-field distance is the product of the buffer's layout, never the domain size)."""
 import json
 import os
 import subprocess
 import tempfile
 
-import numpy as np
 import pytest
 
 import distributedfft_b200 as dfft
-from distributedfft_b200 import _lib
-from distributedfft_b200._lib import check, lib
+import step_replay as R
+from distributedfft_b200._lib import lib
 from oracle import dft_oracle as O
 
-from test_schedule_emulation import A2A, P2P, PE, SL, STREAMS, SYNC, USER_IN, USER_OUT, ZY, Memory, Ordering, describe, view_indices
+from test_schedule_emulation import A2A, P2P, PE, SL, STREAMS, SYNC, ZY, describe
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SIZE_MAX = (1 << 64) - 1
 
 
+def plan_of(P, decomp, transform, shape, p1, p2, batch, comm_method=P2P, send_method=SYNC, prec=None):
+    return R.Plan(P, decomp, tuple(shape), p1, p2, transform=transform, prec=dfft.F64 if prec is None else prec, comm=comm_method, send=send_method,
+                  batch=batch)
+
+
 def create(rank, P, decomp, transform, shape, p1, p2, batch, comm_method=P2P, send_method=SYNC, prec=None):
     """dry batched plan: (rc, message, comm, plan)"""
-    comm = C.c_void_p()
-    check(lib().dfft_comm_create_dry(rank, P, C.byref(comm)))
-    cfg = _lib.dfft_config(1, 0, comm_method, send_method, None, comm_method, send_method)
-    plan = C.c_void_p()
-    rc = lib().dfft_plan_create_batched(comm, C.byref(cfg), decomp, dfft.F64 if prec is None else prec, transform, shape[0], shape[1], shape[2],
-                                        p1, p2, batch, 1, C.byref(plan))
-    return rc, (lib().dfft_last_error_string() or b"").decode(), comm, plan
+    return R.create(plan_of(P, decomp, transform, shape, p1, p2, batch, comm_method, send_method, prec), rank)
 
 
 def describe_batched(rank, P, decomp, transform, shape, p1, p2, comm_method, send_method, inverse, d, batch, prec=None):
-    rc, msg, comm, plan = create(rank, P, decomp, transform, shape, p1, p2, batch, comm_method, send_method, prec)
-    assert rc == 0, msg
-    need = C.c_size_t()
-    check(lib().dfft_plan_describe(plan, inverse, d, None, 0, C.byref(need)))
-    buf = C.create_string_buffer(need.value)
-    check(lib().dfft_plan_describe(plan, inverse, d, buf, need.value, C.byref(need)))
-    assert lib().dfft_get_batch(plan) == batch
-    lib().dfft_plan_destroy(plan)
-    lib().dfft_comm_destroy(comm)
-    return json.loads(buf.value.decode())
+    return R.describe(plan_of(P, decomp, transform, shape, p1, p2, batch, comm_method, send_method, prec), rank, inverse, d)
 
 
 def run_batched(P, decomp, transform, shape, p1, p2, comm_method, send_method, inverse, d, batch, prec=None):
-    """Replays a batched exec on every rank; returns the worst rel-L2 error over all fields and ranks."""
+    """Replays a batched exec on every rank on a distinct input per field; returns the worst rel-L2 error over all fields
+    and ranks."""
     nx, ny, nz = shape
     c2c = transform == dfft.C2C
-    scheds = [describe_batched(r, P, decomp, transform, shape, p1, p2, comm_method, send_method, inverse, d, batch, prec) for r in range(P)]
-    es = scheds[0]["esize"]
+    p = plan_of(P, decomp, transform, shape, p1, p2, batch, comm_method, send_method, prec)
+    scheds = [R.describe(p, r, inverse, d) for r in range(P)]
     if batch > 1:
         assert all(s["batch"] == batch for s in scheds)
-    lay = lambda r, w: dfft.layout(decomp, transform, nx, ny, nz, p1, p2, r, w)
-    xs, specs = [], []
-    for f in range(batch):  # a distinct input per field
-        x = O.complex_input(shape, seed=1234 + f) if c2c else O.real_input(shape, seed=1234 + f)
-        xs.append(x)
-        specs.append(O.fft_c2c(x, d) if c2c else O.fft_r2c(x, d))
-    mem = Memory(es)
-    for r in range(P):
-        for s_ in range(scheds[r]["nslots"]):
-            mem.add(scheds[r]["slots"][s_][r], scheds[r]["slot_bytes"] // es)
-    uin, uout, fin, fout = [], [], [], []  # user buffers and per-field sizes (complex units) per rank
-    for r in range(P):
-        isz, ist = lay(r, 0)
-        osz, ost = lay(r, d)
-        nin, nout = int(np.prod(isz)), int(np.prod(osz))
-        if not c2c:
-            nin //= 2  # reals, two per complex unit
-        fi, fo = (nout, nin) if inverse else (nin, nout)
-        if batch > 1:
-            assert (scheds[r]["field_in"], scheds[r]["field_out"]) == (fi * es, fo * es)
-        fin.append(fi)
-        fout.append(fo)
-        a = mem.add(USER_IN + (r << 48), batch * fi)
-        uout.append(mem.add(USER_OUT + (r << 48), batch * fo))  # exactly batch fields: nothing beyond the last one
-        for f in range(batch):
-            if not inverse:
-                blk = np.ascontiguousarray(O.block(xs[f], ist, isz))
-                src = blk.astype(np.complex128).ravel() if c2c else blk.ravel().view(np.complex128)
-            else:
-                src = np.ascontiguousarray(O.block(specs[f], ost, osz)).ravel()
-            a[f * fi:(f + 1) * fi] = src
-        uin.append(a)
-    in_copy = [a.copy() for a in uin]
-    nsteps = len(scheds[0]["steps"])
-    assert all(len(s["steps"]) == nsteps for s in scheds)
-    order = Ordering(scheds)
-    slot_owner = {}
-    for r in range(P):
-        for s_ in range(scheds[r]["nslots"]):
-            slot_owner[scheds[r]["slots"][s_][r]] = (r, s_)
-
-    def owner_of(addr):
-        for base, (q, s_) in slot_owner.items():
-            if base <= addr < base + scheds[q]["slot_bytes"]:
-                return q, s_
-        return None
-
-    last_remote_write, last_rdv = {}, [-1] * P
-
-    def user_range(r, st, which):
-        """elements of the caller's buffer `which` (1 in, 2 out) this step may touch"""
-        per = fin[r] if which == 1 else fout[r]
-        f = st.get("field", 0)
-        return (0, batch * per) if f < 0 else (f * per, (f + 1) * per)
-
-    def user_base(r, flag):
-        return {1: USER_IN, 2: USER_OUT}[flag] + (r << 48)
-
-    for k in range(nsteps):
-        pending = []
-        for r in range(P):
-            st = scheds[r]["steps"][k]
-            if st["type"] == 1:
-                last_rdv[r] = k
-                continue
-            if st["type"] == 2:
-                sb = scheds[r]["slots"][st["send_slot"]][r]
-                for peer in st["peers"]:
-                    q = peer["rank"]
-                    rb = scheds[q]["slots"][st["recv_slot"]][q]
-                    mine = [pp for pp in scheds[q]["steps"][k]["peers"] if pp["rank"] == r][0]
-                    assert mine["rcount"] == peer["scount"]
-                    src, so = mem.resolve(sb + peer["soff"] * es)
-                    dst, do = mem.resolve(rb + mine["roff"] * es)
-                    order.read(r, k, id(src), src.size, np.arange(so, so + peer["scount"]))
-                    pending.append((dst, do, src[so:so + peer["scount"]].copy(), q))
-                continue
-            N = 1 << st["log2n"]
-            A0, A1, B = st["A0"], st["A1"], st["B"]
-            kind = st["kind"]
-            if st["in_user"] == 0:
-                for seg in st["in"]["segs"]:
-                    own = owner_of(seg["base"])
-                    assert own is not None and own[0] == r, "passes only read local memory"
-                    w = last_remote_write.get(own, -1)
-                    assert w < 0 or w < last_rdv[r] <= k, f"rank {r} step {k} reads slot {own} written remotely at step {w} without a rendezvous"
-            if st["out_user"] == 0:
-                for seg in st["out"]["segs"]:
-                    own = owner_of(seg["base"])
-                    assert own is not None
-                    if own[0] != r:
-                        assert last_rdv[r] >= 0, f"rank {r} writes into rank {own[0]}'s slot before its entry rendezvous"
-                        last_remote_write[own] = k
-            ub_in = user_base(r, st["in_user"]) if st["in_user"] else None
-            ub_out = user_base(r, st["out_user"]) if st["out_user"] else None
-            n_in, n_out = {0: (N, N), 1: (N, N), 2: (N, N + 1), 3: (N + 1, N)}[kind]
-            b_ = B if kind in (0, 1) else 1
-
-            def touched(view, n, ub, flag):
-                """(array, index, ns) per segment; user accesses are checked against the step's field"""
-                out = []
-                for base, ns, off in view_indices(view, A0, A1, n, b_, ub):
-                    arr, o = mem.resolve(base)
-                    idx = o + off
-                    if ub is not None:
-                        lo, hi = user_range(r, st, flag)
-                        assert lo <= idx.min() and idx.max() < hi, (f"rank {r} step {k} ({st['label']}) touches caller buffer {flag} at "
-                                                                    f"[{idx.min()}, {idx.max()}] outside its field [{lo}, {hi})")
-                    out.append((arr, idx, ns))
-                return out
-
-            data = np.zeros((A0, A1, n_in, b_), dtype=np.complex128)
-            for arr, idx, ns in touched(st["in"], n_in, ub_in, st["in_user"]):
-                data[:, :, ns, :] = arr[idx]
-                order.read(r, k, id(arr), arr.size, idx)
-            if kind in (0, 1):
-                res = np.fft.ifft(data, axis=2) * N if st["inverse"] else np.fft.fft(data, axis=2)
-            elif kind == 2:
-                reals = np.ascontiguousarray(data[..., 0]).view(np.float64)
-                res = np.fft.rfft(reals, axis=2)[..., None]
-            else:
-                reals = np.fft.irfft(data[..., 0], n=2 * N, axis=2) * (2 * N)
-                res = np.ascontiguousarray(reals).view(np.complex128)[..., None]
-            for arr, idx, ns in touched(st["out"], n_out, ub_out, st["out_user"]):
-                pending.append((arr, idx, res[:, :, ns, :], r))
-        for arr, idx, val, who in pending:
-            if isinstance(idx, (int, np.integer)):
-                order.write(who, k, id(arr), arr.size, np.arange(idx, idx + val.size))
-                arr[idx:idx + val.size] = val
-            else:
-                order.write(who, k, id(arr), arr.size, idx)
-                arr[idx] = val
-    worst = 0.0
-    for r in range(P):
-        assert np.array_equal(uin[r], in_copy[r]), f"rank {r}: the input was modified"
-        for f in range(batch):
-            if not inverse:
-                osz, ost = lay(r, d)
-                got = uout[r][f * fout[r]:f * fout[r] + int(np.prod(osz))].reshape(osz)
-                worst = max(worst, O.rel_l2(got, O.block(specs[f], ost, osz)))
-            else:
-                isz, ist = lay(r, 0)
-                want = O.block(xs[f], ist, isz).astype(np.complex128 if c2c else np.float64)
-                scale = float(nz * (ny if d >= 2 else 1) * (nx if d >= 3 else 1))
-                seg = uout[r][f * fout[r]:(f + 1) * fout[r]]
-                got = seg.reshape(isz) if c2c else seg.view(np.float64).reshape(isz)
-                worst = max(worst, O.rel_l2(got, want * scale))
-    return worst
+    xs = [O.complex_input(shape, seed=1234 + f) if c2c else O.real_input(shape, seed=1234 + f) for f in range(batch)]
+    specs = [O.fft_c2c(x, d) if c2c else O.fft_r2c(x, d) for x in xs]
+    n = float(nz * (ny if d >= 2 else 1) * (nx if d >= 3 else 1))
+    x, want = (specs, [n * x for x in xs]) if inverse else (xs, specs)
+    return R.error(R.replay(p, inverse, d, x, scheds), want)
 
 
 CASES = [

@@ -1,9 +1,8 @@
 """Interleaved multi-component plans (dfft_plan_create_interleaved) without a GPU: argument checks, the C = 1 identity,
 sizes, and CPU replays of every rank's step list.
 
-The replay runs the step lists dfft_plan_describe returns for every rank, with the numpy machinery of
-test_schedule_emulation.py (memory model, views, happens-before check), on [X][Y][Z][C] inputs with a distinct input per
-field.  The interleaved z pass (kind 8) has the TILED view mapping with b the component.  Every field's block of every
+The replay runs the step lists dfft_plan_describe returns for every rank through step_replay.py, on [X][Y][Z][C] inputs
+with a distinct input per field.  The interleaved z pass (kind 8) has the TILED view mapping with b the component.  Every field's block of every
 component must match the oracle, and every step may only touch the caller's memory of its own field."""
 import ctypes as C
 import json
@@ -15,53 +14,41 @@ import numpy as np
 import pytest
 
 import distributedfft_b200 as dfft
-from distributedfft_b200 import _lib
+import step_replay as R
 from distributedfft_b200._lib import check, lib
 from oracle import dft_oracle as O
 
 from test_batch import describe_batched
-from test_schedule_emulation import A2A, P2P, PE, SL, SYNC, USER_IN, USER_OUT, ZY, Memory, Ordering, view_indices
+from test_padded import drop_rendezvous
+from test_schedule_emulation import A2A, P2P, PE, SL, SYNC, ZY
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SIZE_MAX = (1 << 64) - 1
-ILV, R2C_ILV, C2R_ILV = 8, 9, 10  # PASS_C2C_ILV, PASS_R2C_ILV, PASS_C2R_ILV
+ILV = 8  # PASS_C2C_ILV
+
+
+def plan_of(P, decomp, transform, shape, p1, p2, comps, batch=1, comm_method=P2P, prec=None, scale=1.0):
+    return R.Plan(P, decomp, tuple(shape), p1, p2, transform=transform, prec=dfft.F64 if prec is None else prec, comm=comm_method, batch=batch,
+                  components=comps, scale=None if scale == 1.0 else (scale, scale))
 
 
 def create(rank, P, decomp, transform, shape, p1, p2, comps, batch=1, comm_method=P2P, prec=None):
     """dry interleaved plan: (rc, message, comm, plan)"""
-    comm = C.c_void_p()
-    check(lib().dfft_comm_create_dry(rank, P, C.byref(comm)))
-    cfg = _lib.dfft_config(1, 0, comm_method, SYNC, None, comm_method, SYNC)
-    plan = C.c_void_p()
-    rc = lib().dfft_plan_create_interleaved(comm, C.byref(cfg), decomp, dfft.F64 if prec is None else prec, transform, shape[0], shape[1],
-                                            shape[2], p1, p2, comps, batch, 1, C.byref(plan))
-    return rc, (lib().dfft_last_error_string() or b"").decode(), comm, plan
+    return R.create(plan_of(P, decomp, transform, shape, p1, p2, comps, batch, comm_method, prec), rank)
 
 
 def describe_ilv(rank, P, decomp, transform, shape, p1, p2, comps, batch, comm_method, inverse, d, scale=1.0, prec=None):
-    rc, msg, comm, plan = create(rank, P, decomp, transform, shape, p1, p2, comps, batch, comm_method, prec)
-    assert rc == 0, msg
-    assert lib().dfft_get_components(plan) == comps
-    if scale != 1.0:
-        check(lib().dfft_plan_set_scale(plan, scale, scale))
-    need = C.c_size_t()
-    check(lib().dfft_plan_describe(plan, inverse, d, None, 0, C.byref(need)))
-    buf = C.create_string_buffer(need.value)
-    check(lib().dfft_plan_describe(plan, inverse, d, buf, need.value, C.byref(need)))
-    lib().dfft_plan_destroy(plan)
-    lib().dfft_comm_destroy(comm)
-    return json.loads(buf.value.decode())
+    return R.describe(plan_of(P, decomp, transform, shape, p1, p2, comps, batch, comm_method, prec, scale), rank, inverse, d)
 
 
-def run_interleaved(P, decomp, shape, p1, p2, comm_method, inverse, d, comps, batch=1, scale=1.0, transform=dfft.C2C):
+def run_interleaved(P, decomp, shape, p1, p2, comm_method, inverse, d, comps, batch=1, scale=1.0, transform=dfft.C2C, mutate=None):
     """Replays an interleaved exec on every rank; returns the worst rel-L2 error over fields, components and ranks.  R2C /
     C2R: the z pass is the interleaved R2C / C2R pass (kinds 9 / 10) whose real side is counted in reals."""
     nx, ny, nz = shape
     c2c = transform == dfft.C2C
-    scheds = [describe_ilv(r, P, decomp, transform, shape, p1, p2, comps, batch, comm_method, inverse, d, scale) for r in range(P)]
-    es = scheds[0]["esize"]
+    p = plan_of(P, decomp, transform, shape, p1, p2, comps, batch, comm_method, scale=scale)
+    scheds = [R.describe(p, r, inverse, d) for r in range(P)]
     assert all(s.get("components", 1) == comps for s in scheds)
-    lay = lambda r, w: dfft.layout(decomp, transform, nx, ny, nz, p1, p2, r, w)
     xs, specs = [], []
     for f in range(batch):
         if c2c:
@@ -71,109 +58,9 @@ def run_interleaved(P, decomp, shape, p1, p2, comm_method, inverse, d, comps, ba
         xs.append(x)
         ft = O.fft_c2c if c2c else O.fft_r2c
         specs.append(np.stack([ft(np.ascontiguousarray(x[..., c]), d) for c in range(comps)], axis=-1))
-    mem = Memory(es)
-    for r in range(P):
-        for s_ in range(scheds[r]["nslots"]):
-            mem.add(scheds[r]["slots"][s_][r], scheds[r]["slot_bytes"] // es)
-    uin, uout, fin, fout = [], [], [], []  # user buffers and per-field sizes, complex units
-    for r in range(P):
-        isz, ist = lay(r, 0)
-        osz, ost = lay(r, d)
-        nin, nout = int(np.prod(isz)) * comps, int(np.prod(osz)) * comps
-        if not c2c:
-            nin //= 2  # reals, two per complex unit
-        fi, fo = (nout, nin) if inverse else (nin, nout)
-        if batch > 1:
-            assert (scheds[r]["field_in"], scheds[r]["field_out"]) == (fi * es, fo * es)
-        fin.append(fi)
-        fout.append(fo)
-        a = mem.add(USER_IN + (r << 48), batch * fi)
-        uout.append(mem.add(USER_OUT + (r << 48), batch * fo))
-        for f in range(batch):
-            src = np.ascontiguousarray(O.block(xs[f], ist, isz) if not inverse else O.block(specs[f], ost, osz)).ravel()
-            a[f * fi:(f + 1) * fi] = src if (c2c or inverse) else src.view(np.complex128)
-        uin.append(a)
-    in_copy = [a.copy() for a in uin]
-    nsteps = len(scheds[0]["steps"])
-    assert all(len(s["steps"]) == nsteps for s in scheds)
-    order = Ordering(scheds)
-    for k in range(nsteps):
-        pending = []
-        for r in range(P):
-            st = scheds[r]["steps"][k]
-            if st["type"] == 1:
-                continue
-            if st["type"] == 2:
-                sb = scheds[r]["slots"][st["send_slot"]][r]
-                for peer in st["peers"]:
-                    q = peer["rank"]
-                    rb = scheds[q]["slots"][st["recv_slot"]][q]
-                    mine = [pp for pp in scheds[q]["steps"][k]["peers"] if pp["rank"] == r][0]
-                    assert mine["rcount"] == peer["scount"]
-                    src, so = mem.resolve(sb + peer["soff"] * es)
-                    dst, do = mem.resolve(rb + mine["roff"] * es)
-                    order.read(r, k, id(src), src.size, np.arange(so, so + peer["scount"]))
-                    pending.append((dst, dst, do, src[so:so + peer["scount"]].copy(), q))
-                continue
-            kind = st["kind"]
-            assert kind in ((1, ILV) if c2c else (1, R2C_ILV, C2R_ILV)) or comps == 1, kind
-            if kind in (ILV, R2C_ILV, C2R_ILV):
-                assert st["B"] == comps and st["in"]["sN"] == comps and st["out"]["sN"] == comps
-            N = st.get("n", 1 << st["log2n"])
-            A0, A1, B = st["A0"], st["A1"], st["B"]
-            n_in, n_out = {R2C_ILV: (N, N // 2 + 1), C2R_ILV: (N // 2 + 1, N)}.get(kind, (N, N))
-            real_in, real_out = kind == R2C_ILV, kind == C2R_ILV
-            f = st.get("field", 0)
-            ubase = {1: USER_IN, 2: USER_OUT}
-
-            def touched(view, user, n, real):
-                """(complex array, accessed array, index, ns) per segment; a real view indexes the float64 view"""
-                out = []
-                ub = ubase[user] + (r << 48) if user else None
-                for base, ns, off in view_indices(view, A0, A1, n, B, ub):
-                    arr, o = mem.resolve(base)
-                    idx = (2 * o + off) if real else (o + off)
-                    cidx = idx // 2 if real else idx
-                    if ub is not None:
-                        per = fin[r] if user == 1 else fout[r]
-                        assert f * per <= cidx.min() and cidx.max() < (f + 1) * per, f"rank {r} step {k} ({st['label']}) leaves its field"
-                    out.append((arr, arr.view(np.float64) if real else arr, idx, ns))
-                return out
-
-            data = np.zeros((A0, A1, n_in, B), dtype=np.float64 if real_in else np.complex128)
-            for arr, acc, idx, ns in touched(st["in"], st["in_user"], n_in, real_in):
-                data[:, :, ns, :] = acc[idx]
-                order.read(r, k, id(arr), arr.size, idx // 2 if real_in else idx)
-            if kind == R2C_ILV:
-                res = np.fft.rfft(data, axis=2)
-            elif kind == C2R_ILV:
-                res = np.fft.irfft(data, n=N, axis=2) * N
-            else:
-                res = np.fft.ifft(data, axis=2) * N if st["inverse"] else np.fft.fft(data, axis=2)
-            res = res * st.get("scale", 1.0)
-            for arr, acc, idx, ns in touched(st["out"], st["out_user"], n_out, real_out):
-                pending.append((arr, acc, idx, res[:, :, ns, :], r))
-        for arr, acc, idx, val, who in pending:
-            if isinstance(idx, (int, np.integer)):
-                order.write(who, k, id(arr), arr.size, np.arange(idx, idx + val.size))
-                acc[idx:idx + val.size] = val
-            else:
-                order.write(who, k, id(arr), arr.size, np.unique(idx // 2) if acc is not arr else idx)
-                acc[idx] = val
-    worst = 0.0
-    for r in range(P):
-        assert np.array_equal(uin[r], in_copy[r]), f"rank {r}: the input was modified"
-        for f in range(batch):
-            seg = uout[r][f * fout[r]:(f + 1) * fout[r]]
-            if not inverse:
-                osz, ost = lay(r, d)
-                worst = max(worst, O.rel_l2(seg.reshape(*osz, comps), O.block(specs[f], ost, osz) * scale))
-            else:
-                isz, ist = lay(r, 0)
-                n = float(nz * (ny if d >= 2 else 1) * (nx if d >= 3 else 1))
-                got = seg.reshape(*isz, comps) if c2c else seg.view(np.float64).reshape(*isz, comps)
-                worst = max(worst, O.rel_l2(got, O.block(xs[f], ist, isz) * n * scale))
-    return worst
+    n = float(nz * (ny if d >= 2 else 1) * (nx if d >= 3 else 1))
+    x, want = (specs, [x * n * scale for x in xs]) if inverse else (xs, [s * scale for s in specs])
+    return R.error(R.replay(p, inverse, d, x, scheds, mutate), want)
 
 
 CASES = [
@@ -256,6 +143,15 @@ def test_interleaved_batch_and_scale(inverse):
     assert run_interleaved(4, SL, (8, 8, 64), 4, 1, P2P, inverse, 3, 3, batch=2, scale=0.375) < 1e-12
     assert run_interleaved(4, PE, (8, 8, 32), 2, 2, A2A, inverse, 3, 5, batch=2, scale=1.5) < 1e-12
     assert run_interleaved(1, SL, (64, 64, 64), 1, 1, P2P, inverse, 3, 3, batch=2) < 1e-12  # no batched stage
+
+
+@pytest.mark.parametrize("inverse", [0, 1])
+def test_slot_rule_catches_a_missing_rendezvous(inverse):
+    """the replay's slot rule holds interleaved plans too: without the rendezvous of its transpositions, a pass reads a slot
+    that a peer stored into"""
+    assert run_interleaved(4, SL, (16, 8, 64), 4, 1, P2P, inverse, 3, 3) < 1e-12
+    with pytest.raises(AssertionError, match="without a rendezvous"):
+        run_interleaved(4, SL, (16, 8, 64), 4, 1, P2P, inverse, 3, 3, mutate=drop_rendezvous)
 
 
 ONE = [(1, SL, (64, 64, 64), 1, 1, P2P), (1, SL, (512, 512, 512), 1, 1, P2P), (2, SL, (8, 8, 128), 2, 1, P2P),

@@ -27,8 +27,9 @@ import torch
 import distributedfft_b200 as dfft
 from distributedfft_b200 import _lib
 from distributedfft_b200._lib import check, lib
+from step_replay import view_indices
 from test_inplace import run_inplace
-from test_schedule_emulation import CASES, KNOBS, random_case, run_case, view_indices
+from test_schedule_emulation import CASES, KNOBS, random_case, run_case
 from test_transform_axes import describe_raw, fwd_ref, inv_ref, run as replay_cpu, set_axes
 
 SL, ZY, PE = dfft.SLAB_ZY_THEN_X, dfft.SLAB_Z_THEN_YX, dfft.PENCIL

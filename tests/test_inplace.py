@@ -1,105 +1,39 @@
 """In-place plans (dfft_plan_create_inplace) without a GPU: argument checks, the work area, and CPU replays of every rank's
-step list with the caller's `in` and `out` mapped to ONE address range.
+step list with the caller's `in` and `out` mapped to ONE address range (step_replay.py).
 
-The replay is the numpy machinery of test_schedule_emulation.py with three additions:
-  - the buffer of a rank holds `batch` fields dfft_get_domain_size() bytes apart; real rows of R2C / C2R plans are padded
-    to Nz/2 + 1 complex units, and the padding must never be read or written;
-  - the happens-before check (Ordering) now also sees the read-after-write and write-after-read pairs on the buffer;
-  - a line check inside every step: a line may only write addresses that it reads itself or that no other line of the
-    step reads (the passes load a line or tile completely before they store it, so that is what in place needs), and the
-    two phases of the fused z + y stage and of the one-launch batched stage, which run concurrently, touch disjoint
-    planes / fields."""
+The buffer of a rank holds `batch` fields dfft_get_domain_size() bytes apart; real rows of R2C / C2R plans are padded to
+Nz/2 + 1 complex units, and the padding must never be read or written.  The replay's happens-before check sees the
+read-after-write and write-after-read pairs on the buffer, its line check that a line only writes addresses that it reads
+itself or that no other line of the step reads (the passes load a line or tile completely before they store it, so that is
+what in place needs), and its phase check that the two phases of the fused z + y stage and of the one-launch batched
+stage, which run concurrently, touch disjoint planes / fields."""
 import ctypes as C
-import json
 
 import numpy as np
 import pytest
 
 import distributedfft_b200 as dfft
-from distributedfft_b200 import _lib
+import step_replay as R
 from distributedfft_b200._lib import check, lib
 from oracle import dft_oracle as O
 
-from test_schedule_emulation import A2A, P2P, PE, SL, STREAMS, SYNC, ZY, Memory, Ordering, view_indices
+from test_schedule_emulation import A2A, P2P, PE, SL, STREAMS, SYNC, ZY
 
-USER = 1 << 60  # synthetic address range of the caller's one buffer (rank r: USER + r << 48)
 SIZE_MAX = (1 << 64) - 1
-PAD = 1234.5 - 678.25j  # value of the padding of real rows
+
+
+def plan_of(P, decomp, transform, shape, p1, p2, batch=1, comm=P2P, send=SYNC, prec=None, scale=None, inplace=True):
+    return R.Plan(P, decomp, tuple(shape), p1, p2, transform=transform, prec=dfft.F64 if prec is None else prec, comm=comm, send=send, batch=batch,
+                  inplace=inplace, scale=scale)
 
 
 def create(rank, P, decomp, transform, shape, p1, p2, batch=1, comm=P2P, send=SYNC, prec=None, inplace=True):
     """dry plan: (rc, message, comm, plan)"""
-    c = C.c_void_p()
-    check(lib().dfft_comm_create_dry(rank, P, C.byref(c)))
-    cfg = _lib.dfft_config(1, 0, comm, send, None, comm, send)
-    plan = C.c_void_p()
-    fn = lib().dfft_plan_create_inplace if inplace else lib().dfft_plan_create_batched
-    rc = fn(c, C.byref(cfg), decomp, dfft.F64 if prec is None else prec, transform, *shape, p1, p2, batch, 1, C.byref(plan))
-    return rc, (lib().dfft_last_error_string() or b"").decode(), c, plan
+    return R.create(plan_of(P, decomp, transform, shape, p1, p2, batch, comm, send, prec, inplace=inplace), rank)
 
 
 def describe(rank, P, decomp, transform, shape, p1, p2, comm, send, inverse, d, batch=1, prec=None, scale=None, inplace=True):
-    rc, msg, c, plan = create(rank, P, decomp, transform, shape, p1, p2, batch, comm, send, prec, inplace)
-    assert rc == 0, msg
-    if scale is not None:
-        assert lib().dfft_plan_set_scale(plan, *scale) == 0
-    need = C.c_size_t()
-    check(lib().dfft_plan_describe(plan, inverse, d, None, 0, C.byref(need)))
-    buf = C.create_string_buffer(need.value)
-    check(lib().dfft_plan_describe(plan, inverse, d, buf, need.value, C.byref(need)))
-    sc = json.loads(buf.value.decode())
-    sc["domain_bytes"] = lib().dfft_get_domain_size(plan)
-    sc["work_bytes"] = lib().dfft_get_work_size_device(plan)
-    lib().dfft_plan_destroy(plan)
-    lib().dfft_comm_destroy(c)
-    return sc
-
-
-def _line_check(r, k, st, reads, writes):
-    """reads / writes: [(array, flat indices, line ids)] of one step: a line writes only what it reads itself or what no
-    other line of the step reads"""
-    owner = {}
-    for arr, idx, line in reads:
-        i, l = np.asarray(idx).ravel(), np.broadcast_to(line, np.shape(idx)).ravel()
-        prev = owner.get(id(arr))
-        if prev is not None:
-            i, l = np.concatenate([prev[0], i]), np.concatenate([prev[1], l])
-        owner[id(arr)] = (i, l)
-    table = {}
-    for key, (i, l) in owner.items():
-        u, inv = np.unique(i, return_inverse=True)
-        lo = np.full(u.size, np.iinfo(np.int64).max)
-        hi = np.full(u.size, -1)
-        np.minimum.at(lo, inv, l)
-        np.maximum.at(hi, inv, l)
-        table[key] = (u, np.where(lo == hi, lo, -2))  # the one reading line, or -2: several lines read it
-    for arr, idx, line in writes:
-        if id(arr) not in table:
-            continue
-        u, rl = table[id(arr)]
-        i, l = np.asarray(idx).ravel(), np.broadcast_to(line, np.shape(idx)).ravel()
-        pos = np.searchsorted(u, i)
-        hit = (pos < u.size) & (u[np.minimum(pos, u.size - 1)] == i)
-        reader = np.where(hit, rl[np.minimum(pos, u.size - 1)], -1)
-        bad = (reader != -1) & (reader != l)
-        assert not bad.any(), (f"rank {r} step {k} ({st['label']}): line {int(l[bad][0])} writes an element that line {int(reader[bad][0])} "
-                               f"reads (or that several lines read)")
-
-
-def _phase_check(r, k, acc, groups):
-    """the two phases of a two-phase kernel (steps k-1 and k): every element is touched by one plane / field only"""
-    owner = {}
-    for arr, idx, grp in acc:
-        i, g = np.asarray(idx).ravel(), np.broadcast_to(grp, np.shape(idx)).ravel()
-        prev = owner.get(id(arr))
-        owner[id(arr)] = (i, g) if prev is None else (np.concatenate([prev[0], i]), np.concatenate([prev[1], g]))
-    for i, g in owner.values():
-        u, inv = np.unique(i, return_inverse=True)
-        lo = np.full(u.size, groups)
-        hi = np.full(u.size, -1)
-        np.minimum.at(lo, inv, g)
-        np.maximum.at(hi, inv, g)
-        assert (lo == hi).all(), f"rank {r} steps {k - 1}/{k}: the two phases of one launch share elements across planes / fields"
+    return R.describe(plan_of(P, decomp, transform, shape, p1, p2, batch, comm, send, prec, scale, inplace), rank, inverse, d)
 
 
 def run_inplace(P, decomp, transform, shape, p1, p2, comm, send, inverse, d, batch=1, scale=1.0, prec=None, mutate=None):
@@ -108,150 +42,12 @@ def run_inplace(P, decomp, transform, shape, p1, p2, comm, send, inverse, d, bat
     nx, ny, nz = shape
     c2c = transform == dfft.C2C
     sc_ = None if scale == 1.0 else ((1.0, scale) if inverse else (scale, 1.0))
-    scheds = [describe(r, P, decomp, transform, shape, p1, p2, comm, send, inverse, d, batch, prec, sc_) for r in range(P)]
-    if mutate:
-        mutate(scheds)  # negative tests
-    es = scheds[0]["esize"]
-    nzc = nz if c2c else nz // 2 + 1
-    lay = lambda r, w: dfft.layout(decomp, transform, nx, ny, nz, p1, p2, r, w)
+    p = plan_of(P, decomp, transform, shape, p1, p2, batch, comm, send, prec, sc_)
     xs = [O.complex_input(shape, seed=77 + f) if c2c else O.real_input(shape, seed=77 + f) for f in range(batch)]
     specs = [O.fft_c2c(x, d) if c2c else O.fft_r2c(x, d) for x in xs]
-    mem = Memory(es)
-    for r in range(P):
-        assert scheds[r]["inplace"] is True
-        for s_ in range(scheds[r]["nslots"]):
-            mem.add(scheds[r]["slots"][s_][r], scheds[r]["slot_bytes"] // es)
-    bufs, dom, pads = [], [], []
-    for r in range(P):
-        D = scheds[r]["domain_bytes"] // es
-        if batch > 1:
-            assert scheds[r]["field_in"] == scheds[r]["field_out"] == D * es
-        dom.append(D)
-        buf = mem.add(USER + (r << 48), batch * D)
-        isz, ist = lay(r, 0)
-        osz, ost = lay(r, d)
-        pad = np.zeros(batch * D, dtype=bool)  # padding of the real rows: never read or written
-        for f in range(batch):
-            if not inverse:
-                blk = np.ascontiguousarray(O.block(xs[f], ist, isz))
-                if c2c:
-                    buf[f * D:f * D + blk.size] = blk.astype(np.complex128).ravel()
-                else:  # rows of Nz reals = Nz/2 units, Nzc units apart
-                    rows = buf[f * D:f * D + isz[0] * isz[1] * nzc].reshape(isz[0] * isz[1], nzc)
-                    rows[:, :nz // 2] = blk.reshape(-1, nz).view(np.complex128)
-                    rows[:, nz // 2:] = PAD
-            else:
-                src = np.ascontiguousarray(O.block(specs[f], ost, osz)).ravel()
-                buf[f * D:f * D + src.size] = src
-            if not c2c:  # the real input rows (forward) / output rows (inverse)
-                m = pad[f * D:f * D + isz[0] * isz[1] * nzc].reshape(-1, nzc)
-                m[:, nz // 2:] = True
-        bufs.append(buf)
-        pads.append(pad)
-    nsteps = len(scheds[0]["steps"])
-    assert all(len(sc["steps"]) == nsteps for sc in scheds)
-    order = Ordering(scheds)
-    prev_acc = {}
-    for k in range(nsteps):
-        pending = []
-        for r in range(P):
-            st = scheds[r]["steps"][k]
-            if st["type"] == 1:
-                continue
-            if st["type"] == 2:
-                sb = scheds[r]["slots"][st["send_slot"]][r]
-                for peer in st["peers"]:
-                    q = peer["rank"]
-                    rb = scheds[q]["slots"][st["recv_slot"]][q]
-                    mine = [pp for pp in scheds[q]["steps"][k]["peers"] if pp["rank"] == r][0]
-                    src, so = mem.resolve(sb + peer["soff"] * es)
-                    dst, do = mem.resolve(rb + mine["roff"] * es)
-                    order.read(r, k, id(src), src.size, np.arange(so, so + peer["scount"]))
-                    pending.append((dst, do, src[so:so + peer["scount"]].copy(), q))
-                continue
-            kind = st["kind"]
-            N = st.get("n", 1 << st["log2n"])
-            A0, A1, B = st["A0"], st["A1"], st["B"]
-            ub_in = USER + (r << 48) if st["in_user"] in (1, 2) else None  # `in` and `out` are the same buffer
-            ub_out = USER + (r << 48) if st["out_user"] == 2 else None
-            n_in, n_out = {0: (N, N), 1: (N, N), 2: (N, N + 1), 3: (N + 1, N)}[kind]
-            b_ = B if kind in (0, 1) else 1
-            line = (np.arange(A0)[:, None, None, None] * A1 + np.arange(A1)[None, :, None, None]) * b_ + np.arange(b_)[None, None, None, :]
-            field = st.get("field", -1)
-            reads, writes = [], []
-            data = np.zeros((A0, A1, n_in, b_), dtype=np.complex128)
-            for base, ns, off in view_indices(st["in"], A0, A1, n_in, b_, ub_in):
-                arr, o = mem.resolve(base)
-                data[:, :, ns, :] = arr[o + off]
-                order.read(r, k, id(arr), arr.size, o + off)
-                reads.append((arr, o + off, line))
-            for base, ns, off in view_indices(st["out"], A0, A1, n_out, b_, ub_out):
-                arr, o = mem.resolve(base)
-                writes.append((arr, o + off, line, ns))
-            _line_check(r, k, st, reads, [w[:3] for w in writes])
-            for j, (arr, idx, _) in enumerate(reads + [w[:3] for w in writes]):
-                if arr is not bufs[r] or idx.size == 0:  # empty tail passes of ranks without leftover columns
-                    continue
-                if field >= 0:  # a per-field step stays inside its field
-                    assert field * dom[r] <= idx.min() and idx.max() < (field + 1) * dom[r], f"step {k} leaves field {field}"
-                # forward: the padding of the real input rows is not read (until a complex pass has stored there);
-                # inverse: the C2R pass does not store into it
-                is_read = j < len(reads)
-                if (is_read and not inverse) or (not is_read and kind == 3):
-                    assert not pads[r][idx].any(), f"rank {r} step {k} ({st['label']}) touches the padding of a real row"
-                elif not inverse:
-                    pads[r][idx] = False
-            # the fused z + y stage and the batched stage: both listed phases run concurrently (planes / fields apart)
-            two_phase = st["label"].startswith(("zy pass", "yz pass", "batched pass"))
-            if two_phase:
-                groups = batch if st["label"].startswith("batched") else nx
-                grp = np.arange(A0)[:, None, None, None] * groups // A0
-                acc = [(a, i, grp) for a, i, _ in reads + [w[:3] for w in writes]]
-                if prev_acc.get(r) is not None:
-                    _phase_check(r, k, prev_acc[r] + acc, groups)
-                    prev_acc[r] = None if not st["label"].startswith("batched") else acc
-                else:
-                    prev_acc[r] = acc
-            else:
-                prev_acc[r] = None
-            if kind in (0, 1):
-                res = np.fft.ifft(data, axis=2) * N if st["inverse"] else np.fft.fft(data, axis=2)
-            elif kind == 2:
-                res = np.fft.rfft(np.ascontiguousarray(data[..., 0]).view(np.float64), axis=2)[..., None]
-            else:
-                reals = np.fft.irfft(data[..., 0], n=2 * N, axis=2) * (2 * N)
-                res = np.ascontiguousarray(reals).view(np.complex128)[..., None]
-            res = res * st.get("scale", 1.0)
-            for arr, idx, _, ns in writes:
-                pending.append((arr, idx, res[:, :, ns, :], r))
-        for arr, idx, val, who in pending:
-            if isinstance(idx, (int, np.integer)):
-                order.write(who, k, id(arr), arr.size, np.arange(idx, idx + val.size))
-                arr[idx:idx + val.size] = val
-            else:
-                order.write(who, k, id(arr), arr.size, idx)
-                arr[idx] = val
-    worst = 0.0
-    for r in range(P):
-        D = dom[r]
-        if not inverse:
-            assert (bufs[r][pads[r]] == PAD).all()
-        for f in range(batch):
-            if not inverse:
-                osz, ost = lay(r, d)
-                got = bufs[r][f * D:f * D + int(np.prod(osz))].reshape(osz)
-                worst = max(worst, O.rel_l2(got, scale * O.block(specs[f], ost, osz)))
-            else:
-                isz, ist = lay(r, 0)
-                n = float(nz * (ny if d >= 2 else 1) * (nx if d >= 3 else 1))
-                want = O.block(xs[f], ist, isz).astype(np.complex128 if c2c else np.float64)
-                if c2c:
-                    got = bufs[r][f * D:f * D + int(np.prod(isz))].reshape(isz)
-                else:
-                    rows = bufs[r][f * D:f * D + isz[0] * isz[1] * nzc].reshape(-1, nzc)[:, :nz // 2]
-                    got = np.ascontiguousarray(rows).view(np.float64).reshape(isz)
-                worst = max(worst, O.rel_l2(got, scale * n * want))
-    return worst
+    n = float(nz * (ny if d >= 2 else 1) * (nx if d >= 3 else 1))
+    x, want = (specs, [scale * n * x for x in xs]) if inverse else (xs, [scale * s for s in specs])
+    return R.error(R.replay(p, inverse, d, x, mutate=mutate), want)
 
 
 # ---- argument checks ------------------------------------------------------------------------------------------------
@@ -463,3 +259,14 @@ def test_ordering_check_sees_the_buffer(monkeypatch):
     assert run_inplace(2, SL, dfft.C2C, (8, 8, 128), 2, 1, P2P, STREAMS, 0, 3) < 1e-12
     with pytest.raises(AssertionError, match="without"):
         run_inplace(2, SL, dfft.C2C, (8, 8, 128), 2, 1, P2P, STREAMS, 0, 3, mutate=drop_waits)
+
+
+def test_scale_count_catches_a_second_scale():
+    """the replay's count of scalings is not vacuous: a z pass that also applies the scale to what it stores in the
+    buffer scales every output value twice"""
+    def scale_z(scheds):
+        for sc in scheds:
+            sc["steps"][0]["scale"] = 3.0
+    assert run_inplace(1, SL, dfft.C2C, (8, 16, 64), 1, 1, P2P, SYNC, 0, 3, scale=3.0) < 1e-12
+    with pytest.raises(AssertionError, match="scaled 2..2 times"):
+        run_inplace(1, SL, dfft.C2C, (8, 16, 64), 1, 1, P2P, SYNC, 0, 3, scale=3.0, mutate=scale_z)

@@ -1,141 +1,47 @@
 """C2C plans with axis lengths that are not powers of two, without a GPU: length validation, the step lists (Bluestein
 passes carry "n", their "log2n" is log2 M) and CPU replays of every rank's step list on 1-8 ranks.
 
-The replay follows tests/test_scale.py: it runs the geometry-only plans' step lists in lock step with numpy FFTs of the
-length each pass names ("n" when present, else 2^log2n), multiplies the stores of each step by its "scale", checks the
-happens-before order of every slot access, and compares every rank's output with the oracle (times the scale)."""
-import ctypes as C
-import json
-
-import numpy as np
+The replay (step_replay.py) runs the geometry-only plans' step lists in lock step with numpy FFTs of the length each pass
+names ("n" when present, else 2^log2n; "n" only on lengths that are not powers of two, with log2n = log2 M, M >= 2n - 1 >
+M / 2), multiplies the stores of each step by its "scale", checks the happens-before order of every access, and compares
+every rank's output with the oracle (times the scale)."""
 import pytest
 
 import distributedfft_b200 as dfft
+import step_replay as R
 from distributedfft_b200._lib import lib
 from oracle import dft_oracle as O
 
 from test_batch import create
-from test_schedule_emulation import Memory, Ordering, describe, view_indices
+from test_schedule_emulation import describe
 
 SL, ZY, PE = dfft.SLAB_ZY_THEN_X, dfft.SLAB_Z_THEN_YX, dfft.PENCIL
 P2P, A2A = 0, 1
 SYNC, STREAMS = 0, 1
-USER_IN, USER_OUT = 1 << 60, 1 << 61
 DFFT_ERR_UNSUPPORTED = -5
 
 
-def pow2(n):
-    return n >= 2 and n & (n - 1) == 0
+def plan_of(P, decomp, shape, p1, p2, comm, send, batch=1, scale=None, transform=dfft.C2C):
+    return R.Plan(P, decomp, tuple(shape), p1, p2, transform=transform, comm=comm, send=send, batch=batch, scale=scale)
 
 
 def describe_plan(rank, P, decomp, shape, p1, p2, comm, send, inverse, d, batch=1, scale=None, transform=dfft.C2C):
-    rc, msg, c, plan = create(rank, P, decomp, transform, shape, p1, p2, batch, comm, send)
-    assert rc == 0, msg
-    if scale is not None:
-        assert lib().dfft_plan_set_scale(plan, *scale) == 0
-    need = C.c_size_t()
-    assert lib().dfft_plan_describe(plan, inverse, d, None, 0, C.byref(need)) == 0
-    buf = C.create_string_buffer(need.value)
-    assert lib().dfft_plan_describe(plan, inverse, d, buf, need.value, C.byref(need)) == 0
-    lib().dfft_plan_destroy(plan)
-    lib().dfft_comm_destroy(c)
-    return json.loads(buf.value.decode())
+    return R.describe(plan_of(P, decomp, shape, p1, p2, comm, send, batch, scale, transform), rank, inverse, d)
 
 
 def replay(P, decomp, shape, p1, p2, comm, send, inverse, d, batch=1, s=1.0):
     """worst rel-L2 error of every rank's output against the oracle times s"""
     nx, ny, nz = shape
-    sc_ = (1.0, s) if inverse else (s, 1.0)
-    scheds = [describe_plan(r, P, decomp, shape, p1, p2, comm, send, inverse, d, batch, sc_ if s != 1.0 else None) for r in range(P)]
+    p = plan_of(P, decomp, shape, p1, p2, comm, send, batch, None if s == 1.0 else (1.0, s) if inverse else (s, 1.0))
+    scheds = [R.describe(p, r, inverse, d) for r in range(P)]
     for sc in scheds:
         assert not sc["overlapped"]
-        for st in sc["steps"]:
-            if st["type"] != 0:
-                continue
-            n = st.get("n", 1 << st["log2n"])
-            assert n in shape
-            # "n" exactly on the passes whose length is not a power of two, with log2n = log2 M, M >= 2n - 1 > M / 2
-            assert ("n" in st) == (not pow2(n))
-            if "n" in st:
-                M = 1 << st["log2n"]
-                assert 2 * n - 1 <= M < 4 * n - 2
-    es = scheds[0]["esize"]
-    lay = lambda r, w: dfft.layout(decomp, dfft.C2C, nx, ny, nz, p1, p2, r, w)
+        assert all(st.get("n", 1 << st.get("log2n", 0)) in shape for st in sc["steps"] if st["type"] == 0)
     xs = [O.complex_input(shape, seed=31 + f) for f in range(batch)]
     specs = [O.fft_c2c(x, d) for x in xs]
-    mem = Memory(es)
-    for r in range(P):
-        for k in range(scheds[r]["nslots"]):
-            mem.add(scheds[r]["slots"][k][r], scheds[r]["slot_bytes"] // es)
-    uout, fout = [], []
-    for r in range(P):
-        isz, ist = lay(r, 0)
-        osz, ost = lay(r, d)
-        nin, nout = int(np.prod(isz)), int(np.prod(osz))
-        fi, fo = (nout, nin) if inverse else (nin, nout)
-        fout.append(fo)
-        a = mem.add(USER_IN + (r << 48), batch * fi)
-        uout.append(mem.add(USER_OUT + (r << 48), batch * fo))
-        for f in range(batch):
-            src = O.block(xs[f], ist, isz) if not inverse else O.block(specs[f], ost, osz)
-            a[f * fi:(f + 1) * fi] = np.ascontiguousarray(src).astype(np.complex128).ravel()
-    nsteps = len(scheds[0]["steps"])
-    assert all(len(sc["steps"]) == nsteps for sc in scheds)
-    order = Ordering(scheds)
-    for k in range(nsteps):
-        pending = []
-        for r in range(P):
-            st = scheds[r]["steps"][k]
-            if st["type"] == 1:
-                continue
-            if st["type"] == 2:
-                sb = scheds[r]["slots"][st["send_slot"]][r]
-                for peer in st["peers"]:
-                    q = peer["rank"]
-                    rb = scheds[q]["slots"][st["recv_slot"]][q]
-                    mine = [pp for pp in scheds[q]["steps"][k]["peers"] if pp["rank"] == r][0]
-                    src, so = mem.resolve(sb + peer["soff"] * es)
-                    dst, do = mem.resolve(rb + mine["roff"] * es)
-                    order.read(r, k, id(src), src.size, np.arange(so, so + peer["scount"]))
-                    pending.append((dst, do, src[so:so + peer["scount"]].copy(), q))
-                continue
-            assert st["kind"] in (0, 1)
-            N = st.get("n", 1 << st["log2n"])
-            A0, A1, B = st["A0"], st["A1"], st["B"]
-            ub_in = {1: USER_IN + (r << 48), 2: USER_OUT + (r << 48)}.get(st["in_user"])
-            ub_out = USER_OUT + (r << 48) if st["out_user"] == 2 else None
-            data = np.zeros((A0, A1, N, B), dtype=np.complex128)
-            for base, ns, off in view_indices(st["in"], A0, A1, N, B, ub_in):
-                arr, o = mem.resolve(base)
-                data[:, :, ns, :] = arr[o + off]
-                order.read(r, k, id(arr), arr.size, o + off)
-            res = np.fft.ifft(data, axis=2) * N if st["inverse"] else np.fft.fft(data, axis=2)
-            res = res * st.get("scale", 1.0)
-            for base, ns, off in view_indices(st["out"], A0, A1, N, B, ub_out):
-                arr, o = mem.resolve(base)
-                pending.append((arr, o + off, res[:, :, ns, :], r))
-                if "scale" in st:
-                    assert ub_out is not None, "only stores into the caller's output are scaled"
-        for arr, idx, val, who in pending:
-            if isinstance(idx, (int, np.integer)):
-                order.write(who, k, id(arr), arr.size, np.arange(idx, idx + val.size))
-                arr[idx:idx + val.size] = val
-            else:
-                order.write(who, k, id(arr), arr.size, idx)
-                arr[idx] = val
-    worst = 0.0
-    for r in range(P):
-        for f in range(batch):
-            if not inverse:
-                osz, ost = lay(r, d)
-                got = uout[r][f * fout[r]:f * fout[r] + int(np.prod(osz))].reshape(osz)
-                worst = max(worst, O.rel_l2(got, s * O.block(specs[f], ost, osz)))
-            else:
-                isz, ist = lay(r, 0)
-                n = float(nz * (ny if d >= 2 else 1) * (nx if d >= 3 else 1))
-                got = uout[r][f * fout[r]:(f + 1) * fout[r]].reshape(isz)
-                worst = max(worst, O.rel_l2(got, s * n * O.block(xs[f], ist, isz)))
-    return worst
+    n = float(nz * (ny if d >= 2 else 1) * (nx if d >= 3 else 1))
+    x, want = (specs, [s * n * x for x in xs]) if inverse else (xs, [s * sp for sp in specs])
+    return R.error(R.replay(p, inverse, d, x, scheds), want)
 
 
 CASES = [

@@ -12,14 +12,14 @@ import numpy as np
 import pytest
 
 import distributedfft_b200 as dfft
+import step_replay as R
 from distributedfft_b200 import _lib
 from distributedfft_b200._lib import check, lib
-from test_schedule_emulation import Memory, Ordering, view_indices
+from step_replay import describe_raw, layouts, positions
 
 SL, ZY, PE = dfft.SLAB_ZY_THEN_X, dfft.SLAB_Z_THEN_YX, dfft.PENCIL
 C2C, R2C, DCT, DST, R2HC = dfft.C2C, dfft.R2C, dfft.DCT, dfft.DST, dfft.R2HC
 P2P, A2A = 0, 1
-USER_IN, USER_OUT = 1 << 60, 1 << 61
 ERR_INVALID, ERR_UNSUPPORTED = -1, -5
 
 
@@ -29,11 +29,8 @@ def err():
 
 def create(rank, P, decomp, transform, shape, spec, p1, p2, comm=P2P, batch=1, prec=dfft.F64):
     """dry padded plan: (rc, comm, plan); plan is None when the creator refused"""
-    c = C.c_void_p()
-    check(lib().dfft_comm_create_dry(rank, P, C.byref(c)))
-    cfg = _lib.dfft_config(1, 0, comm, 0, None, comm, 0)
-    plan = C.c_void_p()
-    rc = lib().dfft_plan_create_padded(c, C.byref(cfg), decomp, prec, transform, *shape, *spec, p1, p2, batch, 1, C.byref(plan))
+    p = R.Plan(P, decomp, tuple(shape), p1, p2, transform=transform, prec=prec, comm=comm, batch=batch, spectral=tuple(spec))
+    rc, _, c, plan = R.create(p, rank)
     return rc, c, (plan if rc == 0 else None)
 
 
@@ -43,35 +40,7 @@ def destroy(c, plan):
     lib().dfft_comm_destroy(c)
 
 
-def describe_raw(plan, inverse, d):
-    need = C.c_size_t()
-    check(lib().dfft_plan_describe(plan, inverse, d, None, 0, C.byref(need)))
-    buf = C.create_string_buffer(need.value)
-    check(lib().dfft_plan_describe(plan, inverse, d, buf, need.value, C.byref(need)))
-    return buf.value.decode()
-
-
-def layouts(plan):
-    """[(size, start)] of layouts 0..3 of this rank"""
-    out = []
-    for w in range(4):
-        s, o = (C.c_size_t * 3)(), (C.c_size_t * 3)()
-        if w == 0:
-            check(lib().dfft_get_in_size(plan, s)); check(lib().dfft_get_in_start(plan, o))
-        else:
-            check(lib().dfft_get_partial_size(plan, w, s)); check(lib().dfft_get_partial_start(plan, w, o))
-        out.append(([int(v) for v in s], [int(v) for v in o]))
-    return out
-
-
 # ---- index map ------------------------------------------------------------------------------------------------------------
-def positions(n, k, half=False):
-    """line positions of the k kept spectral indices of an n-point axis (half: the R2C z axis, k modes kept of n/2+1)"""
-    if half:
-        return np.arange(k // 2 + 1)
-    return np.fft.fftfreq(k, 1.0 / k).astype(np.int64) % n
-
-
 def fwd_ref(x, transform, spec, d):
     for axis in (2, 1, 0)[:d]:
         half = transform == R2C and axis == 2
@@ -97,122 +66,22 @@ def inv_ref(X, transform, shape, spec, d):
 
 
 # ---- replay ---------------------------------------------------------------------------------------------------------------
-def replay(P, decomp, transform, shape, spec, p1, p2, inverse, d, comm=P2P, batch=1, scale=None):
+def replay(P, decomp, transform, shape, spec, p1, p2, inverse, d, comm=P2P, batch=1, scale=None, mutate=None):
     """replays every rank's steps in lock step; returns the worst rel-L2 error of any rank's output block"""
-    scheds, lays = [], []
-    for r in range(P):
-        rc, c, plan = create(r, P, decomp, transform, shape, spec, p1, p2, comm, batch)
-        assert rc == 0, err()
-        if scale is not None:
-            check(lib().dfft_plan_set_scale(plan, *scale))
-        sc = json.loads(describe_raw(plan, inverse, d))
-        sc["domain_bytes"] = lib().dfft_get_domain_size(plan)
-        scheds.append(sc)
-        lays.append(layouts(plan))
-        destroy(c, plan)
-    r2c = transform == R2C
-    es = scheds[0]["esize"]
+    p = R.Plan(P, decomp, tuple(shape), p1, p2, transform=transform, comm=comm, batch=batch, spectral=tuple(spec), scale=scale)
+    scheds = [R.describe(p, r, inverse, d) for r in range(P)]
     padded = tuple(spec) != tuple(shape)
     assert not scheds[0]["overlapped"]
     assert ("spectral" in scheds[0]) == padded and (not padded or scheds[0]["spectral"] == list(spec))
     rng = np.random.default_rng(sum(shape) + 7 * sum(spec) + P + 3 * d + inverse)
-    if r2c:
+    if transform == R2C:
         xg = rng.standard_normal((batch,) + shape)
     else:
         xg = rng.standard_normal((batch,) + shape) + 1j * rng.standard_normal((batch,) + shape)
     spec_g = np.stack([fwd_ref(xg[f], transform, spec, d) for f in range(batch)])
-    src_g = spec_g if inverse else xg
     want_g = np.stack([inv_ref(spec_g[f], transform, shape, spec, d) for f in range(batch)]) if inverse else spec_g
     s_used = 1.0 if scale is None else scale[1 if inverse else 0]
-    mem = Memory(es)
-    for r in range(P):
-        for s_ in range(scheds[r]["nslots"]):
-            mem.add(scheds[r]["slots"][s_][r], scheds[r]["slot_bytes"] // es)
-    src_w, dst_w = (d, 0) if inverse else (0, d)
-    real_in, real_out = r2c and not inverse, r2c and bool(inverse)
-    uout = []
-    for r in range(P):
-        (isz, ist), (osz, ost) = lays[r][src_w], lays[r][dst_w]
-        ni = int(np.prod(isz)) // (2 if real_in else 1)
-        no = int(np.prod(osz)) // (2 if real_out else 1)
-        fi, fo = (scheds[r]["field_in"] // es, scheds[r]["field_out"] // es) if batch > 1 else (ni, no)
-        a = mem.add(USER_IN + (r << 48), max(batch * max(fi, ni), 1))
-        for f in range(batch):
-            blk = np.ascontiguousarray(src_g[f][ist[0]:ist[0] + isz[0], ist[1]:ist[1] + isz[1], ist[2]:ist[2] + isz[2]]).ravel()
-            a[f * fi:f * fi + ni] = blk.view(np.complex128) if real_in else blk
-        uout.append((mem.add(USER_OUT + (r << 48), max(batch * max(fo, no), 1)), fo, no))
-    nsteps = len(scheds[0]["steps"])
-    assert all(len(s["steps"]) == nsteps for s in scheds)
-    order = Ordering(scheds)
-    holes = 0
-    for k in range(nsteps):
-        pending = []
-        for r in range(P):
-            st = scheds[r]["steps"][k]
-            if st["type"] == 1:
-                continue
-            if st["type"] == 2:
-                sb = scheds[r]["slots"][st["send_slot"]][r]
-                for peer in st["peers"]:
-                    q = peer["rank"]
-                    rb = scheds[q]["slots"][st["recv_slot"]][q]
-                    mine = [pp for pp in scheds[q]["steps"][k]["peers"] if pp["rank"] == r][0]
-                    assert mine["rcount"] == peer["scount"]
-                    src, so = mem.resolve(sb + peer["soff"] * es)
-                    dst, do = mem.resolve(rb + mine["roff"] * es)
-                    order.read(r, k, id(src), src.size, np.arange(so, so + peer["scount"]))
-                    pending.append((dst, np.arange(do, do + peer["scount"]), src[so:so + peer["scount"]].copy(), q))
-                continue
-            kind = st["kind"]
-            assert kind in (0, 1, 2, 3), st
-            N = 1 << st["log2n"]
-            A0, A1, B = st["A0"], st["A1"], st["B"]
-            ub_in = USER_IN + (r << 48) if st["in_user"] == 1 else None
-            ub_out = USER_OUT + (r << 48) if st["out_user"] == 2 else None
-            n_in, n_out = (N + 1, N) if kind == 3 else (N, N + 1) if kind == 2 else (N, N)
-            keep = st.get("keep")
-            if keep is not None:
-                holes += 1
-                assert 1 <= keep < (N + 1 if kind in (2, 3) else N)
-            # the spectral side: out forward, in inverse
-            kin = keep if keep is not None and st["inverse"] else n_in
-            kout = keep if keep is not None and not st["inverse"] else n_out
-            data = np.zeros((A0, A1, kin, B), dtype=np.complex128)
-            for base, ns, off in view_indices(st["in"], A0, A1, kin, B, ub_in):
-                arr, o = mem.resolve(base)
-                data[:, :, ns, :] = arr[o + off]
-                order.read(r, k, id(arr), arr.size, o + off)
-            if kin != n_in:
-                full = np.zeros((A0, A1, n_in, B), dtype=np.complex128)
-                full[:, :, positions(N, kin) if kind != 3 else np.arange(kin), :] = data
-                data = full
-            if kind == 2:
-                res = np.fft.rfft(np.ascontiguousarray(data[..., 0]).view(np.float64), axis=2)[..., None]
-            elif kind == 3:
-                res = np.ascontiguousarray(np.fft.irfft(data[..., 0], n=2 * N, axis=2) * (2 * N)).view(np.complex128)[..., None]
-            else:
-                res = np.fft.ifft(data, axis=2) * N if st["inverse"] else np.fft.fft(data, axis=2)
-            if kout != n_out:
-                res = res[:, :, positions(N, kout) if kind != 2 else np.arange(kout), :]
-            if "scale" in st:
-                res = res * st["scale"]
-            for base, ns, off in view_indices(st["out"], A0, A1, kout, B, ub_out):
-                arr, o = mem.resolve(base)
-                pending.append((arr, o + off, res[:, :, ns, :], r))
-        for arr, idx, val, who in pending:
-            order.write(who, k, id(arr), arr.size, idx)
-            arr[idx] = val
-    assert holes > 0 or not padded or d < 3 and all(spec[a] == shape[a] for a in (2, 1, 0)[:d])
-    worst = 0.0
-    for r in range(P):
-        osz, ost = lays[r][dst_w]
-        arr, fo, no = uout[r]
-        for f in range(batch):
-            got = arr[f * fo:f * fo + no]
-            got = (got.view(np.float64) if real_out else got).reshape(osz)
-            want = want_g[f][ost[0]:ost[0] + osz[0], ost[1]:ost[1] + osz[1], ost[2]:ost[2] + osz[2]] * s_used
-            worst = max(worst, float(np.linalg.norm(got - want) / max(np.linalg.norm(want), 1e-300)))
-    return worst
+    return R.error(R.replay(p, inverse, d, spec_g if inverse else xg, scheds, mutate), want_g * s_used)
 
 
 # ---- validation -----------------------------------------------------------------------------------------------------------
@@ -365,3 +234,18 @@ def test_replay_batch_scale_uneven_tails(P, decomp, p1, p2, inverse):
     for transform in (C2C, R2C):
         assert replay(P, decomp, transform, (16, 32, 128), (11, 21, 85), p1, p2, inverse, 3, P2P, batch=3, scale=(0.25, 1.0 / 3.0)) < 1e-12
 
+
+def drop_rendezvous(scheds):
+    """schedule mutation: remove every rendezvous but the entry one"""
+    for sc in scheds:
+        sc["steps"] = [st for st in sc["steps"] if st["type"] != 1 or st["group"] == 0]
+
+
+@pytest.mark.parametrize("inverse", [0, 1])
+def test_slot_rule_catches_a_missing_rendezvous(inverse):
+    """the replay's slot rule holds padded plans too: without the rendezvous of its transpositions, a pass reads a slot that
+    a peer stored into"""
+    case = (4, SL, C2C, (16, 32, 64), (11, 21, 43), 4, 1, inverse, 3)
+    assert replay(*case) < 1e-12
+    with pytest.raises(AssertionError, match="without a rendezvous"):
+        replay(*case, mutate=drop_rendezvous)

@@ -7,8 +7,8 @@
 - Lock-step replays of every rank's step list (dfft_plan_describe) with scipy's DCT / DST per pass over the reals of the
   views, checked against scipy.fft.dctn / dstn of the global array: 1-8 ranks, slab, Z_Then_YX and pencil grids, Peer2Peer
   and All2All, partial d, uneven splits with odd column counts, blocked hand-over layouts, batches, in-place plans and
-  output scales (applied exactly once).  Each replay also checks the happens-before order of every access
-  (test_schedule_emulation.Ordering)."""
+  output scales (applied exactly once).  Each replay (step_replay.py) also checks the happens-before order of every
+  access."""
 import ctypes as C
 import os
 import subprocess
@@ -19,16 +19,14 @@ import pytest
 import scipy.fft as sf
 
 import distributedfft_b200 as dfft
-from distributedfft_b200 import _lib
 from distributedfft_b200._lib import check, lib
+import step_replay as R
 from test_inplace import describe
-from test_schedule_emulation import Memory, Ordering, view_indices
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SL, ZY, PE = dfft.SLAB_ZY_THEN_X, dfft.SLAB_Z_THEN_YX, dfft.PENCIL
 P2P, A2A = 0, 1
 SYNC, STREAMS = 0, 1
-USER_IN, USER_OUT = 1 << 60, 1 << 61
 
 
 def test_r2r_kernel_math_matches_naive():
@@ -103,102 +101,20 @@ def global_ref(x, transform, inverse, d):
     return f(x, type=3 if inverse else 2, axes={1: (2,), 2: (1, 2), 3: (0, 1, 2)}[d])
 
 
-class RealMemory(Memory):
-    def add(self, base, nelem):
-        arr = np.zeros(nelem, dtype=np.float64)
-        self.regions.append((base, arr))
-        return arr
-
-
 def run_r2r(P, decomp, transform, shape, p1, p2, comm, send, inverse, d, batch=1, inplace=False, scale=None, prec=dfft.F64):
     """replays every rank's steps in lock step; returns the worst rel-L2 error of any rank's output block"""
     nx, ny, nz = shape
-    scheds = [describe(r, P, decomp, transform, shape, p1, p2, comm, send, inverse, d, batch=batch, prec=prec, scale=scale, inplace=inplace)
-              for r in range(P)]
-    es = scheds[0]["esize"]
-    assert es == (8 if prec == dfft.F64 else 4) and not scheds[0]["overlapped"]
-    lay = lambda r, w: dfft.layout(decomp, transform, nx, ny, nz, p1, p2, r, w)
+    p = R.Plan(P, decomp, tuple(shape), p1, p2, transform=transform, prec=prec, comm=comm, send=send, batch=batch, inplace=inplace, scale=scale)
+    scheds = [R.describe(p, r, inverse, d) for r in range(P)]
+    assert not scheds[0]["overlapped"]
     rng = np.random.default_rng(P * 1000 + nx + ny + nz + batch)
     xg = rng.standard_normal((batch,) + shape)
     spec = np.stack([global_ref(xg[f], transform, False, d) for f in range(batch)])
-    src_g = spec if inverse else xg
     want_g = np.stack([global_ref(spec[f], transform, True, d) for f in range(batch)]) if inverse else spec
     s_used = 1.0 if scale is None else scale[1 if inverse else 0]
     if prec == dfft.F32:
         s_used = float(np.float32(s_used))
-    mem = RealMemory(es)
-    for r in range(P):
-        for s_ in range(scheds[r]["nslots"]):
-            mem.add(scheds[r]["slots"][s_][r], scheds[r]["slot_bytes"] // es)
-    src_w, dst_w = (d, 0) if inverse else (0, d)
-    uin, uout = [], []
-    for r in range(P):
-        isz, ist = lay(r, src_w)
-        osz, ost = lay(r, dst_w)
-        ni, no = int(np.prod(isz)), int(np.prod(osz))
-        fi = scheds[r]["domain_bytes"] // es if inplace else ni
-        fo = scheds[r]["domain_bytes"] // es if inplace else no
-        a = mem.add(USER_IN + (r << 48), batch * fi)
-        for f in range(batch):
-            a[f * fi:f * fi + ni] = src_g[f][ist[0]:ist[0] + isz[0], ist[1]:ist[1] + isz[1], ist[2]:ist[2] + isz[2]].ravel()
-        uin.append((a, fi))
-        uout.append((a, fo) if inplace else (mem.add(USER_OUT + (r << 48), batch * fo), fo))
-    nsteps = len(scheds[0]["steps"])
-    assert all(len(s["steps"]) == nsteps for s in scheds)
-    order = Ordering(scheds)
-    scaled = {}  # output array -> how often each element was scaled
-    for k in range(nsteps):
-        pending = []
-        for r in range(P):
-            st = scheds[r]["steps"][k]
-            if st["type"] == 1:
-                continue
-            if st["type"] == 2:
-                sb = scheds[r]["slots"][st["send_slot"]][r]
-                for peer in st["peers"]:
-                    q = peer["rank"]
-                    rb = scheds[q]["slots"][st["recv_slot"]][q]
-                    mine = [pp for pp in scheds[q]["steps"][k]["peers"] if pp["rank"] == r][0]
-                    assert mine["rcount"] == peer["scount"]
-                    src, so = mem.resolve(sb + peer["soff"] * es)
-                    dst, do = mem.resolve(rb + mine["roff"] * es)
-                    order.read(r, k, id(src), src.size, np.arange(so, so + peer["scount"]))
-                    pending.append((dst, np.arange(do, do + peer["scount"]), src[so:so + peer["scount"]].copy(), q))
-                continue
-            assert st["kind"] in (4, 5), st["kind"]
-            N, A0, A1, B = 1 << st["log2n"], st["A0"], st["A1"], st["B"]
-            ub_in = USER_IN + (r << 48) if st["in_user"] else None
-            ub_out = (USER_IN if inplace else USER_OUT) + (r << 48) if st["out_user"] == 2 else None
-            data = np.zeros((A0, A1, N, B))
-            for base, ns, off in view_indices(st["in"], A0, A1, N, B, ub_in):
-                arr, o = mem.resolve(base)
-                data[:, :, ns, :] = arr[o + off]
-                order.read(r, k, id(arr), arr.size, o + off)
-            res = scipy_r2r(data, transform, st["inverse"], 2)
-            if "scale" in st:
-                res = res * st["scale"]
-            for base, ns, off in view_indices(st["out"], A0, A1, N, B, ub_out):
-                arr, o = mem.resolve(base)
-                pending.append((arr, o + off, res[:, :, ns, :], r))
-                if "scale" in st:
-                    scaled.setdefault(id(arr), np.zeros(arr.size, dtype=np.int64))
-                    np.add.at(scaled[id(arr)], (o + off).ravel(), 1)
-        for arr, idx, val, who in pending:
-            order.write(who, k, id(arr), arr.size, idx)
-            arr[idx] = val
-    worst = 0.0
-    for r in range(P):
-        osz, ost = lay(r, dst_w)
-        arr, fo = uout[r]
-        no = int(np.prod(osz))
-        for f in range(batch):
-            got = arr[f * fo:f * fo + no].reshape(osz)
-            want = want_g[f][ost[0]:ost[0] + osz[0], ost[1]:ost[1] + osz[1], ost[2]:ost[2] + osz[2]] * s_used
-            worst = max(worst, float(np.linalg.norm(got - want) / np.linalg.norm(want)))
-            if scale is not None and s_used != 1.0:
-                cnt = scaled[id(arr)][f * fo:f * fo + no]
-                assert (cnt == 1).all(), f"rank {r} field {f}: an output value is scaled {int(cnt.min())}..{int(cnt.max())} times"
-    return worst
+    return R.error(R.replay(p, inverse, d, spec if inverse else xg, scheds), want_g * s_used)
 
 
 CASES = [

@@ -9,9 +9,8 @@
   the per-axis transform of the global array: 1-8 ranks, slab, Z_Then_YX and pencil, Peer2Peer and All2All, both
   directions, partial d, uneven splits, blocked layouts with tails, type-I / type-II / R2HC mixes, kept axes, batches,
   in-place plans and output scales (applied exactly once), with the happens-before check of every access
-  (test_schedule_emulation.Ordering)."""
+  (step_replay.py)."""
 import ctypes as C
-import json
 import os
 import subprocess
 import tempfile
@@ -22,18 +21,16 @@ import scipy.fft as sf
 
 import distributedfft_b200 as dfft
 from distributedfft_b200._lib import check, lib
-from test_r2r import CASES, RealMemory
-from test_r2r_mixed import create_plain, create_r2r, describe_raw, destroy, hc2r, r2hc
-from test_schedule_emulation import Ordering, view_indices
+import step_replay as R
+from test_r2r import CASES
+from test_r2r_mixed import create_plain, create_r2r, destroy, hc2r, r2hc
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SL, ZY, PE = dfft.SLAB_ZY_THEN_X, dfft.SLAB_Z_THEN_YX, dfft.PENCIL
 P2P, A2A = 0, 1
 SYNC, STREAMS = 0, 1
-USER_IN, USER_OUT = 1 << 60, 1 << 61
 DCT, DST, R2HC, DCT1, DST1 = dfft.DCT, dfft.DST, dfft.R2HC, dfft.DCT1, dfft.DST1
 NAMES = {DCT: "dct", DST: "dst", R2HC: "r2hc", DCT1: "dct1", DST1: "dst1"}
-KIND_OF = {v: k for k, v in NAMES.items()}
 
 
 def test_r2r1_kernel_math_matches_naive():
@@ -160,17 +157,12 @@ def test_get_r2r_kinds():
         destroy(c, plan)
 
 
+def plan_of(P, decomp, kinds, shape, p1, p2, comm, send, batch=1, prec=dfft.F64, scale=None, inplace=False, taxes=None):
+    return R.Plan(P, decomp, tuple(shape), p1, p2, kinds=kinds, prec=prec, comm=comm, send=send, batch=batch, inplace=inplace, scale=scale, axes=taxes)
+
+
 def describe(rank, P, decomp, kinds, shape, p1, p2, comm, send, inverse, d, batch=1, prec=dfft.F64, scale=None, inplace=False, taxes=None):
-    rc, c, plan = create_r2r(rank, P, decomp, kinds, shape, p1, p2, comm, send, batch, inplace, prec)
-    assert rc == 0, (lib().dfft_last_error_string() or b"").decode()
-    if taxes is not None:
-        assert lib().dfft_plan_set_transform_axes(plan, (C.c_int * 3)(*taxes)) == 0
-    if scale is not None:
-        assert lib().dfft_plan_set_scale(plan, *scale) == 0
-    sc = json.loads(describe_raw(plan, inverse, d))
-    sc["domain_bytes"] = lib().dfft_get_domain_size(plan)
-    destroy(c, plan)
-    return sc
+    return R.describe(plan_of(P, decomp, kinds, shape, p1, p2, comm, send, batch, prec, scale, inplace, taxes), rank, inverse, d)
 
 
 @pytest.mark.parametrize("kinds", [(DCT1, R2HC, R2HC), (DST1, DST1, DST1), (DCT1, DST, DST1), (DCT1, DCT1, DCT1)],
@@ -199,101 +191,22 @@ def test_describe(kinds):
 # ---- lock-step replay ---------------------------------------------------------------------------------------------------
 def run_type1(P, decomp, kinds, shape, p1, p2, comm, send, inverse, d, batch=1, inplace=False, scale=None, prec=dfft.F64, taxes=None):
     """replays every rank's steps in lock step, each pass with the kind its description names and the length "n" of
-    type-I passes; returns the worst rel-L2 error of any rank's output block against the per-axis global transform"""
+    type-I passes; returns the worst rel-L2 error of any rank's output block against the per-axis global transform, and
+    whether a type-I pass ran"""
     nx, ny, nz = shape
-    scheds = [describe(r, P, decomp, kinds, shape, p1, p2, comm, send, inverse, d, batch=batch, prec=prec, scale=scale, inplace=inplace,
-                       taxes=taxes) for r in range(P)]
-    es = scheds[0]["esize"]
-    assert es == (8 if prec == dfft.F64 else 4) and not scheds[0]["overlapped"]
-    lay = lambda r, w: dfft.layout(decomp, DCT, nx, ny, nz, p1, p2, r, w)
+    p = plan_of(P, decomp, kinds, shape, p1, p2, comm, send, batch, prec, scale, inplace, taxes)
+    scheds = [R.describe(p, r, inverse, d) for r in range(P)]
+    assert not scheds[0]["overlapped"]
     ta = taxes or (1, 1, 1)
     rng = np.random.default_rng(P * 1000 + nx + ny + nz + batch + 7 * kinds[0] + 3 * kinds[1] + kinds[2])
     xg = rng.standard_normal((batch,) + shape)
     spec = np.stack([global_ref(xg[f], kinds, False, d, ta) for f in range(batch)])
-    src_g = spec if inverse else xg
     want_g = np.stack([global_ref(spec[f], kinds, True, d, ta) for f in range(batch)]) if inverse else spec
     s_used = 1.0 if scale is None else scale[1 if inverse else 0]
     if prec == dfft.F32:
         s_used = float(np.float32(s_used))
-    mem = RealMemory(es)
-    for r in range(P):
-        for s_ in range(scheds[r]["nslots"]):
-            mem.add(scheds[r]["slots"][s_][r], scheds[r]["slot_bytes"] // es)
-    src_w, dst_w = (d, 0) if inverse else (0, d)
-    uout = []
-    for r in range(P):
-        isz, ist = lay(r, src_w)
-        osz, ost = lay(r, dst_w)
-        ni, no = int(np.prod(isz)), int(np.prod(osz))
-        fi = scheds[r]["domain_bytes"] // es if inplace else ni
-        fo = scheds[r]["domain_bytes"] // es if inplace else no
-        a = mem.add(USER_IN + (r << 48), batch * fi)
-        for f in range(batch):
-            a[f * fi:f * fi + ni] = src_g[f][ist[0]:ist[0] + isz[0], ist[1]:ist[1] + isz[1], ist[2]:ist[2] + isz[2]].ravel()
-        uout.append((a, fo) if inplace else (mem.add(USER_OUT + (r << 48), batch * fo), fo))
-    nsteps = len(scheds[0]["steps"])
-    assert all(len(s["steps"]) == nsteps for s in scheds)
-    order = Ordering(scheds)
-    scaled = {}  # output array -> how often each element was scaled
-    seen_type1 = False
-    for k in range(nsteps):
-        pending = []
-        for r in range(P):
-            st = scheds[r]["steps"][k]
-            if st["type"] == 1:
-                continue
-            if st["type"] == 2:
-                sb = scheds[r]["slots"][st["send_slot"]][r]
-                for peer in st["peers"]:
-                    q = peer["rank"]
-                    rb = scheds[q]["slots"][st["recv_slot"]][q]
-                    mine = [pp for pp in scheds[q]["steps"][k]["peers"] if pp["rank"] == r][0]
-                    assert mine["rcount"] == peer["scount"]
-                    src, so = mem.resolve(sb + peer["soff"] * es)
-                    dst, do = mem.resolve(rb + mine["roff"] * es)
-                    order.read(r, k, id(src), src.size, np.arange(so, so + peer["scount"]))
-                    pending.append((dst, np.arange(do, do + peer["scount"]), src[so:so + peer["scount"]].copy(), q))
-                continue
-            copy = st["kind"] in (6, 7)
-            assert st["kind"] in (4, 5) or copy, st["kind"]
-            N = st["n"] if "n" in st else 1 << st["log2n"]
-            A0, A1, B = st["A0"], st["A1"], st["B"]
-            ub_in = USER_IN + (r << 48) if st["in_user"] else None
-            ub_out = (USER_IN if inplace else USER_OUT) + (r << 48) if st["out_user"] == 2 else None
-            data = np.zeros((A0, A1, N, B))
-            for base, ns, off in view_indices(st["in"], A0, A1, N, B, ub_in):
-                arr, o = mem.resolve(base)
-                data[:, :, ns, :] = arr[o + off]
-                order.read(r, k, id(arr), arr.size, o + off)
-            if copy:
-                res = data
-            else:
-                kind = KIND_OF[st["r2r"]]
-                seen_type1 |= kind in (DCT1, DST1)
-                res = r2r_1d(data, kind, st["inverse"], 2)
-            if "scale" in st:
-                res = res * st["scale"]
-            for base, ns, off in view_indices(st["out"], A0, A1, N, B, ub_out):
-                arr, o = mem.resolve(base)
-                pending.append((arr, o + off, res[:, :, ns, :], r))
-                if "scale" in st:
-                    scaled.setdefault(id(arr), np.zeros(arr.size, dtype=np.int64))
-                    np.add.at(scaled[id(arr)], (o + off).ravel(), 1)
-        for arr, idx, val, who in pending:
-            order.write(who, k, id(arr), arr.size, idx)
-            arr[idx] = val
-    worst = 0.0
-    for r in range(P):
-        osz, ost = lay(r, dst_w)
-        arr, fo = uout[r]
-        no = int(np.prod(osz))
-        for f in range(batch):
-            got = arr[f * fo:f * fo + no].reshape(osz)
-            want = want_g[f][ost[0]:ost[0] + osz[0], ost[1]:ost[1] + osz[1], ost[2]:ost[2] + osz[2]] * s_used
-            worst = max(worst, float(np.linalg.norm(got - want) / np.linalg.norm(want)))
-            if scale is not None and s_used != 1.0:
-                cnt = scaled[id(arr)][f * fo:f * fo + no]
-                assert (cnt == 1).all(), f"rank {r} field {f}: an output value is scaled {int(cnt.min())}..{int(cnt.max())} times"
+    worst = R.error(R.replay(p, inverse, d, spec if inverse else xg, scheds), want_g * s_used)
+    seen_type1 = any(st.get("r2r") in ("dct1", "dst1") for sc in scheds for st in sc["steps"] if st["type"] == 0)
     return worst, seen_type1
 
 

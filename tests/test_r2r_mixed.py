@@ -9,10 +9,9 @@
   lengths and a cubic grid with three different kinds, 1-8 ranks, slab, Z_Then_YX and pencil, Peer2Peer and All2All,
   Streams (still the sequential schedule), partial d, the odd column counts of test_r2r's cases, blocked layouts with
   tails, batches, in-place plans and output scales (applied exactly once), with the happens-before check of every access
-  (test_schedule_emulation.Ordering)."""
+  (step_replay.py)."""
 import ctypes as C
 import itertools
-import json
 import os
 import subprocess
 import tempfile
@@ -24,14 +23,14 @@ import scipy.fft as sf
 import distributedfft_b200 as dfft
 from distributedfft_b200 import _lib
 from distributedfft_b200._lib import check, lib
-from test_r2r import CASES, RealMemory
-from test_schedule_emulation import Ordering, view_indices
+import step_replay as R
+from step_replay import hc2r, r2hc
+from test_r2r import CASES
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SL, ZY, PE = dfft.SLAB_ZY_THEN_X, dfft.SLAB_Z_THEN_YX, dfft.PENCIL
 P2P, A2A = 0, 1
 SYNC, STREAMS = 0, 1
-USER_IN, USER_OUT = 1 << 60, 1 << 61
 DCT, DST, R2HC = dfft.DCT, dfft.DST, dfft.R2HC
 NAMES = {DCT: "dct", DST: "dst", R2HC: "r2hc"}
 ALL_KINDS = list(itertools.product((DCT, DST, R2HC), repeat=3))
@@ -47,25 +46,7 @@ def test_r2hc_kernel_math_matches_naive():
         assert "fails=0" in r.stdout
 
 
-# ---- numpy references: FFTW's halfcomplex format and the per-axis transforms ----------------------------------------------
-def r2hc(x, axis):
-    """hc = [Re X_0 .. Re X_{N/2}, Im X_{N/2-1} .. Im X_1] along axis, X = rfft(x)"""
-    n = x.shape[axis]
-    X = np.fft.rfft(x, axis=axis)
-    return np.concatenate([X.real, np.take(X.imag, np.arange(n // 2 - 1, 0, -1), axis=axis)], axis=axis)
-
-
-def hc2r(h, axis):
-    """the unnormalised inverse: hc2r(r2hc(x)) = N x"""
-    n = h.shape[axis]
-    re = np.take(h, np.arange(n // 2 + 1), axis=axis)
-    im = np.zeros_like(re)
-    idx = [slice(None)] * h.ndim
-    idx[axis] = slice(1, n // 2)
-    im[tuple(idx)] = np.take(h, np.arange(n - 1, n // 2, -1), axis=axis)
-    return np.fft.irfft(re + 1j * im, n=n, axis=axis) * n
-
-
+# ---- numpy references: the per-axis transforms (FFTW's halfcomplex format: step_replay.r2hc / hc2r) ----------------------------------------------
 def r2r_1d(x, kind, inverse, axis):
     if kind == R2HC:
         return hc2r(x, axis) if inverse else r2hc(x, axis)
@@ -126,14 +107,8 @@ def describe_raw(plan, inverse, d):
 
 
 def describe(rank, P, decomp, kinds, shape, p1, p2, comm, send, inverse, d, batch=1, prec=dfft.F64, scale=None, inplace=False):
-    rc, c, plan = create_r2r(rank, P, decomp, kinds, shape, p1, p2, comm, send, batch, inplace, prec)
-    assert rc == 0, (lib().dfft_last_error_string() or b"").decode()
-    if scale is not None:
-        assert lib().dfft_plan_set_scale(plan, *scale) == 0
-    sc = json.loads(describe_raw(plan, inverse, d))
-    sc["domain_bytes"] = lib().dfft_get_domain_size(plan)
-    destroy(c, plan)
-    return sc
+    p = R.Plan(P, decomp, tuple(shape), p1, p2, kinds=kinds, prec=prec, comm=comm, send=send, batch=batch, inplace=inplace, scale=scale)
+    return R.describe(p, rank, inverse, d)
 
 
 def test_kind_validation():
@@ -232,94 +207,17 @@ def run_mixed(P, decomp, kinds, shape, p1, p2, comm, send, inverse, d, batch=1, 
     """replays every rank's steps in lock step, each pass with the kind its description names; returns the worst rel-L2
     error of any rank's output block against the per-axis transform of the global array"""
     nx, ny, nz = shape
-    scheds = [describe(r, P, decomp, kinds, shape, p1, p2, comm, send, inverse, d, batch=batch, prec=prec, scale=scale, inplace=inplace)
-              for r in range(P)]
-    es = scheds[0]["esize"]
-    assert es == (8 if prec == dfft.F64 else 4) and not scheds[0]["overlapped"]
-    plan_kind = {"dct": DCT, "dst": DST, "r2hc": R2HC}
-    lay = lambda r, w: dfft.layout(decomp, DCT, nx, ny, nz, p1, p2, r, w)
+    p = R.Plan(P, decomp, tuple(shape), p1, p2, kinds=kinds, prec=prec, comm=comm, send=send, batch=batch, inplace=inplace, scale=scale)
+    scheds = [R.describe(p, r, inverse, d) for r in range(P)]
+    assert not scheds[0]["overlapped"]
     rng = np.random.default_rng(P * 1000 + nx + ny + nz + batch + 7 * kinds[0] + 3 * kinds[1] + kinds[2])
     xg = rng.standard_normal((batch,) + shape)
     spec = np.stack([global_ref(xg[f], kinds, False, d) for f in range(batch)])
-    src_g = spec if inverse else xg
     want_g = np.stack([global_ref(spec[f], kinds, True, d) for f in range(batch)]) if inverse else spec
     s_used = 1.0 if scale is None else scale[1 if inverse else 0]
     if prec == dfft.F32:
         s_used = float(np.float32(s_used))
-    mem = RealMemory(es)
-    for r in range(P):
-        for s_ in range(scheds[r]["nslots"]):
-            mem.add(scheds[r]["slots"][s_][r], scheds[r]["slot_bytes"] // es)
-    src_w, dst_w = (d, 0) if inverse else (0, d)
-    uin, uout = [], []
-    for r in range(P):
-        isz, ist = lay(r, src_w)
-        osz, ost = lay(r, dst_w)
-        ni, no = int(np.prod(isz)), int(np.prod(osz))
-        fi = scheds[r]["domain_bytes"] // es if inplace else ni
-        fo = scheds[r]["domain_bytes"] // es if inplace else no
-        a = mem.add(USER_IN + (r << 48), batch * fi)
-        for f in range(batch):
-            a[f * fi:f * fi + ni] = src_g[f][ist[0]:ist[0] + isz[0], ist[1]:ist[1] + isz[1], ist[2]:ist[2] + isz[2]].ravel()
-        uin.append((a, fi))
-        uout.append((a, fo) if inplace else (mem.add(USER_OUT + (r << 48), batch * fo), fo))
-    nsteps = len(scheds[0]["steps"])
-    assert all(len(s["steps"]) == nsteps for s in scheds)
-    order = Ordering(scheds)
-    scaled = {}  # output array -> how often each element was scaled
-    for k in range(nsteps):
-        pending = []
-        for r in range(P):
-            st = scheds[r]["steps"][k]
-            if st["type"] == 1:
-                continue
-            if st["type"] == 2:
-                sb = scheds[r]["slots"][st["send_slot"]][r]
-                for peer in st["peers"]:
-                    q = peer["rank"]
-                    rb = scheds[q]["slots"][st["recv_slot"]][q]
-                    mine = [pp for pp in scheds[q]["steps"][k]["peers"] if pp["rank"] == r][0]
-                    assert mine["rcount"] == peer["scount"]
-                    src, so = mem.resolve(sb + peer["soff"] * es)
-                    dst, do = mem.resolve(rb + mine["roff"] * es)
-                    order.read(r, k, id(src), src.size, np.arange(so, so + peer["scount"]))
-                    pending.append((dst, np.arange(do, do + peer["scount"]), src[so:so + peer["scount"]].copy(), q))
-                continue
-            assert st["kind"] in (4, 5), st["kind"]
-            kind = plan_kind[st.get("r2r", scheds[r]["r2r"])]
-            N, A0, A1, B = 1 << st["log2n"], st["A0"], st["A1"], st["B"]
-            ub_in = USER_IN + (r << 48) if st["in_user"] else None
-            ub_out = (USER_IN if inplace else USER_OUT) + (r << 48) if st["out_user"] == 2 else None
-            data = np.zeros((A0, A1, N, B))
-            for base, ns, off in view_indices(st["in"], A0, A1, N, B, ub_in):
-                arr, o = mem.resolve(base)
-                data[:, :, ns, :] = arr[o + off]
-                order.read(r, k, id(arr), arr.size, o + off)
-            res = r2r_1d(data, kind, st["inverse"], 2)
-            if "scale" in st:
-                res = res * st["scale"]
-            for base, ns, off in view_indices(st["out"], A0, A1, N, B, ub_out):
-                arr, o = mem.resolve(base)
-                pending.append((arr, o + off, res[:, :, ns, :], r))
-                if "scale" in st:
-                    scaled.setdefault(id(arr), np.zeros(arr.size, dtype=np.int64))
-                    np.add.at(scaled[id(arr)], (o + off).ravel(), 1)
-        for arr, idx, val, who in pending:
-            order.write(who, k, id(arr), arr.size, idx)
-            arr[idx] = val
-    worst = 0.0
-    for r in range(P):
-        osz, ost = lay(r, dst_w)
-        arr, fo = uout[r]
-        no = int(np.prod(osz))
-        for f in range(batch):
-            got = arr[f * fo:f * fo + no].reshape(osz)
-            want = want_g[f][ost[0]:ost[0] + osz[0], ost[1]:ost[1] + osz[1], ost[2]:ost[2] + osz[2]] * s_used
-            worst = max(worst, float(np.linalg.norm(got - want) / np.linalg.norm(want)))
-            if scale is not None and s_used != 1.0:
-                cnt = scaled[id(arr)][f * fo:f * fo + no]
-                assert (cnt == 1).all(), f"rank {r} field {f}: an output value is scaled {int(cnt.min())}..{int(cnt.max())} times"
-    return worst
+    return R.error(R.replay(p, inverse, d, spec if inverse else xg, scheds), want_g * s_used)
 
 
 @pytest.mark.parametrize("inverse", [0, 1])

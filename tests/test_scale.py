@@ -2,38 +2,35 @@
 replays that prove every output value is scaled exactly once.
 
 A scaled plan's dfft_plan_describe must equal the unscaled one except for a "scale" key on the steps whose stores are
-final.  The replay runs the scaled step lists of every rank with the numpy machinery of test_schedule_emulation.py,
-multiplying each step's stores by its "scale", and compares every rank's output with the oracle times the scale: a value
-scaled twice or not at all is off by that factor."""
+final.  The replay runs the scaled step lists of every rank through step_replay.py, which multiplies each step's stores
+by its "scale" and counts how often each output value is scaled, and compares every rank's output with the oracle times
+the scale: a value scaled twice or not at all is off by that factor."""
 import ctypes as C
 import json
 import math
+from dataclasses import replace
 
 import numpy as np
 import pytest
 
 import distributedfft_b200 as dfft
+import step_replay as R
 from distributedfft_b200._lib import lib
 from oracle import dft_oracle as O
 
 from test_batch import create
-from test_schedule_emulation import A2A, P2P, PE, SL, STREAMS, SYNC, USER_IN, USER_OUT, ZY, Memory, Ordering, view_indices
+from test_schedule_emulation import A2A, P2P, PE, SL, STREAMS, SYNC, ZY
 
 S = 3.0  # a scale that no double application or omission can hide
 
 
+def plan_of(P, decomp, transform, shape, p1, p2, comm, send, batch=1, prec=None, scale=None):
+    return R.Plan(P, decomp, tuple(shape), p1, p2, transform=transform, prec=dfft.F64 if prec is None else prec, comm=comm, send=send, batch=batch,
+                  scale=scale)
+
+
 def describe_scaled(rank, P, decomp, transform, shape, p1, p2, comm, send, inverse, d, batch=1, prec=None, scale=None):
-    rc, msg, c, plan = create(rank, P, decomp, transform, shape, p1, p2, batch, comm, send, prec)
-    assert rc == 0, msg
-    if scale is not None:
-        assert lib().dfft_plan_set_scale(plan, *scale) == 0
-    need = C.c_size_t()
-    assert lib().dfft_plan_describe(plan, inverse, d, None, 0, C.byref(need)) == 0
-    buf = C.create_string_buffer(need.value)
-    assert lib().dfft_plan_describe(plan, inverse, d, buf, need.value, C.byref(need)) == 0
-    lib().dfft_plan_destroy(plan)
-    lib().dfft_comm_destroy(c)
-    return buf.value.decode()
+    return R.describe_text(plan_of(P, decomp, transform, shape, p1, p2, comm, send, batch, prec, scale), rank, inverse, d)
 
 
 def run_scaled(P, decomp, transform, shape, p1, p2, comm, send, inverse, d, batch=1, prec=None):
@@ -42,118 +39,23 @@ def run_scaled(P, decomp, transform, shape, p1, p2, comm, send, inverse, d, batc
     "scale" key of the steps that write the caller's output last."""
     nx, ny, nz = shape
     c2c = transform == dfft.C2C
-    sc_ = (1.0, S) if inverse else (S, 1.0)
+    p = plan_of(P, decomp, transform, shape, p1, p2, comm, send, batch, prec, (1.0, S) if inverse else (S, 1.0))
     scheds = []
     for r in range(P):
-        plain = describe_scaled(r, P, decomp, transform, shape, p1, p2, comm, send, inverse, d, batch, prec)
-        scaled = describe_scaled(r, P, decomp, transform, shape, p1, p2, comm, send, inverse, d, batch, prec, sc_)
-        a, b = json.loads(plain), json.loads(scaled)
+        a, b = R.describe(replace(p, scale=None), r, inverse, d), R.describe(p, r, inverse, d)
         marked = [k for k, st in enumerate(b["steps"]) if "scale" in st]
         assert marked and all(b["steps"][k]["scale"] == S for k in marked)
-        for st in b["steps"]:
-            st.pop("scale", None)
-        assert a == b
+        assert a == {**b, "steps": [{key: v for key, v in st.items() if key != "scale"} for st in b["steps"]]}
         # marked: the steps that store into the caller's output with no later step of the same field reading it
         for k, st in enumerate(a["steps"]):
             later_read = any(t.get("in_user") == 2 and t.get("field", 0) == st.get("field", 0) for t in a["steps"][k + 1:])
             assert (k in marked) == (st["type"] == 0 and st["out_user"] == 2 and not later_read), (k, st["label"])
-        scheds.append(json.loads(scaled))
-    es = scheds[0]["esize"]
-    lay = lambda r, w: dfft.layout(decomp, transform, nx, ny, nz, p1, p2, r, w)
-    xs, specs = [], []
-    for f in range(batch):
-        x = O.complex_input(shape, seed=99 + f) if c2c else O.real_input(shape, seed=99 + f)
-        xs.append(x)
-        specs.append(O.fft_c2c(x, d) if c2c else O.fft_r2c(x, d))
-    mem = Memory(es)
-    for r in range(P):
-        for s_ in range(scheds[r]["nslots"]):
-            mem.add(scheds[r]["slots"][s_][r], scheds[r]["slot_bytes"] // es)
-    uin, uout, fin, fout = [], [], [], []
-    for r in range(P):
-        isz, ist = lay(r, 0)
-        osz, ost = lay(r, d)
-        nin, nout = int(np.prod(isz)), int(np.prod(osz))
-        if not c2c:
-            nin //= 2
-        fi, fo = (nout, nin) if inverse else (nin, nout)
-        fin.append(fi)
-        fout.append(fo)
-        a = mem.add(USER_IN + (r << 48), batch * fi)
-        uout.append(mem.add(USER_OUT + (r << 48), batch * fo))
-        for f in range(batch):
-            if not inverse:
-                blk = np.ascontiguousarray(O.block(xs[f], ist, isz))
-                src = blk.astype(np.complex128).ravel() if c2c else blk.ravel().view(np.complex128)
-            else:
-                src = np.ascontiguousarray(O.block(specs[f], ost, osz)).ravel()
-            a[f * fi:(f + 1) * fi] = src
-        uin.append(a)
-    nsteps = len(scheds[0]["steps"])
-    assert all(len(s["steps"]) == nsteps for s in scheds)
-    order = Ordering(scheds)
-    for k in range(nsteps):
-        pending = []
-        for r in range(P):
-            st = scheds[r]["steps"][k]
-            if st["type"] == 1:
-                continue
-            if st["type"] == 2:
-                sb = scheds[r]["slots"][st["send_slot"]][r]
-                for peer in st["peers"]:
-                    q = peer["rank"]
-                    rb = scheds[q]["slots"][st["recv_slot"]][q]
-                    mine = [pp for pp in scheds[q]["steps"][k]["peers"] if pp["rank"] == r][0]
-                    src, so = mem.resolve(sb + peer["soff"] * es)
-                    dst, do = mem.resolve(rb + mine["roff"] * es)
-                    order.read(r, k, id(src), src.size, np.arange(so, so + peer["scount"]))
-                    pending.append((dst, do, src[so:so + peer["scount"]].copy(), q))
-                continue
-            N = 1 << st["log2n"]
-            A0, A1, B, kind = st["A0"], st["A1"], st["B"], st["kind"]
-            # views on the caller's buffers hold byte offsets, already shifted to the step's field
-            ub_in = {1: USER_IN + (r << 48), 2: USER_OUT + (r << 48)}.get(st["in_user"])
-            ub_out = USER_OUT + (r << 48) if st["out_user"] == 2 else None
-            n_in, n_out = {0: (N, N), 1: (N, N), 2: (N, N + 1), 3: (N + 1, N)}[kind]
-            b_ = B if kind in (0, 1) else 1
-            data = np.zeros((A0, A1, n_in, b_), dtype=np.complex128)
-            for base, ns, off in view_indices(st["in"], A0, A1, n_in, b_, ub_in):
-                arr, o = mem.resolve(base)
-                data[:, :, ns, :] = arr[o + off]
-                order.read(r, k, id(arr), arr.size, o + off)
-            if kind in (0, 1):
-                res = np.fft.ifft(data, axis=2) * N if st["inverse"] else np.fft.fft(data, axis=2)
-            elif kind == 2:
-                res = np.fft.rfft(np.ascontiguousarray(data[..., 0]).view(np.float64), axis=2)[..., None]
-            else:
-                reals = np.fft.irfft(data[..., 0], n=2 * N, axis=2) * (2 * N)
-                res = np.ascontiguousarray(reals).view(np.complex128)[..., None]
-            res = res * st.get("scale", 1.0)
-            for base, ns, off in view_indices(st["out"], A0, A1, n_out, b_, ub_out):
-                arr, o = mem.resolve(base)
-                pending.append((arr, o + off, res[:, :, ns, :], r))
-        for arr, idx, val, who in pending:
-            if isinstance(idx, (int, np.integer)):
-                order.write(who, k, id(arr), arr.size, np.arange(idx, idx + val.size))
-                arr[idx:idx + val.size] = val
-            else:
-                order.write(who, k, id(arr), arr.size, idx)
-                arr[idx] = val
-    worst = 0.0
-    for r in range(P):
-        for f in range(batch):
-            if not inverse:
-                osz, ost = lay(r, d)
-                got = uout[r][f * fout[r]:f * fout[r] + int(np.prod(osz))].reshape(osz)
-                worst = max(worst, O.rel_l2(got, S * O.block(specs[f], ost, osz)))
-            else:
-                isz, ist = lay(r, 0)
-                want = O.block(xs[f], ist, isz).astype(np.complex128 if c2c else np.float64)
-                n = float(nz * (ny if d >= 2 else 1) * (nx if d >= 3 else 1))
-                seg = uout[r][f * fout[r]:(f + 1) * fout[r]]
-                got = seg.reshape(isz) if c2c else seg.view(np.float64).reshape(isz)
-                worst = max(worst, O.rel_l2(got, S * n * want))
-    return worst
+        scheds.append(b)
+    xs = [O.complex_input(shape, seed=99 + f) if c2c else O.real_input(shape, seed=99 + f) for f in range(batch)]
+    specs = [O.fft_c2c(x, d) if c2c else O.fft_r2c(x, d) for x in xs]
+    n = float(nz * (ny if d >= 2 else 1) * (nx if d >= 3 else 1))
+    x, want = (specs, [S * n * x for x in xs]) if inverse else (xs, [S * s for s in specs])
+    return R.error(R.replay(p, inverse, d, x, scheds), want)
 
 
 CASES = [

@@ -1,297 +1,36 @@
 """Replays the library's schedules on the CPU for any rank count.
 
 dfft_comm_create_dry gives a geometry-only communicator; dfft_plan_describe returns, per rank, the exact step
-list the GPU executes — every FFT pass with its segmented input / output views (base addresses, strides,
-segment tables), rendezvous points and all-to-all counts.  This test builds the plans of all P ranks, lays
-the synthetic slot addresses out in numpy arrays, executes the steps in lock step (numpy FFTs for the passes,
-the views for all data movement) and compares every rank's output block with the oracle's block of the global
-transform.  It covers what cannot be run here on a GPU: 4- and 8-rank slab / z_then_yx / pencil grids, both
+list the GPU executes.  step_replay.py builds the plans of all P ranks, executes their steps in lock step with
+numpy and checks their ordering; this test compares every rank's output block with the oracle's block of the
+global transform.  It covers what cannot be run here on a GPU: 4- and 8-rank slab / z_then_yx / pencil grids, both
 exchange methods, forward and inverse, partial transforms, the overlapped (Streams) schedule and the blocked
 intermediate layout."""
-import ctypes as C
-import json
-
-import numpy as np
 import pytest
 
 import distributedfft_b200 as dfft
-from distributedfft_b200 import _lib
-from distributedfft_b200._lib import check, lib
+import step_replay as R
 from oracle import dft_oracle as O
 
-USER_IN, USER_OUT = 1 << 60, 1 << 61  # synthetic address ranges of the caller's buffers
+
+def plan_of(P, decomp, transform, shape, p1, p2, comm_method, send_method, prec=None):
+    return R.Plan(P, decomp, tuple(shape), p1, p2, transform=transform, prec=dfft.F64 if prec is None else prec, comm=comm_method, send=send_method)
 
 
 def describe(rank, P, decomp, transform, shape, p1, p2, comm_method, send_method, inverse, d, prec=None):
-    prec = dfft.F64 if prec is None else prec
-    comm = C.c_void_p()
-    check(lib().dfft_comm_create_dry(rank, P, C.byref(comm)))
-    cfg = _lib.dfft_config(1, 0, comm_method, send_method, None, comm_method, send_method)
-    plan = C.c_void_p()
-    check(lib().dfft_plan_create(comm, C.byref(cfg), decomp, prec, transform, shape[0], shape[1], shape[2], p1, p2, 1, C.byref(plan)))
-    need = C.c_size_t()
-    check(lib().dfft_plan_describe(plan, inverse, d, None, 0, C.byref(need)))
-    buf = C.create_string_buffer(need.value)
-    check(lib().dfft_plan_describe(plan, inverse, d, buf, need.value, C.byref(need)))
-    sched = json.loads(buf.value.decode())
-    lib().dfft_plan_destroy(plan)
-    lib().dfft_comm_destroy(comm)
-    return sched
-
-
-class Memory:
-    """complex128 arrays keyed by synthetic base address; `es` = bytes per complex element of the plan under test (the
-    replay always computes in complex128, only the address arithmetic follows the plan's precision)"""
-
-    def __init__(self, es=16):
-        self.regions = []  # (base_bytes, array)
-        self.es = es
-
-    def add(self, base, nelem):
-        arr = np.zeros(nelem, dtype=np.complex128)
-        self.regions.append((base, arr))
-        return arr
-
-    def resolve(self, addr):
-        for base, arr in self.regions:
-            if base <= addr < base + arr.size * self.es:
-                assert (addr - base) % self.es == 0
-                return arr, (addr - base) // self.es
-        raise KeyError(hex(addr))
-
-
-class Ordering:
-    """Happens-before check of a set of per-rank step lists (what the lock-step replay cannot see: a step that runs on
-    another plan stream than its producer is only ordered behind it through an event, and a step that reads what a peer
-    stored only through a rendezvous).  Per rank: step k's ancestors = the previous step on its stream + the steps that
-    recorded the events it waits for (the auxiliary streams fork from the caller's stream before step 0).  Across ranks:
-    everything before rank a's j-th rendezvous of a group happens before everything after rank b's j-th rendezvous of
-    that group.  Every read-after-write and write-after-read on slot memory must be covered by one of the two."""
-
-    def __init__(self, scheds):
-        self.scheds = scheds
-        self.anc, self.rdv = [], []  # per rank: ancestor bit masks; {(phase_id): [step indices]}
-        for sc in scheds:
-            anc, last, recorded, rdv = [], {}, {}, {}
-            for k, st in enumerate(sc["steps"]):
-                preds = [last[st["stream"]]] if st["stream"] in last else []
-                for w in st["waits"]:
-                    assert w in recorded, f"rank {sc['rank']} step {k} ({st['label']}) waits for event {w} that no earlier step records"
-                    preds.append(recorded[w])
-                m = 0
-                for q in preds:
-                    m |= anc[q] | (1 << q)
-                anc.append(m)
-                if st["record"] >= 0:
-                    recorded[st["record"]] = k
-                last[st["stream"]] = k
-                if st["type"] == 1:
-                    rdv.setdefault(st["phase_id"], []).append(k)
-            self.anc.append(anc)
-            self.rdv.append(rdv)
-        self.last_w, self.last_r = {}, {}
-
-    def before(self, a, ka, b, kb):
-        """step ka of rank a happens before step kb of rank b"""
-        if a == b:
-            return ka == kb or bool(self.anc[a][kb] >> ka & 1)
-        for g, mine in self.rdv[a].items():
-            theirs = self.rdv[b].get(g, [])
-            if b not in self.scheds[a]["steps"][mine[0]]["members"]:
-                continue
-            for ra, rb in zip(mine, theirs):
-                if (ra == ka or self.anc[a][ra] >> ka & 1) and (rb == kb or self.anc[b][kb] >> rb & 1):
-                    return True
-        return False
-
-    def _tables(self, key, size):
-        if key not in self.last_w:
-            self.last_w[key] = np.full((2, size), -1, dtype=np.int64)
-            self.last_r[key] = np.full((2, size), -1, dtype=np.int64)
-        return self.last_w[key], self.last_r[key]
-
-    def read(self, r, k, key, size, idx):
-        lw, lr = self._tables(key, size)
-        idx = np.asarray(idx).ravel()
-        for q, kq in {(int(a), int(b)) for a, b in zip(*lw[:, idx])} - {(-1, -1)}:
-            assert self.before(q, kq, r, k), (f"rank {r} step {k} ({self.scheds[r]['steps'][k]['label']}) reads what rank {q} step {kq} "
-                                              f"({self.scheds[q]['steps'][kq]['label']}) wrote, without an event / rendezvous path between them")
-        lr[0, idx], lr[1, idx] = r, k
-
-    def write(self, r, k, key, size, idx):
-        lw, lr = self._tables(key, size)
-        idx = np.asarray(idx).ravel()
-        for q, kq in {(int(a), int(b)) for a, b in zip(*lr[:, idx])} - {(-1, -1), (r, k)}:
-            assert self.before(q, kq, r, k), (f"rank {r} step {k} ({self.scheds[r]['steps'][k]['label']}) overwrites what rank {q} step {kq} "
-                                              f"({self.scheds[q]['steps'][kq]['label']}) reads, without an event / rendezvous path between them")
-        for q, kq in {(int(a), int(b)) for a, b in zip(*lw[:, idx])} - {(-1, -1), (r, k)}:
-            assert self.before(q, kq, r, k), f"rank {r} step {k} overwrites rank {q} step {kq}'s output without ordering"
-        lw[0, idx], lw[1, idx] = r, k
-
-
-def view_indices(view, A0, A1, N, B, user_base=None):
-    """flat (array, index) for every element (a0, a1, n, b) of a view, as index arrays per segment"""
-    out = []
-    seg_of_n = np.array(view["seg_of_n"], dtype=np.int64) if view["nseg"] > 1 else np.zeros(N, dtype=np.int64)
-    a0 = np.arange(A0)[:, None, None, None]
-    a1 = np.arange(A1)[None, :, None, None]
-    b = np.arange(B)[None, None, None, :]
-    for s, seg in enumerate(view["segs"]):
-        ns = np.nonzero(seg_of_n[:N] == s)[0]
-        if ns.size == 0:
-            continue
-        n = ns[None, None, :, None]
-        off = a0 * seg["sA0"] + a1 * seg["sA1"] + (n - seg["n0"]) * view["sN"] + b
-        base = seg["base"] if user_base is None else user_base + seg["base"]
-        out.append((base, ns, off))
-    return out
+    return R.describe(plan_of(P, decomp, transform, shape, p1, p2, comm_method, send_method, prec), rank, inverse, d)
 
 
 def run_case(P, decomp, transform, shape, p1, p2, comm_method, send_method, inverse, d, mutate=None, prec=None):
+    """worst rel-L2 error of every rank's output block against the oracle's block of the global transform"""
     nx, ny, nz = shape
     c2c = transform == dfft.C2C
-    scheds = [describe(r, P, decomp, transform, shape, p1, p2, comm_method, send_method, inverse, d, prec) for r in range(P)]
-    es = scheds[0]["esize"]
-    if mutate:
-        mutate(scheds)  # negative tests: break the schedules on purpose
-    mems = []
-    lay = lambda r, w: dfft.layout(decomp, transform, nx, ny, nz, p1, p2, r, w)
-    # global data and per-rank user buffers (real buffers are stored as complex pairs, like the kernels read them)
-    if c2c:
-        xg = O.complex_input(shape)
-        spec = O.fft_c2c(xg, d)
-    else:
-        xg = O.real_input(shape)
-        spec = O.fft_r2c(xg, d)
-    mem = Memory(es)
-    for r in range(P):
-        sc = scheds[r]
-        for s_ in range(sc["nslots"]):
-            mem.add(sc["slots"][s_][r], sc["slot_bytes"] // es)
-    uin, uout = [], []
-    for r in range(P):
-        isz, ist = lay(r, 0)
-        osz, ost = lay(r, d)
-        dom = max(int(np.prod(lay(r, w)[0][:2])) * (nz if c2c else nz // 2 + 1) for w in (1, 2, 3))
-        if not inverse:
-            blk = np.ascontiguousarray(O.block(xg, ist, isz))
-            src = blk.astype(np.complex128).ravel() if c2c else blk.ravel().view(np.complex128)
-            a = mem.add(USER_IN + (r << 48), max(src.size, 1)); a[:src.size] = src
-            uin.append(a)
-            uout.append(mem.add(USER_OUT + (r << 48), dom))
-        else:
-            blk = np.ascontiguousarray(O.block(spec, ost, osz)).ravel()
-            a = mem.add(USER_IN + (r << 48), dom); a[:blk.size] = blk
-            uin.append(a)
-            nreal = int(np.prod(isz))
-            uout.append(mem.add(USER_OUT + (r << 48), nreal if c2c else nreal // 2))
-    nsteps = len(scheds[0]["steps"])
-    assert all(len(s["steps"]) == nsteps for s in scheds)
-    order = Ordering(scheds)
-    # hazard bookkeeping: a slot written by another rank may only be read after a later rendezvous of the owner,
-    # and nobody may write into a peer's slot before its own entry rendezvous (previous exec finished everywhere)
-    slot_owner = {}
-    for r in range(P):
-        for s_ in range(scheds[r]["nslots"]):
-            slot_owner[scheds[r]["slots"][s_][r]] = (r, s_)
-    last_remote_write = {}
-    last_rdv = [-1] * P
-
-    def owner_of(addr):
-        for base, (q, s_) in slot_owner.items():
-            if base <= addr < base + scheds[q]["slot_bytes"]:
-                return q, s_
-        return None
-
-    for k in range(nsteps):
-        pending = []
-        for r in range(P):
-            st = scheds[r]["steps"][k]
-            if st["type"] == 1:
-                last_rdv[r] = k
-                continue
-            if st["type"] == 2:  # all-to-all-v between staging slots
-                sb = scheds[r]["slots"][st["send_slot"]][r]
-                for peer in st["peers"]:
-                    q = peer["rank"]
-                    rb = scheds[q]["slots"][st["recv_slot"]][q]
-                    mine = [pp for pp in scheds[q]["steps"][k]["peers"] if pp["rank"] == r][0]
-                    assert mine["rcount"] == peer["scount"]
-                    src, so = mem.resolve(sb + peer["soff"] * es)
-                    dst, do = mem.resolve(rb + mine["roff"] * es)
-                    order.read(r, k, id(src), src.size, np.arange(so, so + peer["scount"]))
-                    pending.append((dst, do, src[so:so + peer["scount"]].copy(), q))  # lands in q's stream order (ncclRecv)
-                continue
-            N = 1 << st["log2n"]
-            A0, A1, B = st["A0"], st["A1"], st["B"]
-            kind = st["kind"]
-            if st["in_user"] != 1:
-                for seg in st["in"]["segs"]:
-                    own = owner_of(seg["base"])
-                    assert own is not None and own[0] == r, "passes only read local memory"
-                    w = last_remote_write.get(own, -1)
-                    assert w < 0 or w < last_rdv[r] <= k, f"rank {r} step {k} reads slot {own} written remotely at step {w} without a rendezvous"
-            if st["out_user"] != 2:
-                for seg in st["out"]["segs"]:
-                    own = owner_of(seg["base"])
-                    assert own is not None
-                    if own[0] != r:
-                        assert last_rdv[r] >= 0, f"rank {r} writes into rank {own[0]}'s slot before its entry rendezvous"
-                        last_remote_write[own] = k
-            ub_in = USER_IN + (r << 48) if st["in_user"] == 1 else None
-            ub_out = USER_OUT + (r << 48) if st["out_user"] == 2 else None
-            if kind in (0, 1):  # C2C
-                data = np.zeros((A0, A1, N, B), dtype=np.complex128)
-                for base, ns, off in view_indices(st["in"], A0, A1, N, B, ub_in):
-                    arr, o = mem.resolve(base)
-                    data[:, :, ns, :] = arr[o + off]
-                    order.read(r, k, id(arr), arr.size, o + off)
-                res = np.fft.ifft(data, axis=2) * N if st["inverse"] else np.fft.fft(data, axis=2)
-                for base, ns, off in view_indices(st["out"], A0, A1, N, B, ub_out):
-                    arr, o = mem.resolve(base)
-                    pending.append((arr, o + off, res[:, :, ns, :], r))
-            elif kind == 2:  # R2C: N complex = 2N reals in, N+1 complex out
-                data = np.zeros((A0, A1, N, 1), dtype=np.complex128)
-                for base, ns, off in view_indices(st["in"], A0, A1, N, 1, ub_in):
-                    arr, o = mem.resolve(base)
-                    data[:, :, ns, :] = arr[o + off]
-                    order.read(r, k, id(arr), arr.size, o + off)
-                reals = np.ascontiguousarray(data[..., 0]).view(np.float64)  # (A0, A1, 2N)
-                res = np.fft.rfft(reals, axis=2)[..., None]
-                for base, ns, off in view_indices(st["out"], A0, A1, N + 1, 1, ub_out):
-                    arr, o = mem.resolve(base)
-                    pending.append((arr, o + off, res[:, :, ns, :], r))
-            else:  # C2R
-                data = np.zeros((A0, A1, N + 1, 1), dtype=np.complex128)
-                for base, ns, off in view_indices(st["in"], A0, A1, N + 1, 1, ub_in):
-                    arr, o = mem.resolve(base)
-                    data[:, :, ns, :] = arr[o + off]
-                    order.read(r, k, id(arr), arr.size, o + off)
-                reals = np.fft.irfft(data[..., 0], n=2 * N, axis=2) * (2 * N)
-                res = np.ascontiguousarray(reals).view(np.complex128)[..., None]
-                for base, ns, off in view_indices(st["out"], A0, A1, N, 1, ub_out):
-                    arr, o = mem.resolve(base)
-                    pending.append((arr, o + off, res[:, :, ns, :], r))
-        for arr, idx, val, who in pending:  # stores of step k land after every rank's loads of step k
-            if isinstance(idx, (int, np.integer)):
-                order.write(who, k, id(arr), arr.size, np.arange(idx, idx + val.size))
-                arr[idx:idx + val.size] = val
-            else:
-                order.write(who, k, id(arr), arr.size, idx)
-                arr[idx] = val
-    worst = 0.0
-    for r in range(P):
-        if not inverse:
-            osz, ost = lay(r, d)
-            got = uout[r][:int(np.prod(osz))].reshape(osz)
-            worst = max(worst, O.rel_l2(got, O.block(spec, ost, osz)))
-        else:
-            isz, ist = lay(r, 0)
-            want = O.block(xg, ist, isz).astype(np.complex128 if c2c else np.float64)
-            scale = float(nz * (ny if d >= 2 else 1) * (nx if d >= 3 else 1))
-            got = uout[r].reshape(isz) if c2c else uout[r].view(np.float64).reshape(isz)
-            worst = max(worst, O.rel_l2(got, want * scale))
-    return worst
+    xg = O.complex_input(shape) if c2c else O.real_input(shape)
+    spec = O.fft_c2c(xg, d) if c2c else O.fft_r2c(xg, d)
+    n = float(nz * (ny if d >= 2 else 1) * (nx if d >= 3 else 1))
+    x, want = (spec, xg * n) if inverse else (xg, spec)
+    outs = R.replay(plan_of(P, decomp, transform, shape, p1, p2, comm_method, send_method, prec), inverse, d, [x], mutate=mutate)
+    return R.error(outs, [want])
 
 
 SL, ZY, PE = dfft.SLAB_ZY_THEN_X, dfft.SLAB_Z_THEN_YX, dfft.PENCIL

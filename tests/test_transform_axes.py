@@ -2,7 +2,7 @@
 
 - Validation of the setter and getter, DFFT_ERR_STATE once a schedule exists, and byte-identical descriptions of plans
   whose axes are all transformed, with and without a {1, 1, 1} setter call.
-- Lock-step replays of every rank's step list (test_schedule_emulation's Ordering / view_indices): numpy / scipy per
+- Lock-step replays of every rank's step list (step_replay.py): numpy / scipy per
   pass, a plain element copy for the copy passes (kinds 6 / 7), checked against the transform of only the transformed
   axes among the first d stages: all 8 masks for C2C and for mixed-kind R2R, the 4 R2C masks that transform z, 1-8 ranks,
   slab, Z_Then_YX and pencil, Peer2Peer and All2All, Streams (sequential), partial d, uneven splits, blocked tails,
@@ -16,22 +16,20 @@ import numpy as np
 import pytest
 
 import distributedfft_b200 as dfft
-from distributedfft_b200 import _lib
 from distributedfft_b200._lib import check, lib
+import step_replay as R
+from step_replay import describe_raw
 from test_r2r import CASES as R2R_CASES
 from test_r2r_mixed import r2r_1d
-from test_schedule_emulation import Memory, Ordering, view_indices
 
 SL, ZY, PE = dfft.SLAB_ZY_THEN_X, dfft.SLAB_Z_THEN_YX, dfft.PENCIL
 P2P, A2A = 0, 1
 SYNC, STREAMS = 0, 1
-USER_IN, USER_OUT = 1 << 60, 1 << 61
 C2C, R2C, DCT, DST, R2HC = dfft.C2C, dfft.R2C, dfft.DCT, dfft.DST, dfft.R2HC
 ERR_INVALID, ERR_STATE = -1, -4  # include/dfft.h
 MASKS = list(itertools.product((0, 1), repeat=3))  # (x, y, z)
 R2C_MASKS = [m for m in MASKS if m[2]]
 MIXED = (R2HC, DST, DCT)
-KIND = {"dct": DCT, "dst": DST, "r2hc": R2HC}
 
 
 def mask_id(m):
@@ -39,19 +37,15 @@ def mask_id(m):
 
 
 # ---- plans ------------------------------------------------------------------------------------------------------------
+def plan_of(P, decomp, transform, shape, p1, p2, axes=None, comm=P2P, send=SYNC, batch=1, inplace=False, scale=None, prec=dfft.F64, kinds=None):
+    return R.Plan(P, decomp, tuple(shape), p1, p2, transform=transform, kinds=kinds, prec=prec, comm=comm, send=send, batch=batch, inplace=inplace,
+                  axes=axes, scale=scale)
+
+
 def create(rank, P, decomp, transform, shape, p1, p2, comm=P2P, send=SYNC, batch=1, inplace=False, prec=dfft.F64, kinds=None):
-    """dry plan: (rc, comm, plan); kinds: a per-axis real-to-real plan"""
-    c = C.c_void_p()
-    check(lib().dfft_comm_create_dry(rank, P, C.byref(c)))
-    cfg = _lib.dfft_config(1, 0, comm, send, None, comm, send)
-    plan = C.c_void_p()
-    if kinds is not None:
-        rc = lib().dfft_plan_create_r2r(c, C.byref(cfg), decomp, prec, (C.c_int * 3)(*kinds), *shape, p1, p2, batch, 1 if inplace else 0, 1,
-                                        C.byref(plan))
-    else:
-        fn = lib().dfft_plan_create_inplace if inplace else lib().dfft_plan_create_batched
-        rc = fn(c, C.byref(cfg), decomp, prec, transform, *shape, p1, p2, batch, 1, C.byref(plan))
-    assert rc == 0, (lib().dfft_last_error_string() or b"").decode()
+    """dry plan: (comm, plan); kinds: a per-axis real-to-real plan"""
+    rc, msg, c, plan = R.create(plan_of(P, decomp, transform, shape, p1, p2, None, comm, send, batch, inplace, None, prec, kinds), rank)
+    assert rc == 0, msg
     return c, plan
 
 
@@ -64,25 +58,9 @@ def set_axes(plan, axes):
     return lib().dfft_plan_set_transform_axes(plan, None if axes is None else (C.c_int * 3)(*axes))
 
 
-def describe_raw(plan, inverse, d):
-    need = C.c_size_t()
-    check(lib().dfft_plan_describe(plan, inverse, d, None, 0, C.byref(need)))
-    buf = C.create_string_buffer(need.value)
-    check(lib().dfft_plan_describe(plan, inverse, d, buf, need.value, C.byref(need)))
-    return buf.value.decode()
-
-
 def describe(rank, P, decomp, transform, shape, p1, p2, axes, inverse, d, comm=P2P, send=SYNC, batch=1, inplace=False, scale=None,
              prec=dfft.F64, kinds=None):
-    c, plan = create(rank, P, decomp, transform, shape, p1, p2, comm, send, batch, inplace, prec, kinds)
-    if axes is not None:
-        assert set_axes(plan, axes) == 0, (lib().dfft_last_error_string() or b"").decode()
-    if scale is not None:
-        assert lib().dfft_plan_set_scale(plan, *scale) == 0
-    sc = json.loads(describe_raw(plan, inverse, d))
-    sc["domain_bytes"] = lib().dfft_get_domain_size(plan)
-    destroy(c, plan)
-    return sc
+    return R.describe(plan_of(P, decomp, transform, shape, p1, p2, axes, comm, send, batch, inplace, scale, prec, kinds), rank, inverse, d)
 
 
 # ---- validation ---------------------------------------------------------------------------------------------------------
@@ -182,140 +160,26 @@ def inv_ref(X, transform, kinds, axes, d, nz):
     return X
 
 
-class RealMemory(Memory):
-    def add(self, base, nelem):
-        arr = np.zeros(nelem, dtype=np.float64)
-        self.regions.append((base, arr))
-        return arr
-
-
-def pass_result(st, data, kind_default):
-    """what pass st stores for its loaded lines data[a0, a1, n, b] (n-point lines along axis 2)"""
-    k = st["kind"]
-    if k in (6, 7):
-        return data.copy()
-    if k in (0, 1):
-        return np.fft.ifft(data, axis=2) * data.shape[2] if st["inverse"] else np.fft.fft(data, axis=2)
-    if k in (4, 5):
-        return r2r_1d(data, KIND[st.get("r2r", kind_default)], st["inverse"], 2)
-    raise AssertionError(f"unexpected pass kind {k}")
-
-
 def run(P, decomp, transform, shape, p1, p2, axes, inverse, d, comm=P2P, send=SYNC, kinds=None, batch=1, inplace=False, scale=None,
         prec=dfft.F64, mutate=None):
     """replays every rank's steps in lock step; returns the worst rel-L2 error of any rank's output block"""
     nx, ny, nz = shape
-    scheds = [describe(r, P, decomp, transform, shape, p1, p2, axes, inverse, d, comm, send, batch, inplace, scale, prec, kinds) for r in range(P)]
-    if mutate:
-        mutate(scheds)
-    real = kinds is not None
-    r2c = transform == R2C
-    es = scheds[0]["esize"]
+    p = plan_of(P, decomp, transform, shape, p1, p2, axes, comm, send, batch, inplace, scale, prec, kinds)
+    scheds = [R.describe(p, r, inverse, d) for r in range(P)]
     assert not scheds[0]["overlapped"]
     if axes != (1, 1, 1):
         assert scheds[0]["transform_axes"] == list(axes)
-    lay = lambda r, w: dfft.layout(decomp, DCT if real else transform, nx, ny, nz, p1, p2, r, w)
     rng = np.random.default_rng(P * 1000 + nx + ny + nz + batch + 17 * axes[0] + 5 * axes[1] + axes[2] + 3 * d)
-    if real or r2c:
+    if kinds is not None or transform == R2C:
         xg = rng.standard_normal((batch,) + shape)
     else:
         xg = rng.standard_normal((batch,) + shape) + 1j * rng.standard_normal((batch,) + shape)
     spec = np.stack([fwd_ref(xg[f], transform, kinds, axes, d) for f in range(batch)])
-    src_g = spec if inverse else xg
     want_g = np.stack([inv_ref(spec[f], transform, kinds, axes, d, nz) for f in range(batch)]) if inverse else spec
     s_used = 1.0 if scale is None else scale[1 if inverse else 0]
     if prec == dfft.F32:
         s_used = float(np.float32(s_used))
-    mem = RealMemory(es) if real else Memory(es)
-    for r in range(P):
-        for s_ in range(scheds[r]["nslots"]):
-            mem.add(scheds[r]["slots"][s_][r], scheds[r]["slot_bytes"] // es)
-    src_w, dst_w = (d, 0) if inverse else (0, d)
-    # R2C: the real side is stored as complex pairs, like the kernels read it
-    real_side_in, real_side_out = r2c and not inverse, r2c and bool(inverse)
-    uout = []
-    for r in range(P):
-        isz, ist = lay(r, src_w)
-        osz, ost = lay(r, dst_w)
-        ni = int(np.prod(isz)) // (2 if real_side_in else 1)
-        no = int(np.prod(osz)) // (2 if real_side_out else 1)
-        if batch > 1:
-            fi, fo = scheds[r]["field_in"] // es, scheds[r]["field_out"] // es
-        else:
-            fi, fo = (scheds[r]["domain_bytes"] // es,) * 2 if inplace else (ni, no)
-        a = mem.add(USER_IN + (r << 48), max(batch * max(fi, ni), 1))
-        for f in range(batch):
-            blk = np.ascontiguousarray(src_g[f][ist[0]:ist[0] + isz[0], ist[1]:ist[1] + isz[1], ist[2]:ist[2] + isz[2]]).ravel()
-            a[f * fi:f * fi + ni] = blk.view(np.complex128) if real_side_in else blk
-        uout.append((a, fo, no) if inplace else (mem.add(USER_OUT + (r << 48), max(batch * max(fo, no), 1)), fo, no))
-    nsteps = len(scheds[0]["steps"])
-    assert all(len(s["steps"]) == nsteps for s in scheds)
-    order = Ordering(scheds)
-    scaled = {}  # output array -> how often each element was scaled
-    for k in range(nsteps):
-        pending = []
-        for r in range(P):
-            st = scheds[r]["steps"][k]
-            if st["type"] == 1:
-                continue
-            if st["type"] == 2:
-                sb = scheds[r]["slots"][st["send_slot"]][r]
-                for peer in st["peers"]:
-                    q = peer["rank"]
-                    rb = scheds[q]["slots"][st["recv_slot"]][q]
-                    mine = [pp for pp in scheds[q]["steps"][k]["peers"] if pp["rank"] == r][0]
-                    assert mine["rcount"] == peer["scount"]
-                    src, so = mem.resolve(sb + peer["soff"] * es)
-                    dst, do = mem.resolve(rb + mine["roff"] * es)
-                    order.read(r, k, id(src), src.size, np.arange(so, so + peer["scount"]))
-                    pending.append((dst, np.arange(do, do + peer["scount"]), src[so:so + peer["scount"]].copy(), q))
-                continue
-            kind = st["kind"]
-            if kind in (6, 7):
-                assert "n" in st and st["log2n"] == 0 and "r2r" not in st
-                assert st["label"].split()[0] in "xyz" and "copy" in st["label"]
-            N = st.get("n", 1 << st["log2n"])
-            A0, A1, B = st["A0"], st["A1"], st["B"]
-            ub_in = {1: USER_IN, 2: USER_IN if inplace else USER_OUT}.get(st["in_user"])
-            ub_in = None if ub_in is None else ub_in + (r << 48)
-            ub_out = (USER_IN if inplace else USER_OUT) + (r << 48) if st["out_user"] == 2 else None
-            n_in, n_out = (N + 1, N) if kind == 3 else (N, N + 1) if kind == 2 else (N, N)
-            data = np.zeros((A0, A1, n_in, B), dtype=np.float64 if real else np.complex128)
-            for base, ns, off in view_indices(st["in"], A0, A1, n_in, B, ub_in):
-                arr, o = mem.resolve(base)
-                data[:, :, ns, :] = arr[o + off]
-                order.read(r, k, id(arr), arr.size, o + off)
-            if kind == 2:  # R2C: N complex = 2N reals in, N+1 complex out
-                res = np.fft.rfft(np.ascontiguousarray(data[..., 0]).view(np.float64), axis=2)[..., None]
-            elif kind == 3:
-                res = np.ascontiguousarray(np.fft.irfft(data[..., 0], n=2 * N, axis=2) * (2 * N)).view(np.complex128)[..., None]
-            else:
-                res = pass_result(st, data, scheds[r].get("r2r"))
-            if "scale" in st:
-                res = res * st["scale"]
-            for base, ns, off in view_indices(st["out"], A0, A1, n_out, B, ub_out):
-                arr, o = mem.resolve(base)
-                pending.append((arr, o + off, res[:, :, ns, :], r))
-                if "scale" in st:
-                    assert ub_out is not None, "only stores into the caller's output are scaled"
-                    scaled.setdefault(id(arr), np.zeros(arr.size, dtype=np.int64))
-                    np.add.at(scaled[id(arr)], (o + off).ravel(), 1)
-        for arr, idx, val, who in pending:
-            order.write(who, k, id(arr), arr.size, idx)
-            arr[idx] = val
-    worst = 0.0
-    for r in range(P):
-        osz, ost = lay(r, dst_w)
-        arr, fo, no = uout[r]
-        for f in range(batch):
-            got = arr[f * fo:f * fo + no]
-            got = (got.view(np.float64) if real_side_out else got).reshape(osz)
-            want = want_g[f][ost[0]:ost[0] + osz[0], ost[1]:ost[1] + osz[1], ost[2]:ost[2] + osz[2]] * s_used
-            worst = max(worst, float(np.linalg.norm(got - want) / np.linalg.norm(want)))
-            if scale is not None and s_used != 1.0:
-                cnt = scaled.get(id(arr), np.zeros(arr.size, dtype=np.int64))[f * fo:f * fo + no]
-                assert (cnt == 1).all(), f"rank {r} field {f}: an output value is scaled {int(cnt.min())}..{int(cnt.max())} times"
-    return worst
+    return R.error(R.replay(p, inverse, d, spec if inverse else xg, scheds, mutate), want_g * s_used)
 
 
 # ---- replays --------------------------------------------------------------------------------------------------------------
