@@ -80,6 +80,15 @@ static cudaError_t make_table(size_t count, size_t denom, void** dev) {
     return cudaMemcpy(*dev, h.data(), count * sizeof(cx<T>), cudaMemcpyHostToDevice);
 }
 
+// Type-IV table of N-point real lines: one allocation [p_m (N/2 entries)][q_k (N/2 entries)] (r2r.hpp)
+template <typename T>
+static cudaError_t make_r2r4_table(int n, void** dev) {
+    const std::vector<cx<T>> h = r2r4_table<T>(n);
+    cudaError_t e = cudaMalloc(dev, h.size() * sizeof(cx<T>));
+    if (e != cudaSuccess) return e;
+    return cudaMemcpy(*dev, h.data(), h.size() * sizeof(cx<T>), cudaMemcpyHostToDevice);
+}
+
 // Bluestein table of n-point lines: one allocation [K^ (M entries)][chirp (n entries)] (bluestein.hpp)
 template <typename T>
 static cudaError_t make_bluestein_table(size_t n, void** dev) {
@@ -97,25 +106,37 @@ static bool c2c_length(size_t n) { return (ilog2_exact(n) >= 1 && ilog2_exact(n)
 // DFFT_DST when all three kinds are that one, DFFT_R2HC for any other combination (its kinds are in dfft_plan_s::kinds).
 static bool is_r2r(int transform) { return transform == DFFT_DCT || transform == DFFT_DST || transform == DFFT_R2HC; }
 static const char* r2r_name(int k) {
-    return k == DFFT_DST ? "dst" : k == DFFT_R2HC ? "r2hc" : k == DFFT_DCT1 ? "dct1" : k == DFFT_DST1 ? "dst1" : "dct";
+    return k == DFFT_DST    ? "dst"
+           : k == DFFT_R2HC ? "r2hc"
+           : k == DFFT_DCT1 ? "dct1"
+           : k == DFFT_DST1 ? "dst1"
+           : k == DFFT_DCT4 ? "dct4"
+           : k == DFFT_DST4 ? "dst4"
+                            : "dct";
 }
 static bool r2r_length(size_t n) { return ilog2_exact(n) >= 1 && ilog2_exact(n) <= MAX_LOG2N; }
 // Type-I kinds (DFFT_DCT1, DFFT_DST1): axis kinds of per-axis plans (transform DFFT_R2HC) and of dfft_fft1d_r2r only.  An
 // axis of L points runs N-point complex lines: L = N + 1 (DCT-I, N in [2, 8192]) or L = N - 1 (DST-I, N in [4, 8192]).
 static bool is_type1(int kind) { return kind == DFFT_DCT1 || kind == DFFT_DST1; }
-static bool is_r2r_kind(int kind) { return is_r2r(kind) || is_type1(kind); }
+// Type-IV kinds (DFFT_DCT4, DFFT_DST4): axis kinds like type I, of N points, N a power of two in [4, 8192]; a pass runs
+// N/2-point complex lines
+static bool is_type4(int kind) { return kind == DFFT_DCT4 || kind == DFFT_DST4; }
+static bool is_r2r_kind(int kind) { return is_r2r(kind) || is_type1(kind) || is_type4(kind); }
 // log2 N of a type-I axis of L points, -1 for a length the kind does not take
 static int type1_log2(int kind, size_t L) {
     const int l2 = kind == DFFT_DCT1 ? (L >= 3 ? ilog2_exact(L - 1) : -1) : ilog2_exact(L + 1);
     return l2 >= (kind == DFFT_DCT1 ? 1 : 2) && l2 <= MAX_LOG2N ? l2 : -1;
 }
 // the lengths an axis of R2R kind `kind` takes
-static bool r2r_kind_length(int kind, size_t n) { return is_type1(kind) ? type1_log2(kind, n) > 0 : r2r_length(n); }
+static bool r2r_kind_length(int kind, size_t n) {
+    return is_type1(kind) ? type1_log2(kind, n) > 0 : is_type4(kind) ? n >= 4 && r2r_length(n) : r2r_length(n);
+}
 
 // One FFT pass of n-point lines (R2C / C2R: n complex points) over the views of prm, its stores scaled by `scale`: the
 // power-of-two kernels, or the Bluestein pass when n is not a power of two (prm.tw: the M-point table; blu: the Bluestein
 // table of n).  PASS_R2R_*: the R2R kernel of kind r2r (DFFT_DCT, DFFT_DST with prm.tw2 its w_k table, or DFFT_R2HC), or
-// the type-I kernel (DFFT_DCT1, DFFT_DST1: n = N +- 1 reals, prm.tw2 the 2N-point table).
+// the type-I kernel (DFFT_DCT1, DFFT_DST1: n = N +- 1 reals, prm.tw2 the 2N-point table), or the type-IV kernel
+// (DFFT_DCT4, DFFT_DST4: n reals through n/2-point lines, prm.tw2 the type-IV table).
 // hole: passes of padded plans that keep part of their spectral side, the hole [hole[0], hole[1]) of their lines
 // (pass_hole); the padded twin of the power-of-two kernel runs then.
 static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftParams& prm, const void* blu, double scale, cudaStream_t stream,
@@ -133,9 +154,10 @@ static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftP
         FftR2r r;
         static_cast<FftParams&>(r) = prm;
         r.w = prm.tw2;
-        r.dst = r2r == DFFT_DST || r2r == DFFT_DST1;
+        r.dst = r2r == DFFT_DST || r2r == DFFT_DST1 || r2r == DFFT_DST4;
         r.scale = scale;
         if (is_type1(r2r)) return launch_r2r1(prec, type1_log2(r2r, n), kind, r, stream);
+        if (is_type4(r2r)) return launch_r2r4(prec, log2n - 1, kind, r, stream);
         return launch_r2r(prec, log2n, kind, r, r2r == DFFT_R2HC, stream);
     }
     if (log2n >= 0) return launch_pass(prec, log2n, kind, prm, scale, stream);
@@ -179,6 +201,7 @@ struct Tables {
     std::map<int, void*> tw;   // log2n -> exp(-2 pi i m / n), m < n
     std::map<int, void*> tw2;  // log2m -> exp(-2 pi i k / 2m), k <= m/2
     std::map<size_t, void*> blu;  // n -> Bluestein table of n-point lines
+    std::map<int, void*> r2r4;    // log2 N -> type-IV table of N-point real lines (r2r4_table)
     std::vector<void*> bytes;  // seg_of_n tables
     cudaError_t get_tw(int log2n, void** out) {
         if (dry) { *out = nullptr; return cudaSuccess; }
@@ -218,6 +241,19 @@ struct Tables {
         *out = it->second;
         return cudaSuccess;
     }
+    cudaError_t get_r2r4(int log2n, void** out) {
+        if (dry) { *out = nullptr; return cudaSuccess; }
+        auto it = r2r4.find(log2n);
+        if (it == r2r4.end()) {
+            void* d = nullptr;
+            const int n = 1 << log2n;
+            cudaError_t e = prec == DFFT_F64 ? make_r2r4_table<double>(n, &d) : make_r2r4_table<float>(n, &d);
+            if (e != cudaSuccess) return e;
+            it = r2r4.emplace(log2n, d).first;
+        }
+        *out = it->second;
+        return cudaSuccess;
+    }
     cudaError_t seg_table(const Split& s, const unsigned char** out) {
         size_t n = s.start.back() + s.size.back();
         std::vector<unsigned char> h(n);
@@ -249,9 +285,10 @@ struct Tables {
         for (auto& kv : tw) cudaFree(kv.second);
         for (auto& kv : tw2) cudaFree(kv.second);
         for (auto& kv : blu) cudaFree(kv.second);
+        for (auto& kv : r2r4) cudaFree(kv.second);
         for (void* p : bytes) cudaFree(p);
         for (auto* v : dry_store) delete v;
-        tw.clear(); tw2.clear(); blu.clear(); bytes.clear(); dry_store.clear(); host_tabs.clear();
+        tw.clear(); tw2.clear(); blu.clear(); r2r4.clear(); bytes.clear(); dry_store.clear(); host_tabs.clear();
     }
 };
 
@@ -265,14 +302,18 @@ static int pass_log2(PassKind kind, size_t n, int r2r = 0) {
 
 // The tables such a pass reads, from T: tw of its power-of-two length, tw2 for R2C / C2R and DCT / DST passes (r2r: the kind
 // of R2R passes; DCT / DST take w_k = exp(-i pi k / 2N), k <= N, the R2C table of length 2N), blu for Bluestein lengths.
-// Type-I passes take tw and tw2 of log2 N (W^k = exp(-i pi k / N), k <= N/2).  One rule for plans and for the single-axis
-// calls.
+// Type-I passes take tw and tw2 of log2 N (W^k = exp(-i pi k / N), k <= N/2).  Type-IV passes take tw of log2 N - 1 and, as
+// tw2, the type-IV table of N.  One rule for plans and for the single-axis calls.
 static int pass_tables(Tables& T, PassKind kind, size_t n, int r2r, void** tw, void** tw2, void** blu) {
     const bool rr = kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED;
     const bool type1 = rr && is_type1(r2r);
     const int l2 = pass_log2(kind, n, rr ? r2r : 0);
     const bool with_w = rr && r2r != DFFT_R2HC && !type1;
     *tw = *tw2 = *blu = nullptr;
+    if (rr && is_type4(r2r)) {
+        if (T.get_tw(l2 - 1, tw) != cudaSuccess || T.get_r2r4(l2, tw2) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
+        return DFFT_SUCCESS;
+    }
     if (!type1 && l2 != ilog2_exact(n) && T.get_blu(n, blu) != cudaSuccess) return fail(DFFT_ERR_CUDA, "Bluestein table allocation failed");
     if (T.get_tw(l2, tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
     if ((kind == PASS_R2C || kind == PASS_C2R || with_w || type1) && T.get_tw2(l2 + (with_w ? 1 : 0), tw2) != cudaSuccess)
@@ -2507,6 +2548,7 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
             if (r2r_kind_length(p->kinds[a], n[a])) continue;
             const std::string what = p->kinds[a] == DFFT_DCT1   ? "DCT-I axes must have 2^k + 1 points in [3, 8193]"
                                      : p->kinds[a] == DFFT_DST1 ? "DST-I axes must have 2^k - 1 points in [3, 8191]"
+                                     : is_type4(p->kinds[a])    ? "DCT-IV / DST-IV axes must have 2^k points in [4, 8192]"
                                                                 : "Nx, Ny, Nz of DCT / DST plans must be powers of two in [2, 8192]";
             delete p;
             return fail(DFFT_ERR_UNSUPPORTED, what);
@@ -2731,8 +2773,9 @@ int dfft_plan_create_r2r(dfft_comm_t comm, const dfft_config* config, int decomp
                          size_t nz, size_t p1, size_t p2, size_t batch, int inplace, int allocate, dfft_plan_t* plan) {
     if (!kinds) return fail(DFFT_ERR_INVALID, "null kinds");
     for (int a = 0; a < 3; ++a)
-        if (!is_r2r_kind(kinds[a])) return fail(DFFT_ERR_INVALID, "kinds must be DFFT_DCT, DFFT_DST, DFFT_R2HC, DFFT_DCT1 or DFFT_DST1");
-    // three DCT (DST) axes make exactly the DCT (DST) plan; type-I kinds, like R2HC, make a per-axis plan
+        if (!is_r2r_kind(kinds[a]))
+            return fail(DFFT_ERR_INVALID, "kinds must be DFFT_DCT, DFFT_DST, DFFT_R2HC, DFFT_DCT1, DFFT_DST1, DFFT_DCT4 or DFFT_DST4");
+    // three DCT (DST) axes make exactly the DCT (DST) plan; type-I and type-IV kinds, like R2HC, make a per-axis plan
     const bool uniform = kinds[0] == kinds[1] && kinds[1] == kinds[2] && (kinds[0] == DFFT_DCT || kinds[0] == DFFT_DST);
     return plan_create(comm, config, decomp, precision, uniform ? kinds[0] : DFFT_R2HC, nx, ny, nz, p1, p2, batch, inplace != 0, allocate, plan,
                        kinds);
@@ -3376,10 +3419,12 @@ int dfft_fft1d_strided(int precision, int direction, size_t a, size_t n, size_t 
 
 int dfft_fft1d_r2r(int precision, int transform, int direction, size_t n, size_t a, size_t b, void* out, const void* in, void* stream) {
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
-    if (!is_r2r_kind(transform)) return fail(DFFT_ERR_INVALID, "transform must be DFFT_DCT, DFFT_DST, DFFT_R2HC, DFFT_DCT1 or DFFT_DST1");
+    if (!is_r2r_kind(transform))
+        return fail(DFFT_ERR_INVALID, "transform must be DFFT_DCT, DFFT_DST, DFFT_R2HC, DFFT_DCT1, DFFT_DST1, DFFT_DCT4 or DFFT_DST4");
     if (!r2r_kind_length(transform, n))
         return fail(DFFT_ERR_UNSUPPORTED, transform == DFFT_DCT1   ? "DCT-I length must be 2^k + 1 in [3, 8193]"
                                           : transform == DFFT_DST1 ? "DST-I length must be 2^k - 1 in [3, 8191]"
+                                          : is_type4(transform)    ? "DCT-IV / DST-IV length must be a power of two in [4, 8192]"
                                                                    : "length must be a power of two in [2, 8192]");
     if (a == 0 || b == 0) return DFFT_SUCCESS;
     if (a * b > size_t(0x7fffffff) || n * b > size_t(1) << 62) return fail(DFFT_ERR_INVALID, "array too large");

@@ -43,6 +43,10 @@ cudaError_t launch_r2r1(int prec, int log2n, PassKind kind, const FftR2r& p, cud
     return dispatch<1, MAX_LOG2N>(prec, log2n, [&](auto t, auto l) { return launch_r2r1<decltype(t), decltype(l)::value>(kind, p, stream); });
 }
 
+cudaError_t launch_r2r4(int prec, int log2m, PassKind kind, const FftR2r& p, cudaStream_t stream) {
+    return dispatch<1, MAX_LOG2N - 1>(prec, log2m, [&](auto t, auto l) { return launch_r2r4<decltype(t), decltype(l)::value>(kind, p, stream); });
+}
+
 cudaError_t launch_copy(int prec, bool real, PassKind kind, const FftCopy& p, cudaStream_t stream) {
     if (prec == DFFT_F64) return real ? launch_copy<double>(kind, p, stream) : launch_copy<cx<double>>(kind, p, stream);
     return real ? launch_copy<float>(kind, p, stream) : launch_copy<cx<float>>(kind, p, stream);

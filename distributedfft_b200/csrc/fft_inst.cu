@@ -359,11 +359,13 @@ cudaError_t launch_r2r(PassKind kind, const FftR2r& p, bool hc, cudaStream_t str
 
 template cudaError_t launch_r2r<DFFT_T, DFFT_LOG2N>(PassKind, const FftR2r&, bool, cudaStream_t);
 
-// CONTIG: TBC lines per CTA.  TILED: one real per tile column, so the wide tile of the length (2 TBT columns where it fits
-// 128 KB and 1024 threads) gives rows of 2 TBT reals, the row width of the paired R2R tile (>= 64 bytes); lengths whose
-// wide tile does not fit keep TBT columns.  The tile order is the C2C pass's (tile_swz_for).
-template <typename T, int LOG2N>
-cudaError_t launch_r2r1(PassKind kind, const FftR2r& p_in, cudaStream_t stream) {
+// The passes that run one real line per complex 2^LOG2N-point line of the tile (type I: fft_r2r1_kernel, type IV:
+// fft_r2r4_kernel), KC / KT the kernel's CONTIG / TILED instantiation.  CONTIG: TBC lines per CTA.  TILED: one real per
+// tile column, so the wide tile of the length (2 TBT columns where it fits 128 KB and 1024 threads) gives rows of 2 TBT
+// reals, the row width of the paired R2R tile (>= 64 bytes); lengths whose wide tile does not fit keep TBT columns.  The
+// tile order is the C2C pass's (tile_swz_for).
+template <typename T, int LOG2N, auto KC, auto KT>
+static cudaError_t launch_real_lines(PassKind kind, const FftR2r& p_in, cudaStream_t stream) {
     using S = Shape<T, LOG2N>;
     constexpr int LOG2E = S::LOG2E;
     if (!p_in.w || !p_in.tw) return cudaErrorInvalidValue;
@@ -376,8 +378,7 @@ cudaError_t launch_r2r1(PassKind kind, const FftR2r& p_in, cudaStream_t stream) 
         if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
         const long long grid = (lines + S::TBC - 1) / S::TBC;
         if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-        constexpr auto k = fft_r2r1_kernel<T, LOG2N, LOG2E, S::TBC, false>;
-        return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+        return launch_kernel<KC, KC, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
     }
     if (kind != PASS_R2R_TILED) return cudaErrorInvalidValue;
     if (p.B <= 0) return cudaSuccess;
@@ -385,11 +386,29 @@ cudaError_t launch_r2r1(PassKind kind, const FftR2r& p_in, cudaStream_t stream) 
     using C = CtaFft<T, LOG2N, LOG2E, TB, true>;
     const long long grid = lines * ((p.B + TB - 1) / TB);
     if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-    constexpr auto k = fft_r2r1_kernel<T, LOG2N, LOG2E, TB, true>;
-    return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+    return launch_kernel<KT, KT, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+}
+
+template <typename T, int LOG2N>
+cudaError_t launch_r2r1(PassKind kind, const FftR2r& p, cudaStream_t stream) {
+    using S = Shape<T, LOG2N>;
+    return launch_real_lines<T, LOG2N, fft_r2r1_kernel<T, LOG2N, S::LOG2E, S::TBC, false>, fft_r2r1_kernel<T, LOG2N, S::LOG2E, S::TBT_WIDE, true>>(
+        kind, p, stream);
 }
 
 template cudaError_t launch_r2r1<DFFT_T, DFFT_LOG2N>(PassKind, const FftR2r&, cudaStream_t);
+
+// N = 2^(LOG2M + 1) reals per line, so the longest line (8192) runs 4096-point complex lines: no LOG2M = 13 unit
+#if DFFT_LOG2N < 13
+template <typename T, int LOG2M>
+cudaError_t launch_r2r4(PassKind kind, const FftR2r& p, cudaStream_t stream) {
+    using S = Shape<T, LOG2M>;
+    return launch_real_lines<T, LOG2M, fft_r2r4_kernel<T, LOG2M, S::LOG2E, S::TBC, false>, fft_r2r4_kernel<T, LOG2M, S::LOG2E, S::TBT_WIDE, true>>(
+        kind, p, stream);
+}
+
+template cudaError_t launch_r2r4<DFFT_T, DFFT_LOG2N>(PassKind, const FftR2r&, cudaStream_t);
+#endif
 
 #if DFFT_LOG2N == 1
 // CONTIG: lines of up to COPY_THREADS threads (the power of two >= n), COPY_THREADS / that many lines per CTA; TILED: rows

@@ -1961,6 +1961,64 @@ fft_r2r1_kernel(const __grid_constant__ FftR2r p) {
     if (j == 0) emit(N / 2);
 }
 
+// ---- type-IV real-to-real pass: DCT-IV and DST-IV of N = 2M reals per line ------------------------------------------------
+// One real line per complex M-point line of the tile (r2r.hpp): point m loads x_{2m} and x_{N-1-2m} and multiplies by p_m,
+// CtaFft's stages transform v (p.tw: the M-point table), and point k multiplies V_k by q_k and stores y_{2k} and y_{N-1-2k}
+// straight from its final slot: no shared-memory round trip after the stages.  p.w is the type-IV table [p_m][q_k]
+// (Tables::get_r2r4), p.dst picks the kind, p.inverse is not read: the transform is its own inverse.  The views count in
+// reals.
+//   CONTIG: TB real lines per CTA, one per line slot.
+//   TILED:  one real column per tile column (TB columns: the wide tile of the length where shared memory allows it).
+// One CTA per tile and every load before any store (the stages synchronise the line's threads), so out == in works.  A
+// scale != 1 multiplies the stores (__dmul_rn / __fmul_rn: the scaled output is the unscaled one times s, bit for bit).
+template <typename T, int LOG2M, int LOG2E, int TB, bool TILED>
+__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
+fft_r2r4_kernel(const __grid_constant__ FftR2r p) {
+    using C = CtaFft<T, LOG2M, LOG2E, TB, TILED>;
+    using LA = LineAccess<T, C::LINES, T>;
+    constexpr int E = C::E, TPL = C::TPL, M = C::N, N = 2 * M;
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
+    unsigned long long* tab_in = reinterpret_cast<unsigned long long*>(smem_raw + C::TILE_BYTES);
+    unsigned long long* tab_out = tab_in + C::LINES * MAXSEG;
+    const TileCoord<C, TILED, TB> tc(p);
+    const int j = tc.j, t = tc.t;
+    if (p.in.nseg > 1 || p.out.nseg > 1) {
+        // TILED: one table per CTA, CONTIG: one per line (as in c2c_tile)
+        const int line = TILED ? 0 : t, lane = TILED ? int(threadIdx.x) : j, lanes = TILED ? C::THREADS : TPL;
+        LA::fill_table(p.in, tab_in, line, lane, lanes, tc.a0, tc.a1);
+        LA::fill_table(p.out, tab_out, line, lane, lanes, tc.a0, tc.a1);
+        __syncthreads();
+    }
+    const LA in(p.in, tab_in, TILED ? 0 : t, tc.a0, tc.a1, tc.b), out(p.out, tab_out, TILED ? 0 : t, tc.a0, tc.a1, tc.b);
+    const int dst = p.dst;
+    const cx<T>* w = reinterpret_cast<const cx<T>*>(p.w);
+    auto at = [&](const LA& a, int n) -> T* {
+        if constexpr (TILED) return a.at(n);
+        else return a.at1(n);
+    };
+    cx<T> v[E];
+#pragma unroll
+    for (int e = 0; e < E; ++e) {
+        const int m = j + e * TPL;
+        const T lo = tc.valid ? *at(in, r2r4_lo(m)) : T(0), hi = tc.valid ? *at(in, r2r4_hi(m, N)) : T(0);
+        v[e] = r2r4_pre<T>(lo, hi, ld_tw(w, m), dst);
+    }
+    C::template stages<0>(v, j, t, sm, reinterpret_cast<const cx<T>*>(p.tw));
+    if (!tc.valid) return;
+    const bool scaled = p.scale != 1.0;
+    const T s = T(p.scale);
+#pragma unroll
+    for (int e = 0; e < E; ++e) {
+        const int k = j + e * TPL;
+        T lo, hi;
+        r2r4_post<T>(v[C::Core::final_slot(e)], ld_tw(w, M + k), dst, lo, hi);
+        if (scaled) { lo = rscale<T>(lo, s); hi = rscale<T>(hi, s); }
+        *at(out, r2r4_lo(k)) = lo;
+        *at(out, r2r4_hi(k, N)) = hi;
+    }
+}
+
 // ---- copy pass: an axis the plan keeps (dfft_plan_set_transform_axes) ------------------------------------------------
 // Moves element (a0, a1, n, b) of p.in to the same index of p.out for any line length p.n, through the segmented views of
 // the FFT pass it replaces (scatters into peer slots, gathers from receive slots, blocked layouts and tails unchanged).
@@ -2114,6 +2172,13 @@ cudaError_t launch_r2r(int prec, int log2n, PassKind kind, const FftR2r& p, bool
 template <typename T, int LOG2N>
 cudaError_t launch_r2r1(PassKind kind, const FftR2r& p, cudaStream_t stream);
 cudaError_t launch_r2r1(int prec, int log2n, PassKind kind, const FftR2r& p, cudaStream_t stream);
+
+// DCT-IV / DST-IV pass (fft_r2r4_kernel, p.dst) of real lines of 2^(LOG2M + 1) points through M-point complex lines: kinds
+// and views as for launch_r2r1; p.tw = Tables::get_tw(LOG2M), p.w = Tables::get_r2r4(LOG2M + 1), p.scale scales the
+// stores.  Instantiated for LOG2M 1..12.
+template <typename T, int LOG2M>
+cudaError_t launch_r2r4(PassKind kind, const FftR2r& p, cudaStream_t stream);
+cudaError_t launch_r2r4(int prec, int log2m, PassKind kind, const FftR2r& p, cudaStream_t stream);
 
 // copy pass of p.n-point lines (fft_copy_kernel): kind PASS_COPY_CONTIG or PASS_COPY_TILED, p.ltpl is filled in here.
 // Instantiated for E = T and cx<T> in the LOG2N = 1 unit of each precision; the runtime form takes real != 0 for the

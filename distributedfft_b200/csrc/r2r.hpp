@@ -1,5 +1,5 @@
-// r2r.hpp — per-point arithmetic of the real-to-real passes (fft_r2r_kernel, fft_r2hc_kernel), shared with
-// tests/emu_r2r.cpp and tests/emu_r2hc.cpp.
+// r2r.hpp — per-point arithmetic of the real-to-real passes (fft_r2r_kernel, fft_r2hc_kernel, fft_r2r1_kernel,
+// fft_r2r4_kernel), shared with tests/emu_r2r.cpp, tests/emu_r2hc.cpp, tests/emu_r2r1.cpp and tests/emu_r2r4.cpp.
 //
 // Two real N-point lines a and b are transformed through one complex N-point FFT (CtaFft's stages):
 //   perm:     v[n] = x[2n],  v[N-1-n] = x[2n+1]  (n < N/2);  z = v_a + i v_b
@@ -10,6 +10,9 @@
 //   DST-II(x) = reverse(DCT-II((-1)^n x)),  DST-III(X) = (-1)^n DCT-III(reverse(X))
 // Unnormalised like FFTW's REDFT10 / REDFT01 / RODFT10 / RODFT01: DCT-III(DCT-II(x)) = 2N x.
 #pragma once
+#include <cmath>
+#include <vector>
+
 #include "fft_core.cuh"
 
 namespace dfft {
@@ -105,6 +108,45 @@ DFFT_HD void r2r1_split(cx<T> zk, cx<T> zm, cx<T> w, cx<T>& ek, cx<T>& enk) {
 DFFT_HD int r2r1_out_index(int k, int N, int dst) { return !dst ? k : (k == 0 || k == N ? -1 : k - 1); }
 template <typename T>
 DFFT_HD T r2r1_value(cx<T> e, int dst) { return dst ? -e.y : e.x; }
+
+// ---- DCT-IV / DST-IV (fft_r2r4_kernel): one real line per complex M-point FFT, M = N/2 -----------------------------------
+// FFTW's REDFT11 / RODFT11 of N points, unnormalised like scipy's dct / dst with type=4:
+//   DCT-IV:  y_k = 2 sum_{n<N} x_n cos(pi (2n+1)(2k+1) / 4N)        DST-IV:  the same with sin
+// Point m < M packs the reals x_{2m} and x_{N-1-2m}; with p_m = exp(-i pi (4m+1) / 4N) and q_k = exp(-i pi k / N):
+//   v_m = (x_{2m} + i x_{N-1-2m}) p_m,  V = DFT_M(v),  c_k = V_k q_k,  y_{2k} = 2 Re c_k,  y_{N-1-2k} = -2 Im c_k
+// DST-IV(x)_k = (-1)^k DCT-IV(reverse x)_k: the packed point takes its two reals swapped and y_{N-1-2k} = +2 Im c_k.
+// Point k's outputs sit at the same index pair as point m's inputs, so each point stores its own results.  One line per
+// FFT (no pairing): each line's error follows its own norm.  Each transform is its own inverse up to 2N.
+
+// the reals of packed point m (and outputs of point k): x_{2m} and x_{N-1-2m}
+DFFT_HD int r2r4_lo(int m) { return 2 * m; }
+DFFT_HD int r2r4_hi(int m, int N) { return N - 1 - 2 * m; }
+
+// v_m from x_{2m} (lo), x_{N-1-2m} (hi) and p = p_m
+template <typename T>
+DFFT_HD cx<T> r2r4_pre(T lo, T hi, cx<T> p, int dst) { return cmul(dst ? cx<T>{hi, lo} : cx<T>{lo, hi}, p); }
+
+// y_{2k} (lo) and y_{N-1-2k} (hi) from V_k and q = q_k
+template <typename T>
+DFFT_HD void r2r4_post(cx<T> v, cx<T> q, int dst, T& lo, T& hi) {
+    const cx<T> c = cmul(v, q);
+    lo = T(2) * c.x;
+    hi = (dst ? T(2) : T(-2)) * c.y;
+}
+
+// The type-IV table of N-point lines: [p_m (M entries)][q_k (M entries)], evaluated in long double and rounded once
+template <typename T>
+std::vector<cx<T>> r2r4_table(int N) {
+    const int M = N / 2;
+    const long double pi = 3.14159265358979323846264338327950288L;
+    std::vector<cx<T>> h(size_t(2) * M);
+    for (int m = 0; m < M; ++m) {
+        const long double a = -pi * (4.0L * m + 1.0L) / (4.0L * N), b = -pi * m / N;
+        h[m] = cx<T>{T(cosl(a)), T(sinl(a))};
+        h[M + m] = cx<T>{T(cosl(b)), T(sinl(b))};
+    }
+    return h;
+}
 
 // ---- R2C / C2R z pass of interleaved plans (fft_rc_ilv_kernel)---------------------------------------------------------------
 // Every component runs its own complex Nz-point line z = x + 0i.  (Two components sharing one line as z = x_a + i x_b would

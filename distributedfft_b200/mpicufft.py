@@ -18,7 +18,8 @@ SLAB_ZY_THEN_X, SLAB_Z_THEN_YX, PENCIL = 0, 1, 2
 F32, F64 = 0, 1
 R2C, C2C, DCT, DST, R2HC = 0, 1, 2, 3, 4
 DCT1, DST1 = 16, 17  # type-I kinds (DCT-I / DST-I): per-axis plans and fft1d_r2r only
-_R2R_KINDS = {"dct": DCT, "dst": DST, "r2hc": R2HC, "dct1": DCT1, "dst1": DST1}
+DCT4, DST4 = 19, 20  # type-IV kinds (DCT-IV / DST-IV): per-axis plans and fft1d_r2r only
+_R2R_KINDS = {"dct": DCT, "dst": DST, "r2hc": R2HC, "dct1": DCT1, "dst1": DST1, "dct4": DCT4, "dst4": DST4}
 FORWARD, INVERSE = -1, 1
 
 
@@ -87,10 +88,12 @@ class Comm:
 class MPIcuFFT:
     """Abstract plan (include/mpicufft.hpp:55-105). `precision`: 'double' | 'float' replaces the C++
     template argument; `transform`: 'r2c' (the reference's), 'c2c', or the real-to-real 'dct' / 'dst' (type II forward, type III
-    inverse, on all three axes; execR2R).  A tuple of three names from 'dct', 'dst', 'r2hc', 'dct1', 'dst1', in (x, y, z)
-    order, gives a real-to-real plan with a kind per axis (dfft_plan_create_r2r; 'r2hc': FFTW's R2HC forward, HC2R inverse;
-    'dct1' / 'dst1': DCT-I / DST-I both ways, FFTW's REDFT00 / RODFT00, on axes of 2^k + 1 / 2^k - 1 points), e.g.
-    ("dct1", "r2hc", "r2hc") for a Chebyshev wall-normal x axis."""
+    inverse, on all three axes; execR2R).  A tuple of three names from 'dct', 'dst', 'r2hc', 'dct1', 'dst1', 'dct4', 'dst4',
+    in (x, y, z) order, gives a real-to-real plan with a kind per axis (dfft_plan_create_r2r; 'r2hc': FFTW's R2HC forward,
+    HC2R inverse; 'dct1' / 'dst1': DCT-I / DST-I both ways, FFTW's REDFT00 / RODFT00, on axes of 2^k + 1 / 2^k - 1 points;
+    'dct4' / 'dst4': DCT-IV / DST-IV both ways, FFTW's REDFT11 / RODFT11, on cell-centred axes of 2^k points, 4..8192, with
+    a Neumann wall at one end and a Dirichlet wall at the other), e.g. ("dct1", "r2hc", "r2hc") for a Chebyshev
+    wall-normal x axis or ("dct4", "r2hc", "r2hc") for a channel with a no-slip bed and a free-slip lid."""
 
     _decomp = SLAB_ZY_THEN_X
 
@@ -107,7 +110,7 @@ class MPIcuFFT:
         self.kinds = None
         if isinstance(transform, tuple):
             if len(transform) != 3 or not all(isinstance(k, str) and k.lower() in _R2R_KINDS for k in transform):
-                raise ValueError(f"a per-axis transform is three of 'dct', 'dst', 'r2hc', 'dct1', 'dst1', got {transform!r}")
+                raise ValueError(f"a per-axis transform is three of 'dct', 'dst', 'r2hc', 'dct1', 'dst1', 'dct4', 'dst4', got {transform!r}")
             self.kinds = tuple(_R2R_KINDS[k.lower()] for k in transform)
             # as the library records it: three DCT (DST) axes are the DCT (DST) plan, every other combination a per-axis one
             uniform = len(set(self.kinds)) == 1 and self.kinds[0] in (DCT, DST)
@@ -264,7 +267,7 @@ class MPIcuFFT:
     def execR2R(self, out, in_, direction: int = FORWARD, d: int = 3, stream=None):
         """Real-to-real transform of a 'dct' / 'dst' or per-axis plan (not in the reference): FORWARD is type II (R2HC on
         'r2hc' axes), INVERSE type III (HC2R), all unnormalised like scipy.fft.dct / dst(norm=None); 'dct1' / 'dst1' axes
-        run DCT-I / DST-I (type=1) in both directions.  Real [x][y][z] buffers.  `stream` as for execR2C, capturable the
+        run DCT-I / DST-I (type=1) and 'dct4' / 'dst4' axes DCT-IV / DST-IV (type=4) in both directions.  Real [x][y][z] buffers.  `stream` as for execR2C, capturable the
         same way."""
         self._need()
         if stream is not None:
@@ -276,7 +279,7 @@ class MPIcuFFT:
         return check(lib().dfft_exec_r2r_partial(self._h, _ptr(out), _ptr(in_), direction, d))
 
     def getR2RKinds(self):
-        """(x, y, z) kinds of a real-to-real plan: DCT, DST, R2HC, DCT1 or DST1 each (dfft_plan_get_r2r_kinds)."""
+        """(x, y, z) kinds of a real-to-real plan: DCT, DST, R2HC, DCT1, DST1, DCT4 or DST4 each (dfft_plan_get_r2r_kinds)."""
         self._need()
         k = (C.c_int * 3)()
         check(lib().dfft_plan_get_r2r_kinds(self._h, k))
@@ -427,7 +430,8 @@ def fft1d_strided(precision: int, direction: int, a: int, n: int, b: int, out, i
 def fft1d_r2r(precision: int, transform: int, direction: int, n: int, a: int, b: int, out, in_, stream=None):
     """DCT / DST / R2HC (transform DCT, DST or R2HC; FORWARD type II or R2HC, INVERSE type III or HC2R) along the middle
     axis of a dense real [a][n][b] array, b contiguous; out may be in_.  DCT1 / DST1: DCT-I / DST-I in both directions,
-    n = 2^k + 1 (DCT-I, 3..8193) or 2^k - 1 (DST-I, 3..8191)."""
+    n = 2^k + 1 (DCT-I, 3..8193) or 2^k - 1 (DST-I, 3..8191).  DCT4 / DST4: DCT-IV / DST-IV in both directions, n = 2^k
+    in 4..8192."""
     check(lib().dfft_fft1d_r2r(precision, transform, direction, n, a, b, _ptr(out), _ptr(in_), _stream_ptr(stream)))
 
 

@@ -111,6 +111,17 @@ typedef enum { DFFT_R2C = 0, DFFT_C2C = 1, DFFT_DCT = 2, DFFT_DST = 3, DFFT_R2HC
  * so an axis takes L = 3, 5, 9, ..., 8193 (DCT-I) or 3, 7, 15, ..., 8191 (DST-I); any other length DFFT_ERR_UNSUPPORTED.
  * Each is its own inverse up to 2N: forward and inverse execs run the same transform on such an axis. */
 enum { DFFT_DCT1 = 16, DFFT_DST1 = 17 };
+/* DFFT_DCT4 / DFFT_DST4 (not in the reference; FFTW's REDFT11 / RODFT11, scipy.fft.dct / dst with type=4, norm=None): the
+ * type-IV transforms of cell-centred axes whose two walls differ, N points, N a power of two in [4, 8192] (other lengths,
+ * N = 2 included: DFFT_ERR_UNSUPPORTED):
+ *   DCT-IV:  y_k = 2 sum_{n<N} x_n cos(pi (2n+1)(2k+1) / 4N)   Neumann at the low face (u_{-1} = u_0), Dirichlet at the high
+ *                                                             one (u_N = -u_{N-1})
+ *   DST-IV:  y_k = 2 sum_{n<N} x_n sin(pi (2n+1)(2k+1) / 4N)   Dirichlet at the low face, Neumann at the high one
+ * Each diagonalises the 3-point second difference with those ghost rules, eigenvalues -4 sin^2(pi (2k+1) / 4N) (none zero).
+ * Kinds only, like DFFT_DCT1 / DFFT_DST1: for dfft_plan_create_r2r and dfft_fft1d_r2r; dfft_plan_create* return
+ * DFFT_ERR_INVALID for transforms 19 and 20.  Each is its own inverse up to 2N: forward and inverse execs run the same
+ * transform on such an axis. */
+enum { DFFT_DCT4 = 19, DFFT_DST4 = 20 };
 
 typedef struct dfft_comm_s* dfft_comm_t;
 typedef struct dfft_plan_s* dfft_plan_t;
@@ -173,19 +184,21 @@ int dfft_plan_create_inplace(dfft_comm_t comm, const dfft_config* config, int de
                              size_t nz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan);
 int dfft_plan_is_inplace(dfft_plan_t plan); /* 1 for plans of dfft_plan_create_inplace, 0 otherwise (and for a null plan) */
 /* Real-to-real plans with a kind per axis (FFTW's fftw_plan_r2r with one kind per dimension): kinds[0], [1], [2] are the
- * kinds of the x, y and z axis, each DFFT_DCT (Neumann), DFFT_DST (Dirichlet), DFFT_R2HC (periodic), or DFFT_DCT1 /
- * DFFT_DST1 (Neumann / Dirichlet on vertex-centred or Chebyshev axes).  Everything said of DFFT_DCT / DFFT_DST plans above
- * holds: real [x][y][z] buffers, powers of two in [2, 8192] (type-I axes: the lengths of DFFT_DCT1 / DFFT_DST1; others:
+ * kinds of the x, y and z axis, each DFFT_DCT (Neumann), DFFT_DST (Dirichlet), DFFT_R2HC (periodic), DFFT_DCT1 /
+ * DFFT_DST1 (Neumann / Dirichlet on vertex-centred or Chebyshev axes), or DFFT_DCT4 / DFFT_DST4 (cell-centred, Neumann at
+ * one face and Dirichlet at the other).  Everything said of DFFT_DCT / DFFT_DST plans above holds: real [x][y][z] buffers,
+ * powers of two in [2, 8192] (type-I axes: the lengths of DFFT_DCT1 / DFFT_DST1; type-IV axes: [4, 8192]; others:
  * DFFT_ERR_UNSUPPORTED), dfft_exec_r2r* (forward: DCT-II, DST-II or R2HC on each axis; inverse: DCT-III, DST-III or
- * HC2R; DCT-I and DST-I both ways), partial d over the first d axes in z, y, x order, each with its own kind, and
- * dfft_layout with DFFT_DCT.
+ * HC2R; DCT-I, DST-I, DCT-IV and DST-IV both ways), partial d over the first d axes in z, y, x order, each with its own
+ * kind, and dfft_layout with DFFT_DCT.
  * `batch` and `inplace` (!= 0) mean what they mean for dfft_plan_create_batched / dfft_plan_create_inplace.
- *   - A round trip scales by the product over the transformed axes of N (R2HC) or 2N (DCT, DST, and DCT-I / DST-I with
- *     their N = L - 1 / L + 1).
+ *   - A round trip scales by the product over the transformed axes of N (R2HC) or 2N (DCT, DST, DCT-IV / DST-IV, and
+ *     DCT-I / DST-I with their N = L - 1 / L + 1).
  *   - Three DFFT_DCT (DFFT_DST) kinds make the DFFT_DCT (DFFT_DST) plan: the same steps, description and output.  Other
- *     combinations, type-I kinds included: dfft_plan_describe reports "r2r_kinds" and, per R2R pass, "r2r" (the kind of its
- *     axis: "dct", "dst", "r2hc", "dct1" or "dst1").
- *   - A null kinds or a kind outside {DFFT_DCT, DFFT_DST, DFFT_R2HC, DFFT_DCT1, DFFT_DST1}: DFFT_ERR_INVALID. */
+ *     combinations, type-I and type-IV kinds included: dfft_plan_describe reports "r2r_kinds" and, per R2R pass, "r2r"
+ *     (the kind of its axis: "dct", "dst", "r2hc", "dct1", "dst1", "dct4" or "dst4").
+ *   - A null kinds or a kind outside {DFFT_DCT, DFFT_DST, DFFT_R2HC, DFFT_DCT1, DFFT_DST1, DFFT_DCT4, DFFT_DST4}:
+ *     DFFT_ERR_INVALID. */
 int dfft_plan_create_r2r(dfft_comm_t comm, const dfft_config* config, int decomp /*dfft_decomp*/, int precision /*dfft_prec*/,
                          const int kinds[3], size_t nx, size_t ny, size_t nz, size_t p1, size_t p2, size_t batch, int inplace,
                          int allocate, dfft_plan_t* plan);
@@ -402,7 +415,8 @@ int dfft_fft1d_strided(int precision, int direction, size_t a, size_t n, size_t 
 
 /* DCT / DST / R2HC (transform DFFT_DCT, DFFT_DST or DFFT_R2HC; forward type II or R2HC, inverse type III or HC2R,
  * unnormalised) along the middle axis of a dense real [a][n][b] array, b contiguous; n a power of two in [2, 8192].
- * DFFT_DCT1 / DFFT_DST1: DCT-I / DST-I in both directions, n one of the lengths of that kind.  out == in is allowed. */
+ * DFFT_DCT1 / DFFT_DST1: DCT-I / DST-I in both directions, n one of the lengths of that kind.  DFFT_DCT4 / DFFT_DST4:
+ * DCT-IV / DST-IV in both directions, n a power of two in [4, 8192].  out == in is allowed. */
 int dfft_fft1d_r2r(int precision, int transform, int direction, size_t n, size_t a, size_t b, void* out, const void* in,
                    void* stream);
 

@@ -77,7 +77,7 @@ public:
         pcnt = dfft_comm_size(comm);
     }
     // not in the reference: a real-to-real plan with a kind per axis — kinds_[0..2] of x, y, z, each DFFT_DCT, DFFT_DST,
-    // DFFT_R2HC, DFFT_DCT1 or DFFT_DST1; initFFT creates it with dfft_plan_create_r2r and execR2R runs it
+    // DFFT_R2HC, DFFT_DCT1, DFFT_DST1, DFFT_DCT4 or DFFT_DST4; initFFT creates it with dfft_plan_create_r2r and execR2R runs it
     MPIcuFFT(Configurations config_, dfft_comm_t comm_, int max_world_size, const int (&kinds_)[3])
         : MPIcuFFT(config_, comm_, max_world_size, DFFT_R2HC) {
         per_axis = true;
