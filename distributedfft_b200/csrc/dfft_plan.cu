@@ -21,6 +21,7 @@
 #include <sys/stat.h>
 
 #include <algorithm>
+#include <array>
 #include <chrono>
 #include <cmath>
 #include <fstream>
@@ -446,6 +447,22 @@ struct Schedule {
     int inverse = 0;          // direction (selects the plan's output scale)
 };
 
+// The work slots of the schedules, in the order they lie in the work area: D1 and D2 receive the first and the second
+// transposition by peer stores (or hold it on a one-member group), SS and SR are the send and receive slots of the
+// all-to-all transpositions; -1: the plan has no such slot.
+struct Slots {
+    int D1 = -1, D2 = -1, SS = -1, SR = -1;
+    int count = 0;
+};
+// direct1 / direct2: whether the first / second transposition is direct (peer stores, or a one-member group)
+static Slots plan_slots(bool direct1, bool direct2) {
+    Slots s;
+    if (direct1) s.D1 = s.count++;
+    if (direct2) s.D2 = s.count++;
+    if (!direct1 || !direct2) { s.SS = s.count++; s.SR = s.count++; }
+    return s;
+}
+
 }  // namespace dfft
 
 struct dfft_plan_s {
@@ -467,14 +484,18 @@ struct dfft_plan_s {
     bool inplace = false, buf_slot = false;
     size_t domain_bytes = 0;  // this rank (getDomainSize)
     size_t slot_bytes = 0;    // uniform over ranks
-    int nslots = 2;
+    dfft::Slots slots;        // the schedules' slot ids (plan_slots)
+    int nslots = 2;           // slots allocated in the work area
     size_t work_bytes = 0;
     void* work = nullptr;
     bool work_owned = false;
     bool any_direct = false;  // some transposition uses peer stores across >1 ranks
     bool direct1 = true, direct2 = true;
     // peer mapping
-    std::vector<std::vector<void*>> slot_ptr;  // [slot][rank]
+    std::vector<std::vector<void*>> slot_ptr;  // [allocated slot][rank]
+    // Slot s (Slots) of rank r.  buf_slot: D1 is the caller's buffer, a null base (its views hold byte offsets, which
+    // relocate_buffer_views turns into views on the buffer), and the allocated slots start at the next one.
+    void* slot(int s, int r) const { return !buf_slot ? slot_ptr[s][r] : s == slots.D1 ? nullptr : slot_ptr[s - 1][r]; }
     std::vector<void*> opened;                 // IPC mappings to close
     unsigned long long* flags = nullptr;       // my flags (NPHASE * P)
     unsigned long long** peer_flags_d = nullptr;
@@ -677,7 +698,6 @@ static bool batch_small(const dfft_plan_s* p, int d) {
 
 static int build_batch_small(dfft_plan_s* p, int inverse, Schedule& sc) {
     const size_t N = p->g.nx;
-    sc.steps.clear();
     sc.whole_batch = true;
     Step s;
     s.type = STEP_PASS;
@@ -710,7 +730,6 @@ static int build_batch_small(dfft_plan_s* p, int inverse, Schedule& sc) {
         s.bsf.ctr = reinterpret_cast<unsigned long long*>(c);
     }
     sc.steps.push_back(s);
-    sc.built = true;
     return DFFT_SUCCESS;
 }
 
@@ -787,11 +806,11 @@ struct HandOver {
     const Split* recv = nullptr;  // the receivers' extents along it (forward oy, inverse sx)
     const std::vector<int>* G = nullptr;
     const unsigned char* tab = nullptr;  // segment table of recv (scattering views over more than one receiver)
-    std::vector<void*> slot;             // the hand-over slot of every rank
+    std::vector<void*> slot;             // the hand-over slot (D2) of every rank
 
     // blocked: both transpositions are peer stores and both passes run (d = 3); sequential: the schedule of build_schedule,
     // the only one that takes the x-innermost layout of one rank
-    HandOver(const dfft_plan_s* p, int inverse, bool blocked, bool sequential, const unsigned char* tab_, std::vector<void*> slot_) {
+    HandOver(const dfft_plan_s* p, int inverse, bool blocked, bool sequential, const unsigned char* tab_) {
         const Geometry& g = p->g;
         me = p->rank;
         fwd = !inverse;
@@ -802,9 +821,9 @@ struct HandOver {
         M_me = recv->size[g.pi(me)];
         G = &p->grp[2];
         tab = tab_;
-        slot = std::move(slot_);
         CH = blocked && (fwd || p->blocked_inv) ? size_t(p->blocked_ch) : 0;
         if (!CH) return;
+        for (int r = 0; r < p->P; ++r) slot.push_back(p->slot(p->slots.D2, r));
         rem = nz % CH;
         nzm = nz - rem;
         for (size_t v : g.sz.size) any_rem = any_rem || v % CH != 0;
@@ -883,40 +902,118 @@ struct HandOver {
     }
 };
 
+// The axes of a rank's box of data (x outermost, z innermost), and no axis
+enum BoxAxis { AX = 0, AY = 1, AZ = 2, NO_AXIS = -1 };
+// The box axes a pass's batch indices a0, a1 and its line index n run over (NO_AXIS: stride 0)
+struct Roles {
+    int a0, a1, n;
+};
+using Origin = std::array<size_t, 3>;
+
+// A plain transposition over group 1 or 2: the sending pass transforms axis s and scatters it over the members by `ss`,
+// and the receiving pass gathers axis t, which the senders hold split by `st`, to its whole extent.  The third axis keeps
+// this rank's extent `u`.
+//   direct (peer stores into slot D1 / D2): receiver q's array is the box with ss.size[q] along s and the whole t; each
+//     sender writes its sub-box at st.start of its position along t
+//   all-to-all: the same box with the sender's own extent along t, packed at soff[q] of slot SS, scount[q] elements;
+//     the receive side mirrors it at roff[q] of slot SR — one view when t is x, where the senders' blocks stack
+// The receiving pass transforms t (forward Z_Then_YX: y, with t = x outermost), so its input segments lie along its n axis.
+// `at` moves a view to a sub-box (the plane groups and z chunks of the overlapped schedules).
+struct Transposition {
+    const dfft_plan_s* p;
+    int group, s, t;
+    const Split *ss, *st;
+    size_t u, whole;
+    const unsigned char *tab_s, *tab_t;  // segment tables of ss and st (views over more than one member)
+    const std::vector<int>* G;
+    int pos = 0;  // this rank's position in G
+    bool direct;
+    int D;        // the slot of a direct transposition
+    Step a2a;     // the all-to-all step of one that is not
+
+    Transposition(const dfft_plan_s* p_, int group_, int s_, int t_, const Split& ss_, const Split& st_, size_t u_,
+                  const unsigned char* tab_s_, const unsigned char* tab_t_)
+        : p(p_), group(group_), s(s_), t(t_), ss(&ss_), st(&st_), u(u_), whole(st_.start.back() + st_.size.back()), tab_s(tab_s_),
+          tab_t(tab_t_), G(&p_->grp[group_]) {
+        while ((*G)[pos] != p->rank) ++pos;
+        D = group == 1 ? p->slots.D1 : p->slots.D2;
+        direct = D >= 0;
+        if (direct) return;
+        a2a.type = STEP_A2A;
+        a2a.label = "nccl all-to-all";
+        a2a.group = group;
+        a2a.send_slot = p->slots.SS;
+        a2a.recv_slot = p->slots.SR;
+        size_t so = 0, ro = 0;
+        for (size_t q = 0; q < G->size(); ++q) {
+            a2a.scount.push_back(ss->size[q] * st->size[pos] * u);
+            a2a.rcount.push_back(ss->size[pos] * st->size[q] * u);
+            a2a.soff.push_back(so);
+            a2a.roff.push_back(ro);
+            so += a2a.scount[q];
+            ro += a2a.rcount[q];
+        }
+    }
+    // the sending pass's output: its sub-box of every receiver's array (direct) or of every block of my send slot
+    View send(Roles r, Origin at = {}) const {
+        View v{};
+        if (direct) at[t] += st->start[pos];
+        seg_view(v, tab_s, *G, [&](int q, int rk) {
+            if (direct) return box(p->slot(D, rk), 0, r, ss->size[q], whole, at, ss->start[q]);
+            return box(p->slot(p->slots.SS, p->rank), a2a.soff[q], r, ss->size[q], st->size[pos], at, ss->start[q]);
+        });
+        return v;
+    }
+    // the receiving pass's input: my array in slot D (direct) or the blocks of my receive slot
+    View recv(Roles r, Origin at = {}) const {
+        void* base = p->slot(direct ? D : p->slots.SR, p->rank);
+        if (direct || t == AX) {
+            const SegN b = box(base, 0, r, ss->size[pos], whole, at, 0);
+            return single_view(b.s.base, b.s.sA0, b.s.sA1, b.sN);
+        }
+        View v{};
+        seg_view(v, tab_t, *G, [&](int q, int) { return box(base, a2a.roff[q], r, ss->size[pos], st->size[q], at, st->start[q]); });
+        return v;
+    }
+    // after the sending pass: the all-to-all, or the rendezvous after which every member's stores have landed
+    void finish(Schedule& sc) const {
+        static const char* const names[3][2] = {{"Transpose (Finished Receive)", "Transpose (Finished All2All)"},
+                                                {"First Transpose (Finished Receive)", "First Transpose (Finished All2All)"},
+                                                {"Second Transpose (Finished Receive)", "Second Transpose (Finished All2All)"}};
+        const char* const* name = names[p->g.decomp == DFFT_PENCIL ? group : 0];
+        if (!direct) {
+            sc.steps.push_back(a2a);
+            sc.steps.back().phase = name[1];
+        } else if (G->size() > 1) {
+            sc.steps.push_back(new_rendezvous(group, group, name[0], 0));
+        }
+    }
+
+  private:
+    // the box with extents es_ along s and et along t, from `base` + off elements, at sub-box `at`
+    SegN box(void* base, size_t off, Roles r, size_t es_, size_t et, const Origin& at, size_t n0) const {
+        size_t e[3];
+        e[s] = es_;
+        e[t] = et;
+        e[3 - s - t] = u;
+        const long long stride[3] = {(long long)(e[1] * e[2]), (long long)e[2], 1};
+        auto sr = [&](int axis) { return axis == NO_AXIS ? 0LL : stride[axis]; };
+        return mkseg(eptr(base, off + at[0] * e[1] * e[2] + at[1] * e[2] + at[2], p->esize * p->comps), sr(r.a0), sr(r.a1), sr(r.n), n0);
+    }
+};
+
 static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     const Geometry& g = p->g;
     const int me = p->rank, P = p->P;
     const int pi = g.pi(me), pj = g.pj(me);
-    // bytes per grid point: the views below count points; interleaved plans widen them to values afterwards (widen_views)
-    const size_t es = p->esize * p->comps;
-    // DCT / DST plans run the C2C builders over reals; new_pass turns their C2C kinds into R2R ones
+    // DCT / DST plans run the C2C builders over reals; new_pass turns their C2C kinds into R2R ones.  The views count
+    // points; interleaved plans widen them to values afterwards (widen_views).
     const bool c2c = g.transform != DFFT_R2C;
     Tables& T = p->tabs;
-    sc.steps.clear();
 
     // groups: transposition 1 / 2 member lists (positions along the split axis)
     const std::vector<int>& G1 = p->grp[1];
     const std::vector<int>& G2 = p->grp[2];
-    const bool dir1 = p->direct1 || G1.size() == 1;
-    const bool dir2 = p->direct2 || G2.size() == 1;
-    // slot ids
-    int nxt = 0;
-    int D1 = -1, D2 = -1, SS = -1, SR = -1;
-    if (dir1) D1 = nxt++;
-    if (dir2) D2 = nxt++;
-    if (!dir1 || !dir2) { SS = nxt++; SR = nxt++; }
-    // in-place plans of one rank: D1 is the caller's buffer — its views hold byte offsets (from a null base), which
-    // relocate_buffer_views turns into views on the buffer; the other slots move down by one
-    auto slotp = [&](int s, int r) -> void* {
-        if (p->buf_slot) return s == D1 ? nullptr : p->slot_ptr[s - 1][r];
-        return p->slot_ptr[s][r];
-    };
-    // the second transposition's hand-over in slot D2 (tab: the segment table of the scattering pass's receivers)
-    auto hand_over = [&](bool blocked, const unsigned char* tab) {
-        std::vector<void*> d2(P, nullptr);
-        if (blocked) for (int r = 0; r < P; ++r) d2[r] = slotp(D2, r);
-        return HandOver(p, inverse, blocked, true, tab, d2);
-    };
 
     if (p->any_direct) sc.steps.push_back(new_rendezvous(0, 0, nullptr, 0));  // everyone has left the previous exec: slots are free
 
@@ -928,8 +1025,8 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
 
     // sizes of this rank
     const size_t nx_i = g.sx.size[pi], x0_i = g.sx.start[pi];
-    const size_t ny_j = zyx ? g.ny : g.sy.size[pj], y0_j = zyx ? 0 : g.sy.start[pj];
-    const size_t nz_j = zyx ? g.sz.size[me] : g.sz.size[pj], z0_j = zyx ? g.sz.start[me] : g.sz.start[pj];
+    const size_t ny_j = zyx ? g.ny : g.sy.size[pj];
+    const size_t nz_j = zyx ? g.sz.size[me] : g.sz.size[pj];
     const size_t oy_i = zyx ? ky : g.oy.size[pi], oy0_i = zyx ? 0 : g.oy.start[pi];
 
     const unsigned char *tab_z = nullptr, *tab_y_in = nullptr, *tab_y_out = nullptr, *tab_x = nullptr;
@@ -941,20 +1038,6 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         if (!zyx && T.seg_table(g.oy, &tab_y_out) != cudaSuccess) return fail(DFFT_ERR_CUDA, "segment table");
         if (T.seg_table(g.sx, &tab_x) != cudaSuccess) return fail(DFFT_ERR_CUDA, "segment table");
     }
-
-    auto a2a_counts = [&](Step& s, const std::vector<int>& G, auto send_elems, auto recv_elems) {
-        s.type = STEP_A2A;
-        s.label = "nccl all-to-all";
-        size_t so = 0, ro = 0;
-        s.scount.resize(G.size()); s.soff.resize(G.size()); s.rcount.resize(G.size()); s.roff.resize(G.size());
-        for (size_t q = 0; q < G.size(); ++q) {
-            s.scount[q] = send_elems(int(q));
-            s.rcount[q] = recv_elems(int(q));
-            s.soff[q] = so; s.roff[q] = ro;
-            so += s.scount[q]; ro += s.rcount[q];
-        }
-        s.send_slot = SS; s.recv_slot = SR;
-    };
 
     if (!inverse) {
         // ------------------------------------------------------------------ forward
@@ -972,45 +1055,16 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
             s1.prm.out = single_view(nullptr, (long long)(ny_j * kzc), (long long)kzc, 1);
             s1.out_user = 2;
             sc.steps.push_back(s1);
-            sc.built = true;
             return DFFT_SUCCESS;
         }
-        // transposition 1: scatter along z over G1
-        Step x1;  // optional a2a
-        const bool t1_a2a = !dir1;
-        if (zyx) {
-            // x split -> z split: dest q holds [nx][ny][nz_q]
-            if (dir1) {
-                seg_view(s1.prm.out, tab_z, G1, [&](int q, int r) {
-                    const size_t nzq = g.sz.size[q];
-                    return mkseg(eptr(slotp(D1, r), g.sx.start[me] * g.ny * nzq, es), (long long)(g.ny * nzq), (long long)nzq, 1, g.sz.start[q]);
-                });
-            } else {
-                a2a_counts(x1, G1, [&](int q) { return nx_i * g.ny * g.sz.size[q]; }, [&](int q) { return g.sx.size[q] * g.ny * nz_j; });
-                seg_view(s1.prm.out, tab_z, G1, [&](int q, int) {
-                    const size_t nzq = g.sz.size[q];
-                    return mkseg(eptr(slotp(SS, me), x1.soff[q], es), (long long)(g.ny * nzq), (long long)nzq, 1, g.sz.start[q]);
-                });
-            }
-        } else {
-            // pencil row: dest (i,q) holds [nx_i][ny][nz_q]
-            if (dir1) {
-                seg_view(s1.prm.out, tab_z, G1, [&](int q, int r) {
-                    const size_t nzq = g.sz.size[q];
-                    return mkseg(eptr(slotp(D1, r), y0_j * nzq, es), (long long)(g.ny * nzq), (long long)nzq, 1, g.sz.start[q]);
-                });
-            } else {
-                a2a_counts(x1, G1, [&](int q) { return nx_i * ny_j * g.sz.size[q]; }, [&](int q) { return nx_i * g.sy.size[q] * nz_j; });
-                seg_view(s1.prm.out, tab_z, G1, [&](int q, int) {
-                    const size_t nzq = g.sz.size[q];
-                    return mkseg(eptr(slotp(SS, me), x1.soff[q], es), (long long)(ny_j * nzq), (long long)nzq, 1, g.sz.start[q]);
-                });
-            }
-        }
+        // transposition 1: scatter along z over G1; dest q holds [nx][ny][nz_q] (Z_Then_YX: x split -> z split) or, a pencil
+        // row, [nx_i][ny][nz_q]
+        const Transposition t1 = zyx ? Transposition(p, 1, AZ, AX, g.sz, g.sx, g.ny, tab_z, tab_x)
+                                     : Transposition(p, 1, AZ, AY, g.sz, g.sy, nx_i, tab_z, tab_y_in);
+        s1.prm.out = t1.send({AX, AY, AZ});
         if (g.decomp == DFFT_SLAB_ZY_THEN_X) s1.phase = nullptr;
         if (!zy) sc.steps.push_back(s1);
-        if (t1_a2a) { x1.phase = zyx ? "Transpose (Finished All2All)" : "First Transpose (Finished All2All)"; x1.group = 1; sc.steps.push_back(x1); }
-        else if (G1.size() > 1) sc.steps.push_back(new_rendezvous(1, 1, zyx ? "Transpose (Finished Receive)" : "First Transpose (Finished Receive)", 0));
+        t1.finish(sc);
 
         // pass 2: y (tiled): a0 = x, n = y, b = z in nz_j
         Step s2;
@@ -1019,21 +1073,12 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         if (rc) return rc;
         s2.label = "y pass";
         s2.prm.A0 = int(nx2); s2.prm.A1 = 1; s2.prm.B = int(nz_j);
-        if (t1_a2a && !zyx) {
-            seg_view(s2.prm.in, tab_y_in, G1, [&](int q, int) {
-                const size_t nyq = g.sy.size[q];
-                return mkseg(eptr(slotp(SR, me), x1.roff[q], es), (long long)(nyq * nz_j), 0, (long long)nz_j, g.sy.start[q]);
-            });
-        } else {
-            void* base = t1_a2a ? slotp(SR, me) : slotp(D1, me);
-            s2.prm.in = single_view(base, (long long)(g.ny * nz_j), 0, (long long)nz_j);
-        }
+        s2.prm.in = t1.recv({AX, NO_AXIS, AY});
         if (d == 2 || zyx) {
             if (d == 2) {
                 s2.prm.out = single_view(nullptr, (long long)(ky * nz_j), 0, (long long)nz_j);
                 s2.out_user = 2;
                 sc.steps.push_back(s2);
-                sc.built = true;
                 return DFFT_SUCCESS;
             }
             // z_then_yx: y pass in place (padded: its Ky output rows keep the input's strides, the first Ky * nz_j elements of
@@ -1050,13 +1095,12 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
             s3.prm.out = single_view(nullptr, 0, 0, (long long)(ky * nz_j));
             s3.out_user = 2;
             sc.steps.push_back(s3);
-            sc.built = true;
             return DFFT_SUCCESS;
         }
-        // transposition 2: scatter along y over G2 (column of the grid, or all ranks for the slab)
-        Step x2;
-        const bool t2_a2a = !dir2;
-        const HandOver ho = hand_over(dir1 && dir2, tab_y_out);
+        // transposition 2: scatter along y over G2 (column of the grid, or all ranks for the slab); dest q holds
+        // [nx][oy_q][nz_j]
+        const Transposition t2(p, 2, AY, AX, g.oy, g.sx, nz_j, tab_y_out, tab_x);
+        const HandOver ho(p, inverse, t1.direct && t2.direct, true, tab_y_out);
         Step s2t;
         if (ho.CH) {
             // rows are only adjacent when the tile is CH wide: with remote peers take the wide tile (TB = CH = 8 for
@@ -1066,30 +1110,19 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
             const View in = s2.prm.in;
             ho.scatter(s2, in, x0_i, nx_i, 0, ho.nzm);
             if (ho.any_rem) s2t = ho.scatter_tail(s2, in, x0_i);
-        } else if (dir2) {
-            if (G2.size() > 1) s2.prm.tile_pref = p->xchg_tile_pref;
-            seg_view(s2.prm.out, tab_y_out, G2, [&](int q, int r) {
-                const size_t nyq = g.oy.size[q];
-                return mkseg(eptr(slotp(D2, r), x0_i * nyq * nz_j, es), (long long)(nyq * nz_j), 0, (long long)nz_j, g.oy.start[q]);
-            });
         } else {
-            a2a_counts(x2, G2, [&](int q) { return nx_i * g.oy.size[q] * nz_j; }, [&](int q) { return g.sx.size[q] * oy_i * nz_j; });
-            seg_view(s2.prm.out, tab_y_out, G2, [&](int q, int) {
-                const size_t nyq = g.oy.size[q];
-                return mkseg(eptr(slotp(SS, me), x2.soff[q], es), (long long)(nyq * nz_j), 0, (long long)nz_j, g.oy.start[q]);
-            });
+            if (t2.direct && G2.size() > 1) s2.prm.tile_pref = p->xchg_tile_pref;
+            s2.prm.out = t2.send({AX, NO_AXIS, AY});
         }
         if (zy) {
-            if (ho.any_rem || t1_a2a || t2_a2a || G1.size() > 1 || G2.size() > 1) return fail(DFFT_ERR_STATE, "internal: fused z + y stage");
+            if (ho.any_rem || !t1.direct || !t2.direct || G1.size() > 1 || G2.size() > 1) return fail(DFFT_ERR_STATE, "internal: fused z + y stage");
             Step f;
             rc = fuse_zy(p, s1, s2, "zy pass", s2.phase, f);
             if (rc) return rc;
             sc.steps.push_back(f);
         } else if (ho.any_rem) { const char* ph = s2.phase; s2.phase = nullptr; sc.steps.push_back(s2); s2t.phase = ph; sc.steps.push_back(s2t); }
         else sc.steps.push_back(s2);
-        const bool slab = g.decomp == DFFT_SLAB_ZY_THEN_X;
-        if (t2_a2a) { x2.phase = slab ? "Transpose (Finished All2All)" : "Second Transpose (Finished All2All)"; x2.group = 2; sc.steps.push_back(x2); }
-        else if (G2.size() > 1) sc.steps.push_back(new_rendezvous(2, 2, slab ? "Transpose (Finished Receive)" : "Second Transpose (Finished Receive)", 0));
+        t2.finish(sc);
 
         // pass 3: x (tiled): n = x, b = (y in oy_i, z in nz_j); received blocks are x-major => contiguous
         Step s3;
@@ -1108,12 +1141,11 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
             }
         } else {
             s3.prm.A0 = 1; s3.prm.A1 = 1; s3.prm.B = int(oy_i * nz_j);
-            s3.prm.in = single_view(t2_a2a ? slotp(SR, me) : slotp(D2, me), 0, 0, (long long)(oy_i * nz_j));
+            s3.prm.in = t2.recv({NO_AXIS, NO_AXIS, AX});
             s3.prm.out = single_view(nullptr, 0, 0, (long long)(oy_i * nz_j));
         }
         s3.out_user = 2;
         sc.steps.push_back(s3);
-        sc.built = true;
         return DFFT_SUCCESS;
     }
 
@@ -1133,68 +1165,54 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         s.prm.out = single_view(nullptr, zpitch_out * (long long)ny_j, zpitch_out, 1);
         s.out_user = 2;
         sc.steps.push_back(s);
-        sc.built = true;
         return DFFT_SUCCESS;
     }
 
     if (zyx) {
-        // input [nx][ny][nz_me]: y pass (to a slot), x pass scattering along x to the owners of x,
-        // then z inverse on [nx_me][ny][kzc].
+        // input [nx][ny][nz_me]: y pass (to a slot), x pass scattering along x to the owners of x (dest q holds
+        // [nx_q][ny][kzc]), then z inverse on [nx_me][ny][kzc].
+        const Transposition t1(p, 1, AX, AZ, g.sx, g.sz, g.ny, tab_x, tab_z);
         Step sy_;
         rc = new_pass(p, inverse, PASS_C2C_TILED, g.ny, 1, nullptr, sy_);
         if (rc) return rc;
         sy_.label = "y pass";
-        const int W = dir1 ? D2 : SR;  // a local scratch slot that is not the transposition target
+        const int W = t1.direct ? p->slots.D2 : p->slots.SR;  // a local scratch slot that is not the transposition target
         // one rank with x kept: the y pass leaves [nx][ny][kzc] in D1, where the z pass reads it, and no x copy runs (the
         // other decompositions run their d = 2 steps instead, get_schedule)
         const bool no_x = P == 1 && !p->taxes[0];
         sy_.prm.A0 = int(kx); sy_.prm.B = int(nz_j);
         sy_.prm.in = single_view(nullptr, (long long)(ky * nz_j), 0, (long long)nz_j);
         sy_.in_user = 1;
-        sy_.prm.out = single_view(slotp(no_x ? D1 : W, me), (long long)(g.ny * nz_j), 0, (long long)nz_j);
+        sy_.prm.out = single_view(p->slot(no_x ? p->slots.D1 : W, me), (long long)(g.ny * nz_j), 0, (long long)nz_j);
         sc.steps.push_back(sy_);
         Step sx_;
         rc = new_pass(p, inverse, PASS_C2C_TILED, g.nx, 0, "2D FFT Y-X-Direction", sx_);
         if (rc) return rc;
         sx_.label = "x pass";
         sx_.prm.A0 = 1; sx_.prm.A1 = int(g.ny); sx_.prm.B = int(nz_j);
-        sx_.prm.in = single_view(slotp(W, me), 0, (long long)nz_j, (long long)(g.ny * nz_j));
-        Step xa;
-        if (dir1) {
-            seg_view(sx_.prm.out, tab_x, G1, [&](int q, int r) {
-                return mkseg(eptr(slotp(D1, r), z0_j, es), 0, (long long)kzc, (long long)(g.ny * kzc), g.sx.start[q]);
-            });
-        } else {
-            a2a_counts(xa, G1, [&](int q) { return g.sx.size[q] * g.ny * nz_j; }, [&](int q) { return nx_i * g.ny * g.sz.size[q]; });
-            seg_view(sx_.prm.out, tab_x, G1, [&](int q, int) {
-                return mkseg(eptr(slotp(SS, me), xa.soff[q], es), 0, (long long)nz_j, (long long)(g.ny * nz_j), g.sx.start[q]);
-            });
-        }
+        sx_.prm.in = single_view(p->slot(W, me), 0, (long long)nz_j, (long long)(g.ny * nz_j));
+        sx_.prm.out = t1.send({NO_AXIS, AY, AX});
         if (!no_x) sc.steps.push_back(sx_);
-        if (!dir1) { xa.phase = "Transpose (Finished All2All)"; xa.group = 1; sc.steps.push_back(xa); }
-        else if (G1.size() > 1) sc.steps.push_back(new_rendezvous(1, 1, "Transpose (Finished Receive)", 0));
+        t1.finish(sc);
         Step sz_;
         rc = new_pass(p, inverse, zkind, zlen, 2, "1D FFT Z-Direction", sz_);
         if (rc) return rc;
         sz_.prm.A0 = int(nx_i); sz_.prm.A1 = int(g.ny);
-        if (dir1) sz_.prm.in = single_view(slotp(D1, me), (long long)(g.ny * kzc), (long long)kzc, 1);
-        else
-            seg_view(sz_.prm.in, tab_z, G1, [&](int q, int) {
-                const size_t nzq = g.sz.size[q];
-                return mkseg(eptr(slotp(SR, me), xa.roff[q], es), (long long)(g.ny * nzq), (long long)nzq, 1, g.sz.start[q]);
-            });
+        sz_.prm.in = t1.recv({AX, AY, AZ});
         sz_.prm.out = single_view(nullptr, zpitch_out * (long long)g.ny, zpitch_out, 1);
         sz_.out_user = 2;
         sc.steps.push_back(sz_);
-        sc.built = true;
         return DFFT_SUCCESS;
     }
 
-    // pencil / slab zy_x inverse
+    // pencil / slab zy_x inverse: the x pass scatters x over G2 (dest (q, j) holds [nx_q][ky][nz_j]), the y pass scatters y
+    // over G1 (dest (i, q) holds [nx_i][ny_q][kzc])
     const bool slab = g.decomp == DFFT_SLAB_ZY_THEN_X;
+    const Transposition t2(p, 2, AX, AY, g.sx, g.oy, nz_j, tab_x, tab_y_out);
+    const Transposition t1(p, 1, AY, AZ, g.sy, g.sz, nx_i, tab_y_in, tab_z);
     // Blocked hand-over for the inverse as well (HandOver; DFFT_BLOCKED_INV=0 keeps the plain layout): the y pass reads rows
     // nx_i*CH apart instead of one row per (y, z) plane
-    const HandOver ho = hand_over(d == 3 && dir2 && dir1, tab_x);
+    const HandOver ho(p, inverse, d == 3 && t2.direct && t1.direct, true, tab_x);
     if (ho.CH) {
         // x pass: in = caller's [nx][oy_i][nz_j]; tile = (y_loc, z block); n = x
         Step s3;
@@ -1214,18 +1232,14 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         } else {
             sc.steps.push_back(s3);
         }
-        if (G2.size() > 1) sc.steps.push_back(new_rendezvous(2, 2, slab ? "Transpose (Finished Receive)" : "Second Transpose (Finished Receive)", 0));
-        // y pass: tile = (x_loc, z block); n = y; dest (i, q) holds [nx_i][ny_q][kzc], my columns z in [z0_j, +nz_j)
+        t2.finish(sc);
+        // y pass: tile = (x_loc, z block); n = y
         Step s2;
         rc = new_pass(p, inverse, PASS_C2C_TILED, g.ny, 1, slab ? nullptr : "1D FFT Y-Direction", s2);
         if (rc) return rc;
         s2.label = "y pass";
         s2.prm.tile_pref = G1.size() > 1 ? p->xchg_tile_pref : 1;
-        View out{};
-        seg_view(out, tab_y_in, G1, [&](int q, int r) {
-            const size_t nyq = g.sy.size[q];
-            return mkseg(eptr(slotp(D1, r), z0_j, es), (long long)(nyq * kzc), 0, (long long)kzc, g.sy.start[q]);
-        });
+        const View out = t1.send({AX, NO_AXIS, AY});
         ho.gather(s2, out, 0, nx_i, 0, ho.nzm);
         if (ho.any_rem) {
             Step s2t = ho.gather_tail(s2, out, 0);
@@ -1235,12 +1249,12 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         } else if (!zy) {
             sc.steps.push_back(s2);
         }
-        if (G1.size() > 1) sc.steps.push_back(new_rendezvous(1, 1, "First Transpose (Finished Receive)", 0));
+        t1.finish(sc);
         Step s1;
         rc = new_pass(p, inverse, zkind, zlen, 2, slab ? "2D FFT Y-Z-Direction" : "1D FFT Z-Direction", s1);
         if (rc) return rc;
         s1.prm.A0 = int(nx_i); s1.prm.A1 = int(ny_j);
-        s1.prm.in = single_view(slotp(D1, me), (long long)(ny_j * kzc), (long long)kzc, 1);
+        s1.prm.in = t1.recv({AX, AY, AZ});
         s1.prm.out = single_view(nullptr, zpitch_out * (long long)ny_j, zpitch_out, 1);
         s1.out_user = 2;
         if (zy) {
@@ -1252,11 +1266,8 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         } else {
             sc.steps.push_back(s1);
         }
-        sc.built = true;
         return DFFT_SUCCESS;
     }
-    Step x2;
-    bool have_in_slot = false;  // whether the y pass input is in a slot (d == 3) or the caller's buffer (d == 2)
     if (d == 3) {
         Step s3;
         rc = new_pass(p, inverse, PASS_C2C_TILED, g.nx, 0, "1D FFT X-Direction", s3);
@@ -1265,73 +1276,36 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         s3.prm.A0 = 1; s3.prm.A1 = 1; s3.prm.B = int(oy_i * nz_j);
         s3.prm.in = single_view(nullptr, 0, 0, (long long)(oy_i * nz_j));
         s3.in_user = 1;
-        if (dir2 && G2.size() > 1) s3.prm.tile_pref = p->xchg_tile_pref;
-        if (dir2) {
-            // dest (q,j) holds [nx_q][ky][nz_j]; my rows y in [oy0_i, +oy_i)
-            seg_view(s3.prm.out, tab_x, G2, [&](int q, int r) {
-                return mkseg(eptr(slotp(D2, r), oy0_i * nz_j, es), 0, 0, (long long)(ky * nz_j), g.sx.start[q]);
-            });
-        } else {
-            a2a_counts(x2, G2, [&](int q) { return g.sx.size[q] * oy_i * nz_j; }, [&](int q) { return nx_i * g.oy.size[q] * nz_j; });
-            seg_view(s3.prm.out, tab_x, G2, [&](int q, int) {
-                return mkseg(eptr(slotp(SS, me), x2.soff[q], es), 0, 0, (long long)(oy_i * nz_j), g.sx.start[q]);
-            });
-        }
+        if (t2.direct && G2.size() > 1) s3.prm.tile_pref = p->xchg_tile_pref;
+        s3.prm.out = t2.send({NO_AXIS, NO_AXIS, AX});
         sc.steps.push_back(s3);
-        if (!dir2) { x2.phase = slab ? "Transpose (Finished All2All)" : "Second Transpose (Finished All2All)"; x2.group = 2; sc.steps.push_back(x2); }
-        else if (G2.size() > 1) sc.steps.push_back(new_rendezvous(2, 2, slab ? "Transpose (Finished Receive)" : "Second Transpose (Finished Receive)", 0));
-        have_in_slot = true;
+        t2.finish(sc);
     }
-    // y pass on [nx_i][ky][nz_j]
+    // y pass on [nx_i][ky][nz_j]: from the x pass (d = 3) or the caller's buffer (d = 2)
     Step s2;
     rc = new_pass(p, inverse, PASS_C2C_TILED, g.ny, 1, slab ? nullptr : "1D FFT Y-Direction", s2);
     if (rc) return rc;
     s2.label = "y pass";
     s2.prm.A0 = int(nx_i); s2.prm.A1 = 1; s2.prm.B = int(nz_j);
-    if (!have_in_slot) {
+    if (d == 3) {
+        s2.prm.in = t2.recv({AX, NO_AXIS, AY});
+    } else {
         s2.prm.in = single_view(nullptr, (long long)(ky * nz_j), 0, (long long)nz_j);
         s2.in_user = 1;
-    } else if (dir2) {
-        s2.prm.in = single_view(slotp(D2, me), (long long)(ky * nz_j), 0, (long long)nz_j);
-    } else {
-        seg_view(s2.prm.in, tab_y_out, G2, [&](int q, int) {
-            const size_t nyq = g.oy.size[q];
-            return mkseg(eptr(slotp(SR, me), x2.roff[q], es), (long long)(nyq * nz_j), 0, (long long)nz_j, g.oy.start[q]);
-        });
     }
-    Step x1;
-    if (dir1 && G1.size() > 1) s2.prm.tile_pref = p->xchg_tile_pref;
-    if (dir1) {
-        // dest (i,q) holds [nx_i][ny_q][kzc]; my columns z in [z0_j, +nz_j)
-        seg_view(s2.prm.out, tab_y_in, G1, [&](int q, int r) {
-            const size_t nyq = g.sy.size[q];
-            return mkseg(eptr(slotp(D1, r), z0_j, es), (long long)(nyq * kzc), 0, (long long)kzc, g.sy.start[q]);
-        });
-    } else {
-        a2a_counts(x1, G1, [&](int q) { return nx_i * g.sy.size[q] * nz_j; }, [&](int q) { return nx_i * ny_j * g.sz.size[q]; });
-        seg_view(s2.prm.out, tab_y_in, G1, [&](int q, int) {
-            const size_t nyq = g.sy.size[q];
-            return mkseg(eptr(slotp(SS, me), x1.soff[q], es), (long long)(nyq * nz_j), 0, (long long)nz_j, g.sy.start[q]);
-        });
-    }
+    if (t1.direct && G1.size() > 1) s2.prm.tile_pref = p->xchg_tile_pref;
+    s2.prm.out = t1.send({AX, NO_AXIS, AY});
     sc.steps.push_back(s2);
-    if (!dir1) { x1.phase = "First Transpose (Finished All2All)"; x1.group = 1; sc.steps.push_back(x1); }
-    else if (G1.size() > 1) sc.steps.push_back(new_rendezvous(1, 1, "First Transpose (Finished Receive)", 0));
+    t1.finish(sc);
     // z pass on [nx_i][ny_j][kzc]
     Step s1;
     rc = new_pass(p, inverse, zkind, zlen, 2, slab ? "2D FFT Y-Z-Direction" : "1D FFT Z-Direction", s1);
     if (rc) return rc;
     s1.prm.A0 = int(nx_i); s1.prm.A1 = int(ny_j);
-    if (dir1) s1.prm.in = single_view(slotp(D1, me), (long long)(ny_j * kzc), (long long)kzc, 1);
-    else
-        seg_view(s1.prm.in, tab_z, G1, [&](int q, int) {
-            const size_t nzq = g.sz.size[q];
-            return mkseg(eptr(slotp(SR, me), x1.roff[q], es), (long long)(ny_j * nzq), (long long)nzq, 1, g.sz.start[q]);
-        });
+    s1.prm.in = t1.recv({AX, AY, AZ});
     s1.prm.out = single_view(nullptr, zpitch_out * (long long)ny_j, zpitch_out, 1);
     s1.out_user = 2;
     sc.steps.push_back(s1);
-    sc.built = true;
     return DFFT_SUCCESS;
 }
 
@@ -1376,11 +1350,6 @@ static size_t z_chunk_count(const dfft_plan_s* p, int inverse) {
     return min_nz >= 32 * want ? want : (min_nz >= 32 ? 2 : 1);
 }
 
-// the overlapped schedules' hand-over in slot B (tab: the segment table of the scattering pass's receivers)
-static HandOver overlapped_hand_over(const dfft_plan_s* p, int inverse, const unsigned char* tab) {
-    return HandOver(p, inverse, true, false, tab, p->slot_ptr[1]);
-}
-
 static int build_overlapped_forward(dfft_plan_s* p, Schedule& sc) {
     const Geometry& g = p->g;
     const int me = p->rank;
@@ -1388,17 +1357,13 @@ static int build_overlapped_forward(dfft_plan_s* p, Schedule& sc) {
     const size_t es = p->esize;
     const bool c2c = g.transform == DFFT_C2C;
     Tables& T = p->tabs;
-    sc.steps.clear();
     sc.overlapped = true;
     const size_t ny = g.ny;
     const size_t nx_i = g.sx.size[pi], x0_i = g.sx.start[pi];
-    const size_t ny_j = g.sy.size[pj], y0_j = g.sy.start[pj];
+    const size_t ny_j = g.sy.size[pj];
     const size_t nz_j = g.sz.size[pj];
     const size_t oy_i = g.oy.size[pi];
-    const std::vector<int>& G1 = p->grp[1];
     const std::vector<int>& G2 = p->grp[2];
-    const int D1 = 0, D2 = 1;
-    auto slotp = [&](int s_, int r) -> void* { return p->slot_ptr[s_][r]; };
     int nev = 0;
 
     const size_t NG = plane_groups(p, 0), NS = z_chunk_count(p, 0);
@@ -1409,7 +1374,8 @@ static int build_overlapped_forward(dfft_plan_s* p, Schedule& sc) {
     const unsigned char *tab_z = nullptr, *tab_y = nullptr;
     if ((pencil && T.seg_table(g.sz, &tab_z) != cudaSuccess) || T.seg_table(g.oy, &tab_y) != cudaSuccess)
         return fail(DFFT_ERR_CUDA, "segment table");
-    const HandOver ho = overlapped_hand_over(p, 0, tab_y);
+    const Transposition t1(p, 1, AZ, AY, g.sz, g.sy, nx_i, tab_z, nullptr), t2(p, 2, AY, AX, g.oy, g.sx, nz_j, tab_y, nullptr);
+    const HandOver ho(p, 0, true, false, tab_y);
     const Split chunks = ho.chunks(NS);
     // the ranks of a pencil grid hold different z extents: a chunk count clamped to one rank's blocks could differ
     // between them
@@ -1432,10 +1398,7 @@ static int build_overlapped_forward(dfft_plan_s* p, Schedule& sc) {
         s.prm.A0 = int(npl); s.prm.A1 = int(ny_j);
         s.prm.in = single_view((void*)(size_t)(pl0 * ny_j * pitch * es), pitch * (long long)ny_j, pitch, 1);
         s.in_user = 1;
-        seg_view(s.prm.out, tab_z, G1, [&](int q, int r) {
-            const size_t nzq = g.sz.size[q];
-            return mkseg(eptr(slotp(D1, r), (pl0 * ny + y0_j) * nzq, es), (long long)(ny * nzq), (long long)nzq, 1, g.sz.start[q]);
-        });
+        s.prm.out = t1.send({AX, AY, AZ}, {pl0, 0, 0});
         s.record = ev_z[gi] = nev++;
         sc.steps.push_back(s);
     }
@@ -1459,17 +1422,14 @@ static int build_overlapped_forward(dfft_plan_s* p, Schedule& sc) {
                     s.waits = w;
                 }
             }
-            const View in = single_view(eptr(slotp(D1, me), pl0 * ny * nz_j, es), (long long)(ny * nz_j), 0, (long long)nz_j);
+            const View in = t1.recv({AX, NO_AXIS, AY}, {pl0, 0, 0});
             if (ho.CH) {
                 s.prm.bulk_out = G2.size() > 1 ? p->bulk_store : 0;
                 ho.scatter(s, in, x0_i + pl0, npl, z0, zc);
             } else {
                 s.prm.A0 = int(npl); s.prm.A1 = 1; s.prm.B = int(zc);
-                s.prm.in = single_view(eptr(slotp(D1, me), pl0 * ny * nz_j + z0, es), (long long)(ny * nz_j), 0, (long long)nz_j);
-                seg_view(s.prm.out, tab_y, G2, [&](int q, int r) {
-                    const size_t nyq = g.oy.size[q];
-                    return mkseg(eptr(slotp(D2, r), (x0_i + pl0) * nyq * nz_j + z0, es), (long long)(nyq * nz_j), 0, (long long)nz_j, g.oy.start[q]);
-                });
+                s.prm.in = t1.recv({AX, NO_AXIS, AY}, {pl0, 0, z0});
+                s.prm.out = t2.send({AX, NO_AXIS, AY}, {pl0, 0, z0});
             }
             s.prm.max_ctas = exchange_ctas(p, 0);
             s.prm.tile_pref = G2.size() > 1 ? p->xchg_tile_pref : 0;
@@ -1499,7 +1459,7 @@ static int build_overlapped_forward(dfft_plan_s* p, Schedule& sc) {
             s.prm.tile_swz = p->x_swz;
         } else {
             s.prm.A0 = 1; s.prm.A1 = int(oy_i); s.prm.B = int(zc);
-            s.prm.in = single_view(eptr(slotp(D2, me), z0, es), 0, (long long)nz_j, (long long)(oy_i * nz_j));
+            s.prm.in = t2.recv({NO_AXIS, AY, AX}, {0, 0, z0});
             s.prm.out = single_view((void*)(size_t)(z0 * es), 0, (long long)nz_j, (long long)(oy_i * nz_j));
         }
         s.out_user = 2;
@@ -1508,7 +1468,6 @@ static int build_overlapped_forward(dfft_plan_s* p, Schedule& sc) {
         if (ho.any_rem && c + 1 == NSc) sc.steps.push_back(ho.gather_tail(s, out, 0));
     }
     sc.nevents = nev;
-    sc.built = true;
     return DFFT_SUCCESS;
 }
 
@@ -1518,19 +1477,17 @@ static int build_overlapped_slab_inverse(dfft_plan_s* p, Schedule& sc) {
     const size_t es = p->esize;
     const bool c2c = g.transform == DFFT_C2C;
     Tables& T = p->tabs;
-    sc.steps.clear();
     sc.overlapped = true;
     const size_t nzc = g.nzc, ny = g.ny;
     const size_t nx_p = g.sx.size[me];
     const size_t oy_me = g.oy.size[me], oy0_me = g.oy.start[me];
-    const std::vector<int>& G2 = p->grp[2];
-    const int D1 = 0, D2 = 1;
-    auto slotp = [&](int s_, int r) -> void* { return p->slot_ptr[s_][r]; };
     int nev = 0;
 
     const unsigned char* tab_x = nullptr;
     if (T.seg_table(g.sx, &tab_x) != cudaSuccess) return fail(DFFT_ERR_CUDA, "segment table");
-    const HandOver ho = overlapped_hand_over(p, 1, tab_x);
+    // dest q holds [nx_q][ny][nzc]
+    const Transposition t2(p, 2, AX, AY, g.sx, g.oy, nzc, tab_x, nullptr);
+    const HandOver ho(p, 1, true, false, tab_x);
     const Split chunks = ho.chunks(z_chunk_count(p, 1));
     const size_t NSc = chunks.size.size();
 
@@ -1553,10 +1510,7 @@ static int build_overlapped_slab_inverse(dfft_plan_s* p, Schedule& sc) {
         } else {
             s.prm.A0 = 1; s.prm.A1 = int(oy_me); s.prm.B = int(zc);
             s.prm.in = single_view((void*)(size_t)(z0 * es), 0, (long long)nzc, (long long)(oy_me * nzc));
-            // dest q holds [nx_q][ny][nzc]; my rows y in [oy0_me, +oy_me)
-            seg_view(s.prm.out, tab_x, G2, [&](int q, int r) {
-                return mkseg(eptr(slotp(D2, r), oy0_me * nzc + z0, es), 0, (long long)nzc, (long long)(ny * nzc), g.sx.start[q]);
-            });
+            s.prm.out = t2.send({NO_AXIS, AY, AX}, {0, 0, z0});
         }
         s.prm.max_ctas = exchange_ctas(p, 1);
         s.prm.tile_pref = p->xchg_tile_pref;
@@ -1571,7 +1525,7 @@ static int build_overlapped_slab_inverse(dfft_plan_s* p, Schedule& sc) {
             sc.steps.push_back(t);
         }
     }
-    const View out = single_view(slotp(D1, me), (long long)(ny * nzc), 0, (long long)nzc);
+    const View out = single_view(p->slot(p->slots.D1, me), (long long)(ny * nzc), 0, (long long)nzc);
     for (size_t c = 0; c < NSc; ++c) {
         const size_t z0 = chunks.start[c], zc = chunks.size[c];
         Step r = new_rendezvous(2, 2, nullptr, 2);
@@ -1595,7 +1549,7 @@ static int build_overlapped_slab_inverse(dfft_plan_s* p, Schedule& sc) {
             }
         } else {
             s.prm.A0 = int(nx_p); s.prm.A1 = 1; s.prm.B = int(zc);
-            s.prm.in = single_view(eptr(slotp(D2, me), z0, es), (long long)(ny * nzc), 0, (long long)nzc);
+            s.prm.in = t2.recv({AX, NO_AXIS, AY}, {0, 0, z0});
             s.prm.out = s.prm.in;  // in place
             s.record = ev_yi[c] = nev++;
             sc.steps.push_back(s);
@@ -1606,13 +1560,12 @@ static int build_overlapped_slab_inverse(dfft_plan_s* p, Schedule& sc) {
     rc = new_pass(p, 1, c2c ? PASS_C2C_CONTIG : PASS_C2R, c2c ? g.nz : g.nz / 2, 2, nullptr, s);
     if (rc) return rc;
     s.prm.A0 = int(nx_p); s.prm.A1 = int(ny);
-    s.prm.in = single_view(slotp(ho.CH ? D1 : D2, me), (long long)(ny * nzc), (long long)nzc, 1);
+    s.prm.in = single_view(p->slot(ho.CH ? p->slots.D1 : p->slots.D2, me), (long long)(ny * nzc), (long long)nzc, 1);
     s.prm.out = single_view(nullptr, zpitch * (long long)ny, zpitch, 1);
     s.out_user = 2;
     for (size_t c = 0; c < NSc; ++c) s.waits.push_back(ev_yi[c]);
     sc.steps.push_back(s);
     sc.nevents = nev;
-    sc.built = true;
     return DFFT_SUCCESS;
 }
 
@@ -1636,24 +1589,23 @@ static int build_overlapped_pencil_inverse(dfft_plan_s* p, Schedule& sc) {
     const size_t es = p->esize;
     const bool c2c = g.transform == DFFT_C2C;
     Tables& T = p->tabs;
-    sc.steps.clear();
     sc.overlapped = true;
-    const size_t ny = g.ny, nx = g.nx, nzc = g.nzc;
+    const size_t ny = g.ny, nx = g.nx;
     const size_t nx_i = g.sx.size[pi];
     const size_t ny_j = g.sy.size[pj];
-    const size_t nz_j = g.sz.size[pj], z0_j = g.sz.start[pj];
+    const size_t nz_j = g.sz.size[pj];
     const size_t oy_i = g.oy.size[pi], oy0_i = g.oy.start[pi];
     const std::vector<int>& G1 = p->grp[1];
     const std::vector<int>& G2 = p->grp[2];
-    const int D1 = 0, D2 = 1;
-    auto slotp = [&](int s_, int r) -> void* { return p->slot_ptr[s_][r]; };
     int nev = 0;
     const size_t NG = plane_groups(p, 1);
     Split groups;
     groups.make(nx_i, NG);
     const unsigned char *tab_x = nullptr, *tab_y_in = nullptr;
     if (T.seg_table(g.sx, &tab_x) != cudaSuccess || T.seg_table(g.sy, &tab_y_in) != cudaSuccess) return fail(DFFT_ERR_CUDA, "segment table");
-    const HandOver ho = overlapped_hand_over(p, 1, tab_x);
+    // dest (q, j) holds [nx_q][ny][nz_j], dest (i, q) [nx_i][ny_q][nzc]
+    const Transposition t2(p, 2, AX, AY, g.sx, g.oy, nz_j, tab_x, nullptr), t1(p, 1, AY, AZ, g.sy, g.sz, nx_i, tab_y_in, nullptr);
+    const HandOver ho(p, 1, true, false, tab_x);
     int rc;
 
     sc.steps.push_back(new_rendezvous(0, 0, nullptr, 0));  // everyone has left the previous exec
@@ -1674,10 +1626,7 @@ static int build_overlapped_pencil_inverse(dfft_plan_s* p, Schedule& sc) {
         } else {
             s.prm.A0 = 1; s.prm.A1 = 1; s.prm.B = int(oy_i * nz_j);
             s.prm.in = single_view(nullptr, 0, 0, (long long)(oy_i * nz_j));
-            // dest (q, j) holds [nx_q][ny][nz_j]; my rows y in [oy0_i, +oy_i)
-            seg_view(s.prm.out, tab_x, G2, [&](int q, int r) {
-                return mkseg(eptr(slotp(D2, r), oy0_i * nz_j, es), 0, 0, (long long)(ny * nz_j), g.sx.start[q]);
-            });
+            s.prm.out = t2.send({NO_AXIS, NO_AXIS, AX});
             sc.steps.push_back(s);
         }
     }
@@ -1695,12 +1644,7 @@ static int build_overlapped_pencil_inverse(dfft_plan_s* p, Schedule& sc) {
         if (gi == 0) s.waits.push_back(ev_x);
         s.prm.max_ctas = exchange_ctas(p, 1);
         s.prm.tile_pref = G1.size() > 1 ? p->xchg_tile_pref : 1;
-        // dest (i, q) holds [nx_i][ny_q][nzc]; my columns z in [z0_j, +nz_j)
-        View out{};
-        seg_view(out, tab_y_in, G1, [&](int q, int r) {
-            const size_t nyq = g.sy.size[q];
-            return mkseg(eptr(slotp(D1, r), pl0 * nyq * nzc + z0_j, es), (long long)(nyq * nzc), 0, (long long)nzc, g.sy.start[q]);
-        });
+        const View out = t1.send({AX, NO_AXIS, AY}, {pl0, 0, 0});
         if (ho.CH) {
             ho.gather(s, out, pl0, npl, 0, ho.nzm);
             if (!ho.any_rem) s.record = ev_y[gi] = nev++;
@@ -1712,7 +1656,7 @@ static int build_overlapped_pencil_inverse(dfft_plan_s* p, Schedule& sc) {
             }
         } else {
             s.prm.A0 = int(npl); s.prm.A1 = 1; s.prm.B = int(nz_j);
-            s.prm.in = single_view(eptr(slotp(D2, me), pl0 * ny * nz_j, es), (long long)(ny * nz_j), 0, (long long)nz_j);
+            s.prm.in = t2.recv({AX, NO_AXIS, AY}, {pl0, 0, 0});
             s.prm.out = out;
             s.record = ev_y[gi] = nev++;
             sc.steps.push_back(s);
@@ -1729,14 +1673,13 @@ static int build_overlapped_pencil_inverse(dfft_plan_s* p, Schedule& sc) {
         rc = new_pass(p, 1, zkind, c2c ? g.nz : g.nz / 2, 2, nullptr, s);
         if (rc) return rc;
         s.prm.A0 = int(npl); s.prm.A1 = int(ny_j);
-        s.prm.in = single_view(eptr(slotp(D1, me), pl0 * ny_j * nzc, es), (long long)(ny_j * nzc), (long long)nzc, 1);
+        s.prm.in = t1.recv({AX, AY, AZ}, {pl0, 0, 0});
         s.prm.out = single_view((void*)(size_t)(pl0 * ny_j * size_t(zpitch) * es), zpitch * (long long)ny_j, zpitch, 1);
         s.out_user = 2;
         s.stream = 2;
         sc.steps.push_back(s);
     }
     sc.nevents = nev;
-    sc.built = true;
     return DFFT_SUCCESS;
 }
 
@@ -2030,8 +1973,8 @@ static int run_schedule(dfft_plan_s* p, Schedule& sc, void* out, const void* in,
                 CK_CUDA(mark(phase, 0, s.label));
             } else {
                 const std::vector<int>& G = p->grp[s.group];
-                char* sb = (char*)p->slot_ptr[s.send_slot][me];
-                char* rb = (char*)p->slot_ptr[s.recv_slot][me];
+                char* sb = (char*)p->slot(s.send_slot, me);
+                char* rb = (char*)p->slot(s.recv_slot, me);
                 CK_NCCL(ncclGroupStart());
                 for (size_t q = 0; q < G.size(); ++q) {
                     if (G[q] == me) continue;
@@ -2237,6 +2180,7 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
     Schedule& sc = p->sched[inverse ? 1 : 0][d - 1];
     p->axes_fixed = true;
     if (!sc.built) {
+        sc = Schedule();  // a build that failed may have left steps and flags
         g_view_error = false;
         const bool streams = p->cfg.send_method == DFFT_SEND_STREAMS || (p->g.decomp == DFFT_PENCIL && p->cfg.send_method2 == DFFT_SEND_STREAMS);
         const bool seq_won = p->tuned_seq[inverse ? 1 : 0] != 0;
@@ -2278,6 +2222,7 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
         sc.inverse = inverse ? 1 : 0;
         field_bytes(p, inverse, d, &sc.field_in, &sc.field_out);
         if (g_view_error) return fail(DFFT_ERR_STATE, "internal: segments of one view disagree on the axis stride");
+        sc.built = true;  // only a schedule that every step above accepted is reused
     }
     *out = &sc;
     return DFFT_SUCCESS;
@@ -2600,13 +2545,11 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
     p->direct2 = (decomp == DFFT_PENCIL ? p->cfg.comm_method2 : p->cfg.comm_method) != DFFT_ALL2ALL;
     if (decomp == DFFT_SLAB_ZY_THEN_X) p->direct1 = true;   // trivial group
     if (decomp == DFFT_SLAB_Z_THEN_YX) p->direct2 = true;
-    const bool d1 = p->direct1 || p->grp[1].size() == 1, d2 = p->direct2 || p->grp[2].size() == 1;
     p->any_direct = (p->direct1 && p->grp[1].size() > 1) || (p->direct2 && p->grp[2].size() > 1);
-    p->nslots = (d1 ? 1 : 0) + (d2 ? 1 : 0) + ((!d1 || !d2) ? 2 : 0);
-    if (p->nslots < 2) p->nslots = 2;
+    p->slots = plan_slots(p->direct1 || p->grp[1].size() == 1, p->direct2 || p->grp[2].size() == 1);
     // in place on one rank the caller's buffer is the schedules' first slot (D1; both transpositions are local there)
     p->buf_slot = inplace && P == 1;
-    if (p->buf_slot) p->nslots = 1;
+    p->nslots = p->slots.count - (p->buf_slot ? 1 : 0);
     size_t dom = 0;
     for (int r = 0; r < P; ++r) dom = std::max(dom, g.domain_elems(r));
     p->slot_bytes = ((dom * p->esize * comps + 255) / 256) * 256;
