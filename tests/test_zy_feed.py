@@ -45,9 +45,16 @@ def test_fed_matches_register_fed(shape, prec):
         _run(plan, a, x, direction, 1)
         _run(plan, b, x, direction, 0)
         assert torch.equal(a, b), f"direction {direction}, scale {scale}: max |diff| {float((a - b).abs().max())}"
-        # repeated execs switching between the kernels: both draw from the same counters
+        # repeated execs switching between the kernels, on a new input: both draw from the same counters, and an exec that
+        # read the previous exec's intermediate would not match
+        x2 = torch.complex(torch.rand(shape, generator=g, device="cuda", dtype=rdt), torch.rand(shape, generator=g, device="cuda", dtype=rdt))
+        _run(plan, b, x2, direction, 0)
+        _run(plan, a, x2, direction, 1)
+        assert torch.equal(a, b), f"direction {direction}, scale {scale}, second input: max |diff| {float((a - b).abs().max())}"
         _run(plan, a, x, direction, 1)
-        assert torch.equal(a, b)
+        _run(plan, b, x, direction, 0)
+        assert torch.equal(a, b), f"direction {direction}, scale {scale}, first input again: max |diff| {float((a - b).abs().max())}"
+        del x2
     plan.destroy()
     del x, a, b
     torch.cuda.empty_cache()

@@ -103,10 +103,16 @@ def test_fused_vs_cufft(shape, prec):
     assert plan.lastLaunchCount() == 2
     assert lib.cufft_ref_3d(1 if f64 else 0, 1, *shape, out.data_ptr(), ref.data_ptr(), C.byref(ms), 1) == 0
     assert _rel_l2(back, out) < tol
-    # repeated execs: the fused stage's counters carry over from launch to launch
-    for _ in range(3):
-        plan.execC2C(back, x, dfft.FORWARD)
-    assert _rel_l2(back, ref) < tol
+    # repeated execs, each on a new input into the other output: the fused stage's counters carry over from launch to launch,
+    # and a phase-B item that read the previous exec's intermediate would not match
+    for r in range(3):
+        xr = torch.complex(torch.rand(shape, generator=g, device="cuda", dtype=rdt), torch.rand(shape, generator=g, device="cuda", dtype=rdt))
+        dst = back if r % 2 == 0 else out
+        plan.execC2C(dst, xr, dfft.FORWARD)
+        assert plan.lastLaunchCount() == 2
+        assert lib.cufft_ref_3d(1 if f64 else 0, 0, *shape, ref.data_ptr(), xr.data_ptr(), C.byref(ms), 1) == 0
+        assert _rel_l2(dst, ref) < tol, f"repeated exec {r}"
+        del xr
     plan.destroy()
     del x, out, ref, back
     torch.cuda.empty_cache()
