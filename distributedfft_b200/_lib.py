@@ -62,6 +62,9 @@ SIGNATURES = {
     "dfft_plan_create_interleaved": (C.c_int, [C.c_void_p, C.POINTER(dfft_config), C.c_int, C.c_int, C.c_int, C.c_size_t, C.c_size_t,
                                                C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int, C.POINTER(C.c_void_p)]),
     "dfft_get_components": (C.c_size_t, [C.c_void_p]),
+    "dfft_plan_create_boxes": (C.c_int, [C.c_void_p, C.POINTER(dfft_config), C.c_int, C.c_int, C.c_int, C.c_size_t, C.c_size_t,
+                                         C.c_size_t, C.c_size_t, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.c_size_t,
+                                         C.c_int, C.POINTER(C.c_void_p)]),
     "dfft_plan_set_scale": (C.c_int, [C.c_void_p, C.c_double, C.c_double]),
     "dfft_plan_get_scale": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "dfft_plan_destroy": (C.c_int, [C.c_void_p]),

@@ -449,9 +449,10 @@ struct Schedule {
 
 // The work slots of the schedules, in the order they lie in the work area: D1 and D2 receive the first and the second
 // transposition by peer stores (or hold it on a one-member group), SS and SR are the send and receive slots of the
-// all-to-all transpositions; -1: the plan has no such slot.
+// all-to-all transpositions; -1: the plan has no such slot.  BX: box plans (dfft_plan_create_boxes) only, the staging
+// array of their reshape steps, which no pass of the wrapped schedule touches.
 struct Slots {
-    int D1 = -1, D2 = -1, SS = -1, SR = -1;
+    int D1 = -1, D2 = -1, SS = -1, SR = -1, BX = -1;
     int count = 0;
 };
 // direct1 / direct2: whether the first / second transposition is direct (peer stores, or a one-member group)
@@ -479,6 +480,12 @@ struct dfft_plan_s {
     size_t batch = 1;         // fields per exec, back to back in every caller buffer (dfft_plan_create_batched)
     size_t comps = 1;         // values per grid point, interleaved (dfft_plan_create_interleaved); esize stays one value's
     double scale[2] = {1.0, 1.0};  // [fwd/inv] output scale (dfft_plan_set_scale), applied by the steps marked final_store
+    // dfft_plan_create_boxes: every rank's box of the physical grid (in_boxes) and of the output grid (out_boxes), in rank
+    // order; empty where that side has the natural layout.  box_direct: their reshapes push and gather over peer memory
+    // (comm_method Peer2Peer), otherwise they run through an NCCL all-to-all
+    std::vector<dfft::Box> in_boxes, out_boxes;
+    bool box_direct = false;
+    bool boxed() const { return !in_boxes.empty() || !out_boxes.empty(); }
     // dfft_plan_create_inplace: every exec has out == in, fields domain_bytes apart, real rows of R2C / C2R padded to Nzc
     // complex units.  buf_slot: one rank — the schedules' first slot (D1) is the caller's buffer and is not allocated.
     bool inplace = false, buf_slot = false;
@@ -621,8 +628,11 @@ static bool all_axes(const dfft_plan_s* p) { return p->taxes[0] && p->taxes[1] &
 // Whether the schedules may take another form than the sequential one: the overlapped schedules, the fused z + y stage and
 // the batched stage build their passes for power-of-two lengths, every axis transformed and no padding (their kernels have
 // no padded twins, FftPadded).
-// Interleaved plans (C > 1 values per point) run it too: those kernels address one value per point.
-static bool alt_schedules(const dfft_plan_s* p) { return pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p) && !p->g.padded() && p->comps == 1; }
+// Interleaved plans (C > 1 values per point) run it too: those kernels address one value per point.  So do plans with a
+// box that is not the natural layout: their reshape steps wrap the sequential schedule (wrap_boxes).
+static bool alt_schedules(const dfft_plan_s* p) {
+    return pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p) && !p->g.padded() && p->comps == 1 && !p->boxed();
+}
 
 // Row pitch, in elements (complex units; reals for DCT / DST plans), of the z-contiguous side of the caller's buffers that
 // holds Nz points per row: the input of forward passes, the output of inverse ones.  Real rows of R2C / C2R plans are Nz reals (Nz/2 units) apart, or, in
@@ -637,7 +647,8 @@ static long long z_row_pitch(const dfft_plan_s* p) {
 // three passes are L2-resident already and gain nothing.
 static bool zy_fused(const dfft_plan_s* p, int inverse, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || p->comps > 1) return false;
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || p->comps > 1 || p->boxed())
+        return false;
     if (g.ny != g.nz || !zy_fused_length(ilog2_exact(g.ny))) return false;
     // the fused stage reads and writes the blocked hand-over layout of the x pass
     if (p->blocked_ch <= 0 || g.nz % size_t(p->blocked_ch) || (inverse && !p->blocked_inv)) return false;
@@ -691,7 +702,8 @@ static int fuse_zy(dfft_plan_s* p, Step zs, const Step& ys, const char* label, c
 constexpr size_t BATCH_SMALL_MIN = 2;
 static bool batch_small(const dfft_plan_s* p, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || p->comps > 1) return false;
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || p->comps > 1 || p->boxed())
+        return false;
     if (g.nx != g.ny || g.ny != g.nz || !batch_small_length(ilog2_exact(g.nx))) return false;
     return p->batch >= BATCH_SMALL_MIN && p->batch * g.nx <= 0x7fffffff;
 }
@@ -2016,7 +2028,10 @@ static void field_bytes(const dfft_plan_s* p, int inverse, int d, size_t* in_b, 
     p->g.layout(p->rank, d, sd, o);
     const size_t es = p->esize * p->comps;  // bytes per point
     const size_t real_es = p->g.transform == DFFT_R2C ? es / 2 : es;
-    const size_t b0 = s0[0] * s0[1] * s0[2] * real_es, bd = sd[0] * sd[1] * sd[2] * es;
+    size_t b0 = s0[0] * s0[1] * s0[2] * real_es, bd = sd[0] * sd[1] * sd[2] * es;
+    // box plans: the caller's array on a boxed side is its box (out_boxes: the output of d = 3 only)
+    if (!p->in_boxes.empty()) b0 = p->in_boxes[p->rank].volume() * real_es;
+    if (d == 3 && !p->out_boxes.empty()) bd = p->out_boxes[p->rank].volume() * es;
     *in_b = inverse ? bd : b0;
     *out_b = inverse ? b0 : bd;
 }
@@ -2174,6 +2189,140 @@ static int widen_views(dfft_plan_s* p, Schedule& sc) {
     return DFFT_SUCCESS;
 }
 
+// ---- box-distributed plans (DESIGN.md section 3.17) ------------------------------------------------------------------
+// One side of an exec whose caller arrays are boxes: per rank the caller's box and the natural block of layout `which` (0
+// the physical side, 3 the output) that the wrapped schedule reads or writes, in the elements of the schedule's views.  The
+// real side of R2C / C2R plans is counted in complex pairs there, so its z bounds are halved (dfft_plan_create_boxes keeps
+// them even).
+struct BoxSide {
+    std::vector<Box> box, nat;
+};
+static BoxSide box_side(const dfft_plan_s* p, const std::vector<Box>& boxes, int which) {
+    BoxSide b;
+    const bool pairs = which == 0 && p->g.transform == DFFT_R2C;
+    for (int r = 0; r < p->P; ++r) {
+        size_t s[3], o[3];
+        p->g.layout(r, which, s, o);
+        Box n = Box::of(s, o), c = boxes[size_t(r)];
+        if (pairs) { n.lo[2] /= 2; n.hi[2] /= 2; c.lo[2] /= 2; c.hi[2] /= 2; }
+        b.nat.push_back(n);
+        b.box.push_back(c);
+    }
+    return b;
+}
+
+// One reshape copy: the grid points of `pc` from the dense array of box `src` at `sb` to the dense array of box `dst` at
+// `db` (both contain pc), lines along z.  An empty piece is a copy of no lines, so that every rank lists the same steps.
+static Step piece_copy(const dfft_plan_s* p, int inverse, const char* label, const Box& pc, void* sb, const Box& src, void* db, const Box& dst) {
+    Step s;
+    s.type = STEP_PASS;
+    s.kind = PASS_COPY_CONTIG;
+    s.label = label;
+    s.axis = 2;
+    const bool empty = pc.volume() == 0;
+    s.n = empty ? 0 : pc.extent(2);
+    s.prm.A0 = empty ? 0 : int(pc.extent(0));
+    s.prm.A1 = empty ? 0 : int(pc.extent(1));
+    s.prm.B = 1;
+    s.prm.inverse = inverse;
+    auto view = [&](void* base, const Box& b) {
+        return single_view(eptr(base, empty ? 0 : b.offset(pc.lo), p->esize), (long long)(b.extent(1) * b.extent(2)), (long long)b.extent(2), 1);
+    };
+    s.prm.in = view(sb, src);
+    s.prm.out = view(db, dst);
+    return s;
+}
+
+// The reshape of one boxed side: `pre` — before the first pass, from the caller's boxes (in_user 1) into the natural block
+// in slot BX; otherwise after the last pass, from the natural blocks in BX into the caller's boxes (out_user 2).
+//   Peer2Peer, pre: each rank pushes the piece of its box that every rank q owns into q's BX, then a rendezvous of all ranks.
+//     The caller's buffers are not mapped on the peers, so the owner of the data has to store it.
+//   Peer2Peer, post: a rendezvous, then each rank gathers the pieces of its box from every rank's BX (remote reads).
+//   All2All: the pieces are packed into SS at the all-to-all's send offsets, exchanged, and unpacked from SR.
+static void reshape_steps(const dfft_plan_s* p, int inverse, const BoxSide& S, bool pre, std::vector<Step>& out) {
+    const int me = p->rank, P = p->P;
+    const char* label = pre ? "reshape in" : "reshape out";
+    void* const user = nullptr;  // views on the caller's buffers hold byte offsets (user_view)
+    void* const bx = p->slot(p->slots.BX, me);
+    auto rendezvous = [&]() {
+        Step r = new_rendezvous(0, 0, nullptr, 0);
+        r.label = "reshape rendezvous";
+        out.push_back(r);
+    };
+    if (p->box_direct) {
+        if (!pre) rendezvous();
+        for (int q = 0; q < P; ++q) {
+            Step s = pre ? piece_copy(p, inverse, label, S.box[me] & S.nat[q], user, S.box[me], p->slot(p->slots.BX, q), S.nat[q])
+                         : piece_copy(p, inverse, label, S.nat[q] & S.box[me], p->slot(p->slots.BX, q), S.nat[q], user, S.box[me]);
+            (pre ? s.in_user : s.out_user) = pre ? 1 : 2;
+            out.push_back(s);
+        }
+        if (pre) rendezvous();
+        return;
+    }
+    // all-to-all: what I send to q is my part of q's box (pre: my box's part of q's natural block), what I receive q's
+    Step a;
+    a.type = STEP_A2A;
+    a.label = "nccl all-to-all";
+    a.group = 0;
+    a.send_slot = p->slots.SS;
+    a.recv_slot = p->slots.SR;
+    std::vector<Box> send(static_cast<size_t>(P)), recv(static_cast<size_t>(P));
+    size_t so = 0, ro = 0;
+    for (int q = 0; q < P; ++q) {
+        send[q] = pre ? S.box[me] & S.nat[q] : S.nat[me] & S.box[q];
+        recv[q] = pre ? S.box[q] & S.nat[me] : S.nat[q] & S.box[me];
+        a.scount.push_back(send[q].volume());
+        a.rcount.push_back(recv[q].volume());
+        a.soff.push_back(so);
+        a.roff.push_back(ro);
+        so += send[q].volume();
+        ro += recv[q].volume();
+    }
+    void* const ss = p->slot(p->slots.SS, me);
+    void* const sr = p->slot(p->slots.SR, me);
+    for (int q = 0; q < P; ++q) {
+        Step s = pre ? piece_copy(p, inverse, label, send[q], user, S.box[me], eptr(ss, a.soff[q], p->esize), send[q])
+                     : piece_copy(p, inverse, label, send[q], bx, S.nat[me], eptr(ss, a.soff[q], p->esize), send[q]);
+        if (pre) s.in_user = 1;
+        out.push_back(s);
+    }
+    out.push_back(a);
+    for (int q = 0; q < P; ++q) {
+        Step s = pre ? piece_copy(p, inverse, label, recv[q], eptr(sr, a.roff[q], p->esize), recv[q], bx, S.nat[me])
+                     : piece_copy(p, inverse, label, recv[q], eptr(sr, a.roff[q], p->esize), recv[q], user, S.box[me]);
+        if (!pre) s.out_user = 2;
+        out.push_back(s);
+    }
+}
+
+// Box plans: the schedule of the natural layouts, its views on a boxed side's caller buffer moved to the same offsets in
+// slot BX, with the reshape of that side before it (after its entry rendezvous: the peers have left the previous exec) or
+// after it.  Forward: the physical side is `in`, the output `out`; inverse the other way round.  out_boxes apply to d = 3
+// only: the spectral side of a partial exec keeps its natural layout.  BX holds the natural array of a side only between
+// its reshape and the pass that reads it (pre), or the pass that writes it and its reshape (post); the wrapped schedule
+// reads the pre side's data before it writes the post side's (one slot serves both).
+static int wrap_boxes(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
+    const bool phys = !p->in_boxes.empty(), spec = d == 3 && !p->out_boxes.empty();
+    const bool pre = inverse ? spec : phys, post = inverse ? phys : spec;
+    if (!pre && !post) return DFFT_SUCCESS;
+    if (p->slots.BX < 0) return fail(DFFT_ERR_STATE, "internal: box plan without a staging slot");
+    char* const bx = static_cast<char*>(p->slot(p->slots.BX, p->rank));
+    for (Step& s : sc.steps) {
+        if (s.type != STEP_PASS) continue;
+        if (s.kernel != KERNEL_PASS) return fail(DFFT_ERR_STATE, "internal: box plans run single passes");
+        if (pre && s.in_user == 1) { s.prm.in.seg[0].base = bx + (size_t)s.prm.in.seg[0].base; s.in_user = 0; }
+        if (post && s.out_user == 2) { s.prm.out.seg[0].base = bx + (size_t)s.prm.out.seg[0].base; s.out_user = 0; }
+    }
+    std::vector<Step> head, tail;
+    if (pre) reshape_steps(p, inverse, box_side(p, inverse ? p->out_boxes : p->in_boxes, inverse ? 3 : 0), true, head);
+    if (post) reshape_steps(p, inverse, box_side(p, inverse ? p->in_boxes : p->out_boxes, inverse ? 0 : 3), false, tail);
+    const bool entry = !sc.steps.empty() && sc.steps[0].type == STEP_RENDEZVOUS && sc.steps[0].group == 0;
+    sc.steps.insert(sc.steps.begin() + (entry ? 1 : 0), head.begin(), head.end());
+    sc.steps.insert(sc.steps.end(), tail.begin(), tail.end());
+    return DFFT_SUCCESS;
+}
+
 // The one place that decides which schedule a (direction, d) pair runs — used by exec and by dfft_plan_describe, so
 // the CPU schedule emulation always validates exactly what executes.
 static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
@@ -2209,6 +2358,8 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
             name_copies(sc);
             drop_z_copy(p, sc, inverse ? 1 : 0);
         }
+        rc = wrap_boxes(p, inverse ? 1 : 0, d, sc);
+        if (rc) return rc;
         // No step reads the caller's `out` (views on it are only ever stored to), so every store into it is an output
         // value of the exec: the steps that write `out` are exactly the ones that store final values.  This covers the tail
         // launches of blocked hand-over layouts, every z chunk of overlapped x passes, the last pass of partial transforms
@@ -2452,7 +2603,8 @@ int dfft_plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, in
 // spectral: Kx, Ky, Kz of the plans of dfft_plan_create_padded (checked there), nullptr otherwise.
 static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
                        size_t nz, size_t p1, size_t p2, size_t batch, bool inplace, int allocate, dfft_plan_t* plan,
-                       const int* kinds = nullptr, const size_t* spectral = nullptr, size_t comps = 1) {
+                       const int* kinds = nullptr, const size_t* spectral = nullptr, size_t comps = 1,
+                       const std::vector<dfft::Box>* in_boxes = nullptr, const std::vector<dfft::Box>* out_boxes = nullptr) {
     if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
     if (batch == 0) return fail(DFFT_ERR_INVALID, "batch must be at least 1");
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
@@ -2509,9 +2661,28 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
         return fail(DFFT_ERR_INVALID, "partition leaves a rank without data");
     }
     p->inplace = inplace;
+    // box plans (dfft_plan_create_boxes, which checked the tiling): a side whose boxes are all natural keeps no boxes, so
+    // that it makes exactly the plan of dfft_plan_create_batched
+    auto keep_boxes = [&](const std::vector<Box>* b, int which, std::vector<Box>& dst) {
+        if (!b) return;
+        for (int r = 0; r < p->P; ++r) {
+            size_t s_[3], o_[3];
+            g.layout(r, which, s_, o_);
+            if (!((*b)[size_t(r)] == Box::of(s_, o_))) { dst = *b; return; }
+        }
+    };
+    keep_boxes(in_boxes, 0, p->in_boxes);
+    keep_boxes(out_boxes, 3, p->out_boxes);
+    // elements (of the schedule's views) of rank r's box arrays: the real side of R2C / C2R in complex pairs
+    auto box_elems = [&](int r) {
+        size_t m = 0;
+        if (!p->in_boxes.empty()) m = p->in_boxes[size_t(r)].volume() / (transform == DFFT_R2C ? 2 : 1);
+        if (!p->out_boxes.empty()) m = std::max(m, p->out_boxes[size_t(r)].volume());
+        return m;
+    };
     // the largest stage array of this rank; it also covers the padded real input of in-place R2C plans, which has the
     // extent of the layout after d = 1
-    p->domain_bytes = g.domain_elems(p->rank) * p->esize * comps;
+    p->domain_bytes = std::max(g.domain_elems(p->rank), box_elems(p->rank)) * p->esize * comps;
     {   // the whole batch of every caller buffer (any direction, any partial d) must be addressable
         size_t widest = 0;
         for (int d = 1; d <= 3; ++d) {
@@ -2547,11 +2718,19 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
     if (decomp == DFFT_SLAB_Z_THEN_YX) p->direct2 = true;
     p->any_direct = (p->direct1 && p->grp[1].size() > 1) || (p->direct2 && p->grp[2].size() > 1);
     p->slots = plan_slots(p->direct1 || p->grp[1].size() == 1, p->direct2 || p->grp[2].size() == 1);
+    if (p->boxed()) {
+        // the reshapes: over peer memory with comm_method Peer2Peer (which needs the peer mapping and the entry rendezvous),
+        // else through the all-to-all slots; and their staging slot BX
+        p->box_direct = p->cfg.comm_method != DFFT_ALL2ALL;
+        if (p->box_direct) p->any_direct = true;
+        else if (p->slots.SS < 0) { p->slots.SS = p->slots.count++; p->slots.SR = p->slots.count++; }
+        p->slots.BX = p->slots.count++;
+    }
     // in place on one rank the caller's buffer is the schedules' first slot (D1; both transpositions are local there)
     p->buf_slot = inplace && P == 1;
     p->nslots = p->slots.count - (p->buf_slot ? 1 : 0);
     size_t dom = 0;
-    for (int r = 0; r < P; ++r) dom = std::max(dom, g.domain_elems(r));
+    for (int r = 0; r < P; ++r) dom = std::max(dom, std::max(g.domain_elems(r), box_elems(r)));
     p->slot_bytes = ((dom * p->esize * comps + 255) / 256) * 256;
     p->work_bytes = p->slot_bytes * p->nslots;
     {
@@ -2670,6 +2849,35 @@ int dfft_plan_create_inplace(dfft_comm_t comm, const dfft_config* config, int de
 }
 
 int dfft_plan_is_inplace(dfft_plan_t p) { return p && p->inplace ? 1 : 0; }
+
+// Box plans (DESIGN.md section 3.17): the boxes are checked here, before plan_create allocates anything.
+int dfft_plan_create_boxes(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny, size_t nz,
+                           size_t p1, size_t p2, const size_t* in_boxes, const size_t* out_boxes, size_t batch, int allocate, dfft_plan_t* plan) {
+    if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
+    if (transform != DFFT_C2C && transform != DFFT_R2C && transform != DFFT_DCT && transform != DFFT_DST)
+        return fail(DFFT_ERR_INVALID, "box plans are C2C, R2C / C2R, DCT or DST");
+    const size_t P = size_t(comm->nranks);
+    const size_t grid[2][3] = {{nx, ny, nz}, {nx, ny, transform == DFFT_R2C ? nz / 2 + 1 : nz}};
+    std::vector<Box> boxes[2];
+    const size_t* given[2] = {in_boxes, out_boxes};
+    for (int side = 0; side < 2; ++side) {
+        if (!given[side]) continue;
+        for (size_t r = 0; r < P; ++r) {
+            Box b;
+            for (int a = 0; a < 3; ++a) { b.lo[a] = given[side][6 * r + a]; b.hi[a] = given[side][6 * r + 3 + a]; }
+            boxes[side].push_back(b);
+        }
+        if (!tiles(boxes[side], grid[side]))
+            return fail(DFFT_ERR_INVALID, std::string(side ? "out_boxes" : "in_boxes") +
+                                              " must tile the grid: every box non-empty and inside it, no two overlapping, together all of it");
+    }
+    // the real side of R2C / C2R plans moves as pairs of reals (the z pass's complex units)
+    if (transform == DFFT_R2C)
+        for (const Box& b : boxes[0])
+            if (b.lo[2] % 2 || b.hi[2] % 2) return fail(DFFT_ERR_UNSUPPORTED, "R2C / C2R box plans need even z bounds in in_boxes");
+    return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, false, allocate, plan, nullptr, nullptr, 1,
+                       in_boxes ? &boxes[0] : nullptr, out_boxes ? &boxes[1] : nullptr);
+}
 
 int dfft_plan_create_padded(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
                             size_t nz, size_t kx, size_t ky, size_t kz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan) {
@@ -2822,6 +3030,10 @@ static int layout_of(dfft_plan_t p, int which, size_t size[3], size_t start[3]) 
     if (!p) return fail(DFFT_ERR_INVALID, "null plan");
     size_t s[3], o[3];
     p->g.layout(p->rank, which, s, o);
+    // box plans: this rank's box on a boxed side (the physical side of every d, the output of d = 3)
+    const std::vector<Box>& boxes = which == 0 ? p->in_boxes : p->out_boxes;
+    if ((which == 0 || which == 3) && !boxes.empty())
+        for (int k = 0; k < 3; ++k) { s[k] = boxes[size_t(p->rank)].extent(k); o[k] = boxes[size_t(p->rank)].lo[k]; }
     for (int k = 0; k < 3; ++k) {
         if (size) size[k] = s[k];
         if (start) start[k] = o[k];
@@ -3028,6 +3240,7 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
                          : !all_axes(p)         ? "sequential schedule (no alternatives for this plan: plans with a kept axis run the sequential schedule)"
                          : p->g.padded()        ? "sequential schedule (no alternatives for this plan: padded plans run the sequential schedule)"
                          : p->comps > 1         ? "sequential schedule (no alternatives for this plan: interleaved plans run the sequential schedule)"
+                         : p->boxed()           ? "sequential schedule (no alternatives for this plan: box plans run the sequential schedule)"
                          : pow2_axes(p)         ? "sequential schedule (no alternatives for this plan)"
                                                 : "sequential schedule (no alternatives for this plan: an axis length is not a power of two)";
         return 0;
@@ -3133,6 +3346,17 @@ static void json_view(std::string& o, const View& v, const Tables& T) {
     }
     o += "]}";
 }
+// ,"name":[[lx,ly,lz,hx,hy,hz], ...] of box plans; nothing for a side with the natural layout
+static std::string json_boxes(const char* name, const std::vector<Box>& boxes) {
+    if (boxes.empty()) return std::string();
+    std::string o = std::string(",\"") + name + "\":[";
+    for (size_t r = 0; r < boxes.size(); ++r) {
+        o += r ? ",[" : "[";
+        for (int k = 0; k < 6; ++k) o += (k ? "," : "") + std::to_string(k < 3 ? boxes[r].lo[k] : boxes[r].hi[k - 3]);
+        o += "]";
+    }
+    return o + "]";
+}
 int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capacity, size_t* needed) {
     if (!p || d < 1 || d > 3) return fail(DFFT_ERR_INVALID, "bad arguments");
     Schedule* scp = nullptr;
@@ -3155,6 +3379,7 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
                     (p->g.padded() ? ",\"spectral\":[" + std::to_string(p->g.kx) + "," + std::to_string(p->g.ky) + "," + std::to_string(p->g.kz) + "]"
                                    : std::string()) +
                     (p->comps > 1 ? ",\"components\":" + std::to_string(p->comps) : std::string()) +
+                    json_boxes("in_boxes", p->in_boxes) + json_boxes("out_boxes", p->out_boxes) +
                     (p->batch > 1 ? ",\"batch\":" + std::to_string(p->batch) + ",\"field_in\":" + std::to_string(sc.field_in) +
                                         ",\"field_out\":" + std::to_string(sc.field_out)
                                   : std::string()) +

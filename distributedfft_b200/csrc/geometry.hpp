@@ -24,6 +24,47 @@ struct Split {
     }
 };
 
+// A box of grid points [lo, hi) per axis (x, y, z), the unit of dfft_plan_create_boxes: each rank's caller array is its box,
+// dense, z contiguous.
+struct Box {
+    size_t lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0};
+    static Box of(const size_t size[3], const size_t start[3]) {
+        Box b;
+        for (int a = 0; a < 3; ++a) { b.lo[a] = start[a]; b.hi[a] = start[a] + size[a]; }
+        return b;
+    }
+    size_t extent(int a) const { return hi[a] > lo[a] ? hi[a] - lo[a] : 0; }
+    size_t volume() const { return extent(0) * extent(1) * extent(2); }
+    bool operator==(const Box& o) const {
+        for (int a = 0; a < 3; ++a)
+            if (lo[a] != o.lo[a] || hi[a] != o.hi[a]) return false;
+        return true;
+    }
+    // the common part (volume 0 if there is none)
+    Box operator&(const Box& o) const {
+        Box b;
+        for (int a = 0; a < 3; ++a) { b.lo[a] = std::max(lo[a], o.lo[a]); b.hi[a] = std::max(b.lo[a], std::min(hi[a], o.hi[a])); }
+        return b;
+    }
+    // element offset of grid point p (inside the box) in the box's dense array
+    size_t offset(const size_t p[3]) const { return ((p[0] - lo[0]) * extent(1) + (p[1] - lo[1])) * extent(2) + (p[2] - lo[2]); }
+};
+
+// Whether `boxes` tile the grid n[0] x n[1] x n[2]: none empty or reaching outside it, no two overlapping, and their
+// volumes adding up to the grid's (so that together they cover it).
+inline bool tiles(const std::vector<Box>& boxes, const size_t n[3]) {
+    size_t total = 0;
+    for (size_t i = 0; i < boxes.size(); ++i) {
+        const Box& b = boxes[i];
+        for (int a = 0; a < 3; ++a)
+            if (b.lo[a] >= b.hi[a] || b.hi[a] > n[a]) return false;
+        for (size_t j = 0; j < i; ++j)
+            if ((b & boxes[j]).volume()) return false;
+        total += b.volume();
+    }
+    return total == n[0] * n[1] * n[2];
+}
+
 struct Geometry {
     int decomp = 0, transform = 0;
     size_t nx = 0, ny = 0, nz = 0, nzc = 0;  // nzc: z extent of every complex array (real-to-real: of every real array, Nz)

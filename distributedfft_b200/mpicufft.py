@@ -131,7 +131,7 @@ class MPIcuFFT:
     # -- plan ------------------------------------------------------------------------------------
     def initFFT(self, global_size: GlobalSize, partition: Optional[Partition] = None, allocate: bool = True, batch: int = 1,
                 inplace: bool = False, transform_axes: Optional[Sequence[bool]] = None, spectral: Optional[Sequence[int]] = None,
-                components: int = 1):
+                components: int = 1, in_boxes=None, out_boxes=None):
         """`batch` (not in the reference): every exec transforms that many fields, back to back in each buffer — a
         contiguous [batch, X, Y, Z] tensor; the getters describe one field (dfft_plan_create_batched).
         `inplace` (dfft_plan_create_inplace): every exec gets the same buffer twice and overwrites its input; fields are
@@ -142,7 +142,11 @@ class MPIcuFFT:
         spectrum it keeps — the forward stores only those modes, the inverse zero-pads them (the 3/2 dealiasing rule).
         `components` C (dfft_plan_create_interleaved): every grid point holds C consecutive values, each component
         transformed on its own — buffers are [X, Y, Z, C] tensors ([B, X, Y, Z, C] with a batch), reals on the real side
-        of R2C / C2R; C > 1 plans are C2C or R2C / C2R, out of place and not padded."""
+        of R2C / C2R; C > 1 plans are C2C or R2C / C2R, out of place and not padded.
+        `in_boxes` / `out_boxes` (dfft_plan_create_boxes): one box ((lx, ly, lz), (hx, hy, hz)) per rank, in rank order, of the
+        physical grid and of the output grid (z extent Nz/2 + 1 for R2C); each rank's buffer on that side is its box, a dense
+        [hx-lx, hy-ly, hz-lz] tensor, and the exec redistributes on the GPU.  None keeps the natural layout.  Box plans are
+        out of place, not padded, with one component and one transform for all axes."""
         if global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         cfg = _lib.dfft_config(int(self.config.cuda_aware), int(self.config.warmup_rounds), int(self.config.comm_method),
@@ -154,7 +158,26 @@ class MPIcuFFT:
         if self._decomp == PENCIL and partition is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         h = C.c_void_p()
-        if components != 1:
+        if in_boxes is not None or out_boxes is not None:
+            if inplace or spectral is not None or components != 1 or self.kinds is not None:
+                raise ValueError("box plans are out of place, not padded, with one component and one transform kind for all axes")
+            if batch < 1:
+                raise ValueError("batch must be at least 1")
+
+            def flat(boxes):
+                if boxes is None:
+                    return None
+                boxes = list(boxes)
+                if len(boxes) != self.comm.size:
+                    raise ValueError(f"{len(boxes)} boxes for {self.comm.size} ranks")
+                vals = [int(v) for lo, hi in boxes for v in (*lo, *hi)]
+                if len(vals) != 6 * self.comm.size:
+                    raise ValueError("a box is ((lx, ly, lz), (hx, hy, hz))")
+                return (C.c_size_t * len(vals))(*vals)
+            check(lib().dfft_plan_create_boxes(self.comm._h, C.byref(cfg), self._decomp, self.precision, self.transform, global_size.Nx,
+                                               global_size.Ny, global_size.Nz, p1, p2, flat(in_boxes), flat(out_boxes), batch,
+                                               1 if allocate else 0, C.byref(h)))
+        elif components != 1:
             if spectral is not None or inplace or self.kinds is not None:
                 raise ValueError("interleaved plans are out of place and not padded")
             if batch < 1:
@@ -380,13 +403,14 @@ class MPIcuFFT_Pencil(MPIcuFFT):
     """z FFT -> transpose -> y FFT -> transpose -> x FFT on a P1 x P2 grid. include/mpicufft_pencil.hpp."""
     _decomp = PENCIL
 
-    def initFFT(self, global_size, partition=None, allocate=True, batch=1, inplace=False, transform_axes=None, spectral=None, components=1):
+    def initFFT(self, global_size, partition=None, allocate=True, batch=1, inplace=False, transform_axes=None, spectral=None, components=1,
+                in_boxes=None, out_boxes=None):
         if partition is None or global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         if partition.P1 * partition.P2 != self.comm.size:
             raise RuntimeError("Invalid Input Partition!")
         self.partition = partition
-        super().initFFT(global_size, partition, allocate, batch, inplace, transform_axes, spectral, components)
+        super().initFFT(global_size, partition, allocate, batch, inplace, transform_axes, spectral, components, in_boxes, out_boxes)
 
     def getPartitionDimensions(self):
         """(input_dim, transposed_dim, output_dim), each a dict with size_x/y/z and start_x/y/z lists

@@ -250,6 +250,32 @@ int dfft_plan_create_interleaved(dfft_comm_t comm, const dfft_config* config, in
                                  int transform /*dfft_transform*/, size_t nx, size_t ny, size_t nz, size_t p1, size_t p2,
                                  size_t components, size_t batch, int allocate, dfft_plan_t* plan);
 size_t dfft_get_components(dfft_plan_t plan); /* 1 for every other plan, 0 for a null plan */
+/* Box-distributed plans (heFFTe's box3d in and out, cuFFTMp's cufftXtSetDistribution): each rank's input and output is a
+ * box of the grid the caller chooses, e.g. the Px x Py x Pz bricks of a particle-mesh or PSATD code, and the exec
+ * redistributes between those boxes and the plan's own layouts on the GPU.
+ *   - in_boxes / out_boxes: 6 * P values each, for rank r lo[3], hi[3] (x, y, z; half-open) at 6 r, the same arrays on every
+ *     rank.  in_boxes tile the physical grid Nx x Ny x Nz, out_boxes the output grid Nx x Ny x Nzc (Nzc = Nz/2 + 1 for R2C,
+ *     Nz otherwise).  NULL: that side keeps the natural layout (dfft_layout).  Boxes equal to the natural layout (and any
+ *     box of one rank, which is the whole grid) make the plan of dfft_plan_create_batched: the same steps and output.
+ *   - Each rank's caller buffer on a boxed side is its box as a dense [hx-lx][hy-ly][hz-lz] array, z contiguous (reals on
+ *     the real side of R2C / C2R and for DCT / DST); `batch` fields sit back to back, one box volume apart.
+ *   - in_boxes apply to the physical side of every exec (partial d included), out_boxes to the output of d = 3; the
+ *     spectral side of d < 3 keeps its natural layout.  dfft_get_in_* report this rank's input box, dfft_get_out_* and
+ *     dfft_get_partial_*(3) its output box; dfft_get_domain_size and dfft_get_work_size_device cover the box arrays.
+ *   - The exec copies the boxes into the plan's layout before the first pass and out of it after the last one: with
+ *     comm_method Peer2Peer each rank pushes its pieces into the owners' work areas (input) or gathers them from there
+ *     (output) over peer memory, with All2All through an NCCL all-to-all.  One copy sweep per boxed side and a rendezvous
+ *     or all-to-all; the FFT passes are those of the natural plan.  dfft_plan_describe reports "in_boxes" / "out_boxes"
+ *     and labels the copies "reshape in" / "reshape out".
+ *   - C2C (Bluestein lengths included), R2C / C2R, DCT and DST on every decomposition; batches, dfft_plan_set_scale,
+ *     dfft_plan_set_transform_axes and the timer work as for other plans.  Plans with a box other than the natural one
+ *     run the sequential schedule (dfft_plan_tune has one candidate).
+ *   - DFFT_ERR_INVALID: another transform, a box that is empty or reaches outside its grid, overlapping boxes, or boxes
+ *     that do not cover the grid.  DFFT_ERR_UNSUPPORTED: an odd z bound in the in_boxes of an R2C / C2R plan (its real
+ *     rows move as pairs of reals).  No in-place, padded, interleaved or per-axis R2R form. */
+int dfft_plan_create_boxes(dfft_comm_t comm, const dfft_config* config, int decomp /*dfft_decomp*/, int precision /*dfft_prec*/,
+                           int transform /*dfft_transform*/, size_t nx, size_t ny, size_t nz, size_t p1, size_t p2,
+                           const size_t* in_boxes, const size_t* out_boxes, size_t batch, int allocate, dfft_plan_t* plan);
 int dfft_plan_destroy(dfft_plan_t plan);
 /* setWorkArea(device, host) — mpicufft_slab.cpp:236-281. device must hold dfft_get_work_size_device()
  * bytes; with comm_method Peer2Peer and more than one rank it must be the base of a cudaMalloc

@@ -115,6 +115,15 @@ public:
         initFFT(global_size, partition, allocate, batch);
     }
     size_t getComponents() const { return dfft_get_components(plan); }
+    // not in the reference: a box plan (dfft_plan_create_boxes): in_boxes / out_boxes hold lo[3], hi[3] of every rank in
+    // rank order (6 values each; null: the natural layout), and each rank's buffers are its boxes
+    void initFFT(GlobalSize* global_size, Partition* partition, const size_t* in_boxes, const size_t* out_boxes, bool allocate = true,
+                 size_t batch = 1) {
+        struct Reset { const size_t*& i; const size_t*& o; ~Reset() { i = nullptr; o = nullptr; } } reset{in_boxes_, out_boxes_};
+        in_boxes_ = in_boxes;
+        out_boxes_ = out_boxes;
+        initFFT(global_size, partition, allocate, batch);
+    }
     // kx, ky, kz of a padded plan; Nx, Ny, Nz of every other plan
     void getSpectralSize(size_t* k) const { DFFT_CALL(dfft_plan_get_spectral_size(plan, k)); }
     size_t getBatch() const { return dfft_get_batch(plan); }
@@ -160,7 +169,10 @@ protected:
         c.benchmark_dir = config.benchmark_dir.empty() ? nullptr : config.benchmark_dir.c_str();
         c.comm_method2 = config.comm_method2; c.send_method2 = config.send_method2;
         if (plan) { dfft_plan_destroy(plan); plan = nullptr; }
-        if (components_ != 1)
+        if (in_boxes_ || out_boxes_)
+            DFFT_CALL(dfft_plan_create_boxes(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, p1, p2, in_boxes_,
+                                             out_boxes_, batch_, allocate ? 1 : 0, &plan));
+        else if (components_ != 1)
             DFFT_CALL(dfft_plan_create_interleaved(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, p1, p2,
                                                    components_, batch_, allocate ? 1 : 0, &plan));
         else if (spectral_)
@@ -183,6 +195,8 @@ protected:
     bool inplace_ = false;   // whether initFFT is creating an in-place plan
     GlobalSize* spectral_ = nullptr;  // the spectrum of the padded plan initFFT is creating
     size_t components_ = 1;  // values per point of the interleaved plan initFFTInterleaved is creating
+    const size_t* in_boxes_ = nullptr;   // the boxes of the box plan initFFT is creating
+    const size_t* out_boxes_ = nullptr;
     Configurations config;
     dfft_comm_t comm;
     int transform;
