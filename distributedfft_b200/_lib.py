@@ -83,6 +83,8 @@ SIGNATURES = {
     "dfft_exec_r2r_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "dfft_plan_set_transform_axes": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
     "dfft_plan_get_transform_axes": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
+    "dfft_plan_set_strides": (C.c_int, [C.c_void_p, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]),
+    "dfft_plan_get_strides": (C.c_int, [C.c_void_p, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]),
     "dfft_plan_wait": (C.c_int, [C.c_void_p]),
     "dfft_get_in_size": (C.c_int, [C.c_void_p, C.POINTER(C.c_size_t)]),
     "dfft_get_in_start": (C.c_int, [C.c_void_p, C.POINTER(C.c_size_t)]),

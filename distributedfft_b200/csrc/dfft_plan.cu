@@ -486,6 +486,12 @@ struct dfft_plan_s {
     std::vector<dfft::Box> in_boxes, out_boxes;
     bool box_direct = false;
     bool boxed() const { return !in_boxes.empty() || !out_boxes.empty(); }
+    // dfft_plan_set_strides: the caller's {field, x, y} strides of the physical side (in) and of the output of d = 3 (out),
+    // in that side's elements (reals on the real side of R2C / C2R and for R2R plans); z is contiguous.  A side without
+    // them is dense.
+    long long in_strides[3] = {0, 0, 0}, out_strides[3] = {0, 0, 0};
+    bool in_embedded = false, out_embedded = false;
+    bool embedded() const { return in_embedded || out_embedded; }
     // dfft_plan_create_inplace: every exec has out == in, fields domain_bytes apart, real rows of R2C / C2R padded to Nzc
     // complex units.  buf_slot: one rank — the schedules' first slot (D1) is the caller's buffer and is not allocated.
     bool inplace = false, buf_slot = false;
@@ -629,9 +635,10 @@ static bool all_axes(const dfft_plan_s* p) { return p->taxes[0] && p->taxes[1] &
 // the batched stage build their passes for power-of-two lengths, every axis transformed and no padding (their kernels have
 // no padded twins, FftPadded).
 // Interleaved plans (C > 1 values per point) run it too: those kernels address one value per point.  So do plans with a
-// box that is not the natural layout: their reshape steps wrap the sequential schedule (wrap_boxes).
+// box that is not the natural layout: their reshape steps wrap the sequential schedule (wrap_boxes).  And embedded plans
+// (dfft_plan_set_strides): the other forms read and write dense caller arrays, and every rank must run the same form.
 static bool alt_schedules(const dfft_plan_s* p) {
-    return pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p) && !p->g.padded() && p->comps == 1 && !p->boxed();
+    return pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p) && !p->g.padded() && p->comps == 1 && !p->boxed() && !p->embedded();
 }
 
 // Row pitch, in elements (complex units; reals for DCT / DST plans), of the z-contiguous side of the caller's buffers that
@@ -647,7 +654,8 @@ static long long z_row_pitch(const dfft_plan_s* p) {
 // three passes are L2-resident already and gain nothing.
 static bool zy_fused(const dfft_plan_s* p, int inverse, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || p->comps > 1 || p->boxed())
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || p->comps > 1 || p->boxed() ||
+        p->embedded())
         return false;
     if (g.ny != g.nz || !zy_fused_length(ilog2_exact(g.ny))) return false;
     // the fused stage reads and writes the blocked hand-over layout of the x pass
@@ -702,7 +710,8 @@ static int fuse_zy(dfft_plan_s* p, Step zs, const Step& ys, const char* label, c
 constexpr size_t BATCH_SMALL_MIN = 2;
 static bool batch_small(const dfft_plan_s* p, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || p->comps > 1 || p->boxed())
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || p->comps > 1 || p->boxed() ||
+        p->embedded())
         return false;
     if (g.nx != g.ny || g.ny != g.nz || !batch_small_length(ilog2_exact(g.nx))) return false;
     return p->batch >= BATCH_SMALL_MIN && p->batch * g.nx <= 0x7fffffff;
@@ -2032,6 +2041,9 @@ static void field_bytes(const dfft_plan_s* p, int inverse, int d, size_t* in_b, 
     // box plans: the caller's array on a boxed side is its box (out_boxes: the output of d = 3 only)
     if (!p->in_boxes.empty()) b0 = p->in_boxes[p->rank].volume() * real_es;
     if (d == 3 && !p->out_boxes.empty()) bd = p->out_boxes[p->rank].volume() * es;
+    // embedded sides: the caller's field stride
+    if (p->in_embedded) b0 = size_t(p->in_strides[0]) * real_es;
+    if (d == 3 && p->out_embedded) bd = size_t(p->out_strides[0]) * es;
     *in_b = inverse ? bd : b0;
     *out_b = inverse ? b0 : bd;
 }
@@ -2189,6 +2201,15 @@ static int widen_views(dfft_plan_s* p, Schedule& sc) {
     return DFFT_SUCCESS;
 }
 
+// This rank's block of layout `which` (0 input, 1 and 2 after z and y, 3 output) as the caller holds it: its box on a boxed
+// side of a box plan (the physical side of every d, the output of d = 3), the plan's own layout otherwise
+static void caller_block(const dfft_plan_s* p, int which, size_t s[3], size_t o[3]) {
+    p->g.layout(p->rank, which, s, o);
+    const std::vector<Box>& boxes = which == 0 ? p->in_boxes : p->out_boxes;
+    if ((which == 0 || which == 3) && !boxes.empty())
+        for (int k = 0; k < 3; ++k) { s[k] = boxes[size_t(p->rank)].extent(k); o[k] = boxes[size_t(p->rank)].lo[k]; }
+}
+
 // ---- box-distributed plans (DESIGN.md section 3.17) ------------------------------------------------------------------
 // One side of an exec whose caller arrays are boxes: per rank the caller's box and the natural block of layout `which` (0
 // the physical side, 3 the output) that the wrapped schedule reads or writes, in the elements of the schedule's views.  The
@@ -2323,6 +2344,114 @@ static int wrap_boxes(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     return DFFT_SUCCESS;
 }
 
+// ---- embedded layouts (DESIGN.md section 3.18) -----------------------------------------------------------------------
+// One side of an exec on caller arrays with their own strides (dfft_plan_set_strides): the dense block e[x][y][z] that the
+// schedule's views on that buffer address, and the caller's x and y strides, both in the views' elements (complex pairs on
+// the real side of R2C / C2R, whose strides are even).
+struct EmbedSide {
+    bool on = false;
+    size_t e[3] = {0, 0, 0};
+    long long sx = 0, sy = 0;
+};
+static EmbedSide embed_side(const dfft_plan_s* p, bool physical) {
+    EmbedSide E;
+    E.on = physical ? p->in_embedded : p->out_embedded;
+    if (!E.on) return E;
+    size_t o[3];
+    caller_block(p, physical ? 0 : 3, E.e, o);
+    const long long* s = physical ? p->in_strides : p->out_strides;
+    const long long pairs = physical && p->g.transform == DFFT_R2C ? 2 : 1;
+    E.e[2] /= size_t(pairs);
+    E.sx = s[1] / pairs;
+    E.sy = s[2] / pairs;
+    return E;
+}
+
+// The views of one pass (or one phase of the fused stage) on embedded sides: a view on the dense block maps base offset
+// i Ny Nz + j Nz + k to i X + j Y + k, and each of its dimensions (a0, a1, n and the contiguous b) to the caller's stride of
+// the one axis it runs along.  That is exact when no dimension carries into the next axis: per axis, the base's index plus
+// the reach of every dimension along it stays inside the block, which is checked.  The one dimension that may span two
+// axes is b of a TILED pass whose rows are whole y-z planes (x passes without the blocked hand-over, B = y rows x z
+// columns): it is split into a1 = the y rows and b = z first, for both views, which needs a1 unused.  es: bytes per element;
+// in_len / out_len: points along n of each view.
+static int embed_pass(FftParams& prm, int in_user, int out_user, const EmbedSide& Ein, const EmbedSide& Eout, size_t es, size_t in_len,
+                      size_t out_len) {
+    auto split_needed = [&](const View& v, const EmbedSide& E) {
+        const long long off = (long long)(size_t)v.seg[0].base / (long long)es;
+        return E.on && E.e[2] > 0 && prm.B > 0 && off % (long long)E.e[2] + prm.B > (long long)E.e[2];
+    };
+    for (int w = 0; w < 2; ++w) {
+        const View& v = w ? prm.out : prm.in;
+        const EmbedSide& E = w ? Eout : Ein;
+        if (!(w ? out_user : in_user) || !split_needed(v, E)) continue;
+        const long long nz = (long long)E.e[2], off = (long long)(size_t)v.seg[0].base / (long long)es;
+        if (prm.A1 != 1 || off % nz != 0 || prm.B % nz != 0) return fail(DFFT_ERR_STATE, "internal: an embedded view's rows span more than y and z");
+        prm.A1 = int(prm.B / nz);
+        prm.B = int(nz);
+        for (View* u : {&prm.in, &prm.out})
+            for (int i = 0; i < u->nseg; ++i) u->seg[i].sA1 = nz;
+    }
+    auto map = [&](View& v, const EmbedSide& E, size_t len) -> int {
+        if (v.nseg != 1) return fail(DFFT_ERR_STATE, "internal: an embedded view has segments");
+        const size_t bytes = (size_t)v.seg[0].base;
+        const long long ext[4] = {prm.A0, prm.A1, (long long)len, prm.B};
+        long long* const stride[3] = {&v.seg[0].sA0, &v.seg[0].sA1, &v.sN};
+        const long long plane = (long long)(E.e[1] * E.e[2]), row = (long long)E.e[2];
+        if (ext[0] <= 0 || ext[1] <= 0 || ext[2] <= 0 || ext[3] <= 0) {  // no element: nothing to address
+            v.seg[0].base = nullptr;
+            return DFFT_SUCCESS;
+        }
+        if (plane == 0) return fail(DFFT_ERR_STATE, "internal: an embedded view on an empty block");
+        if (bytes % es) return fail(DFFT_ERR_STATE, "internal: an embedded view's offset is not whole elements");
+        // (x, y, z) of an offset in the dense block; S: the caller's stride of each axis
+        auto split = [&](long long o, long long c[3]) { c[0] = o / plane; c[1] = o % plane / row; c[2] = o % row; };
+        const long long S[3] = {E.sx, E.sy, 1};
+        long long reach[3];
+        split((long long)(bytes / es), reach);
+        long long base = reach[0] * S[0] + reach[1] * S[1] + reach[2] * S[2];
+        for (int k = 0; k < 4; ++k) {
+            const long long s = k < 3 ? *stride[k] : 1;
+            long long c[3];
+            if (s < 0) return fail(DFFT_ERR_STATE, "internal: an embedded view runs backwards");
+            split(s, c);
+            const int axes = (c[0] != 0) + (c[1] != 0) + (c[2] != 0);
+            if (ext[k] > 1 && axes > 1) return fail(DFFT_ERR_STATE, "internal: an embedded view's dimension spans two axes");
+            for (int a = 0; a < 3; ++a) reach[a] += (ext[k] - 1) * c[a];
+            if (k < 3) *stride[k] = ext[k] > 1 ? c[0] * S[0] + c[1] * S[1] + c[2] * S[2] : 0;
+        }
+        for (int a = 0; a < 3; ++a)
+            if (reach[a] >= (long long)E.e[a]) return fail(DFFT_ERR_STATE, "internal: an embedded view leaves its block");
+        v.seg[0].base = reinterpret_cast<void*>(size_t(base) * es);
+        return DFFT_SUCCESS;
+    };
+    int rc = DFFT_SUCCESS;
+    if (in_user && Ein.on) rc = map(prm.in, Ein, in_len);
+    if (!rc && out_user && Eout.on) rc = map(prm.out, Eout, out_len);
+    return rc;
+}
+
+// Embedded plans: every view on a caller buffer with its own strides, mapped by embed_pass.  Forward: `in` is the physical
+// side, `out` the output; inverse the other way round.  out_strides apply to d = 3 only: the spectral side of a partial exec
+// stays dense.  The builders, the box reshapes and the kept-axis copies have laid these views out on the dense blocks.
+static int embed_views(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
+    if (!p->embedded()) return DFFT_SUCCESS;
+    const EmbedSide phys = embed_side(p, true);
+    const EmbedSide spec = d == 3 ? embed_side(p, false) : EmbedSide();
+    const EmbedSide& Ein = inverse ? spec : phys;
+    const EmbedSide& Eout = inverse ? phys : spec;
+    for (Step& s : sc.steps) {
+        if (s.type != STEP_PASS) continue;
+        if (s.kernel != KERNEL_PASS) return fail(DFFT_ERR_STATE, "internal: embedded plans run single passes");
+        // points along n of each view, as dfft_debug_run_step counts them
+        const size_t len = s.n ? s.n : size_t(1) << s.log2n;
+        const size_t in_len = s.keep && s.prm.inverse ? s.keep : len + (s.kind == PASS_C2R ? 1 : 0);
+        const size_t out_len = s.keep && !s.prm.inverse ? s.keep : len + (s.kind == PASS_R2C ? 1 : 0);
+        const int rc = embed_pass(s.prm, s.in_user, s.out_user, Ein, Eout, p->esize, in_len, out_len);
+        if (rc) return rc;
+    }
+    return DFFT_SUCCESS;
+}
+
 // The one place that decides which schedule a (direction, d) pair runs — used by exec and by dfft_plan_describe, so
 // the CPU schedule emulation always validates exactly what executes.
 static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
@@ -2360,6 +2489,8 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
         }
         rc = wrap_boxes(p, inverse ? 1 : 0, d, sc);
         if (rc) return rc;
+        rc = embed_views(p, inverse ? 1 : 0, d, sc);
+        if (rc) return rc;
         // No step reads the caller's `out` (views on it are only ever stored to), so every store into it is an output
         // value of the exec: the steps that write `out` are exactly the ones that store final values.  This covers the tail
         // launches of blocked hand-over layouts, every z chunk of overlapped x passes, the last pass of partial transforms
@@ -2396,6 +2527,13 @@ static int exec_common(dfft_plan_t p, void* out, const void* in, int inverse, in
     if (d < 1 || d > 3) return fail(DFFT_ERR_INVALID, "d must be 1, 2 or 3");
     if (!out || !in) return fail(DFFT_ERR_INVALID, "null buffer");
     if (p->inplace && out != in) return fail(DFFT_ERR_INVALID, "in-place plan: out must equal in");
+    {   // embedded sides: the views address whole elements from the caller's pointer (a pair of reals on the real side of
+        // R2C / C2R, which is esize bytes like a complex element)
+        const bool phys = p->in_embedded, spec = d == 3 && p->out_embedded;
+        const bool in_emb = inverse ? spec : phys, out_emb = inverse ? phys : spec;
+        if ((in_emb && (uintptr_t)in % p->esize) || (out_emb && (uintptr_t)out % p->esize))
+            return fail(DFFT_ERR_INVALID, "a buffer with strides (dfft_plan_set_strides) must be aligned to " + std::to_string(p->esize) + " bytes");
+    }
     CK_CUDA(cudaSetDevice(p->comm->device));
     cudaStream_t st = sync ? p->own_stream : (cudaStream_t)stream;
     // A stream capture records the kernels into a graph without running them, so nothing may be set up on the way
@@ -3029,11 +3167,7 @@ int dfft_plan_wait(dfft_plan_t p) {
 static int layout_of(dfft_plan_t p, int which, size_t size[3], size_t start[3]) {
     if (!p) return fail(DFFT_ERR_INVALID, "null plan");
     size_t s[3], o[3];
-    p->g.layout(p->rank, which, s, o);
-    // box plans: this rank's box on a boxed side (the physical side of every d, the output of d = 3)
-    const std::vector<Box>& boxes = which == 0 ? p->in_boxes : p->out_boxes;
-    if ((which == 0 || which == 3) && !boxes.empty())
-        for (int k = 0; k < 3; ++k) { s[k] = boxes[size_t(p->rank)].extent(k); o[k] = boxes[size_t(p->rank)].lo[k]; }
+    caller_block(p, which, s, o);
     for (int k = 0; k < 3; ++k) {
         if (size) size[k] = s[k];
         if (start) start[k] = o[k];
@@ -3087,6 +3221,52 @@ int dfft_plan_set_transform_axes(dfft_plan_t p, const int transform[3]) {
 int dfft_plan_get_transform_axes(dfft_plan_t p, int transform[3]) {
     if (!p || !transform) return fail(DFFT_ERR_INVALID, "null plan / transform");
     for (int a = 0; a < 3; ++a) transform[a] = p->taxes[a];
+    return DFFT_SUCCESS;
+}
+int dfft_plan_set_strides(dfft_plan_t p, const long long in_strides[3], const long long out_strides[3]) {
+    if (!p) return fail(DFFT_ERR_INVALID, "null plan");
+    const char* const names[2] = {"in_strides", "out_strides"};
+    const long long* const given[2] = {in_strides, out_strides};
+    for (int side = 0; side < 2; ++side) {
+        const long long* s = given[side];
+        if (!s) continue;
+        size_t e[3], o[3];
+        caller_block(p, side ? 3 : 0, e, o);
+        // the field, x and y strides may not let two points of the block (or of two fields) share an element
+        const __int128 need[3] = {(__int128)e[0] * s[1], (__int128)e[1] * s[2], (__int128)e[2]};
+        for (int k = 0; k < 3; ++k)
+            if (s[k] < 1 || s[k] < need[k])
+                return fail(DFFT_ERR_INVALID, std::string(names[side]) + ": strides {field, x, y} must be at least {nx * x, ny * y, nz} of this rank's block (" +
+                                                  std::to_string(e[0]) + " x " + std::to_string(e[1]) + " x " + std::to_string(e[2]) + ")");
+        if (side == 0 && p->g.transform == DFFT_R2C && ((s[0] | s[1] | s[2]) & 1))
+            return fail(DFFT_ERR_INVALID, "in_strides: the real side of R2C / C2R moves pairs of reals, so its strides must be even");
+    }
+    if (p->inplace) return fail(DFFT_ERR_UNSUPPORTED, "in-place plans keep the padded layout of FFTW and cuFFT: strides are for out-of-place plans");
+    if (p->comps > 1) return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans keep their [x][y][z][C] layout: strides are for plans of one component");
+    if (p->axes_fixed) return fail(DFFT_ERR_STATE, "set the strides before the first exec, dfft_plan_tune or dfft_plan_describe");
+    p->in_embedded = in_strides != nullptr;
+    p->out_embedded = out_strides != nullptr;
+    for (int k = 0; k < 3; ++k) {
+        p->in_strides[k] = in_strides ? in_strides[k] : 0;
+        p->out_strides[k] = out_strides ? out_strides[k] : 0;
+    }
+    return DFFT_SUCCESS;
+}
+int dfft_plan_get_strides(dfft_plan_t p, long long in_strides[3], long long out_strides[3]) {
+    if (!p) return fail(DFFT_ERR_INVALID, "null plan");
+    for (int side = 0; side < 2; ++side) {
+        long long* s = side ? out_strides : in_strides;
+        if (!s) continue;
+        if (side ? p->out_embedded : p->in_embedded) {
+            for (int k = 0; k < 3; ++k) s[k] = side ? p->out_strides[k] : p->in_strides[k];
+            continue;
+        }
+        size_t e[3], o[3];  // a dense side: the strides of its dense block
+        caller_block(p, side ? 3 : 0, e, o);
+        s[2] = (long long)e[2];
+        s[1] = (long long)(e[1] * e[2]);
+        s[0] = (long long)(e[0] * e[1] * e[2]);
+    }
     return DFFT_SUCCESS;
 }
 #ifdef DFFT_ZY_TRACE
@@ -3241,6 +3421,7 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
                          : p->g.padded()        ? "sequential schedule (no alternatives for this plan: padded plans run the sequential schedule)"
                          : p->comps > 1         ? "sequential schedule (no alternatives for this plan: interleaved plans run the sequential schedule)"
                          : p->boxed()           ? "sequential schedule (no alternatives for this plan: box plans run the sequential schedule)"
+                         : p->embedded()        ? "sequential schedule (no alternatives for this plan: plans with strides run the sequential schedule)"
                          : pow2_axes(p)         ? "sequential schedule (no alternatives for this plan)"
                                                 : "sequential schedule (no alternatives for this plan: an axis length is not a power of two)";
         return 0;
@@ -3357,6 +3538,11 @@ static std::string json_boxes(const char* name, const std::vector<Box>& boxes) {
     }
     return o + "]";
 }
+// ,"name":[field,x,y] of a side with strides (dfft_plan_set_strides); nothing for a dense side
+static std::string json_strides(const char* name, bool on, const long long s[3]) {
+    if (!on) return std::string();
+    return std::string(",\"") + name + "\":[" + std::to_string(s[0]) + "," + std::to_string(s[1]) + "," + std::to_string(s[2]) + "]";
+}
 int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capacity, size_t* needed) {
     if (!p || d < 1 || d > 3) return fail(DFFT_ERR_INVALID, "bad arguments");
     Schedule* scp = nullptr;
@@ -3380,6 +3566,7 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
                                    : std::string()) +
                     (p->comps > 1 ? ",\"components\":" + std::to_string(p->comps) : std::string()) +
                     json_boxes("in_boxes", p->in_boxes) + json_boxes("out_boxes", p->out_boxes) +
+                    json_strides("in_strides", p->in_embedded, p->in_strides) + json_strides("out_strides", p->out_embedded, p->out_strides) +
                     (p->batch > 1 ? ",\"batch\":" + std::to_string(p->batch) + ",\"field_in\":" + std::to_string(sc.field_in) +
                                         ",\"field_out\":" + std::to_string(sc.field_out)
                                   : std::string()) +

@@ -37,6 +37,22 @@ def _ptr(buf) -> int:
     raise TypeError(f"unsupported buffer type {type(buf)}")
 
 
+def _strided_ptr(buf, block, strides, batch) -> int:
+    """_ptr of a buffer on a side with strides (dfft_plan_set_strides): a tensor of the block's shape ([batch, X, Y, Z] when
+    batched) whose strides are the declared {field, x, y} and 1 along z; dimensions of extent 1 may have any stride"""
+    if buf is None or isinstance(buf, int) or not hasattr(buf, "data_ptr"):
+        return _ptr(buf)
+    shape = (tuple(block) if batch == 1 else (batch, *block))
+    want = (tuple(strides[1:]) + (1,)) if batch == 1 else (tuple(strides) + (1,))
+    if tuple(buf.shape) != shape:
+        raise ValueError(f"a buffer with strides must have the block's shape {shape}, got {tuple(buf.shape)}")
+    if any(n > 1 and s != w for n, s, w in zip(buf.shape, buf.stride(), want)):
+        raise ValueError(f"buffer strides {tuple(buf.stride())} differ from the plan's {want}")
+    if hasattr(buf, "is_cuda") and not buf.is_cuda:
+        raise ValueError("buffers must live in CUDA device memory (use HostExecutor for host buffers)")
+    return int(buf.data_ptr())
+
+
 def _stream_ptr(stream) -> int:
     if stream is None:
         return 0
@@ -131,7 +147,7 @@ class MPIcuFFT:
     # -- plan ------------------------------------------------------------------------------------
     def initFFT(self, global_size: GlobalSize, partition: Optional[Partition] = None, allocate: bool = True, batch: int = 1,
                 inplace: bool = False, transform_axes: Optional[Sequence[bool]] = None, spectral: Optional[Sequence[int]] = None,
-                components: int = 1, in_boxes=None, out_boxes=None):
+                components: int = 1, in_boxes=None, out_boxes=None, in_strides=None, out_strides=None):
         """`batch` (not in the reference): every exec transforms that many fields, back to back in each buffer — a
         contiguous [batch, X, Y, Z] tensor; the getters describe one field (dfft_plan_create_batched).
         `inplace` (dfft_plan_create_inplace): every exec gets the same buffer twice and overwrites its input; fields are
@@ -146,7 +162,11 @@ class MPIcuFFT:
         `in_boxes` / `out_boxes` (dfft_plan_create_boxes): one box ((lx, ly, lz), (hx, hy, hz)) per rank, in rank order, of the
         physical grid and of the output grid (z extent Nz/2 + 1 for R2C); each rank's buffer on that side is its box, a dense
         [hx-lx, hy-ly, hz-lz] tensor, and the exec redistributes on the GPU.  None keeps the natural layout.  Box plans are
-        out of place, not padded, with one component and one transform for all axes."""
+        out of place, not padded, with one component and one transform for all axes.
+        `in_strides` / `out_strides` (field, x, y) (dfft_plan_set_strides): the buffers of the physical side / of the output
+        of d = 3 lie inside larger arrays, e.g. the interior A[h:-h, h:-h, h:-h] of a field with ghost cells, whose strides
+        these are (torch's .stride(), in elements: reals on the real side of R2C / C2R and for R2R plans); such a side then
+        takes exactly those non-contiguous tensors.  None keeps a side dense."""
         if global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         cfg = _lib.dfft_config(int(self.config.cuda_aware), int(self.config.warmup_rounds), int(self.config.comm_method),
@@ -215,13 +235,48 @@ class MPIcuFFT:
         self._h = h
         self.global_size = global_size
         self.initialized = True
-        if transform_axes is not None:
-            try:
+        self._strides = (None, None)
+        try:
+            if in_strides is not None or out_strides is not None:
+                self.setStrides(in_strides, out_strides)
+            if transform_axes is not None:
                 self.setTransformAxes(*transform_axes)
-            except Exception:
-                self.destroy()
-                self.initialized = False
-                raise
+        except Exception:
+            self.destroy()
+            self.initialized = False
+            raise
+
+    def setStrides(self, in_strides=None, out_strides=None):
+        """{field, x, y} strides of the caller's arrays on the physical side (in) and on the output of d = 3 (out), z
+        contiguous (dfft_plan_set_strides).  Only before the first exec, tune or describe; every rank calls it with its own
+        values, or none does."""
+        self._need()
+
+        def arr(s):
+            return None if s is None else (C.c_longlong * 3)(*(int(v) for v in s))
+        check(lib().dfft_plan_set_strides(self._h, arr(in_strides), arr(out_strides)))
+        self._strides = (None if in_strides is None else tuple(int(v) for v in in_strides),
+                         None if out_strides is None else tuple(int(v) for v in out_strides))
+
+    def getStrides(self):
+        """((field, x, y) of the physical side, (field, x, y) of the output), the dense ones for a side without strides"""
+        self._need()
+        i, o = (C.c_longlong * 3)(), (C.c_longlong * 3)()
+        check(lib().dfft_plan_get_strides(self._h, i, o))
+        return tuple(i), tuple(o)
+
+    def _bufs(self, out, in_, physical_in: bool, d: int):
+        """(out, in) pointers of an exec; physical_in: `in_` is the physical side (forward), else `out` is"""
+        phys, spec = getattr(self, "_strides", (None, None))
+        spec = spec if d == 3 else None
+        batch = self.getBatch() if phys is not None or spec is not None else 1
+
+        def one(buf, physical):
+            s = phys if physical else spec
+            if s is None:
+                return _ptr(buf)
+            return _strided_ptr(buf, self.getInSize() if physical else self.getOutSize(), s, batch)
+        return one(out, not physical_in), one(in_, physical_in)
 
     def setTransformAxes(self, x: bool = True, y: bool = True, z: bool = True):
         """Transform (True) or keep (False) each axis (dfft_plan_set_transform_axes).  A kept axis is redistributed as a
@@ -259,10 +314,10 @@ class MPIcuFFT:
         if stream is not None:
             if d != 3:
                 raise ValueError("async partial transforms are not exposed")
-            return check(lib().dfft_exec_r2c_async(self._h, _ptr(out), _ptr(in_), _stream_ptr(stream)))
+            return check(lib().dfft_exec_r2c_async(self._h, *self._bufs(out, in_, True, 3), _stream_ptr(stream)))
         if d == 3:
-            return check(lib().dfft_exec_r2c(self._h, _ptr(out), _ptr(in_)))
-        return check(lib().dfft_exec_r2c_partial(self._h, _ptr(out), _ptr(in_), d))
+            return check(lib().dfft_exec_r2c(self._h, *self._bufs(out, in_, True, 3)))
+        return check(lib().dfft_exec_r2c_partial(self._h, *self._bufs(out, in_, True, d), d))
 
     def execC2R(self, out, in_, d: int = 3, stream=None):
         """Complex-to-real transform; `stream` as for execR2C, capturable the same way."""
@@ -270,10 +325,10 @@ class MPIcuFFT:
         if stream is not None:
             if d != 3:
                 raise ValueError("async partial transforms are not exposed")
-            return check(lib().dfft_exec_c2r_async(self._h, _ptr(out), _ptr(in_), _stream_ptr(stream)))
+            return check(lib().dfft_exec_c2r_async(self._h, *self._bufs(out, in_, False, 3), _stream_ptr(stream)))
         if d == 3:
-            return check(lib().dfft_exec_c2r(self._h, _ptr(out), _ptr(in_)))
-        return check(lib().dfft_exec_c2r_partial(self._h, _ptr(out), _ptr(in_), d))
+            return check(lib().dfft_exec_c2r(self._h, *self._bufs(out, in_, False, 3)))
+        return check(lib().dfft_exec_c2r_partial(self._h, *self._bufs(out, in_, False, d), d))
 
     def execC2C(self, out, in_, direction: int = FORWARD, d: int = 3, stream=None):
         """Complex transform (not in the reference; BASELINE configs 1-4 need it).  `stream` as for execR2C, capturable
@@ -282,10 +337,10 @@ class MPIcuFFT:
         if stream is not None:
             if d != 3:
                 raise ValueError("async partial transforms are not exposed")
-            return check(lib().dfft_exec_c2c_async(self._h, _ptr(out), _ptr(in_), direction, _stream_ptr(stream)))
+            return check(lib().dfft_exec_c2c_async(self._h, *self._bufs(out, in_, direction <= 0, 3), direction, _stream_ptr(stream)))
         if d == 3:
-            return check(lib().dfft_exec_c2c(self._h, _ptr(out), _ptr(in_), direction))
-        return check(lib().dfft_exec_c2c_partial(self._h, _ptr(out), _ptr(in_), direction, d))
+            return check(lib().dfft_exec_c2c(self._h, *self._bufs(out, in_, direction <= 0, 3), direction))
+        return check(lib().dfft_exec_c2c_partial(self._h, *self._bufs(out, in_, direction <= 0, d), direction, d))
 
     def execR2R(self, out, in_, direction: int = FORWARD, d: int = 3, stream=None):
         """Real-to-real transform of a 'dct' / 'dst' or per-axis plan (not in the reference): FORWARD is type II (R2HC on
@@ -296,10 +351,10 @@ class MPIcuFFT:
         if stream is not None:
             if d != 3:
                 raise ValueError("async partial transforms are not exposed")
-            return check(lib().dfft_exec_r2r_async(self._h, _ptr(out), _ptr(in_), direction, _stream_ptr(stream)))
+            return check(lib().dfft_exec_r2r_async(self._h, *self._bufs(out, in_, direction <= 0, 3), direction, _stream_ptr(stream)))
         if d == 3:
-            return check(lib().dfft_exec_r2r(self._h, _ptr(out), _ptr(in_), direction))
-        return check(lib().dfft_exec_r2r_partial(self._h, _ptr(out), _ptr(in_), direction, d))
+            return check(lib().dfft_exec_r2r(self._h, *self._bufs(out, in_, direction <= 0, 3), direction))
+        return check(lib().dfft_exec_r2r_partial(self._h, *self._bufs(out, in_, direction <= 0, d), direction, d))
 
     def getR2RKinds(self):
         """(x, y, z) kinds of a real-to-real plan: DCT, DST, R2HC, DCT1, DST1, DCT4 or DST4 each (dfft_plan_get_r2r_kinds)."""
@@ -315,7 +370,7 @@ class MPIcuFFT:
         """Plan-time measurement: try the sequential and the overlapped schedules on these buffers and keep the fastest
         (collective).  Returns the report string."""
         self._need()
-        check(lib().dfft_plan_tune(self._h, _ptr(out), _ptr(in_), 1 if direction > 0 else 0, reps))
+        check(lib().dfft_plan_tune(self._h, *self._bufs(out, in_, direction <= 0, 3), 1 if direction > 0 else 0, reps))
         return (lib().dfft_plan_tune_report(self._h) or b"").decode()
 
     # -- getters ---------------------------------------------------------------------------------
@@ -404,13 +459,14 @@ class MPIcuFFT_Pencil(MPIcuFFT):
     _decomp = PENCIL
 
     def initFFT(self, global_size, partition=None, allocate=True, batch=1, inplace=False, transform_axes=None, spectral=None, components=1,
-                in_boxes=None, out_boxes=None):
+                in_boxes=None, out_boxes=None, in_strides=None, out_strides=None):
         if partition is None or global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         if partition.P1 * partition.P2 != self.comm.size:
             raise RuntimeError("Invalid Input Partition!")
         self.partition = partition
-        super().initFFT(global_size, partition, allocate, batch, inplace, transform_axes, spectral, components, in_boxes, out_boxes)
+        super().initFFT(global_size, partition, allocate, batch, inplace, transform_axes, spectral, components, in_boxes, out_boxes, in_strides,
+                        out_strides)
 
     def getPartitionDimensions(self):
         """(input_dim, transposed_dim, output_dim), each a dict with size_x/y/z and start_x/y/z lists

@@ -358,6 +358,30 @@ int dfft_plan_get_scale(dfft_plan_t plan, double* forward_scale, double* inverse
  * creation.  Local to the calling rank: set the same values on every rank. */
 int dfft_plan_set_transform_axes(dfft_plan_t plan, const int transform[3]);
 int dfft_plan_get_transform_axes(dfft_plan_t plan, int transform[3]);
+/* Embedded layouts (not in the reference; cuFFT's inembed / istride / idist, FFTW's advanced interface): each rank's block
+ * of a side is read or written inside a larger caller array, e.g. the interior of a field with ghost cells or a torch
+ * slice A[h:-h, h:-h, h:-h], with no pack or unpack around the exec.
+ *   - in_strides / out_strides: {field, x, y} strides of that side's caller array, in its elements (complex values on
+ *     complex sides; reals on the real side of R2C / C2R and on every side of R2R plans); z is contiguous.  NULL keeps that
+ *     side dense.  The caller passes a pointer to the block's first element, as torch's data_ptr() of a slice is.
+ *   - `in` is the physical side: the forward input and the inverse output, partial d included.  `out` is the output of
+ *     d = 3 (the forward output, the inverse input); the spectral side of a partial exec stays dense, as for boxes.
+ *   - The block is this rank's dfft_get_in_size / dfft_get_out_size (its box on box plans).  Strides must keep its points
+ *     apart: y >= the block's z extent, x >= ny * y, field >= nx * x, and every stride even on the real side of R2C / C2R
+ *     (its rows move as pairs of reals); otherwise DFFT_ERR_INVALID.  At exec, a pointer on an embedded side that is not
+ *     aligned to its element (a pair of reals on the real side of R2C / C2R) returns DFFT_ERR_INVALID.
+ *   - The FFT passes read and write the caller's array through the strides: the first pass reads it, the last one writes
+ *     it, and no element outside the block is touched.  Such plans run the sequential schedule (no overlapped schedule,
+ *     fused z + y stage or one-launch batched stage; dfft_plan_tune has one candidate).  Every rank calls this, or none
+ *     does; each with its own values, since the caller's buffers are local.
+ *   - C2C (Bluestein lengths included), R2C / C2R and every R2R kind on every decomposition, with batches, scale, partial
+ *     d, kept axes, padded plans and box plans (the box is the block).  dfft_plan_describe reports "in_strides" /
+ *     "out_strides".  In-place and interleaved plans: DFFT_ERR_UNSUPPORTED.  Once the plan has built a schedule:
+ *     DFFT_ERR_STATE, as for dfft_plan_set_transform_axes.
+ * dfft_plan_get_strides reports the strides of each side, those of the dense block for a side without them; either
+ * pointer may be NULL. */
+int dfft_plan_set_strides(dfft_plan_t plan, const long long in_strides[3], const long long out_strides[3]);
+int dfft_plan_get_strides(dfft_plan_t plan, long long in_strides[3], long long out_strides[3]);
 /* Waits for the stream of the last eager _async call and reports a device-side failure (rendezvous or fused-stage
  * timeout), if any.  After replaying a graph, synchronise the replay stream first; dfft_plan_wait then reports the
  * errors the replayed kernels recorded. */

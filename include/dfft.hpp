@@ -138,6 +138,10 @@ public:
         const int t[3] = {x ? 1 : 0, y ? 1 : 0, z ? 1 : 0};
         DFFT_CALL(dfft_plan_set_transform_axes(plan, t));
     }
+    // not in the reference: {field, x, y} strides of the caller's arrays on the physical side (in) and the output of d = 3
+    // (out), in that side's elements, z contiguous (dfft_plan_set_strides; after initFFT, before the first exec).  Null keeps
+    // a side dense; the exec takes a pointer to each block's first element.
+    void setStrides(const long long in[3], const long long out[3]) { DFFT_CALL(dfft_plan_set_strides(plan, in, out)); }
     virtual void setWorkArea(void* device = nullptr, void* host = nullptr) { DFFT_CALL(dfft_set_work_area(plan, device, host)); }
     virtual void execR2C(void* out, const void* in) = 0;
     // not in the reference: real-to-real transform of a plan constructed with transform_ = DFFT_DCT or DFFT_DST, or with
