@@ -8,9 +8,10 @@ output block of every field.  On the way it checks what the step lists promise a
 each wherever it applies:
   - happens-before (Ordering): every read-after-write and write-after-read is ordered by a stream, an event or a rendezvous;
   - every rank lists as many steps, and both ends of an all-to-all agree on its counts;
-  - slots: a pass reads only its own rank's slots, stores into a peer's slot only after its entry rendezvous, and reads a
-    slot a peer stored into only after a later rendezvous;
+  - slots: a pass reads only its own rank's slots (the "reshape out" gathers of box plans read their peers'), stores into a
+    peer's slot only after its entry rendezvous, and reads a slot a peer stored into only after a later rendezvous;
   - out of place, the caller's input is left intact;
+  - on a side with strides, the ghost elements around each block (poisoned) are neither read nor stored into;
   - a per-field step stays inside its field of the caller's buffers; with a scale, every output value is scaled exactly
     once, and only by stores into the caller's output;
   - a step that stores into an array it also reads stores every element from the line that reads it, or one that no other
@@ -24,6 +25,7 @@ from __future__ import annotations
 
 import ctypes as C
 import json
+from contextlib import contextmanager
 from dataclasses import dataclass
 
 import numpy as np
@@ -36,14 +38,21 @@ from oracle import dft_oracle as O
 
 USER_IN, USER_OUT = 1 << 60, 1 << 61  # synthetic address ranges of the caller's buffers (rank r: + r << 48)
 PAD = 1234.5 - 678.25j  # value of the padding of the real rows of in-place R2C / C2R plans
+POISON = -3.25e300 + 7.5e299j  # every ghost element of a caller array with strides
 
 
 # ---- plans ----------------------------------------------------------------------------------------------------------------
 @dataclass(frozen=True)
 class Plan:
-    """Everything a replayed plan can have.  The creator follows the fields: spectral -> dfft_plan_create_padded,
-    components -> dfft_plan_create_interleaved, kinds -> dfft_plan_create_r2r, inplace -> dfft_plan_create_inplace, a batch
-    -> dfft_plan_create_batched, else dfft_plan_create.  axes and scale go through their setters."""
+    """Everything a replayed plan can have.  The creator follows the fields: boxes -> dfft_plan_create_boxes, spectral ->
+    dfft_plan_create_padded, components -> dfft_plan_create_interleaved, kinds -> dfft_plan_create_r2r, inplace ->
+    dfft_plan_create_inplace, a batch -> dfft_plan_create_batched, else dfft_plan_create.  embed, axes and scale go through
+    their setters.
+
+    in_boxes / out_boxes: one ((lx, ly, lz), (hx, hy, hz)) per rank of the physical and the output grid; None keeps that
+    side's natural layout.  embed ("in", "out" or "both": the physical side, the output of d = 3) puts each rank's block of
+    those sides inside a larger caller array: `halo` ghost layers around it, `gap` more elements between fields (both in the
+    side's elements; even on the real side of R2C / C2R, whose pairs of reals must stay aligned)."""
     P: int
     decomp: int
     shape: tuple
@@ -60,20 +69,42 @@ class Plan:
     components: int | None = None
     axes: tuple | None = None
     scale: tuple | None = None
+    in_boxes: tuple | None = None
+    out_boxes: tuple | None = None
+    embed: str | None = None
+    halo: int = 2
+    gap: int = 0
 
     @property
     def fields(self):
         return 1 if self.batch is None else self.batch
 
 
-def create(p, rank):
-    """rank's dry plan of p, before the setters: (rc, message, comm, plan)"""
-    c = C.c_void_p()
-    check(lib().dfft_comm_create_dry(rank, p.P, C.byref(c)))
+def _flat(boxes):
+    return None if boxes is None else (C.c_size_t * (6 * len(boxes)))(*[v for lo, hi in boxes for v in (*lo, *hi)])
+
+
+def strides(size, halo, gap):
+    """{field, x, y} of a block of `size` inside its ghost layers"""
+    y = size[2] + 2 * halo
+    x = (size[1] + 2 * halo) * y
+    return (size[0] + 2 * halo) * x + gap, x, y
+
+
+def create(p, rank, comm=None):
+    """rank's plan of p on comm (a geometry-only communicator when None) with its strides, before the other setters:
+    (rc, message, comm, plan)"""
+    c = comm
+    if c is None:
+        c = C.c_void_p()
+        check(lib().dfft_comm_create_dry(rank, p.P, C.byref(c)))
     cfg = C.byref(_lib.dfft_config(1, 0, p.comm, p.send, None, p.comm, p.send))
     plan = C.c_void_p()
     head = (c, cfg, p.decomp, p.prec)
-    if p.spectral is not None:
+    if p.in_boxes is not None or p.out_boxes is not None:
+        rc = lib().dfft_plan_create_boxes(*head, p.transform, *p.shape, p.p1, p.p2, _flat(p.in_boxes), _flat(p.out_boxes), p.fields, 1,
+                                          C.byref(plan))
+    elif p.spectral is not None:
         rc = lib().dfft_plan_create_padded(*head, p.transform, *p.shape, *p.spectral, p.p1, p.p2, p.fields, 1, C.byref(plan))
     elif p.components is not None:
         rc = lib().dfft_plan_create_interleaved(*head, p.transform, *p.shape, p.p1, p.p2, p.components, p.fields, 1, C.byref(plan))
@@ -85,6 +116,13 @@ def create(p, rank):
         rc = lib().dfft_plan_create_batched(*head, p.transform, *p.shape, p.p1, p.p2, p.batch, 1, C.byref(plan))
     else:
         rc = lib().dfft_plan_create(*head, p.transform, *p.shape, p.p1, p.p2, 1, C.byref(plan))
+    if rc == 0 and p.embed:
+        sides = []
+        for fn, name in ((lib().dfft_get_in_size, "in"), (lib().dfft_get_out_size, "out")):
+            s = (C.c_size_t * 3)()
+            check(fn(plan, s))
+            sides.append((C.c_longlong * 3)(*strides(list(s), p.halo, p.gap)) if p.embed in (name, "both") else None)
+        rc = lib().dfft_plan_set_strides(plan, *sides)
     return rc, (lib().dfft_last_error_string() or b"").decode(), c, plan
 
 
@@ -109,35 +147,53 @@ def describe_raw(plan, inverse, d):
     return buf.value.decode()
 
 
-def _with_plan(p, rank, fn):
-    rc, msg, c, plan = create(p, rank)
-    assert rc == 0, msg
+def set_options(p, plan):
+    """the setters that follow the creator: transform axes and scale"""
+    if p.axes is not None:
+        check(lib().dfft_plan_set_transform_axes(plan, (C.c_int * 3)(*p.axes)))
+    if p.scale is not None:
+        check(lib().dfft_plan_set_scale(plan, *p.scale))
+
+
+@contextmanager
+def dry_plans(p, ranks=None):
+    """the dry plans of p's ranks (all of them when None) with every setter applied: a list of plan handles, destroyed on
+    exit"""
+    made = []
     try:
-        if p.axes is not None:
-            check(lib().dfft_plan_set_transform_axes(plan, (C.c_int * 3)(*p.axes)))
-        if p.scale is not None:
-            check(lib().dfft_plan_set_scale(plan, *p.scale))
-        return fn(plan)
+        for r in range(p.P) if ranks is None else ranks:
+            rc, msg, c, plan = create(p, r)
+            made.append((c, plan))
+            assert rc == 0, msg
+            set_options(p, plan)
+        yield [plan for _, plan in made]
     finally:
-        lib().dfft_plan_destroy(plan)
-        lib().dfft_comm_destroy(c)
+        for c, plan in made:
+            lib().dfft_plan_destroy(plan)
+            lib().dfft_comm_destroy(c)
+
+
+def schedule(p, plan, inverse, d):
+    """the parsed step list of an open plan, with "domain_bytes", "work_bytes" and "layouts" ([(size, start)] of layouts
+    0..3)"""
+    assert lib().dfft_get_batch(plan) == p.fields and lib().dfft_get_components(plan) == (p.components or 1)
+    sc = json.loads(describe_raw(plan, inverse, d))
+    sc["domain_bytes"] = lib().dfft_get_domain_size(plan)
+    sc["work_bytes"] = lib().dfft_get_work_size_device(plan)
+    sc["layouts"] = layouts(plan)
+    return sc
 
 
 def describe_text(p, rank, inverse, d):
     """rank's step list as dfft_plan_describe writes it"""
-    return _with_plan(p, rank, lambda plan: describe_raw(plan, inverse, d))
+    with dry_plans(p, [rank]) as (plan,):
+        return describe_raw(plan, inverse, d)
 
 
 def describe(p, rank, inverse, d):
-    """rank's parsed step list, with "domain_bytes", "work_bytes" and "layouts" ([(size, start)] of layouts 0..3)"""
-    def parse(plan):
-        assert lib().dfft_get_batch(plan) == p.fields and lib().dfft_get_components(plan) == (p.components or 1)
-        sc = json.loads(describe_raw(plan, inverse, d))
-        sc["domain_bytes"] = lib().dfft_get_domain_size(plan)
-        sc["work_bytes"] = lib().dfft_get_work_size_device(plan)
-        sc["layouts"] = layouts(plan)
-        return sc
-    return _with_plan(p, rank, parse)
+    """rank's parsed step list (see schedule)"""
+    with dry_plans(p, [rank]) as (plan,):
+        return schedule(p, plan, inverse, d)
 
 
 # ---- per-pass math --------------------------------------------------------------------------------------------------------
@@ -363,7 +419,9 @@ def _phase_check(r, k, acc):
 
 # ---- the caller's buffers -------------------------------------------------------------------------------------------------
 class Side:
-    """one rank's caller buffer on one side (in / out) of an exec: where field f's block of layout `which` lies"""
+    """one rank's caller buffer on one side (in / out) of an exec: where field f's block of layout `which` lies.  On a side
+    with strides (in_strides / out_strides of the describe, in the side's elements: reals on the real side of R2C / C2R)
+    the block lies inside ghost layers: field f's block starts `lead` elements into the buffer, behind those of field 0."""
 
     def __init__(self, p, sc, which, pairs, es):
         self.size, self.start = sc["layouts"][which]
@@ -375,9 +433,20 @@ class Side:
         self.row = self.nz // 2 + 1 if self.padded else self.nz * comps // (2 if pairs else 1)
         self.elems = self.size[0] * self.size[1] * self.row
         self.field = sc["domain_bytes"] // es if p.inplace else self.elems
+        self.sx, self.sy, self.lead = self.size[1] * self.row, self.row, 0
+        st = sc.get("in_strides") if which == 0 else sc.get("out_strides") if which == 3 else None
+        self.strided = st is not None
+        if self.strided:
+            unit = 2 if pairs else 1  # the buffer counts pairs of reals on the real side of R2C / C2R
+            assert all(v % unit == 0 for v in st) and p.halo * (st[1] + st[2] + 1) % unit == 0, (st, p.halo)
+            self.field, self.sx, self.sy = (v // unit for v in st)
+            self.lead = p.halo * (st[1] + st[2] + 1) // unit
+        self.total = max(p.fields * self.field, 1)  # elements of the buffer
 
     def rows(self, f):
-        return f * self.field + np.arange(self.elems).reshape(-1, max(self.row, 1))
+        n0, n1, _ = self.size
+        i = (np.arange(n0)[:, None] * self.sx + np.arange(n1)[None, :] * self.sy).reshape(-1, 1) + np.arange(self.row)
+        return self.lead + f * self.field + i
 
     def index(self, f):
         """flat buffer indices of field f's block (the padding of real rows excluded)"""
@@ -385,14 +454,34 @@ class Side:
         return (i[:, :self.nz // 2] if self.padded else i).ravel()
 
     def put(self, buf, f, block):
-        v = np.ascontiguousarray(block, dtype=np.float64 if self.pairs else buf.dtype).ravel()
-        buf[self.index(f)] = v.view(np.complex128) if self.pairs else v
-        if self.padded:
-            buf[self.rows(f)[:, self.nz // 2:].ravel()] = PAD
+        v = np.ascontiguousarray(block, dtype=buf.real.dtype if self.pairs else buf.dtype).ravel()
+        buf[self.index(f)] = v.view(buf.dtype)
 
     def get(self, buf, f):
         v = buf[self.index(f)]
-        return (v.view(np.float64) if self.pairs else v).reshape(self.shape)
+        return (v.view(v.real.dtype) if self.pairs else v).reshape(self.shape)
+
+
+def sides(p, sc, inverse, d, es):
+    """(input side, output side) of the rank whose step list is sc"""
+    r2c = p.transform == dfft.R2C and p.kinds is None
+    src_w, dst_w = (d, 0) if inverse else (0, d)
+    return Side(p, sc, src_w, r2c and not inverse, es), Side(p, sc, dst_w, r2c and bool(inverse), es)
+
+
+def block(a, start, size):
+    return a[start[0]:start[0] + size[0], start[1]:start[1] + size[1], start[2]:start[2] + size[2]]
+
+
+def assemble(outs):
+    """the global output (field, ...) from [field][rank] (start of the output block, output block)"""
+    blocks = outs[0]
+    shape = tuple(max(s[a] + b.shape[a] for s, b in blocks) for a in range(3)) + blocks[0][1].shape[3:]
+    g = np.zeros((len(outs),) + shape, dtype=blocks[0][1].dtype)
+    for f, blocks in enumerate(outs):
+        for s, b in blocks:
+            block(g[f], s, b.shape)[...] = b
+    return g
 
 
 # ---- the engine -----------------------------------------------------------------------------------------------------------
@@ -401,7 +490,9 @@ def replay(p, inverse, d, x, scheds=None, mutate=None):
     that breaks them on purpose, for negative tests) in lock step on x, the global input of the direction: [field][x, y, z]
     (+ [c] for interleaved plans), real on the real side of R2C plans and for R2R plans.  Returns [field][rank] (start of the
     output block, output block)."""
-    scheds = scheds or [describe(p, r, inverse, d) for r in range(p.P)]
+    if scheds is None:
+        with dry_plans(p) as plans:
+            scheds = [schedule(p, plan, inverse, d) for plan in plans]
     if mutate:
         mutate(scheds)
     return _Replay(p, scheds, inverse, d).run(x)
@@ -430,20 +521,27 @@ class _Replay:
             assert sc.get("inplace", False) == p.inplace
             for s in range(sc["nslots"]):
                 self.owner[id(self.mem.add(sc["slots"][s][r], sc["slot_bytes"] // es))] = (r, s)
-        src_w, dst_w = (d, 0) if inverse else (0, d)
-        self.sides, self.bufs, self.pads = [], [], []
+        self.poison = POISON.real if self.real else POISON
+        self.sides, self.bufs, self.pads, self.masks = [], [], [], []
         for r, sc in enumerate(scheds):
-            i = Side(p, sc, src_w, self.r2c and not inverse, es)
-            o = Side(p, sc, dst_w, self.r2c and bool(inverse), es)
+            i, o = sides(p, sc, inverse, d, es)
             if "field_in" in sc:
                 assert (sc["field_in"], sc["field_out"]) == (i.field * es, o.field * es), (sc["field_in"], sc["field_out"], i.field, o.field)
             if p.inplace:
                 assert i.field >= max(i.elems, o.elems) and o.field == i.field
-                one = self.mem.add(USER_IN + (r << 48), max(p.fields * i.field, 1))
+                one = self.mem.add(USER_IN + (r << 48), i.total)
                 bufs = {1: one, 2: one}
-            else:
-                bufs = {1: self.mem.add(USER_IN + (r << 48), max(p.fields * i.field, 1)),
-                        2: self.mem.add(USER_OUT + (r << 48), max(p.fields * o.field, 1))}
+            else:  # a buffer with strides starts `lead` elements before the address the passes take
+                bufs = {1: self.mem.add(USER_IN + (r << 48) - i.lead * es, i.total),
+                        2: self.mem.add(USER_OUT + (r << 48) - o.lead * es, o.total)}
+            masks = {}  # caller buffers with strides: True on the blocks, poison on every ghost element
+            for user, side in ((1, i), (2, o)):
+                if side.strided:
+                    masks[user] = np.zeros(bufs[user].size, dtype=bool)
+                    for f in range(p.fields):
+                        masks[user][side.index(f)] = True
+                    bufs[user][~masks[user]] = self.poison
+            self.masks.append(masks)
             pad = None
             if i.padded or o.padded:  # in place: the real rows' padding, never read (forward) or stored by C2R (inverse)
                 pad = np.zeros(bufs[1].size, dtype=bool)
@@ -464,6 +562,8 @@ class _Replay:
             for f in range(p.fields):
                 (s0, s1, s2), (n0, n1, n2) = i.start, i.size
                 i.put(self.bufs[r][1], f, x[f][s0:s0 + n0, s1:s1 + n1, s2:s2 + n2])
+            if self.pads[r] is not None and not self.inverse:
+                self.bufs[r][1][self.pads[r]] = PAD
         inputs = [self.bufs[r][1].copy() for r in range(P)]
         nsteps = len(scheds[0]["steps"])
         assert all(len(sc["steps"]) == nsteps for sc in scheds), [len(sc["steps"]) for sc in scheds]
@@ -490,6 +590,8 @@ class _Replay:
                 assert np.array_equal(self.bufs[r][1], inputs[r]), f"rank {r}: the input was modified"
             if self.pads[r] is not None and not self.inverse:
                 assert (self.bufs[r][1][self.pads[r]] == PAD).all(), f"rank {r}: the padding of a real row was stored into"
+            for user, mask in self.masks[r].items():
+                assert (self.bufs[r][user][~mask] == self.poison).all(), f"rank {r}: a ghost element of caller buffer {user} changed"
             o = self.sides[r][2]
             for f in range(p.fields):
                 outs[f].append((o.start, o.get(self.bufs[r][2], f)))
@@ -519,6 +621,7 @@ class _Replay:
         (the real side of kinds 9 / 10) indexes the float64 view of its complex array"""
         user = st[which + "_user"]
         ub = {1: USER_IN, 2: USER_IN if self.p.inplace else USER_OUT}[user] + (r << 48) if user else None
+        mask = self.masks[r].get(user) if user else None
         out = []
         for base, ns, off in view_indices(st[which], st["A0"], st["A1"], n, b, ub):
             if off.size == 0:  # empty tail passes of ranks without leftover columns
@@ -526,11 +629,15 @@ class _Replay:
             arr, o = self.mem.resolve(base)
             tgt, idx = (arr.view(np.float64), 2 * o + off) if real else (arr, o + off)
             cidx = idx // 2 if real else idx
+            if mask is not None:
+                bad = ~mask[cidx]
+                assert not bad.any(), (f"rank {r} step {k} ({st['label']}) {'reads' if which == 'in' else 'stores into'} "
+                                       f"{int(bad.sum())} ghost elements of caller buffer {user}")
             if not user:
                 own = self.owner.get(id(arr))
                 assert own is not None, f"rank {r} step {k} ({st['label']}): a slot view outside the slots"
-                if which == "in":
-                    assert own[0] == r, "passes only read local memory"
+                if which == "in":  # the gathers of box plans' output reshape read their peers' slots
+                    assert own[0] == r or st["label"] == "reshape out", "passes other than the output gathers read only local memory"
                     w = self.last_remote_write.get(own, -1)
                     assert w < 0 or w < self.last_rdv[r] <= k, f"rank {r} step {k} reads slot {own} written remotely at step {w} without a rendezvous"
                 elif own[0] != r:
@@ -553,6 +660,10 @@ class _Replay:
     def check_kind(self, r, k, st, N):
         kind, p = st["kind"], self.p
         where = f"rank {r} step {k} ({st['label']}, kind {kind})"
+        if kind == 6 and st["label"].startswith("reshape"):  # box plans: the copies between the boxes and the natural layouts
+            assert p.in_boxes is not None or p.out_boxes is not None, where
+            assert "n" in st and st["log2n"] == 0 and "r2r" not in st and st["B"] == 1, where
+            return
         assert kind in PASSES, f"{where}: unknown pass kind"
         assert (kind in (4, 5, 6, 7)) if self.real else (kind not in (4, 5)), where
         if kind in (0, 1, 8) and "n" in st:  # Bluestein: log2n = log2 M, M >= 2n - 1 > M / 2

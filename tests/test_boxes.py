@@ -1,6 +1,6 @@
 """Box-distributed plans (dfft_plan_create_boxes) without a GPU: validation, getters and sizes, byte-identical descriptions
-for natural boxes, and numpy replays of every rank's step list (box_replay.py, step_replay.py's engine) under the
-happens-before check, checked against fftn / rfftn / dctn of the global field on each rank's box.
+for natural boxes, and numpy replays of every rank's step list (step_replay.py) under the happens-before check, checked
+against fftn / rfftn / dctn of the global field on each rank's box.
 
 The replayed cases cover slab, Z_Then_YX and pencil, Peer2Peer and All2All, C2C (with a Bluestein axis), R2C / C2R and DCT,
 2x2x2 bricks on 8 ranks, 2x2x1 on 4, z-slabs into an x-slab plan, uneven bricks, out_boxes = in_boxes, bricks of the
@@ -15,9 +15,8 @@ import pytest
 import scipy.fft as sf
 
 import distributedfft_b200 as dfft
-import box_replay as R
+import step_replay as R
 from distributedfft_b200._lib import lib
-from step_replay import describe_raw
 
 SL, ZY, PE = dfft.SLAB_ZY_THEN_X, dfft.SLAB_Z_THEN_YX, dfft.PENCIL
 C2C, R2C, DCT = dfft.C2C, dfft.R2C, dfft.DCT
@@ -232,7 +231,7 @@ def test_null_boxes_are_the_plain_plan():
     cfg = C.byref(dfft._lib.dfft_config(1, 0, P2P, STREAMS, None, P2P, STREAMS))
     assert lib().dfft_plan_create_boxes(c, cfg, SL, dfft.F64, C2C, 64, 64, 64, 1, 1, None, None, 1, 1, C.byref(h)) == 0
     want = R.describe_text(plan(4, SL, (64, 64, 64), send=STREAMS, batch=1), 0, 0, 3)
-    assert describe_raw(h, 0, 3) == want
+    assert R.describe_raw(h, 0, 3) == want
     lib().dfft_plan_destroy(h)
     lib().dfft_comm_destroy(c)
 
@@ -311,3 +310,16 @@ def test_slot_rule_catches_a_missing_reshape_rendezvous():
             sc["steps"] = [s for s in sc["steps"] if s["label"] != "reshape rendezvous"]
     with pytest.raises(AssertionError):
         R.replay(p, 0, 3, [np.zeros(S3, dtype=complex)], mutate=drop)
+
+
+def test_slot_rule_refuses_remote_reads_outside_the_output_gathers():
+    """the gathers of the output reshape are the only passes that read a peer's slot: relabelled, they fail the replay"""
+    p = plan(4, SL, S3, out_boxes=bricks(S3, (1, 2, 2)))
+
+    def relabel(scheds):
+        for sc in scheds:
+            for s in sc["steps"]:
+                if s["label"] == "reshape out":
+                    s["label"] = "reshape gather"
+    with pytest.raises(AssertionError, match="output gathers"):
+        R.replay(p, 0, 3, [np.zeros(S3, dtype=complex)], mutate=relabel)

@@ -1,5 +1,5 @@
 """Plans with strides (dfft_plan_set_strides) without a GPU: refusals, getters, descriptions, the schedule they run, and numpy
-replays of every rank's step list (embed_replay.py) under the happens-before check, on caller arrays whose ghost layers
+replays of every rank's step list (step_replay.py) under the happens-before check, on caller arrays whose ghost layers
 hold a poison that no pass may read or overwrite.
 
 Each replay is checked against the same plan without strides, replayed the same way on dense arrays (the step lists of
@@ -11,14 +11,13 @@ from __future__ import annotations
 
 import ctypes as C
 import json
+from dataclasses import replace
 
 import numpy as np
 import pytest
 import scipy.fft as sf
 
 import distributedfft_b200 as dfft
-import box_replay as B
-import embed_replay as E
 import step_replay as R
 from distributedfft_b200._lib import lib
 from test_boxes import bricks
@@ -33,18 +32,19 @@ SYNC, STREAMS = 0, 1
 ERR_INVALID, ERR_STATE, ERR_UNSUPPORTED = -1, -4, -5
 
 
-def plan(P, decomp, shape, p1=1, p2=1, **kw):
-    return E.Plan(P, decomp, tuple(shape), p1, p2, **kw)
+def plan(P, decomp, shape, p1=1, p2=1, embed="both", **kw):
+    return R.Plan(P, decomp, tuple(shape), p1, p2, embed=embed, **kw)
 
 
 def dense(p):
     """the same plan without strides"""
-    return E.Plan(**{**p.__dict__, "embed": ""})
+    return replace(p, embed=None)
 
 
 # ---- refusals, getters, descriptions ----------------------------------------------------------------------------------------
 def make(p, rank=0):
-    rc, msg, c, h = B.create(p, rank)
+    """rank's plan of p before any setter"""
+    rc, msg, c, h = R.create(dense(p), rank)
     assert rc == 0, msg
     return c, h
 
@@ -117,8 +117,8 @@ def test_getters_and_describe():
         assert sc["in_strides"] == [2000, 200, 20] and "out_strides" not in sc
     finally:
         close(c, h)
-    sc = E.describe(plan(2, ZY, (8, 8, 8), embed="both", halo=1, batch=2, gap=3), 1, 1, 3)
-    assert sc["in_strides"] == list(E.strides([4, 8, 8], 1, 3)) and sc["out_strides"] == list(E.strides([8, 8, 4], 1, 3))
+    sc = R.describe(plan(2, ZY, (8, 8, 8), embed="both", halo=1, batch=2, gap=3), 1, 1, 3)
+    assert sc["in_strides"] == list(R.strides([4, 8, 8], 1, 3)) and sc["out_strides"] == list(R.strides([8, 8, 4], 1, 3))
     assert sc["field_in"] == sc["out_strides"][0] * 16 and sc["field_out"] == sc["in_strides"][0] * 16
 
 
@@ -132,7 +132,7 @@ def test_plans_without_strides_keep_their_schedule(P, decomp, shape, send, batch
     base = plan(P, decomp, shape, send=send, batch=batch, embed="")
     for r in range(P):
         for inv in (0, 1):
-            want = E.describe_text(base, r, inv, 3)
+            want = R.describe_text(base, r, inv, 3)
             assert "in_strides" not in want and "out_strides" not in want
             if label:
                 assert label in want or label.replace("zy", "yz") in want
@@ -144,7 +144,7 @@ def test_plans_without_strides_keep_their_schedule(P, decomp, shape, send, batch
                 assert R.describe_raw(h, inv, 3) == want
             finally:
                 close(c, h)
-            got = E.describe(plan(P, decomp, shape, send=send, batch=batch, halo=1), r, inv, 3)
+            got = R.describe(plan(P, decomp, shape, send=send, batch=batch, halo=1), r, inv, 3)
             assert not got["overlapped"]
             labels = [s["label"] for s in got["steps"]]
             assert not any(l.startswith(("zy pass", "yz pass", "batched pass")) for l in labels), labels
@@ -159,25 +159,14 @@ def inputs(p, inv, d, seed=0):
     xs = [rng.standard_normal(p.shape) + (0 if real else 1j * rng.standard_normal(p.shape)) for _ in range(p.fields)]
     if not inv:
         return xs
-    return assemble(B.replay(dense(p), 0, d, xs))
-
-
-def assemble(outs):
-    res = []
-    for blocks in outs:
-        shape = tuple(max(s[a] + b.shape[a] for s, b in blocks) for a in range(3))
-        g = np.zeros(shape, dtype=blocks[0][1].dtype)
-        for (s0, s1, s2), b in blocks:
-            g[s0:s0 + b.shape[0], s1:s1 + b.shape[1], s2:s2 + b.shape[2]] = b
-        res.append(g)
-    return res
+    return R.assemble(R.replay(dense(p), 0, d, xs))
 
 
 def check(p, inv, d=3):
     x = inputs(p, inv, d)
-    want = assemble(B.replay(dense(p), inv, d, x))
-    got = E.replay(p, inv, d, x)
-    assert E.error(got, want) < 1e-14
+    want = R.assemble(R.replay(dense(p), inv, d, x))
+    got = R.replay(p, inv, d, x)
+    assert R.error(got, want) < 1e-14
 
 
 S = (8, 12, 16)
@@ -218,7 +207,7 @@ def test_replay_blocked_tails(decomp, P, p1, p2, nz, inv, comm, monkeypatch):
     monkeypatch.setenv("DFFT_BLOCKED", "4")
     p = plan(P, decomp, (8, 8, nz), p1, p2, comm=comm)
     if comm == P2P:
-        labels = [s["label"] for s in E.describe(p, 0, inv, 3)["steps"]]
+        labels = [s["label"] for s in R.describe(p, 0, inv, 3)["steps"]]
         assert "x pass (tail)" in labels or "y pass (tail)" in labels, labels
     check(p, inv)
 
@@ -241,7 +230,7 @@ def test_replay_partial(decomp, p1, p2, d, inv, comm):
     if decomp == ZY and inv and d == 2:
         pytest.skip("Z_Then_YX offers no partial inverse of d = 2")
     p = plan(4, decomp, S, p1, p2, comm=comm)
-    sc = E.describe(p, 0, inv, d)
+    sc = R.describe(p, 0, inv, d)
     assert "in_strides" in sc and "out_strides" in sc
     check(p, inv, d)
 
@@ -275,4 +264,4 @@ def test_ghost_rule_catches_a_view_off_its_block():
             st = next(s for s in sc["steps"] if s["type"] == 0 and s["in_user"] == 1)
             st["in"]["segs"][0]["base"] -= sc["esize"]
     with pytest.raises(AssertionError, match="ghost"):
-        E.replay(p, 0, 3, inputs(p, 0, 3), mutate=shift)
+        R.replay(p, 0, 3, inputs(p, 0, 3), mutate=shift)

@@ -1,122 +1,41 @@
 """Box-distributed plans (dfft_plan_create_boxes) replayed on one GPU with the real kernels.
 
-The step lists of every rank of a box plan run in lock step through dfft_debug_run_step (the helpers of
-test_gpu_schedule_replay.py): the reshape copies (fft_copy_kernel) move the caller's boxes into and out of the natural
-layouts, the FFT passes are those of the natural plan.  Each case is checked
+The step lists of every rank of a box plan run in lock step through dfft_debug_run_step (gpu_replay.py): the reshape
+copies (fft_copy_kernel) move the caller's boxes into and out of the natural layouts, the FFT passes are those of the
+natural plan.  Each case is checked
   1. bit for bit against the same plan with natural boxes, replayed the same way, its output re-sliced to the boxes (the
      passes are identical and the copies exact);
   2. against the long-double reference within the bounds of test_gpu_schedule_replay (rel-L2 <= 3 u sqrt(sum log2 L),
      max <= 30 times that times rms(ref));
-  3. inputs unchanged, no output element left unwritten, and the ranks of a step in either order giving the same bits.
+  3. the checks gpu_replay.output makes of every plan: inputs unchanged, no output element left unwritten, and the ranks
+     of a step in either order giving the same bits.
 With a scale, the output equals the unscaled output times the scale, bit for bit."""
-import ctypes as C
-import json
 import os
 import subprocess
+from dataclasses import replace
 
 import numpy as np
 import pytest
-import torch
 
 import distributedfft_b200 as dfft
-import box_replay as R
 import test_gpu_schedule_replay as G
-from distributedfft_b200._lib import check, lib
-from step_replay import describe_raw
+from gpu_replay import assemble, output, replay, same_bits
 from test_boxes import CASES, S3, bricks, nzc, plan
 
 SL, ZY, PE = dfft.SLAB_ZY_THEN_X, dfft.SLAB_Z_THEN_YX, dfft.PENCIL
 C2C, R2C, DCT = dfft.C2C, dfft.R2C, dfft.DCT
 P2P, A2A = 0, 1
 HERE = os.path.dirname(os.path.abspath(__file__))
-PLAIN_SIDES = G.sides  # run() swaps G.sides for box_sides while it replays
-
-
-class BoxDryPlans:
-    """the geometry-only box plans of all ranks with their step lists (the interface of G.DryPlans)"""
-
-    def __init__(self, p, inverse, d):
-        self.comms, self.plans, self.scheds = [], [], []
-        for r in range(p.P):
-            rc, msg, c, h = R.create(p, r)
-            assert rc == 0, msg
-            self.comms.append(c)
-            self.plans.append(h)
-            if p.axes is not None:
-                check(lib().dfft_plan_set_transform_axes(h, (C.c_int * 3)(*p.axes)))
-            if p.scale is not None:
-                check(lib().dfft_plan_set_scale(h, *p.scale))
-            sc = json.loads(describe_raw(h, inverse, d))
-            sc["domain_bytes"] = lib().dfft_get_domain_size(h)
-            self.scheds.append(sc)
-
-    close = G.DryPlans.close
-
-
-def spec_of(p, inverse, d):
-    kinds = (DCT,) * 3 if p.transform == DCT else None
-    return G.spec(p.P, p.decomp, None if kinds else p.transform, p.shape, p.p1 if p.decomp == PE else p.P, p.p2, p.comm, inverse=inverse, d=d,
-                  kinds=kinds, axes=p.axes or (1, 1, 1), batch=p.fields, scale=p.scale)
-
-
-def box_sides(s, p, scheds):
-    """G.sides with each boxed side's layout replaced by the rank's box"""
-    es = scheds[0]["esize"]
-    sd = PLAIN_SIDES(s, p.P, s["p1"], s["p2"], [sc["domain_bytes"] for sc in scheds], es)
-    for r, pair in enumerate(sd):
-        for which, side in enumerate(pair):
-            physical = (which == 0) != bool(s["inverse"])
-            boxes = p.in_boxes if physical else (p.out_boxes if s["d"] == 3 else None)
-            if boxes is None:
-                continue
-            lo, hi = boxes[r]
-            side.size, side.start = [h - l for l, h in zip(lo, hi)], list(lo)
-            side.elems = side.size[0] * side.size[1] * (side.size[2] // 2 if side.r2c_real else side.size[2])
-            side.field = side.elems
-            side.nbytes = max(s["batch"] * side.elems, 1) * es
-    return sd
-
-
-def run(p, inverse, d, x, descending=False):
-    """G.replay on the box sides: (ins, outs, sides)"""
-    s = spec_of(p, inverse, d)
-    dry = BoxDryPlans(p, inverse, d)
-    try:
-        G.sides = lambda *a: box_sides(s, p, dry.scheds)
-        return G.replay(s, dry, x, descending)
-    finally:
-        G.sides = PLAIN_SIDES
-        dry.close()
-
-
-def output(p, inverse, d, x):
-    """the global output (batch, ...) of box plan p on x, after checks 3"""
-    s = spec_of(p, inverse, d)
-    ins, outs, sd = run(p, inverse, d, x)
-    got = G.assemble(s, sd, outs, 1)
-    assert not np.isnan(got).any(), f"{int(np.isnan(got).sum())} output elements were never written"
-    for f in range(s["batch"]):
-        for r, (si, _) in enumerate(sd):
-            assert G.same_bits(si.get(ins[r], f), G.block(x[f], si.start, si.size).astype(si.npdt)), f"rank {r} field {f}: input changed"
-    _, outs2, _ = run(p, inverse, d, x, descending=True)
-    assert G.same_bits(G.assemble(s, sd, outs2, 1), got), "the result depends on the order of the ranks within a step"
-    return got
 
 
 def check_box_plan(p, inverse, d=3, seed=0):
-    s = spec_of(p, inverse, d)
-    x, x_ld = G.global_input(s, seed)
+    x, x_ld = G.global_input(p, inverse, d, seed)
     got = output(p, inverse, d, x)
     # 1: the natural plan, replayed the same way
-    nat = G.DryPlans(s)
-    try:
-        _, outs, sd = G.replay(s, nat, x)
-        want = G.assemble(s, sd, outs, 1)
-    finally:
-        nat.close()
-    assert G.same_bits(got, want), f"differs from the natural plan at {np.argwhere(got != want)[:8].tolist()}"
+    want = assemble(replay(replace(p, in_boxes=None, out_boxes=None), inverse, d, x))
+    assert same_bits(got, want), f"differs from the natural plan at {np.argwhere(got != want)[:8].tolist()}"
     # 2: the long-double reference
-    rel, mx = G.error_check(s, got, G.reference(s, x_ld))
+    rel, mx = G.error_check(G.geometry(p, d), got, G.reference(p, inverse, d, x_ld))
     assert rel <= 3.0 and mx <= 30.0, (rel, mx)
     return x, got
 
@@ -164,7 +83,7 @@ def test_box_scale_is_exact(transform, comm):
         # each real value times s (a complex product would turn the sign of zero imaginary parts)
         r = plain.real.dtype
         want = (np.ascontiguousarray(plain).view(r) * r.type(scale[inv])).view(plain.dtype)
-        assert G.same_bits(scaled, want)
+        assert same_bits(scaled, want)
 
 
 @pytest.mark.gpu

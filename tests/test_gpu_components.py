@@ -1,25 +1,21 @@
 """Interleaved multi-component plans on one GPU: one-rank C2C plans against numpy on [X, Y, Z, C] tensors, bit-for-bit
 comparisons with the batched plan on the permuted [C, X, Y, Z] input (512^3 x 3 included, where the batched plan runs the
 fused z + y stage), scale, graph replay and batches, and 2-8 rank schedules replayed with the real kernels through
-dfft_debug_run_step."""
-import ctypes as C
-
+dfft_debug_run_step (gpu_replay.py)."""
 import numpy as np
 import pytest
 
 import distributedfft_b200 as dfft
-from distributedfft_b200 import _lib
-from distributedfft_b200._lib import check, lib
-from test_components import describe_ilv
+import step_replay as R
+from gpu_replay import output
 from test_gpu_accuracy import check_units, ld, spec as unit_spec, unit_scales
-from test_schedule_emulation import A2A, P2P, PE, SL, SYNC, ZY
+from test_schedule_emulation import A2A, P2P, PE, SL, ZY
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 CLASSES = {SL: dfft.MPIcuFFT_Slab, ZY: dfft.MPIcuFFT_Slab_Z_Then_YX, PE: dfft.MPIcuFFT_Pencil}
 TOL = {True: 1e-10, False: 1e-5}
-SLOT_SHIFT = 44
 
 
 def make(shape, comps, decomp=SL, f64=True, batch=1, transform="c2c"):
@@ -161,20 +157,6 @@ def test_partial_scale_graph_and_batch():
 
 
 # ---- multi-rank schedules on one GPU ---------------------------------------------------------------------------------------
-def dry_plans(P, decomp, shape, p1, p2, comm, comps, inverse, d, transform=dfft.C2C):
-    plans, comms, scheds = [], [], []
-    for r in range(P):
-        c = C.c_void_p()
-        check(lib().dfft_comm_create_dry(r, P, C.byref(c)))
-        cfg = _lib.dfft_config(1, 0, comm, SYNC, None, comm, SYNC)
-        p = C.c_void_p()
-        check(lib().dfft_plan_create_interleaved(c, C.byref(cfg), decomp, dfft.F64, transform, *shape, p1, p2, comps, 1, 1, C.byref(p)))
-        plans.append(p)
-        comms.append(c)
-        scheds.append(describe_ilv(r, P, decomp, transform, shape, p1, p2, comps, 1, comm, inverse, d))
-    return plans, comms, scheds
-
-
 @pytest.mark.parametrize("P,decomp,shape,p1,p2,comm,comps", [
     (2, SL, (32, 32, 64), 2, 1, P2P, 3), (4, SL, (16, 24, 64), 4, 1, A2A, 5), (3, ZY, (12, 16, 32), 3, 1, P2P, 2), (3, ZY, (16, 16, 32), 3, 1, P2P, 2),
     (4, ZY, (16, 8, 32), 4, 1, A2A, 17), (4, PE, (16, 16, 64), 2, 2, P2P, 3), (8, PE, (16, 16, 32), 4, 2, A2A, 4),
@@ -194,14 +176,10 @@ def test_multi_rank_replay_r2c(P, decomp, shape, p1, p2, comm, comps, inverse):
 
 
 def replay_case(P, decomp, shape, p1, p2, comm, comps, inverse, transform):
-    """every rank's steps in lock step with the real kernels; against numpy (R2C / C2R: each component against long double
-    on its own norm) and, bit for bit, the one-rank plan"""
+    """every rank's steps in lock step with the real kernels (gpu_replay.py, with the checks it makes of every plan);
+    against numpy (R2C / C2R: each component against long double on its own norm) and, bit for bit, the one-rank plan"""
     d = 3
     c2c = transform == dfft.C2C
-    plans, comms, scheds = dry_plans(P, decomp, shape, p1, p2, comm, comps, inverse, d, transform)
-    es = scheds[0]["esize"]
-    work_bytes = scheds[0]["nslots"] * scheds[0]["slot_bytes"]
-    work = [torch.full((work_bytes,), 0xFF, dtype=torch.uint8, device="cuda") for _ in range(P)]
     one = make(shape, comps, decomp, transform="c2c" if c2c else "r2c")  # same decomposition: Z_Then_YX inverts y before x
     if c2c:
         x = rand(shape + (comps,), seed=4)
@@ -214,50 +192,23 @@ def replay_case(P, decomp, shape, p1, p2, comm, comps, inverse, transform):
         x = x * torch.from_numpy(sc).cuda()
         spec = r2c(one, x)
         src, want = (spec, c2r(one, spec)) if inverse else (x, spec)
+    p = R.Plan(P, decomp, shape, p1, p2, transform=transform, comm=comm, components=comps)
+    full = output(p, inverse, d, src[None].cpu().numpy())[0]
+    want = want.cpu().numpy()
     lay = lambda r, w: dfft.layout(decomp, transform, *shape, p1, p2, r, w)
     blk = lambda a, st, sz: a[st[0]:st[0] + sz[0], st[1]:st[1] + sz[1], st[2]:st[2] + sz[2]]
-    ins, outs = [], []
-    for r in range(P):
-        isz, ist = lay(r, d if inverse else 0)
-        osz, _ = lay(r, 0 if inverse else d)
-        ins.append(blk(src, ist, isz).contiguous().view(torch.uint8).reshape(-1).clone())
-        outs.append(torch.full((int(np.prod(osz)) * comps * want.element_size(),), 0xFF, dtype=torch.uint8, device="cuda"))
-    for k in range(len(scheds[0]["steps"])):
-        for r in range(P):
-            st = scheds[r]["steps"][k]
-            if st["type"] == 1:
-                continue
-            if st["type"] == 2:
-                sb = scheds[r]["slots"][st["send_slot"]][r] - ((r + 1) << SLOT_SHIFT)
-                for peer in st["peers"]:
-                    q = peer["rank"]
-                    rb = scheds[q]["slots"][st["recv_slot"]][q] - ((q + 1) << SLOT_SHIFT)
-                    mine = [pp for pp in scheds[q]["steps"][k]["peers"] if pp["rank"] == r][0]
-                    n = peer["scount"] * es
-                    work[q][rb + mine["roff"] * es:rb + mine["roff"] * es + n].copy_(work[r][sb + peer["soff"] * es:sb + peer["soff"] * es + n])
-                continue
-            ptrs = (C.c_void_p * P)(*[w.data_ptr() for w in work])
-            rc = lib().dfft_debug_run_step(plans[r], inverse, d, 0, k, ptrs, work_bytes, outs[r].data_ptr(), outs[r].numel(), ins[r].data_ptr(),
-                                           ins[r].numel(), torch.cuda.current_stream().cuda_stream)
-            assert rc == 0, (lib().dfft_last_error_string() or b"").decode()
-    torch.cuda.synchronize()
-    full = np.zeros(tuple(want.shape), dtype=want.cpu().numpy().dtype)
     for r in range(P):
         osz, ost = lay(r, 0 if inverse else d)
-        got = outs[r].view(want.dtype).reshape(*osz, comps)
+        got = blk(full, ost, osz)
         if not any(n & (n - 1) for n in shape):  # Bluestein passes: against the reference only
-            assert torch.equal(got, blk(want, ost, osz)), f"rank {r}"
+            assert np.array_equal(got, blk(want, ost, osz)), f"rank {r}"
         if c2c:
             ref = np.fft.ifftn(spec.cpu().numpy(), axes=(0, 1, 2)) * np.prod(shape) if inverse else np.fft.fftn(x.cpu().numpy(), axes=(0, 1, 2))
-            assert rel(got.cpu().numpy(), blk(ref, ost, osz)) < 1e-10
-        blk(full, ost, osz)[...] = got.cpu().numpy()
+            assert rel(got, blk(ref, ost, osz)) < 1e-10
     if not c2c:
         ref = (np.fft.irfftn(ld(spec.cpu().numpy()), s=shape, axes=(0, 1, 2)) * np.prod(shape) if inverse
                else np.fft.rfftn(ld(x.cpu().numpy()), axes=(0, 1, 2)))
         check_units("replay R2C/C2R", unit_spec(dfft.F64, shape), full, ref, 3, sc, f"P={P} {'inv' if inverse else 'fwd'}")
-    for p, c in zip(plans, comms):
-        lib().dfft_plan_destroy(p)
-        lib().dfft_comm_destroy(c)
     one.destroy()
 
 

@@ -9,23 +9,21 @@ sizes).  The caller's whole input array and every output ghost element are uncha
 times the scale bit for bit, and a CUDA graph of the _async execs replays what the eager execs computed.  A 512^3 C2C plan
 with strides is checked against the fused plan without them within the oracle's tolerance.
 
-Multi-rank plans run every rank's step list in lock step through dfft_debug_run_step with the real kernels, on caller
-arrays with poisoned ghost layers, bit for bit against the plan without strides replayed the same way
-(test_gpu_schedule_replay.py's helpers)."""
-import ctypes as C
-import json
+Multi-rank plans run every rank's step list in lock step through dfft_debug_run_step with the real kernels (gpu_replay.py),
+on caller arrays with poisoned ghost layers, bit for bit against the plan without strides replayed the same way."""
 import os
 import subprocess
+from dataclasses import replace
 
 import numpy as np
 import pytest
 import torch
 
 import distributedfft_b200 as dfft
+import step_replay as R
 import test_gpu_schedule_replay as G
 from common import CDT, RDT, TOL
-from distributedfft_b200._lib import check, lib
-from step_replay import describe_raw
+from gpu_replay import assemble, output, replay, same_bits
 
 SL, ZY, PE = dfft.SLAB_ZY_THEN_X, dfft.SLAB_Z_THEN_YX, dfft.PENCIL
 C2C, R2C, DCT, R2HC = dfft.C2C, dfft.R2C, dfft.DCT, dfft.R2HC
@@ -218,124 +216,17 @@ def test_512_cubed_against_the_fused_plan():
 
 
 # ---- multi-rank plans with the real kernels ---------------------------------------------------------------------------------
-class EmbeddedDryPlans(G.DryPlans):
-    """G.DryPlans whose ranks have ghost layers of H around each block on the sides named in `embed`"""
-
-    def __init__(self, s, embed, gap=0):
-        self.comms, self.plans, self.scheds = [], [], []
-        for r in range(s["P"]):
-            c = C.c_void_p()
-            check(lib().dfft_comm_create_dry(r, s["P"], C.byref(c)))
-            self.comms.append(c)
-            plan = G.make_plan(c, s, s["p1"], s["p2"], 1)
-            self.plans.append(plan)
-            sides = []
-            for fn, name in ((lib().dfft_get_in_size, "in"), (lib().dfft_get_out_size, "out")):
-                n = (C.c_size_t * 3)()
-                check(fn(plan, n))
-                y = n[2] + 2 * H
-                x = (n[1] + 2 * H) * y
-                sides.append((C.c_longlong * 3)((n[0] + 2 * H) * x + gap, x, y) if name in embed else None)
-            check(lib().dfft_plan_set_strides(plan, *sides))
-            sc = json.loads(describe_raw(plan, s["inverse"], s["d"]))
-            sc["domain_bytes"] = lib().dfft_get_domain_size(plan)
-            self.scheds.append(sc)
-
-
-class EmbeddedSide:
-    """a caller array with ghost layers around one rank's blocks: G.Side's interface over a strided view"""
-
-    def __init__(self, side, st, batch):
-        self.side, self.st, self.batch = side, st, batch
-        self.start, self.size, self.npdt, self.tdt = side.start, side.size, side.npdt, side.tdt
-        self.eb = torch.empty((), dtype=side.tdt).element_size()
-        self.lead = H * (st[1] + st[2] + 1)  # elements before the first block element
-        self.nbytes = (batch * st[0]) * self.eb
-
-    def view(self, buf, f):
-        return buf.view(self.tdt).as_strided(tuple(self.size), (self.st[1], self.st[2], 1), self.lead + f * self.st[0])
-
-    def put(self, buf, f, block):
-        self.view(buf, f).copy_(torch.from_numpy(np.ascontiguousarray(block.astype(self.npdt))))
-
-    def get(self, buf, f):
-        return self.view(buf, f).cpu().numpy()
-
-
-def replay_embedded(s, dry, x):
-    """G.replay on caller arrays with ghost layers (0xFF: NaN) on the embedded sides; returns (ins, outs, sides, ghosts ok)"""
-    P, scheds = s["P"], dry.scheds
-    es = scheds[0]["esize"]
-    nslots, slot_bytes = scheds[0]["nslots"], scheds[0]["slot_bytes"]
-    work_bytes = nslots * slot_bytes
-    work = [G.nan_buffer(work_bytes) for _ in range(P)]
-    plain = G.sides(s, P, s["p1"], s["p2"], [sc["domain_bytes"] for sc in scheds], es)
-    src_w, dst_w = (s["d"], 0) if s["inverse"] else (0, s["d"])
-    sd, ins, outs = [], [], []
-    for r in range(P):
-        pair = []
-        for side, w in zip(plain[r], (src_w, dst_w)):
-            st = scheds[r].get("in_strides") if w == 0 else scheds[r].get("out_strides") if w == 3 else None
-            pair.append(EmbeddedSide(side, st, s["batch"]) if st else side)
-        si, so = pair
-        bi = G.nan_buffer(si.nbytes)
-        for f in range(s["batch"]):
-            si.put(bi, f, G.block(x[f], si.start, si.size))
-        sd.append((si, so))
-        ins.append(bi)
-        outs.append(G.nan_buffer(so.nbytes))
-    before = [b.clone() for b in ins]
-    per = len(scheds[0]["steps"]) // s["batch"]
-    for k in range(len(scheds[0]["steps"])):
-        for r in range(P):
-            st = scheds[r]["steps"][k]
-            if st["type"] == 1:
-                continue
-            if st["type"] == 2:
-                sb = scheds[r]["slots"][st["send_slot"]][r] - ((r + 1) << G.SLOT_SHIFT)
-                for peer in st["peers"]:
-                    q = peer["rank"]
-                    rb = scheds[q]["slots"][st["recv_slot"]][q] - ((q + 1) << G.SLOT_SHIFT)
-                    mine = [pp for pp in scheds[q]["steps"][k]["peers"] if pp["rank"] == r][0]
-                    n = peer["scount"] * es
-                    work[q][rb + mine["roff"] * es:rb + mine["roff"] * es + n].copy_(work[r][sb + peer["soff"] * es:sb + peer["soff"] * es + n])
-                continue
-            si, so = sd[r]
-            lead_i = getattr(si, "lead", 0) * getattr(si, "eb", 0)
-            lead_o = getattr(so, "lead", 0) * getattr(so, "eb", 0)
-            ptrs = (C.c_void_p * P)(*[w.data_ptr() for w in work])
-            rc = lib().dfft_debug_run_step(dry.plans[r], s["inverse"], s["d"], k // per, k % per, ptrs, work_bytes, outs[r].data_ptr() + lead_o,
-                                           outs[r].numel() - lead_o, ins[r].data_ptr() + lead_i, ins[r].numel() - lead_i,
-                                           torch.cuda.current_stream().cuda_stream)
-            assert rc == 0, f"rank {r} step {k} ({st['label']}): {(lib().dfft_last_error_string() or b'').decode()}"
-    torch.cuda.synchronize()
-    for r, (si, so) in enumerate(sd):
-        assert torch.equal(ins[r], before[r]), f"rank {r}: the input array changed"
-        if isinstance(so, EmbeddedSide):
-            ghost = torch.ones(so.nbytes // so.eb, dtype=torch.bool, device="cuda")
-            for f in range(s["batch"]):
-                ghost.as_strided(tuple(so.size), (so.st[1], so.st[2], 1), so.lead + f * so.st[0]).fill_(False)
-            assert (outs[r].view(-1, so.eb)[ghost] == 0xFF).all(), f"rank {r}: an output ghost element was written"
-    return ins, outs, sd
-
-
-def check_multi(s, embed="both", gap=0, seed=0):
-    x, _ = G.global_input(s, seed)
-    dry = EmbeddedDryPlans(s, embed, gap)
-    try:
-        _, outs, sd = replay_embedded(s, dry, x)
-    finally:
-        dry.close()
-    got = G.assemble(s, sd, outs, 1)
-    assert not np.isnan(got).any(), f"{int(np.isnan(got).sum())} output elements were never written"
-    nat = G.DryPlans(s)
-    try:
-        _, outs, sdn = G.replay(s, nat, x)
-        want = G.assemble(s, sdn, outs, 1)
-    finally:
-        nat.close()
-    assert G.same_bits(got, want), f"differs from the plan without strides at {np.argwhere(got != want)[:8].tolist()}"
+def check_multi(p, inverse, d=3, seed=0):
+    """p's replay (H ghost layers around each block of its embedded sides) against the plan without strides, bit for bit"""
+    x, _ = G.global_input(p, inverse, d, seed)
+    got = output(p, inverse, d, x)
+    want = assemble(replay(replace(p, embed=None), inverse, d, x))
+    assert same_bits(got, want), f"differs from the plan without strides at {np.argwhere(got != want)[:8].tolist()}"
     return x, got
+
+
+def multi(P, decomp, transform, shape, p1, p2, comm=0, embed="both", **kw):
+    return R.Plan(P, decomp, shape, p1, p2, transform=transform, comm=comm, embed=embed, halo=H, **kw)
 
 
 MULTI = [
@@ -359,7 +250,7 @@ MULTI = [
 @pytest.mark.parametrize("case", MULTI, ids=[c[0] for c in MULTI])
 def test_multi_rank(case, inv, comm):
     _, P, decomp, transform, shape, p1, p2, kinds = case
-    check_multi(G.spec(P, decomp, transform, shape, p1, p2, comm, inverse=inv, kinds=kinds))
+    check_multi(multi(P, decomp, transform, shape, p1, p2, comm, kinds=kinds), inv)
 
 
 @pytest.mark.gpu
@@ -367,20 +258,18 @@ def test_multi_rank(case, inv, comm):
 @pytest.mark.parametrize("decomp,P,p1,p2,nz", [(SL, 3, 3, 1, 18), (PE, 4, 2, 2, 36)], ids=["slab", "pencil"])
 def test_multi_rank_blocked_tails(decomp, P, p1, p2, nz, inv, monkeypatch):
     monkeypatch.setenv("DFFT_BLOCKED", "4")
-    check_multi(G.spec(P, decomp, C2C, (8, 8, nz), p1, p2, 0, inverse=inv))
+    check_multi(multi(P, decomp, C2C, (8, 8, nz), p1, p2), inv)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("embed", ["in", "out", "both"])
 def test_multi_rank_batch_gap_scale(embed):
     for inv in (0, 1):
-        s = G.spec(4, PE, C2C, (8, 8, 16), 2, 2, 0, inverse=inv, batch=2)
-        x, plain = check_multi(s, embed, gap=6)
-        s = G.spec(4, PE, C2C, (8, 8, 16), 2, 2, 0, inverse=inv, batch=2, scale=(0.37, 1 / 96))
-        _, scaled = check_multi(s, embed, gap=6)
+        x, plain = check_multi(multi(4, PE, C2C, (8, 8, 16), 2, 2, embed=embed, batch=2, gap=6), inv)
+        _, scaled = check_multi(multi(4, PE, C2C, (8, 8, 16), 2, 2, embed=embed, batch=2, gap=6, scale=(0.37, 1 / 96)), inv)
         r = plain.real.dtype
         want = (np.ascontiguousarray(plain).view(r) * r.type((0.37, 1 / 96)[inv])).view(plain.dtype)
-        assert G.same_bits(scaled, want)
+        assert same_bits(scaled, want)
 
 
 @pytest.mark.gpu
@@ -388,13 +277,13 @@ def test_multi_rank_batch_gap_scale(embed):
 @pytest.mark.parametrize("d", [1, 2])
 @pytest.mark.parametrize("decomp,p1,p2", [(SL, 4, 1), (PE, 2, 2)], ids=["slab", "pencil"])
 def test_multi_rank_partial(decomp, p1, p2, d, inv):
-    check_multi(G.spec(4, decomp, C2C, (8, 8, 16), p1, p2, 0, inverse=inv, d=d))
+    check_multi(multi(4, decomp, C2C, (8, 8, 16), p1, p2), inv, d)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("inv", [0, 1], ids=["fwd", "inv"])
 def test_multi_rank_x_kept(inv):
-    check_multi(G.spec(4, PE, C2C, (8, 8, 16), 2, 2, 0, inverse=inv, axes=(0, 1, 1)))
+    check_multi(multi(4, PE, C2C, (8, 8, 16), 2, 2, axes=(0, 1, 1)), inv)
 
 
 @pytest.mark.gpu

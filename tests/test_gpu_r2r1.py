@@ -9,7 +9,7 @@
   DCT-I compared on the device.
 - Bit for bit: in place against out of place, batch against single fields, scale against unscaled, graph replay against
   eager.
-- 2-8 rank schedules replayed with the real kernels through dfft_debug_run_step (test_gpu_schedule_replay's lock step).
+- 2-8 rank schedules replayed with the real kernels through dfft_debug_run_step (gpu_replay.py).
 - A vertex-centred Dirichlet Poisson solve with DST-I (7-point Laplacian residual) and the Chebyshev check: the DCT-I of
   T_m(cos(pi j / N)) is N delta_km, 2N at m = 0 and m = N.
 - The C++ shim's per-axis constructor with type-I kinds (tests/cpp/r2r1_shim_test.cpp)."""
@@ -23,10 +23,12 @@ import scipy.fft as sf
 import torch
 
 import distributedfft_b200 as dfft
+import step_replay as R
 from common import PNAME, RDT, TOL
 from oracle import dft_oracle as O
 from test_gpu_accuracy import check_units, mixed, on_device, spec as acc_spec
-from test_gpu_schedule_replay import DryPlans, assemble, global_input, replay, same_bits, spec as rspec
+from gpu_replay import output
+from test_gpu_schedule_replay import global_input
 from test_r2r1 import DCT1, DST1, R2HC, DCT, DST, axis_len, global_ref, r2r_1d
 
 pytestmark = pytest.mark.gpu
@@ -259,17 +261,9 @@ REPLAYS = [  # P, decomp, base shape, p1, p2, comm, kinds
 @pytest.mark.parametrize("P,decomp,base,p1,p2,comm,kinds", REPLAYS)
 def test_multi_rank_replay(P, decomp, base, p1, p2, comm, kinds, inverse, prec):
     shape = tuple(axis_len(n, k) for n, k in zip(base, kinds))
-    s = rspec(P, decomp, None, shape, p1, p2, comm=comm, inverse=inverse, prec=prec, kinds=kinds)
-    dry = DryPlans(s)
-    try:
-        x, _ = global_input(s, 1)
-        ins, outs, sd = replay(s, dry, x)
-        got = assemble(s, sd, outs, 1)
-        assert not np.isnan(got).any()
-        _, outs2, _ = replay(s, dry, x, descending=True)
-        assert same_bits(assemble(s, sd, outs2, 1), got), "the result depends on the order of the ranks within a step"
-    finally:
-        dry.close()
+    p = R.Plan(P, decomp, shape, p1, p2, kinds=kinds, prec=prec, comm=comm)
+    x, _ = global_input(p, inverse, 3, 1)
+    got = output(p, inverse, 3, x)
     want = global_ref(x[0].astype(np.float64), kinds, bool(inverse), 3)
     assert O.rel_l2(got[0].astype(np.float64), want) < TOL[prec]
 

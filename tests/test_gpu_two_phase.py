@@ -433,7 +433,8 @@ def test_fused_vs_long_double(prec, nx, n, inverse):
     """the smallest fused shape of 256^2 planes at 50 MiB of L2 (a Bluestein x pass) against np.fft in long double:
     rel-L2 <= 3 and max <= 30 in units of u sqrt(sum log2 L), the bounds of test_gpu_schedule_replay"""
     import torch
-    from test_gpu_schedule_replay import error_check, spec
+    from test_gpu_accuracy import spec
+    from test_gpu_schedule_replay import error_check
 
     c = FusedCase(n, prec, nx)
     direction = dfft.INVERSE if inverse else dfft.FORWARD
@@ -450,7 +451,7 @@ def test_fused_vs_long_double(prec, nx, n, inverse):
     ref = np.fft.fft if not inverse else (lambda v, axis: np.fft.ifft(v, axis=axis) * v.shape[axis])
     for axis in ((2, 1, 0) if not inverse else (0, 1, 2)):
         xl = ref(xl, axis=axis)
-    s = spec(1, SL, dfft.C2C, (nx, n, n), 1, 1, inverse=inverse, prec=prec)
+    s = spec(prec, (nx, n, n))
     rel, mx = error_check(s, out.cpu().numpy(), xl)
     key = ("f64" if prec == F64 else "f32", "inverse" if inverse else "forward")
     print(f"long double {key} {nx}x{n}x{n}: rel-L2 {rel:.2f}, max {mx:.2f} (units of u sqrt(sum log2 L))")
