@@ -138,8 +138,9 @@ static bool r2r_kind_length(int kind, size_t n) {
 // table of n).  PASS_R2R_*: the R2R kernel of kind r2r (DFFT_DCT, DFFT_DST with prm.tw2 its w_k table, or DFFT_R2HC), or
 // the type-I kernel (DFFT_DCT1, DFFT_DST1: n = N +- 1 reals, prm.tw2 the 2N-point table), or the type-IV kernel
 // (DFFT_DCT4, DFFT_DST4: n reals through n/2-point lines, prm.tw2 the type-IV table).
-// hole: passes of padded plans that keep part of their spectral side, the hole [hole[0], hole[1]) of their lines
-// (pass_hole); the padded twin of the power-of-two kernel runs then.
+// hole: passes of padded and pruned plans that keep part of a side, the holes of their lines (pass_hole): [hole[0],
+// hole[1]) on the spectral side, [hole[2], hole[3]) on the physical one; the padded twin of the power-of-two kernel runs
+// then, with the physical hole on its loaded side forward and on its stored side inverse.
 static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftParams& prm, const void* blu, double scale, cudaStream_t stream,
                                    int r2r = DFFT_DCT, const int* hole = nullptr) {
     const int log2n = ilog2_exact(n);
@@ -147,8 +148,10 @@ static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftP
         FftPadded q;
         static_cast<FftParams&>(q) = prm;
         q.scale = scale;
-        q.lo = hole[0];
-        q.hi = hole[1];
+        const int* ld = prm.inverse ? hole : hole + 2;
+        const int* st = prm.inverse ? hole + 2 : hole;
+        q.ld_lo = ld[0]; q.ld_hi = ld[1];
+        q.st_lo = st[0]; q.st_hi = st[1];
         return launch_padded(prec, log2n, kind, q, stream);
     }
     if (kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED) {
@@ -172,14 +175,18 @@ static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftP
     return launch_bluestein(prec, log2m, kind, b, stream);
 }
 
-// The hole of a pass of n-point lines (R2C / C2R: n complex points, n + 1 spectral ones) that keeps `keep` points of its
-// spectral side (0: all of them).  C2C: frequencies 0 .. ceil(K/2) - 1 and the K - ceil(K/2) negative ones, at the end of
-// the line (numpy's fftfreq(K) * K mod N); R2C / C2R: k = 0 .. keep - 1.
-static void pass_hole(PassKind kind, size_t n, size_t keep, int hole[2]) {
+// The holes of a pass of n-point lines (R2C / C2R: n complex points, n + 1 spectral ones) that keeps `keep` points of its
+// spectral side and `data` points of its physical side (0: all of them).  Spectral, C2C: frequencies 0 .. ceil(K/2) - 1
+// and the K - ceil(K/2) negative ones, at the end of the line (numpy's fftfreq(K) * K mod N); R2C / C2R: k = 0 .. keep - 1.
+// Physical: positions 0 .. data - 1; R2C / C2R: data reals, the pairs 0 .. data/2 - 1.  hole[0..1] spectral, hole[2..3]
+// physical, each empty when lo == hi.
+static void pass_hole(PassKind kind, size_t n, size_t keep, size_t data, int hole[4]) {
     const bool half = kind == PASS_R2C || kind == PASS_C2R;
     const size_t full = half ? n + 1 : n, k = keep ? keep : full;
     hole[0] = int(half ? k : (k + 1) / 2);
     hole[1] = int(hole[0] + full - k);
+    hole[2] = int(data ? (half ? data / 2 : data) : n);
+    hole[3] = int(n);
 }
 
 // Passes over an axis the plan keeps (dfft_plan_set_transform_axes): the views of the FFT pass they replace, no transform
@@ -404,6 +411,16 @@ struct Step {
     // padded plans: the points its spectral side keeps of each line (Kx, Ky, Kz; R2C / C2R: Kz/2 + 1 of the Nz/2 + 1), the
     // rest is the hole (fft_kernels.cuh, FftPadded); 0: the whole line
     size_t keep = 0;
+    // pruned plans: the points its physical side holds of each line (Mx, My, Mz; R2C / C2R: Mz reals), the rest is zero
+    // (forward: never loaded, inverse: never stored); 0: the whole line
+    size_t data = 0;
+    // points along n of its input and output views (dfft_debug_run_step and embed_views size views by them)
+    void view_lens(size_t* in_len, size_t* out_len) const {
+        const size_t len = n ? n : size_t(1) << log2n;
+        const size_t phys = data ? (kind == PASS_R2C || kind == PASS_C2R ? data / 2 : data) : len;
+        *in_len = prm.inverse ? (keep ? keep : len + (kind == PASS_C2R ? 1 : 0)) : phys;
+        *out_len = prm.inverse ? phys : (keep ? keep : len + (kind == PASS_R2C ? 1 : 0));
+    }
     FftParams prm{};
     int in_user = 0, out_user = 0;  // 1: patch seg[0].base with the caller's in, 2: with the caller's out
     // RENDEZVOUS
@@ -632,21 +649,23 @@ static bool pow2_axes(const dfft_plan_s* p) { return ilog2_exact(p->g.nx) > 0 &&
 // only: the overlapped schedules, the fused z + y stage and the batched stage transform every axis they touch.
 static bool all_axes(const dfft_plan_s* p) { return p->taxes[0] && p->taxes[1] && p->taxes[2]; }
 // Whether the schedules may take another form than the sequential one: the overlapped schedules, the fused z + y stage and
-// the batched stage build their passes for power-of-two lengths, every axis transformed and no padding (their kernels have
-// no padded twins, FftPadded).
+// the batched stage build their passes for power-of-two lengths, every axis transformed and no padding or pruning (their
+// kernels have no padded twins, FftPadded).
 // Interleaved plans (C > 1 values per point) run it too: those kernels address one value per point.  So do plans with a
 // box that is not the natural layout: their reshape steps wrap the sequential schedule (wrap_boxes).  And embedded plans
 // (dfft_plan_set_strides): the other forms read and write dense caller arrays, and every rank must run the same form.
 static bool alt_schedules(const dfft_plan_s* p) {
-    return pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p) && !p->g.padded() && p->comps == 1 && !p->boxed() && !p->embedded();
+    return pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p) && !p->g.padded() && !p->g.pruned() && p->comps == 1 && !p->boxed() &&
+           !p->embedded();
 }
 
 // Row pitch, in elements (complex units; reals for DCT / DST plans), of the z-contiguous side of the caller's buffers that
 // holds Nz points per row: the input of forward passes, the output of inverse ones.  Real rows of R2C / C2R plans are Nz reals (Nz/2 units) apart, or, in
 // place, Nzc units apart (the padded layout of FFTW and cuFFT: the last one or two reals of a row are never touched).
+// Pruned plans hold Mz points per row (R2C / C2R: Mz reals, Mz/2 units).
 static long long z_row_pitch(const dfft_plan_s* p) {
     const Geometry& g = p->g;
-    return (long long)(g.transform != DFFT_R2C || p->inplace ? g.nzc : g.nz / 2);
+    return (long long)(p->inplace ? g.nzc : g.transform != DFFT_R2C ? g.mz : g.mz / 2);
 }
 
 // Whether the z and y passes run as one fused launch (fft_zy_fused_kernel): one-rank slab C2C plans of the full 3D
@@ -654,8 +673,8 @@ static long long z_row_pitch(const dfft_plan_s* p) {
 // three passes are L2-resident already and gain nothing.
 static bool zy_fused(const dfft_plan_s* p, int inverse, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || p->comps > 1 || p->boxed() ||
-        p->embedded())
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || g.pruned() || p->comps > 1 ||
+        p->boxed() || p->embedded())
         return false;
     if (g.ny != g.nz || !zy_fused_length(ilog2_exact(g.ny))) return false;
     // the fused stage reads and writes the blocked hand-over layout of the x pass
@@ -710,8 +729,8 @@ static int fuse_zy(dfft_plan_s* p, Step zs, const Step& ys, const char* label, c
 constexpr size_t BATCH_SMALL_MIN = 2;
 static bool batch_small(const dfft_plan_s* p, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || p->comps > 1 || p->boxed() ||
-        p->embedded())
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || g.pruned() || p->comps > 1 ||
+        p->boxed() || p->embedded())
         return false;
     if (g.nx != g.ny || g.ny != g.nz || !batch_small_length(ilog2_exact(g.nx))) return false;
     return p->batch >= BATCH_SMALL_MIN && p->batch * g.nx <= 0x7fffffff;
@@ -780,9 +799,11 @@ static int new_pass(dfft_plan_s* p, int inverse, PassKind kind, size_t n, int ax
     // Bluestein lengths: the view mapping stays the kind's; the exec launches the Bluestein kernel.  Type-I R2R passes:
     // log2 N of their N +- 1 reals per line
     s.log2n = pass_log2(kind, n, s.r2r);
-    {   // padded plans: the spectral extent of the axis
+    {   // padded plans: the spectral extent of the axis; pruned plans: its data extent
         const size_t k = axis == 0 ? g.kx : axis == 1 ? g.ky : g.kzc, full = axis == 0 ? g.nx : axis == 1 ? g.ny : g.nzc;
         if (k != full) s.keep = k;
+        const size_t m = axis == 0 ? g.mx : axis == 1 ? g.my : g.mz, phys = axis == 0 ? g.nx : axis == 1 ? g.ny : g.nz;
+        if (m != phys) s.data = m;
     }
     if (s.log2n < 1 || s.log2n > MAX_LOG2N)
         return fail(DFFT_ERR_UNSUPPORTED, "axis length " + std::to_string(n) + " is not a supported power of two (2..8192)");
@@ -809,7 +830,7 @@ static Step new_rendezvous(int group, int phase_id, const char* phase, int strea
 // The blocked hand-over of the second transposition: the scattering pass (forward the y pass, inverse the x pass) stores
 // into the slots of its G2 members, the gathering pass (forward x, inverse y) reads its own.  A receiver's nz columns of z
 // are laid out as
-//   forward  [nzm/CH][nx][ny_q][CH] + tail [nx][ny_q][rem]      (ny_q: the receiver's y rows)
+//   forward  [nzm/CH][mx][ny_q][CH] + tail [mx][ny_q][rem]      (ny_q: the receiver's y rows; mx: the data's x planes)
 //   inverse  [nzm/CH][ky][nx_q][CH] + tail [nx_q][ky][rem]      (nx_q: the receiver's x planes)
 // with rem = nz % CH leftover columns and nzm = nz - rem, so the rows a tile of the scattering pass sends to one receiver
 // are adjacent (one contiguous run per receiver: what NVLink stores need), and the gathering pass reads rows CH apart.
@@ -837,7 +858,7 @@ struct HandOver {
         fwd = !inverse;
         es = p->esize * p->comps;
         nz = g.sz.size[g.pj(me)];
-        L = fwd ? g.nx : g.ky;
+        L = fwd ? g.mx : g.ky;
         recv = fwd ? &g.oy : &g.sx;
         M_me = recv->size[g.pi(me)];
         G = &p->grp[2];
@@ -1038,15 +1059,16 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
 
     if (p->any_direct) sc.steps.push_back(new_rendezvous(0, 0, nullptr, 0));  // everyone has left the previous exec: slots are free
 
-    // spectral extents (padded plans: K; the pass lengths stay the physical N)
-    const size_t kzc = g.kzc, ky = g.ky, kx = g.kx;
+    // spectral extents (padded plans: K; the pass lengths stay the physical N) and data extents (pruned plans: M, the
+    // physical side of the axes not yet transformed).  Z_Then_YX: rows of the y-pass planes in its slots (zyx_rows).
+    const size_t kzc = g.kzc, ky = g.ky, kx = g.kx, mx = g.mx, my = g.my;
     const bool zyx = g.decomp == DFFT_SLAB_Z_THEN_YX;
     const bool zy = zy_fused(p, inverse, d);  // one fused launch for the z and y passes
     int rc;
 
     // sizes of this rank
     const size_t nx_i = g.sx.size[pi], x0_i = g.sx.start[pi];
-    const size_t ny_j = zyx ? g.ny : g.sy.size[pj];
+    const size_t ny_j = zyx ? my : g.sy.size[pj];
     const size_t nz_j = zyx ? g.sz.size[me] : g.sz.size[pj];
     const size_t oy_i = zyx ? ky : g.oy.size[pi], oy0_i = zyx ? 0 : g.oy.start[pi];
 
@@ -1080,7 +1102,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         }
         // transposition 1: scatter along z over G1; dest q holds [nx][ny][nz_q] (Z_Then_YX: x split -> z split) or, a pencil
         // row, [nx_i][ny][nz_q]
-        const Transposition t1 = zyx ? Transposition(p, 1, AZ, AX, g.sz, g.sx, g.ny, tab_z, tab_x)
+        const Transposition t1 = zyx ? Transposition(p, 1, AZ, AX, g.sz, g.sx, g.zyx_rows(), tab_z, tab_x)
                                      : Transposition(p, 1, AZ, AY, g.sz, g.sy, nx_i, tab_z, tab_y_in);
         s1.prm.out = t1.send({AX, AY, AZ});
         if (g.decomp == DFFT_SLAB_ZY_THEN_X) s1.phase = nullptr;
@@ -1089,7 +1111,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
 
         // pass 2: y (tiled): a0 = x, n = y, b = z in nz_j
         Step s2;
-        const size_t nx2 = zyx ? g.nx : nx_i;  // x extent held after transposition 1
+        const size_t nx2 = zyx ? mx : nx_i;  // x extent held after transposition 1
         rc = new_pass(p, inverse, PASS_C2C_TILED, g.ny, 1, g.decomp == DFFT_SLAB_ZY_THEN_X ? "2D FFT Y-Z-Direction" : (zyx ? nullptr : "1D FFT Y-Direction"), s2);
         if (rc) return rc;
         s2.label = "y pass";
@@ -1103,7 +1125,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
                 return DFFT_SUCCESS;
             }
             // z_then_yx: y pass in place (padded: its Ky output rows keep the input's strides, the first Ky * nz_j elements of
-            // every x plane), then x pass into the caller's out
+            // every x plane; pruned: My input rows, Ky output rows, planes of zyx_rows), then x pass into the caller's out
             s2.prm.out = s2.prm.in;
             if (s2.prm.in.nseg != 1) return fail(DFFT_ERR_STATE, "internal: z_then_yx gather view");
             sc.steps.push_back(s2);
@@ -1112,7 +1134,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
             if (rc) return rc;
             s3.label = "x pass";
             s3.prm.A0 = 1; s3.prm.A1 = 1; s3.prm.B = int(ky * nz_j);
-            s3.prm.in = single_view(s2.prm.in.seg[0].base, 0, 0, (long long)(g.ny * nz_j));
+            s3.prm.in = single_view(s2.prm.in.seg[0].base, 0, 0, (long long)(g.zyx_rows() * nz_j));
             s3.prm.out = single_view(nullptr, 0, 0, (long long)(ky * nz_j));
             s3.out_user = 2;
             sc.steps.push_back(s3);
@@ -1192,7 +1214,7 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     if (zyx) {
         // input [nx][ny][nz_me]: y pass (to a slot), x pass scattering along x to the owners of x (dest q holds
         // [nx_q][ny][kzc]), then z inverse on [nx_me][ny][kzc].
-        const Transposition t1(p, 1, AX, AZ, g.sx, g.sz, g.ny, tab_x, tab_z);
+        const Transposition t1(p, 1, AX, AZ, g.sx, g.sz, my, tab_x, tab_z);
         Step sy_;
         rc = new_pass(p, inverse, PASS_C2C_TILED, g.ny, 1, nullptr, sy_);
         if (rc) return rc;
@@ -1204,23 +1226,23 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         sy_.prm.A0 = int(kx); sy_.prm.B = int(nz_j);
         sy_.prm.in = single_view(nullptr, (long long)(ky * nz_j), 0, (long long)nz_j);
         sy_.in_user = 1;
-        sy_.prm.out = single_view(p->slot(no_x ? p->slots.D1 : W, me), (long long)(g.ny * nz_j), 0, (long long)nz_j);
+        sy_.prm.out = single_view(p->slot(no_x ? p->slots.D1 : W, me), (long long)(my * nz_j), 0, (long long)nz_j);
         sc.steps.push_back(sy_);
         Step sx_;
         rc = new_pass(p, inverse, PASS_C2C_TILED, g.nx, 0, "2D FFT Y-X-Direction", sx_);
         if (rc) return rc;
         sx_.label = "x pass";
-        sx_.prm.A0 = 1; sx_.prm.A1 = int(g.ny); sx_.prm.B = int(nz_j);
-        sx_.prm.in = single_view(p->slot(W, me), 0, (long long)nz_j, (long long)(g.ny * nz_j));
+        sx_.prm.A0 = 1; sx_.prm.A1 = int(my); sx_.prm.B = int(nz_j);
+        sx_.prm.in = single_view(p->slot(W, me), 0, (long long)nz_j, (long long)(my * nz_j));
         sx_.prm.out = t1.send({NO_AXIS, AY, AX});
         if (!no_x) sc.steps.push_back(sx_);
         t1.finish(sc);
         Step sz_;
         rc = new_pass(p, inverse, zkind, zlen, 2, "1D FFT Z-Direction", sz_);
         if (rc) return rc;
-        sz_.prm.A0 = int(nx_i); sz_.prm.A1 = int(g.ny);
+        sz_.prm.A0 = int(nx_i); sz_.prm.A1 = int(my);
         sz_.prm.in = t1.recv({AX, AY, AZ});
-        sz_.prm.out = single_view(nullptr, zpitch_out * (long long)g.ny, zpitch_out, 1);
+        sz_.prm.out = single_view(nullptr, zpitch_out * (long long)my, zpitch_out, 1);
         sz_.out_user = 2;
         sc.steps.push_back(sz_);
         return DFFT_SUCCESS;
@@ -1878,9 +1900,9 @@ static cudaError_t run_pass_step(const dfft_plan_s* p, const Schedule& sc, const
                 e = launch_copy_pass(p->prec, is_r2r(p->g.transform), s.kind, s.n, prm, scale, ss);
             } else {
                 const size_t n = s.n ? s.n : size_t(1) << s.log2n;
-                int hole[2];
-                pass_hole(s.kind, n, s.keep, hole);
-                e = launch_fft_pass(p->prec, s.kind, n, prm, s.blu, scale, ss, s.r2r, s.keep ? hole : nullptr);
+                int hole[4];
+                pass_hole(s.kind, n, s.keep, s.data, hole);
+                e = launch_fft_pass(p->prec, s.kind, n, prm, s.blu, scale, ss, s.r2r, s.keep || s.data ? hole : nullptr);
             }
             break;
         case KERNEL_ZY_FUSED: e = launch_zy_fused(p->prec, s.log2n, prm, prm_y, s.zyf, scale, ss); break;
@@ -2443,9 +2465,8 @@ static int embed_views(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
         if (s.type != STEP_PASS) continue;
         if (s.kernel != KERNEL_PASS) return fail(DFFT_ERR_STATE, "internal: embedded plans run single passes");
         // points along n of each view, as dfft_debug_run_step counts them
-        const size_t len = s.n ? s.n : size_t(1) << s.log2n;
-        const size_t in_len = s.keep && s.prm.inverse ? s.keep : len + (s.kind == PASS_C2R ? 1 : 0);
-        const size_t out_len = s.keep && !s.prm.inverse ? s.keep : len + (s.kind == PASS_R2C ? 1 : 0);
+        size_t in_len = 0, out_len = 0;
+        s.view_lens(&in_len, &out_len);
         const int rc = embed_pass(s.prm, s.in_user, s.out_user, Ein, Eout, p->esize, in_len, out_len);
         if (rc) return rc;
     }
@@ -2738,11 +2759,13 @@ int dfft_plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, in
 }  // extern "C"
 
 // kinds: of the plans of dfft_plan_create_r2r (their transform is DFFT_DCT, DFFT_DST or DFFT_R2HC), nullptr otherwise.
-// spectral: Kx, Ky, Kz of the plans of dfft_plan_create_padded (checked there), nullptr otherwise.
+// spectral: Kx, Ky, Kz of the plans of dfft_plan_create_padded and _pruned (checked there), nullptr otherwise.
+// data: Mx, My, Mz of the plans of dfft_plan_create_pruned (checked there), nullptr otherwise.
 static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
                        size_t nz, size_t p1, size_t p2, size_t batch, bool inplace, int allocate, dfft_plan_t* plan,
                        const int* kinds = nullptr, const size_t* spectral = nullptr, size_t comps = 1,
-                       const std::vector<dfft::Box>* in_boxes = nullptr, const std::vector<dfft::Box>* out_boxes = nullptr) {
+                       const std::vector<dfft::Box>* in_boxes = nullptr, const std::vector<dfft::Box>* out_boxes = nullptr,
+                       const size_t* data = nullptr) {
     if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
     if (batch == 0) return fail(DFFT_ERR_INVALID, "batch must be at least 1");
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
@@ -2767,7 +2790,8 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
     p->comps = comps;
     p->tabs.prec = precision;
     p->tabs.dry = dry;
-    if (!p->g.init(decomp, transform, nx, ny, nz, p1, p2, p->P, spectral ? spectral[0] : 0, spectral ? spectral[1] : 0, spectral ? spectral[2] : 0)) {
+    if (!p->g.init(decomp, transform, nx, ny, nz, p1, p2, p->P, spectral ? spectral[0] : 0, spectral ? spectral[1] : 0, spectral ? spectral[2] : 0,
+                   data ? data[0] : 0, data ? data[1] : 0, data ? data[2] : 0)) {
         delete p;
         return fail(DFFT_ERR_INVALID, "invalid partition: P1*P2 must equal the communicator size");
     }
@@ -3017,19 +3041,49 @@ int dfft_plan_create_boxes(dfft_comm_t comm, const dfft_config* config, int deco
                        in_boxes ? &boxes[0] : nullptr, out_boxes ? &boxes[1] : nullptr);
 }
 
+// The checks of padded and pruned plans: sizes[0..2] the spectral (what = "spectral") or data (what = "data") grid
+static int check_sub_grid(int transform, size_t nx, size_t ny, size_t nz, const size_t sizes[3], const char* what) {
+    const bool spectral = what[0] == 's';
+    if (transform == DFFT_DCT || transform == DFFT_DST)
+        return fail(DFFT_ERR_UNSUPPORTED, spectral ? "padded plans are C2C or R2C / C2R" : "pruned plans are C2C or R2C / C2R");
+    if (transform != DFFT_C2C && transform != DFFT_R2C) return fail(DFFT_ERR_INVALID, "bad transform");
+    const size_t n[3] = {nx, ny, nz};
+    for (int a = 0; a < 3; ++a) {
+        if (sizes[a] == 0 || sizes[a] > n[a])
+            return fail(DFFT_ERR_INVALID, std::string(what) + " size " + std::to_string(sizes[a]) + " of axis " + "xyz"[a] + " must be in [1, " +
+                                              std::to_string(n[a]) + "]");
+        if (sizes[a] < n[a] && ilog2_exact(n[a]) < 0)
+            return fail(DFFT_ERR_UNSUPPORTED, std::string("axis ") + "xyz"[a] + " of length " + std::to_string(n[a]) + " is not a power of two: its " +
+                                                  what + " size must be its length");
+    }
+    return DFFT_SUCCESS;
+}
+
 int dfft_plan_create_padded(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
                             size_t nz, size_t kx, size_t ky, size_t kz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan) {
-    if (transform == DFFT_DCT || transform == DFFT_DST) return fail(DFFT_ERR_UNSUPPORTED, "padded plans are C2C or R2C / C2R");
-    if (transform != DFFT_C2C && transform != DFFT_R2C) return fail(DFFT_ERR_INVALID, "bad transform");
-    const size_t n[3] = {nx, ny, nz}, k[3] = {kx, ky, kz};
-    for (int a = 0; a < 3; ++a) {
-        if (k[a] == 0 || k[a] > n[a])
-            return fail(DFFT_ERR_INVALID, "spectral size " + std::to_string(k[a]) + " of axis " + "xyz"[a] + " must be in [1, " + std::to_string(n[a]) + "]");
-        if (k[a] < n[a] && ilog2_exact(n[a]) < 0)
-            return fail(DFFT_ERR_UNSUPPORTED, std::string("axis ") + "xyz"[a] + " of length " + std::to_string(n[a]) +
-                                                  " is not a power of two: its spectral size must be its length");
-    }
+    const size_t k[3] = {kx, ky, kz};
+    if (int rc = check_sub_grid(transform, nx, ny, nz, k, "spectral")) return rc;
     return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, false, allocate, plan, nullptr, k);
+}
+
+// Pruned plans (DESIGN.md section 3.19): the data block [0, M) of each axis, zero beyond, and the spectrum of a padded plan.
+int dfft_plan_create_pruned(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
+                            size_t nz, const size_t data[3], const size_t spectral[3], size_t p1, size_t p2, size_t batch, int allocate,
+                            dfft_plan_t* plan) {
+    const size_t m[3] = {data ? data[0] : nx, data ? data[1] : ny, data ? data[2] : nz};
+    const size_t k[3] = {spectral ? spectral[0] : nx, spectral ? spectral[1] : ny, spectral ? spectral[2] : nz};
+    if (int rc = check_sub_grid(transform, nx, ny, nz, m, "data")) return rc;
+    if (int rc = check_sub_grid(transform, nx, ny, nz, k, "spectral")) return rc;
+    // the real side of R2C / C2R moves as pairs of reals (the z pass's complex units)
+    if (transform == DFFT_R2C && m[2] % 2) return fail(DFFT_ERR_UNSUPPORTED, "R2C / C2R pruned plans need an even data size along z");
+    return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, false, allocate, plan, nullptr, k, 1, nullptr,
+                       nullptr, m);
+}
+
+int dfft_plan_get_data_size(dfft_plan_t p, size_t m[3]) {
+    if (!p || !m) return fail(DFFT_ERR_INVALID, "null plan / size");
+    m[0] = p->g.mx; m[1] = p->g.my; m[2] = p->g.mz;
+    return DFFT_SUCCESS;
 }
 
 // C values per point: the C = 1 plan with every element widened to C consecutive values (DESIGN.md section 3.14).  The
@@ -3211,6 +3265,8 @@ int dfft_plan_set_transform_axes(dfft_plan_t p, const int transform[3]) {
     if (p->g.transform == DFFT_R2C && !transform[2]) return fail(DFFT_ERR_INVALID, "R2C / C2R plans transform z (it turns reals into complex)");
     if (p->g.padded() && !(transform[0] && transform[1] && transform[2]))
         return fail(DFFT_ERR_UNSUPPORTED, "padded plans transform every axis");
+    if (p->g.pruned() && !(transform[0] && transform[1] && transform[2]))
+        return fail(DFFT_ERR_UNSUPPORTED, "pruned plans transform every axis");
     if (p->comps > 1 && !(transform[0] && transform[1] && transform[2]))
         return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans transform every axis");
     // schedules, tuned choices and captured graphs are built for the axes of their time
@@ -3243,6 +3299,7 @@ int dfft_plan_set_strides(dfft_plan_t p, const long long in_strides[3], const lo
     }
     if (p->inplace) return fail(DFFT_ERR_UNSUPPORTED, "in-place plans keep the padded layout of FFTW and cuFFT: strides are for out-of-place plans");
     if (p->comps > 1) return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans keep their [x][y][z][C] layout: strides are for plans of one component");
+    if (p->g.pruned()) return fail(DFFT_ERR_UNSUPPORTED, "pruned plans read and write dense data blocks: strides are for plans without a data size");
     if (p->axes_fixed) return fail(DFFT_ERR_STATE, "set the strides before the first exec, dfft_plan_tune or dfft_plan_describe");
     p->in_embedded = in_strides != nullptr;
     p->out_embedded = out_strides != nullptr;
@@ -3419,6 +3476,7 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
         p->tune_report = is_r2r(p->g.transform) ? "sequential schedule (no alternatives for this plan: DCT / DST plans run the sequential schedule)"
                          : !all_axes(p)         ? "sequential schedule (no alternatives for this plan: plans with a kept axis run the sequential schedule)"
                          : p->g.padded()        ? "sequential schedule (no alternatives for this plan: padded plans run the sequential schedule)"
+                         : p->g.pruned()        ? "sequential schedule (no alternatives for this plan: pruned plans run the sequential schedule)"
                          : p->comps > 1         ? "sequential schedule (no alternatives for this plan: interleaved plans run the sequential schedule)"
                          : p->boxed()           ? "sequential schedule (no alternatives for this plan: box plans run the sequential schedule)"
                          : p->embedded()        ? "sequential schedule (no alternatives for this plan: plans with strides run the sequential schedule)"
@@ -3564,6 +3622,8 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
                                        std::to_string(p->taxes[2]) + "]") +
                     (p->g.padded() ? ",\"spectral\":[" + std::to_string(p->g.kx) + "," + std::to_string(p->g.ky) + "," + std::to_string(p->g.kz) + "]"
                                    : std::string()) +
+                    (p->g.pruned() ? ",\"data\":[" + std::to_string(p->g.mx) + "," + std::to_string(p->g.my) + "," + std::to_string(p->g.mz) + "]"
+                                   : std::string()) +
                     (p->comps > 1 ? ",\"components\":" + std::to_string(p->comps) : std::string()) +
                     json_boxes("in_boxes", p->in_boxes) + json_boxes("out_boxes", p->out_boxes) +
                     json_strides("in_strides", p->in_embedded, p->in_strides) + json_strides("out_strides", p->out_embedded, p->out_strides) +
@@ -3677,7 +3737,8 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
                  (per_axis && !copy ? std::string(",\"r2r\":\"") + r2r_name(s_.r2r) + "\"" : std::string()) +
                  ",\"log2n\":" + std::to_string(s_.log2n) +
                  (s_.bluestein() || copy ? ",\"n\":" + std::to_string(s_.n) : std::string()) +
-                 (s_.keep ? ",\"keep\":" + std::to_string(s_.keep) : std::string()) + ",\"A0\":" + std::to_string(s_.prm.A0) +
+                 (s_.keep ? ",\"keep\":" + std::to_string(s_.keep) : std::string()) +
+                 (s_.data ? ",\"data\":" + std::to_string(s_.data) : std::string()) + ",\"A0\":" + std::to_string(s_.prm.A0) +
                  ",\"A1\":" + std::to_string(s_.prm.A1) + ",\"B\":" + std::to_string(s_.prm.B) + ",\"inverse\":" + std::to_string(s_.prm.inverse) +
                  ",\"in_user\":" + std::to_string(s_.in_user) + ",\"out_user\":" + std::to_string(s_.out_user) + ",\"in\":";
             json_view(o, s_.prm.in, p->tabs);
@@ -3876,10 +3937,10 @@ int dfft_debug_run_step(dfft_plan_t p, int inverse, int d, size_t field, int ste
         }
         return DFFT_SUCCESS;
     };
-    // points along n of each view: padded passes hold `keep` on their spectral side (out forward, in inverse)
-    // (the interleaved R2C / C2R pass: Nz reals, Nz / 2 + 1 complex points)
-    size_t in_len = s.keep && s.prm.inverse ? s.keep : len + (s.kind == PASS_C2R ? 1 : 0);
-    size_t out_len = s.keep && !s.prm.inverse ? s.keep : len + (s.kind == PASS_R2C ? 1 : 0);
+    // points along n of each view: padded passes hold `keep` on their spectral side and pruned passes `data` on their
+    // physical side (the interleaved R2C / C2R pass: Nz reals, Nz / 2 + 1 complex points)
+    size_t in_len = 0, out_len = 0;
+    s.view_lens(&in_len, &out_len);
     if (s.kind == PASS_R2C_ILV) out_len = len / 2 + 1;
     if (s.kind == PASS_C2R_ILV) in_len = len / 2 + 1;
     const size_t es = p->esize;

@@ -254,8 +254,12 @@ cudaError_t launch_padded(PassKind kind, const FftPadded& p, cudaStream_t stream
     constexpr int LOG2E = S::LOG2E;
     const long long lines = (long long)p.A0 * p.A1;
     if (lines <= 0) return cudaSuccess;
-    const int points = (1 << LOG2N) + (kind == PASS_R2C || kind == PASS_C2R ? 1 : 0);  // of the spectral side's line
-    if (p.lo < 0 || p.hi < p.lo || p.hi > points) return cudaErrorInvalidValue;
+    // points of the loaded and the stored side's line: the spectral side of R2C / C2R has one more
+    const bool half = kind == PASS_R2C || kind == PASS_C2R;
+    const int n_ld = (1 << LOG2N) + (kind == PASS_C2R ? 1 : 0), n_st = (1 << LOG2N) + (kind == PASS_R2C ? 1 : 0);
+    if (p.ld_lo < 0 || p.ld_hi < p.ld_lo || p.ld_hi > n_ld || p.st_lo < 0 || p.st_hi < p.st_lo || p.st_hi > n_st) return cudaErrorInvalidValue;
+    // the R2C / C2R twins test k < lo only: their holes reach the end of the line
+    if (half && (p.ld_hi != n_ld || p.st_hi != n_st)) return cudaErrorInvalidValue;
     const long long grid = (lines + S::TBC - 1) / S::TBC;  // CONTIG, R2C and C2R
     switch (kind) {
         case PASS_C2C_CONTIG: {

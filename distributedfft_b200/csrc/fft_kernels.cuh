@@ -388,15 +388,20 @@ struct MemScaled {
     __device__ __forceinline__ void st(cx<T>* p, cx<T> v) const { m.st(p, cscale<T>(v, s)); }
 };
 
-// ---- padded passes (dfft_plan_create_padded) ----------------------------------------------------------------
-// A padded pass transforms N-point lines whose spectral side keeps K of the N points: the forward pass never stores the
-// hole [lo, hi) of the line and the inverse pass reads it as zero without a load.  Position p outside the hole is element
-// m = p (p < lo) or p - (hi - lo) of the spectral view, so the spectral view and its segment table are those of a K-point
-// axis.  The padded twins take the scale at run time (one instantiation per precision and length).
+// ---- padded and pruned passes (dfft_plan_create_padded, dfft_plan_create_pruned) ---------------------------------------
+// A padded pass transforms N-point lines whose spectral side keeps K of the N points, a pruned pass lines whose physical
+// side holds M of them, zero beyond.  Each side has a hole [lo, hi) of the line: the pass reads its loaded side's hole as
+// zero without a load and never stores its stored side's hole.  Position p outside a hole is element m = p (p < lo) or
+// p - (hi - lo) of that side's view, so the view and its segment table are those of a K- (M-) point axis.  Forward the
+// loaded side is the physical one, inverse the spectral one.  The padded twins take the scale at run time (one
+// instantiation per precision and length).
 struct FftPadded : FftScaled {
-    int lo, hi;  // hole of the N-point line (C2C: [ceil(K/2), ceil(K/2) + N - K); R2C / C2R: [K/2 + 1, N/2 + 1))
+    // Spectral hole: C2C [ceil(K/2), ceil(K/2) + N - K), R2C / C2R [K/2 + 1, N/2 + 1).  Physical hole: C2C [M, N), R2C / C2R
+    // the pairs [M/2, N/2).  Empty when lo == hi.
+    int ld_lo, ld_hi;  // of the loaded side
+    int st_lo, st_hi;  // of the stored side
 };
-// spectral index of line position n, -1 in the hole
+// index in the view of line position n, -1 in the hole
 __device__ __forceinline__ int keep_index(int n, int lo, int hi) { return n < lo ? n : (n < hi ? -1 : n - (hi - lo)); }
 
 // store policy of the padded twins: plain stores, scaled when s != 1 (a runtime value)
@@ -412,12 +417,14 @@ struct MemRtScaled {
 __device__ __forceinline__ void l2_discard(const void* p) { asm volatile("discard.global.L2 [%0], 128;" ::"l"(p) : "memory"); }
 
 // ---- one tile of a C2C pass: load, CtaFft::stages, store --------------------------------------------------
-// PADDED: the spectral side (out forward, in inverse) keeps the line positions outside the hole [lo, hi) (FftPadded).
+// PADDED: the loaded side keeps the line positions outside the hole [ld_lo, ld_hi), the stored side those outside
+// [st_lo, st_hi) (FftPadded); a side with an empty hole takes the plain path.
 // ILV (CONTIG mapping): lines of an interleaved z pass, strided by sN along n (TileCoord)
 template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, typename M, typename Hook = NoGatherHook, bool PADDED = false,
           bool ILV = false>
 __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<T>* sm, unsigned long long* tab_in, unsigned long long* tab_out,
-                                         bool multi, const M& mem, const Hook& after_gather = {}, int lo = 0, int hi = 0) {
+                                         bool multi, const M& mem, const Hook& after_gather = {}, int ld_lo = 0, int ld_hi = 0, int st_lo = 0,
+                                         int st_hi = 0) {
     using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
     using LA = LineAccess<T, C::LINES>;
     using TC = TileCoord<C, TILED, TB, ILV>;
@@ -440,10 +447,10 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
 
     cx<T> v[E];
     if (tc.valid) {
-        if constexpr (PADDED && INV) {
+        if (PADDED && ld_lo < ld_hi) {
 #pragma unroll
             for (int e = 0; e < E; ++e) {
-                const int m = keep_index(j + e * TPL, lo, hi);
+                const int m = keep_index(j + e * TPL, ld_lo, ld_hi);
                 v[e] = m < 0 ? cx<T>{T(0), T(0)} : mem.ld(STRIDED ? in.at(m) : in.at1(m));
             }
         } else if (!in.multi) {
@@ -474,11 +481,12 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
     C::template stages<0>(v, j, t, sm, reinterpret_cast<const cx<T>*>(p.tw), after_gather);
 
     if (tc.valid) {
-        if constexpr (PADDED && !INV) {
+        if (PADDED && st_lo < st_hi) {
 #pragma unroll
             for (int e = 0; e < E; ++e) {
-                const int m = keep_index(j + e * TPL, lo, hi);
-                if (m >= 0) mem.st(STRIDED ? out.at(m) : out.at1(m), v[C::Core::final_slot(e)]);
+                const int m = keep_index(j + e * TPL, st_lo, st_hi);
+                const cx<T> x = v[C::Core::final_slot(e)];
+                if (m >= 0) mem.st(STRIDED ? out.at(m) : out.at1(m), INV ? cswap(x) : x);
             }
         } else if (!out.multi) {
             if constexpr (!STRIDED) {
@@ -666,7 +674,8 @@ fft_c2c_padded_kernel(const __grid_constant__ FftPadded p) {
     unsigned long long* tab_out = tab_in + C::LINES * MAXSEG;
     const bool multi = p.in.nseg > 1 || p.out.nseg > 1;
     c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV, MemRtScaled<T>, NoGatherHook, true>(p, blockIdx.x, sm, tab_in, tab_out, multi,
-                                                                                 MemRtScaled<T>{p.scale != 1.0, T(p.scale)}, {}, p.lo, p.hi);
+                                                                                 MemRtScaled<T>{p.scale != 1.0, T(p.scale)}, {}, p.ld_lo, p.ld_hi,
+                                                                                 p.st_lo, p.st_hi);
 }
 
 // ---- mbarrier of an asynchronous tile copy (fft_c2c_tma_kernel, fft_zy_fused_kernel) ------------------------------
@@ -1402,7 +1411,8 @@ __device__ __forceinline__ cx<T> shfl_cx(cx<T> v, int src_lane) {
 // ---- R2C pass (CONTIG): real line of 2M points -> M+1 complex points ------------------------------------
 // The real line is read as M complex points z[m] = x[2m] + i x[2m+1], transformed with the length-M
 // core and split into even/odd spectra in shared memory:  X[k] = Xe[k] + W_2M^k Xo[k].
-// PADDED (P = FftPadded): the points k >= p.lo are not stored; the scale is p.scale at run time.
+// PADDED (P = FftPadded): the pairs m >= p.ld_lo read as zero, the points k >= p.st_lo are not stored; the scale is
+// p.scale at run time.
 template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED, bool PADDED, typename P>
 __device__ __forceinline__ void r2c_lines(const P& p) {
     using C = CtaFft<T, LOG2M, LOG2E, TB, false>;
@@ -1426,7 +1436,10 @@ __device__ __forceinline__ void r2c_lines(const P& p) {
     if (valid) {
         const cx<T>* q = in.p0 + j;
 #pragma unroll
-        for (int e = 0; e < E; ++e) v[e] = ld_elem<T>(q + e * TPL);
+        for (int e = 0; e < E; ++e) {
+            if constexpr (PADDED) v[e] = j + e * TPL < p.ld_lo ? ld_elem<T>(q + e * TPL) : cx<T>{T(0), T(0)};
+            else v[e] = ld_elem<T>(q + e * TPL);
+        }
     } else {
 #pragma unroll
         for (int e = 0; e < E; ++e) v[e] = cx<T>{T(0), T(0)};
@@ -1453,8 +1466,8 @@ __device__ __forceinline__ void r2c_lines(const P& p) {
         if (valid) {
             if constexpr (PADDED) {
                 const MemRtScaled<T> mem{p.scale != 1.0, T(p.scale)};
-                if (k < p.lo) mem.st(out.at1(k), cadd(xe, tt));
-                if (M - k < p.lo) mem.st(out.at1(M - k), cconj(csub(xe, tt)));
+                if (k < p.st_lo) mem.st(out.at1(k), cadd(xe, tt));
+                if (M - k < p.st_lo) mem.st(out.at1(M - k), cconj(csub(xe, tt)));
             } else if constexpr (SCALED) {
                 st_elem<T>(out.at1(k), cscale<T>(cadd(xe, tt), T(p.scale)));
                 st_elem<T>(out.at1(M - k), cscale<T>(cconj(csub(xe, tt)), T(p.scale)));
@@ -1475,7 +1488,7 @@ fft_r2c_kernel(const __grid_constant__ KParams<SCALED> p) {
     r2c_lines<T, LOG2M, LOG2E, TB, SCALED, false>(p);
 }
 
-// padded twin of fft_r2c_kernel: keeps the points k < p.lo (p.hi = M + 1)
+// padded twin of fft_r2c_kernel: reads the pairs m < p.ld_lo (p.ld_hi = M), keeps the points k < p.st_lo (p.st_hi = M + 1)
 template <typename T, int LOG2M, int LOG2E, int TB>
 __global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
 fft_r2c_padded_kernel(const __grid_constant__ FftPadded p) {
@@ -1483,8 +1496,8 @@ fft_r2c_padded_kernel(const __grid_constant__ FftPadded p) {
 }
 
 // ---- C2R pass (CONTIG): M+1 complex points -> real line of 2M points, unnormalised -----------------------
-// PADDED (P = FftPadded): the points k >= p.lo read as zero, their partner loads X[M - k] as well; the scale is p.scale at
-// run time.
+// PADDED (P = FftPadded): the points k >= p.ld_lo read as zero, their partner loads X[M - k] as well; the pairs
+// m >= p.st_lo are not stored; the scale is p.scale at run time.
 template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED, bool PADDED, typename P>
 __device__ __forceinline__ void c2r_lines(const P& p) {
     using C = CtaFft<T, LOG2M, LOG2E, TB, false>;
@@ -1516,8 +1529,8 @@ __device__ __forceinline__ void c2r_lines(const P& p) {
         if (valid) {
             if constexpr (PADDED) {
 #pragma unroll
-                for (int e = 0; e < E; ++e) xk[e] = j + e * TPL < p.lo ? ld_elem<T>(in.at1(j + e * TPL)) : cx<T>{T(0), T(0)};
-                if (j == 0 && M < p.lo) xM = ld_elem<T>(in.at1(M));
+                for (int e = 0; e < E; ++e) xk[e] = j + e * TPL < p.ld_lo ? ld_elem<T>(in.at1(j + e * TPL)) : cx<T>{T(0), T(0)};
+                if (j == 0 && M < p.ld_lo) xM = ld_elem<T>(in.at1(M));
             } else {
 #pragma unroll
                 for (int e = 0; e < E; ++e) xk[e] = ld_elem<T>(in.at1(j + e * TPL));
@@ -1549,8 +1562,8 @@ __device__ __forceinline__ void c2r_lines(const P& p) {
         cx<T> xk{T(0), T(0)}, xm{T(0), T(0)};
         if (valid) {
             if constexpr (PADDED) {
-                if (k < p.lo) xk = ld_elem<T>(in.at1(k));
-                if (M - k < p.lo) xm = cconj(ld_elem<T>(in.at1(M - k)));
+                if (k < p.ld_lo) xk = ld_elem<T>(in.at1(k));
+                if (M - k < p.ld_lo) xm = cconj(ld_elem<T>(in.at1(M - k)));
             } else {
                 xk = ld_elem<T>(in.at1(k));
                 xm = cconj(ld_elem<T>(in.at1(M - k)));
@@ -1574,7 +1587,9 @@ __device__ __forceinline__ void c2r_lines(const P& p) {
         cx<T>* q = out.p0 + j;
 #pragma unroll
         for (int e = 0; e < E; ++e) {
-            if constexpr (PADDED) MemRtScaled<T>{p.scale != 1.0, T(p.scale)}.st(q + e * TPL, cswap(v[C::Core::final_slot(e)]));
+            if constexpr (PADDED) {
+                if (j + e * TPL < p.st_lo) MemRtScaled<T>{p.scale != 1.0, T(p.scale)}.st(q + e * TPL, cswap(v[C::Core::final_slot(e)]));
+            }
             else if constexpr (SCALED) st_elem<T>(q + e * TPL, cscale<T>(cswap(v[C::Core::final_slot(e)]), T(p.scale)));
             else st_elem<T>(q + e * TPL, cswap(v[C::Core::final_slot(e)]));
         }
@@ -1587,7 +1602,8 @@ fft_c2r_kernel(const __grid_constant__ KParams<SCALED> p) {
     c2r_lines<T, LOG2M, LOG2E, TB, SCALED, false>(p);
 }
 
-// padded twin of fft_c2r_kernel: the points k >= p.lo are zero (p.hi = M + 1)
+// padded twin of fft_c2r_kernel: the points k >= p.ld_lo are zero (p.ld_hi = M + 1), the pairs m >= p.st_lo are not stored
+// (p.st_hi = M)
 template <typename T, int LOG2M, int LOG2E, int TB>
 __global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
 fft_c2r_padded_kernel(const __grid_constant__ FftPadded p) {
@@ -2130,7 +2146,8 @@ cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStr
 cudaError_t launch_pass(int prec, int log2n, PassKind kind, const FftParams& p, double scale, cudaStream_t stream);
 
 // padded pass (FftPadded): kind PASS_C2C_CONTIG, PASS_C2C_TILED, PASS_R2C or PASS_C2R over the views of launch_pass, the
-// hole [p.lo, p.hi) of each line on its spectral side (out forward, in inverse); p.scale scales the stores.
+// hole [p.ld_lo, p.ld_hi) of each line on its loaded side and [p.st_lo, p.st_hi) on its stored side (R2C / C2R: both reach
+// the end of the line); p.scale scales the stores.
 template <typename T, int LOG2N>
 cudaError_t launch_padded(PassKind kind, const FftPadded& p, cudaStream_t stream);
 cudaError_t launch_padded(int prec, int log2n, PassKind kind, const FftPadded& p, cudaStream_t stream);

@@ -72,6 +72,10 @@ struct Geometry {
     // every other plan.  An axis is padded by the pass that transforms it: the layout after d stages has K on the first d
     // axes in z, y, x order.
     size_t kx = 0, ky = 0, kz = 0, kzc = 0;
+    // physical extents of the data (dfft_plan_create_pruned): the field holds Mx x My x Mz points at [0, M) of each axis,
+    // zero beyond; nx, ny, nz for every other plan.  The mirror of K: the layout after d stages has M on the axes not yet
+    // transformed, and the physical x (pencil: y) split is made over M.
+    size_t mx = 0, my = 0, mz = 0;
     int P = 1, P1 = 1, P2 = 1;
     // x split of the input (over P1, or over P for both slab sequences)
     Split sx;
@@ -80,9 +84,10 @@ struct Geometry {
     // y split of the output over P1 (slab zy_x: over P)
     Split oy;
 
-    // returns false on an invalid partition.  kx_, ky_, kz_: the spectral grid (0: the physical one)
+    // returns false on an invalid partition.  kx_, ky_, kz_: the spectral grid, mx_, my_, mz_: the data (0: the physical
+    // grid)
     bool init(int decomp_, int transform_, size_t nx_, size_t ny_, size_t nz_, size_t p1, size_t p2, int nranks, size_t kx_ = 0, size_t ky_ = 0,
-              size_t kz_ = 0) {
+              size_t kz_ = 0, size_t mx_ = 0, size_t my_ = 0, size_t mz_ = 0) {
         decomp = decomp_; transform = transform_;
         nx = nx_; ny = ny_; nz = nz_;
         const bool real_z = !(transform == DFFT_C2C || transform == DFFT_DCT || transform == DFFT_DST || transform == DFFT_R2HC);
@@ -91,6 +96,9 @@ struct Geometry {
         ky = ky_ ? ky_ : ny;
         kz = kz_ ? kz_ : nz;
         kzc = real_z ? kz / 2 + 1 : kz;
+        mx = mx_ ? mx_ : nx;
+        my = my_ ? my_ : ny;
+        mz = mz_ ? mz_ : nz;
         P = nranks;
         if (decomp == DFFT_SLAB_ZY_THEN_X) { P1 = P; P2 = 1; }
         else if (decomp == DFFT_SLAB_Z_THEN_YX) { P1 = P; P2 = 1; }  // P1 only used for the x split
@@ -98,19 +106,20 @@ struct Geometry {
         else return false;
         if (P1 < 1 || P2 < 1 || size_t(P1) * size_t(P2) != size_t(P)) return false;
         if (nx == 0 || ny == 0 || nz == 0) return false;
-        sx.make(nx, P1);
+        sx.make(mx, P1);
         if (decomp == DFFT_SLAB_Z_THEN_YX) {
-            sy.make(ny, 1);
+            sy.make(my, 1);
             sz.make(kzc, P);
             oy.make(ky, 1);
         } else {
-            sy.make(ny, P2);
+            sy.make(my, P2);
             sz.make(kzc, P2);
             oy.make(ky, P1);
         }
         return true;
     }
     bool padded() const { return kx != nx || ky != ny || kz != nz; }
+    bool pruned() const { return mx != nx || my != ny || mz != nz; }
     int pi(int rank) const { return decomp == DFFT_PENCIL ? rank / P2 : rank; }
     int pj(int rank) const { return decomp == DFFT_PENCIL ? rank % P2 : 0; }
 
@@ -119,10 +128,10 @@ struct Geometry {
         const int i = pi(rank), j = pj(rank);
         if (decomp == DFFT_SLAB_Z_THEN_YX) {
             if (which <= 1) {
-                size[0] = sx.size[i]; size[1] = ny; size[2] = which == 0 ? nz : kzc;
+                size[0] = sx.size[i]; size[1] = my; size[2] = which == 0 ? mz : kzc;
                 start[0] = sx.start[i]; start[1] = 0; start[2] = 0;
             } else {
-                size[0] = which == 2 ? nx : kx; size[1] = ky; size[2] = sz.size[rank];
+                size[0] = which == 2 ? mx : kx; size[1] = ky; size[2] = sz.size[rank];
                 start[0] = 0; start[1] = 0; start[2] = sz.start[rank];
             }
             return;
@@ -130,7 +139,7 @@ struct Geometry {
         switch (which) {
             case 0:
             case 1:
-                size[0] = sx.size[i]; size[1] = sy.size[j]; size[2] = which == 0 ? nz : kzc;
+                size[0] = sx.size[i]; size[1] = sy.size[j]; size[2] = which == 0 ? mz : kzc;
                 start[0] = sx.start[i]; start[1] = sy.start[j]; start[2] = 0;
                 break;
             case 2:
@@ -144,8 +153,11 @@ struct Geometry {
         }
     }
     // complex elements of the largest per-rank stage array (the reference's domainsize / sizeof(C_t),
-    // mpicufft_slab.cpp:132).  Padded plans have two more: the y pass' physical side [x_i][Ny][z_j] and the x pass' physical
-    // side (Z_Then_YX: [Nx][Ny][z_r]; otherwise [Nx][y_i][z_j], y spectral); in every other plan they are layouts 2 and 3.
+    // mpicufft_slab.cpp:132).  Padded and pruned plans have more: the y pass' physical side [x_i][My][z_j] and the x pass'
+    // physical side [Mx][y_i][z_j] (y spectral).  Z_Then_YX holds its y and x passes in one slot of [X][Y][z_r] planes, X
+    // and Y the larger of M and K (the forward y pass runs in place, from My to Ky rows; the inverse one from Kx planes),
+    // and its first transposition moves zyx_rows rows per x plane.
+    // In every other plan they are layouts 2 and 3.
     size_t domain_elems(int rank) const {
         size_t m = 0;
         for (int w = 1; w <= 3; ++w) {
@@ -153,11 +165,13 @@ struct Geometry {
             layout(rank, w, s, o);
             m = std::max(m, s[0] * s[1] * s[2]);
         }
-        const size_t zr = decomp == DFFT_SLAB_Z_THEN_YX ? sz.size[rank] : sz.size[pj(rank)];
-        const size_t xr = decomp == DFFT_SLAB_Z_THEN_YX ? nx : sx.size[pi(rank)];
-        const size_t yr = decomp == DFFT_SLAB_Z_THEN_YX ? ny : oy.size[pi(rank)];
-        return std::max(m, std::max(xr * ny * zr, nx * yr * zr));
+        if (decomp == DFFT_SLAB_Z_THEN_YX)  // and the all-to-all staging of the z pass's output, [x_i][zyx_rows][Kzc]
+            return std::max(m, std::max(std::max(mx, kx) * zyx_rows() * sz.size[rank], sx.size[pi(rank)] * zyx_rows() * kzc));
+        const size_t zr = sz.size[pj(rank)];
+        return std::max(m, std::max(sx.size[pi(rank)] * my * zr, mx * oy.size[pi(rank)] * zr));
     }
+    // Z_Then_YX: rows of the y-pass planes in its slot, both sides of the in-place forward y pass (My in, Ky out)
+    size_t zyx_rows() const { return std::max(my, ky); }
 };
 
 }  // namespace dfft

@@ -147,7 +147,7 @@ class MPIcuFFT:
     # -- plan ------------------------------------------------------------------------------------
     def initFFT(self, global_size: GlobalSize, partition: Optional[Partition] = None, allocate: bool = True, batch: int = 1,
                 inplace: bool = False, transform_axes: Optional[Sequence[bool]] = None, spectral: Optional[Sequence[int]] = None,
-                components: int = 1, in_boxes=None, out_boxes=None, in_strides=None, out_strides=None):
+                components: int = 1, in_boxes=None, out_boxes=None, in_strides=None, out_strides=None, data: Optional[Sequence[int]] = None):
         """`batch` (not in the reference): every exec transforms that many fields, back to back in each buffer — a
         contiguous [batch, X, Y, Z] tensor; the getters describe one field (dfft_plan_create_batched).
         `inplace` (dfft_plan_create_inplace): every exec gets the same buffer twice and overwrites its input; fields are
@@ -166,7 +166,11 @@ class MPIcuFFT:
         `in_strides` / `out_strides` (field, x, y) (dfft_plan_set_strides): the buffers of the physical side / of the output
         of d = 3 lie inside larger arrays, e.g. the interior A[h:-h, h:-h, h:-h] of a field with ghost cells, whose strides
         these are (torch's .stride(), in elements: reals on the real side of R2C / C2R and for R2R plans); such a side then
-        takes exactly those non-contiguous tensors.  None keeps a side dense."""
+        takes exactly those non-contiguous tensors.  None keeps a side dense.
+        `data` (mx, my, mz) (dfft_plan_create_pruned): a pruned plan, global_size the transform grid and the field an
+        [mx, my, mz] block at the origin, zero beyond — the forward reads only the block, the inverse stores only it (the
+        doubled grid of free-space solvers).  The physical side of every exec is this rank's m-block; combines with
+        `spectral`.  Pruned plans are out of place, C2C or R2C, with one component and no boxes or strides."""
         if global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         cfg = _lib.dfft_config(int(self.config.cuda_aware), int(self.config.warmup_rounds), int(self.config.comm_method),
@@ -178,7 +182,16 @@ class MPIcuFFT:
         if self._decomp == PENCIL and partition is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         h = C.c_void_p()
-        if in_boxes is not None or out_boxes is not None:
+        if data is not None:
+            if inplace or self.kinds is not None or components != 1 or in_boxes is not None or out_boxes is not None:
+                raise ValueError("pruned plans are out of place, C2C or R2C, with one component and no boxes")
+            if batch < 1:
+                raise ValueError("batch must be at least 1")
+            m = (C.c_size_t * 3)(*(int(v) for v in data))
+            k = None if spectral is None else (C.c_size_t * 3)(*(int(v) for v in spectral))
+            check(lib().dfft_plan_create_pruned(self.comm._h, C.byref(cfg), self._decomp, self.precision, self.transform, global_size.Nx,
+                                                global_size.Ny, global_size.Nz, m, k, p1, p2, batch, 1 if allocate else 0, C.byref(h)))
+        elif in_boxes is not None or out_boxes is not None:
             if inplace or spectral is not None or components != 1 or self.kinds is not None:
                 raise ValueError("box plans are out of place, not padded, with one component and one transform kind for all axes")
             if batch < 1:
@@ -387,6 +400,7 @@ class MPIcuFFT:
     def getPartialStart(self, d): return self._triple(lib().dfft_get_partial_start, d)
     def getDomainSize(self): return int(lib().dfft_get_domain_size(self._h))
     def getSpectralSize(self): return self._triple(lib().dfft_plan_get_spectral_size)
+    def getDataSize(self): return self._triple(lib().dfft_plan_get_data_size)
     def getBatch(self): return int(lib().dfft_get_batch(self._h))
     def getComponents(self): return int(lib().dfft_get_components(self._h))
     def isInPlace(self): return bool(lib().dfft_plan_is_inplace(self._h))
@@ -459,14 +473,14 @@ class MPIcuFFT_Pencil(MPIcuFFT):
     _decomp = PENCIL
 
     def initFFT(self, global_size, partition=None, allocate=True, batch=1, inplace=False, transform_axes=None, spectral=None, components=1,
-                in_boxes=None, out_boxes=None, in_strides=None, out_strides=None):
+                in_boxes=None, out_boxes=None, in_strides=None, out_strides=None, data=None):
         if partition is None or global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         if partition.P1 * partition.P2 != self.comm.size:
             raise RuntimeError("Invalid Input Partition!")
         self.partition = partition
         super().initFFT(global_size, partition, allocate, batch, inplace, transform_axes, spectral, components, in_boxes, out_boxes, in_strides,
-                        out_strides)
+                        out_strides, data)
 
     def getPartitionDimensions(self):
         """(input_dim, transposed_dim, output_dim), each a dict with size_x/y/z and start_x/y/z lists

@@ -226,6 +226,31 @@ int dfft_plan_create_padded(dfft_comm_t comm, const dfft_config* config, int dec
                             size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan);
 /* k[0..2] = kx, ky, kz of a padded plan; nx, ny, nz for every other plan. */
 int dfft_plan_get_spectral_size(dfft_plan_t plan, size_t k[3]);
+/* Pruned plans (PFFT's pruned FFTs, the doubled grid of Hockney-Eastwood free-space solvers): a transform grid of
+ * nx x ny x nz points whose physical field holds data = (mx, my, mz) points, 1 <= m <= n per axis, at line positions
+ * [0, m) of each axis; everything from m to n - 1 is zero and is never stored in a caller buffer.  spectral = (kx, ky, kz)
+ * means what it means for dfft_plan_create_padded.  Either pointer may be NULL, which means (nx, ny, nz).
+ *   - Forward: the n-point transform of the zero-embedded field; only the kept spectral modes are stored.  Inverse: the
+ *     unnormalised inverse of the (zero-embedded) spectrum; only positions [0, m) of each axis are stored.
+ *   - The physical side of every exec (the forward input, the inverse output) is an m-block [x_i][my][mz] (R2C / C2R:
+ *     mz reals per row).  The physical x split (pencil: also the y split) is made over mx (my), not nx, so that every
+ *     rank holds data.  The layout after d stages has K on the first d axes in z, y, x order and m on the others; the
+ *     getters, dfft_get_domain_size, dfft_get_work_size_device and batch distances follow.
+ *   - Batch, output scale, partial d, Peer2Peer / All2All, the timer and graph capture of one-rank _async execs work as
+ *     for other plans.  Plans with some m < n run the sequential schedule (dfft_plan_tune has no alternative).
+ *     dfft_plan_describe reports "data": [mx, my, mz] and "data": m on every pass whose physical side holds m < n points.
+ *   - data = (nx, ny, nz) or NULL makes the plan of dfft_plan_create_padded with the same spectral (of
+ *     dfft_plan_create_batched when both are full): the same steps, description and output.
+ *   - An m of 0 or above n, a data split that leaves a rank without data, transform 4, or the spectral arguments that
+ *     dfft_plan_create_padded rejects: DFFT_ERR_INVALID.  DFFT_DCT / DFFT_DST, m < n on an axis whose length is not a power
+ *     of two, or an odd mz on R2C / C2R: DFFT_ERR_UNSUPPORTED.
+ *   - No in-place, boxed or interleaved form; dfft_plan_set_transform_axes other than {1, 1, 1} and
+ *     dfft_plan_set_strides on a plan with some m < n: DFFT_ERR_UNSUPPORTED. */
+int dfft_plan_create_pruned(dfft_comm_t comm, const dfft_config* config, int decomp /*dfft_decomp*/, int precision /*dfft_prec*/,
+                            int transform /*dfft_transform*/, size_t nx, size_t ny, size_t nz, const size_t data[3],
+                            const size_t spectral[3], size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan);
+/* m[0..2] = mx, my, mz of a pruned plan; nx, ny, nz for every other plan. */
+int dfft_plan_get_data_size(dfft_plan_t plan, size_t m[3]);
 /* Interleaved multi-component plans (FFTW-MPI's `howmany`): every grid point holds `components` consecutive values,
  * and each component is transformed on its own.
  *   - Every caller layout is that of the components = 1 plan with each element widened to C = components consecutive

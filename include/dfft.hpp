@@ -106,6 +106,15 @@ public:
         spectral_ = spectral;
         initFFT(global_size, partition, allocate, batch);
     }
+    // not in the reference: a pruned plan (dfft_plan_create_pruned): global_size is the transform grid, data the Mx x My x Mz
+    // block of the field at the origin (zero beyond: the forward reads only it, the inverse stores only it), spectral the
+    // spectrum it keeps (null: all of it), 1 <= M, K <= N per axis
+    void initFFT(GlobalSize* global_size, GlobalSize* data, GlobalSize* spectral, Partition* partition, bool allocate = true, size_t batch = 1) {
+        struct Reset { GlobalSize*& d; GlobalSize*& s; ~Reset() { d = nullptr; s = nullptr; } } reset{data_, spectral_};
+        data_ = data;
+        spectral_ = spectral;
+        initFFT(global_size, partition, allocate, batch);
+    }
     // not in the reference: an interleaved plan (dfft_plan_create_interleaved): every grid point holds `components`
     // consecutive values, each component transformed on its own ([x][y][z][C] buffers).  A named method, so that it cannot
     // be mistaken for the (batch, inplace) overload.
@@ -126,6 +135,8 @@ public:
     }
     // kx, ky, kz of a padded plan; Nx, Ny, Nz of every other plan
     void getSpectralSize(size_t* k) const { DFFT_CALL(dfft_plan_get_spectral_size(plan, k)); }
+    // mx, my, mz of a pruned plan; Nx, Ny, Nz of every other plan
+    void getDataSize(size_t* m) const { DFFT_CALL(dfft_plan_get_data_size(plan, m)); }
     size_t getBatch() const { return dfft_get_batch(plan); }
     bool isInPlace() const { return dfft_plan_is_inplace(plan) != 0; }
     // not in the reference: output scale of every forward / inverse exec (dfft_plan_set_scale; after initFFT).  For
@@ -179,7 +190,12 @@ protected:
         else if (components_ != 1)
             DFFT_CALL(dfft_plan_create_interleaved(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, p1, p2,
                                                    components_, batch_, allocate ? 1 : 0, &plan));
-        else if (spectral_)
+        else if (data_) {
+            const size_t m[3] = {data_->Nx, data_->Ny, data_->Nz};
+            const size_t k[3] = {spectral_ ? spectral_->Nx : gs->Nx, spectral_ ? spectral_->Ny : gs->Ny, spectral_ ? spectral_->Nz : gs->Nz};
+            DFFT_CALL(dfft_plan_create_pruned(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, m, k, p1, p2, batch_,
+                                              allocate ? 1 : 0, &plan));
+        } else if (spectral_)
             DFFT_CALL(dfft_plan_create_padded(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, spectral_->Nx, spectral_->Ny,
                                               spectral_->Nz, p1, p2, batch_, allocate ? 1 : 0, &plan));
         else if (per_axis)
@@ -197,7 +213,8 @@ protected:
     }
     size_t batch_ = 1;       // fields of the plan initFFT is creating
     bool inplace_ = false;   // whether initFFT is creating an in-place plan
-    GlobalSize* spectral_ = nullptr;  // the spectrum of the padded plan initFFT is creating
+    GlobalSize* spectral_ = nullptr;  // the spectrum of the padded (or pruned) plan initFFT is creating
+    GlobalSize* data_ = nullptr;      // the data block of the pruned plan initFFT is creating
     size_t components_ = 1;  // values per point of the interleaved plan initFFTInterleaved is creating
     const size_t* in_boxes_ = nullptr;   // the boxes of the box plan initFFT is creating
     const size_t* out_boxes_ = nullptr;
