@@ -1,6 +1,7 @@
 """Build libdfft.so (sm_90a) in-tree with nvcc.  `python -m distributedfft_b200.build` or build.build().
 
-The kernel instantiations (one translation unit per precision x log2 length) are compiled in parallel;
+The kernel instantiations (one translation unit per precision x log2 length, and per 16-bit format x log2 length) are
+compiled in parallel;
 objects are cached under distributedfft_b200/csrc/build/ keyed by source mtimes.
 """
 from __future__ import annotations
@@ -69,6 +70,11 @@ def build(verbose: bool = False, force: bool = False, defines=(), out: str = LIB
         for l in range(1, MAX_LOG2N + 1):
             obj = os.path.join(OBJ_, f"fft_inst_{tname}_{l}.o")
             jobs.append((inst, obj, [f"-DDFFT_T={tname}", f"-DDFFT_LOG2N={l}", *defines], [inst, *headers]))
+    # the passes of 16-bit plans: f32 arithmetic, one unit per stored format and length
+    for sname, stype in (("half", "__half"), ("bf16", "__nv_bfloat16")):
+        for l in range(1, MAX_LOG2N + 1):
+            obj = os.path.join(OBJ_, f"fft_inst_{sname}_{l}.o")
+            jobs.append((inst, obj, ["-DDFFT_T=float", f"-DDFFT_S={stype}", f"-DDFFT_LOG2N={l}", *defines], [inst, *headers]))
     for name in ("fft_dispatch.cu", "dfft_plan.cu"):
         src = os.path.join(CSRC, name)
         jobs.append((src, os.path.join(OBJ_, name.replace(".cu", ".o")), list(defines), [src, *headers]))

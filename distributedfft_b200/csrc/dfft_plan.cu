@@ -102,7 +102,8 @@ static cudaError_t make_bluestein_table(size_t n, void** dev) {
 // Lengths of C2C axes: powers of two in [2, 2^MAX_LOG2N] (the power-of-two kernels) and any length in [3, BLUESTEIN_MAX_N]
 // (the Bluestein pass)
 static bool bluestein_length(size_t n) { return ilog2_exact(n) < 0 && n >= 3 && n <= size_t(BLUESTEIN_MAX_N); }
-static bool c2c_length(size_t n) { return (ilog2_exact(n) >= 1 && ilog2_exact(n) <= MAX_LOG2N) || bluestein_length(n); }
+static bool pow2_length(size_t n) { return ilog2_exact(n) >= 1 && ilog2_exact(n) <= MAX_LOG2N; }
+static bool c2c_length(size_t n) { return pow2_length(n) || bluestein_length(n); }
 // Real-to-real plans: powers of two in [2, 2^MAX_LOG2N].  The transform of a plan from dfft_plan_create_r2r is DFFT_DCT or
 // DFFT_DST when all three kinds are that one, DFFT_R2HC for any other combination (its kinds are in dfft_plan_s::kinds).
 static bool is_r2r(int transform) { return transform == DFFT_DCT || transform == DFFT_DST || transform == DFFT_R2HC; }
@@ -188,6 +189,10 @@ static void pass_hole(PassKind kind, size_t n, size_t keep, size_t data, int hol
     hole[2] = int(data ? (half ? data / 2 : data) : n);
     hole[3] = int(n);
 }
+
+// 16-bit plans (DFFT_F16, DFFT_BF16; DESIGN.md section 3.20): 4-byte complex elements, f32 arithmetic, the sequential schedule
+static bool is_half(int prec) { return prec == DFFT_F16 || prec == DFFT_BF16; }
+static int refuse_half(const std::string& what) { return fail(DFFT_ERR_UNSUPPORTED, what + " have no 16-bit storage (DFFT_F16 / DFFT_BF16)"); }
 
 // Passes over an axis the plan keeps (dfft_plan_set_transform_axes): the views of the FFT pass they replace, no transform
 static bool is_copy(PassKind kind) { return kind == PASS_COPY_CONTIG || kind == PASS_COPY_TILED; }
@@ -447,6 +452,11 @@ struct Step {
     // a copy whose input and output views are the same elements, kept because it stores final values: it only has work to
     // do when the output scale is not 1, and is not launched otherwise (drop_identity_copies)
     bool identity = false;
+    // 16-bit plans (split_scale): an FFT pass stores its values times |s|^(share_num / share_den) of the direction's scale s
+    // (log2 of its axis length over the sum for the exec's transformed axes), and times the sign of s when `sign`; share_den
+    // 0: never scaled (copy passes, other precisions)
+    int share_num = 0, share_den = 0;
+    bool sign = false;
 };
 
 struct Schedule {
@@ -655,7 +665,7 @@ static bool all_axes(const dfft_plan_s* p) { return p->taxes[0] && p->taxes[1] &
 // box that is not the natural layout: their reshape steps wrap the sequential schedule (wrap_boxes).  And embedded plans
 // (dfft_plan_set_strides): the other forms read and write dense caller arrays, and every rank must run the same form.
 static bool alt_schedules(const dfft_plan_s* p) {
-    return pow2_axes(p) && !is_r2r(p->g.transform) && all_axes(p) && !p->g.padded() && !p->g.pruned() && p->comps == 1 && !p->boxed() &&
+    return pow2_axes(p) && !is_half(p->prec) && !is_r2r(p->g.transform) && all_axes(p) && !p->g.padded() && !p->g.pruned() && p->comps == 1 && !p->boxed() &&
            !p->embedded();
 }
 
@@ -673,7 +683,7 @@ static long long z_row_pitch(const dfft_plan_s* p) {
 // three passes are L2-resident already and gain nothing.
 static bool zy_fused(const dfft_plan_s* p, int inverse, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || g.pruned() || p->comps > 1 ||
+    if (p->P != 1 || is_half(p->prec) || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || g.pruned() || p->comps > 1 ||
         p->boxed() || p->embedded())
         return false;
     if (g.ny != g.nz || !zy_fused_length(ilog2_exact(g.ny))) return false;
@@ -729,7 +739,7 @@ static int fuse_zy(dfft_plan_s* p, Step zs, const Step& ys, const char* label, c
 constexpr size_t BATCH_SMALL_MIN = 2;
 static bool batch_small(const dfft_plan_s* p, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || g.pruned() || p->comps > 1 ||
+    if (p->P != 1 || is_half(p->prec) || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || g.pruned() || p->comps > 1 ||
         p->boxed() || p->embedded())
         return false;
     if (g.nx != g.ny || g.ny != g.nz || !batch_small_length(ilog2_exact(g.nx))) return false;
@@ -1880,14 +1890,43 @@ static void user_view(View& v, int which, const Schedule& sc, size_t f, void* ou
     if (which == 2) v.seg[0].base = (char*)out + f * sc.field_out + (size_t)v.seg[0].base;
 }
 
+// 16-bit plans: the factor f_a the FFT pass step s multiplies its stores by, float(|s|^(log2 n_a / L)) of the direction's
+// scale s, negative on the passes of the exec's last FFT axis when s is; 1 for copy passes and for s = 1
+static double step_factor(const dfft_plan_s* p, const Schedule& sc, const Step& s) {
+    const double sc_ = p->scale[sc.inverse];
+    if (s.share_den == 0 || sc_ == 1.0) return 1.0;
+    // exact for powers of two: log2 |s| * num / den of s = 1/N is -log2 n_a
+    const double m = sc_ == 0.0 ? 0.0 : std::exp2(std::log2(std::fabs(sc_)) * s.share_num / s.share_den);
+    return double(float(s.sign && sc_ < 0 ? -m : m));
+}
+
+// 16-bit plans: the output scale split over the exec's FFT passes (step_factor), so that an FP16 intermediate grows no more
+// than the scaled result does.  L sums log2 n_a over the axes the schedule transforms (log2 Nz for the R2C z axis); the
+// steps of its last FFT axis carry the sign.
+static void split_scale(const dfft_plan_s* p, Schedule& sc) {
+    const size_t n[3] = {p->g.nx, p->g.ny, p->g.nz};
+    bool on[3] = {false, false, false};
+    int last = -1, L = 0;
+    for (const Step& s : sc.steps)
+        if (s.type == STEP_PASS && !is_copy(s.kind)) { on[s.axis] = true; last = s.axis; }
+    for (int a = 0; a < 3; ++a) L += on[a] ? ilog2_exact(n[a]) : 0;
+    for (Step& s : sc.steps) {
+        if (s.type != STEP_PASS || is_copy(s.kind)) continue;
+        s.share_num = ilog2_exact(n[s.axis]);
+        s.share_den = L;
+        s.sign = s.axis == last;
+    }
+}
+
 // Enqueues PASS step s of sc for field f on ss: the copy, FFT, fused or batched kernel over its views, its stores scaled by
 // the direction's output scale when they are final values.  An in-place copy onto itself with nothing to scale is not
 // launched (*launched = false).
 static cudaError_t run_pass_step(const dfft_plan_s* p, const Schedule& sc, const Step& s, size_t f, void* out, const void* in, cudaStream_t ss,
                                  bool* launched) {
     *launched = false;
-    if (s.identity && p->scale[sc.inverse] == 1.0) return cudaSuccess;
-    const double scale = s.final_store ? p->scale[sc.inverse] : 1.0;
+    const bool half = is_half(p->prec);
+    if (s.identity && (half || p->scale[sc.inverse] == 1.0)) return cudaSuccess;  // 16-bit plans never scale a copy
+    const double scale = half ? step_factor(p, sc, s) : s.final_store ? p->scale[sc.inverse] : 1.0;
     FftParams prm = s.prm, prm_y = s.prm_y;
     user_view(prm.in, s.in_user, sc, f, out, in);
     user_view(prm.out, s.out_user, sc, f, out, in);
@@ -2518,6 +2557,7 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
         // and the fused and batched stages (whose earlier phase writes only the work area, or `out` inside the same launch).
         // tests/test_scale.py replays every such schedule and checks that each output value is scaled exactly once.
         for (Step& s : sc.steps) s.final_store = s.type == STEP_PASS && s.out_user == 2;
+        if (is_half(p->prec)) split_scale(p, sc);
         // In place the buffer also holds intermediates: its views from slot D1 are marked after the final stores.
         // tests/test_inplace.py replays these schedules on one address range.
         if (p->buf_slot) relocate_buffer_views(p, sc);
@@ -2768,9 +2808,14 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
                        const size_t* data = nullptr) {
     if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
     if (batch == 0) return fail(DFFT_ERR_INVALID, "batch must be at least 1");
-    if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
+    if (precision < DFFT_F32 || precision > DFFT_BF16) return fail(DFFT_ERR_INVALID, "bad precision");
     if (transform != DFFT_R2C && transform != DFFT_C2C && !is_r2r(transform)) return fail(DFFT_ERR_INVALID, "bad transform");
     if (transform == DFFT_R2HC && !kinds) return fail(DFFT_ERR_INVALID, "bad transform (per-axis kinds: dfft_plan_create_r2r)");
+    if (is_half(precision)) {
+        if (is_r2r(transform)) return refuse_half("DCT / DST plans");
+        if (transform == DFFT_C2C && !(pow2_length(nx) && pow2_length(ny) && pow2_length(nz)))
+            return fail(DFFT_ERR_UNSUPPORTED, "16-bit storage (DFFT_F16 / DFFT_BF16) takes power-of-two lengths in [2, 8192] only (no Bluestein pass)");
+    }
     const bool dry = comm->dry;
     if (!dry) CK_CUDA(cudaSetDevice(comm->device));
     const auto t_init0 = std::chrono::steady_clock::now();
@@ -2786,7 +2831,7 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
     p->rank = comm->rank; p->P = comm->nranks;
     p->prec = precision;
     for (int a = 0; a < 3; ++a) p->kinds[a] = kinds ? kinds[a] : is_r2r(transform) ? transform : 0;
-    p->esize = (precision == DFFT_F64 ? 16 : 8) / (is_r2r(transform) ? 2 : 1);  // DCT / DST: real elements
+    p->esize = (precision == DFFT_F64 ? 16 : is_half(precision) ? 4 : 8) / (is_r2r(transform) ? 2 : 1);  // DCT / DST: real elements
     p->comps = comps;
     p->tabs.prec = precision;
     p->tabs.dry = dry;
@@ -3016,6 +3061,7 @@ int dfft_plan_is_inplace(dfft_plan_t p) { return p && p->inplace ? 1 : 0; }
 int dfft_plan_create_boxes(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny, size_t nz,
                            size_t p1, size_t p2, const size_t* in_boxes, const size_t* out_boxes, size_t batch, int allocate, dfft_plan_t* plan) {
     if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
+    if (is_half(precision)) return refuse_half("box plans");
     if (transform != DFFT_C2C && transform != DFFT_R2C && transform != DFFT_DCT && transform != DFFT_DST)
         return fail(DFFT_ERR_INVALID, "box plans are C2C, R2C / C2R, DCT or DST");
     const size_t P = size_t(comm->nranks);
@@ -3062,6 +3108,7 @@ static int check_sub_grid(int transform, size_t nx, size_t ny, size_t nz, const 
 int dfft_plan_create_padded(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
                             size_t nz, size_t kx, size_t ky, size_t kz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan) {
     const size_t k[3] = {kx, ky, kz};
+    if (is_half(precision)) return refuse_half("padded plans");
     if (int rc = check_sub_grid(transform, nx, ny, nz, k, "spectral")) return rc;
     return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, false, allocate, plan, nullptr, k);
 }
@@ -3072,6 +3119,7 @@ int dfft_plan_create_pruned(dfft_comm_t comm, const dfft_config* config, int dec
                             dfft_plan_t* plan) {
     const size_t m[3] = {data ? data[0] : nx, data ? data[1] : ny, data ? data[2] : nz};
     const size_t k[3] = {spectral ? spectral[0] : nx, spectral ? spectral[1] : ny, spectral ? spectral[2] : nz};
+    if (is_half(precision)) return refuse_half("pruned plans");
     if (int rc = check_sub_grid(transform, nx, ny, nz, m, "data")) return rc;
     if (int rc = check_sub_grid(transform, nx, ny, nz, k, "spectral")) return rc;
     // the real side of R2C / C2R moves as pairs of reals (the z pass's complex units)
@@ -3092,6 +3140,7 @@ int dfft_plan_get_data_size(dfft_plan_t p, size_t m[3]) {
 constexpr size_t MAX_COMPONENTS = 64;
 int dfft_plan_create_interleaved(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
                                  size_t nz, size_t p1, size_t p2, size_t components, size_t batch, int allocate, dfft_plan_t* plan) {
+    if (is_half(precision)) return refuse_half("interleaved plans");
     if (components == 0) return fail(DFFT_ERR_INVALID, "components must be at least 1");
     if (components > MAX_COMPONENTS) return fail(DFFT_ERR_UNSUPPORTED, "at most " + std::to_string(MAX_COMPONENTS) + " components per point");
     if (components > 1) {
@@ -3114,6 +3163,7 @@ int dfft_plan_get_spectral_size(dfft_plan_t p, size_t k[3]) {
 
 int dfft_plan_create_r2r(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, const int kinds[3], size_t nx, size_t ny,
                          size_t nz, size_t p1, size_t p2, size_t batch, int inplace, int allocate, dfft_plan_t* plan) {
+    if (is_half(precision)) return refuse_half("real-to-real plans");
     if (!kinds) return fail(DFFT_ERR_INVALID, "null kinds");
     for (int a = 0; a < 3; ++a)
         if (!is_r2r_kind(kinds[a]))
@@ -3281,6 +3331,7 @@ int dfft_plan_get_transform_axes(dfft_plan_t p, int transform[3]) {
 }
 int dfft_plan_set_strides(dfft_plan_t p, const long long in_strides[3], const long long out_strides[3]) {
     if (!p) return fail(DFFT_ERR_INVALID, "null plan");
+    if (is_half(p->prec)) return refuse_half("plans with strides");
     const char* const names[2] = {"in_strides", "out_strides"};
     const long long* const given[2] = {in_strides, out_strides};
     for (int side = 0; side < 2; ++side) {
@@ -3473,7 +3524,8 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
     }
     p->tune_report.clear();
     if (cands.size() == 1) {
-        p->tune_report = is_r2r(p->g.transform) ? "sequential schedule (no alternatives for this plan: DCT / DST plans run the sequential schedule)"
+        p->tune_report = is_half(p->prec)       ? "sequential schedule (no alternatives for this plan: 16-bit plans run the sequential schedule)"
+                         : is_r2r(p->g.transform) ? "sequential schedule (no alternatives for this plan: DCT / DST plans run the sequential schedule)"
                          : !all_axes(p)         ? "sequential schedule (no alternatives for this plan: plans with a kept axis run the sequential schedule)"
                          : p->g.padded()        ? "sequential schedule (no alternatives for this plan: padded plans run the sequential schedule)"
                          : p->g.pruned()        ? "sequential schedule (no alternatives for this plan: pruned plans run the sequential schedule)"
@@ -3612,6 +3664,7 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
     const bool per_axis = p->g.transform == DFFT_R2HC;
     const bool uniform = p->kinds[0] == p->kinds[1] && p->kinds[1] == p->kinds[2];
     std::string o = "{\"rank\":" + std::to_string(p->rank) + ",\"esize\":" + std::to_string(p->esize) + (p->inplace ? ",\"inplace\":true" : "") +
+                    (is_half(p->prec) ? std::string(",\"precision\":\"") + (p->prec == DFFT_F16 ? "f16" : "bf16") + "\"" : std::string()) +
                     // "mixed" when the axes differ; per-axis plans also list the kinds, and each R2R pass its own below
                     (is_r2r(p->g.transform) ? std::string(",\"r2r\":\"") + (uniform ? r2r_name(p->kinds[0]) : "mixed") + "\"" : std::string()) +
                     (per_axis ? std::string(",\"r2r_kinds\":[\"") + r2r_name(p->kinds[0]) + "\",\"" + r2r_name(p->kinds[1]) + "\",\"" +
@@ -3746,7 +3799,14 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
             json_view(o, s_.prm.out, p->tabs);
             // the scale as the kernels apply it (f32 plans: rounded to float)
             const double scale = p->prec == DFFT_F32 ? double(float(p->scale[sc.inverse])) : p->scale[sc.inverse];
-            if (s_.final_store && p->scale[sc.inverse] != 1.0) {
+            // 16-bit plans: the pass's share of the scale instead (step_factor), under its own key
+            const double factor = is_half(p->prec) ? step_factor(p, sc, s_) : 1.0;
+            if (factor != 1.0) {
+                char num[40];
+                snprintf(num, sizeof num, "%.17g", factor);
+                o += std::string(",\"factor\":") + num;
+            }
+            if (s_.final_store && p->scale[sc.inverse] != 1.0 && !is_half(p->prec)) {
                 char num[40];
                 snprintf(num, sizeof num, "%.17g", scale);
                 o += std::string(",\"scale\":") + num;
@@ -3805,7 +3865,8 @@ static int fft1d_pass(int prec, PassKind kind, size_t n, FftParams prm, void* st
 
 int dfft_fft1d_contig(int precision, int kind, int direction, size_t n, size_t lines, void* out, size_t out_pitch, const void* in,
                       size_t in_pitch, void* stream) {
-    if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
+    if (precision < DFFT_F32 || precision > DFFT_BF16) return fail(DFFT_ERR_INVALID, "bad precision");
+    if (is_half(precision) && kind == 0 && !pow2_length(n)) return fail(DFFT_ERR_UNSUPPORTED, "16-bit storage takes power-of-two lengths only");
     if (kind < 0 || kind > 2) return fail(DFFT_ERR_INVALID, "bad kind");
     const size_t len = kind == 0 ? n : n / 2;
     const int l2 = ilog2_exact(len);
@@ -3823,7 +3884,8 @@ int dfft_fft1d_contig(int precision, int kind, int direction, size_t n, size_t l
 }
 
 int dfft_fft1d_strided(int precision, int direction, size_t a, size_t n, size_t b, void* out, const void* in, void* stream) {
-    if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
+    if (precision < DFFT_F32 || precision > DFFT_BF16) return fail(DFFT_ERR_INVALID, "bad precision");
+    if (is_half(precision) && !pow2_length(n)) return fail(DFFT_ERR_UNSUPPORTED, "16-bit storage takes power-of-two lengths only");
     if (!c2c_length(n)) return fail(DFFT_ERR_UNSUPPORTED, "length must be a power of two in [2, 8192] or any length in [3, 4096]");
     FftParams prm{};
     prm.A0 = int(a); prm.A1 = 1; prm.B = int(b);
@@ -3834,6 +3896,7 @@ int dfft_fft1d_strided(int precision, int direction, size_t a, size_t n, size_t 
 }
 
 int dfft_fft1d_r2r(int precision, int transform, int direction, size_t n, size_t a, size_t b, void* out, const void* in, void* stream) {
+    if (is_half(precision)) return refuse_half("real-to-real transforms");
     if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
     if (!is_r2r_kind(transform))
         return fail(DFFT_ERR_INVALID, "transform must be DFFT_DCT, DFFT_DST, DFFT_R2HC, DFFT_DCT1, DFFT_DST1, DFFT_DCT4 or DFFT_DST4");
@@ -3860,7 +3923,8 @@ int dfft_fft1d_r2r(int precision, int transform, int direction, size_t n, size_t
 
 int dfft_fft1d_general(int precision, int direction, size_t n, size_t a0, size_t a1, size_t b, void* out, const long long out_strides[3],
                        const void* in, const long long in_strides[3], void* stream) {
-    if (precision != DFFT_F32 && precision != DFFT_F64) return fail(DFFT_ERR_INVALID, "bad precision");
+    if (precision < DFFT_F32 || precision > DFFT_BF16) return fail(DFFT_ERR_INVALID, "bad precision");
+    if (is_half(precision) && !pow2_length(n)) return fail(DFFT_ERR_UNSUPPORTED, "16-bit storage takes power-of-two lengths only");
     if (!c2c_length(n)) return fail(DFFT_ERR_UNSUPPORTED, "length must be a power of two in [2, 8192] or any length in [3, 4096]");
     FftParams prm{};
     prm.A0 = int(a0); prm.A1 = int(a1); prm.B = int(b);

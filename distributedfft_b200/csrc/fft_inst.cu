@@ -1,5 +1,6 @@
-// fft_inst.cu — compiled once per (precision, log2 length): -DDFFT_T=double -DDFFT_LOG2N=10.
-// Splitting the instantiations over translation units lets build.py compile them in parallel.
+// fft_inst.cu — compiled once per (precision, log2 length): -DDFFT_T=double -DDFFT_LOG2N=10, and once per (16-bit format,
+// log2 length) of 16-bit plans: -DDFFT_T=float -DDFFT_S=__half (or __nv_bfloat16) -DDFFT_LOG2N=10, which compiles
+// launch_pass16 only.  Splitting the instantiations over translation units lets build.py compile them in parallel.
 #include <cstdlib>
 
 #include "fft_kernels.cuh"
@@ -113,6 +114,7 @@ static int wide_tiles() {
     return e ? atoi(e) : 0;
 }
 
+#ifndef DFFT_S
 template <typename T, int LOG2N, int TB>
 static cudaError_t launch_tiled(const FftParams& p_in, double scale, cudaStream_t stream, long long lines) {
     FftParams p = p_in;
@@ -549,5 +551,74 @@ cudaError_t launch_batch_small(const void* in, void* out, long long batch, int i
 
 template cudaError_t launch_batch_small<DFFT_T, DFFT_LOG2N>(const void*, void*, long long, int, const BatchSmall&, double, cudaStream_t);
 #endif
+
+#else  // DFFT_S: the 16-bit passes
+
+// the C2C kernels of 16-bit plans over TILED tiles TB wide; tile order as in launch_tiled, no TMA-fed kernel
+template <typename H, int LOG2N, int TB>
+static cudaError_t launch_tiled16(const FftParams& p_in, double scale, cudaStream_t stream, long long lines) {
+    FftParams p = p_in;
+    const int swz = env_int("DFFT_TILE_SWZ", -1);
+    p.tile_swz = tile_swz_for(swz >= 0 ? swz : p.tile_swz, p.A0, p.A1);
+    constexpr int LOG2E = Shape<float, LOG2N>::LOG2E;
+    using C = CtaFft<float, LOG2N, LOG2E, TB, true>;
+    if (p.B <= 0) return cudaSuccess;
+    const long long grid = lines * ((p.B + TB - 1) / TB);
+    if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+    const unsigned g = unsigned((p.max_ctas > 0 && grid > p.max_ctas) ? p.max_ctas : grid);
+    return launch_kernel<fft_c2c16_kernel<H, LOG2N, LOG2E, TB, true, false, false>, fft_c2c16_kernel<H, LOG2N, LOG2E, TB, true, true, false>,
+                         fft_c2c16_kernel<H, LOG2N, LOG2E, TB, true, false, true>, fft_c2c16_kernel<H, LOG2N, LOG2E, TB, true, true, true>>(
+        p, scale, g, C::THREADS, C::SMEM_BYTES, stream);
+}
+
+// launch_pass for 16-bit plans: the shapes of the f32 pass, TILED tiles included (narrow, or wide by launch_pass's rule).
+// The TILED rows are the f32 tile's 8 elements wide from 512-point lines on, 32 bytes of 16-bit pairs: at 512^3 on an H100
+// the y and x passes took 0.43-0.50 ms with them against 0.69-0.72 ms with 64-byte rows (16 elements, twice the threads and
+// shared memory per CTA), DESIGN.md section 3.20.
+template <typename H, int LOG2N>
+cudaError_t launch_pass16(PassKind kind, const FftParams& p, double scale, cudaStream_t stream) {
+    using S = Shape<float, LOG2N>;
+    constexpr int LOG2E = S::LOG2E;
+    using C = CtaFft<float, LOG2N, LOG2E, S::TBC, false>;
+    const long long lines = (long long)p.A0 * p.A1;
+    if (lines <= 0) return cudaSuccess;
+    const long long grid = (lines + S::TBC - 1) / S::TBC;  // CONTIG, R2C and C2R
+    switch (kind) {
+        case PASS_C2C_CONTIG:
+            if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
+            if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+            return launch_kernel<fft_c2c16_kernel<H, LOG2N, LOG2E, S::TBC, false, false, false>, fft_c2c16_kernel<H, LOG2N, LOG2E, S::TBC, false, true, false>,
+                                 fft_c2c16_kernel<H, LOG2N, LOG2E, S::TBC, false, false, true>, fft_c2c16_kernel<H, LOG2N, LOG2E, S::TBC, false, true, true>>(
+                p, scale, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+        case PASS_C2C_TILED: {
+            if constexpr (S::TBT_WIDE != S::TBT) {
+                const int w = wide_tiles();
+                const bool far_rows = (unsigned long long)p.in.sN * sizeof(cx16<H>) >= (1ull << 20) ||
+                                      (unsigned long long)p.out.sN * sizeof(cx16<H>) >= (1ull << 20);
+                const bool wide = w > 0 || p.tile_pref == 2 || (w == 0 && p.tile_pref == 0 && LOG2N >= 10 && far_rows);
+                if (wide && w >= 0 && p.tile_pref != 1 && p.B > S::TBT) return launch_tiled16<H, LOG2N, S::TBT_WIDE>(p, scale, stream, lines);
+            }
+            return launch_tiled16<H, LOG2N, S::TBT>(p, scale, stream, lines);
+        }
+        case PASS_R2C: {
+            if (p.in.nseg != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
+            if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+            constexpr auto k = fft_r2c16_kernel<H, LOG2N, LOG2E, S::TBC, false>;
+            constexpr auto ks = fft_r2c16_kernel<H, LOG2N, LOG2E, S::TBC, true>;
+            return launch_kernel<k, k, ks, ks>(p, scale, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+        }
+        case PASS_C2R: {
+            if (p.out.nseg != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
+            if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+            constexpr auto k = fft_c2r16_kernel<H, LOG2N, LOG2E, S::TBC, false>;
+            constexpr auto ks = fft_c2r16_kernel<H, LOG2N, LOG2E, S::TBC, true>;
+            return launch_kernel<k, k, ks, ks>(p, scale, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+        }
+        default: return cudaErrorInvalidValue;
+    }
+}
+
+template cudaError_t launch_pass16<DFFT_S, DFFT_LOG2N>(PassKind, const FftParams&, double, cudaStream_t);
+#endif  // DFFT_S
 
 }  // namespace dfft

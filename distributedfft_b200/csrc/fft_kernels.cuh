@@ -22,6 +22,8 @@
 // per-thread base plus compile-time constants (SmemLayout in fft_core.cuh).
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 #include <type_traits>
@@ -157,6 +159,28 @@ template <typename T>
 __device__ __forceinline__ void st_elem(cx<T>* p, cx<T> v) {
     if constexpr (sizeof(T) == 8) *reinterpret_cast<double2*>(p) = make_double2(v.x, v.y);
     else *reinterpret_cast<float2*>(p) = make_float2(v.x, v.y);
+}
+
+// 16-bit storage (DFFT_F16 / DFFT_BF16): a complex value is a pair of IEEE binary16 (H = __half) or bfloat16 (H =
+// __nv_bfloat16) numbers, 4 bytes.  The passes compute in f32: a load widens the pair to float exactly, a store rounds the
+// finished float pair once, to nearest even.
+template <typename H>
+struct alignas(4) cx16 {
+    H x, y;
+};
+template <typename T, typename H>
+__device__ __forceinline__ cx<T> ld_elem(const cx16<H>* p) {
+    static_assert(sizeof(T) == 4, "16-bit storage computes in f32");
+    float2 f;
+    if constexpr (std::is_same_v<H, __half>) f = __half22float2(*reinterpret_cast<const __half2*>(p));
+    else f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p));
+    return cx<T>{f.x, f.y};
+}
+template <typename T, typename H>
+__device__ __forceinline__ void st_elem(cx16<H>* p, cx<T> v) {
+    static_assert(sizeof(T) == 4, "16-bit storage computes in f32");
+    if constexpr (std::is_same_v<H, __half>) *reinterpret_cast<__half2*>(p) = __float22half2_rn(make_float2(v.x, v.y));
+    else *reinterpret_cast<__nv_bfloat162*>(p) = __float22bfloat162_rn(make_float2(v.x, v.y));
 }
 
 // ---- per-thread access to one line of a view ----------------------------------------------------------
@@ -330,10 +354,21 @@ struct TileCoord {
 // ---- global-memory access of a C2C tile ------------------------------------------------------------------
 // MemPlain: default caching, what every standalone pass uses.  MemHint: per-instruction L2 eviction priorities
 // (createpolicy.fractional policies), used by the fused z/y kernel to keep its intermediate in the L2.
-template <typename T>
+// S: the stored element (cx<T>, or cx16<H> for 16-bit storage with T = float).
+template <typename T, typename S = cx<T>>
 struct MemPlain {
-    __device__ __forceinline__ cx<T> ld(const cx<T>* p) const { return ld_elem<T>(p); }
-    __device__ __forceinline__ void st(cx<T>* p, cx<T> v) const { st_elem<T>(p, v); }
+    using Stored = S;
+    __device__ __forceinline__ cx<T> ld(const S* p) const { return ld_elem<T>(p); }
+    __device__ __forceinline__ void st(S* p, cx<T> v) const { st_elem<T>(p, v); }
+};
+// the element a memory policy loads and stores: M::Stored where the policy names one, cx<T> otherwise
+template <typename T, typename M, typename = void>
+struct StoredOf {
+    using type = cx<T>;
+};
+template <typename T, typename M>
+struct StoredOf<T, M, std::void_t<typename M::Stored>> {
+    using type = typename M::Stored;
 };
 
 __device__ __forceinline__ unsigned long long l2_evict_first() {
@@ -382,10 +417,11 @@ __device__ __forceinline__ cx<T> cscale(cx<T> v, T s) {
 // store policy of the scaled twins: the policy M, with every stored value scaled first
 template <typename T, typename M>
 struct MemScaled {
+    using Stored = typename StoredOf<T, M>::type;
     M m;
     T s;
-    __device__ __forceinline__ cx<T> ld(const cx<T>* p) const { return m.ld(p); }
-    __device__ __forceinline__ void st(cx<T>* p, cx<T> v) const { m.st(p, cscale<T>(v, s)); }
+    __device__ __forceinline__ cx<T> ld(const Stored* p) const { return m.ld(p); }
+    __device__ __forceinline__ void st(Stored* p, cx<T> v) const { m.st(p, cscale<T>(v, s)); }
 };
 
 // ---- padded and pruned passes (dfft_plan_create_padded, dfft_plan_create_pruned) ---------------------------------------
@@ -426,7 +462,8 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
                                          bool multi, const M& mem, const Hook& after_gather = {}, int ld_lo = 0, int ld_hi = 0, int st_lo = 0,
                                          int st_hi = 0) {
     using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
-    using LA = LineAccess<T, C::LINES>;
+    using S = typename StoredOf<T, M>::type;
+    using LA = LineAccess<T, C::LINES, S>;
     using TC = TileCoord<C, TILED, TB, ILV>;
     constexpr bool STRIDED = TILED || ILV;
     constexpr int E = C::E, TPL = C::TPL;
@@ -456,12 +493,12 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
         } else if (!in.multi) {
             if constexpr (!STRIDED) {
                 // contiguous line: sN == 1, immediate offsets
-                const cx<T>* q = in.p0 + j;
+                const S* q = in.p0 + j;
 #pragma unroll
                 for (int e = 0; e < E; ++e) v[e] = mem.ld(q + e * TPL);
             } else {
                 const long long step = (long long)TPL * p.in.sN;
-                const cx<T>* q = in.p0 + (long long)j * p.in.sN;
+                const S* q = in.p0 + (long long)j * p.in.sN;
 #pragma unroll
                 for (int e = 0; e < E; ++e) { v[e] = mem.ld(q); q += step; }
             }
@@ -490,7 +527,7 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
             }
         } else if (!out.multi) {
             if constexpr (!STRIDED) {
-                cx<T>* q = out.p0 + j;
+                S* q = out.p0 + j;
 #pragma unroll
                 for (int e = 0; e < E; ++e) {
                     const cx<T> x = v[C::Core::final_slot(e)];
@@ -498,7 +535,7 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
                 }
             } else {
                 const long long step = (long long)TPL * p.out.sN;
-                cx<T>* q = out.p0 + (long long)j * p.out.sN;
+                S* q = out.p0 + (long long)j * p.out.sN;
 #pragma unroll
                 for (int e = 0; e < E; ++e) {
                     const cx<T> x = v[C::Core::final_slot(e)];
@@ -520,9 +557,9 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
 // Grid-stride over tiles: launched with one CTA per tile it is the plain kernel; launched with fewer CTAs
 // (FftParams::max_ctas) it is persistent and occupies only that many CTA slots, which is how the overlapped
 // schedule leaves the rest of the GPU to the other passes.
-template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, bool SCALED>
-__global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
-fft_c2c_kernel(const __grid_constant__ KParams<SCALED> p) {
+// S: the stored element (MemPlain).
+template <typename T, typename S, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, bool SCALED>
+__device__ __forceinline__ void c2c_pass(const KParams<SCALED>& p) {
     using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
     using TC = TileCoord<C, TILED, TB>;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -534,8 +571,9 @@ fft_c2c_kernel(const __grid_constant__ KParams<SCALED> p) {
 
 #pragma unroll 1
     for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        if constexpr (SCALED) c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV>(p, tile, sm, tab_in, tab_out, multi, MemScaled<T, MemPlain<T>>{{}, T(p.scale)});
-        else c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV>(p, tile, sm, tab_in, tab_out, multi, MemPlain<T>{});
+        if constexpr (SCALED)
+            c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV>(p, tile, sm, tab_in, tab_out, multi, MemScaled<T, MemPlain<T, S>>{{}, T(p.scale)});
+        else c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV>(p, tile, sm, tab_in, tab_out, multi, MemPlain<T, S>{});
         const int t = TILED ? int(threadIdx.x) % TB : int(threadIdx.x) / C::TPL;
         if (tile + gridDim.x < ntiles) {
             // persistent use: the next tile's first scatter must not overtake this tile's last gather, and
@@ -544,6 +582,20 @@ fft_c2c_kernel(const __grid_constant__ KParams<SCALED> p) {
             else if constexpr (C::NST > 1) C::sync(t);
         }
     }
+}
+
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, bool SCALED>
+__global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
+fft_c2c_kernel(const __grid_constant__ KParams<SCALED> p) {
+    c2c_pass<T, cx<T>, LOG2N, LOG2E, TB, TILED, INV, SCALED>(p);
+}
+
+// The C2C pass of 16-bit plans (H = __half or __nv_bfloat16): cx16<H> in memory, the f32 core, tile and twiddles of the
+// f32 pass, so each line is the f32 pass's result rounded once to 16 bits (the scaled twin: times float(p.scale) first).
+template <typename H, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, bool SCALED>
+__global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<float, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
+fft_c2c16_kernel(const __grid_constant__ KParams<SCALED> p) {
+    c2c_pass<float, cx16<H>, LOG2N, LOG2E, TB, TILED, INV, SCALED>(p);
 }
 
 // Interleaved z pass (PASS_C2C_ILV, C = p.B components per point, below the TILED tile width): the CONTIG shape with its
@@ -1413,10 +1465,11 @@ __device__ __forceinline__ cx<T> shfl_cx(cx<T> v, int src_lane) {
 // core and split into even/odd spectra in shared memory:  X[k] = Xe[k] + W_2M^k Xo[k].
 // PADDED (P = FftPadded): the pairs m >= p.ld_lo read as zero, the points k >= p.st_lo are not stored; the scale is
 // p.scale at run time.
-template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED, bool PADDED, typename P>
+// S: the stored element, of both sides (the real side in pairs: cx16<H> holds two 16-bit reals).
+template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED, bool PADDED, typename P, typename S = cx<T>>
 __device__ __forceinline__ void r2c_lines(const P& p) {
     using C = CtaFft<T, LOG2M, LOG2E, TB, false>;
-    using LA = LineAccess<T, C::LINES>;
+    using LA = LineAccess<T, C::LINES, S>;
     constexpr int E = C::E, TPL = C::TPL, M = C::N, NST = C::NST;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
@@ -1434,7 +1487,7 @@ __device__ __forceinline__ void r2c_lines(const P& p) {
 
     cx<T> v[E];
     if (valid) {
-        const cx<T>* q = in.p0 + j;
+        const S* q = in.p0 + j;
 #pragma unroll
         for (int e = 0; e < E; ++e) {
             if constexpr (PADDED) v[e] = j + e * TPL < p.ld_lo ? ld_elem<T>(q + e * TPL) : cx<T>{T(0), T(0)};
@@ -1495,13 +1548,20 @@ fft_r2c_padded_kernel(const __grid_constant__ FftPadded p) {
     r2c_lines<T, LOG2M, LOG2E, TB, false, true>(p);
 }
 
+// the R2C z pass of 16-bit plans: fft_r2c_kernel's f32 line with cx16<H> loads and stores (fft_c2c16_kernel)
+template <typename H, int LOG2M, int LOG2E, int TB, bool SCALED>
+__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<float, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
+fft_r2c16_kernel(const __grid_constant__ KParams<SCALED> p) {
+    r2c_lines<float, LOG2M, LOG2E, TB, SCALED, false, KParams<SCALED>, cx16<H>>(p);
+}
+
 // ---- C2R pass (CONTIG): M+1 complex points -> real line of 2M points, unnormalised -----------------------
 // PADDED (P = FftPadded): the points k >= p.ld_lo read as zero, their partner loads X[M - k] as well; the pairs
 // m >= p.st_lo are not stored; the scale is p.scale at run time.
-template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED, bool PADDED, typename P>
+template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED, bool PADDED, typename P, typename S = cx<T>>
 __device__ __forceinline__ void c2r_lines(const P& p) {
     using C = CtaFft<T, LOG2M, LOG2E, TB, false>;
-    using LA = LineAccess<T, C::LINES>;
+    using LA = LineAccess<T, C::LINES, S>;
     constexpr int E = C::E, TPL = C::TPL, M = C::N;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
@@ -1584,7 +1644,7 @@ __device__ __forceinline__ void c2r_lines(const P& p) {
     }
     C::template stages<0>(v, j, t, sm, reinterpret_cast<const cx<T>*>(p.tw));
     if (valid) {
-        cx<T>* q = out.p0 + j;
+        S* q = out.p0 + j;
 #pragma unroll
         for (int e = 0; e < E; ++e) {
             if constexpr (PADDED) {
@@ -1608,6 +1668,13 @@ template <typename T, int LOG2M, int LOG2E, int TB>
 __global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
 fft_c2r_padded_kernel(const __grid_constant__ FftPadded p) {
     c2r_lines<T, LOG2M, LOG2E, TB, false, true>(p);
+}
+
+// the C2R z pass of 16-bit plans: fft_c2r_kernel's f32 line with cx16<H> loads and stores (fft_c2c16_kernel)
+template <typename H, int LOG2M, int LOG2E, int TB, bool SCALED>
+__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<float, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
+fft_c2r16_kernel(const __grid_constant__ KParams<SCALED> p) {
+    c2r_lines<float, LOG2M, LOG2E, TB, SCALED, false, KParams<SCALED>, cx16<H>>(p);
 }
 
 // ---- Bluestein pass: C2C lines of any length n through two transforms of length M = 2^LOG2M >= 2n - 1 ----------------
@@ -2145,6 +2212,12 @@ cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStr
 // first; it returns cudaErrorInvalidValue for a length that is not instantiated.
 cudaError_t launch_pass(int prec, int log2n, PassKind kind, const FftParams& p, double scale, cudaStream_t stream);
 
+// 16-bit plans (cx16<H> views, H = __half for DFFT_F16, __nv_bfloat16 for DFFT_BF16): kind PASS_C2C_CONTIG, PASS_C2C_TILED,
+// PASS_R2C or PASS_C2R over the views of launch_pass, the f32 kernels' arithmetic; scale != 1 launches the scaled twins.
+// The runtime form launch_pass(prec, ...) takes DFFT_F16 / DFFT_BF16 to them.
+template <typename H, int LOG2N>
+cudaError_t launch_pass16(PassKind kind, const FftParams& p, double scale, cudaStream_t stream);
+
 // padded pass (FftPadded): kind PASS_C2C_CONTIG, PASS_C2C_TILED, PASS_R2C or PASS_C2R over the views of launch_pass, the
 // hole [p.ld_lo, p.ld_hi) of each line on its loaded side and [p.st_lo, p.st_hi) on its stored side (R2C / C2R: both reach
 // the end of the line); p.scale scales the stores.
@@ -2199,7 +2272,7 @@ cudaError_t launch_r2r4(int prec, int log2m, PassKind kind, const FftR2r& p, cud
 
 // copy pass of p.n-point lines (fft_copy_kernel): kind PASS_COPY_CONTIG or PASS_COPY_TILED, p.ltpl is filled in here.
 // Instantiated for E = T and cx<T> in the LOG2N = 1 unit of each precision; the runtime form takes real != 0 for the
-// real elements of R2R plans.
+// real elements of R2R plans, and moves the 4-byte elements of 16-bit plans as E = float, unscaled.
 template <typename E>
 cudaError_t launch_copy(PassKind kind, const FftCopy& p, cudaStream_t stream);
 cudaError_t launch_copy(int prec, bool real, PassKind kind, const FftCopy& p, cudaStream_t stream);

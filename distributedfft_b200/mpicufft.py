@@ -15,7 +15,7 @@ from ._lib import check, lib
 from .params import CommunicationMethod, Configurations, GlobalSize, Partition, SendMethod
 
 SLAB_ZY_THEN_X, SLAB_Z_THEN_YX, PENCIL = 0, 1, 2
-F32, F64 = 0, 1
+F32, F64, F16, BF16 = 0, 1, 2, 3
 R2C, C2C, DCT, DST, R2HC = 0, 1, 2, 3, 4
 DCT1, DST1 = 16, 17  # type-I kinds (DCT-I / DST-I): per-axis plans and fft1d_r2r only
 DCT4, DST4 = 19, 20  # type-IV kinds (DCT-IV / DST-IV): per-axis plans and fft1d_r2r only
@@ -103,7 +103,10 @@ class Comm:
 
 class MPIcuFFT:
     """Abstract plan (include/mpicufft.hpp:55-105). `precision`: 'double' | 'float' replaces the C++
-    template argument; `transform`: 'r2c' (the reference's), 'c2c', or the real-to-real 'dct' / 'dst' (type II forward, type III
+    template argument; 'half' ('f16', 'float16') and 'bfloat16' ('bf16') make 16-bit plans (C2C and R2C / C2R, power-of-two
+    lengths; f32 arithmetic inside the passes, include/dfft.h): their buffers are torch.complex32 / torch.float16 tensors
+    (FP16) or torch.bfloat16 tensors with a trailing dimension of 2 on complex sides and plain torch.bfloat16 on real sides
+    (BF16), and the output scale is split over the FFT passes (setScale).  `transform`: 'r2c' (the reference's), 'c2c', or the real-to-real 'dct' / 'dst' (type II forward, type III
     inverse, on all three axes; execR2R).  A tuple of three names from 'dct', 'dst', 'r2hc', 'dct1', 'dst1', 'dct4', 'dst4',
     in (x, y, z) order, gives a real-to-real plan with a kind per axis (dfft_plan_create_r2r; 'r2hc': FFTW's R2HC forward,
     HC2R inverse; 'dct1' / 'dst1': DCT-I / DST-I both ways, FFTW's REDFT00 / RODFT00, on axes of 2^k + 1 / 2^k - 1 points;
@@ -121,8 +124,12 @@ class MPIcuFFT:
             self.precision = F64
         elif precision in ("float", "f32", "float32"):
             self.precision = F32
+        elif precision in ("half", "f16", "float16"):
+            self.precision = F16
+        elif precision in ("bfloat16", "bf16"):
+            self.precision = BF16
         else:
-            raise ValueError(f"precision must be 'double' or 'float', got {precision!r}")
+            raise ValueError(f"precision must be 'double', 'float', 'half' or 'bfloat16', got {precision!r}")
         self.kinds = None
         if isinstance(transform, tuple):
             if len(transform) != 3 or not all(isinstance(k, str) and k.lower() in _R2R_KINDS for k in transform):

@@ -72,7 +72,30 @@ typedef enum {
     DFFT_PENCIL = 2          /* MPIcuFFT_Pencil: z FFT, transpose, y FFT, transpose, x FFT on a P1 x P2 grid */
 } dfft_decomp;
 
-typedef enum { DFFT_F32 = 0, DFFT_F64 = 1 } dfft_prec; /* cuFFT<float> / cuFFT<double>, include/cufft.hpp:22-60 */
+typedef enum { DFFT_F32 = 0, DFFT_F64 = 1, DFFT_F16 = 2, DFFT_BF16 = 3 } dfft_prec; /* cuFFT<float> / cuFFT<double>, include/cufft.hpp:22-60 */
+/* DFFT_F16 / DFFT_BF16 (not in the reference): 16-bit plans.  Every caller buffer, work-area slot, peer store and NCCL
+ * message holds 16-bit values; every pass widens them to float exactly, runs the f32 pass arithmetic with the f32 tables
+ * and rounds once, to nearest even, as it stores.  Each pass moves half the bytes of the f32 plan.
+ *   - A complex element is a pair (re, im) of IEEE binary16 (DFFT_F16, torch.complex32) or bfloat16 (DFFT_BF16) numbers,
+ *     4 bytes; the real side of R2C / C2R holds 2-byte reals.  dfft_get_domain_size, dfft_get_work_size_device and the
+ *     batch distances follow: half those of the F32 plan of the same geometry (slots rounded up to 256 bytes).  Partitions,
+ *     dfft_layout and every extent getter are unchanged.
+ *   - dfft_plan_create, dfft_plan_create_batched and dfft_plan_create_inplace take them, for C2C and R2C / C2R with the
+ *     power-of-two lengths of f32 plans; every decomposition, Peer2Peer and All2All, partial d, batches, in place,
+ *     dfft_plan_set_transform_axes, the timer, dfft_plan_describe, dfft_debug_run_step and graph capture of one-rank
+ *     _async execs work as on f32 plans.  They always run the sequential schedule (dfft_plan_tune has one candidate).
+ *   - DFFT_ERR_UNSUPPORTED: other lengths, DFFT_DCT / DFFT_DST and dfft_plan_create_r2r, dfft_plan_create_padded, _pruned,
+ *     _interleaved and _boxes, and dfft_plan_set_strides.  A precision outside 0..3: DFFT_ERR_INVALID.
+ *   - dfft_fft1d_contig, _strided and _general take them; dfft_fft1d_r2r returns DFFT_ERR_UNSUPPORTED.
+ *   - Output scale (dfft_plan_set_scale): a direction's scale s is split over the FFT passes of the exec, so that no
+ *     intermediate overflows that the result would not.  With L = sum of log2 n_a over the axes the exec transforms (log2 Nz
+ *     for the R2C z axis), the pass over axis a multiplies each value it stores by f_a = float(|s|^(log2 n_a / L)) before
+ *     rounding it, and the last FFT pass of the exec also carries the sign of s.  s = 1 runs unscaled; s = 1/N gives
+ *     f_a = 1/n_a exactly.  Copy passes of kept axes and execs that transform no axis never scale.  So the f32 / f64 rule
+ *     "the output is the unscaled output times s, bit for bit" does not hold here.  FP16 tops out at 65504: an
+ *     unnormalised forward of a large grid (a 512^3 field with a non-zero mean) overflows to inf; BF16 has the range of
+ *     FP32.  Use (1/N, 1) or (1/sqrt(N), 1/sqrt(N)) with FP16.  dfft_plan_describe lists "precision" ("f16" / "bf16") and
+ *     each pass's f_a != 1 as "factor". */
 
 /* The reference only offers real<->complex (execR2C/execC2R).  DFFT_C2C plans add the complex
  * transform the benchmark configurations name; the z extent of every complex array is then Nz instead

@@ -59,6 +59,13 @@ namespace dfft_shim {
 template <typename T> struct prec;
 template <> struct prec<float> { static constexpr int value = DFFT_F32; };
 template <> struct prec<double> { static constexpr int value = DFFT_F64; };
+// 16-bit plans (DFFT_F16 / DFFT_BF16): MPIcuFFT_Slab<__half> etc. once the caller has included cuda_fp16.h / cuda_bf16.h
+#ifdef __CUDA_FP16_H__
+template <> struct prec<__half> { static constexpr int value = DFFT_F16; };
+#endif
+#ifdef __CUDA_BF16_H__
+template <> struct prec<__nv_bfloat16> { static constexpr int value = DFFT_BF16; };
+#endif
 inline void die(int rc, const char* file, int line) {
     if (rc < 0) {
         std::printf("Error %d at %s:%d: %s\n", rc, file, line, dfft_last_error_string());
