@@ -5,7 +5,8 @@ geometry-only plans of all P ranks, every rank gets its own work area and caller
 f32 and f64), and the ranks run in lock step: rendezvous are no-ops (the lock step orders everything), all-to-all steps are
 device copies between the ranks' staging slots, and pass steps run through dfft_debug_run_step.  The caller buffers
 follow step_replay.Side, so natural layouts, boxes, strides with their ghost layers, the padded real rows of in-place
-R2C / C2R plans, interleaved components and batches all take one geometry.
+R2C / C2R plans, interleaved components and batches all take one geometry.  Pruned plans come from the same creator, and
+the 4-byte pairs of 16-bit plans move as uint32 elements.
 
 `output` checks what holds for every plan: no output element is still NaN; out of place, the caller's input buffers are
 unchanged byte for byte, ghosts included; every ghost byte of a strided output side is still 0xFF; and a second run with
@@ -36,7 +37,10 @@ def same_bits(a, b):
 
 
 def element_type(sc):
-    """the numpy type of the elements the passes of step list sc address: real for R2R plans, else complex"""
+    """the numpy type of the elements the passes of step list sc address: real for R2R plans, else complex, and uint32 for
+    the 4-byte complex elements of 16-bit plans (numpy has no complex type of two 16-bit numbers)"""
+    if sc["esize"] == 4 and "r2r" not in sc:
+        return np.dtype(np.uint32)
     return np.dtype(("f" if "r2r" in sc else "c") + str(sc["esize"]))
 
 

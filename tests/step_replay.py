@@ -19,8 +19,11 @@ each wherever it applies:
   - the two listed phases of the fused z + y stage and of the batched stage, which run concurrently, touch disjoint
     planes / fields;
   - in-place R2C / C2R plans: the padding of the real rows is not read before a store, and the C2R pass never stores there;
-  - every pass names a kind this module knows, with the lengths, line counts and strides that kind takes, and a padded plan
-    has a hole pass ("keep") wherever one of the first d axes is truncated."""
+  - every pass names a kind this module knows, with the lengths, line counts and strides that kind takes, a padded plan
+    has a hole pass ("keep") wherever one of the first d axes is truncated, and a pruned plan has a data-hole pass
+    ("data") wherever its data is smaller than one of the first d axes.
+16-bit plans (F16 / BF16) address 4-byte elements; the replay computes in double as for every plan and rounds each pass's
+stores to 16 bits, after its "factor", as the kernels do."""
 from __future__ import annotations
 
 import ctypes as C
@@ -44,15 +47,17 @@ POISON = -3.25e300 + 7.5e299j  # every ghost element of a caller array with stri
 # ---- plans ----------------------------------------------------------------------------------------------------------------
 @dataclass(frozen=True)
 class Plan:
-    """Everything a replayed plan can have.  The creator follows the fields: boxes -> dfft_plan_create_boxes, spectral ->
-    dfft_plan_create_padded, components -> dfft_plan_create_interleaved, kinds -> dfft_plan_create_r2r, inplace ->
-    dfft_plan_create_inplace, a batch -> dfft_plan_create_batched, else dfft_plan_create.  embed, axes and scale go through
-    their setters.
+    """Everything a replayed plan can have.  The creator follows the fields: data -> dfft_plan_create_pruned, boxes ->
+    dfft_plan_create_boxes, spectral -> dfft_plan_create_padded, components -> dfft_plan_create_interleaved, kinds ->
+    dfft_plan_create_r2r, inplace -> dfft_plan_create_inplace, a batch -> dfft_plan_create_batched, else dfft_plan_create.
+    embed, axes and scale go through their setters.
 
     in_boxes / out_boxes: one ((lx, ly, lz), (hx, hy, hz)) per rank of the physical and the output grid; None keeps that
     side's natural layout.  embed ("in", "out" or "both": the physical side, the output of d = 3) puts each rank's block of
     those sides inside a larger caller array: `halo` ghost layers around it, `gap` more elements between fields (both in the
-    side's elements; even on the real side of R2C / C2R, whose pairs of reals must stay aligned)."""
+    side's elements; even on the real side of R2C / C2R, whose pairs of reals must stay aligned).  data: the (mx, my, mz)
+    block of a pruned plan, made together with `spectral` (None: the whole grid); pruned plans have no boxes, strides,
+    components, kinds or in-place form."""
     P: int
     decomp: int
     shape: tuple
@@ -74,6 +79,7 @@ class Plan:
     embed: str | None = None
     halo: int = 2
     gap: int = 0
+    data: tuple | None = None
 
     @property
     def fields(self):
@@ -101,7 +107,11 @@ def create(p, rank, comm=None):
     cfg = C.byref(_lib.dfft_config(1, 0, p.comm, p.send, None, p.comm, p.send))
     plan = C.c_void_p()
     head = (c, cfg, p.decomp, p.prec)
-    if p.in_boxes is not None or p.out_boxes is not None:
+    if p.data is not None:
+        assert p.in_boxes is None and p.out_boxes is None and p.embed is None and p.components is None and p.kinds is None and not p.inplace
+        k = None if p.spectral is None else (C.c_size_t * 3)(*p.spectral)
+        rc = lib().dfft_plan_create_pruned(*head, p.transform, *p.shape, (C.c_size_t * 3)(*p.data), k, p.p1, p.p2, p.fields, 1, C.byref(plan))
+    elif p.in_boxes is not None or p.out_boxes is not None:
         rc = lib().dfft_plan_create_boxes(*head, p.transform, *p.shape, p.p1, p.p2, _flat(p.in_boxes), _flat(p.out_boxes), p.fields, 1,
                                           C.byref(plan))
     elif p.spectral is not None:
@@ -258,6 +268,27 @@ PASSES = {
     9: (lambda N: (N, N // 2 + 1), True, False, lambda st, x, N: np.fft.rfft(x, axis=2)),  # real side counted in reals
     10: (lambda N: (N // 2 + 1, N), False, True, lambda st, x, N: np.fft.irfft(x, n=N, axis=2) * N),
 }
+
+
+def round16(v, prec):
+    """v rounded to binary16 (numpy, round to nearest even) or bfloat16 (nearest even on the float32 bits), as float64"""
+    v = np.asarray(v)
+    if np.iscomplexobj(v):
+        return round16(v.real, prec) + 1j * round16(v.imag, prec)
+    if prec == dfft.F16:
+        return v.astype(np.float16).astype(np.float64)
+    u = v.astype(np.float32).view(np.uint32).astype(np.uint64)
+    u = ((u + 0x7FFF + ((u >> 16) & 1)) & 0xFFFF0000).astype(np.uint32)
+    return u.view(np.float32).astype(np.float64)
+
+
+def store16(st, res, prec):
+    """what a 16-bit pass st stores of its values res: times its factor in f32, rounded once"""
+    f = st.get("factor")
+    if f is not None:
+        res = (res.real.astype(np.float32) * np.float32(f)).astype(np.float64) + (
+            1j * (res.imag.astype(np.float32) * np.float32(f)).astype(np.float64) if np.iscomplexobj(res) else 0)
+    return round16(res, prec)
 
 
 # ---- memory, views and the happens-before check -------------------------------------------------------------------------
@@ -513,7 +544,7 @@ class _Replay:
         sc0 = scheds[0]
         self.real = "r2r" in sc0  # R2R plans: real elements everywhere
         self.es = es = sc0["esize"]
-        assert es == (16 if p.prec == dfft.F64 else 8) // (2 if self.real else 1), es
+        assert es == {dfft.F64: 16, dfft.F32: 8, dfft.F16: 4, dfft.BF16: 4}[p.prec] // (2 if self.real else 1), es
         self.r2c = p.transform == dfft.R2C and not self.real
         self.mem = Memory(es, np.float64 if self.real else np.complex128)
         self.owner = {}  # id(slot array) -> (rank, slot)
@@ -568,7 +599,7 @@ class _Replay:
         nsteps = len(scheds[0]["steps"])
         assert all(len(sc["steps"]) == nsteps for sc in scheds), [len(sc["steps"]) for sc in scheds]
         self.order = Ordering(scheds)
-        self.last_remote_write, self.last_rdv, self.prev_acc, self.holes = {}, [-1] * P, {}, 0
+        self.last_remote_write, self.last_rdv, self.prev_acc, self.holes, self.data_holes = {}, [-1] * P, {}, 0, 0
         for k in range(nsteps):
             pending = []  # stores of step k land after every rank's loads of step k
             for r in range(P):
@@ -584,6 +615,8 @@ class _Replay:
                 tgt[idx] = val
         if p.spectral is not None and any(p.spectral[a] != p.shape[a] for a in (2, 1, 0)[:self.d]):
             assert self.holes > 0, "a padded plan that truncates one of its first d axes runs no hole pass"
+        if p.data is not None and any(p.data[a] != p.shape[a] for a in (2, 1, 0)[:self.d]):
+            assert self.data_holes > 0, "a pruned plan with data smaller than one of its first d axes runs no pass with a data hole"
         outs = [[] for _ in range(p.fields)]
         for r in range(P):
             if not p.inplace:
@@ -686,6 +719,10 @@ class _Replay:
         if "keep" in st:
             self.holes += 1
             assert kind in (0, 1, 2, 3) and 1 <= st["keep"] < (N + 1 if kind in (2, 3) else N), where
+        if "data" in st:
+            self.data_holes += 1
+            assert kind in (0, 1, 2, 3) and 1 <= st["data"] < (2 * N if kind in (2, 3) else N), where
+            assert kind not in (2, 3) or st["data"] % 2 == 0, where
 
     def run_pass(self, r, k, st, pending):
         kind = st["kind"]
@@ -695,9 +732,15 @@ class _Replay:
         n_in, n_out = points(N)
         b = 1 if kind in (2, 3) else st["B"]
         A0, A1 = st["A0"], st["A1"]
-        keep = st.get("keep")  # padded plans: the spectral side (out forward, in inverse) holds the kept indices only
-        kin = keep if keep is not None and st["inverse"] else n_in
-        kout = keep if keep is not None and not st["inverse"] else n_out
+        # the line positions a side holds (None: all), the rest of the line being zero: padded plans keep the "keep"
+        # spectral indices (out forward, in inverse), pruned plans the positions [0, "data") of the physical side (in
+        # forward, out inverse; R2C / C2R: data reals, data / 2 pairs).  The pairs and the R2C half spectrum are prefixes.
+        pairs = kind in (2, 3)
+        spec = None if "keep" not in st else np.arange(st["keep"]) if pairs else positions(N, st["keep"])
+        phys = None if "data" not in st else np.arange(st["data"] // 2 if pairs else st["data"])
+        at_in, at_out = (spec, phys) if st["inverse"] else (phys, spec)
+        kin = n_in if at_in is None else at_in.size
+        kout = n_out if at_out is None else at_out.size
         reads = self.access(r, k, st, "in", kin, b, real_in)
         writes = self.access(r, k, st, "out", kout, b, real_out)
         data = np.zeros((A0, A1, kin, b), dtype=np.float64 if self.real or real_in else np.complex128)
@@ -707,16 +750,16 @@ class _Replay:
         self.check_buffer(r, k, st, reads, writes)
         self.check_bounds(r, k, st, "in", reads)
         self.check_bounds(r, k, st, "out", writes)
-        if kin != n_in:
+        if at_in is not None:
             full = np.zeros((A0, A1, n_in, b), dtype=data.dtype)
-            full[:, :, positions(N, kin) if kind != 3 else np.arange(kin), :] = data
+            full[:, :, at_in, :] = data
             data = full
         if math is None:
             res = R2R[st.get("r2r", self.scheds[r].get("r2r"))](data, st["inverse"])
         else:
             res = math(st, data, N)
-        if kout != n_out:
-            res = res[:, :, positions(N, kout) if kind != 2 else np.arange(kout), :]
+        if at_out is not None:
+            res = res[:, :, at_out, :]
         if "scale" in st:
             res = res * st["scale"]
             for arr, tgt, idx, cidx, ns in writes:
@@ -728,6 +771,8 @@ class _Replay:
                         np.add.at(cnt, units * idx.ravel() + j, 1)
                 else:
                     np.add.at(cnt, idx.ravel(), 1)
+        if self.p.prec in (dfft.F16, dfft.BF16):
+            res = store16(st, res, self.p.prec)
         for arr, tgt, idx, cidx, ns in writes:
             pending.append((arr, tgt, idx, cidx, res[:, :, ns, :], r))
 

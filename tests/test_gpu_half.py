@@ -7,7 +7,7 @@ have an exact reference: the f32 pass on the widened input, times the pass's fac
   - one-rank plans: the exec against the composition of f32 single-axis passes in the schedule's axis order, bit for bit;
   - accuracy: 256^3 and 512^3 against the float64 transform of the widened input, and round trips;
   - the scale split: an FP16 512^3 forward of a constant field is exact with (1/N, 1) and overflows unscaled, as documented;
-  - multi-rank schedules: the one-GPU lock-step replay (gpu_replay.py, half_replay.py) of 2..8 ranks equals the one-rank replay bit for bit;
+  - multi-rank schedules: the one-GPU lock-step replay (gpu_replay.py) of 2..8 ranks equals the one-rank replay bit for bit;
   - graph capture, the timer, dfft_plan_tune, the Python binding with torch.complex32 and the C++ shim."""
 from __future__ import annotations
 
@@ -20,7 +20,6 @@ import pytest
 
 import distributedfft_b200 as dfft
 import gpu_replay as G
-import half_replay as HR
 import step_replay as R
 
 torch = pytest.importorskip("torch")
@@ -280,10 +279,9 @@ def test_replay_of_ranks_equals_one_rank(prec, case):
         scale = (1.0, -1.0 / 4096) if inverse else (1.0 / 2048, 1.0)
         plan = lambda P_, decomp_, p1_, p2_: R.Plan(P_, decomp_, shape, p1_, p2_, transform=dfft.C2C, prec=prec, comm=comm, batch=batch,
                                                     inplace=inplace, axes=axes, scale=scale)
-        with HR.elements():
-            got = G.assemble(G.replay(plan(P, decomp, p1, p2), inverse, d, x))
-            again = G.assemble(G.replay(plan(P, decomp, p1, p2), inverse, d, x, descending=True))
-            one = G.assemble(G.replay(plan(1, decomp, 1, 1), inverse, d, x))
+        got = G.assemble(G.replay(plan(P, decomp, p1, p2), inverse, d, x))
+        again = G.assemble(G.replay(plan(P, decomp, p1, p2), inverse, d, x, descending=True))
+        one = G.assemble(G.replay(plan(1, decomp, 1, 1), inverse, d, x))
         assert not torch.isnan(unpacked(got, prec).float()).any(), "output elements never written"
         assert G.same_bits(again, got), "the result depends on the order of the ranks within a step"
         assert G.same_bits(got, one), f"inverse={inverse}: {int((got != one).sum())} elements differ from the one-rank plan"

@@ -270,11 +270,11 @@ def test_free_space_convolution(transform):
 def replay_gpu(P, decomp, transform, shape, data, spec, p1, p2, comm, inverse, f64):
     """every rank's pruned steps in lock step on this GPU (gpu_replay.py: the real kernels, multi-segment views, and the
     checks it makes of every plan); returns (the global output, the numpy reference)"""
-    import pruned_replay as PR
+    import step_replay as R
     from gpu_replay import output
 
     t = C2C_ if transform == "c2c" else R2C_
-    p = PR.Plan(P, decomp, tuple(shape), p1, p2, transform=t, prec=dfft.F64 if f64 else dfft.F32, comm=comm, batch=1, data=tuple(data),
+    p = R.Plan(P, decomp, tuple(shape), p1, p2, transform=t, prec=dfft.F64 if f64 else dfft.F32, comm=comm, batch=1, data=tuple(data),
                spectral=tuple(spec))
     rng = np.random.default_rng(P * 100 + decomp * 10 + p1)
     x = rng.standard_normal(data) if t == R2C_ else rng.standard_normal(data) + 1j * rng.standard_normal(data)
@@ -282,8 +282,7 @@ def replay_gpu(P, decomp, transform, shape, data, spec, p1, p2, comm, inverse, f
     src, want = (X, inv_ref(X, t, shape, data, spec, 3)) if inverse else (x, X)
     if t == R2C_ and inverse:
         want = want.real
-    with PR.plans():
-        return output(p, inverse, 3, src[None])[0], want
+    return output(p, inverse, 3, src[None])[0], want
 
 
 REPLAY_GRIDS = [(P, SL_, P, 1) for P in (2, 4, 8)] + [(P, ZY_, P, 1) for P in (2, 4, 8)] + \

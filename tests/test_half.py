@@ -1,6 +1,6 @@
 """16-bit plans (DFFT_F16 / DFFT_BF16) without a GPU: the precisions every entry point accepts or refuses, the geometry
 of 16-bit plans against the F32 plan of the same shape, the output scale split over the FFT passes, and a numpy replay of
-every rank's step list with each pass's stores rounded to 16 bits (half_replay.py).
+every rank's step list with each pass's stores rounded to 16 bits (step_replay.py).
 
 A 16-bit plan runs the F32 plan's sequential schedule with 4-byte elements: the same steps over the same element counts,
 half the bytes.  Each FFT pass multiplies its stores by its "factor" (f_a = |s|^(log2 n_a / L), the sign of s on the last
@@ -14,12 +14,10 @@ import numpy as np
 import pytest
 
 import distributedfft_b200 as dfft
-import half_replay as HR
-import pruned_replay as PR
 import step_replay as R
 from distributedfft_b200._lib import lib
-from half_replay import round16
 from oracle import dft_oracle as O
+from step_replay import round16
 
 SL, ZY, PE = dfft.SLAB_ZY_THEN_X, dfft.SLAB_Z_THEN_YX, dfft.PENCIL
 C2C, R2C = dfft.C2C, dfft.R2C
@@ -57,14 +55,14 @@ def test_creators_accept_16bit(prec, kw):
     ("DCT / DST plans", lambda prec: R.Plan(1, SL, (8, 8, 8), transform=dfft.DST, prec=prec)),
     ("real-to-real plans", lambda prec: R.Plan(1, SL, (8, 8, 8), kinds=(dfft.DCT, dfft.DCT, dfft.DCT), prec=prec)),
     ("padded plans", lambda prec: R.Plan(1, SL, (8, 8, 8), spectral=(4, 8, 8), prec=prec)),
-    ("pruned plans", lambda prec: PR.Plan(1, SL, (8, 8, 8), data=(4, 8, 8), prec=prec)),
+    ("pruned plans", lambda prec: R.Plan(1, SL, (8, 8, 8), data=(4, 8, 8), prec=prec)),
     ("interleaved plans", lambda prec: R.Plan(1, SL, (8, 8, 8), components=2, prec=prec)),
     ("interleaved plans", lambda prec: R.Plan(1, SL, (8, 8, 8), components=1, prec=prec)),
     ("box plans", lambda prec: R.Plan(1, SL, (8, 8, 8), in_boxes=(((0, 0, 0), (8, 8, 8)),), prec=prec)),
     ("plans with strides", lambda prec: R.Plan(1, SL, (8, 8, 8), embed="in", prec=prec)),
 ])
 def test_refused_options(prec, what, p):
-    rc, msg, c, plan = (PR.create if isinstance(p(prec), PR.Plan) else R.create)(p(prec), 0)
+    rc, msg, c, plan = R.create(p(prec), 0)
     if plan:  # strides are refused by their setter, after the plan was made
         lib().dfft_plan_destroy(plan)
     lib().dfft_comm_destroy(c)
@@ -266,7 +264,7 @@ def replay_case(case, prec, inverse, d, scale):
     else:
         ins = [round16(x, prec) for x in xs]
         want = [scale[0] * fwd(x) for x in ins]
-    outs = HR.replay(p, inverse, d, ins)
+    outs = R.replay(p, inverse, d, ins)
     return R.error(outs, want)
 
 

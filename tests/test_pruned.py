@@ -13,7 +13,6 @@ import numpy as np
 import pytest
 
 import distributedfft_b200 as dfft
-import pruned_replay as PR
 import step_replay as R
 from distributedfft_b200 import _lib
 from distributedfft_b200._lib import check, lib
@@ -30,13 +29,13 @@ def err():
 
 
 def plan_of(P, decomp, transform, shape, data, spec, p1, p2, comm=P2P, batch=1, scale=None):
-    return PR.Plan(P, decomp, tuple(shape), p1, p2, transform=transform, comm=comm, batch=batch, scale=scale,
-                  data=tuple(data), spectral=None if spec is None else tuple(spec))
+    return R.Plan(P, decomp, tuple(shape), p1, p2, transform=transform, comm=comm, batch=batch, scale=scale,
+                 data=tuple(data), spectral=None if spec is None else tuple(spec))
 
 
 def create(rank, P, decomp, transform, shape, data, spec, p1, p2, comm=P2P, batch=1):
     """dry pruned plan: (rc, comm, plan); plan is None when the creator refused"""
-    rc, _, c, plan = PR.create(plan_of(P, decomp, transform, shape, data, spec, p1, p2, comm, batch), rank)
+    rc, _, c, plan = R.create(plan_of(P, decomp, transform, shape, data, spec, p1, p2, comm, batch), rank)
     return rc, c, (plan if rc == 0 else None)
 
 
@@ -82,7 +81,7 @@ def replay(P, decomp, transform, shape, data, spec, p1, p2, inverse, d, comm=P2P
     """replays every rank's steps in lock step; returns the worst rel-L2 error of any rank's output block"""
     spec = tuple(shape) if spec is None else tuple(spec)
     p = plan_of(P, decomp, transform, shape, data, spec, p1, p2, comm, batch, scale)
-    scheds = [PR.describe(p, r, inverse, d) for r in range(P)]
+    scheds = [R.describe(p, r, inverse, d) for r in range(P)]
     pruned = tuple(data) != tuple(shape)
     assert not scheds[0]["overlapped"]
     assert ("data" in scheds[0]) == pruned and (not pruned or scheds[0]["data"] == list(data))
@@ -94,7 +93,7 @@ def replay(P, decomp, transform, shape, data, spec, p1, p2, inverse, d, comm=P2P
     spec_g = np.stack([fwd_ref(xg[f], transform, shape, spec, d) for f in range(batch)])
     want_g = np.stack([inv_ref(spec_g[f], transform, shape, data, spec, d) for f in range(batch)]) if inverse else spec_g
     s_used = 1.0 if scale is None else scale[1 if inverse else 0]
-    return R.error(PR.replay(p, inverse, d, spec_g if inverse else xg, scheds), want_g * s_used)
+    return R.error(R.replay(p, inverse, d, spec_g if inverse else xg, scheds), want_g * s_used)
 
 
 # ---- validation -----------------------------------------------------------------------------------------------------------
@@ -264,7 +263,7 @@ def test_slab_forward_transposition_moves_the_data_planes_only(P, transform):
         p = plan_of(P, SL, transform, shape, dat, spec, P, 1, A2A)
         total = 0
         for r in range(P):
-            sc = PR.describe(p, r, 0, 3)
+            sc = R.describe(p, r, 0, 3)
             a2a = [st for st in sc["steps"] if st["type"] == 2]
             assert len(a2a) == 1
             total += sum(peer["scount"] for peer in a2a[0]["peers"])
