@@ -71,6 +71,8 @@ SIGNATURES = {
                                          C.c_int, C.POINTER(C.c_void_p)]),
     "dfft_plan_set_scale": (C.c_int, [C.c_void_p, C.c_double, C.c_double]),
     "dfft_plan_get_scale": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
+    "dfft_plan_set_weights": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
+    "dfft_plan_get_weights": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "dfft_plan_destroy": (C.c_int, [C.c_void_p]),
     "dfft_set_work_area": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "dfft_exec_r2c": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),

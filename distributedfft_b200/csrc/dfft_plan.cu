@@ -142,18 +142,21 @@ static bool r2r_kind_length(int kind, size_t n) {
 // hole: passes of padded and pruned plans that keep part of a side, the holes of their lines (pass_hole): [hole[0],
 // hole[1]) on the spectral side, [hole[2], hole[3]) on the physical one; the padded twin of the power-of-two kernel runs
 // then, with the physical hole on its loaded side forward and on its stored side inverse.
+// w: the spectral weights of the pass's axis (dfft_plan_set_weights), or null.  Weighted passes run the weighted twins:
+// of the padded kernels (with hole, empty where the plan keeps a whole side) or of the Bluestein kernel.
 static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftParams& prm, const void* blu, double scale, cudaStream_t stream,
-                                   int r2r = DFFT_DCT, const int* hole = nullptr) {
+                                   int r2r = DFFT_DCT, const int* hole = nullptr, const void* w = nullptr) {
     const int log2n = ilog2_exact(n);
     if (hole && log2n >= 0) {
-        FftPadded q;
+        FftWeighted q;
         static_cast<FftParams&>(q) = prm;
         q.scale = scale;
         const int* ld = prm.inverse ? hole : hole + 2;
         const int* st = prm.inverse ? hole + 2 : hole;
         q.ld_lo = ld[0]; q.ld_hi = ld[1];
         q.st_lo = st[0]; q.st_hi = st[1];
-        return launch_padded(prec, log2n, kind, q, stream);
+        q.w = w;
+        return w ? launch_weighted(prec, log2n, kind, q, stream) : launch_padded(prec, log2n, kind, q, stream);
     }
     if (kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED) {
         FftR2r r;
@@ -173,6 +176,12 @@ static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftP
     b.kspec = blu;
     b.chirp = blu ? static_cast<const char*>(blu) + (size_t(1) << log2m) * (prec == DFFT_F64 ? 16 : 8) : nullptr;
     b.scale = scale;
+    if (w) {
+        FftBluesteinW bw;
+        static_cast<FftBluestein&>(bw) = b;
+        bw.w = w;
+        return launch_bluestein(prec, log2m, kind, bw, stream);
+    }
     return launch_bluestein(prec, log2m, kind, b, stream);
 }
 
@@ -457,6 +466,9 @@ struct Step {
     // 0: never scaled (copy passes, other precisions)
     int share_num = 0, share_den = 0;
     bool sign = false;
+    // weighted plans (dfft_plan_set_weights): an FFT pass that multiplies its spectral side by the weights of its axis (the
+    // plan's pointer for `axis` at exec time, none while it is null): forward its stores, inverse its loads
+    bool weighted = false;
 };
 
 struct Schedule {
@@ -507,6 +519,10 @@ struct dfft_plan_s {
     size_t batch = 1;         // fields per exec, back to back in every caller buffer (dfft_plan_create_batched)
     size_t comps = 1;         // values per grid point, interleaved (dfft_plan_create_interleaved); esize stays one value's
     double scale[2] = {1.0, 1.0};  // [fwd/inv] output scale (dfft_plan_set_scale), applied by the steps marked final_store
+    // dfft_plan_set_weights: the caller's per-axis spectral weights (device pointers, null = all ones), read by the steps
+    // marked weighted at every exec.  weighted: the first call came before any schedule was built.
+    const void* weights[3] = {nullptr, nullptr, nullptr};
+    bool weighted = false;
     // dfft_plan_create_boxes: every rank's box of the physical grid (in_boxes) and of the output grid (out_boxes), in rank
     // order; empty where that side has the natural layout.  box_direct: their reshapes push and gather over peer memory
     // (comm_method Peer2Peer), otherwise they run through an NCCL all-to-all
@@ -664,9 +680,10 @@ static bool all_axes(const dfft_plan_s* p) { return p->taxes[0] && p->taxes[1] &
 // Interleaved plans (C > 1 values per point) run it too: those kernels address one value per point.  So do plans with a
 // box that is not the natural layout: their reshape steps wrap the sequential schedule (wrap_boxes).  And embedded plans
 // (dfft_plan_set_strides): the other forms read and write dense caller arrays, and every rank must run the same form.
+// Weighted plans (dfft_plan_set_weights) too: only the single-axis passes have weighted twins.
 static bool alt_schedules(const dfft_plan_s* p) {
     return pow2_axes(p) && !is_half(p->prec) && !is_r2r(p->g.transform) && all_axes(p) && !p->g.padded() && !p->g.pruned() && p->comps == 1 && !p->boxed() &&
-           !p->embedded();
+           !p->embedded() && !p->weighted;
 }
 
 // Row pitch, in elements (complex units; reals for DCT / DST plans), of the z-contiguous side of the caller's buffers that
@@ -684,7 +701,7 @@ static long long z_row_pitch(const dfft_plan_s* p) {
 static bool zy_fused(const dfft_plan_s* p, int inverse, int d) {
     const Geometry& g = p->g;
     if (p->P != 1 || is_half(p->prec) || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || g.pruned() || p->comps > 1 ||
-        p->boxed() || p->embedded())
+        p->boxed() || p->embedded() || p->weighted)
         return false;
     if (g.ny != g.nz || !zy_fused_length(ilog2_exact(g.ny))) return false;
     // the fused stage reads and writes the blocked hand-over layout of the x pass
@@ -740,7 +757,7 @@ constexpr size_t BATCH_SMALL_MIN = 2;
 static bool batch_small(const dfft_plan_s* p, int d) {
     const Geometry& g = p->g;
     if (p->P != 1 || is_half(p->prec) || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || g.pruned() || p->comps > 1 ||
-        p->boxed() || p->embedded())
+        p->boxed() || p->embedded() || p->weighted)
         return false;
     if (g.nx != g.ny || g.ny != g.nz || !batch_small_length(ilog2_exact(g.nx))) return false;
     return p->batch >= BATCH_SMALL_MIN && p->batch * g.nx <= 0x7fffffff;
@@ -1941,7 +1958,8 @@ static cudaError_t run_pass_step(const dfft_plan_s* p, const Schedule& sc, const
                 const size_t n = s.n ? s.n : size_t(1) << s.log2n;
                 int hole[4];
                 pass_hole(s.kind, n, s.keep, s.data, hole);
-                e = launch_fft_pass(p->prec, s.kind, n, prm, s.blu, scale, ss, s.r2r, s.keep || s.data ? hole : nullptr);
+                const void* w = s.weighted ? p->weights[s.axis] : nullptr;  // null: the unweighted kernel
+                e = launch_fft_pass(p->prec, s.kind, n, prm, s.blu, scale, ss, s.r2r, s.keep || s.data || w ? hole : nullptr, w);
             }
             break;
         case KERNEL_ZY_FUSED: e = launch_zy_fused(p->prec, s.log2n, prm, prm_y, s.zyf, scale, ss); break;
@@ -2557,6 +2575,7 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
         // and the fused and batched stages (whose earlier phase writes only the work area, or `out` inside the same launch).
         // tests/test_scale.py replays every such schedule and checks that each output value is scaled exactly once.
         for (Step& s : sc.steps) s.final_store = s.type == STEP_PASS && s.out_user == 2;
+        for (Step& s : sc.steps) s.weighted = p->weighted && s.type == STEP_PASS && s.kernel == KERNEL_PASS && !is_copy(s.kind);
         if (is_half(p->prec)) split_scale(p, sc);
         // In place the buffer also holds intermediates: its views from slot D1 are marked after the final stores.
         // tests/test_inplace.py replays these schedules on one address range.
@@ -3394,6 +3413,30 @@ int dfft_zy_trace_copy(dfft_plan_t p, int inverse, void* host, size_t bytes) {
 }
 #endif
 
+int dfft_plan_set_weights(dfft_plan_t p, const void* const weights[3]) {
+    if (!p || !weights) return fail(DFFT_ERR_INVALID, "null plan / weights");
+    if (p->comps > 1) return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans of more than one component have no spectral weights");
+    if (is_r2r(p->g.transform)) return fail(DFFT_ERR_UNSUPPORTED, "real-to-real plans (DCT / DST and per-axis kinds) have no spectral weights");
+    if (is_half(p->prec)) return refuse_half("spectral weights");
+    for (int a = 0; a < 3; ++a)
+        if ((uintptr_t)weights[a] % p->esize)
+            return fail(DFFT_ERR_INVALID, std::string("weights[") + std::to_string(a) + "] must be aligned to its " + std::to_string(p->esize) + "-byte element");
+    // the schedules of unweighted plans may run stages that have no weighted twins
+    if (!p->weighted && p->axes_fixed)
+        return fail(DFFT_ERR_STATE, "set the weights for the first time before the first exec, dfft_plan_tune or dfft_plan_describe");
+    for (int a = 0; a < 3; ++a) p->weights[a] = weights[a];
+    p->weighted = true;
+    // a step whose pointer turns from null to a table launches another kernel: run each direction eagerly before a capture
+    for (auto& dir : p->sched)
+        for (Schedule& sc : dir) sc.executed = false;
+    return DFFT_SUCCESS;
+}
+int dfft_plan_get_weights(dfft_plan_t p, const void* weights[3]) {
+    if (!p || !weights) return fail(DFFT_ERR_INVALID, "null plan / weights");
+    for (int a = 0; a < 3; ++a) weights[a] = p->weights[a];
+    return DFFT_SUCCESS;
+}
+
 int dfft_plan_get_scale(dfft_plan_t p, double* forward_scale, double* inverse_scale) {
     if (!p) return fail(DFFT_ERR_INVALID, "null plan");
     if (forward_scale) *forward_scale = p->scale[0];
@@ -3525,6 +3568,7 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
     p->tune_report.clear();
     if (cands.size() == 1) {
         p->tune_report = is_half(p->prec)       ? "sequential schedule (no alternatives for this plan: 16-bit plans run the sequential schedule)"
+                         : p->weighted          ? "sequential schedule (no alternatives for this plan: weighted plans run the sequential schedule)"
                          : is_r2r(p->g.transform) ? "sequential schedule (no alternatives for this plan: DCT / DST plans run the sequential schedule)"
                          : !all_axes(p)         ? "sequential schedule (no alternatives for this plan: plans with a kept axis run the sequential schedule)"
                          : p->g.padded()        ? "sequential schedule (no alternatives for this plan: padded plans run the sequential schedule)"
@@ -3678,6 +3722,9 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
                     (p->g.pruned() ? ",\"data\":[" + std::to_string(p->g.mx) + "," + std::to_string(p->g.my) + "," + std::to_string(p->g.mz) + "]"
                                    : std::string()) +
                     (p->comps > 1 ? ",\"components\":" + std::to_string(p->comps) : std::string()) +
+                    (p->weighted ? ",\"weights\":[" + std::to_string(p->weights[0] ? 1 : 0) + "," + std::to_string(p->weights[1] ? 1 : 0) + "," +
+                                       std::to_string(p->weights[2] ? 1 : 0) + "]"
+                                 : std::string()) +
                     json_boxes("in_boxes", p->in_boxes) + json_boxes("out_boxes", p->out_boxes) +
                     json_strides("in_strides", p->in_embedded, p->in_strides) + json_strides("out_strides", p->out_embedded, p->out_strides) +
                     (p->batch > 1 ? ",\"batch\":" + std::to_string(p->batch) + ",\"field_in\":" + std::to_string(sc.field_in) +
@@ -3791,7 +3838,8 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
                  ",\"log2n\":" + std::to_string(s_.log2n) +
                  (s_.bluestein() || copy ? ",\"n\":" + std::to_string(s_.n) : std::string()) +
                  (s_.keep ? ",\"keep\":" + std::to_string(s_.keep) : std::string()) +
-                 (s_.data ? ",\"data\":" + std::to_string(s_.data) : std::string()) + ",\"A0\":" + std::to_string(s_.prm.A0) +
+                 (s_.data ? ",\"data\":" + std::to_string(s_.data) : std::string()) + (s_.weighted ? ",\"weighted\":1,\"axis\":" + std::to_string(s_.axis) : std::string()) +
+                 ",\"A0\":" + std::to_string(s_.prm.A0) +
                  ",\"A1\":" + std::to_string(s_.prm.A1) + ",\"B\":" + std::to_string(s_.prm.B) + ",\"inverse\":" + std::to_string(s_.prm.inverse) +
                  ",\"in_user\":" + std::to_string(s_.in_user) + ",\"out_user\":" + std::to_string(s_.out_user) + ",\"in\":";
             json_view(o, s_.prm.in, p->tabs);

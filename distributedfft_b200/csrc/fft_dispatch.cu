@@ -46,6 +46,14 @@ cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluest
     return dispatch<3, MAX_LOG2N>(prec, log2m, [&](auto t, auto l) { return launch_bluestein<decltype(t), decltype(l)::value>(kind, p, stream); });
 }
 
+cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluesteinW& p, cudaStream_t stream) {
+    return dispatch<3, MAX_LOG2N>(prec, log2m, [&](auto t, auto l) { return launch_bluestein<decltype(t), decltype(l)::value>(kind, p, stream); });
+}
+
+cudaError_t launch_weighted(int prec, int log2n, PassKind kind, const FftWeighted& p, cudaStream_t stream) {
+    return dispatch<1, MAX_LOG2N>(prec, log2n, [&](auto t, auto l) { return launch_weighted<decltype(t), decltype(l)::value>(kind, p, stream); });
+}
+
 cudaError_t launch_r2r(int prec, int log2n, PassKind kind, const FftR2r& p, bool hc, cudaStream_t stream) {
     return dispatch<1, MAX_LOG2N>(prec, log2n, [&](auto t, auto l) { return launch_r2r<decltype(t), decltype(l)::value>(kind, p, hc, stream); });
 }

@@ -237,21 +237,29 @@ cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStr
 
 template cudaError_t launch_pass<DFFT_T, DFFT_LOG2N>(PassKind, const FftParams&, double, cudaStream_t);
 
-template <typename T, int LOG2N, int TB>
-static cudaError_t launch_padded_tiled(const FftPadded& p, long long lines, cudaStream_t stream) {
-    using C = CtaFft<T, LOG2N, Shape<T, LOG2N>::LOG2E, TB, true>;
-    FftPadded q = p;
+// P: FftPadded (the padded twins) or FftWeighted (the weighted twins)
+template <typename T, int LOG2N, int TB, typename P>
+static cudaError_t launch_padded_tiled(const P& p, long long lines, cudaStream_t stream) {
+    constexpr int LOG2E = Shape<T, LOG2N>::LOG2E;
+    using C = CtaFft<T, LOG2N, LOG2E, TB, true>;
+    P q = p;
     q.tile_swz = tile_swz_for(p.tile_swz, p.A0, p.A1);
     const long long g = lines * ((p.B + TB - 1) / TB);
     if (g > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-    return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, Shape<T, LOG2N>::LOG2E, TB, true, false>, fft_c2c_padded_kernel<T, LOG2N, Shape<T, LOG2N>::LOG2E, TB, true, true>,
-                         nullptr, nullptr>(q, 1.0, unsigned(g), C::THREADS, C::SMEM_BYTES, stream);
+    if constexpr (std::is_same_v<P, FftWeighted>)
+        return launch_kernel<fft_c2c_weighted_kernel<T, LOG2N, LOG2E, TB, true, false>, fft_c2c_weighted_kernel<T, LOG2N, LOG2E, TB, true, true>, nullptr,
+                             nullptr>(q, 1.0, unsigned(g), C::THREADS, C::SMEM_BYTES, stream);
+    else
+        return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, LOG2E, TB, true, false>, fft_c2c_padded_kernel<T, LOG2N, LOG2E, TB, true, true>, nullptr,
+                             nullptr>(q, 1.0, unsigned(g), C::THREADS, C::SMEM_BYTES, stream);
 }
 
-// the padded twins (fft_c2c_padded_kernel, fft_r2c_padded_kernel, fft_c2r_padded_kernel): the tiles of launch_pass (TILED:
-// narrow or wide by its rule), one CTA per tile, the register-fed kernel only
-template <typename T, int LOG2N>
-cudaError_t launch_padded(PassKind kind, const FftPadded& p, cudaStream_t stream) {
+// the padded twins (fft_c2c_padded_kernel, fft_r2c_padded_kernel, fft_c2r_padded_kernel), or with P = FftWeighted the
+// weighted twins (fft_c2c_weighted_kernel, ...): the tiles of launch_pass (TILED: narrow or wide by its rule), one CTA per
+// tile, the register-fed kernel only
+template <typename T, int LOG2N, typename P>
+static cudaError_t launch_twin(PassKind kind, const P& p, cudaStream_t stream) {
+    constexpr bool W = std::is_same_v<P, FftWeighted>;
     using S = Shape<T, LOG2N>;
     constexpr int LOG2E = S::LOG2E;
     const long long lines = (long long)p.A0 * p.A1;
@@ -268,8 +276,13 @@ cudaError_t launch_padded(PassKind kind, const FftPadded& p, cudaStream_t stream
             using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
             if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
             if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, false, false>, fft_c2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, false, true>,
-                                 nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+            if constexpr (W)
+                return launch_kernel<fft_c2c_weighted_kernel<T, LOG2N, LOG2E, S::TBC, false, false>,
+                                     fft_c2c_weighted_kernel<T, LOG2N, LOG2E, S::TBC, false, true>, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS,
+                                                                                                                      C::SMEM_BYTES, stream);
+            else
+                return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, false, false>, fft_c2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, false, true>,
+                                     nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
         }
         case PASS_C2C_TILED: {
             if (p.B <= 0) return cudaSuccess;
@@ -288,37 +301,62 @@ cudaError_t launch_padded(PassKind kind, const FftPadded& p, cudaStream_t stream
             using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
             if ((kind == PASS_R2C ? p.in.nseg : p.out.nseg) != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
             if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            if (kind == PASS_R2C) {
-                constexpr auto k = fft_r2c_padded_kernel<T, LOG2N, LOG2E, S::TBC>;
+            if constexpr (W) {
+                if (kind == PASS_R2C) {
+                    constexpr auto k = fft_r2c_weighted_kernel<T, LOG2N, LOG2E, S::TBC>;
+                    return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+                }
+                constexpr auto k = fft_c2r_weighted_kernel<T, LOG2N, LOG2E, S::TBC>;
+                return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+            } else {
+                if (kind == PASS_R2C) {
+                    constexpr auto k = fft_r2c_padded_kernel<T, LOG2N, LOG2E, S::TBC>;
+                    return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+                }
+                constexpr auto k = fft_c2r_padded_kernel<T, LOG2N, LOG2E, S::TBC>;
                 return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
             }
-            constexpr auto k = fft_c2r_padded_kernel<T, LOG2N, LOG2E, S::TBC>;
-            return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
         }
         default: return cudaErrorInvalidValue;
     }
 }
 
-template cudaError_t launch_padded<DFFT_T, DFFT_LOG2N>(PassKind, const FftPadded&, cudaStream_t);
-
-#if DFFT_LOG2N >= 3
-template <typename T, int LOG2M, int TB, bool TILED>
-static cudaError_t launch_bluestein_tiles(const FftBluestein& p, long long grid, cudaStream_t stream) {
-    using C = CtaFft<T, LOG2M, Shape<T, LOG2M>::LOG2E, TB, TILED>;
-    if (grid <= 0) return cudaSuccess;
-    if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-    return launch_kernel<fft_bluestein_kernel<T, LOG2M, Shape<T, LOG2M>::LOG2E, TB, TILED, false>,
-                         fft_bluestein_kernel<T, LOG2M, Shape<T, LOG2M>::LOG2E, TB, TILED, true>, nullptr, nullptr>(
-        p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+template <typename T, int LOG2N>
+cudaError_t launch_padded(PassKind kind, const FftPadded& p, cudaStream_t stream) {
+    return launch_twin<T, LOG2N>(kind, p, stream);
+}
+template <typename T, int LOG2N>
+cudaError_t launch_weighted(PassKind kind, const FftWeighted& p, cudaStream_t stream) {
+    if (!p.w) return cudaErrorInvalidValue;
+    return launch_twin<T, LOG2N>(kind, p, stream);
 }
 
-template <typename T, int LOG2M>
-cudaError_t launch_bluestein(PassKind kind, const FftBluestein& p_in, cudaStream_t stream) {
+template cudaError_t launch_padded<DFFT_T, DFFT_LOG2N>(PassKind, const FftPadded&, cudaStream_t);
+template cudaError_t launch_weighted<DFFT_T, DFFT_LOG2N>(PassKind, const FftWeighted&, cudaStream_t);
+
+#if DFFT_LOG2N >= 3
+// P: FftBluestein, or FftBluesteinW for the weighted twin
+template <typename T, int LOG2M, int TB, bool TILED, typename P>
+static cudaError_t launch_bluestein_tiles(const P& p, long long grid, cudaStream_t stream) {
+    constexpr int LOG2E = Shape<T, LOG2M>::LOG2E;
+    using C = CtaFft<T, LOG2M, LOG2E, TB, TILED>;
+    if (grid <= 0) return cudaSuccess;
+    if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+    if constexpr (std::is_same_v<P, FftBluesteinW>)
+        return launch_kernel<fft_bluestein_weighted_kernel<T, LOG2M, LOG2E, TB, TILED, false>, fft_bluestein_weighted_kernel<T, LOG2M, LOG2E, TB, TILED, true>,
+                             nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+    else
+        return launch_kernel<fft_bluestein_kernel<T, LOG2M, LOG2E, TB, TILED, false>, fft_bluestein_kernel<T, LOG2M, LOG2E, TB, TILED, true>, nullptr,
+                             nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+}
+
+template <typename T, int LOG2M, typename P>
+static cudaError_t launch_bluestein_lines(PassKind kind, const P& p_in, cudaStream_t stream) {
     using S = Shape<T, LOG2M>;
     if (p_in.n < 1 || 2 * (long long)p_in.n - 1 > (1LL << LOG2M) || !p_in.chirp || !p_in.kspec) return cudaErrorInvalidValue;
     const long long lines = (long long)p_in.A0 * p_in.A1;
     if (lines <= 0) return cudaSuccess;
-    FftBluestein p = p_in;
+    P p = p_in;
     if (kind == PASS_C2C_CONTIG) {
         if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
         return launch_bluestein_tiles<T, LOG2M, S::TBC, false>(p, (lines + S::TBC - 1) / S::TBC, stream);
@@ -329,7 +367,18 @@ cudaError_t launch_bluestein(PassKind kind, const FftBluestein& p_in, cudaStream
     return launch_bluestein_tiles<T, LOG2M, S::TBT, true>(p, lines * ((p.B + S::TBT - 1) / S::TBT), stream);
 }
 
+template <typename T, int LOG2M>
+cudaError_t launch_bluestein(PassKind kind, const FftBluestein& p, cudaStream_t stream) {
+    return launch_bluestein_lines<T, LOG2M>(kind, p, stream);
+}
+template <typename T, int LOG2M>
+cudaError_t launch_bluestein(PassKind kind, const FftBluesteinW& p, cudaStream_t stream) {
+    if (!p.w) return cudaErrorInvalidValue;
+    return launch_bluestein_lines<T, LOG2M>(kind, p, stream);
+}
+
 template cudaError_t launch_bluestein<DFFT_T, DFFT_LOG2N>(PassKind, const FftBluestein&, cudaStream_t);
+template cudaError_t launch_bluestein<DFFT_T, DFFT_LOG2N>(PassKind, const FftBluesteinW&, cudaStream_t);
 #endif
 
 template <typename T, int LOG2N, int TB, bool TILED>

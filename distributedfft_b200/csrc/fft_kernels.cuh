@@ -440,6 +440,15 @@ struct FftPadded : FftScaled {
 // index in the view of line position n, -1 in the hole
 __device__ __forceinline__ int keep_index(int n, int lo, int hi) { return n < lo ? n : (n < hi ? -1 : n - (hi - lo)); }
 
+// ---- weighted passes (dfft_plan_set_weights) ------------------------------------------------------------------------
+// A weighted pass multiplies each value of its spectral side by w[m], m the value's index in the spectral view (the K
+// stored points of a padded side): forward as it stores, inverse as it loads, before the transform.  The weighted twins
+// are the padded twins with the table: holes (empty for plans without padding) and the scale are runtime values, so one
+// instantiation per kind and length serves every weighted plan.  The unweighted kernels do not change.
+struct FftWeighted : FftPadded {
+    const void* w;  // cx<T>[spectral points of the line]: Kx, Ky, Kz (C2C) or Kz/2 + 1 (R2C / C2R)
+};
+
 // store policy of the padded twins: plain stores, scaled when s != 1 (a runtime value)
 template <typename T>
 struct MemRtScaled {
@@ -456,11 +465,13 @@ __device__ __forceinline__ void l2_discard(const void* p) { asm volatile("discar
 // PADDED: the loaded side keeps the line positions outside the hole [ld_lo, ld_hi), the stored side those outside
 // [st_lo, st_hi) (FftPadded); a side with an empty hole takes the plain path.
 // ILV (CONTIG mapping): lines of an interleaved z pass, strided by sN along n (TileCoord)
+// WEIGHTED: the spectral side's values times w[m] (FftWeighted), m their index in its view: inverse after the load,
+// forward before the store
 template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, typename M, typename Hook = NoGatherHook, bool PADDED = false,
-          bool ILV = false>
+          bool ILV = false, bool WEIGHTED = false>
 __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<T>* sm, unsigned long long* tab_in, unsigned long long* tab_out,
                                          bool multi, const M& mem, const Hook& after_gather = {}, int ld_lo = 0, int ld_hi = 0, int st_lo = 0,
-                                         int st_hi = 0) {
+                                         int st_hi = 0, const cx<T>* w = nullptr) {
     using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
     using S = typename StoredOf<T, M>::type;
     using LA = LineAccess<T, C::LINES, S>;
@@ -506,6 +517,13 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
 #pragma unroll
             for (int e = 0; e < E; ++e) v[e] = mem.ld(STRIDED ? in.at(j + e * TPL) : in.at1(j + e * TPL));
         }
+        if constexpr (WEIGHTED && INV) {
+#pragma unroll
+            for (int e = 0; e < E; ++e) {
+                const int m = PADDED && ld_lo < ld_hi ? keep_index(j + e * TPL, ld_lo, ld_hi) : j + e * TPL;
+                if (m >= 0) v[e] = cmul(v[e], ld_tw(w, m));
+            }
+        }
         if constexpr (INV) {
 #pragma unroll
             for (int e = 0; e < E; ++e) v[e] = cswap(v[e]);
@@ -517,6 +535,16 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
 
     C::template stages<0>(v, j, t, sm, reinterpret_cast<const cx<T>*>(p.tw), after_gather);
 
+    if constexpr (WEIGHTED && !INV) {
+        if (tc.valid) {
+#pragma unroll
+            for (int e = 0; e < E; ++e) {
+                const int m = PADDED && st_lo < st_hi ? keep_index(j + e * TPL, st_lo, st_hi) : j + e * TPL;
+                cx<T>& x = v[C::Core::final_slot(e)];
+                if (m >= 0) x = cmul(x, ld_tw(w, m));
+            }
+        }
+    }
     if (tc.valid) {
         if (PADDED && st_lo < st_hi) {
 #pragma unroll
@@ -728,6 +756,21 @@ fft_c2c_padded_kernel(const __grid_constant__ FftPadded p) {
     c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV, MemRtScaled<T>, NoGatherHook, true>(p, blockIdx.x, sm, tab_in, tab_out, multi,
                                                                                  MemRtScaled<T>{p.scale != 1.0, T(p.scale)}, {}, p.ld_lo, p.ld_hi,
                                                                                  p.st_lo, p.st_hi);
+}
+
+// weighted twin of fft_c2c_kernel and fft_c2c_padded_kernel (FftWeighted): one CTA per tile
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV>
+__global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
+fft_c2c_weighted_kernel(const __grid_constant__ FftWeighted p) {
+    using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
+    unsigned long long* tab_in = reinterpret_cast<unsigned long long*>(smem_raw + C::TILE_BYTES);
+    unsigned long long* tab_out = tab_in + C::LINES * MAXSEG;
+    const bool multi = p.in.nseg > 1 || p.out.nseg > 1;
+    c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV, MemRtScaled<T>, NoGatherHook, true, false, true>(
+        p, blockIdx.x, sm, tab_in, tab_out, multi, MemRtScaled<T>{p.scale != 1.0, T(p.scale)}, {}, p.ld_lo, p.ld_hi, p.st_lo, p.st_hi,
+        reinterpret_cast<const cx<T>*>(p.w));
 }
 
 // ---- mbarrier of an asynchronous tile copy (fft_c2c_tma_kernel, fft_zy_fused_kernel) ------------------------------
@@ -1466,7 +1509,8 @@ __device__ __forceinline__ cx<T> shfl_cx(cx<T> v, int src_lane) {
 // PADDED (P = FftPadded): the pairs m >= p.ld_lo read as zero, the points k >= p.st_lo are not stored; the scale is
 // p.scale at run time.
 // S: the stored element, of both sides (the real side in pairs: cx16<H> holds two 16-bit reals).
-template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED, bool PADDED, typename P, typename S = cx<T>>
+// WEIGHTED (P = FftWeighted): X[k] times p.w[k] as it is stored.
+template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED, bool PADDED, typename P, typename S = cx<T>, bool WEIGHTED = false>
 __device__ __forceinline__ void r2c_lines(const P& p) {
     using C = CtaFft<T, LOG2M, LOG2E, TB, false>;
     using LA = LineAccess<T, C::LINES, S>;
@@ -1517,7 +1561,13 @@ __device__ __forceinline__ void r2c_lines(const P& p) {
         const cx<T> xo = cx<T>{T(0.5) * d.y, T(-0.5) * d.x};  // -i/2 * d
         const cx<T> tt = cmul(ld_tw(tw2, k), xo);
         if (valid) {
-            if constexpr (PADDED) {
+            if constexpr (WEIGHTED) {
+                static_assert(PADDED, "the weighted R2C pass is the padded twin's");
+                const cx<T>* w = reinterpret_cast<const cx<T>*>(p.w);
+                const MemRtScaled<T> mem{p.scale != 1.0, T(p.scale)};
+                if (k < p.st_lo) mem.st(out.at1(k), cmul(cadd(xe, tt), ld_tw(w, k)));
+                if (M - k < p.st_lo) mem.st(out.at1(M - k), cmul(cconj(csub(xe, tt)), ld_tw(w, M - k)));
+            } else if constexpr (PADDED) {
                 const MemRtScaled<T> mem{p.scale != 1.0, T(p.scale)};
                 if (k < p.st_lo) mem.st(out.at1(k), cadd(xe, tt));
                 if (M - k < p.st_lo) mem.st(out.at1(M - k), cconj(csub(xe, tt)));
@@ -1548,6 +1598,13 @@ fft_r2c_padded_kernel(const __grid_constant__ FftPadded p) {
     r2c_lines<T, LOG2M, LOG2E, TB, false, true>(p);
 }
 
+// weighted twin of fft_r2c_kernel and fft_r2c_padded_kernel (FftWeighted)
+template <typename T, int LOG2M, int LOG2E, int TB>
+__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
+fft_r2c_weighted_kernel(const __grid_constant__ FftWeighted p) {
+    r2c_lines<T, LOG2M, LOG2E, TB, false, true, FftWeighted, cx<T>, true>(p);
+}
+
 // the R2C z pass of 16-bit plans: fft_r2c_kernel's f32 line with cx16<H> loads and stores (fft_c2c16_kernel)
 template <typename H, int LOG2M, int LOG2E, int TB, bool SCALED>
 __global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<float, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
@@ -1558,7 +1615,8 @@ fft_r2c16_kernel(const __grid_constant__ KParams<SCALED> p) {
 // ---- C2R pass (CONTIG): M+1 complex points -> real line of 2M points, unnormalised -----------------------
 // PADDED (P = FftPadded): the points k >= p.ld_lo read as zero, their partner loads X[M - k] as well; the pairs
 // m >= p.st_lo are not stored; the scale is p.scale at run time.
-template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED, bool PADDED, typename P, typename S = cx<T>>
+// WEIGHTED (P = FftWeighted): X[k] and its partner X[M - k] times p.w at their index as they are loaded.
+template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED, bool PADDED, typename P, typename S = cx<T>, bool WEIGHTED = false>
 __device__ __forceinline__ void c2r_lines(const P& p) {
     using C = CtaFft<T, LOG2M, LOG2E, TB, false>;
     using LA = LineAccess<T, C::LINES, S>;
@@ -1591,6 +1649,13 @@ __device__ __forceinline__ void c2r_lines(const P& p) {
 #pragma unroll
                 for (int e = 0; e < E; ++e) xk[e] = j + e * TPL < p.ld_lo ? ld_elem<T>(in.at1(j + e * TPL)) : cx<T>{T(0), T(0)};
                 if (j == 0 && M < p.ld_lo) xM = ld_elem<T>(in.at1(M));
+                if constexpr (WEIGHTED) {
+                    const cx<T>* w = reinterpret_cast<const cx<T>*>(p.w);
+#pragma unroll
+                    for (int e = 0; e < E; ++e)
+                        if (j + e * TPL < p.ld_lo) xk[e] = cmul(xk[e], ld_tw(w, j + e * TPL));
+                    if (j == 0 && M < p.ld_lo) xM = cmul(xM, ld_tw(w, M));
+                }
             } else {
 #pragma unroll
                 for (int e = 0; e < E; ++e) xk[e] = ld_elem<T>(in.at1(j + e * TPL));
@@ -1621,7 +1686,11 @@ __device__ __forceinline__ void c2r_lines(const P& p) {
     auto build = [&](int k) {
         cx<T> xk{T(0), T(0)}, xm{T(0), T(0)};
         if (valid) {
-            if constexpr (PADDED) {
+            if constexpr (WEIGHTED) {
+                const cx<T>* w = reinterpret_cast<const cx<T>*>(p.w);
+                if (k < p.ld_lo) xk = cmul(ld_elem<T>(in.at1(k)), ld_tw(w, k));
+                if (M - k < p.ld_lo) xm = cconj(cmul(ld_elem<T>(in.at1(M - k)), ld_tw(w, M - k)));
+            } else if constexpr (PADDED) {
                 if (k < p.ld_lo) xk = ld_elem<T>(in.at1(k));
                 if (M - k < p.ld_lo) xm = cconj(ld_elem<T>(in.at1(M - k)));
             } else {
@@ -1670,6 +1739,13 @@ fft_c2r_padded_kernel(const __grid_constant__ FftPadded p) {
     c2r_lines<T, LOG2M, LOG2E, TB, false, true>(p);
 }
 
+// weighted twin of fft_c2r_kernel and fft_c2r_padded_kernel (FftWeighted)
+template <typename T, int LOG2M, int LOG2E, int TB>
+__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
+fft_c2r_weighted_kernel(const __grid_constant__ FftWeighted p) {
+    c2r_lines<T, LOG2M, LOG2E, TB, false, true, FftWeighted, cx<T>, true>(p);
+}
+
 // the C2R z pass of 16-bit plans: fft_c2r_kernel's f32 line with cx16<H> loads and stores (fft_c2c16_kernel)
 template <typename H, int LOG2M, int LOG2E, int TB, bool SCALED>
 __global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<float, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
@@ -1690,9 +1766,14 @@ struct FftBluestein : FftParams {
     double scale;       // output scale, applied when != 1 (rounded to the kernel's precision once)
 };
 
-template <typename T, int LOG2M, int LOG2E, int TB, bool TILED, bool INV>
-__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
-fft_bluestein_kernel(const __grid_constant__ FftBluestein p) {
+// weighted Bluestein pass (dfft_plan_set_weights): w[k], k < n, multiplies X_k forward as it is stored and x_k inverse as it
+// is loaded
+struct FftBluesteinW : FftBluestein {
+    const void* w;
+};
+
+template <typename T, int LOG2M, int LOG2E, int TB, bool TILED, bool INV, bool WEIGHTED, typename P>
+__device__ __forceinline__ void bluestein_lines(const P& p) {
     using C = CtaFft<T, LOG2M, LOG2E, TB, TILED>;
     using LA = LineAccess<T, C::LINES>;
     using TC = TileCoord<C, TILED, TB>;
@@ -1724,7 +1805,8 @@ fft_bluestein_kernel(const __grid_constant__ FftBluestein p) {
         const int k = j + e * TPL;
         v[e] = cx<T>{T(0), T(0)};
         if (tc.valid && k < n) {
-            const cx<T> x = ld_elem<T>(TILED ? in.at(k) : in.at1(k));
+            cx<T> x = ld_elem<T>(TILED ? in.at(k) : in.at1(k));
+            if constexpr (WEIGHTED && INV) x = cmul(x, ld_tw(reinterpret_cast<const cx<T>*>(p.w), k));
             v[e] = cmul(INV ? cswap(x) : x, ld_tw(chirp, k));
         }
     }
@@ -1744,10 +1826,23 @@ fft_bluestein_kernel(const __grid_constant__ FftBluestein p) {
         if (tc.valid && k < n) {
             cx<T> x = cmul(ld_tw(chirp, k), cswap(z[C::Core::final_slot(e)]));
             if (INV) x = cswap(x);
+            if constexpr (WEIGHTED && !INV) x = cmul(x, ld_tw(reinterpret_cast<const cx<T>*>(p.w), k));
             if (scaled) x = cscale<T>(x, s);
             st_elem<T>(TILED ? out.at(k) : out.at1(k), x);
         }
     }
+}
+
+template <typename T, int LOG2M, int LOG2E, int TB, bool TILED, bool INV>
+__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
+fft_bluestein_kernel(const __grid_constant__ FftBluestein p) {
+    bluestein_lines<T, LOG2M, LOG2E, TB, TILED, INV, false>(p);
+}
+
+template <typename T, int LOG2M, int LOG2E, int TB, bool TILED, bool INV>
+__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
+fft_bluestein_weighted_kernel(const __grid_constant__ FftBluesteinW p) {
+    bluestein_lines<T, LOG2M, LOG2E, TB, TILED, INV, true>(p);
 }
 
 // ---- real-to-real pass: DCT-II / DCT-III, DST-II / DST-III and R2HC / HC2R of real N-point lines ------------------------
@@ -2225,6 +2320,12 @@ template <typename T, int LOG2N>
 cudaError_t launch_padded(PassKind kind, const FftPadded& p, cudaStream_t stream);
 cudaError_t launch_padded(int prec, int log2n, PassKind kind, const FftPadded& p, cudaStream_t stream);
 
+// weighted pass (FftWeighted, dfft_plan_set_weights): the padded pass with p.w multiplying its spectral side (holes may be
+// empty); the weighted twins, the tiles of launch_padded
+template <typename T, int LOG2N>
+cudaError_t launch_weighted(PassKind kind, const FftWeighted& p, cudaStream_t stream);
+cudaError_t launch_weighted(int prec, int log2n, PassKind kind, const FftWeighted& p, cudaStream_t stream);
+
 // fused z + y stage (fft_zy_fused_kernel), instantiated for the lengths zy_fused_length accepts.  pz: the z pass, py: the y
 // pass, f: counters and plane groups (f.order.na / nb are filled in here).  Every launch of one step must use the same
 // counters and the same grid (zy_launch_of), which the launcher's fixed grid for a given work list provides.  scale: of the
@@ -2248,6 +2349,10 @@ cudaError_t launch_batch_small(int prec, int log2n, const void* in, void* out, l
 template <typename T, int LOG2M>
 cudaError_t launch_bluestein(PassKind kind, const FftBluestein& p, cudaStream_t stream);
 cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluestein& p, cudaStream_t stream);
+// its weighted twin (fft_bluestein_weighted_kernel)
+template <typename T, int LOG2M>
+cudaError_t launch_bluestein(PassKind kind, const FftBluesteinW& p, cudaStream_t stream);
+cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluesteinW& p, cudaStream_t stream);
 
 // R2R pass of 2^LOG2N-point real lines: kind PASS_R2R_CONTIG (sN == 1, line pairs) or PASS_R2R_TILED (column pairs), views
 // in reals, one CTA per tile; p.scale scales the stores.  hc: R2HC / HC2R (fft_r2hc_kernel), otherwise DCT / DST

@@ -432,6 +432,42 @@ class MPIcuFFT:
         check(lib().dfft_plan_get_scale(self._h, C.byref(f), C.byref(i)))
         return f.value, i.value
 
+    # -- spectral weights (not in the reference) --------------------------------------------------
+    def setWeights(self, wx=None, wy=None, wz=None):
+        """Per-axis spectral weights (dfft_plan_set_weights): forward execs return W * F(x), inverse ones F^-1(W * X), with
+        W[kx, ky, kz] = wx[kx] * wy[ky] * wz[kz] multiplied inside the FFT passes.  Each is None (all ones) or a contiguous
+        1-D complex128 (double plans) / complex64 (float plans) CUDA tensor on the plan's device, as long as the axis's
+        spectral extent: getSpectralSize(), Kz // 2 + 1 on z for R2C / C2R.  The plan reads the tensors at every exec and
+        keeps references to them; rewrite them in place between execs, or call again to re-point.  The first call must come
+        before the first exec, tune or describe.  C2R plans: make W Hermitian (e.g. zero the Nyquist entry of i k)."""
+        import torch
+
+        self._need()
+        ptrs = (C.c_void_p * 3)()
+        want = {F64: torch.complex128, F32: torch.complex64}.get(self.precision)
+        if want is None:  # 16-bit plans: the library's refusal
+            check(lib().dfft_plan_set_weights(self._h, ptrs))
+        k = list(self.getSpectralSize())
+        if self.transform == R2C:
+            k[2] = k[2] // 2 + 1
+        for a, (name, w) in enumerate((("wx", wx), ("wy", wy), ("wz", wz))):
+            if w is None:
+                continue
+            if not isinstance(w, torch.Tensor) or w.dtype != want:
+                raise TypeError(f"{name} must be a {want} tensor")
+            if not w.is_cuda or w.device.index != self.comm.device:
+                raise ValueError(f"{name} must be on cuda:{self.comm.device}, the plan's device")
+            if w.dim() != 1 or not w.is_contiguous() or w.numel() != k[a]:
+                raise ValueError(f"{name} must be a contiguous 1-D tensor of {k[a]} values, got shape {tuple(w.shape)}")
+            ptrs[a] = w.data_ptr()
+        check(lib().dfft_plan_set_weights(self._h, ptrs))
+        self._weights = (wx, wy, wz)  # the plan reads these at every exec: keep them alive
+
+    def getWeights(self):
+        """(wx, wy, wz): the tensors given to the last setWeights, None where none was given."""
+        self._need()
+        return getattr(self, "_weights", (None, None, None))
+
     # -- timer -----------------------------------------------------------------------------------
     def enableTimer(self, on: bool = True):
         check(lib().dfft_timer_enable(self._h, 1 if on else 0))

@@ -387,6 +387,34 @@ int dfft_exec_r2r_async(dfft_plan_t plan, void* out, const void* in, int directi
 int dfft_plan_set_scale(dfft_plan_t plan, double forward_scale, double inverse_scale);
 /* Either pointer may be NULL. */
 int dfft_plan_get_scale(dfft_plan_t plan, double* forward_scale, double* inverse_scale);
+/* Per-axis spectral weights (not in the reference; cuFFT offers this through load and store callbacks only).  Every exec
+ * multiplies the spectrum by the separable table W[kx,ky,kz] = wx[kx] * wy[ky] * wz[kz]: derivatives (i k), half-cell
+ * shifts (exp(-+i pi k / N)) and separable filters without an extra sweep over the spectrum.
+ *   - weights[0], [1], [2] belong to the x, y and z axis, the order of dfft_plan_create_r2r's kinds.  Each is NULL (all
+ *     ones) or a device pointer on the plan's device to complex values of the plan's precision (double2 for DFFT_F64,
+ *     float2 for DFFT_F32), as many as the axis's spectral extent: Kx, Ky, Kz for C2C, Kz / 2 + 1 on z for R2C / C2R (K = N
+ *     without padding).  Entry m belongs to spectral position m as the caller stores it: numpy's fftfreq order for C2C,
+ *     the K stored positions of padded and pruned plans.
+ *   - Forward: out = W * F(x).  Inverse: out = F^-1(W * X).  Both unnormalised, then times the direction's output scale
+ *     (dfft_plan_set_scale).  Partial d: the weights of the first d axes in z, y, x order; kept axes
+ *     (dfft_plan_set_transform_axes) ignore theirs.  C2R transforms the stored half spectrum times W: for a real result to
+ *     mean anything W must be Hermitian, e.g. i k with its Nyquist entry zeroed.
+ *   - The pass that transforms an axis multiplies its spectral side as the values pass through the registers: forward as
+ *     it stores, inverse as it loads.  No extra launch and no extra memory traffic beyond one table read per value.
+ *   - The caller owns the arrays.  The plan keeps the pointers, not copies: every exec reads the current contents, which
+ *     may change between execs in stream order like an input buffer.
+ *   - The first call must come before the plan builds a schedule (its first exec, dfft_plan_tune or dfft_plan_describe),
+ *     DFFT_ERR_STATE otherwise; it makes the plan a weighted plan, which runs the sequential schedule (no fused z + y stage,
+ *     batched stage or overlapped schedule).  Later calls may re-point any axis, or set it to NULL, at any time.
+ *   - Local to the calling rank: every rank of a multi-rank plan makes the first call or none does, each with its own
+ *     pointers to the same values.  Geometry-only plans accept any pointer value and never dereference it.
+ *   - A CUDA graph keeps the pointers in effect when it was captured and reads their contents at replay.  A call makes
+ *     every direction run eagerly once more before it can be captured again (DFFT_ERR_STATE otherwise).
+ *   - DFFT_ERR_INVALID: a null plan or array, or a pointer not aligned to its element.  DFFT_ERR_UNSUPPORTED: interleaved
+ *     plans of more than one component, real-to-real plans (DCT / DST and per-axis kinds) and 16-bit plans. */
+int dfft_plan_set_weights(dfft_plan_t plan, const void* const weights[3]);
+/* The pointers set last, NULL where none was set. */
+int dfft_plan_get_weights(dfft_plan_t plan, const void* weights[3]);
 /* Untransformed axes (not in the reference; FFTW's guru "howmany" dimensions, 2DECOMP&FFT's standalone transposes).
  * transform[0], [1], [2] belong to the x, y and z axis, the order of dfft_plan_create_r2r's kinds: 1 transforms that axis,
  * 0 keeps it.  A kept axis is redistributed exactly as a transformed one would be, but its values are not transformed: an

@@ -150,6 +150,12 @@ public:
     // normalised round trips use setScale(1, 1.0 / (Nx * Ny * Nz)).
     void setScale(double forward_scale, double inverse_scale) { DFFT_CALL(dfft_plan_set_scale(plan, forward_scale, inverse_scale)); }
     void getScale(double& forward_scale, double& inverse_scale) const { DFFT_CALL(dfft_plan_get_scale(plan, &forward_scale, &inverse_scale)); }
+    // not in the reference: per-axis spectral weights (dfft_plan_set_weights; after initFFT, the first call before the
+    // first exec).  Device arrays of complex T (nullptr = all ones); the plan reads them at every exec.
+    void setWeights(const void* wx, const void* wy, const void* wz) {
+        const void* const w[3] = {wx, wy, wz};
+        DFFT_CALL(dfft_plan_set_weights(plan, w));
+    }
     // not in the reference: transform (true) or keep (false) the x, y, z axis (dfft_plan_set_transform_axes; after
     // initFFT, before the first exec).  setTransformAxes(false, true, true) leaves x untransformed and whole on every rank.
     void setTransformAxes(bool x, bool y, bool z) {
