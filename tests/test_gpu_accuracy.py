@@ -14,7 +14,8 @@ Families:
      Bluestein y axis), R2C / C2R with Nz = 4..8192; C on both sides of every tile width, d = 1, 2, 3, both directions,
      f32 and f64, a scale != 1 per length;
   2. padded plans, per field (batch 3): every N = 2..8192 on z (R2C up to 16384), and on x with narrow and wide tiles,
-     K in {1, 2, ceil(N/2), N/2 + 1, N - 1};
+     K in {1, 2, ceil(N/2), N/2 + 1, N - 1}; the x pass's column count B is above the narrow tile width of the length
+     (asserted from dfft_plan_describe) and leaves a part-full tile;
   3. the single-axis entry points, per line: dfft_fft1d_contig (C2C, R2C, C2R) and dfft_fft1d_general (default, TMA-fed,
      narrow and wide tiles) at every length, Bluestein lengths 2^k +- 1, 3 and 5, with line and column counts that leave
      partial CTAs and tiles;
@@ -37,6 +38,7 @@ rms(unit), f64 then f32:
 The bounds (3 and 30) hold every family.  With the paired split the interleaved R2C / C2R pass used before, that family
 missed the rel-L2 bound by a factor of 2.7e4 to 1.4e5 in both precisions.  The module takes about 85 s on the H100; the
 long-double references of the interleaved family, the largest, take about 26 s of CPU time."""
+import json
 import math
 
 import numpy as np
@@ -47,6 +49,7 @@ import distributedfft_b200 as dfft
 from test_gpu_schedule_replay import UNIT, error_check, run_lengths, same_bits
 from test_gpu_transform_axes import canary_ok, canary_out
 from test_padded import fwd_ref as padded_fwd, inv_ref as padded_inv
+from step_replay import describe_raw
 from test_r2r_mixed import r2r_1d
 from test_transform_axes import fwd_ref, inv_ref
 
@@ -130,21 +133,22 @@ def on_device(fn, x, out_shape, out_dtype):
     return got
 
 
-def note(family, prec, rel, mx):
+def note(family, prec, rel, mx, worst=WORST):
     key = (family, "f64" if prec == F64 else "f32")
-    w = WORST.get(key, (0.0, 0.0))
-    WORST[key] = (max(w[0], rel), max(w[1], mx))
+    w = worst.get(key, (0.0, 0.0))
+    worst[key] = (max(w[0], rel), max(w[1], mx))
 
 
-def check_units(family, s, got, ref, axis, scales, what=""):
-    """the per-unit bounds, unit i being index i along `axis`; scales[i] == 0: the unit must be exact zeros"""
+def check_units(family, s, got, ref, axis, scales, what="", worst=WORST):
+    """the per-unit bounds, unit i being index i along `axis`; scales[i] == 0: the unit must be exact zeros.  The worst
+    errors go to `worst` (the calling module's report)"""
     g, r = np.moveaxis(got, axis, 0), np.moveaxis(np.asarray(ref), axis, 0)
     for i in range(r.shape[0]):
         if scales[i] == 0:
             assert not np.any(g[i]), f"{family} {what}: unit {i} has a zero input but a nonzero output"
             continue
         rel, mx = error_check(s, g[i], r[i])
-        note(family, s["prec"], rel, mx)
+        note(family, s["prec"], rel, mx, worst)
         assert rel <= REL_BOUND and mx <= MAX_BOUND, \
             f"{family} {what}: unit {i} of {r.shape[0]} (input scale {scales[i]:g}): rel-L2 {rel:.2f}, max {mx:.2f} u sqrt(sum log2 L)"
 
@@ -255,12 +259,24 @@ def spectral_sizes(n):
     return sorted(k for k in {1, 2, (n + 1) // 2, n // 2 + 1, n - 1} if 1 <= k <= n)
 
 
+def x_extent(transform, n):
+    """(ny, nz) of the x cases: the x pass's column count B = ny nz (C2C) or ny (nz/2 + 1) (R2C) is above the narrow tile
+    width TBT of both precisions and leaves the last tile part-full (C2C: a Bluestein y axis of 3, R2C: B = TBT + 2)"""
+    tbt = max(shape_of(prec, n.bit_length() - 1)[1] for prec in PRECS)
+    if transform == "r2c":
+        return 2, max(tbt, 4)
+    return 3, max(tbt // 2, 2)
+
+
+def x_columns(transform, shape):
+    return shape[1] * (shape[2] // 2 + 1 if transform == "r2c" else shape[2])
+
+
 def padded_case(transform, axis, n):
     """batch 3 on a grid whose `axis` is n points long, for every K of spectral_sizes(n) on that axis"""
     r2c = transform == "r2c"
     t = R2C if r2c else C2C
-    shape = [4, 2, n] if axis == 2 else [n, 2, 8]
-    shape = tuple(shape)
+    shape = (4, 2, n) if axis == 2 else (n,) + x_extent(transform, n)
     family = f"padded {'xyz'[axis]} " + ("R2C/C2R" if r2c else "C2C")
     for ki, kk in enumerate(spectral_sizes(n)):
         sp = list(shape)
@@ -269,6 +285,10 @@ def padded_case(transform, axis, n):
             prec = PRECS[(ki + inverse) % 2]
             plan = plan_of(prec, transform, shape, batch=3, spectral=sp)
             try:
+                if axis == 0:  # the x pass runs the intended columns, more than a narrow tile holds
+                    _, tbt, wtile = shape_of(prec, n.bit_length() - 1)
+                    xs = [st for st in json.loads(describe_raw(plan._h, inverse, 3))["steps"] if st["type"] == 0 and st["label"] == "x pass"]
+                    assert xs and all(st["B"] == x_columns(transform, shape) > tbt for st in xs), (shape, [st["B"] for st in xs], tbt)
                 seed = n * 100 + ki * 2 + inverse
                 if not inverse:
                     x, sc = mixed((3,) + shape, 0, prec, not r2c, seed, off=ki)

@@ -113,7 +113,7 @@ class Case:
                 n = self.shape[axis]
                 full = list(Y.shape)
                 full[axis] = n // 2 + 1 if half else n
-                E = np.zeros(full, dtype=np.complex128)
+                E = np.zeros(full, dtype=np.result_type(Y.dtype, np.complex128))  # long double stays long double
                 idx = [slice(None)] * 3
                 idx[axis] = np.arange(self.spec[2] // 2 + 1) if half else np.fft.fftfreq(self.spec[axis], 1.0 / self.spec[axis]).astype(np.int64) % n
                 E[tuple(idx)] = Y

@@ -67,7 +67,7 @@ def inv_ref(X, transform, shape, data, spec, d):
         n = shape[axis]
         full = list(X.shape)
         full[axis] = n // 2 + 1 if half else n
-        E = np.zeros(full, dtype=np.complex128)
+        E = np.zeros(full, dtype=np.result_type(X.dtype, np.complex128))  # long double stays long double
         idx = [slice(None)] * 3
         idx[axis] = positions(n, spec[axis], half)
         E[tuple(idx)] = X
