@@ -143,12 +143,12 @@ static bool r2r_kind_length(int kind, size_t n) {
 // hole[1]) on the spectral side, [hole[2], hole[3]) on the physical one; the padded twin of the power-of-two kernel runs
 // then, with the physical hole on its loaded side forward and on its stored side inverse.
 // w: the spectral weights of the pass's axis (dfft_plan_set_weights), or null.  Weighted passes run the weighted twins:
-// of the padded kernels (with hole, empty where the plan keeps a whole side) or of the Bluestein kernel.
+// of the padded kernels (with hole, empty where the plan keeps a whole side) or of the Bluestein kernel (WEIGHTED = true).
 static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftParams& prm, const void* blu, double scale, cudaStream_t stream,
                                    int r2r = DFFT_DCT, const int* hole = nullptr, const void* w = nullptr) {
     const int log2n = ilog2_exact(n);
     if (hole && log2n >= 0) {
-        FftWeighted q;
+        FftPadded q;
         static_cast<FftParams&>(q) = prm;
         q.scale = scale;
         const int* ld = prm.inverse ? hole : hole + 2;
@@ -156,7 +156,7 @@ static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftP
         q.ld_lo = ld[0]; q.ld_hi = ld[1];
         q.st_lo = st[0]; q.st_hi = st[1];
         q.w = w;
-        return w ? launch_weighted(prec, log2n, kind, q, stream) : launch_padded(prec, log2n, kind, q, stream);
+        return launch_twin(prec, log2n, kind, q, stream);
     }
     if (kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED) {
         FftR2r r;
@@ -176,12 +176,7 @@ static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftP
     b.kspec = blu;
     b.chirp = blu ? static_cast<const char*>(blu) + (size_t(1) << log2m) * (prec == DFFT_F64 ? 16 : 8) : nullptr;
     b.scale = scale;
-    if (w) {
-        FftBluesteinW bw;
-        static_cast<FftBluestein&>(bw) = b;
-        bw.w = w;
-        return launch_bluestein(prec, log2m, kind, bw, stream);
-    }
+    b.w = w;
     return launch_bluestein(prec, log2m, kind, b, stream);
 }
 
@@ -674,17 +669,28 @@ static bool pow2_axes(const dfft_plan_s* p) { return ilog2_exact(p->g.nx) > 0 &&
 // Whether every axis is transformed.  Plans with a kept axis (dfft_plan_set_transform_axes) run the sequential schedule
 // only: the overlapped schedules, the fused z + y stage and the batched stage transform every axis they touch.
 static bool all_axes(const dfft_plan_s* p) { return p->taxes[0] && p->taxes[1] && p->taxes[2]; }
-// Whether the schedules may take another form than the sequential one: the overlapped schedules, the fused z + y stage and
-// the batched stage build their passes for power-of-two lengths, every axis transformed and no padding or pruning (their
-// kernels have no padded twins, FftPadded).
-// Interleaved plans (C > 1 values per point) run it too: those kernels address one value per point.  So do plans with a
-// box that is not the natural layout: their reshape steps wrap the sequential schedule (wrap_boxes).  And embedded plans
-// (dfft_plan_set_strides): the other forms read and write dense caller arrays, and every rank must run the same form.
-// Weighted plans (dfft_plan_set_weights) too: only the single-axis passes have weighted twins.
-static bool alt_schedules(const dfft_plan_s* p) {
-    return pow2_axes(p) && !is_half(p->prec) && !is_r2r(p->g.transform) && all_axes(p) && !p->g.padded() && !p->g.pruned() && p->comps == 1 && !p->boxed() &&
-           !p->embedded() && !p->weighted;
+// Why a plan's features keep it on the sequential schedule, or null: the overlapped schedules, the fused z + y stage and the
+// batched stage run none of them.  Their kernels have no 16-bit, weighted or padded twins (FftPadded), and run C2C and
+// R2C / C2R passes over every axis.  Interleaved plans (C > 1 values per point): those kernels address one value per
+// point.  Plans with a box that is not the natural layout: their reshape steps wrap the sequential schedule (wrap_boxes).
+// Embedded plans (dfft_plan_set_strides): the other forms read and write dense caller arrays, and every rank must run the
+// same form.  The text completes dfft_plan_tune's report.
+static const char* sequential_only(const dfft_plan_s* p) {
+    if (is_half(p->prec)) return "16-bit plans";
+    if (p->weighted) return "weighted plans";
+    if (is_r2r(p->g.transform)) return "DCT / DST plans";
+    if (!all_axes(p)) return "plans with a kept axis";
+    if (p->g.padded()) return "padded plans";
+    if (p->g.pruned()) return "pruned plans";
+    if (p->comps > 1) return "interleaved plans";
+    if (p->boxed()) return "box plans";
+    if (p->embedded()) return "plans with strides";
+    return nullptr;
 }
+
+// Whether the schedules may take another form than the sequential one: the overlapped schedules build their passes for
+// power-of-two lengths.
+static bool alt_schedules(const dfft_plan_s* p) { return pow2_axes(p) && !sequential_only(p); }
 
 // Row pitch, in elements (complex units; reals for DCT / DST plans), of the z-contiguous side of the caller's buffers that
 // holds Nz points per row: the input of forward passes, the output of inverse ones.  Real rows of R2C / C2R plans are Nz reals (Nz/2 units) apart, or, in
@@ -700,9 +706,7 @@ static long long z_row_pitch(const dfft_plan_s* p) {
 // three passes are L2-resident already and gain nothing.
 static bool zy_fused(const dfft_plan_s* p, int inverse, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || is_half(p->prec) || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || g.pruned() || p->comps > 1 ||
-        p->boxed() || p->embedded() || p->weighted)
-        return false;
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || sequential_only(p)) return false;
     if (g.ny != g.nz || !zy_fused_length(ilog2_exact(g.ny))) return false;
     // the fused stage reads and writes the blocked hand-over layout of the x pass
     if (p->blocked_ch <= 0 || g.nz % size_t(p->blocked_ch) || (inverse && !p->blocked_inv)) return false;
@@ -756,9 +760,7 @@ static int fuse_zy(dfft_plan_s* p, Step zs, const Step& ys, const char* label, c
 constexpr size_t BATCH_SMALL_MIN = 2;
 static bool batch_small(const dfft_plan_s* p, int d) {
     const Geometry& g = p->g;
-    if (p->P != 1 || is_half(p->prec) || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || !all_axes(p) || g.padded() || g.pruned() || p->comps > 1 ||
-        p->boxed() || p->embedded() || p->weighted)
-        return false;
+    if (p->P != 1 || g.decomp != DFFT_SLAB_ZY_THEN_X || g.transform != DFFT_C2C || d != 3 || sequential_only(p)) return false;
     if (g.nx != g.ny || g.ny != g.nz || !batch_small_length(ilog2_exact(g.nx))) return false;
     return p->batch >= BATCH_SMALL_MIN && p->batch * g.nx <= 0x7fffffff;
 }
@@ -3567,17 +3569,10 @@ int dfft_plan_tune(dfft_plan_t p, void* out, const void* in, int inverse, int re
     }
     p->tune_report.clear();
     if (cands.size() == 1) {
-        p->tune_report = is_half(p->prec)       ? "sequential schedule (no alternatives for this plan: 16-bit plans run the sequential schedule)"
-                         : p->weighted          ? "sequential schedule (no alternatives for this plan: weighted plans run the sequential schedule)"
-                         : is_r2r(p->g.transform) ? "sequential schedule (no alternatives for this plan: DCT / DST plans run the sequential schedule)"
-                         : !all_axes(p)         ? "sequential schedule (no alternatives for this plan: plans with a kept axis run the sequential schedule)"
-                         : p->g.padded()        ? "sequential schedule (no alternatives for this plan: padded plans run the sequential schedule)"
-                         : p->g.pruned()        ? "sequential schedule (no alternatives for this plan: pruned plans run the sequential schedule)"
-                         : p->comps > 1         ? "sequential schedule (no alternatives for this plan: interleaved plans run the sequential schedule)"
-                         : p->boxed()           ? "sequential schedule (no alternatives for this plan: box plans run the sequential schedule)"
-                         : p->embedded()        ? "sequential schedule (no alternatives for this plan: plans with strides run the sequential schedule)"
-                         : pow2_axes(p)         ? "sequential schedule (no alternatives for this plan)"
-                                                : "sequential schedule (no alternatives for this plan: an axis length is not a power of two)";
+        const char* why = sequential_only(p);
+        p->tune_report = why           ? std::string("sequential schedule (no alternatives for this plan: ") + why + " run the sequential schedule)"
+                         : pow2_axes(p) ? "sequential schedule (no alternatives for this plan)"
+                                        : "sequential schedule (no alternatives for this plan: an axis length is not a power of two)";
         return 0;
     }
     const bool was_timing = p->timing;

@@ -33,25 +33,17 @@ static cudaError_t dispatch(int prec, int log2n, const F& launch) {
 cudaError_t launch_pass(int prec, int log2n, PassKind kind, const FftParams& p, double scale, cudaStream_t stream) {
     return dispatch<1, MAX_LOG2N, true>(prec, log2n, [&](auto t, auto l) {
         using T = decltype(t);
-        if constexpr (std::is_same_v<T, __half> || std::is_same_v<T, __nv_bfloat16>) return launch_pass16<T, decltype(l)::value>(kind, p, scale, stream);
-        else return launch_pass<T, decltype(l)::value>(kind, p, scale, stream);
+        if constexpr (std::is_same_v<T, __half> || std::is_same_v<T, __nv_bfloat16>) return launch_pass<float, cx16<T>, decltype(l)::value>(kind, p, scale, stream);
+        else return launch_pass<T, cx<T>, decltype(l)::value>(kind, p, scale, stream);
     });
 }
 
-cudaError_t launch_padded(int prec, int log2n, PassKind kind, const FftPadded& p, cudaStream_t stream) {
-    return dispatch<1, MAX_LOG2N>(prec, log2n, [&](auto t, auto l) { return launch_padded<decltype(t), decltype(l)::value>(kind, p, stream); });
+cudaError_t launch_twin(int prec, int log2n, PassKind kind, const FftPadded& p, cudaStream_t stream) {
+    return dispatch<1, MAX_LOG2N>(prec, log2n, [&](auto t, auto l) { return launch_twin<decltype(t), decltype(l)::value>(kind, p, stream); });
 }
 
 cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluestein& p, cudaStream_t stream) {
     return dispatch<3, MAX_LOG2N>(prec, log2m, [&](auto t, auto l) { return launch_bluestein<decltype(t), decltype(l)::value>(kind, p, stream); });
-}
-
-cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluesteinW& p, cudaStream_t stream) {
-    return dispatch<3, MAX_LOG2N>(prec, log2m, [&](auto t, auto l) { return launch_bluestein<decltype(t), decltype(l)::value>(kind, p, stream); });
-}
-
-cudaError_t launch_weighted(int prec, int log2n, PassKind kind, const FftWeighted& p, cudaStream_t stream) {
-    return dispatch<1, MAX_LOG2N>(prec, log2n, [&](auto t, auto l) { return launch_weighted<decltype(t), decltype(l)::value>(kind, p, stream); });
 }
 
 cudaError_t launch_r2r(int prec, int log2n, PassKind kind, const FftR2r& p, bool hc, cudaStream_t stream) {

@@ -1,6 +1,6 @@
 // fft_inst.cu — compiled once per (precision, log2 length): -DDFFT_T=double -DDFFT_LOG2N=10, and once per (16-bit format,
 // log2 length) of 16-bit plans: -DDFFT_T=float -DDFFT_S=__half (or __nv_bfloat16) -DDFFT_LOG2N=10, which compiles
-// launch_pass16 only.  Splitting the instantiations over translation units lets build.py compile them in parallel.
+// launch_pass<float, cx16<DFFT_S>, 10> only.  Splitting the instantiations over translation units lets build.py compile them in parallel.
 #include <cstdlib>
 
 #include "fft_kernels.cuh"
@@ -109,24 +109,34 @@ static int tile_swz_for(int swz, int A0, int A1) {
     return swz > 0 && swz <= 4 && A0 % (1 << swz) == 0 && A1 % (1 << swz) == 0 ? swz : 0;
 }
 
-static int wide_tiles() {
-    const char* e = getenv("DFFT_WIDE_TILES");
-    return e ? atoi(e) : 0;
+// Wide tiles (S::TBT_WIDE: 128-byte rows, one CTA per SM) or narrow ones (S::TBT) for a TILED pass of 2^LOG2N-point lines.
+// Wide when the rows of a tile sit in different 2 MB pages (x passes: a row pitch of es-byte stored elements >= 1 MiB),
+// narrow otherwise (y passes); a choice still to be confirmed on the H100 (tools/axis_bench.py).  tma: the pass can run the
+// TMA-fed kernel (launch_tiled), which takes the wide tile for near rows as well unless DFFT_TMA=0.  DFFT_WIDE_TILES=1 / -1
+// and p.tile_pref force either.  Never a wide tile for a view that is only one narrow tile wide (blocked hand-over with
+// CH = TBT): half of its columns would be empty.
+template <typename T, int LOG2N>
+static bool wide_tile(const FftParams& p, size_t es, bool tma) {
+    using S = Shape<T, LOG2N>;
+    const int w = env_int("DFFT_WIDE_TILES", 0);
+    const bool far_rows = (unsigned long long)p.in.sN * es >= (1ull << 20) || (unsigned long long)p.out.sN * es >= (1ull << 20);
+    const bool tma_auto = tma && env_int("DFFT_TMA", -1) != 0 && p.in.nseg == 1;
+    const bool wide = w > 0 || p.tile_pref == 2 || (w == 0 && p.tile_pref == 0 && LOG2N >= 10 && (far_rows || tma_auto));
+    return wide && w >= 0 && p.tile_pref != 1 && p.B > S::TBT;
 }
 
-#ifndef DFFT_S
-template <typename T, int LOG2N, int TB>
+// S: the stored element; the TMA-fed kernel serves cx<T> passes only
+template <typename T, typename S, int LOG2N, int TB>
 static cudaError_t launch_tiled(const FftParams& p_in, double scale, cudaStream_t stream, long long lines) {
     FftParams p = p_in;
     const int swz = env_int("DFFT_TILE_SWZ", -1);  // experiment override of the tile-order blocking
     p.tile_swz = tile_swz_for(swz >= 0 ? swz : p.tile_swz, p.A0, p.A1);
-    using S = Shape<T, LOG2N>;
-    constexpr int LOG2E = S::LOG2E;
+    constexpr int LOG2E = Shape<T, LOG2N>::LOG2E;
     using C = CtaFft<T, LOG2N, LOG2E, TB, true>;
     if (p.B <= 0) return cudaSuccess;
     const long long grid = lines * ((p.B + TB - 1) / TB);
     if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-    if constexpr (C::NST >= 2 && LOG2N >= 7) {
+    if constexpr (std::is_same_v<S, cx<T>> && C::NST >= 2 && LOG2N >= 7) {
         // TMA-fed persistent kernel (fft_c2c_tma_kernel).  Design rationale, not yet measured on the H100
         // (tools/axis_bench.py times both kernels per pass): the TMA engine relieves the register-fed kernel where its
         // strided 64/128-byte row loads load the L1TEX pipe most, f64 lines of >= 1024 points.  Lines of <= 512 points
@@ -150,116 +160,97 @@ static cudaError_t launch_tiled(const FftParams& p_in, double scale, cudaStream_
         }
     }
     const unsigned g = unsigned((p.max_ctas > 0 && grid > p.max_ctas) ? p.max_ctas : grid);
-    return launch_kernel<fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, false, false>, fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, true, false>,
-                         fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, false, true>, fft_c2c_kernel<T, LOG2N, LOG2E, TB, true, true, true>>(
+    return launch_kernel<fft_c2c_kernel<T, S, LOG2N, LOG2E, TB, true, false, false>, fft_c2c_kernel<T, S, LOG2N, LOG2E, TB, true, true, false>,
+                         fft_c2c_kernel<T, S, LOG2N, LOG2E, TB, true, false, true>, fft_c2c_kernel<T, S, LOG2N, LOG2E, TB, true, true, true>>(
         p, scale, g, C::THREADS, C::SMEM_BYTES, stream);
 }
 
-template <typename T, int LOG2N>
+// S = cx16<H> (16-bit plans): the shapes of the f32 pass, TILED tiles included.  Their TILED rows are the f32 tile's 8
+// elements wide from 512-point lines on, 32 bytes of 16-bit pairs: at 512^3 on an H100 the y and x passes took 0.43-0.50 ms
+// with them against 0.69-0.72 ms with 64-byte rows (16 elements, twice the threads and shared memory per CTA), DESIGN.md
+// section 3.20.  16-bit plans have no interleaved passes.
+template <typename T, typename S, int LOG2N>
 cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStream_t stream) {
-    using S = Shape<T, LOG2N>;
-    constexpr int LOG2E = S::LOG2E;
-    using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
+    using SH = Shape<T, LOG2N>;
+    constexpr int LOG2E = SH::LOG2E;
+    constexpr bool PLAIN = std::is_same_v<S, cx<T>>;
+    using C = CtaFft<T, LOG2N, LOG2E, SH::TBC, false>;
     const long long lines = (long long)p.A0 * p.A1;
     if (lines <= 0) return cudaSuccess;
-    const long long grid = (lines + S::TBC - 1) / S::TBC;  // CONTIG, R2C and C2R
+    const long long grid = (lines + SH::TBC - 1) / SH::TBC;  // CONTIG, R2C and C2R
     switch (kind) {
         case PASS_C2C_CONTIG:
             if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
             if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            return launch_kernel<fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, false, false>, fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, true, false>,
-                                 fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, false, true>, fft_c2c_kernel<T, LOG2N, LOG2E, S::TBC, false, true, true>>(
+            return launch_kernel<fft_c2c_kernel<T, S, LOG2N, LOG2E, SH::TBC, false, false, false>, fft_c2c_kernel<T, S, LOG2N, LOG2E, SH::TBC, false, true, false>,
+                                 fft_c2c_kernel<T, S, LOG2N, LOG2E, SH::TBC, false, false, true>, fft_c2c_kernel<T, S, LOG2N, LOG2E, SH::TBC, false, true, true>>(
                 p, scale, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
-        case PASS_C2C_TILED: {
-            // Wide tiles (128-byte rows, one CTA per SM) are chosen when the rows of a tile sit in different 2 MB pages
-            // (x passes with a row pitch >= 1 MiB), narrow ones otherwise (y passes); a choice still to be confirmed on
-            // the H100 (tools/axis_bench.py).  DFFT_WIDE_TILES=1 / -1 forces them
-            // on / off.
-            if constexpr (S::TBT_WIDE != S::TBT) {
-                const int w = wide_tiles();
-                const bool far_rows = (unsigned long long)p.in.sN * sizeof(cx<T>) >= (1ull << 20) ||
-                                      (unsigned long long)p.out.sN * sizeof(cx<T>) >= (1ull << 20);
-                // with the TMA-fed kernel (f64, >= 1024 points) the wide tile is chosen for near rows as well
-                const bool tma_auto = env_int("DFFT_TMA", -1) != 0 && sizeof(T) == 8 && LOG2N >= 10 && p.in.nseg == 1;
-                const bool wide = w > 0 || p.tile_pref == 2 || (w == 0 && p.tile_pref == 0 && LOG2N >= 10 && (far_rows || tma_auto));
-                // never a wide tile for a view that is only one narrow tile wide (blocked hand-over with CH = TBT): half of
-                // its columns would be empty
-                if (wide && w >= 0 && p.tile_pref != 1 && p.B > S::TBT) return launch_tiled<T, LOG2N, S::TBT_WIDE>(p, scale, stream, lines);
-            }
-            return launch_tiled<T, LOG2N, S::TBT>(p, scale, stream, lines);
-        }
+        case PASS_C2C_TILED:
+            if (wide_tile<T, LOG2N>(p, sizeof(S), PLAIN && sizeof(T) == 8 && LOG2N >= 10)) return launch_tiled<T, S, LOG2N, SH::TBT_WIDE>(p, scale, stream, lines);
+            return launch_tiled<T, S, LOG2N, SH::TBT>(p, scale, stream, lines);
         case PASS_C2C_ILV: {
-            // C = B components per point, lines C apart along n.  From the tile width on, the TILED kernel's tiles are full
-            // rows of components; below it the interleaved kernel keeps every thread busy.
-            if (p.B < 1 || p.in.sN != p.B || p.out.sN != p.B) return cudaErrorInvalidValue;
-            if (p.B >= S::TBT) return launch_tiled<T, LOG2N, S::TBT>(p, scale, stream, lines);
-            const long long g = (lines * p.B + S::TBC - 1) / S::TBC;
-            if (g > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            const unsigned grid_ilv = unsigned((p.max_ctas > 0 && g > p.max_ctas) ? p.max_ctas : g);
-            return launch_kernel<fft_c2c_ilv_kernel<T, LOG2N, LOG2E, S::TBC, false, false>, fft_c2c_ilv_kernel<T, LOG2N, LOG2E, S::TBC, true, false>,
-                                 fft_c2c_ilv_kernel<T, LOG2N, LOG2E, S::TBC, false, true>, fft_c2c_ilv_kernel<T, LOG2N, LOG2E, S::TBC, true, true>>(
-                p, scale, grid_ilv, C::THREADS, C::SMEM_BYTES, stream);
+            if constexpr (!PLAIN) return cudaErrorInvalidValue;
+            else {
+                // C = B components per point, lines C apart along n.  From the tile width on, the TILED kernel's tiles are
+                // full rows of components; below it the interleaved kernel keeps every thread busy.
+                if (p.B < 1 || p.in.sN != p.B || p.out.sN != p.B) return cudaErrorInvalidValue;
+                if (p.B >= SH::TBT) return launch_tiled<T, S, LOG2N, SH::TBT>(p, scale, stream, lines);
+                const long long g = (lines * p.B + SH::TBC - 1) / SH::TBC;
+                if (g > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+                const unsigned grid_ilv = unsigned((p.max_ctas > 0 && g > p.max_ctas) ? p.max_ctas : g);
+                return launch_kernel<fft_c2c_ilv_kernel<T, LOG2N, LOG2E, SH::TBC, false, false>, fft_c2c_ilv_kernel<T, LOG2N, LOG2E, SH::TBC, true, false>,
+                                     fft_c2c_ilv_kernel<T, LOG2N, LOG2E, SH::TBC, false, true>, fft_c2c_ilv_kernel<T, LOG2N, LOG2E, SH::TBC, true, true>>(
+                    p, scale, grid_ilv, C::THREADS, C::SMEM_BYTES, stream);
+            }
         }
         case PASS_R2C_ILV:
         case PASS_C2R_ILV: {
-            // C = B components, one line per component; the real side is one segment
-            const bool c2r = kind == PASS_C2R_ILV;
-            if (p.B < 1 || (c2r ? p.out.nseg : p.in.nseg) != 1) return cudaErrorInvalidValue;
-            const long long g = (lines * p.B + S::TBC - 1) / S::TBC;
-            if (g > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            const unsigned grid_rc = unsigned((p.max_ctas > 0 && g > p.max_ctas) ? p.max_ctas : g);
-            if (c2r) {
-                constexpr auto k = fft_rc_ilv_kernel<T, LOG2N, LOG2E, S::TBC, true, false>;
-                constexpr auto ks = fft_rc_ilv_kernel<T, LOG2N, LOG2E, S::TBC, true, true>;
+            if constexpr (!PLAIN) return cudaErrorInvalidValue;
+            else {
+                // C = B components, one line per component; the real side is one segment
+                const bool c2r = kind == PASS_C2R_ILV;
+                if (p.B < 1 || (c2r ? p.out.nseg : p.in.nseg) != 1) return cudaErrorInvalidValue;
+                const long long g = (lines * p.B + SH::TBC - 1) / SH::TBC;
+                if (g > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+                const unsigned grid_rc = unsigned((p.max_ctas > 0 && g > p.max_ctas) ? p.max_ctas : g);
+                if (c2r) {
+                    constexpr auto k = fft_rc_ilv_kernel<T, LOG2N, LOG2E, SH::TBC, true, false>;
+                    constexpr auto ks = fft_rc_ilv_kernel<T, LOG2N, LOG2E, SH::TBC, true, true>;
+                    return launch_kernel<k, k, ks, ks>(p, scale, grid_rc, C::THREADS, C::SMEM_BYTES, stream);
+                }
+                constexpr auto k = fft_rc_ilv_kernel<T, LOG2N, LOG2E, SH::TBC, false, false>;
+                constexpr auto ks = fft_rc_ilv_kernel<T, LOG2N, LOG2E, SH::TBC, false, true>;
                 return launch_kernel<k, k, ks, ks>(p, scale, grid_rc, C::THREADS, C::SMEM_BYTES, stream);
             }
-            constexpr auto k = fft_rc_ilv_kernel<T, LOG2N, LOG2E, S::TBC, false, false>;
-            constexpr auto ks = fft_rc_ilv_kernel<T, LOG2N, LOG2E, S::TBC, false, true>;
-            return launch_kernel<k, k, ks, ks>(p, scale, grid_rc, C::THREADS, C::SMEM_BYTES, stream);
         }
         case PASS_R2C: {
             if (p.in.nseg != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
             if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            constexpr auto k = fft_r2c_kernel<T, LOG2N, LOG2E, S::TBC, false>;
-            constexpr auto ks = fft_r2c_kernel<T, LOG2N, LOG2E, S::TBC, true>;
+            constexpr auto k = fft_r2c_kernel<T, S, LOG2N, LOG2E, SH::TBC, false>;
+            constexpr auto ks = fft_r2c_kernel<T, S, LOG2N, LOG2E, SH::TBC, true>;
             return launch_kernel<k, k, ks, ks>(p, scale, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
         }
         case PASS_C2R: {
             if (p.out.nseg != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
             if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            constexpr auto k = fft_c2r_kernel<T, LOG2N, LOG2E, S::TBC, false>;
-            constexpr auto ks = fft_c2r_kernel<T, LOG2N, LOG2E, S::TBC, true>;
+            constexpr auto k = fft_c2r_kernel<T, S, LOG2N, LOG2E, SH::TBC, false>;
+            constexpr auto ks = fft_c2r_kernel<T, S, LOG2N, LOG2E, SH::TBC, true>;
             return launch_kernel<k, k, ks, ks>(p, scale, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
         }
         default: return cudaErrorInvalidValue;
     }
 }
 
-template cudaError_t launch_pass<DFFT_T, DFFT_LOG2N>(PassKind, const FftParams&, double, cudaStream_t);
+#ifdef DFFT_S
+template cudaError_t launch_pass<float, cx16<DFFT_S>, DFFT_LOG2N>(PassKind, const FftParams&, double, cudaStream_t);
+#else
+template cudaError_t launch_pass<DFFT_T, cx<DFFT_T>, DFFT_LOG2N>(PassKind, const FftParams&, double, cudaStream_t);
 
-// P: FftPadded (the padded twins) or FftWeighted (the weighted twins)
-template <typename T, int LOG2N, int TB, typename P>
-static cudaError_t launch_padded_tiled(const P& p, long long lines, cudaStream_t stream) {
-    constexpr int LOG2E = Shape<T, LOG2N>::LOG2E;
-    using C = CtaFft<T, LOG2N, LOG2E, TB, true>;
-    P q = p;
-    q.tile_swz = tile_swz_for(p.tile_swz, p.A0, p.A1);
-    const long long g = lines * ((p.B + TB - 1) / TB);
-    if (g > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-    if constexpr (std::is_same_v<P, FftWeighted>)
-        return launch_kernel<fft_c2c_weighted_kernel<T, LOG2N, LOG2E, TB, true, false>, fft_c2c_weighted_kernel<T, LOG2N, LOG2E, TB, true, true>, nullptr,
-                             nullptr>(q, 1.0, unsigned(g), C::THREADS, C::SMEM_BYTES, stream);
-    else
-        return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, LOG2E, TB, true, false>, fft_c2c_padded_kernel<T, LOG2N, LOG2E, TB, true, true>, nullptr,
-                             nullptr>(q, 1.0, unsigned(g), C::THREADS, C::SMEM_BYTES, stream);
-}
-
-// the padded twins (fft_c2c_padded_kernel, fft_r2c_padded_kernel, fft_c2r_padded_kernel), or with P = FftWeighted the
-// weighted twins (fft_c2c_weighted_kernel, ...): the tiles of launch_pass (TILED: narrow or wide by its rule), one CTA per
-// tile, the register-fed kernel only
-template <typename T, int LOG2N, typename P>
-static cudaError_t launch_twin(PassKind kind, const P& p, cudaStream_t stream) {
-    constexpr bool W = std::is_same_v<P, FftWeighted>;
+// the padded twins (fft_c2c_padded_kernel, fft_r2c_padded_kernel, fft_c2r_padded_kernel), their weighted instantiations
+// (WEIGHTED = true) where p.w is set: the tiles of launch_pass (TILED: narrow or wide by wide_tile, without the TMA-fed
+// kernel), one CTA per tile
+template <typename T, int LOG2N>
+cudaError_t launch_twin(PassKind kind, const FftPadded& p, cudaStream_t stream) {
     using S = Shape<T, LOG2N>;
     constexpr int LOG2E = S::LOG2E;
     const long long lines = (long long)p.A0 * p.A1;
@@ -271,92 +262,72 @@ static cudaError_t launch_twin(PassKind kind, const P& p, cudaStream_t stream) {
     // the R2C / C2R twins test k < lo only: their holes reach the end of the line
     if (half && (p.ld_hi != n_ld || p.st_hi != n_st)) return cudaErrorInvalidValue;
     const long long grid = (lines + S::TBC - 1) / S::TBC;  // CONTIG, R2C and C2R
-    switch (kind) {
-        case PASS_C2C_CONTIG: {
-            using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
-            if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
-            if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            if constexpr (W)
-                return launch_kernel<fft_c2c_weighted_kernel<T, LOG2N, LOG2E, S::TBC, false, false>,
-                                     fft_c2c_weighted_kernel<T, LOG2N, LOG2E, S::TBC, false, true>, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS,
-                                                                                                                      C::SMEM_BYTES, stream);
-            else
-                return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, false, false>, fft_c2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, false, true>,
+    const auto launch = [&](auto weighted) -> cudaError_t {
+        constexpr bool W = decltype(weighted)::value;
+        using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
+        // TILED, tiles TB columns wide
+        const auto tiled = [&](auto tb) -> cudaError_t {
+            constexpr int TB = decltype(tb)::value;
+            using CT = CtaFft<T, LOG2N, LOG2E, TB, true>;
+            FftPadded q = p;
+            q.tile_swz = tile_swz_for(p.tile_swz, p.A0, p.A1);
+            const long long g = lines * ((p.B + TB - 1) / TB);
+            if (g > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+            return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, LOG2E, TB, true, false, W>, fft_c2c_padded_kernel<T, LOG2N, LOG2E, TB, true, true, W>, nullptr,
+                                 nullptr>(q, 1.0, unsigned(g), CT::THREADS, CT::SMEM_BYTES, stream);
+        };
+        switch (kind) {
+            case PASS_C2C_CONTIG:
+                if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
+                if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+                return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, false, false, W>, fft_c2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, false, true, W>,
                                      nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
-        }
-        case PASS_C2C_TILED: {
-            if (p.B <= 0) return cudaSuccess;
-            if constexpr (S::TBT_WIDE != S::TBT) {
-                // the wide-tile rule of launch_pass, without the TMA-fed kernel
-                const int w = wide_tiles();
-                const bool far_rows = (unsigned long long)p.in.sN * sizeof(cx<T>) >= (1ull << 20) ||
-                                      (unsigned long long)p.out.sN * sizeof(cx<T>) >= (1ull << 20);
-                const bool wide = w > 0 || p.tile_pref == 2 || (w == 0 && p.tile_pref == 0 && LOG2N >= 10 && far_rows);
-                if (wide && w >= 0 && p.tile_pref != 1 && p.B > S::TBT) return launch_padded_tiled<T, LOG2N, S::TBT_WIDE>(p, lines, stream);
-            }
-            return launch_padded_tiled<T, LOG2N, S::TBT>(p, lines, stream);
-        }
-        case PASS_R2C:
-        case PASS_C2R: {
-            using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
-            if ((kind == PASS_R2C ? p.in.nseg : p.out.nseg) != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
-            if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            if constexpr (W) {
+            case PASS_C2C_TILED:
+                if (p.B <= 0) return cudaSuccess;
+                if (wide_tile<T, LOG2N>(p, sizeof(cx<T>), false)) return tiled(std::integral_constant<int, S::TBT_WIDE>());
+                return tiled(std::integral_constant<int, S::TBT>());
+            case PASS_R2C:
+            case PASS_C2R: {
+                if ((kind == PASS_R2C ? p.in.nseg : p.out.nseg) != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
+                if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
                 if (kind == PASS_R2C) {
-                    constexpr auto k = fft_r2c_weighted_kernel<T, LOG2N, LOG2E, S::TBC>;
+                    constexpr auto k = fft_r2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, W>;
                     return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
                 }
-                constexpr auto k = fft_c2r_weighted_kernel<T, LOG2N, LOG2E, S::TBC>;
-                return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
-            } else {
-                if (kind == PASS_R2C) {
-                    constexpr auto k = fft_r2c_padded_kernel<T, LOG2N, LOG2E, S::TBC>;
-                    return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
-                }
-                constexpr auto k = fft_c2r_padded_kernel<T, LOG2N, LOG2E, S::TBC>;
+                constexpr auto k = fft_c2r_padded_kernel<T, LOG2N, LOG2E, S::TBC, W>;
                 return launch_kernel<k, k, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
             }
+            default: return cudaErrorInvalidValue;
         }
-        default: return cudaErrorInvalidValue;
-    }
+    };
+    if (p.w) return launch(std::true_type());
+    return launch(std::false_type());
 }
 
-template <typename T, int LOG2N>
-cudaError_t launch_padded(PassKind kind, const FftPadded& p, cudaStream_t stream) {
-    return launch_twin<T, LOG2N>(kind, p, stream);
-}
-template <typename T, int LOG2N>
-cudaError_t launch_weighted(PassKind kind, const FftWeighted& p, cudaStream_t stream) {
-    if (!p.w) return cudaErrorInvalidValue;
-    return launch_twin<T, LOG2N>(kind, p, stream);
-}
-
-template cudaError_t launch_padded<DFFT_T, DFFT_LOG2N>(PassKind, const FftPadded&, cudaStream_t);
-template cudaError_t launch_weighted<DFFT_T, DFFT_LOG2N>(PassKind, const FftWeighted&, cudaStream_t);
+template cudaError_t launch_twin<DFFT_T, DFFT_LOG2N>(PassKind, const FftPadded&, cudaStream_t);
 
 #if DFFT_LOG2N >= 3
-// P: FftBluestein, or FftBluesteinW for the weighted twin
-template <typename T, int LOG2M, int TB, bool TILED, typename P>
-static cudaError_t launch_bluestein_tiles(const P& p, long long grid, cudaStream_t stream) {
+// the Bluestein kernel, its weighted instantiation (WEIGHTED = true) where p.w is set
+template <typename T, int LOG2M, int TB, bool TILED>
+static cudaError_t launch_bluestein_tiles(const FftBluestein& p, long long grid, cudaStream_t stream) {
     constexpr int LOG2E = Shape<T, LOG2M>::LOG2E;
     using C = CtaFft<T, LOG2M, LOG2E, TB, TILED>;
     if (grid <= 0) return cudaSuccess;
     if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-    if constexpr (std::is_same_v<P, FftBluesteinW>)
-        return launch_kernel<fft_bluestein_weighted_kernel<T, LOG2M, LOG2E, TB, TILED, false>, fft_bluestein_weighted_kernel<T, LOG2M, LOG2E, TB, TILED, true>,
+    if (p.w)
+        return launch_kernel<fft_bluestein_kernel<T, LOG2M, LOG2E, TB, TILED, false, true>, fft_bluestein_kernel<T, LOG2M, LOG2E, TB, TILED, true, true>,
                              nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
-    else
-        return launch_kernel<fft_bluestein_kernel<T, LOG2M, LOG2E, TB, TILED, false>, fft_bluestein_kernel<T, LOG2M, LOG2E, TB, TILED, true>, nullptr,
-                             nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+    return launch_kernel<fft_bluestein_kernel<T, LOG2M, LOG2E, TB, TILED, false, false>, fft_bluestein_kernel<T, LOG2M, LOG2E, TB, TILED, true, false>,
+                         nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
 }
 
-template <typename T, int LOG2M, typename P>
-static cudaError_t launch_bluestein_lines(PassKind kind, const P& p_in, cudaStream_t stream) {
+template <typename T, int LOG2M>
+cudaError_t launch_bluestein(PassKind kind, const FftBluestein& p_in, cudaStream_t stream) {
     using S = Shape<T, LOG2M>;
     if (p_in.n < 1 || 2 * (long long)p_in.n - 1 > (1LL << LOG2M) || !p_in.chirp || !p_in.kspec) return cudaErrorInvalidValue;
     const long long lines = (long long)p_in.A0 * p_in.A1;
     if (lines <= 0) return cudaSuccess;
-    P p = p_in;
+    FftBluestein p = p_in;
     if (kind == PASS_C2C_CONTIG) {
         if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
         return launch_bluestein_tiles<T, LOG2M, S::TBC, false>(p, (lines + S::TBC - 1) / S::TBC, stream);
@@ -367,18 +338,7 @@ static cudaError_t launch_bluestein_lines(PassKind kind, const P& p_in, cudaStre
     return launch_bluestein_tiles<T, LOG2M, S::TBT, true>(p, lines * ((p.B + S::TBT - 1) / S::TBT), stream);
 }
 
-template <typename T, int LOG2M>
-cudaError_t launch_bluestein(PassKind kind, const FftBluestein& p, cudaStream_t stream) {
-    return launch_bluestein_lines<T, LOG2M>(kind, p, stream);
-}
-template <typename T, int LOG2M>
-cudaError_t launch_bluestein(PassKind kind, const FftBluesteinW& p, cudaStream_t stream) {
-    if (!p.w) return cudaErrorInvalidValue;
-    return launch_bluestein_lines<T, LOG2M>(kind, p, stream);
-}
-
 template cudaError_t launch_bluestein<DFFT_T, DFFT_LOG2N>(PassKind, const FftBluestein&, cudaStream_t);
-template cudaError_t launch_bluestein<DFFT_T, DFFT_LOG2N>(PassKind, const FftBluesteinW&, cudaStream_t);
 #endif
 
 template <typename T, int LOG2N, int TB, bool TILED>
@@ -601,73 +561,6 @@ cudaError_t launch_batch_small(const void* in, void* out, long long batch, int i
 template cudaError_t launch_batch_small<DFFT_T, DFFT_LOG2N>(const void*, void*, long long, int, const BatchSmall&, double, cudaStream_t);
 #endif
 
-#else  // DFFT_S: the 16-bit passes
-
-// the C2C kernels of 16-bit plans over TILED tiles TB wide; tile order as in launch_tiled, no TMA-fed kernel
-template <typename H, int LOG2N, int TB>
-static cudaError_t launch_tiled16(const FftParams& p_in, double scale, cudaStream_t stream, long long lines) {
-    FftParams p = p_in;
-    const int swz = env_int("DFFT_TILE_SWZ", -1);
-    p.tile_swz = tile_swz_for(swz >= 0 ? swz : p.tile_swz, p.A0, p.A1);
-    constexpr int LOG2E = Shape<float, LOG2N>::LOG2E;
-    using C = CtaFft<float, LOG2N, LOG2E, TB, true>;
-    if (p.B <= 0) return cudaSuccess;
-    const long long grid = lines * ((p.B + TB - 1) / TB);
-    if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-    const unsigned g = unsigned((p.max_ctas > 0 && grid > p.max_ctas) ? p.max_ctas : grid);
-    return launch_kernel<fft_c2c16_kernel<H, LOG2N, LOG2E, TB, true, false, false>, fft_c2c16_kernel<H, LOG2N, LOG2E, TB, true, true, false>,
-                         fft_c2c16_kernel<H, LOG2N, LOG2E, TB, true, false, true>, fft_c2c16_kernel<H, LOG2N, LOG2E, TB, true, true, true>>(
-        p, scale, g, C::THREADS, C::SMEM_BYTES, stream);
-}
-
-// launch_pass for 16-bit plans: the shapes of the f32 pass, TILED tiles included (narrow, or wide by launch_pass's rule).
-// The TILED rows are the f32 tile's 8 elements wide from 512-point lines on, 32 bytes of 16-bit pairs: at 512^3 on an H100
-// the y and x passes took 0.43-0.50 ms with them against 0.69-0.72 ms with 64-byte rows (16 elements, twice the threads and
-// shared memory per CTA), DESIGN.md section 3.20.
-template <typename H, int LOG2N>
-cudaError_t launch_pass16(PassKind kind, const FftParams& p, double scale, cudaStream_t stream) {
-    using S = Shape<float, LOG2N>;
-    constexpr int LOG2E = S::LOG2E;
-    using C = CtaFft<float, LOG2N, LOG2E, S::TBC, false>;
-    const long long lines = (long long)p.A0 * p.A1;
-    if (lines <= 0) return cudaSuccess;
-    const long long grid = (lines + S::TBC - 1) / S::TBC;  // CONTIG, R2C and C2R
-    switch (kind) {
-        case PASS_C2C_CONTIG:
-            if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
-            if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            return launch_kernel<fft_c2c16_kernel<H, LOG2N, LOG2E, S::TBC, false, false, false>, fft_c2c16_kernel<H, LOG2N, LOG2E, S::TBC, false, true, false>,
-                                 fft_c2c16_kernel<H, LOG2N, LOG2E, S::TBC, false, false, true>, fft_c2c16_kernel<H, LOG2N, LOG2E, S::TBC, false, true, true>>(
-                p, scale, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
-        case PASS_C2C_TILED: {
-            if constexpr (S::TBT_WIDE != S::TBT) {
-                const int w = wide_tiles();
-                const bool far_rows = (unsigned long long)p.in.sN * sizeof(cx16<H>) >= (1ull << 20) ||
-                                      (unsigned long long)p.out.sN * sizeof(cx16<H>) >= (1ull << 20);
-                const bool wide = w > 0 || p.tile_pref == 2 || (w == 0 && p.tile_pref == 0 && LOG2N >= 10 && far_rows);
-                if (wide && w >= 0 && p.tile_pref != 1 && p.B > S::TBT) return launch_tiled16<H, LOG2N, S::TBT_WIDE>(p, scale, stream, lines);
-            }
-            return launch_tiled16<H, LOG2N, S::TBT>(p, scale, stream, lines);
-        }
-        case PASS_R2C: {
-            if (p.in.nseg != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
-            if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            constexpr auto k = fft_r2c16_kernel<H, LOG2N, LOG2E, S::TBC, false>;
-            constexpr auto ks = fft_r2c16_kernel<H, LOG2N, LOG2E, S::TBC, true>;
-            return launch_kernel<k, k, ks, ks>(p, scale, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
-        }
-        case PASS_C2R: {
-            if (p.out.nseg != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
-            if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            constexpr auto k = fft_c2r16_kernel<H, LOG2N, LOG2E, S::TBC, false>;
-            constexpr auto ks = fft_c2r16_kernel<H, LOG2N, LOG2E, S::TBC, true>;
-            return launch_kernel<k, k, ks, ks>(p, scale, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
-        }
-        default: return cudaErrorInvalidValue;
-    }
-}
-
-template cudaError_t launch_pass16<DFFT_S, DFFT_LOG2N>(PassKind, const FftParams&, double, cudaStream_t);
 #endif  // DFFT_S
 
 }  // namespace dfft

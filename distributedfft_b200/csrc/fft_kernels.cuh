@@ -431,23 +431,19 @@ struct MemScaled {
 // p - (hi - lo) of that side's view, so the view and its segment table are those of a K- (M-) point axis.  Forward the
 // loaded side is the physical one, inverse the spectral one.  The padded twins take the scale at run time (one
 // instantiation per precision and length).
+// Weighted passes (dfft_plan_set_weights) multiply each value of their spectral side by w[m], m the value's index in the
+// spectral view (the K stored points of a padded side): forward as it stores, inverse as it loads, before the transform.
+// They run the padded twins with WEIGHTED = true: holes (empty for plans without padding) and the scale are runtime
+// values, so one instantiation per kind and length serves every weighted plan.  The unweighted twins never read w.
 struct FftPadded : FftScaled {
     // Spectral hole: C2C [ceil(K/2), ceil(K/2) + N - K), R2C / C2R [K/2 + 1, N/2 + 1).  Physical hole: C2C [M, N), R2C / C2R
     // the pairs [M/2, N/2).  Empty when lo == hi.
     int ld_lo, ld_hi;  // of the loaded side
     int st_lo, st_hi;  // of the stored side
+    const void* w;     // weighted passes: cx<T>[spectral points of the line], Kx, Ky, Kz (C2C) or Kz/2 + 1 (R2C / C2R); else null
 };
 // index in the view of line position n, -1 in the hole
 __device__ __forceinline__ int keep_index(int n, int lo, int hi) { return n < lo ? n : (n < hi ? -1 : n - (hi - lo)); }
-
-// ---- weighted passes (dfft_plan_set_weights) ------------------------------------------------------------------------
-// A weighted pass multiplies each value of its spectral side by w[m], m the value's index in the spectral view (the K
-// stored points of a padded side): forward as it stores, inverse as it loads, before the transform.  The weighted twins
-// are the padded twins with the table: holes (empty for plans without padding) and the scale are runtime values, so one
-// instantiation per kind and length serves every weighted plan.  The unweighted kernels do not change.
-struct FftWeighted : FftPadded {
-    const void* w;  // cx<T>[spectral points of the line]: Kx, Ky, Kz (C2C) or Kz/2 + 1 (R2C / C2R)
-};
 
 // store policy of the padded twins: plain stores, scaled when s != 1 (a runtime value)
 template <typename T>
@@ -465,7 +461,7 @@ __device__ __forceinline__ void l2_discard(const void* p) { asm volatile("discar
 // PADDED: the loaded side keeps the line positions outside the hole [ld_lo, ld_hi), the stored side those outside
 // [st_lo, st_hi) (FftPadded); a side with an empty hole takes the plain path.
 // ILV (CONTIG mapping): lines of an interleaved z pass, strided by sN along n (TileCoord)
-// WEIGHTED: the spectral side's values times w[m] (FftWeighted), m their index in its view: inverse after the load,
+// WEIGHTED: the spectral side's values times w[m] (FftPadded::w), m their index in its view: inverse after the load,
 // forward before the store
 template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, typename M, typename Hook = NoGatherHook, bool PADDED = false,
           bool ILV = false, bool WEIGHTED = false>
@@ -612,18 +608,13 @@ __device__ __forceinline__ void c2c_pass(const KParams<SCALED>& p) {
     }
 }
 
-template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, bool SCALED>
+// S = cx16<H> (H = __half or __nv_bfloat16, T = float): the C2C pass of 16-bit plans, cx16<H> in memory, the f32 core, tile
+// and twiddles of the f32 pass, so each line is the f32 pass's result rounded once to 16 bits (the scaled twin: times
+// float(p.scale) first).
+template <typename T, typename S, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, bool SCALED>
 __global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
 fft_c2c_kernel(const __grid_constant__ KParams<SCALED> p) {
-    c2c_pass<T, cx<T>, LOG2N, LOG2E, TB, TILED, INV, SCALED>(p);
-}
-
-// The C2C pass of 16-bit plans (H = __half or __nv_bfloat16): cx16<H> in memory, the f32 core, tile and twiddles of the
-// f32 pass, so each line is the f32 pass's result rounded once to 16 bits (the scaled twin: times float(p.scale) first).
-template <typename H, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, bool SCALED>
-__global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<float, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
-fft_c2c16_kernel(const __grid_constant__ KParams<SCALED> p) {
-    c2c_pass<float, cx16<H>, LOG2N, LOG2E, TB, TILED, INV, SCALED>(p);
+    c2c_pass<T, S, LOG2N, LOG2E, TB, TILED, INV, SCALED>(p);
 }
 
 // Interleaved z pass (PASS_C2C_ILV, C = p.B components per point, below the TILED tile width): the CONTIG shape with its
@@ -743,8 +734,8 @@ fft_rc_ilv_kernel(const __grid_constant__ KParams<SCALED> p) {
     }
 }
 
-// padded twin of fft_c2c_kernel (FftPadded): one CTA per tile
-template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV>
+// padded twin of fft_c2c_kernel (FftPadded), and with WEIGHTED its weighted twin (p.w): one CTA per tile
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, bool WEIGHTED>
 __global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
 fft_c2c_padded_kernel(const __grid_constant__ FftPadded p) {
     using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
@@ -753,24 +744,9 @@ fft_c2c_padded_kernel(const __grid_constant__ FftPadded p) {
     unsigned long long* tab_in = reinterpret_cast<unsigned long long*>(smem_raw + C::TILE_BYTES);
     unsigned long long* tab_out = tab_in + C::LINES * MAXSEG;
     const bool multi = p.in.nseg > 1 || p.out.nseg > 1;
-    c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV, MemRtScaled<T>, NoGatherHook, true>(p, blockIdx.x, sm, tab_in, tab_out, multi,
-                                                                                 MemRtScaled<T>{p.scale != 1.0, T(p.scale)}, {}, p.ld_lo, p.ld_hi,
-                                                                                 p.st_lo, p.st_hi);
-}
-
-// weighted twin of fft_c2c_kernel and fft_c2c_padded_kernel (FftWeighted): one CTA per tile
-template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV>
-__global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
-fft_c2c_weighted_kernel(const __grid_constant__ FftWeighted p) {
-    using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
-    unsigned long long* tab_in = reinterpret_cast<unsigned long long*>(smem_raw + C::TILE_BYTES);
-    unsigned long long* tab_out = tab_in + C::LINES * MAXSEG;
-    const bool multi = p.in.nseg > 1 || p.out.nseg > 1;
-    c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV, MemRtScaled<T>, NoGatherHook, true, false, true>(
+    c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV, MemRtScaled<T>, NoGatherHook, true, false, WEIGHTED>(
         p, blockIdx.x, sm, tab_in, tab_out, multi, MemRtScaled<T>{p.scale != 1.0, T(p.scale)}, {}, p.ld_lo, p.ld_hi, p.st_lo, p.st_hi,
-        reinterpret_cast<const cx<T>*>(p.w));
+        WEIGHTED ? reinterpret_cast<const cx<T>*>(p.w) : nullptr);
 }
 
 // ---- mbarrier of an asynchronous tile copy (fft_c2c_tma_kernel, fft_zy_fused_kernel) ------------------------------
@@ -1509,7 +1485,7 @@ __device__ __forceinline__ cx<T> shfl_cx(cx<T> v, int src_lane) {
 // PADDED (P = FftPadded): the pairs m >= p.ld_lo read as zero, the points k >= p.st_lo are not stored; the scale is
 // p.scale at run time.
 // S: the stored element, of both sides (the real side in pairs: cx16<H> holds two 16-bit reals).
-// WEIGHTED (P = FftWeighted): X[k] times p.w[k] as it is stored.
+// WEIGHTED (P = FftPadded with p.w): X[k] times p.w[k] as it is stored.
 template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED, bool PADDED, typename P, typename S = cx<T>, bool WEIGHTED = false>
 __device__ __forceinline__ void r2c_lines(const P& p) {
     using C = CtaFft<T, LOG2M, LOG2E, TB, false>;
@@ -1585,37 +1561,25 @@ __device__ __forceinline__ void r2c_lines(const P& p) {
     if (j == 0) emit(M / 2);
 }
 
-template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED>
+// S = cx16<H>, T = float: the R2C z pass of 16-bit plans, the f32 line with cx16<H> loads and stores (fft_c2c_kernel)
+template <typename T, typename S, int LOG2M, int LOG2E, int TB, bool SCALED>
 __global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
 fft_r2c_kernel(const __grid_constant__ KParams<SCALED> p) {
-    r2c_lines<T, LOG2M, LOG2E, TB, SCALED, false>(p);
+    r2c_lines<T, LOG2M, LOG2E, TB, SCALED, false, KParams<SCALED>, S>(p);
 }
 
-// padded twin of fft_r2c_kernel: reads the pairs m < p.ld_lo (p.ld_hi = M), keeps the points k < p.st_lo (p.st_hi = M + 1)
-template <typename T, int LOG2M, int LOG2E, int TB>
+// padded twin of fft_r2c_kernel: reads the pairs m < p.ld_lo (p.ld_hi = M), keeps the points k < p.st_lo (p.st_hi = M + 1);
+// with WEIGHTED its weighted twin (p.w)
+template <typename T, int LOG2M, int LOG2E, int TB, bool WEIGHTED>
 __global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
 fft_r2c_padded_kernel(const __grid_constant__ FftPadded p) {
-    r2c_lines<T, LOG2M, LOG2E, TB, false, true>(p);
-}
-
-// weighted twin of fft_r2c_kernel and fft_r2c_padded_kernel (FftWeighted)
-template <typename T, int LOG2M, int LOG2E, int TB>
-__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
-fft_r2c_weighted_kernel(const __grid_constant__ FftWeighted p) {
-    r2c_lines<T, LOG2M, LOG2E, TB, false, true, FftWeighted, cx<T>, true>(p);
-}
-
-// the R2C z pass of 16-bit plans: fft_r2c_kernel's f32 line with cx16<H> loads and stores (fft_c2c16_kernel)
-template <typename H, int LOG2M, int LOG2E, int TB, bool SCALED>
-__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<float, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
-fft_r2c16_kernel(const __grid_constant__ KParams<SCALED> p) {
-    r2c_lines<float, LOG2M, LOG2E, TB, SCALED, false, KParams<SCALED>, cx16<H>>(p);
+    r2c_lines<T, LOG2M, LOG2E, TB, false, true, FftPadded, cx<T>, WEIGHTED>(p);
 }
 
 // ---- C2R pass (CONTIG): M+1 complex points -> real line of 2M points, unnormalised -----------------------
 // PADDED (P = FftPadded): the points k >= p.ld_lo read as zero, their partner loads X[M - k] as well; the pairs
 // m >= p.st_lo are not stored; the scale is p.scale at run time.
-// WEIGHTED (P = FftWeighted): X[k] and its partner X[M - k] times p.w at their index as they are loaded.
+// WEIGHTED (P = FftPadded with p.w): X[k] and its partner X[M - k] times p.w at their index as they are loaded.
 template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED, bool PADDED, typename P, typename S = cx<T>, bool WEIGHTED = false>
 __device__ __forceinline__ void c2r_lines(const P& p) {
     using C = CtaFft<T, LOG2M, LOG2E, TB, false>;
@@ -1725,32 +1689,19 @@ __device__ __forceinline__ void c2r_lines(const P& p) {
     }
 }
 
-template <typename T, int LOG2M, int LOG2E, int TB, bool SCALED>
+// S = cx16<H>, T = float: the C2R z pass of 16-bit plans, the f32 line with cx16<H> loads and stores (fft_c2c_kernel)
+template <typename T, typename S, int LOG2M, int LOG2E, int TB, bool SCALED>
 __global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
 fft_c2r_kernel(const __grid_constant__ KParams<SCALED> p) {
-    c2r_lines<T, LOG2M, LOG2E, TB, SCALED, false>(p);
+    c2r_lines<T, LOG2M, LOG2E, TB, SCALED, false, KParams<SCALED>, S>(p);
 }
 
 // padded twin of fft_c2r_kernel: the points k >= p.ld_lo are zero (p.ld_hi = M + 1), the pairs m >= p.st_lo are not stored
-// (p.st_hi = M)
-template <typename T, int LOG2M, int LOG2E, int TB>
+// (p.st_hi = M); with WEIGHTED its weighted twin (p.w)
+template <typename T, int LOG2M, int LOG2E, int TB, bool WEIGHTED>
 __global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
 fft_c2r_padded_kernel(const __grid_constant__ FftPadded p) {
-    c2r_lines<T, LOG2M, LOG2E, TB, false, true>(p);
-}
-
-// weighted twin of fft_c2r_kernel and fft_c2r_padded_kernel (FftWeighted)
-template <typename T, int LOG2M, int LOG2E, int TB>
-__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
-fft_c2r_weighted_kernel(const __grid_constant__ FftWeighted p) {
-    c2r_lines<T, LOG2M, LOG2E, TB, false, true, FftWeighted, cx<T>, true>(p);
-}
-
-// the C2R z pass of 16-bit plans: fft_c2r_kernel's f32 line with cx16<H> loads and stores (fft_c2c16_kernel)
-template <typename H, int LOG2M, int LOG2E, int TB, bool SCALED>
-__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<float, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
-fft_c2r16_kernel(const __grid_constant__ KParams<SCALED> p) {
-    c2r_lines<float, LOG2M, LOG2E, TB, SCALED, false, KParams<SCALED>, cx16<H>>(p);
+    c2r_lines<T, LOG2M, LOG2E, TB, false, true, FftPadded, cx<T>, WEIGHTED>(p);
 }
 
 // ---- Bluestein pass: C2C lines of any length n through two transforms of length M = 2^LOG2M >= 2n - 1 ----------------
@@ -1764,16 +1715,12 @@ struct FftBluestein : FftParams {
     const void* chirp;  // c_k, k < n
     const void* kspec;  // K^_m, m < M
     double scale;       // output scale, applied when != 1 (rounded to the kernel's precision once)
+    const void* w;      // weighted passes (dfft_plan_set_weights, WEIGHTED): w[k], k < n, multiplies X_k forward as it is
+                        // stored and x_k inverse as it is loaded; else null
 };
 
-// weighted Bluestein pass (dfft_plan_set_weights): w[k], k < n, multiplies X_k forward as it is stored and x_k inverse as it
-// is loaded
-struct FftBluesteinW : FftBluestein {
-    const void* w;
-};
-
-template <typename T, int LOG2M, int LOG2E, int TB, bool TILED, bool INV, bool WEIGHTED, typename P>
-__device__ __forceinline__ void bluestein_lines(const P& p) {
+template <typename T, int LOG2M, int LOG2E, int TB, bool TILED, bool INV, bool WEIGHTED>
+__device__ __forceinline__ void bluestein_lines(const FftBluestein& p) {
     using C = CtaFft<T, LOG2M, LOG2E, TB, TILED>;
     using LA = LineAccess<T, C::LINES>;
     using TC = TileCoord<C, TILED, TB>;
@@ -1833,16 +1780,10 @@ __device__ __forceinline__ void bluestein_lines(const P& p) {
     }
 }
 
-template <typename T, int LOG2M, int LOG2E, int TB, bool TILED, bool INV>
+template <typename T, int LOG2M, int LOG2E, int TB, bool TILED, bool INV, bool WEIGHTED>
 __global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
 fft_bluestein_kernel(const __grid_constant__ FftBluestein p) {
-    bluestein_lines<T, LOG2M, LOG2E, TB, TILED, INV, false>(p);
-}
-
-template <typename T, int LOG2M, int LOG2E, int TB, bool TILED, bool INV>
-__global__ void __launch_bounds__((1 << (LOG2M - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2M - LOG2E)) * TB))
-fft_bluestein_weighted_kernel(const __grid_constant__ FftBluesteinW p) {
-    bluestein_lines<T, LOG2M, LOG2E, TB, TILED, INV, true>(p);
+    bluestein_lines<T, LOG2M, LOG2E, TB, TILED, INV, WEIGHTED>(p);
 }
 
 // ---- real-to-real pass: DCT-II / DCT-III, DST-II / DST-III and R2HC / HC2R of real N-point lines ------------------------
@@ -2299,32 +2240,23 @@ __global__ void __launch_bounds__(COPY_THREADS) fft_copy_kernel(const __grid_con
 }
 
 // ---- host launchers (one explicit instantiation per precision and size, see fft_inst.cu) ----------------
+// S: the stored element, cx<T>, or cx16<H> with T = float for 16-bit plans (H = __half for DFFT_F16, __nv_bfloat16 for
+// DFFT_BF16: kind PASS_C2C_CONTIG, PASS_C2C_TILED, PASS_R2C or PASS_C2R, the f32 kernels' arithmetic).
 // scale: the output scale of the pass' stores; 1 launches the unscaled kernels, anything else their scaled twins.
-template <typename T, int LOG2N>
+template <typename T, typename S, int LOG2N>
 cudaError_t launch_pass(PassKind kind, const FftParams& p, double scale, cudaStream_t stream);
 
-// Each launcher also has a runtime form (fft_dispatch.cu) that takes the precision (DFFT_F64 / DFFT_F32) and the log2 length
-// first; it returns cudaErrorInvalidValue for a length that is not instantiated.
+// Each launcher also has a runtime form (fft_dispatch.cu) that takes the precision (DFFT_F64 / DFFT_F32; launch_pass also
+// DFFT_F16 / DFFT_BF16) and the log2 length first; it returns cudaErrorInvalidValue for a length that is not instantiated.
 cudaError_t launch_pass(int prec, int log2n, PassKind kind, const FftParams& p, double scale, cudaStream_t stream);
-
-// 16-bit plans (cx16<H> views, H = __half for DFFT_F16, __nv_bfloat16 for DFFT_BF16): kind PASS_C2C_CONTIG, PASS_C2C_TILED,
-// PASS_R2C or PASS_C2R over the views of launch_pass, the f32 kernels' arithmetic; scale != 1 launches the scaled twins.
-// The runtime form launch_pass(prec, ...) takes DFFT_F16 / DFFT_BF16 to them.
-template <typename H, int LOG2N>
-cudaError_t launch_pass16(PassKind kind, const FftParams& p, double scale, cudaStream_t stream);
 
 // padded pass (FftPadded): kind PASS_C2C_CONTIG, PASS_C2C_TILED, PASS_R2C or PASS_C2R over the views of launch_pass, the
 // hole [p.ld_lo, p.ld_hi) of each line on its loaded side and [p.st_lo, p.st_hi) on its stored side (R2C / C2R: both reach
-// the end of the line); p.scale scales the stores.
+// the end of the line); p.scale scales the stores.  With p.w set (dfft_plan_set_weights) the weighted twins run: p.w
+// multiplies the spectral side, whose holes may be empty.
 template <typename T, int LOG2N>
-cudaError_t launch_padded(PassKind kind, const FftPadded& p, cudaStream_t stream);
-cudaError_t launch_padded(int prec, int log2n, PassKind kind, const FftPadded& p, cudaStream_t stream);
-
-// weighted pass (FftWeighted, dfft_plan_set_weights): the padded pass with p.w multiplying its spectral side (holes may be
-// empty); the weighted twins, the tiles of launch_padded
-template <typename T, int LOG2N>
-cudaError_t launch_weighted(PassKind kind, const FftWeighted& p, cudaStream_t stream);
-cudaError_t launch_weighted(int prec, int log2n, PassKind kind, const FftWeighted& p, cudaStream_t stream);
+cudaError_t launch_twin(PassKind kind, const FftPadded& p, cudaStream_t stream);
+cudaError_t launch_twin(int prec, int log2n, PassKind kind, const FftPadded& p, cudaStream_t stream);
 
 // fused z + y stage (fft_zy_fused_kernel), instantiated for the lengths zy_fused_length accepts.  pz: the z pass, py: the y
 // pass, f: counters and plane groups (f.order.na / nb are filled in here).  Every launch of one step must use the same
@@ -2345,14 +2277,11 @@ cudaError_t launch_batch_small(int prec, int log2n, const void* in, void* out, l
                                cudaStream_t stream);
 
 // Bluestein pass (fft_bluestein_kernel) of p.n-point lines, M = 2^LOG2M >= 2 p.n - 1: kind PASS_C2C_CONTIG or PASS_C2C_TILED
-// (the view mapping of the power-of-two pass), one CTA per tile; p.scale scales the stores.  Instantiated for LOG2M 3..13.
+// (the view mapping of the power-of-two pass), one CTA per tile; p.scale scales the stores, p.w (if set) weights them (the
+// weighted twin, WEIGHTED = true).  Instantiated for LOG2M 3..13.
 template <typename T, int LOG2M>
 cudaError_t launch_bluestein(PassKind kind, const FftBluestein& p, cudaStream_t stream);
 cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluestein& p, cudaStream_t stream);
-// its weighted twin (fft_bluestein_weighted_kernel)
-template <typename T, int LOG2M>
-cudaError_t launch_bluestein(PassKind kind, const FftBluesteinW& p, cudaStream_t stream);
-cudaError_t launch_bluestein(int prec, int log2m, PassKind kind, const FftBluesteinW& p, cudaStream_t stream);
 
 // R2R pass of 2^LOG2N-point real lines: kind PASS_R2R_CONTIG (sN == 1, line pairs) or PASS_R2R_TILED (column pairs), views
 // in reals, one CTA per tile; p.scale scales the stores.  hc: R2HC / HC2R (fft_r2hc_kernel), otherwise DCT / DST
