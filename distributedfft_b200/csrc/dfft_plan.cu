@@ -2819,25 +2819,195 @@ int dfft_plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, in
 
 }  // extern "C"
 
-// kinds: of the plans of dfft_plan_create_r2r (their transform is DFFT_DCT, DFFT_DST or DFFT_R2HC), nullptr otherwise.
-// spectral: Kx, Ky, Kz of the plans of dfft_plan_create_padded and _pruned (checked there), nullptr otherwise.
-// data: Mx, My, Mz of the plans of dfft_plan_create_pruned (checked there), nullptr otherwise.
-static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
-                       size_t nz, size_t p1, size_t p2, size_t batch, bool inplace, int allocate, dfft_plan_t* plan,
-                       const int* kinds = nullptr, const size_t* spectral = nullptr, size_t comps = 1,
-                       const std::vector<dfft::Box>* in_boxes = nullptr, const std::vector<dfft::Box>* out_boxes = nullptr,
-                       const size_t* data = nullptr) {
-    if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
-    if (batch == 0) return fail(DFFT_ERR_INVALID, "batch must be at least 1");
-    if (precision < DFFT_F32 || precision > DFFT_BF16) return fail(DFFT_ERR_INVALID, "bad precision");
-    if (transform != DFFT_R2C && transform != DFFT_C2C && !is_r2r(transform)) return fail(DFFT_ERR_INVALID, "bad transform");
-    if (transform == DFFT_R2HC && !kinds) return fail(DFFT_ERR_INVALID, "bad transform (per-axis kinds: dfft_plan_create_r2r)");
-    if (is_half(precision)) {
-        if (is_r2r(transform)) return refuse_half("DCT / DST plans");
-        if (transform == DFFT_C2C && !(pow2_length(nx) && pow2_length(ny) && pow2_length(nz)))
-            return fail(DFFT_ERR_UNSUPPORTED, "16-bit storage (DFFT_F16 / DFFT_BF16) takes power-of-two lengths in [2, 8192] only (no Bluestein pass)");
+// Plan features, as bits: what a plan description or a plan has, and what a creator or a setter adds.  A description
+// has the feature of the creator that made it (F_BOXES, F_PADDED, F_PRUNED, F_INTERLEAVED or F_KINDS) whatever its
+// arguments; a plan has F_PADDED, F_PRUNED and F_INTERLEAVED when its K, M or C says so.
+enum Feature : unsigned {
+    F_HALF = 1u << 0,         // 16-bit storage (DFFT_F16 / DFFT_BF16)
+    F_R2R = 1u << 1,          // a DCT / DST transform or per-axis kinds
+    F_INPLACE = 1u << 2,      // dfft_plan_create_inplace, or in place by dfft_plan_create_r2r
+    F_BOXES = 1u << 3,        // dfft_plan_create_boxes
+    F_PADDED = 1u << 4,       // dfft_plan_create_padded; a plan with K < N
+    F_PRUNED = 1u << 5,       // dfft_plan_create_pruned; a plan with M < N
+    F_INTERLEAVED = 1u << 6,  // dfft_plan_create_interleaved; a plan of more than one component
+    F_KINDS = 1u << 7,        // dfft_plan_create_r2r
+    F_KEPT_AXES = 1u << 8,    // dfft_plan_set_transform_axes with an axis kept
+    F_STRIDES = 1u << 9,      // dfft_plan_set_strides
+    F_WEIGHTS = 1u << 10,     // dfft_plan_set_weights
+};
+
+// The features that do not combine, in the order they are refused: adding `adds` to a description or a plan that has
+// `with` returns DFFT_ERR_UNSUPPORTED.  A row with F_HALF names what has no 16-bit storage.
+struct Refusal { unsigned adds, with; const char* what; };
+static const Refusal refusals[] = {
+    {F_BOXES, F_HALF, "box plans"},
+    {F_PADDED, F_HALF, "padded plans"},
+    {F_PRUNED, F_HALF, "pruned plans"},
+    {F_INTERLEAVED, F_HALF, "interleaved plans"},
+    {F_KINDS, F_HALF, "real-to-real plans"},
+    {F_HALF, F_R2R, "DCT / DST plans"},
+    {F_KEPT_AXES, F_PADDED, "padded plans transform every axis"},
+    {F_KEPT_AXES, F_PRUNED, "pruned plans transform every axis"},
+    {F_KEPT_AXES, F_INTERLEAVED, "interleaved plans transform every axis"},
+    {F_STRIDES, F_HALF, "plans with strides"},
+    {F_STRIDES, F_INPLACE, "in-place plans keep the padded layout of FFTW and cuFFT: strides are for out-of-place plans"},
+    {F_STRIDES, F_INTERLEAVED, "interleaved plans keep their [x][y][z][C] layout: strides are for plans of one component"},
+    {F_STRIDES, F_PRUNED, "pruned plans read and write dense data blocks: strides are for plans without a data size"},
+    {F_WEIGHTS, F_INTERLEAVED, "interleaved plans of more than one component have no spectral weights"},
+    {F_WEIGHTS, F_R2R, "real-to-real plans (DCT / DST and per-axis kinds) have no spectral weights"},
+    {F_WEIGHTS, F_HALF, "spectral weights"},
+};
+// The first refusal of adding `adds` to a description or a plan with the features `has`, or DFFT_SUCCESS
+static int refuse(unsigned has, unsigned adds) {
+    for (const Refusal& r : refusals)
+        if ((r.adds & adds) && (r.with & has))
+            return (r.adds | r.with) & F_HALF ? refuse_half(r.what) : fail(DFFT_ERR_UNSUPPORTED, r.what);
+    return DFFT_SUCCESS;
+}
+static unsigned features(const dfft_plan_s* p) {
+    return (is_half(p->prec) ? F_HALF : 0) | (is_r2r(p->g.transform) ? F_R2R : 0) | (p->inplace ? F_INPLACE : 0) | (p->g.padded() ? F_PADDED : 0) |
+           (p->g.pruned() ? F_PRUNED : 0) | (p->comps > 1 ? F_INTERLEAVED : 0);
+}
+
+// bytes of one element: complex, or real for DCT / DST plans
+static size_t elem_bytes(int precision, int transform) {
+    return (precision == DFFT_F64 ? 16 : is_half(precision) ? 4 : 8) / (is_r2r(transform) ? 2 : 1);
+}
+
+// The description of a plan: what one dfft_plan_create* entry point asks for.  Each creator sets the fields of its feature.
+struct PlanSpec {
+    unsigned made_by;  // F_BOXES, F_PADDED, F_PRUNED, F_INTERLEAVED or F_KINDS; 0 for dfft_plan_create_batched / _inplace
+    int decomp, precision, transform;
+    size_t n[3], p1, p2, batch;
+    bool inplace = false;
+    const int* kinds = nullptr;                 // dfft_plan_create_r2r: the kinds of the x, y and z axis
+    size_t comps = 1;                           // values per grid point
+    size_t k[3] = {0, 0, 0}, m[3] = {0, 0, 0};  // the spectral and data sizes; 0: the grid
+    std::vector<Box> boxes[2];                  // the in and out box of every rank; empty: that side has its natural layout
+    PlanSpec(unsigned made_by_, int decomp_, int precision_, int transform_, size_t nx, size_t ny, size_t nz, size_t p1_, size_t p2_, size_t batch_)
+        : made_by(made_by_), decomp(decomp_), precision(precision_), transform(transform_), n{nx, ny, nz}, p1(p1_), p2(p2_), batch(batch_) {}
+    unsigned features() const { return made_by | (is_half(precision) ? F_HALF : 0) | (is_r2r(transform) ? F_R2R : 0) | (inplace ? F_INPLACE : 0); }
+};
+
+// The spectral (padded, pruned) or data (pruned) sizes of a plan
+static int check_sub_grid(const size_t n[3], const size_t sizes[3], const char* what) {
+    for (int a = 0; a < 3; ++a) {
+        if (sizes[a] == 0 || sizes[a] > n[a])
+            return fail(DFFT_ERR_INVALID, std::string(what) + " size " + std::to_string(sizes[a]) + " of axis " + "xyz"[a] + " must be in [1, " +
+                                              std::to_string(n[a]) + "]");
+        if (sizes[a] < n[a] && ilog2_exact(n[a]) < 0)
+            return fail(DFFT_ERR_UNSUPPORTED, std::string("axis ") + "xyz"[a] + " of length " + std::to_string(n[a]) + " is not a power of two: its " +
+                                                  what + " size must be its length");
     }
-    const bool dry = comm->dry;
+    return DFFT_SUCCESS;
+}
+
+// C values per point: the C = 1 plan with every element widened to C consecutive values (DESIGN.md section 3.14).  The
+// z pass of C > 1 runs interleaved lines (PASS_C2C_ILV) or R2C / C2R lines of Nz points, one per component (PASS_R2C_ILV /
+// PASS_C2R_ILV), which exist for a power-of-two Nz (R2C: up to 8192).
+constexpr size_t MAX_COMPONENTS = 64;
+
+// Every rule a plan description must meet, checked before anything is allocated: first the rules of the creator that
+// made it, then those of every plan.  The order decides which error an input with several faults gets.  g: the plan's
+// geometry.
+static int check_spec(dfft_comm_t comm, const dfft_plan_t* plan, const PlanSpec& s, Geometry& g) {
+    const unsigned has = s.features();
+    const size_t* n = s.n;
+    if (s.made_by == F_BOXES && (!comm || !plan)) return fail(DFFT_ERR_INVALID, "null comm / plan");
+    if (int rc = refuse(has, s.made_by)) return rc;
+    if (s.made_by == F_BOXES) {  // DESIGN.md section 3.17
+        if (s.transform != DFFT_C2C && s.transform != DFFT_R2C && s.transform != DFFT_DCT && s.transform != DFFT_DST)
+            return fail(DFFT_ERR_INVALID, "box plans are C2C, R2C / C2R, DCT or DST");
+        const size_t grid[2][3] = {{n[0], n[1], n[2]}, {n[0], n[1], s.transform == DFFT_R2C ? n[2] / 2 + 1 : n[2]}};
+        for (int side = 0; side < 2; ++side)
+            if (!s.boxes[side].empty() && !tiles(s.boxes[side], grid[side]))
+                return fail(DFFT_ERR_INVALID, std::string(side ? "out_boxes" : "in_boxes") +
+                                                  " must tile the grid: every box non-empty and inside it, no two overlapping, together all of it");
+        // the real side of R2C / C2R plans moves as pairs of reals (the z pass's complex units)
+        if (s.transform == DFFT_R2C)
+            for (const Box& b : s.boxes[0])
+                if (b.lo[2] % 2 || b.hi[2] % 2) return fail(DFFT_ERR_UNSUPPORTED, "R2C / C2R box plans need even z bounds in in_boxes");
+    } else if (s.made_by == F_PADDED || s.made_by == F_PRUNED) {
+        if (s.transform == DFFT_DCT || s.transform == DFFT_DST)
+            return fail(DFFT_ERR_UNSUPPORTED, s.made_by == F_PADDED ? "padded plans are C2C or R2C / C2R" : "pruned plans are C2C or R2C / C2R");
+        if (s.transform != DFFT_C2C && s.transform != DFFT_R2C) return fail(DFFT_ERR_INVALID, "bad transform");
+        if (s.made_by == F_PRUNED)
+            if (int rc = check_sub_grid(n, s.m, "data")) return rc;
+        if (int rc = check_sub_grid(n, s.k, "spectral")) return rc;
+        // the real side of R2C / C2R moves as pairs of reals (the z pass's complex units)
+        if (s.made_by == F_PRUNED && s.transform == DFFT_R2C && s.m[2] % 2)
+            return fail(DFFT_ERR_UNSUPPORTED, "R2C / C2R pruned plans need an even data size along z");
+    } else if (s.made_by == F_INTERLEAVED) {
+        if (s.comps == 0) return fail(DFFT_ERR_INVALID, "components must be at least 1");
+        if (s.comps > MAX_COMPONENTS) return fail(DFFT_ERR_UNSUPPORTED, "at most " + std::to_string(MAX_COMPONENTS) + " components per point");
+        if (s.comps > 1) {
+            if (s.transform != DFFT_C2C && s.transform != DFFT_R2C && !is_r2r(s.transform)) return fail(DFFT_ERR_INVALID, "bad transform");
+            if (is_r2r(s.transform)) return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans with more than one component are C2C or R2C / C2R");
+            if (ilog2_exact(n[2]) < 1) return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans need a power-of-two Nz (x and y may have any C2C length)");
+            // the interleaved R2C / C2R z pass runs Nz-point complex lines
+            if (s.transform == DFFT_R2C && ilog2_exact(n[2]) > MAX_LOG2N)
+                return fail(DFFT_ERR_UNSUPPORTED, "interleaved R2C / C2R plans need Nz <= " + std::to_string(1 << MAX_LOG2N));
+        }
+    } else if (s.made_by == F_KINDS) {
+        if (!s.kinds) return fail(DFFT_ERR_INVALID, "null kinds");
+        for (int a = 0; a < 3; ++a)
+            if (!is_r2r_kind(s.kinds[a]))
+                return fail(DFFT_ERR_INVALID, "kinds must be DFFT_DCT, DFFT_DST, DFFT_R2HC, DFFT_DCT1, DFFT_DST1, DFFT_DCT4 or DFFT_DST4");
+    }
+
+    if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
+    if (s.batch == 0) return fail(DFFT_ERR_INVALID, "batch must be at least 1");
+    if (s.precision < DFFT_F32 || s.precision > DFFT_BF16) return fail(DFFT_ERR_INVALID, "bad precision");
+    if (s.transform != DFFT_R2C && s.transform != DFFT_C2C && !is_r2r(s.transform)) return fail(DFFT_ERR_INVALID, "bad transform");
+    if (s.transform == DFFT_R2HC && !s.kinds) return fail(DFFT_ERR_INVALID, "bad transform (per-axis kinds: dfft_plan_create_r2r)");
+    if (int rc = refuse(has, has & F_HALF)) return rc;
+    if (is_half(s.precision) && s.transform == DFFT_C2C && !(pow2_length(n[0]) && pow2_length(n[1]) && pow2_length(n[2])))
+        return fail(DFFT_ERR_UNSUPPORTED, "16-bit storage (DFFT_F16 / DFFT_BF16) takes power-of-two lengths in [2, 8192] only (no Bluestein pass)");
+    if (!g.init(s.decomp, s.transform, n[0], n[1], n[2], s.p1, s.p2, comm->nranks, s.k[0], s.k[1], s.k[2], s.m[0], s.m[1], s.m[2]))
+        return fail(DFFT_ERR_INVALID, "invalid partition: P1*P2 must equal the communicator size");
+    if (s.transform == DFFT_C2C) {
+        if (!c2c_length(n[0]) || !c2c_length(n[1]) || !c2c_length(n[2]))
+            return fail(DFFT_ERR_UNSUPPORTED, "Nx, Ny, Nz of C2C plans must be powers of two in [2, 8192] or any length in [3, 4096]");
+    } else if (is_r2r(s.transform)) {
+        for (int a = 0; a < 3; ++a) {
+            const int kind = s.kinds ? s.kinds[a] : s.transform;
+            if (!r2r_kind_length(kind, n[a]))
+                return fail(DFFT_ERR_UNSUPPORTED, kind == DFFT_DCT1   ? "DCT-I axes must have 2^k + 1 points in [3, 8193]"
+                                                  : kind == DFFT_DST1 ? "DST-I axes must have 2^k - 1 points in [3, 8191]"
+                                                  : is_type4(kind)    ? "DCT-IV / DST-IV axes must have 2^k points in [4, 8192]"
+                                                                      : "Nx, Ny, Nz of DCT / DST plans must be powers of two in [2, 8192]");
+        }
+    } else if (ilog2_exact(n[0]) < 1 || ilog2_exact(n[1]) < 1 || ilog2_exact(n[2]) < 1 || ilog2_exact(n[0]) > MAX_LOG2N ||
+               ilog2_exact(n[1]) > MAX_LOG2N || ilog2_exact(n[2]) > MAX_LOG2N + 1 || n[2] < 4) {
+        return fail(DFFT_ERR_UNSUPPORTED, "Nx, Ny, Nz must be powers of two in [2, 8192] (Nz >= 4 for R2C)");
+    }
+    // every rank needs a non-empty share along each split axis
+    if (g.sx.size.back() == 0 || g.sy.size.back() == 0 || g.sz.size.back() == 0 || g.oy.size.back() == 0)
+        return fail(DFFT_ERR_INVALID, "partition leaves a rank without data");
+    // the whole batch of every caller buffer (any direction, any partial d: field_bytes) must be addressable
+    const int r = comm->rank;
+    const size_t es = elem_bytes(s.precision, s.transform) * s.comps, real_es = s.transform == DFFT_R2C ? es / 2 : es;
+    auto points = [&](int which) {  // of this rank's caller array of layout `which`: its box, if that side has boxes
+        const std::vector<Box>* b = which == 0 ? &s.boxes[0] : which == 3 ? &s.boxes[1] : nullptr;
+        if (b && !b->empty()) return (*b)[size_t(r)].volume();
+        size_t sz[3], o[3];
+        g.layout(r, which, sz, o);
+        return sz[0] * sz[1] * sz[2];
+    };
+    size_t widest = s.inplace ? g.domain_elems(r) * es : points(0) * real_es;
+    for (int d = 1; d <= 3 && !s.inplace; ++d) widest = std::max(widest, points(d) * es);
+    if (s.batch > SIZE_MAX / widest)
+        return fail(DFFT_ERR_INVALID, "batch of " + std::to_string(s.batch) + " fields of " + std::to_string(widest) +
+                                          " bytes overflows the address range (size_t)");
+    return DFFT_SUCCESS;
+}
+
+static int plan_create(dfft_comm_t comm, const dfft_config* config, const PlanSpec& s, int allocate, dfft_plan_t* plan) {
+    Geometry geom;
+    if (int rc = check_spec(comm, plan, s, geom)) return rc;
+    const int decomp = s.decomp, precision = s.precision, transform = s.transform;
+    const size_t nx = s.n[0], ny = s.n[1], nz = s.n[2], comps = s.comps;
+    const bool dry = comm->dry, inplace = s.inplace;
     if (!dry) CK_CUDA(cudaSetDevice(comm->device));
     const auto t_init0 = std::chrono::steady_clock::now();
     dfft_plan_s* p = new dfft_plan_s();
@@ -2851,56 +3021,26 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
     }
     p->rank = comm->rank; p->P = comm->nranks;
     p->prec = precision;
-    for (int a = 0; a < 3; ++a) p->kinds[a] = kinds ? kinds[a] : is_r2r(transform) ? transform : 0;
-    p->esize = (precision == DFFT_F64 ? 16 : is_half(precision) ? 4 : 8) / (is_r2r(transform) ? 2 : 1);  // DCT / DST: real elements
+    for (int a = 0; a < 3; ++a) p->kinds[a] = s.kinds ? s.kinds[a] : is_r2r(transform) ? transform : 0;
+    p->esize = elem_bytes(precision, transform);
     p->comps = comps;
     p->tabs.prec = precision;
     p->tabs.dry = dry;
-    if (!p->g.init(decomp, transform, nx, ny, nz, p1, p2, p->P, spectral ? spectral[0] : 0, spectral ? spectral[1] : 0, spectral ? spectral[2] : 0,
-                   data ? data[0] : 0, data ? data[1] : 0, data ? data[2] : 0)) {
-        delete p;
-        return fail(DFFT_ERR_INVALID, "invalid partition: P1*P2 must equal the communicator size");
-    }
+    p->g = geom;
     const Geometry& g = p->g;
-    if (transform == DFFT_C2C) {
-        if (!c2c_length(nx) || !c2c_length(ny) || !c2c_length(nz)) {
-            delete p;
-            return fail(DFFT_ERR_UNSUPPORTED, "Nx, Ny, Nz of C2C plans must be powers of two in [2, 8192] or any length in [3, 4096]");
-        }
-    } else if (is_r2r(transform)) {
-        const size_t n[3] = {nx, ny, nz};
-        for (int a = 0; a < 3; ++a) {
-            if (r2r_kind_length(p->kinds[a], n[a])) continue;
-            const std::string what = p->kinds[a] == DFFT_DCT1   ? "DCT-I axes must have 2^k + 1 points in [3, 8193]"
-                                     : p->kinds[a] == DFFT_DST1 ? "DST-I axes must have 2^k - 1 points in [3, 8191]"
-                                     : is_type4(p->kinds[a])    ? "DCT-IV / DST-IV axes must have 2^k points in [4, 8192]"
-                                                                : "Nx, Ny, Nz of DCT / DST plans must be powers of two in [2, 8192]";
-            delete p;
-            return fail(DFFT_ERR_UNSUPPORTED, what);
-        }
-    } else if (ilog2_exact(nx) < 1 || ilog2_exact(ny) < 1 || ilog2_exact(nz) < 1 || ilog2_exact(nx) > MAX_LOG2N || ilog2_exact(ny) > MAX_LOG2N ||
-               ilog2_exact(nz) > MAX_LOG2N + 1 || nz < 4) {
-        delete p;
-        return fail(DFFT_ERR_UNSUPPORTED, "Nx, Ny, Nz must be powers of two in [2, 8192] (Nz >= 4 for R2C)");
-    }
-    // every rank needs a non-empty share along each split axis
-    if (g.sx.size.back() == 0 || g.sy.size.back() == 0 || g.sz.size.back() == 0 || g.oy.size.back() == 0) {
-        delete p;
-        return fail(DFFT_ERR_INVALID, "partition leaves a rank without data");
-    }
     p->inplace = inplace;
-    // box plans (dfft_plan_create_boxes, which checked the tiling): a side whose boxes are all natural keeps no boxes, so
-    // that it makes exactly the plan of dfft_plan_create_batched
-    auto keep_boxes = [&](const std::vector<Box>* b, int which, std::vector<Box>& dst) {
-        if (!b) return;
-        for (int r = 0; r < p->P; ++r) {
+    p->batch = s.batch;
+    // box plans: a side whose boxes are all natural keeps no boxes, so that it makes exactly the plan of
+    // dfft_plan_create_batched
+    auto keep_boxes = [&](const std::vector<Box>& b, int which, std::vector<Box>& dst) {
+        for (int r = 0; r < int(b.size()); ++r) {
             size_t s_[3], o_[3];
             g.layout(r, which, s_, o_);
-            if (!((*b)[size_t(r)] == Box::of(s_, o_))) { dst = *b; return; }
+            if (!(b[size_t(r)] == Box::of(s_, o_))) { dst = b; return; }
         }
     };
-    keep_boxes(in_boxes, 0, p->in_boxes);
-    keep_boxes(out_boxes, 3, p->out_boxes);
+    keep_boxes(s.boxes[0], 0, p->in_boxes);
+    keep_boxes(s.boxes[1], 3, p->out_boxes);
     // elements (of the schedule's views) of rank r's box arrays: the real side of R2C / C2R in complex pairs
     auto box_elems = [&](int r) {
         size_t m = 0;
@@ -2911,20 +3051,6 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, int decomp, 
     // the largest stage array of this rank; it also covers the padded real input of in-place R2C plans, which has the
     // extent of the layout after d = 1
     p->domain_bytes = std::max(g.domain_elems(p->rank), box_elems(p->rank)) * p->esize * comps;
-    {   // the whole batch of every caller buffer (any direction, any partial d) must be addressable
-        size_t widest = 0;
-        for (int d = 1; d <= 3; ++d) {
-            size_t bi = 0, bo = 0;
-            field_bytes(p, 0, d, &bi, &bo);
-            widest = std::max(widest, std::max(bi, bo));
-        }
-        if (batch > SIZE_MAX / widest) {
-            delete p;
-            return fail(DFFT_ERR_INVALID, "batch of " + std::to_string(batch) + " fields of " + std::to_string(widest) +
-                                              " bytes overflows the address range (size_t)");
-        }
-        p->batch = batch;
-    }
     // groups
     const int me = p->rank, P = p->P;
     p->grp[0].clear();
@@ -3068,85 +3194,49 @@ extern "C" {
 
 int dfft_plan_create_batched(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
                              size_t nz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan) {
-    return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, false, allocate, plan);
+    return plan_create(comm, config, PlanSpec(0, decomp, precision, transform, nx, ny, nz, p1, p2, batch), allocate, plan);
 }
 
 int dfft_plan_create_inplace(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
                              size_t nz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan) {
-    return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, true, allocate, plan);
+    PlanSpec s(0, decomp, precision, transform, nx, ny, nz, p1, p2, batch);
+    s.inplace = true;
+    return plan_create(comm, config, s, allocate, plan);
 }
 
 int dfft_plan_is_inplace(dfft_plan_t p) { return p && p->inplace ? 1 : 0; }
 
-// Box plans (DESIGN.md section 3.17): the boxes are checked here, before plan_create allocates anything.
+// Box plans (DESIGN.md section 3.17): six values (lo, hi) per rank on each side that has boxes
 int dfft_plan_create_boxes(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny, size_t nz,
                            size_t p1, size_t p2, const size_t* in_boxes, const size_t* out_boxes, size_t batch, int allocate, dfft_plan_t* plan) {
-    if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
-    if (is_half(precision)) return refuse_half("box plans");
-    if (transform != DFFT_C2C && transform != DFFT_R2C && transform != DFFT_DCT && transform != DFFT_DST)
-        return fail(DFFT_ERR_INVALID, "box plans are C2C, R2C / C2R, DCT or DST");
-    const size_t P = size_t(comm->nranks);
-    const size_t grid[2][3] = {{nx, ny, nz}, {nx, ny, transform == DFFT_R2C ? nz / 2 + 1 : nz}};
-    std::vector<Box> boxes[2];
+    PlanSpec s(F_BOXES, decomp, precision, transform, nx, ny, nz, p1, p2, batch);
     const size_t* given[2] = {in_boxes, out_boxes};
-    for (int side = 0; side < 2; ++side) {
-        if (!given[side]) continue;
-        for (size_t r = 0; r < P; ++r) {
+    for (int side = 0; side < 2; ++side)
+        for (int r = 0; given[side] && comm && r < comm->nranks; ++r) {
             Box b;
             for (int a = 0; a < 3; ++a) { b.lo[a] = given[side][6 * r + a]; b.hi[a] = given[side][6 * r + 3 + a]; }
-            boxes[side].push_back(b);
+            s.boxes[side].push_back(b);
         }
-        if (!tiles(boxes[side], grid[side]))
-            return fail(DFFT_ERR_INVALID, std::string(side ? "out_boxes" : "in_boxes") +
-                                              " must tile the grid: every box non-empty and inside it, no two overlapping, together all of it");
-    }
-    // the real side of R2C / C2R plans moves as pairs of reals (the z pass's complex units)
-    if (transform == DFFT_R2C)
-        for (const Box& b : boxes[0])
-            if (b.lo[2] % 2 || b.hi[2] % 2) return fail(DFFT_ERR_UNSUPPORTED, "R2C / C2R box plans need even z bounds in in_boxes");
-    return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, false, allocate, plan, nullptr, nullptr, 1,
-                       in_boxes ? &boxes[0] : nullptr, out_boxes ? &boxes[1] : nullptr);
-}
-
-// The checks of padded and pruned plans: sizes[0..2] the spectral (what = "spectral") or data (what = "data") grid
-static int check_sub_grid(int transform, size_t nx, size_t ny, size_t nz, const size_t sizes[3], const char* what) {
-    const bool spectral = what[0] == 's';
-    if (transform == DFFT_DCT || transform == DFFT_DST)
-        return fail(DFFT_ERR_UNSUPPORTED, spectral ? "padded plans are C2C or R2C / C2R" : "pruned plans are C2C or R2C / C2R");
-    if (transform != DFFT_C2C && transform != DFFT_R2C) return fail(DFFT_ERR_INVALID, "bad transform");
-    const size_t n[3] = {nx, ny, nz};
-    for (int a = 0; a < 3; ++a) {
-        if (sizes[a] == 0 || sizes[a] > n[a])
-            return fail(DFFT_ERR_INVALID, std::string(what) + " size " + std::to_string(sizes[a]) + " of axis " + "xyz"[a] + " must be in [1, " +
-                                              std::to_string(n[a]) + "]");
-        if (sizes[a] < n[a] && ilog2_exact(n[a]) < 0)
-            return fail(DFFT_ERR_UNSUPPORTED, std::string("axis ") + "xyz"[a] + " of length " + std::to_string(n[a]) + " is not a power of two: its " +
-                                                  what + " size must be its length");
-    }
-    return DFFT_SUCCESS;
+    return plan_create(comm, config, s, allocate, plan);
 }
 
 int dfft_plan_create_padded(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
                             size_t nz, size_t kx, size_t ky, size_t kz, size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan) {
-    const size_t k[3] = {kx, ky, kz};
-    if (is_half(precision)) return refuse_half("padded plans");
-    if (int rc = check_sub_grid(transform, nx, ny, nz, k, "spectral")) return rc;
-    return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, false, allocate, plan, nullptr, k);
+    PlanSpec s(F_PADDED, decomp, precision, transform, nx, ny, nz, p1, p2, batch);
+    s.k[0] = kx; s.k[1] = ky; s.k[2] = kz;
+    return plan_create(comm, config, s, allocate, plan);
 }
 
 // Pruned plans (DESIGN.md section 3.19): the data block [0, M) of each axis, zero beyond, and the spectrum of a padded plan.
 int dfft_plan_create_pruned(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
                             size_t nz, const size_t data[3], const size_t spectral[3], size_t p1, size_t p2, size_t batch, int allocate,
                             dfft_plan_t* plan) {
-    const size_t m[3] = {data ? data[0] : nx, data ? data[1] : ny, data ? data[2] : nz};
-    const size_t k[3] = {spectral ? spectral[0] : nx, spectral ? spectral[1] : ny, spectral ? spectral[2] : nz};
-    if (is_half(precision)) return refuse_half("pruned plans");
-    if (int rc = check_sub_grid(transform, nx, ny, nz, m, "data")) return rc;
-    if (int rc = check_sub_grid(transform, nx, ny, nz, k, "spectral")) return rc;
-    // the real side of R2C / C2R moves as pairs of reals (the z pass's complex units)
-    if (transform == DFFT_R2C && m[2] % 2) return fail(DFFT_ERR_UNSUPPORTED, "R2C / C2R pruned plans need an even data size along z");
-    return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, false, allocate, plan, nullptr, k, 1, nullptr,
-                       nullptr, m);
+    PlanSpec s(F_PRUNED, decomp, precision, transform, nx, ny, nz, p1, p2, batch);
+    for (int a = 0; a < 3; ++a) {
+        s.m[a] = data ? data[a] : s.n[a];
+        s.k[a] = spectral ? spectral[a] : s.n[a];
+    }
+    return plan_create(comm, config, s, allocate, plan);
 }
 
 int dfft_plan_get_data_size(dfft_plan_t p, size_t m[3]) {
@@ -3155,24 +3245,11 @@ int dfft_plan_get_data_size(dfft_plan_t p, size_t m[3]) {
     return DFFT_SUCCESS;
 }
 
-// C values per point: the C = 1 plan with every element widened to C consecutive values (DESIGN.md section 3.14).  The
-// z pass of C > 1 runs interleaved lines (PASS_C2C_ILV) or R2C / C2R lines of Nz points, one per component (PASS_R2C_ILV /
-// PASS_C2R_ILV), which exist for a power-of-two Nz (R2C: up to 8192).
-constexpr size_t MAX_COMPONENTS = 64;
 int dfft_plan_create_interleaved(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, int transform, size_t nx, size_t ny,
                                  size_t nz, size_t p1, size_t p2, size_t components, size_t batch, int allocate, dfft_plan_t* plan) {
-    if (is_half(precision)) return refuse_half("interleaved plans");
-    if (components == 0) return fail(DFFT_ERR_INVALID, "components must be at least 1");
-    if (components > MAX_COMPONENTS) return fail(DFFT_ERR_UNSUPPORTED, "at most " + std::to_string(MAX_COMPONENTS) + " components per point");
-    if (components > 1) {
-        if (transform != DFFT_C2C && transform != DFFT_R2C && !is_r2r(transform)) return fail(DFFT_ERR_INVALID, "bad transform");
-        if (is_r2r(transform)) return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans with more than one component are C2C or R2C / C2R");
-        if (ilog2_exact(nz) < 1) return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans need a power-of-two Nz (x and y may have any C2C length)");
-        // the interleaved R2C / C2R z pass runs Nz-point complex lines
-        if (transform == DFFT_R2C && ilog2_exact(nz) > MAX_LOG2N)
-            return fail(DFFT_ERR_UNSUPPORTED, "interleaved R2C / C2R plans need Nz <= " + std::to_string(1 << MAX_LOG2N));
-    }
-    return plan_create(comm, config, decomp, precision, transform, nx, ny, nz, p1, p2, batch, false, allocate, plan, nullptr, nullptr, components);
+    PlanSpec s(F_INTERLEAVED, decomp, precision, transform, nx, ny, nz, p1, p2, batch);
+    s.comps = components;
+    return plan_create(comm, config, s, allocate, plan);
 }
 size_t dfft_get_components(dfft_plan_t p) { return p ? p->comps : 0; }
 
@@ -3184,15 +3261,12 @@ int dfft_plan_get_spectral_size(dfft_plan_t p, size_t k[3]) {
 
 int dfft_plan_create_r2r(dfft_comm_t comm, const dfft_config* config, int decomp, int precision, const int kinds[3], size_t nx, size_t ny,
                          size_t nz, size_t p1, size_t p2, size_t batch, int inplace, int allocate, dfft_plan_t* plan) {
-    if (is_half(precision)) return refuse_half("real-to-real plans");
-    if (!kinds) return fail(DFFT_ERR_INVALID, "null kinds");
-    for (int a = 0; a < 3; ++a)
-        if (!is_r2r_kind(kinds[a]))
-            return fail(DFFT_ERR_INVALID, "kinds must be DFFT_DCT, DFFT_DST, DFFT_R2HC, DFFT_DCT1, DFFT_DST1, DFFT_DCT4 or DFFT_DST4");
     // three DCT (DST) axes make exactly the DCT (DST) plan; type-I and type-IV kinds, like R2HC, make a per-axis plan
-    const bool uniform = kinds[0] == kinds[1] && kinds[1] == kinds[2] && (kinds[0] == DFFT_DCT || kinds[0] == DFFT_DST);
-    return plan_create(comm, config, decomp, precision, uniform ? kinds[0] : DFFT_R2HC, nx, ny, nz, p1, p2, batch, inplace != 0, allocate, plan,
-                       kinds);
+    const bool uniform = kinds && kinds[0] == kinds[1] && kinds[1] == kinds[2] && (kinds[0] == DFFT_DCT || kinds[0] == DFFT_DST);
+    PlanSpec s(F_KINDS, decomp, precision, uniform ? kinds[0] : DFFT_R2HC, nx, ny, nz, p1, p2, batch);
+    s.kinds = kinds;
+    s.inplace = inplace != 0;
+    return plan_create(comm, config, s, allocate, plan);
 }
 
 int dfft_plan_get_r2r_kinds(dfft_plan_t p, int kinds[3]) {
@@ -3334,12 +3408,8 @@ int dfft_plan_set_transform_axes(dfft_plan_t p, const int transform[3]) {
     for (int a = 0; a < 3; ++a)
         if (transform[a] != 0 && transform[a] != 1) return fail(DFFT_ERR_INVALID, "transform axes must be 0 (keep) or 1 (transform)");
     if (p->g.transform == DFFT_R2C && !transform[2]) return fail(DFFT_ERR_INVALID, "R2C / C2R plans transform z (it turns reals into complex)");
-    if (p->g.padded() && !(transform[0] && transform[1] && transform[2]))
-        return fail(DFFT_ERR_UNSUPPORTED, "padded plans transform every axis");
-    if (p->g.pruned() && !(transform[0] && transform[1] && transform[2]))
-        return fail(DFFT_ERR_UNSUPPORTED, "pruned plans transform every axis");
-    if (p->comps > 1 && !(transform[0] && transform[1] && transform[2]))
-        return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans transform every axis");
+    if (!(transform[0] && transform[1] && transform[2]))
+        if (int rc = refuse(features(p), F_KEPT_AXES)) return rc;
     // schedules, tuned choices and captured graphs are built for the axes of their time
     if (p->axes_fixed) return fail(DFFT_ERR_STATE, "set the transform axes before the first exec, dfft_plan_tune or dfft_plan_describe");
     for (int a = 0; a < 3; ++a) p->taxes[a] = transform[a];
@@ -3352,7 +3422,7 @@ int dfft_plan_get_transform_axes(dfft_plan_t p, int transform[3]) {
 }
 int dfft_plan_set_strides(dfft_plan_t p, const long long in_strides[3], const long long out_strides[3]) {
     if (!p) return fail(DFFT_ERR_INVALID, "null plan");
-    if (is_half(p->prec)) return refuse_half("plans with strides");
+    if (int rc = refuse(features(p) & F_HALF, F_STRIDES)) return rc;  // 16-bit plans before the strides are looked at
     const char* const names[2] = {"in_strides", "out_strides"};
     const long long* const given[2] = {in_strides, out_strides};
     for (int side = 0; side < 2; ++side) {
@@ -3369,9 +3439,7 @@ int dfft_plan_set_strides(dfft_plan_t p, const long long in_strides[3], const lo
         if (side == 0 && p->g.transform == DFFT_R2C && ((s[0] | s[1] | s[2]) & 1))
             return fail(DFFT_ERR_INVALID, "in_strides: the real side of R2C / C2R moves pairs of reals, so its strides must be even");
     }
-    if (p->inplace) return fail(DFFT_ERR_UNSUPPORTED, "in-place plans keep the padded layout of FFTW and cuFFT: strides are for out-of-place plans");
-    if (p->comps > 1) return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans keep their [x][y][z][C] layout: strides are for plans of one component");
-    if (p->g.pruned()) return fail(DFFT_ERR_UNSUPPORTED, "pruned plans read and write dense data blocks: strides are for plans without a data size");
+    if (int rc = refuse(features(p), F_STRIDES)) return rc;
     if (p->axes_fixed) return fail(DFFT_ERR_STATE, "set the strides before the first exec, dfft_plan_tune or dfft_plan_describe");
     p->in_embedded = in_strides != nullptr;
     p->out_embedded = out_strides != nullptr;
@@ -3417,9 +3485,7 @@ int dfft_zy_trace_copy(dfft_plan_t p, int inverse, void* host, size_t bytes) {
 
 int dfft_plan_set_weights(dfft_plan_t p, const void* const weights[3]) {
     if (!p || !weights) return fail(DFFT_ERR_INVALID, "null plan / weights");
-    if (p->comps > 1) return fail(DFFT_ERR_UNSUPPORTED, "interleaved plans of more than one component have no spectral weights");
-    if (is_r2r(p->g.transform)) return fail(DFFT_ERR_UNSUPPORTED, "real-to-real plans (DCT / DST and per-axis kinds) have no spectral weights");
-    if (is_half(p->prec)) return refuse_half("spectral weights");
+    if (int rc = refuse(features(p), F_WEIGHTS)) return rc;
     for (int a = 0; a < 3; ++a)
         if ((uintptr_t)weights[a] % p->esize)
             return fail(DFFT_ERR_INVALID, std::string("weights[") + std::to_string(a) + "] must be aligned to its " + std::to_string(p->esize) + "-byte element");

@@ -189,69 +189,51 @@ class MPIcuFFT:
         if self._decomp == PENCIL and partition is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         h = C.c_void_p()
-        if data is not None:
-            if inplace or self.kinds is not None or components != 1 or in_boxes is not None or out_boxes is not None:
-                raise ValueError("pruned plans are out of place, C2C or R2C, with one component and no boxes")
-            if batch < 1:
-                raise ValueError("batch must be at least 1")
-            m = (C.c_size_t * 3)(*(int(v) for v in data))
-            k = None if spectral is None else (C.c_size_t * 3)(*(int(v) for v in spectral))
-            check(lib().dfft_plan_create_pruned(self.comm._h, C.byref(cfg), self._decomp, self.precision, self.transform, global_size.Nx,
-                                                global_size.Ny, global_size.Nz, m, k, p1, p2, batch, 1 if allocate else 0, C.byref(h)))
-        elif in_boxes is not None or out_boxes is not None:
-            if inplace or spectral is not None or components != 1 or self.kinds is not None:
-                raise ValueError("box plans are out of place, not padded, with one component and one transform kind for all axes")
-            if batch < 1:
-                raise ValueError("batch must be at least 1")
+        L, head, n = lib(), (self.comm._h, C.byref(cfg), self._decomp, self.precision), (global_size.Nx, global_size.Ny, global_size.Nz)
+        tail = (batch, 1 if allocate else 0, C.byref(h))
 
-            def flat(boxes):
-                if boxes is None:
-                    return None
-                boxes = list(boxes)
-                if len(boxes) != self.comm.size:
-                    raise ValueError(f"{len(boxes)} boxes for {self.comm.size} ranks")
-                vals = [int(v) for lo, hi in boxes for v in (*lo, *hi)]
-                if len(vals) != 6 * self.comm.size:
-                    raise ValueError("a box is ((lx, ly, lz), (hx, hy, hz))")
-                return (C.c_size_t * len(vals))(*vals)
-            check(lib().dfft_plan_create_boxes(self.comm._h, C.byref(cfg), self._decomp, self.precision, self.transform, global_size.Nx,
-                                               global_size.Ny, global_size.Nz, p1, p2, flat(in_boxes), flat(out_boxes), batch,
-                                               1 if allocate else 0, C.byref(h)))
-        elif components != 1:
-            if spectral is not None or inplace or self.kinds is not None:
-                raise ValueError("interleaved plans are out of place and not padded")
-            if batch < 1:
-                raise ValueError("batch must be at least 1")
-            check(lib().dfft_plan_create_interleaved(self.comm._h, C.byref(cfg), self._decomp, self.precision, self.transform,
-                                                     global_size.Nx, global_size.Ny, global_size.Nz, p1, p2, int(components), batch,
-                                                     1 if allocate else 0, C.byref(h)))
-        elif spectral is not None:
-            if inplace or self.kinds is not None:
-                raise ValueError("padded plans are out of place and C2C or R2C")
-            if batch < 1:
-                raise ValueError("batch must be at least 1")
-            kx, ky, kz = (int(k) for k in spectral)
-            check(lib().dfft_plan_create_padded(self.comm._h, C.byref(cfg), self._decomp, self.precision, self.transform, global_size.Nx,
-                                                global_size.Ny, global_size.Nz, kx, ky, kz, p1, p2, batch, 1 if allocate else 0, C.byref(h)))
-        elif self.kinds is not None:
-            if batch < 0:
-                raise ValueError("batch must be at least 1")
-            check(lib().dfft_plan_create_r2r(self.comm._h, C.byref(cfg), self._decomp, self.precision, (C.c_int * 3)(*self.kinds),
-                                             global_size.Nx, global_size.Ny, global_size.Nz, p1, p2, batch, 1 if inplace else 0,
-                                             1 if allocate else 0, C.byref(h)))
-        elif inplace:
-            if batch < 0:
-                raise ValueError("batch must be at least 1")
-            check(lib().dfft_plan_create_inplace(self.comm._h, C.byref(cfg), self._decomp, self.precision, self.transform, global_size.Nx,
-                                                 global_size.Ny, global_size.Nz, p1, p2, batch, 1 if allocate else 0, C.byref(h)))
-        elif batch == 1:
-            check(lib().dfft_plan_create(self.comm._h, C.byref(cfg), self._decomp, self.precision, self.transform,
-                                         global_size.Nx, global_size.Ny, global_size.Nz, p1, p2, 1 if allocate else 0, C.byref(h)))
-        else:
-            if batch < 0:
-                raise ValueError("batch must be at least 1")
-            check(lib().dfft_plan_create_batched(self.comm._h, C.byref(cfg), self._decomp, self.precision, self.transform, global_size.Nx,
-                                                 global_size.Ny, global_size.Nz, p1, p2, batch, 1 if allocate else 0, C.byref(h)))
+        def sizes(v):
+            return None if v is None else (C.c_size_t * 3)(*(int(k) for k in v))
+
+        def xyz(v):
+            x, y, z = (int(k) for k in v)
+            return x, y, z
+
+        def flat(boxes):
+            if boxes is None:
+                return None
+            boxes = list(boxes)
+            if len(boxes) != self.comm.size:
+                raise ValueError(f"{len(boxes)} boxes for {self.comm.size} ranks")
+            vals = [int(v) for lo, hi in boxes for v in (*lo, *hi)]
+            if len(vals) != 6 * self.comm.size:
+                raise ValueError("a box is ((lx, ly, lz), (hx, hy, hz))")
+            return (C.c_size_t * len(vals))(*vals)
+        # The creators, in the order they are chosen: (keyword, given, the other keywords it takes, why it refuses the rest,
+        # call).  The first one given makes the plan, and any other keyword given that it does not take raises ValueError
+        # before the library is called.
+        creators = (
+            ("data", data is not None, ("spectral",), "pruned plans are out of place, C2C or R2C, with one component and no boxes",
+             lambda: L.dfft_plan_create_pruned(*head, self.transform, *n, sizes(data), sizes(spectral), p1, p2, *tail)),
+            ("boxes", in_boxes is not None or out_boxes is not None, (),
+             "box plans are out of place, not padded, with one component and one transform kind for all axes",
+             lambda: L.dfft_plan_create_boxes(*head, self.transform, *n, p1, p2, flat(in_boxes), flat(out_boxes), *tail)),
+            ("components", components != 1, (), "interleaved plans are out of place and not padded",
+             lambda: L.dfft_plan_create_interleaved(*head, self.transform, *n, p1, p2, int(components), *tail)),
+            ("spectral", spectral is not None, (), "padded plans are out of place and C2C or R2C",
+             lambda: L.dfft_plan_create_padded(*head, self.transform, *n, *xyz(spectral), p1, p2, *tail)),
+            ("kinds", self.kinds is not None, ("inplace",), None,
+             lambda: L.dfft_plan_create_r2r(*head, (C.c_int * 3)(*self.kinds), *n, p1, p2, batch, 1 if inplace else 0, *tail[1:])),
+            ("inplace", bool(inplace), (), None, lambda: L.dfft_plan_create_inplace(*head, self.transform, *n, p1, p2, *tail)),
+            (None, True, (), None, lambda: L.dfft_plan_create(*head, self.transform, *n, p1, p2, *tail[1:]) if batch == 1 else
+             L.dfft_plan_create_batched(*head, self.transform, *n, p1, p2, *tail)),
+        )
+        keyword, _, takes, refusal, create = next(c for c in creators if c[1])
+        if any(c[0] not in (keyword, *takes) for c in creators[:-1] if c[1]):
+            raise ValueError(refusal)
+        if batch < 1:
+            raise ValueError("batch must be at least 1")
+        check(create())
         self._h = h
         self.global_size = global_size
         self.initialized = True

@@ -258,3 +258,8 @@ def test_python_binding_refusals():
     for kw in ({"inplace": True}, {"spectral": (4, 4, 4)}, {"batch": 0}):
         with pytest.raises(ValueError):
             p.initFFT(dfft.GlobalSize(8, 8, 8), None, True, components=3, **kw)
+    # batch 0 on the plain, in-place and per-axis-kind paths too
+    for kinds, kw in ((None, {}), (None, {"inplace": True}), ((dfft.DCT, dfft.R2HC, dfft.DCT), {})):
+        p.kinds = kinds
+        with pytest.raises(ValueError):
+            p.initFFT(dfft.GlobalSize(8, 8, 8), None, True, batch=0, **kw)
