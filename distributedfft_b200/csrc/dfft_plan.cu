@@ -90,6 +90,30 @@ static cudaError_t make_r2r4_table(int n, void** dev) {
     return cudaMemcpy(*dev, h.data(), h.size() * sizeof(cx<T>), cudaMemcpyHostToDevice);
 }
 
+// Twiddle table of 1D plans of N = 2^log2n points (FftPadded::tw1d, DESIGN.md section 3.22): one allocation
+// [W_N^l, l < 2^lo][W_N^(h 2^lo), h < N / 2^lo], lo = ceil(log2n / 2), about 2 sqrt(N) entries.  Each entry is evaluated in
+// long double from an exact integer numerator and rounded once; a pass multiplies one entry of each half, W_N^m =
+// W_N^(m_hi 2^lo) W_N^(m_lo), m = m_hi 2^lo + m_lo reduced mod N in 64-bit integers.
+static int tw1d_lo_bits(int log2n) { return (log2n + 1) / 2; }
+template <typename T>
+static cudaError_t make_tw1d_table(int log2n, void** dev) {
+    const int lo = tw1d_lo_bits(log2n);
+    const size_t nlo = size_t(1) << lo, nhi = size_t(1) << (log2n - lo);
+    std::vector<cx<T>> h(nlo + nhi);
+    const long double two_pi = 2.0L * 3.14159265358979323846264338327950288L;
+    for (size_t l = 0; l < nlo; ++l) {
+        const long double a = -two_pi * (long double)l / (long double)(1ull << log2n);
+        h[l] = cx<T>{T(cosl(a)), T(sinl(a))};
+    }
+    for (size_t k = 0; k < nhi; ++k) {
+        const long double a = -two_pi * (long double)k / (long double)nhi;
+        h[nlo + k] = cx<T>{T(cosl(a)), T(sinl(a))};
+    }
+    cudaError_t e = cudaMalloc(dev, h.size() * sizeof(cx<T>));
+    if (e != cudaSuccess) return e;
+    return cudaMemcpy(*dev, h.data(), h.size() * sizeof(cx<T>), cudaMemcpyHostToDevice);
+}
+
 // Bluestein table of n-point lines: one allocation [K^ (M entries)][chirp (n entries)] (bluestein.hpp)
 template <typename T>
 static cudaError_t make_bluestein_table(size_t n, void** dev) {
@@ -144,8 +168,15 @@ static bool r2r_kind_length(int kind, size_t n) {
 // then, with the physical hole on its loaded side forward and on its stored side inverse.
 // w: the spectral weights of the pass's axis (dfft_plan_set_weights), or null.  Weighted passes run the weighted twins:
 // of the padded kernels (with hole, empty where the plan keeps a whole side) or of the Bluestein kernel (WEIGHTED = true).
+// tw: the twiddle of a pass of a 1D plan (Twiddle1d), or null.  Twiddled passes run the twiddled twin of the padded C2C
+// kernel (TWIDDLED = true), with empty holes.
+struct Twiddle1d {
+    const void* table;              // make_tw1d_table of log2n
+    long long line0, c1, mul;       // FftPadded::tw_line0, tw_c1, tw_mul
+    int log2n;                      // N = 2^log2n, the signal's length
+};
 static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftParams& prm, const void* blu, double scale, cudaStream_t stream,
-                                   int r2r = DFFT_DCT, const int* hole = nullptr, const void* w = nullptr) {
+                                   int r2r = DFFT_DCT, const int* hole = nullptr, const void* w = nullptr, const Twiddle1d* tw = nullptr) {
     const int log2n = ilog2_exact(n);
     if (hole && log2n >= 0) {
         FftPadded q;
@@ -156,6 +187,12 @@ static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftP
         q.ld_lo = ld[0]; q.ld_hi = ld[1];
         q.st_lo = st[0]; q.st_hi = st[1];
         q.w = w;
+        q.tw1d = tw ? tw->table : nullptr;
+        q.tw_line0 = tw ? tw->line0 : 0;
+        q.tw_c1 = tw ? tw->c1 : 0;
+        q.tw_mul = tw ? tw->mul : 0;
+        q.tw_log2n = tw ? tw->log2n : 0;
+        q.tw_lo_bits = tw ? tw1d_lo_bits(tw->log2n) : 0;
         return launch_twin(prec, log2n, kind, q, stream);
     }
     if (kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED) {
@@ -219,6 +256,7 @@ struct Tables {
     std::map<int, void*> tw2;  // log2m -> exp(-2 pi i k / 2m), k <= m/2
     std::map<size_t, void*> blu;  // n -> Bluestein table of n-point lines
     std::map<int, void*> r2r4;    // log2 N -> type-IV table of N-point real lines (r2r4_table)
+    std::map<int, void*> tw1d;    // log2 N -> twiddle table of 1D plans of N points (make_tw1d_table)
     std::vector<void*> bytes;  // seg_of_n tables
     cudaError_t get_tw(int log2n, void** out) {
         if (dry) { *out = nullptr; return cudaSuccess; }
@@ -271,6 +309,18 @@ struct Tables {
         *out = it->second;
         return cudaSuccess;
     }
+    cudaError_t get_tw1d(int log2n, void** out) {
+        if (dry) { *out = nullptr; return cudaSuccess; }
+        auto it = tw1d.find(log2n);
+        if (it == tw1d.end()) {
+            void* d = nullptr;
+            cudaError_t e = prec == DFFT_F64 ? make_tw1d_table<double>(log2n, &d) : make_tw1d_table<float>(log2n, &d);
+            if (e != cudaSuccess) return e;
+            it = tw1d.emplace(log2n, d).first;
+        }
+        *out = it->second;
+        return cudaSuccess;
+    }
     cudaError_t seg_table(const Split& s, const unsigned char** out) {
         size_t n = s.start.back() + s.size.back();
         std::vector<unsigned char> h(n);
@@ -303,9 +353,10 @@ struct Tables {
         for (auto& kv : tw2) cudaFree(kv.second);
         for (auto& kv : blu) cudaFree(kv.second);
         for (auto& kv : r2r4) cudaFree(kv.second);
+        for (auto& kv : tw1d) cudaFree(kv.second);
         for (void* p : bytes) cudaFree(p);
         for (auto* v : dry_store) delete v;
-        tw.clear(); tw2.clear(); blu.clear(); r2r4.clear(); bytes.clear(); dry_store.clear(); host_tabs.clear();
+        tw.clear(); tw2.clear(); blu.clear(); r2r4.clear(); tw1d.clear(); bytes.clear(); dry_store.clear(); host_tabs.clear();
     }
 };
 
@@ -464,6 +515,10 @@ struct Step {
     // weighted plans (dfft_plan_set_weights): an FFT pass that multiplies its spectral side by the weights of its axis (the
     // plan's pointer for `axis` at exec time, none while it is null): forward its stores, inverse its loads
     bool weighted = false;
+    // 1D plans (dfft_plan_create_1d): the twiddled y or z pass ("y" / "z", null for none) and its twiddle; tw.table is
+    // null on geometry-only plans
+    const char* twiddle = nullptr;
+    Twiddle1d tw{};
 };
 
 struct Schedule {
@@ -518,6 +573,8 @@ struct dfft_plan_s {
     // marked weighted at every exec.  weighted: the first call came before any schedule was built.
     const void* weights[3] = {nullptr, nullptr, nullptr};
     bool weighted = false;
+    // dfft_plan_create_1d: the signal's length N = Nx * Ny * Nz (the factors are the grid), 0 for 3D plans
+    size_t n1d = 0;
     // dfft_plan_create_boxes: every rank's box of the physical grid (in_boxes) and of the output grid (out_boxes), in rank
     // order; empty where that side has the natural layout.  box_direct: their reshapes push and gather over peer memory
     // (comm_method Peer2Peer), otherwise they run through an NCCL all-to-all
@@ -674,8 +731,10 @@ static bool all_axes(const dfft_plan_s* p) { return p->taxes[0] && p->taxes[1] &
 // R2C / C2R passes over every axis.  Interleaved plans (C > 1 values per point): those kernels address one value per
 // point.  Plans with a box that is not the natural layout: their reshape steps wrap the sequential schedule (wrap_boxes).
 // Embedded plans (dfft_plan_set_strides): the other forms read and write dense caller arrays, and every rank must run the
-// same form.  The text completes dfft_plan_tune's report.
+// same form.  1D plans: their schedule (build_1d) has its own transpositions and twiddled passes.  The text completes
+// dfft_plan_tune's report.
 static const char* sequential_only(const dfft_plan_s* p) {
+    if (p->n1d) return "1D plans";
     if (is_half(p->prec)) return "16-bit plans";
     if (p->weighted) return "weighted plans";
     if (is_r2r(p->g.transform)) return "DCT / DST plans";
@@ -989,7 +1048,8 @@ using Origin = std::array<size_t, 3>;
 //   all-to-all: the same box with the sender's own extent along t, packed at soff[q] of slot SS, scount[q] elements;
 //     the receive side mirrors it at roff[q] of slot SR — one view when t is x, where the senders' blocks stack
 // The receiving pass transforms t (forward Z_Then_YX: y, with t = x outermost), so its input segments lie along its n axis.
-// `at` moves a view to a sub-box (the plane groups and z chunks of the overlapped schedules).
+// `at` moves a view to a sub-box (the plane groups and z chunks of the overlapped schedules).  slot: the slot a direct
+// transposition stores into, when not the group's own (D1 for group 1, D2 for group 2).
 struct Transposition {
     const dfft_plan_s* p;
     int group, s, t;
@@ -1003,11 +1063,12 @@ struct Transposition {
     Step a2a;     // the all-to-all step of one that is not
 
     Transposition(const dfft_plan_s* p_, int group_, int s_, int t_, const Split& ss_, const Split& st_, size_t u_,
-                  const unsigned char* tab_s_, const unsigned char* tab_t_)
+                  const unsigned char* tab_s_, const unsigned char* tab_t_, int slot = -1)
         : p(p_), group(group_), s(s_), t(t_), ss(&ss_), st(&st_), u(u_), whole(st_.start.back() + st_.size.back()), tab_s(tab_s_),
           tab_t(tab_t_), G(&p_->grp[group_]) {
         while ((*G)[pos] != p->rank) ++pos;
         D = group == 1 ? p->slots.D1 : p->slots.D2;
+        if (D >= 0 && slot >= 0) D = slot;
         direct = D >= 0;
         if (direct) return;
         a2a.type = STEP_A2A;
@@ -1378,6 +1439,113 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
     s1.prm.out = single_view(nullptr, zpitch_out * (long long)ny_j, zpitch_out, 1);
     s1.out_user = 2;
     sc.steps.push_back(s1);
+    return DFFT_SUCCESS;
+}
+
+// 1D plans (dfft_plan_create_1d, DESIGN.md section 3.22): the N-point signal as the slab grid [N1][N2][N3], each rank
+// holding an x-slab [nx_i][N2][N3] of it on both sides.  Forward:
+//   transpose  copy pass along y: my x-slab into every rank's y-slab [N1][oy_q][N3] (slot D1, or the all-to-all slots)
+//   x pass     gathers x, scatters it back to x-slabs (slot D2 or the all-to-all slots): the 3D inverse's x pass
+//   y pass     each point n2 of line (k1, n3) loaded times W_(N1 N2)^(n2 k1) = W_N^(n2 k1 N3), into slot D1
+//   z pass     each point n3 of line (k1, k2) loaded times W_N^(n3 (k1 + N1 k2)), into the caller's out
+// out[k1][k2][k3] = X[k1 + N1 k2 + N1 N2 k3], FFTW-MPI's scrambled order.  The inverse is the adjoint: the z and y passes
+// store times the conjugate twiddles, then the 3D forward's y -> x transposition and x pass, and the copy back to x-slabs.
+// On one rank the copy passes are not needed: the x pass reads the caller's in (forward) or writes its out (inverse).
+// Every slot is free when a peer stores into it: D1 (forward) was last read by the z pass of the previous exec, before
+// the entry rendezvous, and D2 by nobody; inverse, D1 was read by the y pass before the rendezvous of the y -> x
+// transposition.
+static int build_1d(dfft_plan_s* p, int inverse, Schedule& sc) {
+    const Geometry& g = p->g;
+    const int me = p->rank, P = p->P;
+    const size_t nx_i = g.sx.size[me], x0_i = g.sx.start[me], oy_i = g.oy.size[me], ny = g.ny, nz = g.nz;
+    Tables& T = p->tabs;
+    int rc;
+    const unsigned char *tab_y = nullptr, *tab_x = nullptr;
+    if (P > 1 && (T.seg_table(g.oy, &tab_y) != cudaSuccess || T.seg_table(g.sx, &tab_x) != cudaSuccess)) return fail(DFFT_ERR_CUDA, "segment table");
+    if (p->any_direct) sc.steps.push_back(new_rendezvous(0, 0, nullptr, 0));
+    // x-slabs -> y-slabs (the 3D forward's y -> x transposition) into slot D1, and back (the 3D inverse's x -> y one)
+    const Transposition to_y(p, 2, AY, AX, g.oy, g.sx, nz, tab_y, tab_x, inverse ? -1 : p->slots.D1);
+    const Transposition to_x(p, 2, AX, AY, g.sx, g.oy, nz, tab_x, tab_y, inverse ? p->slots.D1 : -1);
+    void* d1 = p->slot(p->slots.D1, me);
+    void* tw = nullptr;
+    if (T.get_tw1d(ilog2_exact(p->n1d), &tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
+    // the y and z passes over my x-slab [nx_i][N2][N3] in slot D1 and the caller's buffer, twiddled
+    auto twiddled = [&](int axis, Step& s) -> int {
+        rc = axis == 1 ? new_pass(p, inverse, PASS_C2C_TILED, ny, 1, nullptr, s) : new_pass(p, inverse, PASS_C2C_CONTIG, nz, 2, nullptr, s);
+        if (rc) return rc;
+        s.twiddle = axis == 1 ? "y" : "z";
+        s.tw = Twiddle1d{tw, (long long)x0_i, axis == 1 ? 0 : (long long)g.nx, axis == 1 ? (long long)nz : 1, ilog2_exact(p->n1d)};
+        if (axis == 1) {
+            s.label = "y pass";
+            s.prm.A0 = int(nx_i); s.prm.A1 = 1; s.prm.B = int(nz);
+            s.prm.in = s.prm.out = single_view(d1, (long long)(ny * nz), 0, (long long)nz);
+        } else {  // forward from slot D1 into the caller's out, inverse from the caller's in into slot D1
+            s.prm.A0 = int(nx_i); s.prm.A1 = int(ny);
+            s.prm.in = single_view(inverse ? nullptr : d1, (long long)(ny * nz), (long long)nz, 1);
+            s.prm.out = single_view(inverse ? d1 : nullptr, (long long)(ny * nz), (long long)nz, 1);
+            if (inverse) s.in_user = 1;
+            else s.out_user = 2;
+        }
+        return DFFT_SUCCESS;
+    };
+    // the copy pass between my x-slab on the caller's side and the y-slabs (one line per (x, z), n = y)
+    auto transpose = [&](const View& in, const View& out, Step& s) {
+        s = Step();
+        s.label = "transpose";
+        s.kind = PASS_COPY_TILED;
+        s.n = ny;
+        s.axis = 1;
+        s.prm.A0 = int(nx_i); s.prm.A1 = 1; s.prm.B = int(nz);
+        s.prm.inverse = inverse;
+        s.prm.in = in;
+        s.prm.out = out;
+    };
+    const View slab = single_view(nullptr, (long long)(ny * nz), 0, (long long)nz);
+    Step x, y, z, c;
+    rc = new_pass(p, inverse, PASS_C2C_TILED, g.nx, 0, "1D FFT X-Direction", x);
+    if (rc) return rc;
+    x.label = "x pass";
+    x.prm.A0 = 1; x.prm.A1 = 1; x.prm.B = int(oy_i * nz);
+    if ((rc = twiddled(1, y)) || (rc = twiddled(2, z))) return rc;
+    if (!inverse) {
+        if (P > 1) {
+            transpose(slab, to_y.send({AX, NO_AXIS, AY}), c);
+            c.in_user = 1;
+            sc.steps.push_back(c);
+            to_y.finish(sc);
+            x.prm.in = to_y.recv({NO_AXIS, NO_AXIS, AX});
+        } else {
+            x.prm.in = single_view(nullptr, 0, 0, (long long)(ny * nz));
+            x.in_user = 1;
+        }
+        x.prm.out = to_x.send({NO_AXIS, NO_AXIS, AX});
+        sc.steps.push_back(x);
+        to_x.finish(sc);
+        y.prm.in = to_x.recv({AX, NO_AXIS, AY});
+        z.phase = "2D FFT Y-Z-Direction";
+        sc.steps.push_back(y);
+        sc.steps.push_back(z);
+        return DFFT_SUCCESS;
+    }
+    z.phase = nullptr;
+    sc.steps.push_back(z);
+    y.prm.out = to_y.send({AX, NO_AXIS, AY});
+    y.phase = "2D FFT Y-Z-Direction";
+    sc.steps.push_back(y);
+    to_y.finish(sc);
+    x.prm.in = to_y.recv({NO_AXIS, NO_AXIS, AX});
+    if (P > 1) {
+        x.prm.out = to_x.send({NO_AXIS, NO_AXIS, AX});
+        sc.steps.push_back(x);
+        to_x.finish(sc);
+        transpose(to_x.recv({AX, NO_AXIS, AY}), slab, c);
+        c.out_user = 2;
+        sc.steps.push_back(c);
+    } else {
+        x.prm.out = single_view(nullptr, 0, 0, (long long)(ny * nz));
+        x.out_user = 2;
+        sc.steps.push_back(x);
+    }
     return DFFT_SUCCESS;
 }
 
@@ -1961,7 +2129,8 @@ static cudaError_t run_pass_step(const dfft_plan_s* p, const Schedule& sc, const
                 int hole[4];
                 pass_hole(s.kind, n, s.keep, s.data, hole);
                 const void* w = s.weighted ? p->weights[s.axis] : nullptr;  // null: the unweighted kernel
-                e = launch_fft_pass(p->prec, s.kind, n, prm, s.blu, scale, ss, s.r2r, s.keep || s.data || w ? hole : nullptr, w);
+                e = launch_fft_pass(p->prec, s.kind, n, prm, s.blu, scale, ss, s.r2r, s.keep || s.data || w || s.twiddle ? hole : nullptr, w,
+                                    s.twiddle ? &s.tw : nullptr);
             }
             break;
         case KERNEL_ZY_FUSED: e = launch_zy_fused(p->prec, s.log2n, prm, prm_y, s.zyf, scale, ss); break;
@@ -2283,9 +2452,10 @@ static int widen_views(dfft_plan_s* p, Schedule& sc) {
 }
 
 // This rank's block of layout `which` (0 input, 1 and 2 after z and y, 3 output) as the caller holds it: its box on a boxed
-// side of a box plan (the physical side of every d, the output of d = 3), the plan's own layout otherwise
+// side of a box plan (the physical side of every d, the output of d = 3), the plan's own layout otherwise.  1D plans hold
+// the x-slab of the input layout on both sides.
 static void caller_block(const dfft_plan_s* p, int which, size_t s[3], size_t o[3]) {
-    p->g.layout(p->rank, which, s, o);
+    p->g.layout(p->rank, p->n1d ? 0 : which, s, o);
     const std::vector<Box>& boxes = which == 0 ? p->in_boxes : p->out_boxes;
     if ((which == 0 || which == 3) && !boxes.empty())
         for (int k = 0; k < 3; ++k) { s[k] = boxes[size_t(p->rank)].extent(k); o[k] = boxes[size_t(p->rank)].lo[k]; }
@@ -2535,6 +2705,7 @@ static int embed_views(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
 // The one place that decides which schedule a (direction, d) pair runs — used by exec and by dfft_plan_describe, so
 // the CPU schedule emulation always validates exactly what executes.
 static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
+    if (p->n1d && d != 3) return fail(DFFT_ERR_UNSUPPORTED, "1D plans run the whole transform (d = 3)");
     Schedule& sc = p->sched[inverse ? 1 : 0][d - 1];
     p->axes_fixed = true;
     if (!sc.built) {
@@ -2554,7 +2725,8 @@ static int get_schedule(dfft_plan_s* p, int inverse, int d, Schedule** out) {
         // one rank with x kept: the layout after d = 2 is the output layout, so d = 3 runs the d = 2 steps (no x copy)
         const int db = p->P == 1 && !p->taxes[0] && d == 3 ? 2 : d;
         int rc;
-        if (batch_small(p, d)) rc = build_batch_small(p, inverse ? 1 : 0, sc);
+        if (p->n1d) rc = build_1d(p, inverse ? 1 : 0, sc);
+        else if (batch_small(p, d)) rc = build_batch_small(p, inverse ? 1 : 0, sc);
         // the overlapped slab and pencil schedules share their forward builder; their inverses run different pipelines
         else if ((want_overlap || want_pencil_overlap) && !inverse) rc = build_overlapped_forward(p, sc);
         else if (want_overlap) rc = build_overlapped_slab_inverse(p, sc);
@@ -2834,6 +3006,7 @@ enum Feature : unsigned {
     F_KEPT_AXES = 1u << 8,    // dfft_plan_set_transform_axes with an axis kept
     F_STRIDES = 1u << 9,      // dfft_plan_set_strides
     F_WEIGHTS = 1u << 10,     // dfft_plan_set_weights
+    F_1D = 1u << 11,          // dfft_plan_create_1d
 };
 
 // The features that do not combine, in the order they are refused: adding `adds` to a description or a plan that has
@@ -2856,6 +3029,10 @@ static const Refusal refusals[] = {
     {F_WEIGHTS, F_INTERLEAVED, "interleaved plans of more than one component have no spectral weights"},
     {F_WEIGHTS, F_R2R, "real-to-real plans (DCT / DST and per-axis kinds) have no spectral weights"},
     {F_WEIGHTS, F_HALF, "spectral weights"},
+    {F_1D, F_HALF, "1D plans"},
+    {F_KEPT_AXES, F_1D, "1D plans transform every axis of their grid"},
+    {F_STRIDES, F_1D, "1D plans read and write dense chunks of the signal: strides are for 3D plans"},
+    {F_WEIGHTS, F_1D, "1D plans have no spectral weights"},
 };
 // The first refusal of adding `adds` to a description or a plan with the features `has`, or DFFT_SUCCESS
 static int refuse(unsigned has, unsigned adds) {
@@ -2866,7 +3043,7 @@ static int refuse(unsigned has, unsigned adds) {
 }
 static unsigned features(const dfft_plan_s* p) {
     return (is_half(p->prec) ? F_HALF : 0) | (is_r2r(p->g.transform) ? F_R2R : 0) | (p->inplace ? F_INPLACE : 0) | (p->g.padded() ? F_PADDED : 0) |
-           (p->g.pruned() ? F_PRUNED : 0) | (p->comps > 1 ? F_INTERLEAVED : 0);
+           (p->g.pruned() ? F_PRUNED : 0) | (p->comps > 1 ? F_INTERLEAVED : 0) | (p->n1d ? F_1D : 0);
 }
 
 // bytes of one element: complex, or real for DCT / DST plans
@@ -2876,7 +3053,7 @@ static size_t elem_bytes(int precision, int transform) {
 
 // The description of a plan: what one dfft_plan_create* entry point asks for.  Each creator sets the fields of its feature.
 struct PlanSpec {
-    unsigned made_by;  // F_BOXES, F_PADDED, F_PRUNED, F_INTERLEAVED or F_KINDS; 0 for dfft_plan_create_batched / _inplace
+    unsigned made_by;  // F_BOXES, F_PADDED, F_PRUNED, F_INTERLEAVED, F_KINDS or F_1D; 0 for dfft_plan_create_batched / _inplace
     int decomp, precision, transform;
     size_t n[3], p1, p2, batch;
     bool inplace = false;
@@ -2884,6 +3061,7 @@ struct PlanSpec {
     size_t comps = 1;                           // values per grid point
     size_t k[3] = {0, 0, 0}, m[3] = {0, 0, 0};  // the spectral and data sizes; 0: the grid
     std::vector<Box> boxes[2];                  // the in and out box of every rank; empty: that side has its natural layout
+    size_t signal = 0;                          // dfft_plan_create_1d: N, with n the factors N1, N2, N3 (0 where none was found)
     PlanSpec(unsigned made_by_, int decomp_, int precision_, int transform_, size_t nx, size_t ny, size_t nz, size_t p1_, size_t p2_, size_t batch_)
         : made_by(made_by_), decomp(decomp_), precision(precision_), transform(transform_), n{nx, ny, nz}, p1(p1_), p2(p2_), batch(batch_) {}
     unsigned features() const { return made_by | (is_half(precision) ? F_HALF : 0) | (is_r2r(transform) ? F_R2R : 0) | (inplace ? F_INPLACE : 0); }
@@ -2948,6 +3126,19 @@ static int check_spec(dfft_comm_t comm, const dfft_plan_t* plan, const PlanSpec&
             if (s.transform == DFFT_R2C && ilog2_exact(n[2]) > MAX_LOG2N)
                 return fail(DFFT_ERR_UNSUPPORTED, "interleaved R2C / C2R plans need Nz <= " + std::to_string(1 << MAX_LOG2N));
         }
+    } else if (s.made_by == F_1D) {  // DESIGN.md section 3.22
+        if (!comm || !plan) return fail(DFFT_ERR_INVALID, "null comm / plan");
+        const int l = ilog2_exact(s.signal);
+        if (l < 3 || l > 3 * MAX_LOG2N)
+            return fail(DFFT_ERR_UNSUPPORTED, "1D plans take n a power of two in [8, 2^" + std::to_string(3 * MAX_LOG2N) + "]");
+        if (n[0] == 0)
+            return fail(DFFT_ERR_UNSUPPORTED, "n = " + std::to_string(s.signal) + " has no split into three powers of two in [2, 8192] with N1 " +
+                                                  "and N2 at least the rank count");
+        if (!pow2_length(n[0]) || !pow2_length(n[1]) || !pow2_length(n[2]))
+            return fail(DFFT_ERR_UNSUPPORTED, "the factors of a 1D plan must be powers of two in [2, 8192]");
+        if (n[0] * n[1] * n[2] != s.signal) return fail(DFFT_ERR_INVALID, "the factors of a 1D plan must multiply to n");
+        if (n[0] < size_t(comm->nranks) || n[1] < size_t(comm->nranks))
+            return fail(DFFT_ERR_INVALID, "the factors N1 and N2 of a 1D plan must be at least the rank count, so that every rank holds data");
     } else if (s.made_by == F_KINDS) {
         if (!s.kinds) return fail(DFFT_ERR_INVALID, "null kinds");
         for (int a = 0; a < 3; ++a)
@@ -3030,6 +3221,7 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, const PlanSp
     const Geometry& g = p->g;
     p->inplace = inplace;
     p->batch = s.batch;
+    p->n1d = s.signal;
     // box plans: a side whose boxes are all natural keeps no boxes, so that it makes exactly the plan of
     // dfft_plan_create_batched
     auto keep_boxes = [&](const std::vector<Box>& b, int which, std::vector<Box>& dst) {
@@ -3273,6 +3465,42 @@ int dfft_plan_get_r2r_kinds(dfft_plan_t p, int kinds[3]) {
     if (!p || !kinds) return fail(DFFT_ERR_INVALID, "null plan / kinds");
     if (!is_r2r(p->g.transform)) return fail(DFFT_ERR_INVALID, std::string("plan was created for ") + transform_name(p->g.transform));
     for (int a = 0; a < 3; ++a) kinds[a] = p->kinds[a];
+    return DFFT_SUCCESS;
+}
+
+// 1D plans (DESIGN.md section 3.22).  Default factors: log2 N split into l1 + l2 + l3 with every l in [1, 13] and l1, l2
+// at least ceil(log2 P) (N1, N2 >= P: no rank without data), the split with the smallest spread max(l) - min(l), and of
+// those the largest l1, then the largest l2 (so N1 >= N2 >= N3 when nothing else decides).  All zero when none exists.
+static void default_factors(size_t n, int P, size_t f[3]) {
+    f[0] = f[1] = f[2] = 0;
+    const int L = ilog2_exact(n);
+    int lp = 1;
+    while ((1 << lp) < P) ++lp;
+    int best = -1;
+    for (int l1 = MAX_LOG2N; l1 >= lp; --l1)
+        for (int l2 = MAX_LOG2N; l2 >= lp; --l2) {
+            const int l3 = L - l1 - l2;
+            if (L < 0 || l3 < 1 || l3 > MAX_LOG2N) continue;
+            const int spread = std::max({l1, l2, l3}) - std::min({l1, l2, l3});
+            if (best >= 0 && spread >= best) continue;
+            best = spread;
+            f[0] = size_t(1) << l1; f[1] = size_t(1) << l2; f[2] = size_t(1) << l3;
+        }
+}
+
+int dfft_plan_create_1d(dfft_comm_t comm, const dfft_config* config, int precision, size_t n, const size_t factors[3], dfft_plan_t* plan) {
+    size_t f[3] = {0, 0, 0};
+    if (factors) for (int a = 0; a < 3; ++a) f[a] = factors[a];
+    else default_factors(n, comm ? comm->nranks : 1, f);
+    PlanSpec s(F_1D, DFFT_SLAB_ZY_THEN_X, precision, DFFT_C2C, f[0], f[1], f[2], comm ? size_t(comm->nranks) : 1, 1, 1);
+    s.signal = n;
+    return plan_create(comm, config, s, 1, plan);
+}
+
+int dfft_plan_get_1d_factors(dfft_plan_t p, size_t f[3]) {
+    if (!p || !f) return fail(DFFT_ERR_INVALID, "null plan / factors");
+    if (!p->n1d) return fail(DFFT_ERR_INVALID, "not a 1D plan (dfft_plan_create_1d)");
+    f[0] = p->g.nx; f[1] = p->g.ny; f[2] = p->g.nz;
     return DFFT_SUCCESS;
 }
 
@@ -3783,6 +4011,7 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
                     (p->g.pruned() ? ",\"data\":[" + std::to_string(p->g.mx) + "," + std::to_string(p->g.my) + "," + std::to_string(p->g.mz) + "]"
                                    : std::string()) +
                     (p->comps > 1 ? ",\"components\":" + std::to_string(p->comps) : std::string()) +
+                    (p->n1d ? ",\"signal\":" + std::to_string(p->n1d) : std::string()) +
                     (p->weighted ? ",\"weights\":[" + std::to_string(p->weights[0] ? 1 : 0) + "," + std::to_string(p->weights[1] ? 1 : 0) + "," +
                                        std::to_string(p->weights[2] ? 1 : 0) + "]"
                                  : std::string()) +
@@ -3900,6 +4129,9 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
                  (s_.bluestein() || copy ? ",\"n\":" + std::to_string(s_.n) : std::string()) +
                  (s_.keep ? ",\"keep\":" + std::to_string(s_.keep) : std::string()) +
                  (s_.data ? ",\"data\":" + std::to_string(s_.data) : std::string()) + (s_.weighted ? ",\"weighted\":1,\"axis\":" + std::to_string(s_.axis) : std::string()) +
+                 (s_.twiddle ? std::string(",\"twiddle\":\"") + s_.twiddle + "\",\"tw\":[" + std::to_string(s_.tw.line0) + "," +
+                                   std::to_string(s_.tw.c1) + "," + std::to_string(s_.tw.mul) + "]"
+                             : std::string()) +
                  ",\"A0\":" + std::to_string(s_.prm.A0) +
                  ",\"A1\":" + std::to_string(s_.prm.A1) + ",\"B\":" + std::to_string(s_.prm.B) + ",\"inverse\":" + std::to_string(s_.prm.inverse) +
                  ",\"in_user\":" + std::to_string(s_.in_user) + ",\"out_user\":" + std::to_string(s_.out_user) + ",\"in\":";
@@ -4067,6 +4299,8 @@ int dfft_debug_run_step(dfft_plan_t p, int inverse, int d, size_t field, int ste
         s.prm.tw = tw;
         s.prm.tw2 = tw2;
         s.blu = blu;
+        if (s.twiddle && fft1d_tables(p->prec).get_tw1d(s.tw.log2n, const_cast<void**>(&s.tw.table)) != cudaSuccess)
+            return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
     }
     // the views as the kernel sees them: slot addresses on the work areas, the caller's on in / out; each segment's range
     struct Range { const char *lo, *hi, *buf; size_t bytes; };

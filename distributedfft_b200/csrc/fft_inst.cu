@@ -247,8 +247,8 @@ template cudaError_t launch_pass<float, cx16<DFFT_S>, DFFT_LOG2N>(PassKind, cons
 template cudaError_t launch_pass<DFFT_T, cx<DFFT_T>, DFFT_LOG2N>(PassKind, const FftParams&, double, cudaStream_t);
 
 // the padded twins (fft_c2c_padded_kernel, fft_r2c_padded_kernel, fft_c2r_padded_kernel), their weighted instantiations
-// (WEIGHTED = true) where p.w is set: the tiles of launch_pass (TILED: narrow or wide by wide_tile, without the TMA-fed
-// kernel), one CTA per tile
+// (WEIGHTED = true) where p.w is set, and the twiddled C2C passes of 1D plans (TWIDDLED = true) where p.tw1d is set: the tiles
+// of launch_pass (TILED: narrow or wide by wide_tile, without the TMA-fed kernel), one CTA per tile
 template <typename T, int LOG2N>
 cudaError_t launch_twin(PassKind kind, const FftPadded& p, cudaStream_t stream) {
     using S = Shape<T, LOG2N>;
@@ -262,8 +262,8 @@ cudaError_t launch_twin(PassKind kind, const FftPadded& p, cudaStream_t stream) 
     // the R2C / C2R twins test k < lo only: their holes reach the end of the line
     if (half && (p.ld_hi != n_ld || p.st_hi != n_st)) return cudaErrorInvalidValue;
     const long long grid = (lines + S::TBC - 1) / S::TBC;  // CONTIG, R2C and C2R
-    const auto launch = [&](auto weighted) -> cudaError_t {
-        constexpr bool W = decltype(weighted)::value;
+    const auto launch = [&](auto weighted, auto twiddled) -> cudaError_t {
+        constexpr bool W = decltype(weighted)::value, TW = decltype(twiddled)::value;
         using C = CtaFft<T, LOG2N, LOG2E, S::TBC, false>;
         // TILED, tiles TB columns wide
         const auto tiled = [&](auto tb) -> cudaError_t {
@@ -273,21 +273,22 @@ cudaError_t launch_twin(PassKind kind, const FftPadded& p, cudaStream_t stream) 
             q.tile_swz = tile_swz_for(p.tile_swz, p.A0, p.A1);
             const long long g = lines * ((p.B + TB - 1) / TB);
             if (g > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-            return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, LOG2E, TB, true, false, W>, fft_c2c_padded_kernel<T, LOG2N, LOG2E, TB, true, true, W>, nullptr,
-                                 nullptr>(q, 1.0, unsigned(g), CT::THREADS, CT::SMEM_BYTES, stream);
+            return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, LOG2E, TB, true, false, W, TW>, fft_c2c_padded_kernel<T, LOG2N, LOG2E, TB, true, true, W, TW>,
+                                 nullptr, nullptr>(q, 1.0, unsigned(g), CT::THREADS, CT::SMEM_BYTES, stream);
         };
         switch (kind) {
             case PASS_C2C_CONTIG:
                 if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
                 if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-                return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, false, false, W>, fft_c2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, false, true, W>,
-                                     nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
+                return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, false, false, W, TW>,
+                                     fft_c2c_padded_kernel<T, LOG2N, LOG2E, S::TBC, false, true, W, TW>, nullptr, nullptr>(p, 1.0, unsigned(grid), C::THREADS, C::SMEM_BYTES, stream);
             case PASS_C2C_TILED:
                 if (p.B <= 0) return cudaSuccess;
                 if (wide_tile<T, LOG2N>(p, sizeof(cx<T>), false)) return tiled(std::integral_constant<int, S::TBT_WIDE>());
                 return tiled(std::integral_constant<int, S::TBT>());
             case PASS_R2C:
             case PASS_C2R: {
+                if constexpr (TW) return cudaErrorInvalidValue;  // 1D plans are C2C
                 if ((kind == PASS_R2C ? p.in.nseg : p.out.nseg) != 1 || p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;
                 if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
                 if (kind == PASS_R2C) {
@@ -300,8 +301,10 @@ cudaError_t launch_twin(PassKind kind, const FftPadded& p, cudaStream_t stream) 
             default: return cudaErrorInvalidValue;
         }
     };
-    if (p.w) return launch(std::true_type());
-    return launch(std::false_type());
+    if (p.tw1d && p.w) return cudaErrorInvalidValue;  // 1D plans have no spectral weights
+    if (p.tw1d) return launch(std::false_type(), std::true_type());
+    if (p.w) return launch(std::true_type(), std::false_type());
+    return launch(std::false_type(), std::false_type());
 }
 
 template cudaError_t launch_twin<DFFT_T, DFFT_LOG2N>(PassKind, const FftPadded&, cudaStream_t);

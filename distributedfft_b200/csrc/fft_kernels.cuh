@@ -441,9 +441,25 @@ struct FftPadded : FftScaled {
     int ld_lo, ld_hi;  // of the loaded side
     int st_lo, st_hi;  // of the stored side
     const void* w;     // weighted passes: cx<T>[spectral points of the line], Kx, Ky, Kz (C2C) or Kz/2 + 1 (R2C / C2R); else null
+    // Twiddled passes of 1D plans (dfft_plan_create_1d, TWIDDLED; DESIGN.md section 3.22): point n of line (a0, a1) is
+    // multiplied by W_N^(n * (line0 + a0 + c1 * a1) * mul mod N), W_N = exp(-2 pi i / N), N = 2^log2n: forward as it is
+    // loaded, inverse by the conjugate as it is stored.  tw1d: the two-level table of W_N (tw1d_at); else null.
+    const void* tw1d;
+    long long tw_line0, tw_c1, tw_mul;
+    int tw_log2n, tw_lo_bits;
 };
 // index in the view of line position n, -1 in the hole
 __device__ __forceinline__ int keep_index(int n, int lo, int hi) { return n < lo ? n : (n < hi ? -1 : n - (hi - lo)); }
+
+// W_N^m of a twiddled pass, m reduced mod N = 2^tw_log2n: from the table [W_N^l, l < 2^lo_bits][W_N^(h 2^lo_bits), h < N / 2^lo_bits]
+// (built in long double and rounded once), W_N^m = W_N^(m_hi 2^lo_bits) * W_N^(m_lo)
+template <typename T>
+__device__ __forceinline__ cx<T> tw1d_at(const FftPadded& p, unsigned long long m) {
+    const cx<T>* t = reinterpret_cast<const cx<T>*>(p.tw1d);
+    m &= (1ull << p.tw_log2n) - 1;
+    const unsigned long long lo = m & ((1ull << p.tw_lo_bits) - 1), hi = m >> p.tw_lo_bits;
+    return cmul(t[(size_t(1) << p.tw_lo_bits) + hi], t[lo]);
+}
 
 // store policy of the padded twins: plain stores, scaled when s != 1 (a runtime value)
 template <typename T>
@@ -463,11 +479,13 @@ __device__ __forceinline__ void l2_discard(const void* p) { asm volatile("discar
 // ILV (CONTIG mapping): lines of an interleaved z pass, strided by sN along n (TileCoord)
 // WEIGHTED: the spectral side's values times w[m] (FftPadded::w), m their index in its view: inverse after the load,
 // forward before the store
+// TWIDDLED (tp: the FftPadded of a 1D plan's pass): point n of the line times W_N^(n * line index * mul) (tw1d_at):
+// forward after the load, inverse its conjugate before the store
 template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, typename M, typename Hook = NoGatherHook, bool PADDED = false,
-          bool ILV = false, bool WEIGHTED = false>
+          bool ILV = false, bool WEIGHTED = false, bool TWIDDLED = false>
 __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<T>* sm, unsigned long long* tab_in, unsigned long long* tab_out,
                                          bool multi, const M& mem, const Hook& after_gather = {}, int ld_lo = 0, int ld_hi = 0, int st_lo = 0,
-                                         int st_hi = 0, const cx<T>* w = nullptr) {
+                                         int st_hi = 0, const cx<T>* w = nullptr, const FftPadded* tp = nullptr) {
     using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
     using S = typename StoredOf<T, M>::type;
     using LA = LineAccess<T, C::LINES, S>;
@@ -520,6 +538,11 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
                 if (m >= 0) v[e] = cmul(v[e], ld_tw(w, m));
             }
         }
+        if constexpr (TWIDDLED && !INV) {
+            const unsigned long long step = ((unsigned long long)(tp->tw_line0 + tc.a0) + (unsigned long long)tp->tw_c1 * tc.a1) * (unsigned long long)tp->tw_mul;
+#pragma unroll
+            for (int e = 0; e < E; ++e) v[e] = cmul(v[e], tw1d_at<T>(*tp, (unsigned long long)(j + e * TPL) * step));
+        }
         if constexpr (INV) {
 #pragma unroll
             for (int e = 0; e < E; ++e) v[e] = cswap(v[e]);
@@ -538,6 +561,17 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
                 const int m = PADDED && st_lo < st_hi ? keep_index(j + e * TPL, st_lo, st_hi) : j + e * TPL;
                 cx<T>& x = v[C::Core::final_slot(e)];
                 if (m >= 0) x = cmul(x, ld_tw(w, m));
+            }
+        }
+    }
+    if constexpr (TWIDDLED && INV) {
+        // v holds the swapped values (cswap(z) = i conj(z)): multiplying them by W stores conj(W) times the result
+        if (tc.valid) {
+            const unsigned long long step = ((unsigned long long)(tp->tw_line0 + tc.a0) + (unsigned long long)tp->tw_c1 * tc.a1) * (unsigned long long)tp->tw_mul;
+#pragma unroll
+            for (int e = 0; e < E; ++e) {
+                cx<T>& x = v[C::Core::final_slot(e)];
+                x = cmul(x, tw1d_at<T>(*tp, (unsigned long long)(j + e * TPL) * step));
             }
         }
     }
@@ -734,8 +768,9 @@ fft_rc_ilv_kernel(const __grid_constant__ KParams<SCALED> p) {
     }
 }
 
-// padded twin of fft_c2c_kernel (FftPadded), and with WEIGHTED its weighted twin (p.w): one CTA per tile
-template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, bool WEIGHTED>
+// padded twin of fft_c2c_kernel (FftPadded), with WEIGHTED its weighted twin (p.w), with TWIDDLED the twiddled pass of
+// 1D plans (p.tw1d): one CTA per tile
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, bool WEIGHTED, bool TWIDDLED = false>
 __global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
 fft_c2c_padded_kernel(const __grid_constant__ FftPadded p) {
     using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
@@ -744,9 +779,9 @@ fft_c2c_padded_kernel(const __grid_constant__ FftPadded p) {
     unsigned long long* tab_in = reinterpret_cast<unsigned long long*>(smem_raw + C::TILE_BYTES);
     unsigned long long* tab_out = tab_in + C::LINES * MAXSEG;
     const bool multi = p.in.nseg > 1 || p.out.nseg > 1;
-    c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV, MemRtScaled<T>, NoGatherHook, true, false, WEIGHTED>(
+    c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV, MemRtScaled<T>, NoGatherHook, true, false, WEIGHTED, TWIDDLED>(
         p, blockIdx.x, sm, tab_in, tab_out, multi, MemRtScaled<T>{p.scale != 1.0, T(p.scale)}, {}, p.ld_lo, p.ld_hi, p.st_lo, p.st_hi,
-        WEIGHTED ? reinterpret_cast<const cx<T>*>(p.w) : nullptr);
+        WEIGHTED ? reinterpret_cast<const cx<T>*>(p.w) : nullptr, TWIDDLED ? &p : nullptr);
 }
 
 // ---- mbarrier of an asynchronous tile copy (fft_c2c_tma_kernel, fft_zy_fused_kernel) ------------------------------

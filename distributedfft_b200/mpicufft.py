@@ -154,7 +154,8 @@ class MPIcuFFT:
     # -- plan ------------------------------------------------------------------------------------
     def initFFT(self, global_size: GlobalSize, partition: Optional[Partition] = None, allocate: bool = True, batch: int = 1,
                 inplace: bool = False, transform_axes: Optional[Sequence[bool]] = None, spectral: Optional[Sequence[int]] = None,
-                components: int = 1, in_boxes=None, out_boxes=None, in_strides=None, out_strides=None, data: Optional[Sequence[int]] = None):
+                components: int = 1, in_boxes=None, out_boxes=None, in_strides=None, out_strides=None, data: Optional[Sequence[int]] = None,
+                signal: Optional[int] = None, factors: Optional[Sequence[int]] = None):
         """`batch` (not in the reference): every exec transforms that many fields, back to back in each buffer — a
         contiguous [batch, X, Y, Z] tensor; the getters describe one field (dfft_plan_create_batched).
         `inplace` (dfft_plan_create_inplace): every exec gets the same buffer twice and overwrites its input; fields are
@@ -177,8 +178,22 @@ class MPIcuFFT:
         `data` (mx, my, mz) (dfft_plan_create_pruned): a pruned plan, global_size the transform grid and the field an
         [mx, my, mz] block at the origin, zero beyond — the forward reads only the block, the inverse stores only it (the
         doubled grid of free-space solvers).  The physical side of every exec is this rank's m-block; combines with
-        `spectral`.  Pruned plans are out of place, C2C or R2C, with one component and no boxes or strides."""
-        if global_size is None:
+        `spectral`.  Pruned plans are out of place, C2C or R2C, with one component and no boxes or strides.
+        `signal` n (dfft_plan_create_1d, MPIcuFFT_Slab only): a distributed 1D C2C transform of one n-point signal, seen as
+        the grid (N1, N2, N3) = `factors` (None: the library's balanced choice, getFactors()) with global_size None.  Each
+        rank's buffers are its x-slab [in_size[0], N2, N3] of that grid on both sides, the forward output in scrambled order
+        (frequency k at [k % N1][(k // N1) % N2][k // (N1 N2)]); 1D plans are C2C, out of place, batch 1, without
+        partition, strides or kept axes."""
+        if signal is not None:
+            if self._decomp != SLAB_ZY_THEN_X:
+                raise ValueError("1D plans are slab plans (MPIcuFFT_Slab)")
+            if self.transform != C2C or global_size is not None or partition is not None or batch != 1 or not allocate or \
+                    transform_axes is not None or in_strides is not None or out_strides is not None:
+                raise ValueError("1D plans are C2C, out of place and allocated, batch 1, with no global_size, partition, strides or "
+                                 "transform_axes")
+        elif factors is not None:
+            raise ValueError("factors belong to a 1D plan (signal=n)")
+        elif global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         cfg = _lib.dfft_config(int(self.config.cuda_aware), int(self.config.warmup_rounds), int(self.config.comm_method),
                                int(self.config.send_method),
@@ -189,7 +204,7 @@ class MPIcuFFT:
         if self._decomp == PENCIL and partition is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         h = C.c_void_p()
-        L, head, n = lib(), (self.comm._h, C.byref(cfg), self._decomp, self.precision), (global_size.Nx, global_size.Ny, global_size.Nz)
+        L, head, n = lib(), (self.comm._h, C.byref(cfg), self._decomp, self.precision), (global_size.Nx, global_size.Ny, global_size.Nz) if global_size else ()
         tail = (batch, 1 if allocate else 0, C.byref(h))
 
         def sizes(v):
@@ -213,6 +228,8 @@ class MPIcuFFT:
         # call).  The first one given makes the plan, and any other keyword given that it does not take raises ValueError
         # before the library is called.
         creators = (
+            ("signal", signal is not None, (), "1D plans are out of place and C2C, with one component, no boxes and the whole grid",
+             lambda: L.dfft_plan_create_1d(self.comm._h, C.byref(cfg), self.precision, int(signal), sizes(factors), C.byref(h))),
             ("data", data is not None, ("spectral",), "pruned plans are out of place, C2C or R2C, with one component and no boxes",
              lambda: L.dfft_plan_create_pruned(*head, self.transform, *n, sizes(data), sizes(spectral), p1, p2, *tail)),
             ("boxes", in_boxes is not None or out_boxes is not None, (),
@@ -235,6 +252,8 @@ class MPIcuFFT:
             raise ValueError("batch must be at least 1")
         check(create())
         self._h = h
+        if signal is not None:
+            global_size = GlobalSize(*self.getFactors())
         self.global_size = global_size
         self.initialized = True
         self._strides = (None, None)
@@ -390,6 +409,7 @@ class MPIcuFFT:
     def getDomainSize(self): return int(lib().dfft_get_domain_size(self._h))
     def getSpectralSize(self): return self._triple(lib().dfft_plan_get_spectral_size)
     def getDataSize(self): return self._triple(lib().dfft_plan_get_data_size)
+    def getFactors(self): return self._triple(lib().dfft_plan_get_1d_factors)
     def getBatch(self): return int(lib().dfft_get_batch(self._h))
     def getComponents(self): return int(lib().dfft_get_components(self._h))
     def isInPlace(self): return bool(lib().dfft_plan_is_inplace(self._h))

@@ -274,6 +274,28 @@ int dfft_plan_create_pruned(dfft_comm_t comm, const dfft_config* config, int dec
                             const size_t spectral[3], size_t p1, size_t p2, size_t batch, int allocate, dfft_plan_t* plan);
 /* m[0..2] = mx, my, mz of a pruned plan; nx, ny, nz for every other plan. */
 int dfft_plan_get_data_size(dfft_plan_t plan, size_t m[3]);
+/* Distributed 1D complex transforms (FFTW-MPI's fftw_mpi_plan_dft_1d with FFTW_MPI_SCRAMBLED_OUT / _IN): one signal of
+ * n = N1 * N2 * N3 points, split over the ranks in contiguous chunks.
+ *   - The signal x[n] is the grid [N1][N2][N3], n = n1 N2 N3 + n2 N3 + n3, and the plan's geometry is the
+ *     DFFT_SLAB_ZY_THEN_X plan of that grid: dfft_get_in_size / _start and dfft_get_out_size / _start both give this rank's
+ *     x-slab [in_size[0]][N2][N3].  This rank's chunk of the signal starts at point in_start[0] * N2 * N3.
+ *   - Forward (dfft_exec_c2c, _async): out[k1][k2][k3] = X[k1 + N1 k2 + N1 N2 k3], X[k] = sum_n x[n] exp(-2 pi i n k / n):
+ *     the scrambled order.  Frequency k sits at position [k % N1][(k / N1) % N2][k / (N1 N2)].  Inverse: takes that
+ *     scrambled array and returns the natural-order signal, unnormalised: inverse(forward(x)) = n x.
+ *   - factors: N1, N2, N3, each a power of two in [2, 8192], with N1 and N2 at least the rank count; NULL lets the
+ *     library pick them: log2 n split into three parts in [1, 13], N1 and N2 >= the rank count, as balanced as possible,
+ *     of equally balanced splits the one with the largest N1, then the largest N2.  dfft_plan_get_1d_factors reports them.
+ *   - C2C only, DFFT_F64 or DFFT_F32, out of place, batch 1, Peer2Peer or All2All, the sequential schedule
+ *     (dfft_plan_tune reports "1D plans").  dfft_plan_set_scale works as for every plan.  dfft_plan_describe reports
+ *     "signal": n and "twiddle": "y" / "z" on the twiddled passes.
+ *   - n not a power of two in [8, 2^39], a factor outside [2, 8192], or no default split: DFFT_ERR_UNSUPPORTED; factors
+ *     whose product is not n, or N1 or N2 below the rank count: DFFT_ERR_INVALID.  DFFT_F16 / DFFT_BF16,
+ *     dfft_plan_set_transform_axes other than {1, 1, 1}, dfft_plan_set_strides, dfft_plan_set_weights and partial execs
+ *     (d < 3, also for dfft_plan_describe): DFFT_ERR_UNSUPPORTED. */
+int dfft_plan_create_1d(dfft_comm_t comm, const dfft_config* config, int precision /*dfft_prec*/, size_t n, const size_t factors[3],
+                        dfft_plan_t* plan);
+/* f[0..2] = N1, N2, N3 of a 1D plan; DFFT_ERR_INVALID for other plans. */
+int dfft_plan_get_1d_factors(dfft_plan_t plan, size_t f[3]);
 /* Interleaved multi-component plans (FFTW-MPI's `howmany`): every grid point holds `components` consecutive values,
  * and each component is transformed on its own.
  *   - Every caller layout is that of the components = 1 plan with each element widened to C = components consecutive

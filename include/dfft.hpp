@@ -131,6 +131,18 @@ public:
         initFFT(global_size, partition, allocate, batch);
     }
     size_t getComponents() const { return dfft_get_components(plan); }
+    // not in the reference: a distributed 1D C2C transform of one n-point signal (dfft_plan_create_1d), the slab plan of the
+    // grid factors[0..2] = N1 x N2 x N3 (null: the library's choice, getFactors).  Each rank's buffers are its x-slab of that
+    // grid on both sides, its chunk of the signal from point getInStart()[0] * N2 * N3; the forward output is in scrambled
+    // order, frequency k at [k % N1][(k / N1) % N2][k / (N1 N2)] (dfft.h).  The plan's class runs it with its C2C exec.
+    void initFFT1d(size_t n, const size_t* factors = nullptr) {
+        const dfft_config c = make_config();
+        if (plan) { dfft_plan_destroy(plan); plan = nullptr; }
+        DFFT_CALL(dfft_plan_create_1d(comm, &c, dfft_shim::prec<T>::value, n, factors, &plan));
+        initialized = true;
+    }
+    // N1, N2, N3 of a 1D plan
+    void getFactors(size_t* f) const { DFFT_CALL(dfft_plan_get_1d_factors(plan, f)); }
     // not in the reference: a box plan (dfft_plan_create_boxes): in_boxes / out_boxes hold lo[3], hi[3] of every rank in
     // rank order (6 values each; null: the natural layout), and each rank's buffers are its boxes
     void initFFT(GlobalSize* global_size, Partition* partition, const size_t* in_boxes, const size_t* out_boxes, bool allocate = true,
@@ -190,12 +202,16 @@ public:
     dfft_plan_t handle() const { return plan; }
 
 protected:
-    void create(int decomp, GlobalSize* gs, size_t p1, size_t p2, bool allocate) {
+    dfft_config make_config() const {
         dfft_config c{};
         c.cuda_aware = config.cuda_aware; c.warmup_rounds = config.warmup_rounds;
         c.comm_method = config.comm_method; c.send_method = config.send_method;
         c.benchmark_dir = config.benchmark_dir.empty() ? nullptr : config.benchmark_dir.c_str();
         c.comm_method2 = config.comm_method2; c.send_method2 = config.send_method2;
+        return c;
+    }
+    void create(int decomp, GlobalSize* gs, size_t p1, size_t p2, bool allocate) {
+        const dfft_config c = make_config();
         if (plan) { dfft_plan_destroy(plan); plan = nullptr; }
         if (in_boxes_ || out_boxes_)
             DFFT_CALL(dfft_plan_create_boxes(comm, &c, decomp, dfft_shim::prec<T>::value, transform, gs->Nx, gs->Ny, gs->Nz, p1, p2, in_boxes_,
