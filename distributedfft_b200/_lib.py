@@ -64,6 +64,8 @@ SIGNATURES = {
                                           C.c_int, C.POINTER(C.c_void_p)]),
     "dfft_plan_get_data_size": (C.c_int, [C.c_void_p, C.POINTER(C.c_size_t)]),
     "dfft_plan_create_1d": (C.c_int, [C.c_void_p, C.POINTER(dfft_config), C.c_int, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_void_p)]),
+    "dfft_plan_create_1d_natural": (C.c_int, [C.c_void_p, C.POINTER(dfft_config), C.c_int, C.c_size_t, C.POINTER(C.c_size_t),
+                                              C.POINTER(C.c_void_p)]),
     "dfft_plan_get_1d_factors": (C.c_int, [C.c_void_p, C.POINTER(C.c_size_t)]),
     "dfft_plan_create_interleaved": (C.c_int, [C.c_void_p, C.POINTER(dfft_config), C.c_int, C.c_int, C.c_int, C.c_size_t, C.c_size_t,
                                                C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int, C.POINTER(C.c_void_p)]),

@@ -174,6 +174,7 @@ struct Twiddle1d {
     const void* table;              // make_tw1d_table of log2n
     long long line0, c1, mul;       // FftPadded::tw_line0, tw_c1, tw_mul
     int log2n;                      // N = 2^log2n, the signal's length
+    long long sB = 0;               // FftPadded::tw_sB: the transposing z pass of natural-order plans; 0 for the others
 };
 static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftParams& prm, const void* blu, double scale, cudaStream_t stream,
                                    int r2r = DFFT_DCT, const int* hole = nullptr, const void* w = nullptr, const Twiddle1d* tw = nullptr) {
@@ -193,6 +194,7 @@ static cudaError_t launch_fft_pass(int prec, PassKind kind, size_t n, const FftP
         q.tw_mul = tw ? tw->mul : 0;
         q.tw_log2n = tw ? tw->log2n : 0;
         q.tw_lo_bits = tw ? tw1d_lo_bits(tw->log2n) : 0;
+        q.tw_sB = tw ? tw->sB : 0;
         return launch_twin(prec, log2n, kind, q, stream);
     }
     if (kind == PASS_R2R_CONTIG || kind == PASS_R2R_TILED) {
@@ -575,6 +577,9 @@ struct dfft_plan_s {
     bool weighted = false;
     // dfft_plan_create_1d: the signal's length N = Nx * Ny * Nz (the factors are the grid), 0 for 3D plans
     size_t n1d = 0;
+    // dfft_plan_create_1d_natural: the split of N3 over the ranks, rank r's output chunk [oz.size[r]][N2][N1] from k3 =
+    // oz.start[r]; empty for every other plan
+    dfft::Split oz;
     // dfft_plan_create_boxes: every rank's box of the physical grid (in_boxes) and of the output grid (out_boxes), in rank
     // order; empty where that side has the natural layout.  box_direct: their reshapes push and gather over peer memory
     // (comm_method Peer2Peer), otherwise they run through an NCCL all-to-all
@@ -1454,6 +1459,16 @@ static int build_schedule(dfft_plan_s* p, int inverse, int d, Schedule& sc) {
 // Every slot is free when a peer stores into it: D1 (forward) was last read by the z pass of the previous exec, before
 // the entry rendezvous, and D2 by nobody; inverse, D1 was read by the y pass before the rendezvous of the y -> x
 // transposition.
+// Natural-order plans (dfft_plan_create_1d_natural, DESIGN.md section 3.23) hold their spectrum as [N3][N2][N1], each rank
+// the chunk [oz_i][N2][N1] of the N3 split p->oz.  Their z pass runs TILED in its transposing form (Twiddle1d::sB): it reads
+// the rows [k1][k2][:] of my x-slab and scatters k3 to the owners' chunks, at column x0_i.  On one rank it stores into the
+// caller's out (forward) or reads its in (inverse).  On more ranks:
+//   forward  ... y pass | rendezvous | z pass into every rank's D2 | rendezvous | landing copy: D2 -> the caller's out
+//   inverse  scatter copy: the caller's in -> every rank's D2 [N3][N2][nx_q] | rendezvous | z pass: D2 -> D1 | rendezvous
+//            | the y pass, x pass and copy of the scrambled inverse
+// The landing slot is D2: forward its last reader is my y pass, inverse the next writer into it is a peer's y pass, so a
+// rendezvous between the y and z passes frees it without a slot more.  All-to-all plans exchange through SS / SR
+// instead, in stream order, and need no such rendezvous.
 static int build_1d(dfft_plan_s* p, int inverse, Schedule& sc) {
     const Geometry& g = p->g;
     const int me = p->rank, P = p->P;
@@ -1467,6 +1482,9 @@ static int build_1d(dfft_plan_s* p, int inverse, Schedule& sc) {
     const Transposition to_y(p, 2, AY, AX, g.oy, g.sx, nz, tab_y, tab_x, inverse ? -1 : p->slots.D1);
     const Transposition to_x(p, 2, AX, AY, g.sx, g.oy, nz, tab_x, tab_y, inverse ? p->slots.D1 : -1);
     void* d1 = p->slot(p->slots.D1, me);
+    const bool natural = !p->oz.size.empty();
+    const unsigned char* tab_z = nullptr;
+    if (natural && P > 1 && T.seg_table(p->oz, &tab_z) != cudaSuccess) return fail(DFFT_ERR_CUDA, "segment table");
     void* tw = nullptr;
     if (T.get_tw1d(ilog2_exact(p->n1d), &tw) != cudaSuccess) return fail(DFFT_ERR_CUDA, "twiddle table allocation failed");
     // the y and z passes over my x-slab [nx_i][N2][N3] in slot D1 and the caller's buffer, twiddled
@@ -1507,6 +1525,58 @@ static int build_1d(dfft_plan_s* p, int inverse, Schedule& sc) {
     x.label = "x pass";
     x.prm.A0 = 1; x.prm.A1 = 1; x.prm.B = int(oy_i * nz);
     if ((rc = twiddled(1, y)) || (rc = twiddled(2, z))) return rc;
+    // the z pass and, natural order on more ranks, its exchange and copy
+    auto push_z = [&]() {
+        z.phase = inverse ? nullptr : "2D FFT Y-Z-Direction";
+        if (!natural) { sc.steps.push_back(z); return; }
+        // the transposing z pass: tiles of TB consecutive k1 of one k2 (a0 = k2, b = k1 - x0_i), its row side my x-slab in
+        // slot D1, lines N2 N3 apart; the other side [k3][k2][k1] with k1 contiguous
+        z.kind = PASS_C2C_TILED;
+        z.prm.A0 = int(ny); z.prm.A1 = 1; z.prm.B = int(nx_i);
+        z.tw.sB = (long long)(ny * nz);
+        const View rows = single_view(d1, (long long)nz, 0, 1);
+        const View chunk = single_view(nullptr, (long long)g.nx, 0, (long long)(ny * g.nx));  // [N3][N2][N1] (one rank)
+        z.in_user = z.out_user = 0;
+        if (inverse) { z.prm.in = chunk; z.in_user = 1; z.prm.out = rows; }
+        else { z.prm.in = rows; z.prm.out = chunk; z.out_user = 2; }
+        if (P == 1) { sc.steps.push_back(z); return; }
+        // the output chunks [oz_q][N2][N1] as boxes with k3, k2, k1 for x, y, z: the forward z pass sends k3 to its owners at
+        // column x0_i, the inverse scatter copy k1 to the x-slabs [N3][N2][nx_q] at row z0_i
+        const Transposition to_n(p, 2, AX, AZ, p->oz, g.sx, ny, tab_z, tab_x), from_n(p, 2, AZ, AX, g.sx, p->oz, ny, tab_x, tab_z);
+        // the copy between the caller's chunk and the landing slot, one line per (k3, k2), n = k1
+        auto natural_copy = [&](const char* label, const View& in, const View& out, Step& s) {
+            s = Step();
+            s.label = label;
+            s.kind = PASS_COPY_CONTIG;
+            s.n = g.nx;
+            s.axis = 2;
+            s.prm.A0 = int(p->oz.size[me]); s.prm.A1 = int(ny); s.prm.B = 1;
+            s.prm.inverse = inverse;
+            s.prm.in = in;
+            s.prm.out = out;
+        };
+        const View mine = single_view(nullptr, (long long)(ny * g.nx), (long long)g.nx, 1);
+        z.prm.tile_pref = p->xchg_tile_pref;
+        if (!inverse) {
+            z.out_user = 0;
+            z.prm.out = to_n.send({AY, NO_AXIS, AX});
+            if (to_n.direct) sc.steps.push_back(new_rendezvous(2, 2, nullptr, 0));  // my y pass has read D2
+            sc.steps.push_back(z);
+            to_n.finish(sc);
+            natural_copy("landing copy", to_n.recv({AX, AY, AZ}), mine, c);
+            c.out_user = 2;
+            sc.steps.push_back(c);
+            return;
+        }
+        natural_copy("scatter copy", mine, from_n.send({AX, AY, AZ}), c);
+        c.in_user = 1;
+        sc.steps.push_back(c);
+        from_n.finish(sc);
+        z.in_user = 0;
+        z.prm.in = from_n.recv({AY, NO_AXIS, AX});
+        sc.steps.push_back(z);
+        if (from_n.direct) sc.steps.push_back(new_rendezvous(2, 2, nullptr, 0));  // every z pass has read D2
+    };
     if (!inverse) {
         if (P > 1) {
             transpose(slab, to_y.send({AX, NO_AXIS, AY}), c);
@@ -1522,13 +1592,11 @@ static int build_1d(dfft_plan_s* p, int inverse, Schedule& sc) {
         sc.steps.push_back(x);
         to_x.finish(sc);
         y.prm.in = to_x.recv({AX, NO_AXIS, AY});
-        z.phase = "2D FFT Y-Z-Direction";
         sc.steps.push_back(y);
-        sc.steps.push_back(z);
+        push_z();
         return DFFT_SUCCESS;
     }
-    z.phase = nullptr;
-    sc.steps.push_back(z);
+    push_z();
     y.prm.out = to_y.send({AX, NO_AXIS, AY});
     y.phase = "2D FFT Y-Z-Direction";
     sc.steps.push_back(y);
@@ -2453,9 +2521,14 @@ static int widen_views(dfft_plan_s* p, Schedule& sc) {
 
 // This rank's block of layout `which` (0 input, 1 and 2 after z and y, 3 output) as the caller holds it: its box on a boxed
 // side of a box plan (the physical side of every d, the output of d = 3), the plan's own layout otherwise.  1D plans hold
-// the x-slab of the input layout on both sides.
+// the x-slab of the input layout on both sides, natural-order ones their chunk [oz_r][N2][N1] of the output grid
+// [N3][N2][N1] on the output side.
 static void caller_block(const dfft_plan_s* p, int which, size_t s[3], size_t o[3]) {
     p->g.layout(p->rank, p->n1d ? 0 : which, s, o);
+    if (which == 3 && !p->oz.size.empty()) {
+        s[0] = p->oz.size[size_t(p->rank)]; s[1] = p->g.ny; s[2] = p->g.nx;
+        o[0] = p->oz.start[size_t(p->rank)]; o[1] = o[2] = 0;
+    }
     const std::vector<Box>& boxes = which == 0 ? p->in_boxes : p->out_boxes;
     if ((which == 0 || which == 3) && !boxes.empty())
         for (int k = 0; k < 3; ++k) { s[k] = boxes[size_t(p->rank)].extent(k); o[k] = boxes[size_t(p->rank)].lo[k]; }
@@ -3062,6 +3135,7 @@ struct PlanSpec {
     size_t k[3] = {0, 0, 0}, m[3] = {0, 0, 0};  // the spectral and data sizes; 0: the grid
     std::vector<Box> boxes[2];                  // the in and out box of every rank; empty: that side has its natural layout
     size_t signal = 0;                          // dfft_plan_create_1d: N, with n the factors N1, N2, N3 (0 where none was found)
+    bool natural = false;                       // dfft_plan_create_1d_natural: the output in natural order
     PlanSpec(unsigned made_by_, int decomp_, int precision_, int transform_, size_t nx, size_t ny, size_t nz, size_t p1_, size_t p2_, size_t batch_)
         : made_by(made_by_), decomp(decomp_), precision(precision_), transform(transform_), n{nx, ny, nz}, p1(p1_), p2(p2_), batch(batch_) {}
     unsigned features() const { return made_by | (is_half(precision) ? F_HALF : 0) | (is_r2r(transform) ? F_R2R : 0) | (inplace ? F_INPLACE : 0); }
@@ -3132,13 +3206,16 @@ static int check_spec(dfft_comm_t comm, const dfft_plan_t* plan, const PlanSpec&
         if (l < 3 || l > 3 * MAX_LOG2N)
             return fail(DFFT_ERR_UNSUPPORTED, "1D plans take n a power of two in [8, 2^" + std::to_string(3 * MAX_LOG2N) + "]");
         if (n[0] == 0)
-            return fail(DFFT_ERR_UNSUPPORTED, "n = " + std::to_string(s.signal) + " has no split into three powers of two in [2, 8192] with N1 " +
-                                                  "and N2 at least the rank count");
+            return fail(DFFT_ERR_UNSUPPORTED, "n = " + std::to_string(s.signal) + " has no split into three powers of two in [2, 8192] with " +
+                                                  (s.natural ? "N1, N2 and N3" : "N1 and N2") + " at least the rank count");
         if (!pow2_length(n[0]) || !pow2_length(n[1]) || !pow2_length(n[2]))
             return fail(DFFT_ERR_UNSUPPORTED, "the factors of a 1D plan must be powers of two in [2, 8192]");
         if (n[0] * n[1] * n[2] != s.signal) return fail(DFFT_ERR_INVALID, "the factors of a 1D plan must multiply to n");
         if (n[0] < size_t(comm->nranks) || n[1] < size_t(comm->nranks))
             return fail(DFFT_ERR_INVALID, "the factors N1 and N2 of a 1D plan must be at least the rank count, so that every rank holds data");
+        if (s.natural && n[2] < size_t(comm->nranks))
+            return fail(DFFT_ERR_INVALID, "the factor N3 of a natural-order 1D plan must be at least the rank count, so that every rank holds "
+                                          "output");
     } else if (s.made_by == F_KINDS) {
         if (!s.kinds) return fail(DFFT_ERR_INVALID, "null kinds");
         for (int a = 0; a < 3; ++a)
@@ -3222,6 +3299,7 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, const PlanSp
     p->inplace = inplace;
     p->batch = s.batch;
     p->n1d = s.signal;
+    if (s.natural) p->oz.make(nz, size_t(comm->nranks));
     // box plans: a side whose boxes are all natural keeps no boxes, so that it makes exactly the plan of
     // dfft_plan_create_batched
     auto keep_boxes = [&](const std::vector<Box>& b, int which, std::vector<Box>& dst) {
@@ -3242,7 +3320,9 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, const PlanSp
     };
     // the largest stage array of this rank; it also covers the padded real input of in-place R2C plans, which has the
     // extent of the layout after d = 1
-    p->domain_bytes = std::max(g.domain_elems(p->rank), box_elems(p->rank)) * p->esize * comps;
+    // natural-order 1D plans: and the output chunk [oz_r][N2][N1], which the landing slot holds too
+    auto chunk_elems = [&](int r) { return p->oz.size.empty() ? 0 : p->oz.size[size_t(r)] * ny * nx; };
+    p->domain_bytes = std::max({g.domain_elems(p->rank), box_elems(p->rank), chunk_elems(p->rank)}) * p->esize * comps;
     // groups
     const int me = p->rank, P = p->P;
     p->grp[0].clear();
@@ -3276,7 +3356,7 @@ static int plan_create(dfft_comm_t comm, const dfft_config* config, const PlanSp
     p->buf_slot = inplace && P == 1;
     p->nslots = p->slots.count - (p->buf_slot ? 1 : 0);
     size_t dom = 0;
-    for (int r = 0; r < P; ++r) dom = std::max(dom, std::max(g.domain_elems(r), box_elems(r)));
+    for (int r = 0; r < P; ++r) dom = std::max({dom, g.domain_elems(r), box_elems(r), chunk_elems(r)});
     p->slot_bytes = ((dom * p->esize * comps + 255) / 256) * 256;
     p->work_bytes = p->slot_bytes * p->nslots;
     {
@@ -3471,7 +3551,8 @@ int dfft_plan_get_r2r_kinds(dfft_plan_t p, int kinds[3]) {
 // 1D plans (DESIGN.md section 3.22).  Default factors: log2 N split into l1 + l2 + l3 with every l in [1, 13] and l1, l2
 // at least ceil(log2 P) (N1, N2 >= P: no rank without data), the split with the smallest spread max(l) - min(l), and of
 // those the largest l1, then the largest l2 (so N1 >= N2 >= N3 when nothing else decides).  All zero when none exists.
-static void default_factors(size_t n, int P, size_t f[3]) {
+// natural: l3 at least ceil(log2 P) as well (N3 >= P: no rank without output, section 3.23).
+static void default_factors(size_t n, int P, size_t f[3], bool natural) {
     f[0] = f[1] = f[2] = 0;
     const int L = ilog2_exact(n);
     int lp = 1;
@@ -3480,7 +3561,7 @@ static void default_factors(size_t n, int P, size_t f[3]) {
     for (int l1 = MAX_LOG2N; l1 >= lp; --l1)
         for (int l2 = MAX_LOG2N; l2 >= lp; --l2) {
             const int l3 = L - l1 - l2;
-            if (L < 0 || l3 < 1 || l3 > MAX_LOG2N) continue;
+            if (L < 0 || l3 < (natural ? lp : 1) || l3 > MAX_LOG2N) continue;
             const int spread = std::max({l1, l2, l3}) - std::min({l1, l2, l3});
             if (best >= 0 && spread >= best) continue;
             best = spread;
@@ -3488,13 +3569,23 @@ static void default_factors(size_t n, int P, size_t f[3]) {
         }
 }
 
-int dfft_plan_create_1d(dfft_comm_t comm, const dfft_config* config, int precision, size_t n, const size_t factors[3], dfft_plan_t* plan) {
+static int create_1d(dfft_comm_t comm, const dfft_config* config, int precision, size_t n, const size_t factors[3], bool natural, dfft_plan_t* plan) {
     size_t f[3] = {0, 0, 0};
     if (factors) for (int a = 0; a < 3; ++a) f[a] = factors[a];
-    else default_factors(n, comm ? comm->nranks : 1, f);
+    else default_factors(n, comm ? comm->nranks : 1, f, natural);
     PlanSpec s(F_1D, DFFT_SLAB_ZY_THEN_X, precision, DFFT_C2C, f[0], f[1], f[2], comm ? size_t(comm->nranks) : 1, 1, 1);
     s.signal = n;
+    s.natural = natural;
     return plan_create(comm, config, s, 1, plan);
+}
+
+int dfft_plan_create_1d(dfft_comm_t comm, const dfft_config* config, int precision, size_t n, const size_t factors[3], dfft_plan_t* plan) {
+    return create_1d(comm, config, precision, n, factors, false, plan);
+}
+
+// natural-order output (DESIGN.md section 3.23): the same plan with N3 at least the rank count, and the z pass transposing
+int dfft_plan_create_1d_natural(dfft_comm_t comm, const dfft_config* config, int precision, size_t n, const size_t factors[3], dfft_plan_t* plan) {
+    return create_1d(comm, config, precision, n, factors, true, plan);
 }
 
 int dfft_plan_get_1d_factors(dfft_plan_t p, size_t f[3]) {
@@ -4011,7 +4102,7 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
                     (p->g.pruned() ? ",\"data\":[" + std::to_string(p->g.mx) + "," + std::to_string(p->g.my) + "," + std::to_string(p->g.mz) + "]"
                                    : std::string()) +
                     (p->comps > 1 ? ",\"components\":" + std::to_string(p->comps) : std::string()) +
-                    (p->n1d ? ",\"signal\":" + std::to_string(p->n1d) : std::string()) +
+                    (p->n1d ? ",\"signal\":" + std::to_string(p->n1d) : std::string()) + (p->oz.size.empty() ? "" : ",\"order\":\"natural\"") +
                     (p->weighted ? ",\"weights\":[" + std::to_string(p->weights[0] ? 1 : 0) + "," + std::to_string(p->weights[1] ? 1 : 0) + "," +
                                        std::to_string(p->weights[2] ? 1 : 0) + "]"
                                  : std::string()) +
@@ -4132,6 +4223,8 @@ int dfft_plan_describe(dfft_plan_t p, int inverse, int d, char* buf, size_t capa
                  (s_.twiddle ? std::string(",\"twiddle\":\"") + s_.twiddle + "\",\"tw\":[" + std::to_string(s_.tw.line0) + "," +
                                    std::to_string(s_.tw.c1) + "," + std::to_string(s_.tw.mul) + "]"
                              : std::string()) +
+                 // the transposing z pass of natural-order 1D plans: its row side's line stride
+                 (s_.tw.sB ? ",\"transposed\":" + std::to_string(s_.tw.sB) : std::string()) +
                  ",\"A0\":" + std::to_string(s_.prm.A0) +
                  ",\"A1\":" + std::to_string(s_.prm.A1) + ",\"B\":" + std::to_string(s_.prm.B) + ",\"inverse\":" + std::to_string(s_.prm.inverse) +
                  ",\"in_user\":" + std::to_string(s_.in_user) + ",\"out_user\":" + std::to_string(s_.out_user) + ",\"in\":";
@@ -4334,7 +4427,9 @@ int dfft_debug_run_step(dfft_plan_t p, int inverse, int d, size_t field, int ste
             for (size_t n = 0; n < n_len; ++n)
                 if (v.nseg == 1 || (*tab)[n] == g) { if (n_lo < 0) n_lo = (long long)n; n_hi = (long long)n; }
             if (n_lo < 0 || s.prm.A0 <= 0 || s.prm.A1 <= 0 || s.prm.B <= 0) continue;  // the segment holds no element
-            long long lo = 0, hi = s.prm.B - 1;
+            // b is contiguous, except on the row side of the transposing z pass of natural-order 1D plans (lines tw.sB apart)
+            const bool row = s.tw.sB && &v == (s.prm.inverse ? &s.prm.out : &s.prm.in);
+            long long lo = 0, hi = (long long)(s.prm.B - 1) * (row ? s.tw.sB : 1);
             for (const long long t : {(long long)(s.prm.A0 - 1) * sg.sA0, (long long)(s.prm.A1 - 1) * sg.sA1}) { lo += std::min(0ll, t); hi += std::max(0ll, t); }
             const long long t0 = (n_lo - sg.n0) * v.sN, t1 = (n_hi - sg.n0) * v.sN;
             lo += std::min(t0, t1);

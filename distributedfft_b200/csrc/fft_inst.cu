@@ -247,8 +247,9 @@ template cudaError_t launch_pass<float, cx16<DFFT_S>, DFFT_LOG2N>(PassKind, cons
 template cudaError_t launch_pass<DFFT_T, cx<DFFT_T>, DFFT_LOG2N>(PassKind, const FftParams&, double, cudaStream_t);
 
 // the padded twins (fft_c2c_padded_kernel, fft_r2c_padded_kernel, fft_c2r_padded_kernel), their weighted instantiations
-// (WEIGHTED = true) where p.w is set, and the twiddled C2C passes of 1D plans (TWIDDLED = true) where p.tw1d is set: the tiles
-// of launch_pass (TILED: narrow or wide by wide_tile, without the TMA-fed kernel), one CTA per tile
+// (WEIGHTED = true) where p.w is set, and the twiddled C2C passes of 1D plans (TWIDDLED = true) where p.tw1d is set, TILED
+// ones in their transposing form (TRANSPOSED = true) where p.tw_sB is set: the tiles of launch_pass (TILED: narrow or wide
+// by wide_tile, without the TMA-fed kernel), one CTA per tile
 template <typename T, int LOG2N>
 cudaError_t launch_twin(PassKind kind, const FftPadded& p, cudaStream_t stream) {
     using S = Shape<T, LOG2N>;
@@ -273,9 +274,19 @@ cudaError_t launch_twin(PassKind kind, const FftPadded& p, cudaStream_t stream) 
             q.tile_swz = tile_swz_for(p.tile_swz, p.A0, p.A1);
             const long long g = lines * ((p.B + TB - 1) / TB);
             if (g > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+            if constexpr (TW) {
+                if (p.tw_sB) {  // the transposing form: its row side is one segment with contiguous lines
+                    const View& row = p.inverse ? p.out : p.in;
+                    if (row.nseg != 1 || row.sN != 1 || q.tile_swz) return cudaErrorInvalidValue;
+                    return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, LOG2E, TB, true, false, false, true, true>,
+                                         fft_c2c_padded_kernel<T, LOG2N, LOG2E, TB, true, true, false, true, true>, nullptr, nullptr>(
+                        q, 1.0, unsigned(g), CT::THREADS, CT::SMEM_BYTES, stream);
+                }
+            }
             return launch_kernel<fft_c2c_padded_kernel<T, LOG2N, LOG2E, TB, true, false, W, TW>, fft_c2c_padded_kernel<T, LOG2N, LOG2E, TB, true, true, W, TW>,
                                  nullptr, nullptr>(q, 1.0, unsigned(g), CT::THREADS, CT::SMEM_BYTES, stream);
         };
+        if (p.tw_sB && !(TW && kind == PASS_C2C_TILED)) return cudaErrorInvalidValue;  // TRANSPOSED: twiddled TILED passes only
         switch (kind) {
             case PASS_C2C_CONTIG:
                 if (p.in.sN != 1 || p.out.sN != 1) return cudaErrorInvalidValue;

@@ -447,6 +447,10 @@ struct FftPadded : FftScaled {
     const void* tw1d;
     long long tw_line0, tw_c1, tw_mul;
     int tw_log2n, tw_lo_bits;
+    // TRANSPOSED twiddled passes (the z pass of natural-order 1D plans, DESIGN.md section 3.23): a TILED pass whose row
+    // side (forward its loaded, inverse its stored side; one segment, sN = 1) holds line b's point n at b * tw_sB + n, and
+    // whose twiddle's line index is tw_line0 + b + tw_c1 * a0.  0: the plain form.
+    long long tw_sB;
 };
 // index in the view of line position n, -1 in the hole
 __device__ __forceinline__ int keep_index(int n, int lo, int hi) { return n < lo ? n : (n < hi ? -1 : n - (hi - lo)); }
@@ -460,6 +464,39 @@ __device__ __forceinline__ cx<T> tw1d_at(const FftPadded& p, unsigned long long 
     const unsigned long long lo = m & ((1ull << p.tw_lo_bits) - 1), hi = m >> p.tw_lo_bits;
     return cmul(t[(size_t(1) << p.tw_lo_bits) + hi], t[lo]);
 }
+
+// the line index of a twiddled pass's tile: line0 + a0 + c1 a1, or, TRANSPOSED, line0 + b + c1 a0 (b: the thread's column)
+template <bool TRANSPOSED, typename TC>
+__device__ __forceinline__ unsigned long long tw1d_line(const FftPadded& p, const TC& tc) {
+    if constexpr (TRANSPOSED) return (unsigned long long)(p.tw_line0 + tc.b) + (unsigned long long)p.tw_c1 * tc.a0;
+    else return (unsigned long long)(p.tw_line0 + tc.a0) + (unsigned long long)p.tw_c1 * tc.a1;
+}
+
+// the row side of a TRANSPOSED pass: element n = 0 of line (a0, a1, b) of its one segment, lines tw_sB apart along b
+template <typename S>
+__device__ __forceinline__ S* row_line(const View& v, int a0, int a1, int b, long long sB) {
+    const Seg& g = v.seg[0];
+    return reinterpret_cast<S*>(g.base) + (a0 * g.sA0 + a1 * g.sA1 + (long long)b * sB);
+}
+
+// The stored row side of a TRANSPOSED pass (the inverse's) where a warp's direct stores would cover less than a 32-byte
+// sector of each row (TB lines x 32 / TB points: TB > ROW_LINES): the finished tile goes through shared memory instead.
+// Element i = threadIdx.x + e * THREADS of the tile is point n of column bb, a warp covering ROW_LINES columns x ROW_PTS
+// consecutive points, so each row takes one 32-byte run (a whole line where it is shorter) and a quarter warp's
+// shared-memory reads are consecutive columns.  The forward's row loads stay direct: the other half of a sector one warp
+// reads is read by a neighbouring warp of the same tile, from L1, and staging them measured slower (DESIGN.md 3.23).
+template <typename T, int N, int TB>
+struct RowStage {
+    static constexpr int ROW_PTS = 32 / int(sizeof(cx<T>)) < N ? 32 / int(sizeof(cx<T>)) : N;
+    static constexpr int ROW_LINES = 32 / ROW_PTS;
+    static constexpr bool ON = TB > ROW_LINES;
+    static __device__ __forceinline__ void point(int i, int& bb, int& n) {
+        constexpr int GB = ON ? TB / ROW_LINES : 1;  // column groups of a tile
+        const int rest = i / 32;
+        bb = (rest % GB) * ROW_LINES + i % ROW_LINES;
+        n = (rest / GB) * ROW_PTS + (i / ROW_LINES) % ROW_PTS;
+    }
+};
 
 // store policy of the padded twins: plain stores, scaled when s != 1 (a runtime value)
 template <typename T>
@@ -481,8 +518,12 @@ __device__ __forceinline__ void l2_discard(const void* p) { asm volatile("discar
 // forward before the store
 // TWIDDLED (tp: the FftPadded of a 1D plan's pass): point n of the line times W_N^(n * line index * mul) (tw1d_at):
 // forward after the load, inverse its conjugate before the store
+// TRANSPOSED (TILED and TWIDDLED): the row side (forward in, inverse out) holds each line contiguously, line b at
+// b * tw_sB (row_line); the other side is the plain TILED view, b contiguous.  A warp's direct access covers TB lines x
+// 32 / TB consecutive points, whole 32-byte sectors of each row while TB <= sizeof(cx<T>) (16 lines in f64, 8 in f32);
+// wider tiles of the inverse store the row side through the tile in shared memory (RowStage).
 template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, typename M, typename Hook = NoGatherHook, bool PADDED = false,
-          bool ILV = false, bool WEIGHTED = false, bool TWIDDLED = false>
+          bool ILV = false, bool WEIGHTED = false, bool TWIDDLED = false, bool TRANSPOSED = false>
 __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<T>* sm, unsigned long long* tab_in, unsigned long long* tab_out,
                                          bool multi, const M& mem, const Hook& after_gather = {}, int ld_lo = 0, int ld_hi = 0, int st_lo = 0,
                                          int st_hi = 0, const cx<T>* w = nullptr, const FftPadded* tp = nullptr) {
@@ -492,6 +533,9 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
     using TC = TileCoord<C, TILED, TB, ILV>;
     constexpr bool STRIDED = TILED || ILV;
     constexpr int E = C::E, TPL = C::TPL;
+    static_assert(!TRANSPOSED || (TILED && TWIDDLED && !WEIGHTED), "TRANSPOSED: the TILED twiddled pass");
+    using RS = RowStage<T, C::N, TB>;
+    constexpr bool STAGED = TRANSPOSED && INV && RS::ON;
     const TC tc(p, tile);
     const int j = tc.j, t = tc.t;
     if (multi) {
@@ -509,7 +553,11 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
 
     cx<T> v[E];
     if (tc.valid) {
-        if (PADDED && ld_lo < ld_hi) {
+        if constexpr (TRANSPOSED && !INV) {
+            const S* q = row_line<const S>(p.in, tc.a0, tc.a1, tc.b, tp->tw_sB) + j;
+#pragma unroll
+            for (int e = 0; e < E; ++e) v[e] = mem.ld(q + e * TPL);
+        } else if (PADDED && ld_lo < ld_hi) {
 #pragma unroll
             for (int e = 0; e < E; ++e) {
                 const int m = keep_index(j + e * TPL, ld_lo, ld_hi);
@@ -539,7 +587,7 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
             }
         }
         if constexpr (TWIDDLED && !INV) {
-            const unsigned long long step = ((unsigned long long)(tp->tw_line0 + tc.a0) + (unsigned long long)tp->tw_c1 * tc.a1) * (unsigned long long)tp->tw_mul;
+            const unsigned long long step = tw1d_line<TRANSPOSED>(*tp, tc) * (unsigned long long)tp->tw_mul;
 #pragma unroll
             for (int e = 0; e < E; ++e) v[e] = cmul(v[e], tw1d_at<T>(*tp, (unsigned long long)(j + e * TPL) * step));
         }
@@ -567,7 +615,7 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
     if constexpr (TWIDDLED && INV) {
         // v holds the swapped values (cswap(z) = i conj(z)): multiplying them by W stores conj(W) times the result
         if (tc.valid) {
-            const unsigned long long step = ((unsigned long long)(tp->tw_line0 + tc.a0) + (unsigned long long)tp->tw_c1 * tc.a1) * (unsigned long long)tp->tw_mul;
+            const unsigned long long step = tw1d_line<TRANSPOSED>(*tp, tc) * (unsigned long long)tp->tw_mul;
 #pragma unroll
             for (int e = 0; e < E; ++e) {
                 cx<T>& x = v[C::Core::final_slot(e)];
@@ -575,8 +623,27 @@ __device__ __forceinline__ void c2c_tile(const FftParams& p, long long tile, cx<
             }
         }
     }
-    if (tc.valid) {
-        if (PADDED && st_lo < st_hi) {
+    if constexpr (STAGED) {  // the finished lines through shared memory, then sector-wide rows by every thread
+        __syncthreads();              // every thread's last gather has left the tile
+        if (tc.valid) {
+#pragma unroll
+            for (int e = 0; e < E; ++e) sm[C::sidx(j + e * TPL, t)] = cswap(v[C::Core::final_slot(e)]);
+        }
+        __syncthreads();
+        const int b0 = tc.b - t;
+        S* q = row_line<S>(p.out, tc.a0, tc.a1, b0, tp->tw_sB);
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            int bb, n;
+            RS::point(int(threadIdx.x) + e * C::THREADS, bb, n);
+            if (b0 + bb < p.B) mem.st(q + (long long)bb * tp->tw_sB + n, sm[C::sidx(n, bb)]);
+        }
+    } else if (tc.valid) {
+        if constexpr (TRANSPOSED && INV) {
+            S* q = row_line<S>(p.out, tc.a0, tc.a1, tc.b, tp->tw_sB) + j;
+#pragma unroll
+            for (int e = 0; e < E; ++e) mem.st(q + e * TPL, cswap(v[C::Core::final_slot(e)]));
+        } else if (PADDED && st_lo < st_hi) {
 #pragma unroll
             for (int e = 0; e < E; ++e) {
                 const int m = keep_index(j + e * TPL, st_lo, st_hi);
@@ -769,8 +836,8 @@ fft_rc_ilv_kernel(const __grid_constant__ KParams<SCALED> p) {
 }
 
 // padded twin of fft_c2c_kernel (FftPadded), with WEIGHTED its weighted twin (p.w), with TWIDDLED the twiddled pass of
-// 1D plans (p.tw1d): one CTA per tile
-template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, bool WEIGHTED, bool TWIDDLED = false>
+// 1D plans (p.tw1d), with TRANSPOSED its transposing form (p.tw_sB): one CTA per tile
+template <typename T, int LOG2N, int LOG2E, int TB, bool TILED, bool INV, bool WEIGHTED, bool TWIDDLED = false, bool TRANSPOSED = false>
 __global__ void __launch_bounds__((1 << (LOG2N - LOG2E)) * TB, min_ctas_per_sm<T, LOG2E>((1 << (LOG2N - LOG2E)) * TB))
 fft_c2c_padded_kernel(const __grid_constant__ FftPadded p) {
     using C = CtaFft<T, LOG2N, LOG2E, TB, TILED>;
@@ -779,7 +846,7 @@ fft_c2c_padded_kernel(const __grid_constant__ FftPadded p) {
     unsigned long long* tab_in = reinterpret_cast<unsigned long long*>(smem_raw + C::TILE_BYTES);
     unsigned long long* tab_out = tab_in + C::LINES * MAXSEG;
     const bool multi = p.in.nseg > 1 || p.out.nseg > 1;
-    c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV, MemRtScaled<T>, NoGatherHook, true, false, WEIGHTED, TWIDDLED>(
+    c2c_tile<T, LOG2N, LOG2E, TB, TILED, INV, MemRtScaled<T>, NoGatherHook, true, false, WEIGHTED, TWIDDLED, TRANSPOSED>(
         p, blockIdx.x, sm, tab_in, tab_out, multi, MemRtScaled<T>{p.scale != 1.0, T(p.scale)}, {}, p.ld_lo, p.ld_hi, p.st_lo, p.st_hi,
         WEIGHTED ? reinterpret_cast<const cx<T>*>(p.w) : nullptr, TWIDDLED ? &p : nullptr);
 }

@@ -155,7 +155,7 @@ class MPIcuFFT:
     def initFFT(self, global_size: GlobalSize, partition: Optional[Partition] = None, allocate: bool = True, batch: int = 1,
                 inplace: bool = False, transform_axes: Optional[Sequence[bool]] = None, spectral: Optional[Sequence[int]] = None,
                 components: int = 1, in_boxes=None, out_boxes=None, in_strides=None, out_strides=None, data: Optional[Sequence[int]] = None,
-                signal: Optional[int] = None, factors: Optional[Sequence[int]] = None):
+                signal: Optional[int] = None, factors: Optional[Sequence[int]] = None, natural: bool = False):
         """`batch` (not in the reference): every exec transforms that many fields, back to back in each buffer — a
         contiguous [batch, X, Y, Z] tensor; the getters describe one field (dfft_plan_create_batched).
         `inplace` (dfft_plan_create_inplace): every exec gets the same buffer twice and overwrites its input; fields are
@@ -183,7 +183,10 @@ class MPIcuFFT:
         the grid (N1, N2, N3) = `factors` (None: the library's balanced choice, getFactors()) with global_size None.  Each
         rank's buffers are its x-slab [in_size[0], N2, N3] of that grid on both sides, the forward output in scrambled order
         (frequency k at [k % N1][(k // N1) % N2][k // (N1 N2)]); 1D plans are C2C, out of place, batch 1, without
-        partition, strides or kept axes."""
+        partition, strides or kept axes.
+        `natural` (with `signal`, dfft_plan_create_1d_natural): the forward output in natural order instead: each rank's out
+        is its chunk [out_size[0], N2, N1] of the spectrum, frequencies getOutStart()[0] * N1 * N2 on, k increasing (flat
+        index k - that start); the inverse takes that chunk.  N3 must then be at least the rank count as well."""
         if signal is not None:
             if self._decomp != SLAB_ZY_THEN_X:
                 raise ValueError("1D plans are slab plans (MPIcuFFT_Slab)")
@@ -193,6 +196,8 @@ class MPIcuFFT:
                                  "transform_axes")
         elif factors is not None:
             raise ValueError("factors belong to a 1D plan (signal=n)")
+        elif natural:
+            raise ValueError("natural belongs to a 1D plan (signal=n)")
         elif global_size is None:
             raise RuntimeError("GlobalSize or Partition not initialized!")
         cfg = _lib.dfft_config(int(self.config.cuda_aware), int(self.config.warmup_rounds), int(self.config.comm_method),
@@ -228,6 +233,9 @@ class MPIcuFFT:
         # call).  The first one given makes the plan, and any other keyword given that it does not take raises ValueError
         # before the library is called.
         creators = (
+            ("natural", signal is not None and bool(natural), ("signal",),
+             "1D plans are out of place and C2C, with one component, no boxes and the whole grid",
+             lambda: L.dfft_plan_create_1d_natural(self.comm._h, C.byref(cfg), self.precision, int(signal), sizes(factors), C.byref(h))),
             ("signal", signal is not None, (), "1D plans are out of place and C2C, with one component, no boxes and the whole grid",
              lambda: L.dfft_plan_create_1d(self.comm._h, C.byref(cfg), self.precision, int(signal), sizes(factors), C.byref(h))),
             ("data", data is not None, ("spectral",), "pruned plans are out of place, C2C or R2C, with one component and no boxes",

@@ -294,7 +294,22 @@ int dfft_plan_get_data_size(dfft_plan_t plan, size_t m[3]);
  *     (d < 3, also for dfft_plan_describe): DFFT_ERR_UNSUPPORTED. */
 int dfft_plan_create_1d(dfft_comm_t comm, const dfft_config* config, int precision /*dfft_prec*/, size_t n, const size_t factors[3],
                         dfft_plan_t* plan);
-/* f[0..2] = N1, N2, N3 of a 1D plan; DFFT_ERR_INVALID for other plans. */
+/* Distributed 1D complex transforms with natural-order output (FFTW-MPI's default for fftw_mpi_plan_dft_1d): the plan
+ * of dfft_plan_create_1d, with the same signal, input chunk, factors rule, precisions and refusals, and these differences.
+ *   - Forward output in natural order.  With (oz_r, z0_r) rank r's part of the split of N3 over the P ranks
+ *     (dfft_partition(N3, P)), rank r's out holds X[k] for k in [z0_r N1 N2, (z0_r + oz_r) N1 N2), dense, k increasing: the
+ *     block [oz_r][N2][N1] of the grid [N3][N2][N1], k1 contiguous.  dfft_get_out_size gives {oz_r, N2, N1} and
+ *     dfft_get_out_start {z0_r, 0, 0}, as do dfft_get_partial_size / _start for d = 3; dfft_get_domain_size covers the
+ *     larger of the in and the out chunk.
+ *   - Inverse: takes that natural-order chunk and returns the natural signal on the x-slabs, unnormalised:
+ *     inverse(forward(x)) = n x.
+ *   - Factors: N3 must also be at least the rank count (DFFT_ERR_INVALID otherwise); the default split meets that too.
+ *   - dfft_plan_describe adds "order": "natural" to the plan and "transposed" to the z pass, which reads the rows of the
+ *     x-slabs and stores with k1 contiguous.  On more than one rank each direction adds one exchange and one local copy
+ *     (the "landing copy" forward, the "scatter copy" inverse) to the schedule of dfft_plan_create_1d. */
+int dfft_plan_create_1d_natural(dfft_comm_t comm, const dfft_config* config, int precision /*dfft_prec*/, size_t n, const size_t factors[3],
+                                dfft_plan_t* plan);
+/* f[0..2] = N1, N2, N3 of a 1D plan (either order); DFFT_ERR_INVALID for other plans. */
 int dfft_plan_get_1d_factors(dfft_plan_t plan, size_t f[3]);
 /* Interleaved multi-component plans (FFTW-MPI's `howmany`): every grid point holds `components` consecutive values,
  * and each component is transformed on its own.

@@ -135,10 +135,13 @@ public:
     // grid factors[0..2] = N1 x N2 x N3 (null: the library's choice, getFactors).  Each rank's buffers are its x-slab of that
     // grid on both sides, its chunk of the signal from point getInStart()[0] * N2 * N3; the forward output is in scrambled
     // order, frequency k at [k % N1][(k / N1) % N2][k / (N1 N2)] (dfft.h).  The plan's class runs it with its C2C exec.
-    void initFFT1d(size_t n, const size_t* factors = nullptr) {
+    // natural (dfft_plan_create_1d_natural): the forward output in natural order instead, each rank's out its chunk
+    // [getOutSize()[0]][N2][N1] of the spectrum, frequencies from getOutStart()[0] * N1 * N2 on.
+    void initFFT1d(size_t n, const size_t* factors = nullptr, bool natural = false) {
         const dfft_config c = make_config();
         if (plan) { dfft_plan_destroy(plan); plan = nullptr; }
-        DFFT_CALL(dfft_plan_create_1d(comm, &c, dfft_shim::prec<T>::value, n, factors, &plan));
+        if (natural) DFFT_CALL(dfft_plan_create_1d_natural(comm, &c, dfft_shim::prec<T>::value, n, factors, &plan));
+        else DFFT_CALL(dfft_plan_create_1d(comm, &c, dfft_shim::prec<T>::value, n, factors, &plan));
         initialized = true;
     }
     // N1, N2, N3 of a 1D plan

@@ -1,10 +1,14 @@
 """Times one-rank 1D plans (dfft_plan_create_1d) forward and inverse at N = 2^20 .. 2^30 against torch.fft.fft / ifft
-(cuFFT) on the same GPU.
+(cuFFT) on the same GPU.  --natural adds the natural-order plan (dfft_plan_create_1d_natural) as a third arm of the same
+rounds; --profile then also lists every kernel's time per exec of both 1D plans (torch.profiler, a run of its own after the
+timed rounds), so that the transposing z pass stands next to the scrambled plan's z pass.
 
 Each size warms up both, then runs `--rounds` rounds that alternate the plan and cuFFT, each round `--reps` execs between
 two CUDA events; the median per exec is reported.  The GPU's name, power limit and maximum SM clock are read in the same
 run.  Both transforms hold their buffers at once: in f64 2^30 points need more than 80 GB (in, out, the plan's two work
-slots and cuFFT's output), so f64 runs end at 2^29 there.  python tools/fft1d_bench.py [--precision double|float] [--min 20] [--max 30] [--json out.json]"""
+slots and cuFFT's output), so f64 runs end at 2^29 there.
+python tools/fft1d_bench.py [--precision double|float] [--min 20] [--max 30 | --sizes 20,24,29] [--natural] [--profile]
+                            [--json out.json]"""
 from __future__ import annotations
 
 import argparse
@@ -38,14 +42,37 @@ def timed(fn, reps):
     return a.elapsed_time(b) / reps
 
 
+def kernel_times(fn, execs=5):
+    """{kernel name: device ms per exec} of fn under torch.profiler"""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(execs):
+            fn()
+        torch.cuda.synchronize()
+    out = {}
+    for ev in prof.key_averages():
+        t = getattr(ev, "device_time_total", None)
+        if t is None:
+            t = ev.cuda_time_total
+        if t > 0:
+            out[ev.key] = t / 1000.0 / execs
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--precision", default="double", choices=["double", "float"])
     ap.add_argument("--min", type=int, default=20)
     ap.add_argument("--max", type=int, default=30)
+    ap.add_argument("--sizes", default=None, help="comma-separated log2 N to time instead of --min .. --max")
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--json", default=None)
+    ap.add_argument("--natural", action="store_true", help="also time the natural-order plan, alternating with the others")
+    ap.add_argument("--profile", action="store_true", help="with --natural: kernel times per exec of both 1D plans")
     a = ap.parse_args()
     import torch
 
@@ -56,8 +83,9 @@ def main():
     cdt = torch.complex128 if a.precision == "double" else torch.complex64
     rows = []
     print(f"# {torch.cuda.get_device_name(0)} | {gpu_info()} | {a.precision}")
-    print(f"{'N':>6} {'factors':>18} {'fwd ms':>9} {'cuFFT fwd':>10} {'inv ms':>9} {'cuFFT inv':>10}")
-    for L in range(a.min, a.max + 1):
+    print(f"{'N':>6} {'factors':>18} {'fwd ms':>9} {'cuFFT fwd':>10} {'inv ms':>9} {'cuFFT inv':>10}" +
+          (f" {'nat fwd':>9} {'nat inv':>9}" if a.natural else ""))
+    for L in [int(v) for v in a.sizes.split(",")] if a.sizes else range(a.min, a.max + 1):
         n = 1 << L
         plan = dfft.MPIcuFFT_Slab(dfft.Configurations(), dfft.Comm(0, 1, None, 0), precision=a.precision, transform="c2c")
         plan.initFFT(None, signal=n)
@@ -69,19 +97,33 @@ def main():
         inv = lambda: plan.execC2C(xv, y, dfft.INVERSE, stream=torch.cuda.current_stream())  # noqa: E731
         ref_f = lambda: torch.fft.fft(x)  # noqa: E731
         ref_i = lambda: torch.fft.ifft(x)  # noqa: E731
-        times = {"fwd": [], "inv": [], "cufft_fwd": [], "cufft_inv": []}
-        for fn in (fwd, inv, ref_f, ref_i):
+        arms = {"fwd": fwd, "cufft_fwd": ref_f, "inv": inv, "cufft_inv": ref_i}
+        if a.natural:  # the natural-order plan of the same factors, its own output [N3][N2][N1]
+            nat = dfft.MPIcuFFT_Slab(dfft.Configurations(), dfft.Comm(0, 1, None, 0), precision=a.precision, transform="c2c")
+            nat.initFFT(None, signal=n, factors=f, natural=True)
+            yn = torch.empty(f[::-1], dtype=cdt, device="cuda")
+            arms["nat_fwd"] = lambda: nat.execC2C(yn, xv, dfft.FORWARD, stream=torch.cuda.current_stream())  # noqa: E731
+            arms["nat_inv"] = lambda: nat.execC2C(xv, yn, dfft.INVERSE, stream=torch.cuda.current_stream())  # noqa: E731
+        times = {k: [] for k in arms}
+        for fn in arms.values():
             fn()
         torch.cuda.synchronize()
         for _ in range(a.rounds):
-            times["fwd"].append(timed(fwd, a.reps))
-            times["cufft_fwd"].append(timed(ref_f, a.reps))
-            times["inv"].append(timed(inv, a.reps))
-            times["cufft_inv"].append(timed(ref_i, a.reps))
+            for k, fn in arms.items():
+                times[k].append(timed(fn, a.reps))
         med = {k: statistics.median(v) for k, v in times.items()}
-        rows.append({"log2n": L, "factors": f, **med, "precision": a.precision})
-        print(f"  2^{L:2d} {str(f):>18} {med['fwd']:9.3f} {med['cufft_fwd']:10.3f} {med['inv']:9.3f} {med['cufft_inv']:10.3f}", flush=True)
+        row = {"log2n": L, "factors": f, **med, "precision": a.precision}
+        print(f"  2^{L:2d} {str(f):>18} {med['fwd']:9.3f} {med['cufft_fwd']:10.3f} {med['inv']:9.3f} {med['cufft_inv']:10.3f}" +
+              (f" {med['nat_fwd']:9.3f} {med['nat_inv']:9.3f}" if a.natural else ""), flush=True)
+        if a.natural and a.profile:
+            row["kernels"] = {k: kernel_times(arms[k]) for k in ("fwd", "nat_fwd", "inv", "nat_inv")}
+            for k, ks in row["kernels"].items():
+                print(f"    {k}: " + "; ".join(f"{name[:120]} {ms:.3f} ms" for name, ms in sorted(ks.items(), key=lambda kv: -kv[1])), flush=True)
+        rows.append(row)
         plan.destroy()
+        if a.natural:
+            nat.destroy()
+            del yn
         del x, y, xv
         torch.cuda.empty_cache()
     if a.json:
